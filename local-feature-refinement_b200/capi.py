@@ -248,6 +248,22 @@ class Library:
         return r, jac, rho
 
 
+PROFILE_TIERS = {1: "warp2", 2: "tile", 3: "warp", 4: "cta"}  # LmProfile::Tier (csrc/lfr_lm.cuh)
+
+
+def profile_record(cycles: np.ndarray) -> dict:
+    """Decode LFR_DBG_PROFILE records ([n, 8] uint64, one per dispatch slot, csrc/lfr_lm.cuh LmProfile)
+    into named [n] arrays.  `tier` is 0 for a slot without a record (a component with no free node);
+    `counter` is the tier's own: line-search polynomial cycles (warp2, tile, warp) or CG iterations (cta)."""
+    c = np.asarray(cycles, dtype=np.uint64).reshape(-1, 8)
+    w6, w7 = c[:, 6], c[:, 7]
+    return {
+        "total": c[:, 0], "setup": c[:, 1], "eval": c[:, 2], "assemble": c[:, 3], "solve": c[:, 4], "rest": c[:, 5],
+        "ls_steps": (w6 >> np.uint64(32)).astype(np.int64), "smid": (w6 & np.uint64(0xffffffff)).astype(np.int64),
+        "tier": (w7 >> np.uint64(56)).astype(np.int64), "counter": w7 & np.uint64((1 << 56) - 1),
+    }
+
+
 class Plan:
     """Device-resident problem (lfr_plan_*), used by bench.py's `value` leg."""
 
@@ -272,6 +288,18 @@ class Plan:
         self.lib.check(self.lib.lib.lfr_plan_download(self.handle, C.c_void_p(stream), _ptr(pos), C.byref(st)),
                        "lfr_plan_download")
         return pos, Library.stats_dict(st, bufs)
+
+    def profile(self):
+        """Of the last solve of a plan created with LFR_DBG_PROFILE: the decoded cycle record of every slot
+        (profile_record) and the [n, 2] %globaltimer ns at which each component's solve started / finished."""
+        n = self.problem.n_components
+        cyc = np.zeros((n, 8), dtype=np.uint64)
+        tm = np.zeros((n, 2), dtype=np.uint64)
+        f, g = self.lib.lib.lfr_debug_plan_cycles, self.lib.lib.lfr_debug_plan_times
+        f.argtypes = g.argtypes = [C.c_void_p, C.c_void_p]
+        self.lib.check(f(self.handle, _ptr(cyc)), "lfr_debug_plan_cycles")
+        self.lib.check(g(self.handle, _ptr(tm)), "lfr_debug_plan_times")
+        return profile_record(cyc), tm
 
     def num_launches(self) -> int:
         return int(self.lib.lib.lfr_plan_num_launches(self.handle))

@@ -129,7 +129,6 @@ struct Bucket {
   uint32_t offset = 0;  // into the bucket-list buffer
   uint32_t n = 0;
   int emax = 0, ncmax = 0, n2max = 0, smem_per_warp = 0, warps = 4;
-  uint64_t scratch_offset = 0;  // tile tier: first double of this launch's global scratch (12 * emax per CTA)
   int variant = 0;  // 0: shared-memory Cholesky kernel (n <= 64); 16 / 32: register Gauss-Jordan kernel (n <= variant)
   bool stages_edges() const { return variant != 0; }  // warp2 / tile tiers pull their edge records into shared memory
 };
@@ -156,7 +155,7 @@ struct lfr_plan {
   uint32_t N = 0, C = 0;
   uint64_t E = 0;
   uint32_t total_slots = 0;
-  DevBuf row_ptr, edges, track, comp, is_root, comp_ptr, comp_nodes, local_of, pos, pos_init, stats, cycles, times, lists, tile_scratch;
+  DevBuf row_ptr, edges, track, comp, is_root, comp_ptr, comp_nodes, local_of, pos, pos_init, stats, cycles, times, lists;
   // `stats` is one block (one memset, one D2H copy): cost0[Cp] cost1[Cp] iter[Cp] term[Cp] ls[Cp] kept[Cp] err[2] pull[2 x u64]
   uint32_t Cp = 0;               // C rounded up to an even count
   bool pos_is_staged = false;    // lfr_solve(): the start point was uploaded straight into `pos`
@@ -266,7 +265,7 @@ namespace {
 void free_plan(lfr_plan* pl) {
   if (!pl) return;
   DevBuf* bufs[] = {&pl->row_ptr, &pl->edges, &pl->track, &pl->comp, &pl->is_root, &pl->comp_ptr, &pl->comp_nodes,
-                    &pl->local_of, &pl->pos, &pl->pos_init, &pl->stats, &pl->cycles, &pl->times, &pl->lists, &pl->tile_scratch, &pl->L_comps, &pl->L_rec, &pl->L_meta,
+                    &pl->local_of, &pl->pos, &pl->pos_init, &pl->stats, &pl->cycles, &pl->times, &pl->lists, &pl->L_comps, &pl->L_rec, &pl->L_meta,
                     &pl->L_inlist, &pl->L_twin, &pl->L_fdst, &pl->L_bE01, &pl->L_bE23, &pl->L_fdstE, &pl->L_ell_base, &pl->L_scr, &pl->L_q, &pl->L_node, &pl->L_outptr, &pl->L_inptr, &pl->L_freeof,
                     &pl->L_x, &pl->L_xc, &pl->L_lof, &pl->L_vec};
   for (DevBuf* b : bufs) b->release();
@@ -692,15 +691,6 @@ int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const do
   host_mark(0);
   LFR_TRY(build_buckets(pl, p));  // host work overlaps the copies above
   host_mark(1);
-  {
-    uint64_t scratch = 0;
-    for (Bucket& b : pl->buckets)
-      if (LFR_TILE_SCRATCH_GLOBAL && (b.variant >= 48 || b.variant == 132)) {
-        b.scratch_offset = scratch;
-        scratch += 12ull * (uint64_t)b.emax * b.n;
-      }
-    if (scratch) LFR_TRY(pl->tile_scratch.reserve(sizeof(double) * scratch));
-  }
   // Zero-copy and the CTA tier: its preparation kernel can pull the records it keeps straight from the
   // pinned array, but SM loads over PCIe are slower than the copy engine, so that pays only while
   // those components hold less than ~0.3 of the edges
@@ -859,7 +849,6 @@ int launch_solve(lfr_plan* pl, cudaStream_t s) {
     wb.ncmax = b.ncmax;
     wb.n2max = b.n2max;
     wb.smem_per_warp = b.smem_per_warp;
-    wb.scratch = (LFR_TILE_SCRATCH_GLOBAL && (b.variant >= 48 || b.variant == 132)) ? pl->tile_scratch.as<double>() + b.scratch_offset : nullptr;
     const size_t smem = (size_t)b.smem_per_warp * b.warps;
     const unsigned grid = (b.n + b.warps - 1) / b.warps;
     const lfr::DevProblem& P = b.stages_edges() ? P_stage : P_hbm;
@@ -1125,9 +1114,11 @@ int lfr_plan_traffic(lfr_plan* pl, void* stream, uint64_t* algorithmic_bytes, ui
   return LFR_OK;
 }
 
-/* debug (LFR_PROFILE=1): per-slot cycle counters, 8 x uint64 each */
+/* debug (LFR_DBG_PROFILE): one lfr::LmProfile record per slot, 8 x uint64 each:
+   0 total cycles, 1 setup, 2 evaluation, 3 assembly, 4 linear solve, 5 line search and the rest,
+   6 line-search steps << 32 | SM id, 7 tier << 56 | tier counter (see lfr_lm.cuh) */
 int lfr_debug_plan_cycles(lfr_plan* pl, unsigned long long* out) {
-  if (!pl || !pl->profile) return fail(LFR_EINVAL, "plan was not created with LFR_PROFILE=1");
+  if (!pl || !pl->profile) return fail(LFR_EINVAL, "plan was not created with LFR_DBG_PROFILE");
   LFR_CUDA(cudaSetDevice(pl->device));
   LFR_CUDA(cudaMemcpy(out, pl->cycles.p, sizeof(unsigned long long) * 8 * (size_t)pl->C, cudaMemcpyDeviceToHost));
   return LFR_OK;

@@ -2,7 +2,7 @@
 // unknowns: Madrid-scale scenes cap a component at #images = 1000 nodes,
 // solve.cc:586), or every component when lfr_options.linear_solver = 2.
 //
-// Same trust-region loop as the warp kernels (SURVEY Appendix A.6), but the
+// Same trust-region driver as the warp kernels (lfr_lm.cuh, SURVEY Appendix A.6), but the
 // damped normal equations (S H S + D^2) y = S g are never formed: they are
 // solved matrix-free by conjugate gradients preconditioned with the inverse of
 // the 2x2 diagonal blocks (block-Jacobi), iterated to a relative residual of
@@ -348,8 +348,7 @@ __device__ __forceinline__ double cta_matvec_bcsr(const CtaCtx& C, const double*
 // Block-Jacobi PCG for (S H S + D^2) y = S g; dl = -S y.  Returns validity and
 // {model_cost_change, g . dl, |dl|_inf}.
 __device__ __forceinline__ bool cta_lm_step(const CtaCtx& C, double radius, const DevConsts& K, double* model_change,
-                                            double* gd, double* dmax, unsigned* cg_iters, bool diag_mode,
-                                            double* worst_res, unsigned* n_maxit, long long* tph = nullptr) {
+                                            double* gd, double* dmax, unsigned* cg_iters) {
   // damping, preconditioner, initial residual
   double bb = 0.0, rz = 0.0, bad = 0.0;
   for (int f = C.tid; f < C.nf; f += C.nt) {
@@ -395,8 +394,6 @@ __device__ __forceinline__ bool cta_lm_step(const CtaCtx& C, double radius, cons
     for (; it < max_it; ++it) {
       // three barriers per iteration: (1) inside the p.w reduction (also publishes w), (2) inside the
       // {r.r, r.z} reduction, (3) after the update of p, which the next product gathers
-      long long c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0;
-      if (tph) c0 = clock64();
       double s1[1] = {0.0};
       if (C.regular) {
         s1[0] = cta_matvec_bcsr<false>(C, C.p, C.w, C.pblk);
@@ -404,9 +401,7 @@ __device__ __forceinline__ bool cta_lm_step(const CtaCtx& C, double radius, cons
         cta_matvec(C, C.p, C.w);
         for (int i = C.tid; i < C.n; i += C.nt) s1[0] += C.p[i] * C.w[i];
       }
-      if (tph) c1 = clock64();
       block_sum_db(C, s1, 0);
-      if (tph) c2 = clock64();
       const double pw = s1[0];
       if (!(pw > 0.0) || !isfinite(pw)) {  // not positive definite in working precision
         ok = false;
@@ -425,15 +420,7 @@ __device__ __forceinline__ bool cta_lm_step(const CtaCtx& C, double radius, cons
         s2[0] += r0 * r0 + r1 * r1;
         s2[1] += r0 * z0 + r1 * zz1;
       }
-      if (tph) c3 = clock64();
       block_sum_db(C, s2, 1);
-      if (tph) c4 = clock64();
-      if (tph) {
-        tph[0] += c1 - c0;  // product
-        tph[1] += c2 - c1;  // reduction 1
-        tph[2] += c3 - c2;  // vector update
-        tph[3] += c4 - c3;  // reduction 2
-      }
       const double rr = s2[0], rz_new = s2[1];
       if (rr <= tol2) {
         ++it;
@@ -469,17 +456,6 @@ __device__ __forceinline__ bool cta_lm_step(const CtaCtx& C, double radius, cons
     ++restarts;
   }
   *cg_iters += (unsigned)it;
-  if (diag_mode && ok && bb > 0.0) {  // LFR_PROFILE: true residual |b - A y| / |b| of the returned solution
-    if (it >= max_it) ++*n_maxit;
-    if (C.regular) cta_matvec_bcsr(C, C.y, C.w, C.pblk); else cta_matvec(C, C.y, C.w);
-    double e2 = 0.0, z1 = 0.0, z2 = 0.0;
-    for (int i = C.tid; i < C.n; i += C.nt) {
-      const double d = C.S[i] * C.g[i] - C.w[i];
-      e2 += d * d;
-    }
-    block_sum3(C, e2, z1, z2);
-    *worst_res = fmax(*worst_res, sqrt(e2 / bb));
-  }
   double mc = 0.0, dot = 0.0, nonfinite = 0.0, mx = 0.0;
   for (int i = C.tid; i < C.n; i += C.nt) {
     const double y = C.y[i], si = C.S[i], gi = C.g[i];
@@ -507,6 +483,70 @@ __device__ __forceinline__ void cta_candidate(const CtaCtx& C, double alpha, con
   }
   __syncthreads();
 }
+
+// The CTA tier's primitives as the driver's operations (see lfr_lm.cuh).
+template <int NT>
+struct CtaTier {
+  static constexpr int kStride = NT;
+  static constexpr unsigned kTier = LmProfile::kCta;
+  static constexpr int kPolyWord = LmProfile::kRest;
+  CtaCtx& C;
+  const DevConsts& K;
+  unsigned cg_iters;
+  __device__ int tid() const { return C.tid; }
+  __device__ int lane() const { return C.tid & 31; }
+  __device__ bool lead() const { return C.tid == 0; }
+  __device__ double eval_x() { return cta_eval(C, C.x, K); }
+  __device__ double assemble(bool first) { return cta_assemble<false>(C, first, K); }
+  __device__ bool lm_step(double radius, double* model_change, double* gd, double* dmax) {
+    return cta_lm_step(C, radius, K, model_change, gd, dmax, &cg_iters);
+  }
+  __device__ double trial(double alpha) {
+    cta_candidate(C, alpha, K);
+    return cta_eval(C, C.xc, K);
+  }
+  __device__ double trial_slope(double alpha, double* dphi) {
+    const double cost = trial(alpha);
+    if (isfinite(cost)) *dphi = cta_assemble<true>(C, false, K);
+    return cost;
+  }
+  __device__ double slope() { return cta_assemble<true>(C, false, K); }
+  __device__ void scale_step(double s) {
+    for (int i = C.tid; i < C.n; i += NT) C.dl[i] *= s;
+    __syncthreads();
+  }
+  __device__ double x_norm() {
+    double a = 0.0, z1 = 0.0, z2 = 0.0;
+    for (int i = C.tid; i < C.n; i += NT) {
+      const int l = C.lof[i >> 1];
+      const double xv = C.x[2 * l + (i & 1)];
+      a += xv * xv;
+    }
+    block_sum3(C, a, z1, z2);
+    return sqrt(a);
+  }
+  __device__ double step_norm() {
+    double dn2 = 0.0, z1 = 0.0, z2 = 0.0;
+    for (int i = C.tid; i < C.n; i += NT) {
+      const int l = C.lof[i >> 1];
+      const double dv = C.x[2 * l + (i & 1)] - C.xc[2 * l + (i & 1)];
+      dn2 += dv * dv;
+    }
+    block_sum3(C, dn2, z1, z2);
+    return sqrt(dn2);
+  }
+  __device__ double accept() {
+    double a2 = 0.0, z1 = 0.0, z2 = 0.0;
+    for (int i = C.tid; i < 2 * C.Nc; i += NT) {
+      const double v = C.xc[i];
+      C.x[i] = v;
+      if (C.freeof[i >> 1] >= 0) a2 += v * v;
+    }
+    block_sum3(C, a2, z1, z2);
+    return sqrt(a2);
+  }
+  __device__ unsigned long long counter() const { return cg_iters; }
+};
 
 // MINB = CTAs per SM the register allocation is capped for (65536 / (256 x MINB) registers per thread;
 // ptxas: 128 registers at MINB = 2 spill no more than 255 do): the CG loop is a chain of
@@ -588,15 +628,11 @@ solve_cta_kernel(const DevProblem P, const DevConsts K, const CtaArrays A, const
   C.red = red;
   C.red2 = red2;
   const uint32_t c = cc.slot;
-  const int tid = C.tid, lane = tid & 31;
-  if (P.st_times && tid == 0) {
-    unsigned long long ns;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-    P.st_times[2 * (size_t)c] = ns;
-  }
+  const int tid = C.tid;
+  LmProfile prof(P, c, tid == 0);
 
   // start point: IterationZero projects the free blocks onto the box
-  for (int l = tid; l < C.Nc; l += C.nt) {
+  for (int l = tid; l < C.Nc; l += NT) {
     const uint32_t v = C.node[l];
     double p0 = P.positions[2 * (size_t)v], p1 = P.positions[2 * (size_t)v + 1];
     if (C.freeof[l] >= 0) {
@@ -607,171 +643,8 @@ solve_cta_kernel(const DevProblem P, const DevConsts K, const CtaArrays A, const
     C.x[2 * l + 1] = p1;
   }
   __syncthreads();
-  if (tid == 0) P.st_kept[c] = cc.Ec;
-  if (C.nf == 0) {
-    if (tid == 0) {
-      P.st_iter[c] = 0;
-      P.st_term[c] = LFR_TERM_EMPTY;
-      P.st_cost0[c] = 0.0;
-      P.st_cost1[c] = 0.0;
-      P.st_ls[c] = 0;
-    }
-    return;
-  }
-  const bool prof = P.st_cycles != nullptr;
-  long long t_begin = 0, t_lm = 0, t_eval = 0, t_mark = 0;
-  long long tph[4] = {0, 0, 0, 0};
-  if (prof) t_begin = clock64();
-  double cost = cta_eval(C, C.x, K);
-  double gmax = cta_assemble<false>(C, true, K);
-  const double cost0 = cost;
-  double radius = K.radius0, nu = 2.0;
-  int iter = 0, n_invalid = 0, term = LFR_TERM_NO_CONVERGENCE;
-  unsigned ls_steps = 0, cg_iters = 0, n_maxit = 0;
-  double worst_res = 0.0;
-  bool success = true;
-  auto norms = [&](double* xn2, double* dn2) {
-    double a = 0.0, b = 0.0, z = 0.0;
-    for (int i = tid; i < C.n; i += C.nt) {
-      const int l = C.lof[i >> 1];
-      const double xv = C.x[2 * l + (i & 1)], dv = xv - C.xc[2 * l + (i & 1)];
-      a += xv * xv;
-      b += dv * dv;
-    }
-    block_sum3(C, a, b, z);
-    *xn2 = a;
-    *dn2 = b;
-  };
-  double x_norm;
-  {
-    double a = 0.0, b = 0.0, z = 0.0;
-    for (int i = tid; i < C.n; i += C.nt) {
-      const int l = C.lof[i >> 1];
-      const double xv = C.x[2 * l + (i & 1)];
-      a += xv * xv;
-    }
-    block_sum3(C, a, b, z);
-    x_norm = sqrt(a);
-  }
-  for (;;) {
-    if (iter >= K.max_iter) { term = LFR_TERM_NO_CONVERGENCE; break; }
-    if (success && gmax <= K.g_tol) { term = LFR_TERM_GRADIENT_TOL; break; }
-    if (radius <= K.radius_min) { term = LFR_TERM_MIN_RADIUS; break; }
-    ++iter;
-    success = false;
-    double model_change = 0.0, gd = 0.0, dmax = 0.0;
-    if (prof) t_mark = clock64();
-    bool valid = cta_lm_step(C, radius, K, &model_change, &gd, &dmax, &cg_iters, false, &worst_res, &n_maxit,
-                             prof ? tph : nullptr);
-    if (prof) t_lm += clock64() - t_mark;
-    valid = valid && (model_change > 0.0);
-    if (!valid) {
-      if (++n_invalid >= K.max_invalid) { term = LFR_TERM_FAILURE; break; }
-      radius /= nu;
-      nu *= 2.0;
-      continue;
-    }
-    n_invalid = 0;
-    cta_candidate(C, 1.0, K);
-    if (prof) t_mark = clock64();
-    double cost_c = cta_eval(C, C.xc, K);
-    if (prof) t_eval += clock64() - t_mark;
-    bool c_valid = isfinite(cost_c);
-    if (!c_valid || cost_c > cost + K.ls_suff * gd * 1.0) {
-      LsSample initial{0.0, cost, gd, true, true};
-      LsSample previous{0.0, 0.0, 0.0, false, false};
-      LsSample current{1.0, cost_c, 0.0, c_valid, false};
-      if (c_valid) {
-        current.gradient = cta_assemble<true>(C, false, K);
-        current.gradient_valid = isfinite(current.gradient);
-      }
-      int ls_iter = 0;
-      bool ls_ok = false;
-      for (;;) {
-        ++ls_iter;
-        ++ls_steps;
-        if (ls_iter >= K.max_ls_iter) break;
-        const double step = ls_next_step(initial, previous, current, K, lane);
-        if (step * dmax < K.ls_min_step) break;
-        previous = current;
-        cta_candidate(C, step, K);
-        cost_c = cta_eval(C, C.xc, K);
-        c_valid = isfinite(cost_c);
-        current = LsSample{step, cost_c, 0.0, c_valid, false};
-        if (c_valid) {
-          current.gradient = cta_assemble<true>(C, false, K);
-          current.gradient_valid = isfinite(current.gradient);
-        }
-        if (c_valid && !(cost_c > cost + K.ls_suff * gd * step)) { ls_ok = true; break; }
-      }
-      if (ls_ok) {
-        for (int i = tid; i < C.n; i += C.nt) C.dl[i] *= current.x;
-        __syncthreads();
-      } else {
-        cta_candidate(C, 1.0, K);
-        cost_c = cta_eval(C, C.xc, K);
-        c_valid = isfinite(cost_c);
-      }
-    }
-    if (!c_valid) cost_c = 1.7976931348623157e308;
-    double xn2, dn2;
-    norms(&xn2, &dn2);
-    const double step_norm = sqrt(dn2);
-    if (step_norm <= K.p_tol * (x_norm + K.p_tol)) { term = LFR_TERM_PARAMETER_TOL; break; }
-    if (fabs(cost - cost_c) <= K.f_tol * cost) { term = LFR_TERM_FUNCTION_TOL; break; }
-    const double rho = (cost - cost_c) / model_change;
-    if (rho > K.min_rel_decrease) {
-      double a2 = 0.0, z1 = 0.0, z2 = 0.0;
-      for (int i = tid; i < 2 * C.Nc; i += C.nt) {
-        const double v = C.xc[i];
-        C.x[i] = v;
-        if (C.freeof[i >> 1] >= 0) a2 += v * v;
-      }
-      block_sum3(C, a2, z1, z2);
-      x_norm = sqrt(a2);
-      cost = cost_c;
-      gmax = cta_assemble<false>(C, false, K);
-      success = true;
-      const double t = 2.0 * rho - 1.0;
-      radius = fmin(K.radius_max, radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-      nu = 2.0;
-    } else {
-      radius /= nu;
-      nu *= 2.0;
-    }
-  }
-  // (not after FAILURE: Ceres only commits a usable solution, solver.cc Minimize / IsSolutionUsable)
-  if (term != LFR_TERM_FAILURE) {
-    for (int i = tid; i < C.n; i += C.nt) {
-      const int l = C.lof[i >> 1];
-      P.positions_out[2 * (size_t)C.node[l] + (i & 1)] = C.x[2 * l + (i & 1)];
-    }
-  }
-  if (tid == 0) {
-    P.st_iter[c] = iter;
-    P.st_term[c] = term;
-    P.st_cost0[c] = cost0;
-    P.st_cost1[c] = cost;
-    P.st_ls[c] = ls_steps;
-    if (P.st_cycles) {
-      unsigned long long* o = P.st_cycles + 8 * (size_t)c;
-      o[0] = (unsigned long long)(clock64() - t_begin);  // total, of which o[2] in the PCG solves
-      o[2] = (unsigned long long)t_lm;
-      o[3] = ((unsigned long long)(tph[0] >> 8) << 32) | (unsigned long long)min((long long)0xffffffffll, tph[1] >> 8);  // product | reduction 1, 256-cycle units
-      o[5] = ((unsigned long long)(tph[2] >> 8) << 32) | (unsigned long long)min((long long)0xffffffffll, tph[3] >> 8);  // update | reduction 2
-      o[4] = cg_iters;
-      o[1] = 1;  // marks a CTA-tier component
-      o[6] = ((unsigned long long)ls_steps << 32) | (unsigned long long)min((long long)0xffffffffll, t_eval >> 10);  // + first-candidate evaluations, kcycles
-      unsigned smid;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      o[7] = smid;
-    }
-    if (P.st_times) {
-      unsigned long long ns;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-      P.st_times[2 * (size_t)c + 1] = ns;
-    }
-  }
+  CtaTier<NT> T{C, K, 0u};
+  lm_solve(T, P, K, c, prof);
 }
 
 // ---- device-side preparation of the CTA-tier components (solve.cc:98-143 for each) --------------

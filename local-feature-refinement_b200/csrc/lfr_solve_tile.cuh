@@ -11,13 +11,6 @@
 
 namespace lfr {
 
-// 1: the per-edge evaluation / assembly scratch (96 of 186 bytes per candidate edge) lives in a per-CTA
-// global area instead of shared memory: more resident components, each slower by the scratch latency;
-// left off.
-#ifndef LFR_TILE_SCRATCH_GLOBAL
-#define LFR_TILE_SCRATCH_GLOBAL 0
-#endif
-
 struct TileLayout {
   int stage, bar;
   int x, xc, g, S, dl, H, scr, tup, prow, red, hdr;
@@ -35,16 +28,8 @@ struct TileLayout {
     S = o; o += 8 * n2max;
     dl = o; o += 8 * n2max;
     H = o; o += 8 * n2max * ldh;
-    // scr (7 doubles per candidate edge: the staged evaluation) and tup (5: the assembly tuples) live
-    // in a per-CTA global scratch area (WarpBucket::scratch), not here: at 96 of 186 bytes per edge they
-    // were what held this tier to 1-2 CTAs (2-4 warps) per SM on ETH3D-scale scenes
-#if LFR_TILE_SCRATCH_GLOBAL
-    scr = 0;
-    tup = 0;
-#else
-    scr = o; o += 8 * 7 * emax;
-    tup = o; o += 8 * 5 * emax;
-#endif
+    scr = o; o += 8 * 7 * emax;  // the staged evaluation (7 doubles per candidate edge)
+    tup = o; o += 8 * 5 * emax;  // the assembly tuples (5)
     o = align_up(o, 16);
     prow = o; o += 8 * 4 * 84;   // double-buffered pair of pivot rows: 2 x 2 x (80 columns, rhs, spare)
     red = o; o += 8 * 3 * 4;     // block reductions (<= 4 warps)
@@ -369,6 +354,68 @@ __device__ __forceinline__ void tile_candidate(const TileCtx<T>& C, double alpha
   __syncthreads();
 }
 
+// The tile tier's primitives as the driver's operations (see lfr_lm.cuh).
+template <int T, int NREG>
+struct TileTier {
+  static constexpr int kStride = T;
+  static constexpr unsigned kTier = LmProfile::kTile;
+  static constexpr int kPolyWord = LmProfile::kTierWord;
+  TileCtx<T>& C;
+  const DevConsts& K;
+  __device__ int tid() const { return C.tid; }
+  __device__ int lane() const { return C.tid & 31; }
+  __device__ bool lead() const { return C.tid == 0; }
+  __device__ double eval_x() { return tile_eval<T, false>(C, C.x, K); }
+  __device__ double assemble(bool first) { return tile_assemble<T, false>(C, first, K); }
+  __device__ bool lm_step(double radius, double* model_change, double* gd, double* dmax) {
+    return tile_lm_step<T, NREG>(C, radius, K, model_change, gd, dmax);
+  }
+  __device__ double trial(double alpha) {
+    tile_candidate(C, alpha, K);
+    return tile_eval<T, false>(C, C.xc, K);
+  }
+  __device__ double trial_slope(double alpha, double* dphi) {
+    tile_candidate(C, alpha, K);
+    return tile_eval<T, true>(C, C.xc, K, dphi);
+  }
+  __device__ double slope() { return tile_assemble<T, true>(C, false, K); }
+  __device__ void scale_step(double s) {
+    for (int i = C.tid; i < C.n; i += T) C.dl[i] *= s;
+    __syncthreads();
+  }
+  __device__ double x_norm() {
+    double a = 0.0, z1 = 0.0, z2 = 0.0;
+    for (int i = C.tid; i < C.n; i += T) {
+      const int l = C.lof[i >> 1];
+      const double xv = C.x[2 * l + (i & 1)];
+      a += xv * xv;
+    }
+    tile_sum3(C, a, z1, z2);
+    return sqrt(a);
+  }
+  __device__ double step_norm() {
+    double dn2 = 0.0, z1 = 0.0, z2 = 0.0;
+    for (int i = C.tid; i < C.n; i += T) {
+      const int l = C.lof[i >> 1];
+      const double dv = C.x[2 * l + (i & 1)] - C.xc[2 * l + (i & 1)];
+      dn2 += dv * dv;
+    }
+    tile_sum3(C, dn2, z1, z2);
+    return sqrt(dn2);
+  }
+  __device__ double accept() {
+    double a2 = 0.0, z1 = 0.0, z2 = 0.0;
+    for (int i = C.tid; i < 2 * C.Nc; i += T) {
+      const double v = C.xc[i];
+      C.x[i] = v;
+      if (C.freeof[i >> 1] >= 0) a2 += v * v;
+    }
+    tile_sum3(C, a2, z1, z2);
+    return sqrt(a2);
+  }
+  __device__ unsigned long long counter() const { return 0; }
+};
+
 template <int T, int NREG>
 __global__ void __launch_bounds__(T)
 solve_tile_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
@@ -387,13 +434,8 @@ solve_tile_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
   C.S = (double*)(base + L.S);
   C.dl = (double*)(base + L.dl);
   C.H = (double*)(base + L.H);
-#if LFR_TILE_SCRATCH_GLOBAL
-  C.scr = B.scratch + (size_t)blockIdx.x * 12 * (size_t)B.emax;  // global (L1/L2-resident): lanes <-> edges, SoA
-  C.tup = C.scr + 7 * (size_t)B.emax;
-#else
   C.scr = (double*)(base + L.scr);
   C.tup = (double*)(base + L.tup);
-#endif
   C.prow = (double*)(base + L.prow);
   C.red = (double*)(base + L.red);
   int* hdr = (int*)(base + L.hdr);
@@ -410,15 +452,8 @@ solve_tile_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
   C.stage = (float4*)(base + L.stage);
   C.bar = (uint64_t*)(base + L.bar);
 
-  const int Nc = (int)(P.comp_ptr[c + 1] - P.comp_ptr[c]);
-  C.Nc = Nc;
-  long long t_begin = 0, t_lm = 0, t_mark = 0;
-  if (P.st_cycles) t_begin = clock64();
-  if (P.st_times && tid == 0) {
-    unsigned long long ns;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-    P.st_times[2 * (size_t)c] = ns;
-  }
+  C.Nc = (int)(P.comp_ptr[c + 1] - P.comp_ptr[c]);
+  LmProfile prof(P, c, tid == 0);
   // ---- setup by warp 0 (solve.cc:98-143), shared with the warp kernel -----------------------
   if (tid < 32) {
     int Ec = 0, nf = 0;
@@ -428,7 +463,6 @@ solve_tile_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
       hdr[0] = Ec;
       hdr[1] = nf;
       hdr[2] = irregular ? 1 : 0;
-      P.st_kept[c] = (uint32_t)Ec;
     }
   }
   __syncthreads();
@@ -436,156 +470,8 @@ solve_tile_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
   C.nf = hdr[1];
   C.n = 2 * C.nf;
   C.irregular = hdr[2] != 0;
-  if (C.nf == 0) {
-    if (tid == 0) {
-      P.st_iter[c] = 0;
-      P.st_term[c] = LFR_TERM_EMPTY;
-      P.st_cost0[c] = 0.0;
-      P.st_cost1[c] = 0.0;
-      P.st_ls[c] = 0;
-    }
-    return;
-  }
-
-  double cost = tile_eval<T, false>(C, C.x, K);
-  double gmax = tile_assemble<T, false>(C, true, K);
-  const double cost0 = cost;
-  double radius = K.radius0, nu = 2.0;
-  int iter = 0, n_invalid = 0, term = LFR_TERM_NO_CONVERGENCE;
-  unsigned ls_steps = 0;
-  bool success = true;
-  double x_norm;
-  {
-    double a = 0.0, z1 = 0.0, z2 = 0.0;
-    for (int i = tid; i < C.n; i += T) {
-      const int l = C.lof[i >> 1];
-      const double xv = C.x[2 * l + (i & 1)];
-      a += xv * xv;
-    }
-    tile_sum3(C, a, z1, z2);
-    x_norm = sqrt(a);
-  }
-  for (;;) {
-    if (iter >= K.max_iter) { term = LFR_TERM_NO_CONVERGENCE; break; }
-    if (success && gmax <= K.g_tol) { term = LFR_TERM_GRADIENT_TOL; break; }
-    if (radius <= K.radius_min) { term = LFR_TERM_MIN_RADIUS; break; }
-    ++iter;
-    success = false;
-    double model_change = 0.0, gd = 0.0, dmax = 0.0;
-    if (P.st_cycles) t_mark = clock64();
-    bool valid = tile_lm_step<T, NREG>(C, radius, K, &model_change, &gd, &dmax);
-    if (P.st_cycles) t_lm += clock64() - t_mark;
-    valid = valid && (model_change > 0.0);
-    if (!valid) {
-      if (++n_invalid >= K.max_invalid) { term = LFR_TERM_FAILURE; break; }
-      radius /= nu;
-      nu *= 2.0;
-      continue;
-    }
-    n_invalid = 0;
-    tile_candidate(C, 1.0, K);
-    double cost_c = tile_eval<T, false>(C, C.xc, K);
-    bool c_valid = isfinite(cost_c);
-    if (!c_valid || cost_c > cost + K.ls_suff * gd * 1.0) {
-      LsSample initial{0.0, cost, gd, true, true};
-      LsSample previous{0.0, 0.0, 0.0, false, false};
-      LsSample current{1.0, cost_c, 0.0, c_valid, false};
-      if (c_valid) {
-        current.gradient = tile_assemble<T, true>(C, false, K);
-        current.gradient_valid = isfinite(current.gradient);
-      }
-      int ls_iter = 0;
-      bool ls_ok = false;
-      for (;;) {
-        ++ls_iter;
-        ++ls_steps;
-        if (ls_iter >= K.max_ls_iter) break;
-        const double step = ls_next_step(initial, previous, current, K, lane);
-        if (step * dmax < K.ls_min_step) break;
-        previous = current;
-        tile_candidate(C, step, K);
-        double dphi;
-        cost_c = tile_eval<T, true>(C, C.xc, K, &dphi);
-        c_valid = isfinite(cost_c);
-        current = LsSample{step, cost_c, 0.0, c_valid, false};
-        if (c_valid) {
-          current.gradient = dphi;
-          current.gradient_valid = isfinite(dphi);
-        }
-        if (c_valid && !(cost_c > cost + K.ls_suff * gd * step)) { ls_ok = true; break; }
-      }
-      if (ls_ok) {
-        for (int i = tid; i < C.n; i += T) C.dl[i] *= current.x;
-        __syncthreads();
-      } else {
-        tile_candidate(C, 1.0, K);
-        cost_c = tile_eval<T, false>(C, C.xc, K);
-        c_valid = isfinite(cost_c);
-      }
-    }
-    if (!c_valid) cost_c = 1.7976931348623157e308;
-    double dn2 = 0.0, z1 = 0.0, z2 = 0.0;
-    for (int i = tid; i < C.n; i += T) {
-      const int l = C.lof[i >> 1];
-      const double dv = C.x[2 * l + (i & 1)] - C.xc[2 * l + (i & 1)];
-      dn2 += dv * dv;
-    }
-    tile_sum3(C, dn2, z1, z2);
-    const double step_norm = sqrt(dn2);
-    if (step_norm <= K.p_tol * (x_norm + K.p_tol)) { term = LFR_TERM_PARAMETER_TOL; break; }
-    if (fabs(cost - cost_c) <= K.f_tol * cost) { term = LFR_TERM_FUNCTION_TOL; break; }
-    const double rho = (cost - cost_c) / model_change;
-    if (rho > K.min_rel_decrease) {
-      double a2 = 0.0;
-      z1 = z2 = 0.0;
-      for (int i = tid; i < 2 * Nc; i += T) {
-        const double v = C.xc[i];
-        C.x[i] = v;
-        if (C.freeof[i >> 1] >= 0) a2 += v * v;
-      }
-      tile_sum3(C, a2, z1, z2);
-      x_norm = sqrt(a2);
-      cost = cost_c;
-      gmax = tile_assemble<T, false>(C, false, K);
-      success = true;
-      const double t = 2.0 * rho - 1.0;
-      radius = fmin(K.radius_max, radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-      nu = 2.0;
-    } else {
-      radius /= nu;
-      nu *= 2.0;
-    }
-  }
-  // (not after FAILURE: Ceres only commits a usable solution, solver.cc Minimize / IsSolutionUsable)
-  if (term != LFR_TERM_FAILURE) {
-    for (int i = tid; i < C.n; i += T) {
-      const int l = C.lof[i >> 1];
-      P.positions_out[2 * (size_t)C.node[l] + (i & 1)] = C.x[2 * l + (i & 1)];
-    }
-  }
-  if (tid == 0) {
-    P.st_iter[c] = iter;
-    P.st_term[c] = term;
-    P.st_cost0[c] = cost0;
-    P.st_cost1[c] = cost;
-    P.st_ls[c] = ls_steps;
-    if (P.st_cycles) {
-      unsigned long long* o = P.st_cycles + 8 * (size_t)c;
-      o[2] = o[3] = o[5] = 0;
-      o[0] = (unsigned long long)(clock64() - t_begin);
-      o[4] = (unsigned long long)t_lm;  // of which in the linear solves
-      o[1] = 2;  // marks a tile-tier component
-      o[6] = (unsigned long long)ls_steps << 32;
-      unsigned smid;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      o[7] = smid;
-    }
-    if (P.st_times) {
-      unsigned long long ns;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-      P.st_times[2 * (size_t)c + 1] = ns;
-    }
-  }
+  TileTier<T, NREG> Tr{C, K};
+  lm_solve(Tr, P, K, c, prof);
 }
 
 }  // namespace lfr

@@ -647,6 +647,55 @@ __device__ __forceinline__ void warp_setup(Ctx& C, uint32_t* rowstart, uint32_t*
   *nf_out = frun;
 }
 
+// The warp2 tier's primitives as the driver's operations (see lfr_lm.cuh).  Both norms of the
+// parameter test come from the CandNorms fused into the candidate's evaluation.
+template <int NREG>
+struct Warp2Tier {
+  static constexpr int kStride = 32;
+  static constexpr unsigned kTier = LmProfile::kWarp2;
+  static constexpr int kPolyWord = LmProfile::kTierWord;
+  Warp2Ctx& C;
+  const DevConsts& K;
+  CandNorms nr;  // of the last candidate
+  __device__ int tid() const { return C.lane; }
+  __device__ int lane() const { return C.lane; }
+  __device__ bool lead() const { return C.lane == 0; }
+  __device__ double eval_x() { return eval_pass2<false, false>(C, C.x, K); }
+  __device__ double assemble(bool first) { return assemble2<false>(C, first, K); }
+  __device__ bool lm_step(double radius, double* model_change, double* gd, double* dmax) {
+    return lm_step2<NREG>(C, radius, K, model_change, gd, dmax);
+  }
+  __device__ double trial(double alpha) {
+    nr = make_candidate2(C, alpha, K);
+    return eval_pass2<false, true>(C, C.xc, K, nullptr, &nr);
+  }
+  __device__ double trial_slope(double alpha, double* dphi) {
+    nr = make_candidate2(C, alpha, K);
+    return eval_pass2<true, true>(C, C.xc, K, dphi, &nr);
+  }
+  __device__ double slope() { return assemble2<true>(C, false, K); }
+  __device__ void scale_step(double s) {
+    for (int i = C.lane; i < C.n; i += 32) C.dl[i] *= s;
+    __syncwarp();
+  }
+  __device__ double x_norm() {
+    double a = 0.0;
+    for (int i = C.lane; i < C.n; i += 32) {
+      const int l = C.lof[i >> 1];
+      const double xv = C.x[2 * l + (i & 1)];
+      a += xv * xv;
+    }
+    return sqrt(warp_sum(a));
+  }
+  __device__ double step_norm() { return sqrt(nr.dn2); }
+  __device__ double accept() {
+    for (int i = C.lane; i < 2 * C.Nc; i += 32) C.x[i] = C.xc[i];
+    __syncwarp();
+    return sqrt(nr.xn2);
+  }
+  __device__ unsigned long long counter() const { return 0; }
+};
+
 // (12 resident warps per SM = 168 registers for NREG <= 16; 8 (255 registers) and 16 (128 registers)
 // are the alternatives)
 template <int WARPS, int NREG>
@@ -686,176 +735,18 @@ solve_warp2_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
   C.freeof = (int16_t*)(base + L.freeof);
   C.lof = (uint16_t*)(base + L.lof);
 
-  const bool prof = (P.st_cycles != nullptr);
-  if (prof && lane == 0) {
-    unsigned long long ns;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-    P.st_times[2 * (size_t)c] = ns;
-  }
-  long long t_begin = prof ? clock64() : 0, t_mark = t_begin;
-  long long cyc_eval = 0, cyc_asm = 0, cyc_lm = 0, cyc_ls = 0, cyc_setup = 0, cyc_poly = 0;
-#define LFR_TICK(acc) do { if (prof) { const long long now__ = clock64(); acc += now__ - t_mark; t_mark = now__; } } while (0)
-
+  LmProfile prof(P, c, lane == 0);
   // ---- component setup (solve.cc:98-143) --------------------------------------
-  int Ec = 0, nf_setup = 0;
-  bool irregular_setup = false;
-  warp_setup(C, rowstart, candptr, cnt, B.ncmax, P, K, c, lane, &Ec, &nf_setup, &irregular_setup);
+  int Ec = 0, nf = 0;
+  bool irregular = false;
+  warp_setup(C, rowstart, candptr, cnt, B.ncmax, P, K, c, lane, &Ec, &nf, &irregular);
   C.Ec = Ec;
-  C.irregular = irregular_setup;
-  const int Nc = C.Nc;
-  const int frun = nf_setup;
-  const int nf = frun;
+  C.irregular = irregular;
   C.nf = nf;
   C.n = 2 * nf;
   __syncwarp();
-  if (lane == 0) P.st_kept[c] = (uint32_t)Ec;
-  if (nf == 0) {  // "No non-constant parameter blocks found."
-    if (lane == 0) {
-      P.st_iter[c] = 0;
-      P.st_term[c] = LFR_TERM_EMPTY;
-      P.st_cost0[c] = 0.0;
-      P.st_cost1[c] = 0.0;
-      P.st_ls[c] = 0;
-    }
-    return;
-  }
-  LFR_TICK(cyc_setup);
-
-  // ---- iteration 0 -----------------------------------------------------------------
-  double cost = eval_pass2<false, false>(C, C.x, K);
-  LFR_TICK(cyc_eval);
-  double gmax = assemble2<false>(C, true, K);
-  LFR_TICK(cyc_asm);
-  const double cost0 = cost;
-  double radius = K.radius0, nu = 2.0;
-  int iter = 0, n_invalid = 0, term = LFR_TERM_NO_CONVERGENCE;
-  unsigned ls_steps = 0;
-  bool success = true;
-  double x_norm;
-  {
-    double a = 0.0;
-    for (int i = lane; i < C.n; i += 32) {
-      const int l = C.lof[i >> 1];
-      const double xv = C.x[2 * l + (i & 1)];
-      a += xv * xv;
-    }
-    x_norm = sqrt(warp_sum(a));
-  }
-
-  // ---- trust-region loop (A.6) ---------------------------------------------------------
-  for (;;) {
-    if (iter >= K.max_iter) { term = LFR_TERM_NO_CONVERGENCE; break; }
-    if (success && gmax <= K.g_tol) { term = LFR_TERM_GRADIENT_TOL; break; }
-    if (radius <= K.radius_min) { term = LFR_TERM_MIN_RADIUS; break; }
-    ++iter;
-    success = false;
-    double model_change = 0.0, gd = 0.0, dmax = 0.0;
-    LFR_TICK(cyc_ls);
-    bool valid = lm_step2<NREG>(C, radius, K, &model_change, &gd, &dmax);
-    LFR_TICK(cyc_lm);
-    valid = valid && (model_change > 0.0);
-    if (!valid) {
-      if (++n_invalid >= K.max_invalid) { term = LFR_TERM_FAILURE; break; }
-      radius /= nu;
-      nu *= 2.0;
-      continue;
-    }
-    n_invalid = 0;
-    // projected Armijo line search along dl (bounds-constrained problem, A.7b)
-    CandNorms nr = make_candidate2(C, 1.0, K);
-    double cost_c = eval_pass2<false, true>(C, C.xc, K, nullptr, &nr);
-    LFR_TICK(cyc_eval);
-    bool c_valid = isfinite(cost_c);
-    if (!c_valid || cost_c > cost + K.ls_suff * gd * 1.0) {
-      LsSample initial{0.0, cost, gd, true, true};
-      LsSample previous{0.0, 0.0, 0.0, false, false};
-      LsSample current{1.0, cost_c, 0.0, c_valid, false};
-      if (c_valid) {
-        current.gradient = assemble2<true>(C, false, K);
-        current.gradient_valid = isfinite(current.gradient);
-      }
-      int ls_iter = 0;
-      bool ls_ok = false;
-      for (;;) {
-        ++ls_iter;
-        ++ls_steps;
-        if (ls_iter >= K.max_ls_iter) break;
-        LFR_TICK(cyc_ls);
-        const double step = ls_next_step(initial, previous, current, K, lane);
-        LFR_TICK(cyc_poly);
-        if (step * dmax < K.ls_min_step) break;
-        previous = current;
-        nr = make_candidate2(C, step, K);
-        double dphi;
-        cost_c = eval_pass2<true, true>(C, C.xc, K, &dphi, &nr);
-        c_valid = isfinite(cost_c);
-        current = LsSample{step, cost_c, 0.0, c_valid, false};
-        if (c_valid) {
-          current.gradient = dphi;
-          current.gradient_valid = isfinite(dphi);
-        }
-        if (c_valid && !(cost_c > cost + K.ls_suff * gd * step)) { ls_ok = true; break; }
-      }
-      if (ls_ok) {
-        for (int i = lane; i < C.n; i += 32) C.dl[i] *= current.x;
-        __syncwarp();
-      } else {  // line search failed: delta unchanged, candidate = P(x + delta)
-        nr = make_candidate2(C, 1.0, K);
-        cost_c = eval_pass2<false, true>(C, C.xc, K, nullptr, &nr);
-        c_valid = isfinite(cost_c);
-      }
-    }
-    if (!c_valid) cost_c = 1.7976931348623157e308;
-    const double step_norm = sqrt(nr.dn2);
-    if (step_norm <= K.p_tol * (x_norm + K.p_tol)) { term = LFR_TERM_PARAMETER_TOL; break; }
-    if (fabs(cost - cost_c) <= K.f_tol * cost) { term = LFR_TERM_FUNCTION_TOL; break; }
-    const double rho = (cost - cost_c) / model_change;
-    if (rho > K.min_rel_decrease) {
-      for (int i = lane; i < 2 * Nc; i += 32) C.x[i] = C.xc[i];
-      __syncwarp();
-      cost = cost_c;
-      LFR_TICK(cyc_ls);
-      gmax = assemble2<false>(C, false, K);
-      x_norm = sqrt(nr.xn2);
-      LFR_TICK(cyc_asm);
-      success = true;
-      const double t = 2.0 * rho - 1.0;
-      radius = fmin(K.radius_max, radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-      nu = 2.0;
-    } else {
-      radius /= nu;
-      nu *= 2.0;
-    }
-  }
-  // ---- write back the last accepted x ---------------------------------------------------
-  // (not after FAILURE: Ceres only commits a usable solution, solver.cc Minimize / IsSolutionUsable)
-  if (term != LFR_TERM_FAILURE) {
-    for (int i = lane; i < C.n; i += 32) {
-      const int l = C.lof[i >> 1];
-      P.positions_out[2 * (size_t)C.node[l] + (i & 1)] = C.x[2 * l + (i & 1)];
-    }
-  }
-  if (lane == 0) {
-    P.st_iter[c] = iter;
-    P.st_term[c] = term;
-    P.st_cost0[c] = cost0;
-    P.st_cost1[c] = cost;
-    P.st_ls[c] = ls_steps;
-    if (prof) {
-      LFR_TICK(cyc_ls);
-      unsigned long long* o = P.st_cycles + 8 * (size_t)c;
-      o[0] = (unsigned long long)(t_mark - t_begin);
-      o[1] = cyc_setup; o[2] = cyc_eval; o[3] = cyc_asm; o[4] = cyc_lm; o[5] = cyc_ls;
-      unsigned smid;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      o[6] = (unsigned long long)smid | ((unsigned long long)ls_steps << 32);
-      o[7] = (unsigned long long)cyc_poly;
-      unsigned long long ns;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-      P.st_times[2 * (size_t)c + 1] = ns;
-    }
-  }
-#undef LFR_TICK
+  Warp2Tier<NREG> T{C, K, {0.0, 0.0}};
+  lm_solve(T, P, K, c, prof);
 }
 
 }  // namespace lfr

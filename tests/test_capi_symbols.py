@@ -123,3 +123,27 @@ def test_schedule_does_not_depend_on_the_thread_count(b200, monkeypatch):
             assert f(C.byref(s), None, 1, C.byref(us), C.byref(nl), C.byref(dg)) == 0
             seen.add((nl.value, dg.value))
         assert len(seen) == 1, (name, seen)
+
+
+def test_profile_record_decodes_every_word():
+    """capi.profile_record on hand-built LFR_DBG_PROFILE records: the word layout and tier codes of
+    LmProfile in csrc/lfr_lm.cuh."""
+    from lfr_b200.capi import PROFILE_TIERS, profile_record
+    src = open(os.path.join(ROOT, "local-feature-refinement_b200", "csrc", "lfr_lm.cuh")).read()
+    words = re.search(r"enum Word \{([^}]*)\}", src).group(1)
+    assert [w.split("=")[0].strip() for w in words.split(",")] == [
+        "kTotal", "kSetup", "kEval", "kAssemble", "kSolve", "kRest", "kSteps", "kTierWord"]
+    tiers = dict(re.findall(r"k(\w+) = (\d+)", re.search(r"enum Tier : unsigned \{([^}]*)\}", src).group(1)))
+    assert {int(v): k.lower() for k, v in tiers.items()} == PROFILE_TIERS
+    rec = np.zeros((3, 8), dtype=np.uint64)
+    rec[0] = [1000, 10, 200, 300, 400, 50, (7 << 32) | 131, (1 << 56) | 40]   # warp2, 40 polynomial cycles
+    rec[1] = [5000, 0, 600, 700, 3000, 700, (0 << 32) | 3, (4 << 56) | 1234]  # CTA, 1234 CG iterations
+    d = profile_record(rec)                                                   # rec[2]: no record (empty component)
+    for k, col in (("total", 0), ("setup", 1), ("eval", 2), ("assemble", 3), ("solve", 4), ("rest", 5)):
+        assert d[k].tolist() == rec[:, col].tolist(), k
+    assert d["ls_steps"].tolist() == [7, 0, 0]
+    assert d["smid"].tolist() == [131, 3, 0]
+    assert d["tier"].tolist() == [1, 4, 0]
+    assert d["counter"].tolist() == [40, 1234, 0]
+    assert [PROFILE_TIERS.get(t) for t in d["tier"].tolist()] == ["warp2", "cta", None]
+    assert profile_record(rec.ravel())["total"].shape == (3,)

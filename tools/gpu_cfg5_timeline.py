@@ -1,6 +1,5 @@
 """cfg5, one GPU, plan path with LFR_DBG_PROFILE: per-component start / end (%globaltimer) and SM of
 the CTA tier for consecutive solves — why is the same solve 382 ms one time and 541 ms the next?"""
-import ctypes as C
 import os
 import sys
 
@@ -21,10 +20,6 @@ plan = Plan(lib, p, lib.default_options(debug_flags=0x10))
 s = torch.cuda.current_stream().cuda_stream
 sizes = np.diff(p.comp_ptr.astype(np.int64))
 Cn = p.n_components
-fc = lib.lib.lfr_debug_plan_cycles
-ft = lib.lib.lfr_debug_plan_times
-fc.argtypes = [C.c_void_p, C.c_void_p]
-ft.argtypes = [C.c_void_p, C.c_void_p]
 for i in range(n_solves):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
@@ -33,43 +28,35 @@ for i in range(n_solves):
     torch.cuda.synchronize()
     _, stt = plan.download(s)
     p_iters = stt["iterations"].astype(np.float64)
-    cyc = np.zeros((Cn, 8), dtype=np.uint64)
-    tm = np.zeros((Cn, 2), dtype=np.uint64)
-    assert fc(plan.handle, cyc.ctypes.data) == 0 and ft(plan.handle, tm.ctypes.data) == 0
+    rec, tm = plan.profile()
     ran = tm[:, 0] > 0
     t0 = tm[ran, 0].min()
     st = (tm[:, 0].astype(np.float64) - t0) / 1e6
     en = (tm[:, 1].astype(np.float64) - t0) / 1e6
     dur = en - st
-    cta = ran & (cyc[:, 1] == 1)
+    cta = ran & (rec["tier"] == 4)
     print("solve %d: %.1f ms by events; components timed %d (CTA tier %d); last end %.1f ms" % (
         i, e0.elapsed_time(e1), int(ran.sum()), int(cta.sum()), en[ran].max()))
     if cta.any():
-        sm = cyc[cta, 7].astype(np.int64)
+        sm = rec["smid"][cta]
         print("   CTA tier: sum of durations %.0f ms over %d SMs -> /296 = %.1f ms;  start p50 %.1f p90 %.1f max %.1f;  duration p50 %.2f p99 %.1f max %.1f" % (
             dur[cta].sum(), len(np.unique(sm)), dur[cta].sum() / 296.0, np.median(st[cta]), np.percentile(st[cta], 90), st[cta].max(),
             np.median(dur[cta]), np.percentile(dur[cta], 99), dur[cta].max()))
-        tot = cyc[cta, 0].astype(np.float64); lm = cyc[cta, 2].astype(np.float64); ev = (cyc[cta, 6] & np.uint64(0xffffffff)).astype(np.float64) * 1024
-        cg = cyc[cta, 4].astype(np.float64); its = np.maximum(1, p_iters[cta])
-        print("   CTA tier cycles: total %.3g  PCG %.1f%%  first-candidate eval %.1f%%;  cycles per CG iteration p50 %.0f p90 %.0f;  CG iterations per LM step p50 %.0f p90 %.0f" % (
+        tot = rec["total"][cta].astype(np.float64); lm = rec["solve"][cta].astype(np.float64); ev = rec["eval"][cta].astype(np.float64)
+        cg = rec["counter"][cta].astype(np.float64); its = np.maximum(1, p_iters[cta])
+        print("   CTA tier cycles: total %.3g  PCG %.1f%%  eval %.1f%%;  cycles per CG iteration p50 %.0f p90 %.0f;  CG iterations per LM step p50 %.0f p90 %.0f" % (
             tot.sum(), 100 * lm.sum() / tot.sum(), 100 * ev.sum() / tot.sum(), np.median(lm / np.maximum(cg, 1)), np.percentile(lm / np.maximum(cg, 1), 90),
             np.median(cg / its), np.percentile(cg / its, 90)))
-        mv = (cyc[cta, 3] >> np.uint64(32)).astype(np.float64) * 256; r1 = (cyc[cta, 3] & np.uint64(0xffffffff)).astype(np.float64) * 256
-        up = (cyc[cta, 5] >> np.uint64(32)).astype(np.float64) * 256; r2 = (cyc[cta, 5] & np.uint64(0xffffffff)).astype(np.float64) * 256
-        print("   PCG split (thread 0's clock): product %.1f%%  reduction1 %.1f%%  update %.1f%%  reduction2 %.1f%%  rest %.1f%%" % tuple(
-            100 * x / lm.sum() for x in (mv.sum(), r1.sum(), up.sum(), r2.sum(), lm.sum() - mv.sum() - r1.sum() - up.sum() - r2.sum())))
         for lo, hi in ((49, 100), (101, 250), (251, 504), (505, 1000)):
             m = (sizes[cta] >= lo) & (sizes[cta] <= hi)
-            print("      nodes %4d-%4d per CG iteration: product %.0f  red1 %.0f  update %.0f  red2 %.0f" % (lo, hi, np.median((mv / np.maximum(cg, 1))[m]),
-                  np.median((r1 / np.maximum(cg, 1))[m]), np.median((up / np.maximum(cg, 1))[m]), np.median((r2 / np.maximum(cg, 1))[m])))
             if m.any():
                 print("      nodes %4d-%4d: n %5d  cycles/CG-iteration p50 %.0f  CG its/LM step p50 %.0f  LM its p50 %.0f  duration p50 %.2f ms" % (
                     lo, hi, int(m.sum()), np.median((lm / np.maximum(cg, 1))[m]), np.median((cg / its)[m]), np.median(its[m]), np.median(dur[cta][m])))
         idx = np.where(cta)[0]
         order = idx[np.argsort(-en[idx])[:5]]
         for k in order:
-            print("     slot %5d nodes %4d start %7.1f dur %7.1f end %7.1f  sm %3d  cg_iters %d  lm %d" % (
-                k, sizes[k], st[k], dur[k], en[k], int(cyc[k, 7]), int(cyc[k, 4]), int(cyc[k, 3])))
+            print("     slot %5d nodes %4d start %7.1f dur %7.1f end %7.1f  sm %3d  cg_iters %d" % (
+                k, sizes[k], st[k], dur[k], en[k], int(rec["smid"][k]), int(rec["counter"][k])))
         # concurrency: CTA-tier components running at a few instants
         for t in (5, 50, 100, 200, 300, 350, 400, 500):
             print("     t=%3d ms running %d" % (t, int(((st[cta] <= t) & (en[cta] > t)).sum())), end="")

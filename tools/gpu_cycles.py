@@ -1,15 +1,13 @@
-"""Per-component cycle breakdown of the solve kernel (LFR_PROFILE=1)."""
+"""Per-component cycle breakdown of the solve kernels (LFR_DBG_PROFILE)."""
 import os
 import sys
 
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, R)
-import ctypes as C  # noqa: E402
-
 import numpy as np  # noqa: E402
 
 from lfr_b200 import build_problem, synth  # noqa: E402
-from lfr_b200.capi import Plan, load_b200  # noqa: E402
+from lfr_b200.capi import PROFILE_TIERS, Plan, load_b200  # noqa: E402
 
 lib = load_b200()
 cfg = sys.argv[1] if len(sys.argv) > 1 else "cfg2"
@@ -28,22 +26,20 @@ e1.record()
 torch.cuda.synchronize()
 print("solve ms", e0.elapsed_time(e1), "launches", plan.num_launches())
 pos, st = plan.download()
-cyc = np.zeros((p.n_components, 8), dtype=np.uint64)
-lib.lib.lfr_debug_plan_cycles.argtypes = [C.c_void_p, C.c_void_p]
-assert lib.lib.lfr_debug_plan_cycles(plan.handle, cyc.ctypes.data) == 0
+rec, _ = plan.profile()
 it = st["iterations"]
 sel = it > 0
-tot = cyc[sel, 0].astype(np.float64)
+tot = rec["total"][sel].astype(np.float64)
 print("components", sel.sum(), "iters sum", it.sum())
 print("cycles per component: mean %.0f  p50 %.0f  p99 %.0f  max %.0f" % (
     tot.mean(), np.median(tot), np.percentile(tot, 99), tot.max()))
-names = ["total", "setup", "eval", "assemble", "lm_step", "ls+misc"]
-for k in range(6):
+names = ["total", "setup", "eval", "assemble", "solve", "rest"]
+for k in names:
     print("  %-9s sum %.3e  share %.1f%%  per-iter %.0f" % (
-        names[k], cyc[sel, k].sum(), 100.0 * cyc[sel, k].sum() / cyc[sel, 0].sum(),
-        cyc[sel, k].sum() / max(1, it[sel].sum())))
+        k, rec[k][sel].sum(), 100.0 * rec[k][sel].sum() / tot.sum(), rec[k][sel].sum() / max(1, it[sel].sum())))
 w = np.argsort(-tot)[:8]
 idx = np.nonzero(sel)[0][w]
 for i in idx:
-    print("  slot", i, "nodes", int(p.comp_ptr[i + 1] - p.comp_ptr[i]), "iters", it[i],
-          "ls_steps", int(cyc[i, 6]) >> 32, "cycles", cyc[i, :6].tolist(), "poly", int(cyc[i, 7]), "sm", int(cyc[i, 6]) & 0xffffffff)
+    print("  slot", i, "tier", PROFILE_TIERS.get(int(rec["tier"][i])), "nodes", int(p.comp_ptr[i + 1] - p.comp_ptr[i]),
+          "iters", it[i], "ls_steps", int(rec["ls_steps"][i]), "cycles", [int(rec[k][i]) for k in names],
+          "counter", int(rec["counter"][i]), "sm", int(rec["smid"][i]))

@@ -10,7 +10,7 @@ R = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, R)
 import torch  # noqa: E402
 from lfr_b200 import build_problem, synth  # noqa: E402
-from lfr_b200.capi import load_b200  # noqa: E402
+from lfr_b200.capi import load_b200, profile_record  # noqa: E402
 
 sys.path.insert(0, R)
 import bench  # noqa: E402
@@ -32,13 +32,14 @@ tm = np.zeros((p.n_components, 2), dtype=np.uint64)
 f = lib.lib.lfr_debug_last_solve_profile
 f.argtypes = [C.c_int, C.c_void_p, C.c_void_p]
 assert f(0, cyc.ctypes.data, tm.ctypes.data) == 0
+rec = profile_record(cyc)
 sel = tm[:, 0] > 0
 t0 = tm[sel, 0].min()
 start = (tm[:, 0].astype(np.float64) - t0) / 1e3
 end = (tm[:, 1].astype(np.float64) - t0) / 1e3
 sizes = np.diff(p.comp_ptr.astype(np.int64))
 print("components", int(sel.sum()), "span us: first start 0, last end %.1f" % end[sel].max())
-setup_us = cyc[:, 1].astype(np.float64) / 1965.0
+setup_us = rec["setup"].astype(np.float64) / 1965.0
 for lo, hi in ((2, 4), (5, 8), (9, 12), (13, 16), (17, 64)):
     m = sel & (sizes >= lo) & (sizes <= hi)
     if m.any():
@@ -47,4 +48,4 @@ for lo, hi in ((2, 4), (5, 8), (9, 12), (13, 16), (17, 64)):
             np.percentile(setup_us[m], 99), setup_us[m].max(), np.median(end[m]), end[m].max()))
 w = np.argsort(-end)[:6]
 for i in w:
-    print("  slot", int(i), "nodes", int(sizes[i]), "start %.1f setup %.1f end %.1f  total cycles %d" % (start[i], setup_us[i], end[i], int(cyc[i, 0])))
+    print("  slot", int(i), "nodes", int(sizes[i]), "start %.1f setup %.1f end %.1f  total cycles %d" % (start[i], setup_us[i], end[i], int(rec["total"][i])))
