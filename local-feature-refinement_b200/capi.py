@@ -13,7 +13,7 @@ from typing import Optional
 
 import numpy as np
 
-from .graph import EDGE_DTYPE, Problem
+from .graph import EDGE_DTYPE, HOST_SIZES_FIELDS, HostInput, HostSizes, Problem, host_input_arrays, stage_outputs
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 B200_LIB_PATH = os.path.join(HERE, "csrc", "liblfr_b200.so")
@@ -70,12 +70,14 @@ class LfrMultiInfo(C.Structure):
                 ("n_edges", C.c_uint64 * 16), ("zero_copy", C.c_int32), ("reserved", C.c_int32)]
 
 
-#: every symbol include/lfr.h declares
+#: every symbol include/lfr.h declares (include/lfr_graph.h adds GRAPH_SYMBOLS)
 ABI_SYMBOLS = [
     "lfr_abi_version", "lfr_backend", "lfr_last_error", "lfr_options_default", "lfr_solve", "lfr_solve_multi", "lfr_shutdown", "lfr_host_alloc", "lfr_host_free",
     "lfr_plan_create", "lfr_plan_solve", "lfr_plan_download", "lfr_plan_num_launches",
     "lfr_plan_traffic", "lfr_plan_destroy", "lfr_debug_edge_eval",
 ]
+#: the symbols include/lfr_graph.h declares
+GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_export_graph"]
 
 
 def _ptr(a: Optional[np.ndarray]) -> Optional[int]:
@@ -119,6 +121,12 @@ class Library:
         L.lfr_debug_edge_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                           C.POINTER(LfrOptions), C.c_void_p, C.c_void_p, C.c_void_p]
         L.lfr_debug_edge_eval.restype = C.c_int
+        if hasattr(L, "lfr_plan_create_from_matches"):  # include/lfr_graph.h
+            L.lfr_plan_create_from_matches.argtypes = [C.POINTER(HostInput), C.POINTER(LfrOptions), C.c_void_p,
+                                                       C.POINTER(C.c_void_p), C.POINTER(HostSizes)]
+            L.lfr_plan_create_from_matches.restype = C.c_int
+            L.lfr_plan_export_graph.argtypes = [C.c_void_p] * 11
+            L.lfr_plan_export_graph.restype = C.c_int
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -271,6 +279,7 @@ class Plan:
                  positions: Optional[np.ndarray] = None):
         self.lib = lib
         self.problem = p
+        self.n_nodes, self.n_components = p.graph.n_nodes, p.n_components
         s, keep = lib.marshal(p)
         o = options if options is not None else lib.default_options()
         init = None if positions is None else np.ascontiguousarray(positions, dtype=np.float64)
@@ -278,13 +287,59 @@ class Plan:
         lib.check(lib.lib.lfr_plan_create(C.byref(s), C.byref(o), _ptr(init), C.byref(h)), "lfr_plan_create")
         self.handle = h
 
+    @classmethod
+    def from_matches(cls, lib: Library, matches, banned_images=(), options: Optional[LfrOptions] = None,
+                     positions: Optional[np.ndarray] = None, n_images: Optional[int] = None) -> "Plan":
+        """lfr_plan_create_from_matches (include/lfr_graph.h): the graph stage runs on the device and the
+        problem stays there.  `matches` is a MatchSet or a dict of the flat lfr_host_input arrays
+        (pair_img1, pair_img2, pair_skip, pair_ptr, feat1, feat2, sim, disp1, disp2; n_images required).
+        `self.sizes` is the lfr_host_sizes of the stage as a dict."""
+        if isinstance(matches, dict):
+            arrs = {k: np.ascontiguousarray(v, dtype=dt) for k, (v, dt) in
+                    ((k, (matches[k], dt)) for k, dt in (("pair_img1", np.uint32), ("pair_img2", np.uint32),
+                                                         ("pair_skip", np.uint8), ("pair_ptr", np.uint64),
+                                                         ("feat1", np.uint32), ("feat2", np.uint32), ("sim", np.float32),
+                                                         ("disp1", np.float32), ("disp2", np.float32)))}
+            if n_images is None:
+                raise ValueError("n_images is required with flat arrays")
+        else:
+            _, arrs = host_input_arrays(matches, banned_images)
+            n_images = len(matches.image_names) if n_images is None else n_images
+        inp = HostInput(n_pairs=arrs["pair_img1"].shape[0], n_matches=arrs["feat1"].shape[0], n_images=n_images,
+                        edges_out=None, edges_out_capacity=0,
+                        **{k: (v.ctypes.data if v.size else None) for k, v in arrs.items()})
+        if not hasattr(lib.lib, "lfr_plan_create_from_matches"):  # e.g. the CPU oracle: no device, no plans
+            raise RuntimeError("lfr: lfr_plan_create_from_matches failed (-5): %s does not provide the graph stage "
+                               "on the GPU (include/lfr_graph.h)" % lib.path)
+        o = options if options is not None else lib.default_options()
+        init = None if positions is None else np.ascontiguousarray(positions, dtype=np.float64)
+        self = cls.__new__(cls)
+        self.lib, self.problem, self.handle = lib, None, None
+        h = C.c_void_p()
+        sz = HostSizes()
+        lib.check(lib.lib.lfr_plan_create_from_matches(C.byref(inp), C.byref(o), _ptr(init), C.byref(h), C.byref(sz)),
+                  "lfr_plan_create_from_matches")
+        self.handle = h
+        self.sizes = {k: getattr(sz, k) for k in HOST_SIZES_FIELDS}
+        self.n_nodes, self.n_components = int(sz.n_nodes), int(sz.n_components)
+        return self
+
+    def export_graph(self) -> dict:
+        """lfr_plan_export_graph: the stage's arrays of a plan made by from_matches(), named as in
+        lfr_host_stage_export (edges: [E] EDGE_DTYPE records, copied from the device)."""
+        out = stage_outputs(self.n_nodes, self.n_components, int(self.sizes["n_edges"]))
+        self.lib.check(self.lib.lib.lfr_plan_export_graph(self.handle, *[(a.ctypes.data if a.size else None)
+                                                                          for a in out.values()]),
+                       "lfr_plan_export_graph")
+        return out
+
     def solve(self, stream: int = 0) -> None:
         self.lib.check(self.lib.lib.lfr_plan_solve(self.handle, C.c_void_p(stream)), "lfr_plan_solve")
 
     def download(self, stream: int = 0):
-        N = self.problem.graph.n_nodes
+        N = self.n_nodes
         pos = np.zeros((N, 2), dtype=np.float64)
-        st, bufs = Library.make_stats(self.problem.n_components)
+        st, bufs = Library.make_stats(self.n_components)
         self.lib.check(self.lib.lib.lfr_plan_download(self.handle, C.c_void_p(stream), _ptr(pos), C.byref(st)),
                        "lfr_plan_download")
         return pos, Library.stats_dict(st, bufs)
@@ -292,7 +347,7 @@ class Plan:
     def profile(self):
         """Of the last solve of a plan created with LFR_DBG_PROFILE: the decoded cycle record of every slot
         (profile_record) and the [n, 2] %globaltimer ns at which each component's solve started / finished."""
-        n = self.problem.n_components
+        n = self.n_components
         cyc = np.zeros((n, 8), dtype=np.uint64)
         tm = np.zeros((n, 2), dtype=np.uint64)
         f, g = self.lib.lib.lfr_debug_plan_cycles, self.lib.lib.lfr_debug_plan_times

@@ -7,11 +7,15 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
 #include <vector>
 
+#include "../../include/lfr_graph.h"
+#include "lfr_cut.h"
+#include "lfr_graph.cuh"
 #include "lfr_solve_cta.cuh"
 #include "lfr_solve_tile.cuh"
 
@@ -205,6 +209,12 @@ struct lfr_plan {
   cudaStream_t streams[kMaxStreams] = {};
   cudaEvent_t ev_fork = nullptr, ev_join[kMaxStreams] = {};
   int n_streams = 0;
+  // a plan built from matches (lfr_plan_create_from_matches): the host copies of the stage's arrays
+  struct GraphArrays {
+    std::vector<uint32_t> row_ptr, track, comp, comp_ptr, comp_nodes, comp_order, node_image, node_feat;
+    std::vector<uint8_t> is_root;
+  };
+  std::unique_ptr<GraphArrays> graph;
 
   lfr::CtaArrays cta_arrays() const {
     lfr::CtaArrays A;
@@ -625,7 +635,7 @@ void* device_view_of_pinned(const void* host_ptr) {
 // — 95 % of the input bytes — are copied to HBM only if some non-staging tier needs them.
 int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const double* initial_positions,
               cudaStream_t s, bool stage_positions_directly = false, const float4* zc_edges = nullptr,
-              double* zc_positions = nullptr) {
+              double* zc_positions = nullptr, bool graph_resident = false) {
   pl->opt = o;
   pl->K = make_consts(o);
   pl->N = p->n_nodes;
@@ -635,8 +645,10 @@ int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const do
   pl->profile = (o.debug_flags & LFR_DBG_PROFILE) != 0;
   pl->zc_edges = zc_edges;
   pl->zc_positions = zc_positions;
-  pl->edges_in_hbm = false;
-  if (!zc_edges) {
+  // graph_resident: lfr_plan_create_from_matches() built the edge records and the six per-node / dispatch
+  // arrays in the plan's buffers already; only the host copies in `p` are read (by the schedule builder)
+  pl->edges_in_hbm = graph_resident;
+  if (!zc_edges && !graph_resident) {
     LFR_TRY(upload(&pl->edges, p->edges, (size_t)p->n_edges, s));  // the bulk first: the DMA runs while the host schedules
     pl->edges_in_hbm = true;
   }
@@ -650,12 +662,14 @@ int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const do
     LFR_CUDA(cudaEventRecord(pl->ev_small, s));          // orders s2's copies after whatever `s` ran before
     LFR_CUDA(cudaStreamWaitEvent(s2, pl->ev_small, 0));
   }
-  LFR_TRY(upload(&pl->row_ptr, p->row_ptr, (size_t)p->n_nodes + 1, s));
-  LFR_TRY(upload(&pl->track, p->track, (size_t)p->n_nodes, s2));
-  LFR_TRY(upload(&pl->comp, p->comp, (size_t)p->n_nodes, s2));
-  LFR_TRY(upload(&pl->is_root, p->is_root, (size_t)p->n_nodes, s2));
-  LFR_TRY(upload(&pl->comp_ptr, p->comp_ptr, (size_t)p->n_components + 1, s));
-  LFR_TRY(upload(&pl->comp_nodes, p->comp_nodes, (size_t)pl->total_slots, s));
+  if (!graph_resident) {
+    LFR_TRY(upload(&pl->row_ptr, p->row_ptr, (size_t)p->n_nodes + 1, s));
+    LFR_TRY(upload(&pl->track, p->track, (size_t)p->n_nodes, s2));
+    LFR_TRY(upload(&pl->comp, p->comp, (size_t)p->n_nodes, s2));
+    LFR_TRY(upload(&pl->is_root, p->is_root, (size_t)p->n_nodes, s2));
+    LFR_TRY(upload(&pl->comp_ptr, p->comp_ptr, (size_t)p->n_components + 1, s));
+    LFR_TRY(upload(&pl->comp_nodes, p->comp_nodes, (size_t)pl->total_slots, s));
+  }
   if (s2 != s) {
     LFR_CUDA(cudaEventRecord(pl->ev_small, s2));
     LFR_CUDA(cudaStreamWaitEvent(s, pl->ev_small, 0));
@@ -756,6 +770,534 @@ unsigned zero_copy_pull_window() {
     return 512u * 1024u;
   }();
   return w;
+}
+
+// ---- the graph stage on the device (include/lfr_graph.h, lfr_graph.cuh) ----------------------------
+struct TmpBuf : DevBuf {
+  ~TmpBuf() { release(); }
+};
+
+inline unsigned blocks_for(uint64_t n) { return (unsigned)((n + 255) / 256); }
+
+int bits_for(uint64_t max_value) {  // radix-sort key width that covers 0..max_value
+  int b = 1;
+  while (b < 64 && (max_value >> b)) ++b;
+  return b;
+}
+
+struct MaxOp {
+  __device__ __forceinline__ uint32_t operator()(uint32_t a, uint32_t b) const { return a > b ? a : b; }
+};
+
+// one CUB device call: size query, temporary storage, run
+template <typename F>
+int cub_run(DevBuf& tmp, F&& f) {
+  size_t bytes = 0;
+  LFR_CUDA(f(static_cast<void*>(nullptr), bytes));
+  LFR_TRY(tmp.reserve(std::max<size_t>(bytes, 1)));
+  LFR_CUDA(f(tmp.p, bytes));
+  return LFR_OK;
+}
+
+template <typename T>
+int fetch(T* h, const void* d, size_t count, cudaStream_t s) {
+  if (!count) return LFR_OK;
+  LFR_CUDA(cudaMemcpyAsync(h, d, count * sizeof(T), cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaStreamSynchronize(s));
+  return LFR_OK;
+}
+
+#define LFR_LAUNCHED() LFR_CUDA(cudaGetLastError())
+
+// Connected components of 0..n-1 over the edges (a[i], b[i]) (only those inside one group of `gc`
+// when given), labelled in order of their lowest member: label[n], returns the count in *n_out.
+int components_on_device(uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t m, const uint32_t* gc, uint32_t* label,
+                         uint32_t* n_out, DevBuf& tmp, cudaStream_t s) {
+  TmpBuf par, rep, lab;
+  LFR_TRY(par.reserve(4 * (size_t)n));
+  LFR_TRY(rep.reserve(4 * ((size_t)n + 1)));
+  LFR_TRY(lab.reserve(4 * ((size_t)n + 1)));
+  lfr::graph::iota_kernel<<<blocks_for(n), 256, 0, s>>>(par.as<uint32_t>(), n);
+  if (m) lfr::graph::cc_hook_kernel<<<blocks_for(m), 256, 0, s>>>(a, b, m, gc, par.as<uint32_t>());
+  lfr::graph::cc_flatten_kernel<<<blocks_for(n), 256, 0, s>>>(par.as<uint32_t>(), n, rep.as<uint32_t>());
+  LFR_LAUNCHED();
+  LFR_CUDA(cudaMemsetAsync(rep.as<uint32_t>() + n, 0, 4, s));
+  uint32_t* rp = rep.as<uint32_t>();
+  uint32_t* lp = lab.as<uint32_t>();
+  LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rp, lp, (int)n + 1, s); }));
+  lfr::graph::cc_label_kernel<<<blocks_for(n), 256, 0, s>>>(par.as<uint32_t>(), lp, n, label);
+  LFR_LAUNCHED();
+  return fetch(n_out, lp + n, 1, s);
+}
+
+using Clock = std::chrono::steady_clock;
+double ms_since(Clock::time_point t0) { return std::chrono::duration<double, std::milli>(Clock::now() - t0).count(); }
+
+// lfr_host_stage_create() on the device, block for block (lfr_host.cc): the edge records go into
+// pl->edges, the other arrays come back to pl->graph (the schedule builder is host code and reads them).
+int build_graph_on_device(const lfr_host_input* in, lfr_plan* pl, lfr_host_sizes* S, cudaStream_t s) {
+  using namespace lfr::graph;
+  std::memset(S, 0, sizeof *S);
+  auto G = std::make_unique<lfr_plan::GraphArrays>();
+  const uint64_t P = in->n_pairs, M_all = in->n_matches;
+  const uint32_t n_images = in->n_images;
+  TmpBuf tmp, d_img1, d_img2, d_skip, d_ptr, d_feat1, d_feat2, d_sim, d_disp1, d_disp2, d_cnt, d_off, d_seen, d_err;
+  const auto t_graph = Clock::now();
+  // ---- H1: the match list -------------------------------------------------------------------------
+  uint64_t M = 0;
+  if (P) {
+    LFR_TRY(upload(&d_img1, in->pair_img1, P, s));
+    LFR_TRY(upload(&d_img2, in->pair_img2, P, s));
+    if (in->pair_skip) LFR_TRY(upload(&d_skip, in->pair_skip, P, s));
+    LFR_TRY(upload(&d_ptr, in->pair_ptr, P + 1, s));
+    LFR_TRY(d_cnt.reserve(8 * (P + 1)));
+    LFR_TRY(d_off.reserve(8 * (P + 1)));
+    LFR_TRY(d_seen.reserve(std::max<size_t>(n_images, 1)));
+    LFR_TRY(d_err.reserve(8));
+    LFR_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8 * (P + 1), s));
+    LFR_CUDA(cudaMemsetAsync(d_seen.p, 0, std::max<size_t>(n_images, 1), s));
+    LFR_CUDA(cudaMemsetAsync(d_err.p, 0, 8, s));
+    pair_count_kernel<<<blocks_for(P), 256, 0, s>>>(d_img1.as<uint32_t>(), d_img2.as<uint32_t>(),
+                                                    in->pair_skip ? d_skip.as<uint8_t>() : nullptr, d_ptr.as<uint64_t>(), P,
+                                                    n_images, d_cnt.as<uint64_t>(), d_seen.as<uint8_t>(), d_err.as<int>());
+    LFR_LAUNCHED();
+    uint64_t* cp = d_cnt.as<uint64_t>();
+    uint64_t* op = d_off.as<uint64_t>();
+    if (P + 1 >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "more than 2^31 - 2 pairs");
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, cp, op, (int)(P + 1), s); }));
+    int err[2];
+    LFR_TRY(fetch(err, d_err.p, 2, s));
+    if (err[0]) return fail(LFR_EINVAL, "image id out of range");
+    LFR_TRY(fetch(&M, op + P, 1, s));
+    std::vector<uint8_t> seen(n_images);
+    LFR_TRY(fetch(seen.data(), d_seen.p, n_images, s));
+    for (uint8_t v : seen) S->n_images_seen += v;
+  }
+  if (2 * M >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "more than 2^31 - 1 directed edges");
+  const uint64_t E = 2 * M;
+  TmpBuf d_kept, d_key, d_key2, d_pos, d_pos2, d_first, d_id, d_head, d_headof, d_nop;
+  uint32_t N = 0;
+  if (M) {
+    LFR_TRY(upload(&d_feat1, in->feat1, M_all, s));
+    LFR_TRY(upload(&d_feat2, in->feat2, M_all, s));
+    LFR_TRY(upload(&d_sim, in->sim, M_all, s));
+    LFR_TRY(d_kept.reserve(8 * M));
+    LFR_TRY(d_key.reserve(8 * E));
+    LFR_TRY(d_key2.reserve(8 * E));
+    LFR_TRY(d_pos.reserve(4 * E));
+    LFR_TRY(d_pos2.reserve(4 * E));
+    expand_matches_kernel<<<blocks_for(M), 256, 0, s>>>(d_off.as<uint64_t>(), P, d_img1.as<uint32_t>(), d_img2.as<uint32_t>(),
+                                                        d_ptr.as<uint64_t>(), d_feat1.as<uint32_t>(), d_feat2.as<uint32_t>(),
+                                                        d_sim.as<float>(), M, d_kept.as<uint64_t>(),
+                                                        d_key.as<unsigned long long>(), d_pos.as<uint32_t>(), d_err.as<int>());
+    LFR_LAUNCHED();
+    int err[2];
+    LFR_TRY(fetch(err, d_err.p, 2, s));
+    if (err[1]) return fail(LFR_EINVAL, "non-finite similarity");
+    // (image, feature) -> node id in order of first appearance: stable sort of (key, position); the
+    // first position of every key gets the next id in position order
+    {
+      unsigned long long *k1 = d_key.as<unsigned long long>(), *k2 = d_key2.as<unsigned long long>();
+      uint32_t *p1 = d_pos.as<uint32_t>(), *p2 = d_pos2.as<uint32_t>();
+      const int end_bit = 32 + bits_for(n_images);
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+        return cub::DeviceRadixSort::SortPairs(t, nb, k1, k2, p1, p2, (int)E, 0, end_bit, s);
+      }));
+    }
+    LFR_TRY(d_first.reserve(4 * E));
+    LFR_TRY(d_id.reserve(4 * E));
+    LFR_TRY(d_head.reserve(4 * E));
+    LFR_TRY(d_headof.reserve(4 * E));
+    first_flags_kernel<<<blocks_for(E), 256, 0, s>>>(d_key2.as<unsigned long long>(), d_pos2.as<uint32_t>(), E,
+                                                     d_first.as<uint32_t>(), d_head.as<uint32_t>());
+    LFR_LAUNCHED();
+    {
+      uint32_t *f = d_first.as<uint32_t>(), *id = d_id.as<uint32_t>(), *h = d_head.as<uint32_t>(), *ho = d_headof.as<uint32_t>();
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, f, id, (int)E, s); }));
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::InclusiveScan(t, nb, h, ho, MaxOp(), (int)E, s); }));
+      uint32_t last[2];
+      LFR_TRY(fetch(&last[0], id + E - 1, 1, s));
+      LFR_TRY(fetch(&last[1], f + E - 1, 1, s));
+      N = last[0] + last[1];
+    }
+  }
+  pl->graph.reset();
+  if (N == 0) {
+    G->row_ptr.assign(1, 0);
+    G->comp_ptr.assign(1, 0);
+    pl->graph = std::move(G);
+    return LFR_OK;
+  }
+  if (n_images > 65535) return fail(LFR_EUNSUPPORTED, "more than 65535 images");
+  TmpBuf d_nimg, d_nfeat, d_ssrc, d_perm, d_cdst, d_csim;
+  // the six arrays fill_plan() would upload are built in the plan's own buffers and stay there
+  DevBuf &d_rowptr = pl->row_ptr, &d_track = pl->track, &d_isroot = pl->is_root, &d_comp = pl->comp,
+         &d_cptr = pl->comp_ptr, &d_cnodes = pl->comp_nodes;
+  LFR_TRY(d_nop.reserve(4 * E));
+  LFR_TRY(d_nimg.reserve(4 * (size_t)N));
+  LFR_TRY(d_nfeat.reserve(4 * (size_t)N));
+  assign_nodes_kernel<<<blocks_for(E), 256, 0, s>>>(d_key2.as<unsigned long long>(), d_pos2.as<uint32_t>(), d_headof.as<uint32_t>(),
+                                                    d_id.as<uint32_t>(), E, d_nop.as<uint32_t>(), d_nimg.as<uint32_t>(),
+                                                    d_nfeat.as<uint32_t>());
+  LFR_LAUNCHED();
+  // CSR: a stable sort of the directed edges (position j = 2k + side) by source keeps add_edge order
+  LFR_TRY(d_ssrc.reserve(4 * E));
+  LFR_TRY(d_perm.reserve(4 * E));
+  {
+    uint32_t* iota = d_pos.as<uint32_t>();
+    iota_kernel<<<blocks_for(E), 256, 0, s>>>(iota, E);
+    LFR_LAUNCHED();
+    uint32_t *src = d_nop.as<uint32_t>(), *ssrc = d_ssrc.as<uint32_t>(), *perm = d_perm.as<uint32_t>();
+    const int end_bit = bits_for(N);
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, src, ssrc, iota, perm, (int)E, 0, end_bit, s);
+    }));
+  }
+  LFR_TRY(d_rowptr.reserve(4 * ((size_t)N + 1)));
+  row_ptr_kernel<<<blocks_for(E), 256, 0, s>>>(d_ssrc.as<uint32_t>(), E, N, d_rowptr.as<uint32_t>());
+  LFR_TRY(upload(&d_disp1, in->disp1, 18 * M_all, s));
+  LFR_TRY(upload(&d_disp2, in->disp2, 18 * M_all, s));
+  LFR_TRY(pl->edges.reserve(sizeof(lfr_edge) * E));
+  LFR_TRY(d_cdst.reserve(4 * E));
+  LFR_TRY(d_csim.reserve(4 * E));
+  edge_records_kernel<<<blocks_for(E), 256, 0, s>>>(d_perm.as<uint32_t>(), E, d_kept.as<uint64_t>(), d_nop.as<uint32_t>(),
+                                                    d_sim.as<float>(), d_disp1.as<float>(), d_disp2.as<float>(),
+                                                    pl->edges.as<lfr_edge>(), d_cdst.as<uint32_t>(), d_csim.as<float>());
+  LFR_LAUNCHED();
+  d_disp1.release();
+  d_disp2.release();
+  LFR_CUDA(cudaStreamSynchronize(s));
+  S->graph_ms = ms_since(t_graph);
+  const auto t_tracks = Clock::now();
+  // ---- H2: constrained Kruskal: the sequential loop's order is descending (sim, n1, n2, k) ------------
+  TmpBuf d_order, d_parent, d_size, d_res, d_mask, d_lists, d_slot, d_pool, d_pool_next;
+  LFR_TRY(d_order.reserve(4 * M));
+  {
+    uint32_t *iota = d_pos.as<uint32_t>(), *n2k = d_first.as<uint32_t>(), *n2s = d_head.as<uint32_t>(), *perm1 = d_id.as<uint32_t>();
+    iota_kernel<<<blocks_for(M), 256, 0, s>>>(iota, M);
+    kruskal_keys_kernel<<<blocks_for(M), 256, 0, s>>>(d_nop.as<uint32_t>(), M, n2k);
+    LFR_LAUNCHED();
+    const int nb1 = bits_for(N);
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, n2k, n2s, iota, perm1, (int)M, 0, nb1, s);
+    }));
+    unsigned long long *k1 = d_key.as<unsigned long long>(), *k2 = d_key2.as<unsigned long long>();
+    kruskal_keys2_kernel<<<blocks_for(M), 256, 0, s>>>(perm1, d_kept.as<uint64_t>(), d_nop.as<uint32_t>(), d_sim.as<float>(), M, nb1, k1);
+    LFR_LAUNCHED();
+    uint32_t* ord = d_order.as<uint32_t>();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, k1, k2, perm1, ord, (int)M, 0, 32 + nb1, s);
+    }));
+  }
+  UfState U;
+  std::memset(&U, 0, sizeof U);
+  U.small_sets = n_images <= 64;
+  U.W = (n_images + 63) / 64;
+  LFR_TRY(d_parent.reserve(4 * (size_t)N));
+  LFR_TRY(d_size.reserve(4 * (size_t)N));
+  LFR_TRY(d_res.reserve(4 * (size_t)N));
+  U.parent = d_parent.as<int32_t>();
+  U.size = d_size.as<uint32_t>();
+  U.res = d_res.as<uint32_t>();
+  U.node_image = d_nimg.as<uint32_t>();
+  if (U.small_sets) {
+    LFR_TRY(d_mask.reserve(8 * (size_t)N));
+    U.mask = d_mask.as<unsigned long long>();
+  } else {
+    // a set crosses kListMax at most N / (kListMax + 1) times, and only then takes a bitset
+    const size_t slots = (size_t)N / (kListMax + 1) + 1;
+    LFR_TRY(d_lists.reserve(2 * kListMax * (size_t)N));
+    LFR_TRY(d_slot.reserve(4 * (size_t)N));
+    LFR_TRY(d_pool.reserve(8 * slots * U.W));
+    LFR_TRY(d_pool_next.reserve(4));
+    LFR_CUDA(cudaMemsetAsync(d_pool.p, 0, 8 * slots * U.W, s));
+    LFR_CUDA(cudaMemsetAsync(d_pool_next.p, 0, 4, s));
+    U.lists = d_lists.as<uint16_t>();
+    U.slot = d_slot.as<int32_t>();
+    U.pool = d_pool.as<unsigned long long>();
+    U.pool_next = d_pool_next.as<uint32_t>();
+  }
+  uf_init_kernel<<<blocks_for(N), 256, 0, s>>>(U, N);
+  LFR_LAUNCHED();
+  {
+    uint32_t w_max = 1u << 18;
+    if (const char* e = std::getenv("LFR_KRUSKAL_WINDOW")) w_max = (uint32_t)std::max(1l, std::atol(e));
+    w_max = (uint32_t)std::min<uint64_t>(w_max, M);
+    TmpBuf win[2], wr1, wr2, wst, keep, nsel;
+    LFR_TRY(win[0].reserve(4 * (size_t)w_max));
+    LFR_TRY(win[1].reserve(4 * (size_t)w_max));
+    LFR_TRY(wr1.reserve(4 * (size_t)w_max));
+    LFR_TRY(wr2.reserve(4 * (size_t)w_max));
+    LFR_TRY(wst.reserve(w_max));
+    LFR_TRY(keep.reserve(4 * (size_t)w_max));
+    LFR_TRY(nsel.reserve(4));
+    iota_kernel<<<blocks_for(w_max), 256, 0, s>>>(win[0].as<uint32_t>(), w_max);
+    LFR_LAUNCHED();
+    uint32_t n_win = w_max, next = w_max;
+    int cur = 0;
+    while (n_win) {
+      uint32_t* w = win[cur].as<uint32_t>();
+      uint32_t* w2 = win[1 - cur].as<uint32_t>();
+      kr_reserve_kernel<<<blocks_for(n_win), 256, 0, s>>>(U, w, n_win, d_order.as<uint32_t>(), (uint32_t)M, d_nop.as<uint32_t>(),
+                                                          wr1.as<uint32_t>(), wr2.as<uint32_t>(), wst.as<uint8_t>());
+      kr_decide_kernel<<<blocks_for(n_win), 256, 0, s>>>(U, w, n_win, wr1.as<uint32_t>(), wr2.as<uint32_t>(), wst.as<uint8_t>());
+      kr_release_kernel<<<blocks_for(n_win), 256, 0, s>>>(U, n_win, wr1.as<uint32_t>(), wr2.as<uint32_t>(), wst.as<uint8_t>(),
+                                                          keep.as<uint32_t>());
+      LFR_LAUNCHED();
+      uint32_t *kp = keep.as<uint32_t>(), *ns_d = nsel.as<uint32_t>();
+      const int nw = (int)n_win;
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, w, kp, w2, ns_d, nw, s); }));
+      uint32_t ns = 0;
+      LFR_TRY(fetch(&ns, ns_d, 1, s));
+      const uint32_t add = (uint32_t)std::min<uint64_t>(w_max - ns, M - next);
+      if (add) {
+        kr_refill_kernel<<<blocks_for(add), 256, 0, s>>>(w2, ns, add, next);
+        LFR_LAUNCHED();
+      }
+      next += add;
+      n_win = ns + add;
+      cur = 1 - cur;
+    }
+  }
+  // ---- H3: track ids (roots in node order) and roots ---------------------------------------------------
+  TmpBuf d_flag, d_tid, d_nit, d_score, d_best, d_bestnode, d_red;
+  uint32_t T = 0;
+  LFR_TRY(d_flag.reserve(4 * ((size_t)N + 1)));
+  LFR_TRY(d_tid.reserve(4 * ((size_t)N + 1)));
+  root_flags_kernel<<<blocks_for(N), 256, 0, s>>>(d_parent.as<int32_t>(), N, d_flag.as<uint32_t>());
+  LFR_LAUNCHED();
+  LFR_CUDA(cudaMemsetAsync(d_flag.as<uint32_t>() + N, 0, 4, s));
+  {
+    uint32_t *f = d_flag.as<uint32_t>(), *tid = d_tid.as<uint32_t>();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, f, tid, (int)N + 1, s); }));
+    LFR_TRY(fetch(&T, tid + N, 1, s));
+  }
+  LFR_TRY(d_track.reserve(4 * (size_t)N));
+  LFR_TRY(d_nit.reserve(4 * (size_t)T));
+  LFR_CUDA(cudaMemsetAsync(d_nit.p, 0, 4 * (size_t)T, s));
+  track_ids_kernel<<<blocks_for(N), 256, 0, s>>>(d_parent.as<int32_t>(), d_tid.as<uint32_t>(), N, d_track.as<uint32_t>(),
+                                                 d_nit.as<uint32_t>());
+  LFR_LAUNCHED();
+  LFR_TRY(d_red.reserve(8));
+  {
+    uint32_t *nit = d_nit.as<uint32_t>(), *out = d_red.as<uint32_t>();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceReduce::Reduce(t, nb, nit, out, (int)T, MaxOp(), 0u, s); }));
+    LFR_TRY(fetch(&S->max_track_size, out, 1, s));
+  }
+  LFR_TRY(d_score.reserve(8 * (size_t)N));
+  LFR_TRY(d_best.reserve(8 * (size_t)T));
+  LFR_TRY(d_bestnode.reserve(4 * (size_t)T));
+  LFR_TRY(d_isroot.reserve(N));
+  LFR_CUDA(cudaMemsetAsync(d_best.p, 0, 8 * (size_t)T, s));
+  LFR_CUDA(cudaMemsetAsync(d_bestnode.p, 0, 4 * (size_t)T, s));
+  LFR_CUDA(cudaMemsetAsync(d_isroot.p, 0, N, s));
+  root_score_kernel<<<blocks_for(N), 256, 0, s>>>(d_rowptr.as<uint32_t>(), d_cdst.as<uint32_t>(), d_csim.as<float>(),
+                                                  d_track.as<uint32_t>(), N, d_score.as<double>(), d_best.as<unsigned long long>());
+  root_pick_kernel<<<blocks_for(N), 256, 0, s>>>(d_score.as<double>(), d_best.as<unsigned long long>(), d_track.as<uint32_t>(), N,
+                                                 d_bestnode.as<uint32_t>());
+  root_mark_kernel<<<blocks_for(T), 256, 0, s>>>(d_bestnode.as<uint32_t>(), T, d_isroot.as<uint8_t>());
+  LFR_LAUNCHED();
+  LFR_CUDA(cudaStreamSynchronize(s));
+  S->tracks_ms = ms_since(t_tracks);
+  const auto t_cut = Clock::now();
+  // ---- H4: meta-graph: inter-track edges in CSR order, stable-sorted by (source, destination) track ----
+  d_parent.release();
+  d_size.release();
+  d_res.release();
+  d_mask.release();
+  d_lists.release();
+  d_pool.release();
+  TmpBuf d_mkey, d_inter, d_ikey, d_ikey2, d_isim, d_isim2, d_nint, d_seg, d_nseg, d_ma, d_mb, d_wsum;
+  uint32_t n_inter = 0, n_meta = 0;
+  LFR_TRY(d_mkey.reserve(8 * E));
+  LFR_TRY(d_inter.reserve(4 * E));
+  meta_keys_kernel<<<blocks_for(E), 256, 0, s>>>(d_ssrc.as<uint32_t>(), d_cdst.as<uint32_t>(), d_track.as<uint32_t>(), E, T,
+                                                 d_mkey.as<unsigned long long>(), d_inter.as<uint32_t>());
+  LFR_LAUNCHED();
+  LFR_TRY(d_ikey.reserve(8 * E));
+  LFR_TRY(d_isim.reserve(4 * E));
+  LFR_TRY(d_nint.reserve(4));
+  {
+    unsigned long long *mk = d_mkey.as<unsigned long long>(), *ik = d_ikey.as<unsigned long long>();
+    uint32_t *fl = d_inter.as<uint32_t>(), *cnt = d_nint.as<uint32_t>();
+    float *cs = d_csim.as<float>(), *is = d_isim.as<float>();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, mk, fl, ik, cnt, (int)E, s); }));
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, cs, fl, is, cnt, (int)E, s); }));
+    LFR_TRY(fetch(&n_inter, cnt, 1, s));
+  }
+  if (n_inter) {
+    LFR_TRY(d_ikey2.reserve(8 * (size_t)n_inter));
+    LFR_TRY(d_isim2.reserve(4 * (size_t)n_inter));
+    LFR_TRY(d_seg.reserve(4 * (size_t)n_inter));
+    LFR_TRY(d_nseg.reserve(4));
+    unsigned long long *ik = d_ikey.as<unsigned long long>(), *ik2 = d_ikey2.as<unsigned long long>();
+    float *is = d_isim.as<float>(), *is2 = d_isim2.as<float>();
+    const int end_bit = bits_for((uint64_t)T * T - 1);
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, ik, ik2, is, is2, (int)n_inter, 0, end_bit, s);
+    }));
+    uint32_t* head = d_inter.as<uint32_t>();  // reused
+    seg_heads_kernel<<<blocks_for(n_inter), 256, 0, s>>>(ik2, n_inter, head);
+    LFR_LAUNCHED();
+    uint32_t *seg = d_seg.as<uint32_t>(), *cnt = d_nseg.as<uint32_t>();
+    uint32_t* idx = d_pos.as<uint32_t>();  // 0, 1, ... (n_inter <= E)
+    iota_kernel<<<blocks_for(n_inter), 256, 0, s>>>(idx, n_inter);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, idx, head, seg, cnt, (int)n_inter, s); }));
+    LFR_TRY(fetch(&n_meta, cnt, 1, s));
+    LFR_TRY(d_ma.reserve(4 * (size_t)n_meta));
+    LFR_TRY(d_mb.reserve(4 * (size_t)n_meta));
+    LFR_TRY(d_wsum.reserve(8 * (size_t)n_meta));
+    meta_sum_kernel<<<blocks_for(n_meta), 256, 0, s>>>(ik2, is2, seg, n_meta, n_inter, T, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(),
+                                                       d_wsum.as<double>());
+    LFR_LAUNCHED();
+  }
+  // components of the meta-graph, the oversized ones cut on the host, the final components
+  TmpBuf d_cc, d_ccn, d_big, d_gc, d_fcc;
+  uint32_t n_cc = 0, n_final = 0;
+  LFR_TRY(d_cc.reserve(4 * (size_t)T));
+  LFR_TRY(components_on_device(T, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(), n_meta, nullptr, d_cc.as<uint32_t>(), &n_cc, tmp, s));
+  S->n_meta_components = n_cc;
+  LFR_TRY(d_ccn.reserve(8 * (size_t)n_cc));
+  LFR_TRY(d_big.reserve(4 * (size_t)n_cc));
+  LFR_CUDA(cudaMemsetAsync(d_ccn.p, 0, 8 * (size_t)n_cc, s));
+  cc_weight_kernel<<<blocks_for(T), 256, 0, s>>>(d_cc.as<uint32_t>(), d_nit.as<uint32_t>(), T, d_ccn.as<unsigned long long>());
+  oversized_kernel<<<blocks_for(n_cc), 256, 0, s>>>(d_ccn.as<unsigned long long>(), n_cc, S->n_images_seen, d_big.as<uint32_t>());
+  LFR_LAUNCHED();
+  {
+    uint32_t *big = d_big.as<uint32_t>(), *out = d_red.as<uint32_t>();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceReduce::Sum(t, nb, big, out, (int)n_cc, s); }));
+    LFR_TRY(fetch(&S->n_oversized_meta_components, out, 1, s));
+  }
+  LFR_TRY(d_gc.reserve(4 * (size_t)T));
+  LFR_CUDA(cudaMemcpyAsync(d_gc.p, d_cc.p, 4 * (size_t)T, cudaMemcpyDeviceToDevice, s));
+  if (S->n_oversized_meta_components) {
+    // the undirected edges of the oversized components, in meta-edge order, go to the host cut
+    TmpBuf d_cflag, d_cidx, d_ncut, d_recs, d_gidx, d_gval;
+    uint32_t n_cut = 0;
+    LFR_TRY(d_cflag.reserve(4 * (size_t)n_meta));
+    LFR_TRY(d_cidx.reserve(4 * (size_t)n_meta));
+    LFR_TRY(d_ncut.reserve(4));
+    cut_edges_flag_kernel<<<blocks_for(n_meta), 256, 0, s>>>(d_ma.as<uint32_t>(), d_mb.as<uint32_t>(), d_cc.as<uint32_t>(),
+                                                            d_big.as<uint32_t>(), n_meta, d_cflag.as<uint32_t>());
+    LFR_LAUNCHED();
+    uint32_t *fl = d_cflag.as<uint32_t>(), *ci = d_cidx.as<uint32_t>(), *cnt = d_ncut.as<uint32_t>();
+    uint32_t* idx = d_pos.as<uint32_t>();  // 0, 1, ... (n_meta <= E)
+    iota_kernel<<<blocks_for(n_meta), 256, 0, s>>>(idx, n_meta);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, idx, fl, ci, cnt, (int)n_meta, s); }));
+    LFR_TRY(fetch(&n_cut, cnt, 1, s));
+    LFR_TRY(d_recs.reserve(sizeof(CutRec) * std::max<size_t>(n_cut, 1)));
+    if (n_cut) {
+      cut_edges_gather_kernel<<<blocks_for(n_cut), 256, 0, s>>>(ci, n_cut, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(),
+                                                                d_wsum.as<double>(), d_cc.as<uint32_t>(), d_recs.as<CutRec>());
+      LFR_LAUNCHED();
+    }
+    std::vector<CutRec> recs(n_cut);
+    std::vector<uint32_t> node_weight(T);
+    LFR_TRY(fetch(recs.data(), d_recs.p, n_cut, s));
+    LFR_TRY(fetch(node_weight.data(), d_nit.p, T, s));
+    // one edge list per oversized component, components ascending (lfr_host.cc's per_cc)
+    std::vector<uint32_t> comps;
+    for (const CutRec& r : recs) comps.push_back(r.comp);
+    std::sort(comps.begin(), comps.end());
+    comps.erase(std::unique(comps.begin(), comps.end()), comps.end());
+    std::vector<std::vector<lfr::CutEdge>> per_cc(comps.size());
+    for (const CutRec& r : recs) {
+      const size_t sl = (size_t)(std::lower_bound(comps.begin(), comps.end(), r.comp) - comps.begin());
+      per_cc[sl].push_back(lfr::CutEdge{r.a, r.b, lfr::cut_weight(r.wsum)});
+    }
+    std::vector<std::vector<uint32_t>> groups;
+    lfr::recursive_cut_all(std::move(per_cc), node_weight, S->n_images_seen, &groups);
+    std::vector<uint32_t> gidx, gval;
+    for (size_t g = 0; g < groups.size(); ++g)
+      for (uint32_t t : groups[g]) {
+        gidx.push_back(t);
+        gval.push_back(n_cc + (uint32_t)g);
+      }
+    S->n_cut_groups = (uint32_t)groups.size();
+    if (!gidx.empty()) {
+      LFR_TRY(upload(&d_gidx, gidx.data(), gidx.size(), s));
+      LFR_TRY(upload(&d_gval, gval.data(), gval.size(), s));
+      scatter_kernel<<<blocks_for(gidx.size()), 256, 0, s>>>(d_gidx.as<uint32_t>(), d_gval.as<uint32_t>(), (uint32_t)gidx.size(),
+                                                             d_gc.as<uint32_t>());
+      LFR_LAUNCHED();
+    }
+    LFR_CUDA(cudaStreamSynchronize(s));  // the uploads above read host vectors that end with this scope
+  }
+  LFR_TRY(d_fcc.reserve(4 * (size_t)T));
+  LFR_TRY(components_on_device(T, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(), n_meta, d_gc.as<uint32_t>(), d_fcc.as<uint32_t>(),
+                               &n_final, tmp, s));
+  LFR_TRY(d_comp.reserve(4 * (size_t)N));
+  gather_kernel<<<blocks_for(N), 256, 0, s>>>(d_track.as<uint32_t>(), d_fcc.as<uint32_t>(), N, d_comp.as<uint32_t>());
+  LFR_LAUNCHED();
+  LFR_CUDA(cudaStreamSynchronize(s));
+  S->graph_cut_ms = ms_since(t_cut);
+  const auto t_disp = Clock::now();
+  // ---- H5: dispatch list: slots by (size desc, id desc), nodes ascending inside a slot ----------------
+  const uint32_t C = n_final;
+  TmpBuf d_csize, d_ckey, d_ckey2, d_corder, d_slotof, d_ssize, d_nslot, d_nslot2, d_iota;
+  LFR_TRY(d_csize.reserve(4 * (size_t)C));
+  LFR_TRY(d_ckey.reserve(8 * (size_t)C));
+  LFR_TRY(d_ckey2.reserve(8 * (size_t)C));
+  LFR_TRY(d_corder.reserve(4 * (size_t)C));
+  LFR_TRY(d_slotof.reserve(4 * (size_t)C));
+  LFR_TRY(d_ssize.reserve(4 * ((size_t)C + 1)));
+  LFR_TRY(d_cptr.reserve(4 * ((size_t)C + 1)));
+  LFR_CUDA(cudaMemsetAsync(d_csize.p, 0, 4 * (size_t)C, s));
+  LFR_CUDA(cudaMemsetAsync(d_ssize.p, 0, 4 * ((size_t)C + 1), s));
+  comp_size_kernel<<<blocks_for(N), 256, 0, s>>>(d_comp.as<uint32_t>(), N, d_csize.as<uint32_t>());
+  comp_keys_kernel<<<blocks_for(C), 256, 0, s>>>(d_csize.as<uint32_t>(), C, d_ckey.as<unsigned long long>());
+  LFR_LAUNCHED();
+  {
+    unsigned long long *k1 = d_ckey.as<unsigned long long>(), *k2 = d_ckey2.as<unsigned long long>();
+    const int end_bit = 32 + bits_for(N);
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceRadixSort::SortKeysDescending(t, nb, k1, k2, (int)C, 0, end_bit, s); }));
+    comp_slots_kernel<<<blocks_for(C), 256, 0, s>>>(k2, C, d_corder.as<uint32_t>(), d_slotof.as<uint32_t>(), d_ssize.as<uint32_t>());
+    LFR_LAUNCHED();
+    uint32_t *ss = d_ssize.as<uint32_t>(), *cp = d_cptr.as<uint32_t>();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, ss, cp, (int)C + 1, s); }));
+  }
+  LFR_TRY(d_nslot.reserve(4 * (size_t)N));
+  LFR_TRY(d_nslot2.reserve(4 * (size_t)N));
+  LFR_TRY(d_cnodes.reserve(4 * (size_t)N));
+  LFR_TRY(d_iota.reserve(4 * (size_t)N));
+  node_slot_kernel<<<blocks_for(N), 256, 0, s>>>(d_comp.as<uint32_t>(), d_slotof.as<uint32_t>(), N, d_nslot.as<uint32_t>());
+  iota_kernel<<<blocks_for(N), 256, 0, s>>>(d_iota.as<uint32_t>(), N);
+  LFR_LAUNCHED();
+  {
+    uint32_t *k1 = d_nslot.as<uint32_t>(), *k2 = d_nslot2.as<uint32_t>(), *v1 = d_iota.as<uint32_t>(), *v2 = d_cnodes.as<uint32_t>();
+    const int end_bit = bits_for(C);
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceRadixSort::SortPairs(t, nb, k1, k2, v1, v2, (int)N, 0, end_bit, s); }));
+  }
+  // the per-node arrays to the host: the schedule builder and lfr_plan_export_graph() read them
+  G->row_ptr.resize((size_t)N + 1);
+  G->track.resize(N);
+  G->comp.resize(N);
+  G->is_root.resize(N);
+  G->comp_ptr.resize((size_t)C + 1);
+  G->comp_nodes.resize(N);
+  G->comp_order.resize(C);
+  G->node_image.resize(N);
+  G->node_feat.resize(N);
+  LFR_CUDA(cudaMemcpyAsync(G->row_ptr.data(), d_rowptr.p, 4 * ((size_t)N + 1), cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->track.data(), d_track.p, 4 * (size_t)N, cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->comp.data(), d_comp.p, 4 * (size_t)N, cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->is_root.data(), d_isroot.p, N, cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->comp_ptr.data(), d_cptr.p, 4 * ((size_t)C + 1), cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->comp_nodes.data(), d_cnodes.p, 4 * (size_t)N, cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->comp_order.data(), d_corder.p, 4 * (size_t)C, cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->node_image.data(), d_nimg.p, 4 * (size_t)N, cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaMemcpyAsync(G->node_feat.data(), d_nfeat.p, 4 * (size_t)N, cudaMemcpyDeviceToHost, s));
+  LFR_CUDA(cudaStreamSynchronize(s));
+  S->dispatch_ms = ms_since(t_disp);
+  S->n_nodes = N;
+  S->n_edges = E;
+  S->n_tracks = T;
+  S->n_components = C;
+  S->max_component_size = C ? G->comp_ptr[1] - G->comp_ptr[0] : 0;
+  pl->graph = std::move(G);
+  return LFR_OK;
 }
 
 int set_kernel_attrs() {
@@ -1073,6 +1615,70 @@ int lfr_plan_create(const lfr_problem* p, const lfr_options* opt, const double* 
     return rc;
   }
   *out = pl;
+  return LFR_OK;
+}
+
+int lfr_plan_create_from_matches(const lfr_host_input* in, const lfr_options* opt, const double* initial_positions,
+                                 lfr_plan** out, lfr_host_sizes* sizes) {
+  if (!out) return fail(LFR_EINVAL, "out is NULL");
+  *out = nullptr;
+  if (!in) return fail(LFR_EINVAL, "input is NULL");
+  lfr_options o;
+  if (opt) o = *opt; else lfr_options_default(&o);
+  LFR_TRY(select_device(o));
+  lfr_plan* pl = new lfr_plan();
+  pl->device = o.device;
+  lfr_host_sizes S;
+  int rc = build_graph_on_device(in, pl, &S, 0);
+  if (rc == LFR_OK) {
+    const lfr_plan::GraphArrays& G = *pl->graph;
+    lfr_problem p;
+    p.n_nodes = S.n_nodes;
+    p.n_components = S.n_components;
+    p.n_edges = S.n_edges;
+    p.row_ptr = G.row_ptr.data();
+    p.edges = nullptr;  // already in pl->edges
+    p.track = G.track.data();
+    p.comp = G.comp.data();
+    p.is_root = G.is_root.data();
+    p.comp_ptr = G.comp_ptr.data();
+    p.comp_nodes = G.comp_nodes.data();
+    rc = fill_plan(pl, &p, o, initial_positions, 0, false, nullptr, nullptr, /*graph_resident=*/true);
+  }
+  if (rc == LFR_OK) {
+    cudaError_t e = cudaStreamSynchronize(0);
+    if (e != cudaSuccess) rc = fail(cuda_code(e), cudaGetErrorString(e));
+  }
+  if (rc) {
+    free_plan(pl);
+    return rc;
+  }
+  if (sizes) *sizes = S;
+  *out = pl;
+  return LFR_OK;
+}
+
+int lfr_plan_export_graph(const lfr_plan* pl, uint32_t* row_ptr, lfr_edge* edges, uint32_t* track, uint32_t* comp,
+                          uint8_t* is_root, uint32_t* comp_ptr, uint32_t* comp_nodes, uint32_t* comp_order,
+                          uint32_t* node_image, uint32_t* node_feat) {
+  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
+  const lfr_plan::GraphArrays& G = *pl->graph;
+  auto cp = [](void* dst, const void* src, size_t bytes) {
+    if (dst && bytes) std::memcpy(dst, src, bytes);
+  };
+  cp(row_ptr, G.row_ptr.data(), G.row_ptr.size() * 4);
+  cp(track, G.track.data(), G.track.size() * 4);
+  cp(comp, G.comp.data(), G.comp.size() * 4);
+  cp(is_root, G.is_root.data(), G.is_root.size());
+  cp(comp_ptr, G.comp_ptr.data(), G.comp_ptr.size() * 4);
+  cp(comp_nodes, G.comp_nodes.data(), G.comp_nodes.size() * 4);
+  cp(comp_order, G.comp_order.data(), G.comp_order.size() * 4);
+  cp(node_image, G.node_image.data(), G.node_image.size() * 4);
+  cp(node_feat, G.node_feat.data(), G.node_feat.size() * 4);
+  if (edges && pl->E) {
+    LFR_CUDA(cudaSetDevice(pl->device));
+    LFR_CUDA(cudaMemcpy(edges, pl->edges.p, sizeof(lfr_edge) * (size_t)pl->E, cudaMemcpyDeviceToHost));
+  }
   return LFR_OK;
 }
 

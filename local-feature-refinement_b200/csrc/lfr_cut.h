@@ -8,7 +8,9 @@
 // quantity a normalized cut normalises by.  One definition, used by the product host stage
 // (lfr_host.cc), by its numpy twin (graph.py::two_way_cut, checked to agree) and by the COLMAP
 // shim behind which the reference's own solve.cc is compiled as a checker
-// (oracle/ref_shims/colmap/base/graph_cut.h).
+// (oracle/ref_shims/colmap/base/graph_cut.h).  The recursive cut built on it (cut_step,
+// recursive_cut_all, at the end of this file) is shared by the host stage and the graph stage on the
+// GPU (lfr_capi.cu), so both split oversized meta-components with the same code.
 //
 // Algorithm (all ties broken by ascending node id, so the result is unique):
 //   1. adjacency with parallel edges merged, neighbours ascending; vol(x) = sum of incident weights
@@ -21,7 +23,11 @@
 //      that lowers the cut and does not empty its side.
 #pragma once
 #include <algorithm>
+#include <condition_variable>
 #include <cstdint>
+#include <cstdlib>
+#include <mutex>
+#include <thread>
 #include <utility>
 #include <vector>
 
@@ -31,6 +37,16 @@ struct CutEdge {
   uint32_t a, b;
   int64_t w;
 };
+
+// The weight of an undirected meta-edge: static_cast<int>(100 * sum of similarities) (solve.cc:329).
+// Out of int range that cast is undefined in C++; here it saturates at INT_MIN / INT_MAX (truncation
+// toward zero inside), so the host stage and the graph stage on the GPU agree on every finite input.
+inline int64_t cut_weight(double sim_sum) {
+  const double x = 100.0 * sim_sum;
+  if (x >= 2147483647.0) return 2147483647;
+  if (x <= -2147483648.0) return -2147483647 - 1;
+  return (int64_t)(int)x;
+}
 
 struct CutWorkspace {
   std::vector<int32_t> local;  // node id -> index in `nodes` (-1 outside a call); grown on demand
@@ -175,6 +191,136 @@ inline void two_way_cut(const CutEdge* edges, size_t m, CutWorkspace& W) {
 
 inline void cut_release(CutWorkspace& W) {
   for (uint32_t g : W.nodes) W.local[g] = -1;
+}
+
+// graph.py::recursive_cut (solve.cc:185-250 as a work list): split until every group weighs
+// <= max_weight (node weight = nodes of the track, solve.cc:198) or has no internal edge (then its
+// nodes become singleton groups, solve.cc:240-246).  The 2-way cut itself is lfr_cut.h.
+// One step: cut `edges`, emit the finished groups, return the edge lists of the two sides that
+// have to be cut again (empty when done).  A pure function of `edges` (in their order).
+inline void cut_step(const std::vector<CutEdge>& edges, const std::vector<uint32_t>& node_weight, uint32_t max_weight,
+              CutWorkspace& W, std::vector<uint8_t>& covered, std::vector<std::vector<uint32_t>>* groups,
+              std::vector<CutEdge> (&sub)[2]) {
+  // a third of all sub-problems are two tracks joined by (parallel) edges: whatever their weights, each
+  // side of the cut is one node with no edge inside — two singleton groups (solve.cc:205-211 / :240-246)
+  {
+    const uint32_t a = edges[0].a, b = edges[0].b;
+    bool two_nodes = a != b;
+    for (size_t i = 1; two_nodes && i < edges.size(); ++i)
+      two_nodes = (edges[i].a == a && edges[i].b == b) || (edges[i].a == b && edges[i].b == a);
+    if (two_nodes) {
+      sub[0].clear();
+      sub[1].clear();
+      groups->push_back(std::vector<uint32_t>(1, a));
+      groups->push_back(std::vector<uint32_t>(1, b));
+      return;
+    }
+  }
+  two_way_cut(edges.data(), edges.size(), W);
+  const uint32_t n = (uint32_t)W.nodes.size();
+  for (int s = 0; s < 2; ++s) {
+    sub[s].clear();
+    std::vector<uint32_t> members;
+    int64_t w = 0;
+    for (uint32_t i = 0; i < n; ++i)
+      if (W.side[i] == s) {
+        members.push_back(W.nodes[i]);  // ascending
+        w += node_weight[W.nodes[i]];
+      }
+    if (members.empty()) continue;
+    if (w <= (int64_t)max_weight) {
+      groups->push_back(std::move(members));  // solve.cc:205-211
+      continue;
+    }
+    covered.assign(n, 0);
+    for (const CutEdge& e : edges) {
+      const int32_t la = W.local[e.a], lb = W.local[e.b];
+      if (W.side[la] == s && W.side[lb] == s) {
+        sub[s].push_back(e);
+        covered[la] = 1;
+        covered[lb] = 1;
+      }
+    }
+    for (uint32_t x : members)  // no edge left inside the subset: singleton groups
+      if (!covered[W.local[x]]) groups->push_back(std::vector<uint32_t>(1, x));
+  }
+  cut_release(W);
+}
+
+// All oversized meta-components, cut down to groups.  The groups form a partition that does not
+// depend on the order in which the sub-problems are processed (each cut is a function of its own edge
+// list only), so the work list is shared by a few threads; only membership is used afterwards.
+inline void recursive_cut_all(std::vector<std::vector<CutEdge>> roots, const std::vector<uint32_t>& node_weight,
+                       uint32_t max_weight, std::vector<std::vector<uint32_t>>* groups) {
+  uint64_t total_edges = 0;
+  for (const auto& r : roots) total_edges += r.size();
+  unsigned n_thr = 1;
+  if (total_edges >= 2048) {
+    const unsigned hw = std::thread::hardware_concurrency();
+    n_thr = std::min(8u, hw ? hw : 1u);
+  }
+  if (const char* e = std::getenv("LFR_HOST_THREADS")) n_thr = (unsigned)std::max(1, std::min(64, std::atoi(e)));
+  std::vector<std::vector<CutEdge>> work;
+  for (auto it = roots.rbegin(); it != roots.rend(); ++it) work.push_back(std::move(*it));
+  if (n_thr <= 1) {
+    CutWorkspace W;
+    std::vector<uint8_t> covered;
+    std::vector<CutEdge> sub[2];
+    while (!work.empty()) {
+      const std::vector<CutEdge> edges = std::move(work.back());
+      work.pop_back();
+      cut_step(edges, node_weight, max_weight, W, covered, groups, sub);
+      if (!sub[1].empty()) work.push_back(std::move(sub[1]));
+      if (!sub[0].empty()) work.push_back(std::move(sub[0]));
+    }
+    return;
+  }
+  // shared list: sub-problems of at least kShare edges (a handful per scene: the top of each recursion
+  // tree); anything smaller is finished by the thread that produced it, on its own stack
+  constexpr size_t kShare = 1024;
+  std::mutex mu;
+  std::condition_variable cv;
+  unsigned active = 0;
+  std::vector<std::vector<std::vector<uint32_t>>> found(n_thr);
+  auto worker = [&](unsigned t) {
+    CutWorkspace W;
+    std::vector<uint8_t> covered;
+    std::vector<CutEdge> sub[2];
+    std::vector<std::vector<CutEdge>> mine;
+    std::unique_lock<std::mutex> lk(mu);
+    for (;;) {
+      cv.wait(lk, [&] { return !work.empty() || active == 0; });
+      if (work.empty()) return;  // and nobody is producing more
+      mine.push_back(std::move(work.back()));
+      work.pop_back();
+      ++active;
+      lk.unlock();
+      while (!mine.empty()) {
+        const std::vector<CutEdge> edges = std::move(mine.back());
+        mine.pop_back();
+        cut_step(edges, node_weight, max_weight, W, covered, &found[t], sub);
+        for (int sd = 1; sd >= 0; --sd) {
+          if (sub[sd].empty()) continue;
+          if (sub[sd].size() >= kShare) {
+            std::lock_guard<std::mutex> g(mu);
+            work.push_back(std::move(sub[sd]));
+            cv.notify_one();
+          } else {
+            mine.push_back(std::move(sub[sd]));
+          }
+        }
+      }
+      lk.lock();
+      --active;
+      cv.notify_all();
+    }
+  };
+  std::vector<std::thread> helpers;
+  for (unsigned t = 1; t < n_thr; ++t) helpers.emplace_back(worker, t);
+  worker(0);
+  for (std::thread& h : helpers) h.join();
+  for (auto& f : found)
+    for (auto& g : f) groups->push_back(std::move(g));
 }
 
 }  // namespace lfr
