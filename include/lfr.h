@@ -120,12 +120,11 @@ typedef struct lfr_options {
   int32_t debug_flags;   /* LFR_DBG_* test / profiling hooks; 0 in production      */
 } lfr_options;
 
-/* lfr_options.debug_flags (b200 only): route components through the fallback tiers, switch the
- * staging / zero-copy mechanisms off, collect per-component cycle counters.  Results do not
+/* lfr_options.debug_flags (b200 only): route components through the fallback tiers, switch
+ * zero-copy off or on, collect per-component cycle counters.  Results do not
  * depend on them (tests/test_gpu_parity.py). */
 #define LFR_DBG_FORCE_SMEM_CHOLESKY 0x1 /* every warp-tier component through the shared-memory Cholesky kernel */
 #define LFR_DBG_NO_TILE 0x2             /* no 64/128-thread tile kernels                                       */
-#define LFR_DBG_STAGE_LDG 0x4           /* stage edge records with LDG -> STS instead of TMA bulk copies       */
 #define LFR_DBG_NO_ZERO_COPY 0x8        /* lfr_solve_multi(): copy edges / positions through HBM even when the caller's buffers are pinned */
 #define LFR_DBG_PROFILE 0x10            /* per-component clock64() counters (lfr_debug_plan_cycles)            */
 #define LFR_DBG_ZERO_COPY 0x20          /* lfr_solve(): use pinned caller buffers in place, as lfr_solve_multi() does */

@@ -18,6 +18,8 @@
 #include "lfr_graph.cuh"
 #include "lfr_solve_cta.cuh"
 #include "lfr_solve_tile.cuh"
+#include "lfr_solve_warp.cuh"
+#include "lfr_solve_warp2.cuh"
 
 namespace {
 
@@ -133,7 +135,9 @@ struct Bucket {
   uint32_t offset = 0;  // into the bucket-list buffer
   uint32_t n = 0;
   int emax = 0, ncmax = 0, n2max = 0, smem_per_warp = 0, warps = 4;
-  int variant = 0;  // 0: shared-memory Cholesky kernel (n <= 64); 16 / 32: register Gauss-Jordan kernel (n <= variant)
+  // 0: shared-memory Cholesky warp kernel (80 < n <= 96, and components whose staged records do not
+  // fit); 8..32: register Gauss-Jordan warp kernel (n <= variant); 132, 48, 64, 80: tile kernels
+  int variant = 0;
   bool stages_edges() const { return variant != 0; }  // warp2 / tile tiers pull their edge records into shared memory
 };
 
@@ -145,8 +149,9 @@ int validate(const lfr_problem* p) {
   if (p->n_nodes && p->row_ptr[p->n_nodes] != p->n_edges) return fail(LFR_EINVAL, "row_ptr[n_nodes] != n_edges");
   if (p->n_edges && !p->edges) return fail(LFR_EINVAL, "edges is NULL");
   if (p->n_edges >= (1ull << 32)) return fail(LFR_EUNSUPPORTED, "more than 2^32 directed edges");
-  // per-edge checks (dst range, self edges) run on the device while the edges are
-  // staged (solve_warp_kernel), so the host never walks the 80-byte records.
+  // the per-edge checks (dst range, self edges, a component node list that disagrees with `comp`)
+  // run on the device as every tier classifies its edges (classify_edge), so the host never walks the
+  // 80-byte records.
   return LFR_OK;
 }
 
@@ -254,7 +259,6 @@ struct lfr_plan {
     P.local_of = local_of.as<uint32_t>();
     P.positions = pos.as<double>();
     P.positions_out = zc_positions ? zc_positions : pos.as<double>();
-    P.stage_mode = (opt.debug_flags & LFR_DBG_STAGE_LDG) ? 0 : 1;
     P.pull_ctr = d_pull();
     P.pull_window = 0;  // set by launch_solve for zero-copy staging only
     P.st_iter = d_iter();
@@ -1448,7 +1452,9 @@ int download(lfr_plan* pl, cudaStream_t s, double* positions, lfr_stats* st) {
   // the error flag is checked BEFORE anything is copied into the caller's position array (with
   // zero-copy write-back the components that did solve have already been written: on LFR_EINVAL
   // the array holds a mixture of start values and results)
-  if (err) return fail(LFR_EINVAL, "edge with dst out of range or a self edge (found while staging edges on the device)");
+  if (err)
+    return fail(LFR_EINVAL, "edge with dst out of range, a self edge, or a component node list (comp_nodes) that "
+                            "disagrees with comp (found while classifying edges on the device)");
   if (positions && pl->N && !pl->zc_positions) {
     LFR_CUDA(cudaMemcpyAsync(positions, pl->pos.p, sizeof(double) * 2 * (size_t)pl->N, cudaMemcpyDeviceToHost, s));
     LFR_CUDA(cudaStreamSynchronize(s));

@@ -30,7 +30,8 @@ namespace lfr {
 
 struct DevProblem {
   uint32_t n_nodes;
-  int* err_flag;  // set when a malformed edge (dst out of range, self edge) is met
+  int* err_flag;  // set by classify_edge on malformed input: a dst out of range, a self edge, or a
+                  // component node list that disagrees with `comp`
   const uint32_t* row_ptr;
   const float4* edges;  // 5 x float4 per edge
   const uint32_t* track;
@@ -44,8 +45,6 @@ struct DevProblem {
                              // (zero-copy write-back: only free nodes are written, solve.cc:131-141)
   unsigned long long* pull_ctr;  // [2] bytes of staging pulls {ticketed, arrived} (zero-copy pacing, see stage_edges)
   unsigned pull_window;      // 0 = unpaced; else at most this many bytes of staging pulls are outstanding per device
-  int stage_mode;            // how the staging tiers pull a component's edge records into shared memory:
-                             // 1 = TMA 1-D bulk copies (cp.async.bulk + mbarrier), 0 = LDG -> STS
   // per dispatch slot
   int32_t* st_iter;
   int32_t* st_term;

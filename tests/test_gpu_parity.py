@@ -166,25 +166,24 @@ def test_fallback_tiers_match_oracle(b200, oracle, flags, cfg):
 
 
 @pytest.mark.parametrize("cfg", ["cfg2", "cfg4", "ring60"])
-def test_staging_and_zero_copy_variants_are_bitwise_identical(b200, oracle, cfg):
+def test_pinned_and_zero_copy_solves_are_bitwise_identical(b200, oracle, cfg):
     """The same solve with (a) TMA bulk staging from the caller's pinned buffers (zero-copy: edge
     records pulled over PCIe straight into shared memory, results written straight back), (b) the
-    same through HBM, (c) LDG -> STS staging: identical bits, all equal to the oracle to 1e-4 px.
+    same through HBM, from pageable and from pinned buffers: identical bits, all equal to the oracle
+    to 1e-4 px.
     ring60 adds the CTA tier: its preparation kernel copies the kept records out of the pinned array."""
     import ctypes as C
     import torch
     from lfr_b200 import capi
     _, p = get_problem(cfg)
     pos_ref, st_ref = _compare_dbg(b200, oracle, p, capi.DBG_NO_ZERO_COPY)
-    pos_ldg, st_ldg = b200.solve(p, b200.default_options(debug_flags=capi.DBG_NO_ZERO_COPY | capi.DBG_STAGE_LDG))
-    assert np.array_equal(pos_ref, pos_ldg) and np.array_equal(st_ref["iterations"], st_ldg["iterations"])
     # pinned caller buffers: through the copy engine (default) and in place (zero-copy)
     s, keep = b200.marshal(p)
     e_pin = torch.empty(keep["edges"].nbytes, dtype=torch.uint8).pin_memory()
     e_pin.numpy()[:] = keep["edges"].view(np.uint8).reshape(-1)
     s.edges = e_pin.data_ptr()
     N = p.graph.n_nodes
-    for dbg in (0, capi.DBG_STAGE_LDG, capi.DBG_ZERO_COPY, capi.DBG_ZERO_COPY | capi.DBG_STAGE_LDG):
+    for dbg in (0, capi.DBG_ZERO_COPY):
         pos_pin = torch.zeros(2 * N, dtype=torch.float64).pin_memory()
         st, bufs = b200.make_stats(p.n_components)
         o = b200.default_options(debug_flags=dbg)
@@ -193,6 +192,53 @@ def test_staging_and_zero_copy_variants_are_bitwise_identical(b200, oracle, cfg)
         assert np.array_equal(pos_pin.numpy().reshape(N, 2), pos_ref), dbg
         assert np.array_equal(bufs["iterations"], st_ref["iterations"])
         assert np.array_equal(bufs["termination"], st_ref["termination"])
+
+
+def test_component_list_that_disagrees_with_comp_is_refused_on_every_route(b200):
+    """comp_nodes must list exactly the nodes whose `comp` names the component: the device's node ->
+    local index map is filled from comp_nodes alone, so a node listed in the wrong component would
+    index a tier's shared-memory node arrays with another component's local index.  Two non-root
+    nodes of different components swapped in comp_nodes (comp and the sizes unchanged) give
+    LFR_EINVAL on the warp2, tile, shared-memory Cholesky, CTA and zero-copy routes, and the library
+    then solves the consistent problem as before."""
+    import ctypes as C
+    import dataclasses
+    import torch
+    from lfr_b200 import capi
+    _, p = get_problem("cfg1")
+    lists = [p.comp_nodes[p.comp_ptr[c]:p.comp_ptr[c + 1]] for c in (0, 1)]
+    pick = [int(np.flatnonzero(p.is_root[nodes] == 0)[0]) + int(p.comp_ptr[c]) for c, nodes in enumerate(lists)]
+    assert p.comp[p.comp_nodes[pick[0]]] != p.comp[p.comp_nodes[pick[1]]]
+    swapped = p.comp_nodes.copy()
+    swapped[pick] = swapped[pick[::-1]]
+    bad = dataclasses.replace(p, comp_nodes=swapped)
+    N = p.graph.n_nodes
+
+    def solve_pinned(prob, dbg):  # lfr_solve on pinned caller buffers: in place with DBG_ZERO_COPY
+        s, keep = b200.marshal(prob)
+        e_pin = torch.empty(keep["edges"].nbytes, dtype=torch.uint8).pin_memory()
+        e_pin.numpy()[:] = keep["edges"].view(np.uint8).reshape(-1)
+        s.edges = e_pin.data_ptr()
+        pos_pin = torch.zeros(2 * N, dtype=torch.float64).pin_memory()
+        st, _ = b200.make_stats(prob.n_components)
+        o = b200.default_options(debug_flags=dbg)
+        rc = b200.lib.lfr_solve(C.byref(s), C.byref(o), C.c_void_p(pos_pin.data_ptr()), C.byref(st))
+        return rc, pos_pin.numpy().reshape(N, 2).copy()
+
+    routes = {"warp2": {}, "tile": dict(debug_flags=1 << capi.DBG_TILE_FROM_SHIFT),
+              "warp": dict(debug_flags=capi.DBG_FORCE_SMEM_CHOLESKY), "cta": dict(linear_solver=2)}
+    for name, opts in routes.items():
+        pos_ref, st_ref = b200.solve(p, b200.default_options(**opts))
+        with pytest.raises(RuntimeError, match=r"\(-1\).*comp_nodes"):
+            b200.solve(bad, b200.default_options(**opts))
+        pos, st = b200.solve(p, b200.default_options(**opts))
+        assert np.array_equal(pos, pos_ref) and np.array_equal(st["iterations"], st_ref["iterations"]), name
+    rc, pos_ref = solve_pinned(p, capi.DBG_ZERO_COPY)
+    assert rc == 0
+    rc, _ = solve_pinned(bad, capi.DBG_ZERO_COPY)
+    assert rc == -1 and "comp_nodes" in b200.last_error()
+    rc, pos = solve_pinned(p, capi.DBG_ZERO_COPY)
+    assert rc == 0 and np.array_equal(pos, pos_ref)
 
 
 def _quartic_cases(rng, n):
