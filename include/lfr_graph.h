@@ -14,7 +14,7 @@
  * reports; tracks_ms / graph_cut_ms / graph_ms / dispatch_ms time the device phases (host clock,
  * stream synchronised at each phase boundary).  Errors: LFR_EINVAL for an image id out of range or a
  * non-finite similarity, LFR_EUNSUPPORTED for more than 65 535 images (as the host stage) or more than
- * 2^31 - 1 directed edges.  Only liblfr_b200.so provides these two symbols; the CPU oracle has no
+ * 2^31 - 1 directed edges.  Only liblfr_b200.so provides this header's symbols; the CPU oracle has no
  * plans and does not (the Python binding refuses Plan.from_matches() on it with LFR_EUNSUPPORTED).
  *
  * Cost: the Kruskal runs in rounds over a window of pending edges (LFR_KRUSKAL_WINDOW in the
@@ -48,6 +48,15 @@ int lfr_plan_export_graph(const lfr_plan* plan, uint32_t* row_ptr /* [N+1] */, l
                           uint32_t* comp_ptr /* [C+1] */, uint32_t* comp_nodes /* [N] */,
                           uint32_t* comp_order /* [C] */, uint32_t* node_image /* [N] */,
                           uint32_t* node_feat /* [N] */);
+
+/* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
+ * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from
+ * sizes known before either stage runs — the directed edges (2 x the matches of the pairs not skipped),
+ * the number of images and of devices — and from nothing else: it needs no device and makes no CUDA
+ * call.  0 below a size threshold measured on an H100 (DESIGN.md §4), for more than one device
+ * (lfr_solve_multi() takes a host lfr_problem; plans are single-device), for NULL or malformed input and
+ * for inputs the device stage refuses. */
+int lfr_graph_stage_on_device(const lfr_host_input* in, int32_t n_devices);
 
 #ifdef __cplusplus
 }

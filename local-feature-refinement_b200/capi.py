@@ -77,11 +77,18 @@ ABI_SYMBOLS = [
     "lfr_plan_traffic", "lfr_plan_destroy", "lfr_debug_edge_eval",
 ]
 #: the symbols include/lfr_graph.h declares
-GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_export_graph"]
+GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_export_graph", "lfr_graph_stage_on_device"]
 
 
 def _ptr(a: Optional[np.ndarray]) -> Optional[int]:
     return None if a is None else a.ctypes.data
+
+
+def _host_input(arrs: dict, n_images: int) -> HostInput:
+    """lfr_host_input over the flat arrays of host_input_arrays (no edges_out)."""
+    return HostInput(n_pairs=arrs["pair_img1"].shape[0], n_matches=arrs["feat1"].shape[0], n_images=n_images,
+                     edges_out=None, edges_out_capacity=0,
+                     **{k: (v.ctypes.data if v.size else None) for k, v in arrs.items()})
 
 
 class Library:
@@ -127,6 +134,8 @@ class Library:
             L.lfr_plan_create_from_matches.restype = C.c_int
             L.lfr_plan_export_graph.argtypes = [C.c_void_p] * 11
             L.lfr_plan_export_graph.restype = C.c_int
+            L.lfr_graph_stage_on_device.argtypes = [C.POINTER(HostInput), C.c_int32]
+            L.lfr_graph_stage_on_device.restype = C.c_int
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -140,6 +149,20 @@ class Library:
     def check(self, rc: int, what: str) -> None:
         if rc != LFR_OK:
             raise RuntimeError("lfr: %s failed (%d): %s" % (what, rc, self.last_error()))
+
+    @property
+    def has_graph_stage(self) -> bool:
+        """Whether the library has the graph stage on the GPU (include/lfr_graph.h); the CPU oracle has not."""
+        return hasattr(self.lib, "lfr_plan_create_from_matches")
+
+    def graph_stage_on_device(self, arrs: dict, n_images: int, n_devices: int = 1) -> bool:
+        """lfr_graph_stage_on_device (include/lfr_graph.h) on the flat lfr_host_input arrays `arrs`
+        (host_input_arrays): whether the graph stage of this input should run on the device.  Needs no
+        device; False for a library without the stage."""
+        if not self.has_graph_stage:
+            return False
+        inp = _host_input(arrs, n_images)
+        return self.lib.lfr_graph_stage_on_device(C.byref(inp), int(n_devices)) == 1
 
     def default_options(self, **overrides) -> LfrOptions:
         o = LfrOptions()
@@ -305,10 +328,8 @@ class Plan:
         else:
             _, arrs = host_input_arrays(matches, banned_images)
             n_images = len(matches.image_names) if n_images is None else n_images
-        inp = HostInput(n_pairs=arrs["pair_img1"].shape[0], n_matches=arrs["feat1"].shape[0], n_images=n_images,
-                        edges_out=None, edges_out_capacity=0,
-                        **{k: (v.ctypes.data if v.size else None) for k, v in arrs.items()})
-        if not hasattr(lib.lib, "lfr_plan_create_from_matches"):  # e.g. the CPU oracle: no device, no plans
+        inp = _host_input(arrs, n_images)
+        if not lib.has_graph_stage:  # e.g. the CPU oracle: no device, no plans
             raise RuntimeError("lfr: lfr_plan_create_from_matches failed (-5): %s does not provide the graph stage "
                                "on the GPU (include/lfr_graph.h)" % lib.path)
         o = options if options is not None else lib.default_options()

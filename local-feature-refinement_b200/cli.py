@@ -10,6 +10,13 @@ the output cannot be written, solve.cc:433-436,674-677), so
 local-feature-evaluation/benchmark.py:100-104, eth/benchmark.py:108-112 and
 custom_demo.py:101-105 run unchanged.  `--n_threads` is accepted and ignored
 (the solve runs on the GPU).  Opt-in extras: --device, --gpus N (one process drives N GPUs), --stats_json.
+
+The graph stage (solve.cc:438-606) runs where the library's size rule says
+(lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
+(Plan.from_matches; the problem is solved where it was built), on the host
+otherwise and for torchrun ranks and --gpus N.  LFR_GRAPH_STAGE=host|device
+forces a route (a test and measurement hook); `--stats_json` reports it as
+info.host_stage ("device", or "native" / "numpy" on the host route).
 """
 from __future__ import annotations
 
@@ -120,7 +127,7 @@ def main(argv=None) -> int:
     args = parse_args(sys.argv[1:] if argv is None else argv)
 
     from . import wire
-    from .solver import refine
+    from .solver import GraphStageRouteError, refine
     from .capi import load_b200
     from .graph import refined_track_count
 
@@ -166,7 +173,15 @@ def main(argv=None) -> int:
         timing["solver_ms"] = (time.perf_counter() - t1) * 1e3
         return pos, st
 
-    p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn)
+    # torchrun ranks and --gpus N solve a host lfr_problem: the size rule keeps them on the host route
+    torchrun = "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1
+    n_devices = int(os.environ["WORLD_SIZE"]) if torchrun else max(args.gpus, 1)
+    try:
+        p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
+                                 timing=timing)
+    except GraphStageRouteError as e:
+        sys.stderr.write("ERROR: %s\n" % e)
+        return 2
     say("Solver time: %dms" % int(timing.get("solver_ms", 0.0)))                       # solve.cc:638
     say("Total time: %dms" % int((time.perf_counter() - t_start) * 1e3))               # solve.cc:641
     say("# points with at least one coordinate > 0.5: %d" % sol.n_outside)             # solve.cc:670

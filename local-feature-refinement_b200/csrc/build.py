@@ -55,7 +55,8 @@ def build_host(force: bool = False) -> str:
 def build_exe(force: bool = False, out: str = OUT_EXE, solve_lib_dir: str = HERE, solve_lib: str = "lfr_b200") -> str:
     """The native `solve`.  The product links csrc/liblfr_b200.so; tests/ link the same source against the
     CPU checker (oracle/liblfr_ref.so exports the same C ABI) to compare it with the reference binary."""
-    deps = [EXE_SOURCE, os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"), os.path.join(INC, "lfr_host.h")]
+    deps = [EXE_SOURCE, os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"), os.path.join(INC, "lfr_host.h"),
+            os.path.join(INC, "lfr_graph.h")]
     if force or _stale(out, deps) or not os.path.exists(out):
         os.makedirs(os.path.dirname(out), exist_ok=True)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-Wall", "-o", out, os.path.join(HERE, EXE_SOURCE),

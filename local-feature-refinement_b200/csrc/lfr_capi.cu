@@ -837,6 +837,12 @@ int components_on_device(uint32_t n, const uint32_t* a, const uint32_t* b, uint3
 using Clock = std::chrono::steady_clock;
 double ms_since(Clock::time_point t0) { return std::chrono::duration<double, std::milli>(Clock::now() - t0).count(); }
 
+// lfr_graph_stage_on_device(): the directed edges from which the graph stage runs on the device.  The
+// native drop-in's "Total time" on an H100 80GB HBM3 at 700 W (tools/gpu_graph_stage_time.py, DESIGN.md
+// §4): the host route is faster up to ~10 K directed edges and the device route from 200 K on; in between
+// the two trade places from run to run within their spread, and the switch sits inside that tie.
+constexpr uint64_t kDeviceGraphStageMinEdges = 32768;
+
 // lfr_host_stage_create() on the device, block for block (lfr_host.cc): the edge records go into
 // pl->edges, the other arrays come back to pl->graph (the schedule builder is host code and reads them).
 int build_graph_on_device(const lfr_host_input* in, lfr_plan* pl, lfr_host_sizes* S, cudaStream_t s) {
@@ -1686,6 +1692,20 @@ int lfr_plan_export_graph(const lfr_plan* pl, uint32_t* row_ptr, lfr_edge* edges
     LFR_CUDA(cudaMemcpy(edges, pl->edges.p, sizeof(lfr_edge) * (size_t)pl->E, cudaMemcpyDeviceToHost));
   }
   return LFR_OK;
+}
+
+int lfr_graph_stage_on_device(const lfr_host_input* in, int32_t n_devices) {
+  // host code only: decided before any CUDA call, so a one-shot process can choose its route while the
+  // context is still being created
+  if (!in || n_devices != 1) return 0;
+  if (in->n_images > 65535 || in->n_pairs + 1 >= (1ull << 31)) return 0;  // the device stage refuses these
+  if (in->n_pairs && (!in->pair_ptr || in->pair_ptr[in->n_pairs] > in->n_matches)) return 0;
+  uint64_t e = 0;
+  for (uint64_t p = 0; p < in->n_pairs; ++p) {
+    if (in->pair_ptr[p + 1] < in->pair_ptr[p]) return 0;  // malformed: the host stage reports it
+    if (!(in->pair_skip && in->pair_skip[p])) e += 2 * (in->pair_ptr[p + 1] - in->pair_ptr[p]);
+  }
+  return e >= kDeviceGraphStageMinEdges && e < (1ull << 31) ? 1 : 0;
 }
 
 int lfr_plan_solve(lfr_plan* pl, void* stream) {

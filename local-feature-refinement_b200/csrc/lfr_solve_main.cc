@@ -6,10 +6,15 @@
 // Same flags (solve.cc:379-385, Boost.Program_options semantics and messages), same `.part.N` handling
 // (:416-424), same stdout lines (:484-485,534,549,589,591,606,638,641,670) and exit codes (0; 1 on a
 // command-line error, :397-401; -1 = 255 when the input does not parse or the output cannot be
-// written, :433-436,674-677).  The work is three library calls: lfr_wire_decode_matches()
-// (include/lfr_wire.h), lfr_host_stage_create() (include/lfr_host.h) and lfr_solve() /
-// lfr_solve_multi() (include/lfr.h) on page-locked arrays, then lfr_wire_encode_solution().
-// Opt-in extras: --device D, --gpus N (one process drives N GPUs).  `--n_threads` is accepted and
+// written, :433-436,674-677).  The work is lfr_wire_decode_matches() (include/lfr_wire.h), the graph
+// stage and the solve, then lfr_wire_encode_solution().  The graph stage runs where
+// lfr_graph_stage_on_device() (include/lfr_graph.h) says, from the input's size:
+//   device: lfr_plan_create_from_matches(), lfr_plan_solve() + lfr_plan_download() on the plan it left
+//           in HBM, and lfr_plan_export_graph() for the node -> (image, feature) ids;
+//   host:   lfr_host_stage_create() (include/lfr_host.h) writing the edge records into page-locked
+//           memory, then lfr_solve() / lfr_solve_multi() (include/lfr.h).
+// Both routes give the same bytes and lines.  LFR_GRAPH_STAGE=host|device forces a route (a test and
+// measurement hook).  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -31,8 +36,20 @@
 #include <unistd.h>
 
 #include "../../include/lfr.h"
+#include "../../include/lfr_graph.h"
 #include "../../include/lfr_host.h"
 #include "../../include/lfr_wire.h"
+
+// The graph stage on the GPU is resolved weakly: the same source links against the CPU checker
+// (oracle/liblfr_ref.so), which has no plans; there the three are NULL and every input takes the host route.
+extern "C" {
+int lfr_graph_stage_on_device(const lfr_host_input* in, int32_t n_devices) __attribute__((weak));
+int lfr_plan_create_from_matches(const lfr_host_input* in, const lfr_options* o, const double* initial_positions,
+                                 lfr_plan** out, lfr_host_sizes* sizes) __attribute__((weak));
+int lfr_plan_export_graph(const lfr_plan* plan, uint32_t* row_ptr, lfr_edge* edges, uint32_t* track, uint32_t* comp,
+                          uint8_t* is_root, uint32_t* comp_ptr, uint32_t* comp_nodes, uint32_t* comp_order,
+                          uint32_t* node_image, uint32_t* node_feat) __attribute__((weak));
+}
 
 namespace {
 
@@ -334,39 +351,92 @@ int main(int argc, char** argv) {
     if (!have_fact[pair_img2[p]]) { have_fact[pair_img2[p]] = 1; image_fact[pair_img2[p]] = pair_fact2[p]; }
   }
 
-  cuda_start.join();  // page-locked memory needs the context
-  const Clock::time_point t_start = Clock::now();  // "Total time" (solve.cc:487-641): the graph work and the solve
-  // ---- host graph stage (solve.cc:438-606); the edge records go straight into page-locked memory
-  lfr_edge* edges = nullptr;
-  bool edges_pinned = false;
-  if (e_cap) {
-    edges = static_cast<lfr_edge*>(lfr_host_alloc(e_cap * sizeof(lfr_edge)));
-    edges_pinned = edges != nullptr;
-    if (!edges) edges = static_cast<lfr_edge*>(std::malloc(e_cap * sizeof(lfr_edge)));
-  }
   lfr_host_input in;
   std::memset(&in, 0, sizeof in);
   in.n_pairs = P; in.n_matches = M; in.n_images = (uint32_t)names.size();
   in.pair_img1 = pair_img1.data(); in.pair_img2 = pair_img2.data(); in.pair_skip = skip.data();
   in.pair_ptr = pair_ptr.data(); in.feat1 = feat1; in.feat2 = feat2; in.sim = sim; in.disp1 = disp1; in.disp2 = disp2;
-  in.edges_out = edges; in.edges_out_capacity = e_cap;
-  lfr_host_stage* hs = nullptr;
+
+  // ---- which graph stage: the library's size rule, or LFR_GRAPH_STAGE=host|device (a test and
+  // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
+  // takes the host route; forcing the device route there is an error, never a silent host run.
+  const bool have_device_stage = lfr_graph_stage_on_device && lfr_plan_create_from_matches && lfr_plan_export_graph;
+  bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
+  const char* force = std::getenv("LFR_GRAPH_STAGE");
+  if (force && *force) {
+    if (std::strcmp(force, "host") == 0) {
+      on_device = false;
+    } else if (std::strcmp(force, "device") == 0) {
+      if (!have_device_stage) {
+        std::fprintf(stderr, "ERROR: LFR_GRAPH_STAGE=device: the solve library has no graph stage on the GPU\n");
+        return 2;
+      }
+      if (gpus > 1) {
+        std::fprintf(stderr, "ERROR: LFR_GRAPH_STAGE=device: the graph stage on the GPU drives one device (--gpus 1)\n");
+        return 2;
+      }
+      on_device = true;
+    } else {
+      std::fprintf(stderr, "ERROR: LFR_GRAPH_STAGE must be 'host' or 'device'\n");
+      return 2;
+    }
+  }
+
+  cuda_start.join();  // page-locked memory needs the context
+  const Clock::time_point t_start = Clock::now();  // "Total time" (solve.cc:487-641): the graph work and the solve
+  lfr_edge* edges = nullptr;
+  bool edges_pinned = false;
+  lfr_plan* plan = nullptr;
   lfr_host_sizes sz;
-  if (lfr_host_stage_create(&in, &hs, &sz) != LFR_OK) {
-    std::fprintf(stderr, "ERROR: the host graph stage rejected the input\n");
-    return 2;
+  std::vector<uint32_t> row_ptr, track, comp, comp_ptr, comp_nodes, comp_order, node_image, node_feat;
+  std::vector<uint8_t> is_root;
+  if (on_device) {
+    // ---- the graph stage on the GPU (include/lfr_graph.h): the problem stays in HBM for the solve and
+    // only the per-node image / feature ids come back for the SolutionFile
+    lfr_options opt;
+    lfr_options_default(&opt);
+    opt.device = (int32_t)device;
+    const int rc = lfr_plan_create_from_matches(&in, &opt, nullptr, &plan, &sz);
+    if (rc == LFR_EINVAL || rc == LFR_EUNSUPPORTED) {  // the input, as the host stage would reject it
+      std::fprintf(stderr, "ERROR: the host graph stage rejected the input\n");
+      return 2;
+    }
+    if (rc != LFR_OK) {  // no device: the host route's message, from the same device check
+      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
+      return 2;
+    }
+    node_image.resize(sz.n_nodes);
+    node_feat.resize(sz.n_nodes);
+    if (lfr_plan_export_graph(plan, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                              node_image.data(), node_feat.data()) != LFR_OK) {
+      std::fprintf(stderr, "ERROR: lfr_plan_export_graph failed\n");
+      return 2;
+    }
+  } else {
+    // ---- host graph stage (solve.cc:438-606); the edge records go straight into page-locked memory
+    if (e_cap) {
+      edges = static_cast<lfr_edge*>(lfr_host_alloc(e_cap * sizeof(lfr_edge)));
+      edges_pinned = edges != nullptr;
+      if (!edges) edges = static_cast<lfr_edge*>(std::malloc(e_cap * sizeof(lfr_edge)));
+    }
+    in.edges_out = edges; in.edges_out_capacity = e_cap;
+    lfr_host_stage* hs = nullptr;
+    if (lfr_host_stage_create(&in, &hs, &sz) != LFR_OK) {
+      std::fprintf(stderr, "ERROR: the host graph stage rejected the input\n");
+      return 2;
+    }
+    const uint32_t n = sz.n_nodes, c = sz.n_components;
+    row_ptr.assign((size_t)n + 1, 0); track.resize(n); comp.resize(n); comp_ptr.assign((size_t)c + 1, 0);
+    comp_nodes.resize(n); comp_order.resize(c); node_image.resize(n); node_feat.resize(n); is_root.resize(n);
+    if (lfr_host_stage_export(hs, row_ptr.data(), edges, track.data(), comp.data(), is_root.data(), comp_ptr.data(),
+                              comp_nodes.data(), comp_order.data(), node_image.data(), node_feat.data()) != LFR_OK) {
+      std::fprintf(stderr, "ERROR: lfr_host_stage_export failed\n");
+      return 2;
+    }
+    lfr_host_stage_destroy(hs);
   }
   const uint32_t N = sz.n_nodes, C = sz.n_components;
   const uint64_t E = sz.n_edges;
-  std::vector<uint32_t> row_ptr((size_t)N + 1, 0), track(N), comp(N), comp_ptr((size_t)C + 1, 0), comp_nodes(N), comp_order(C),
-      node_image(N), node_feat(N);
-  std::vector<uint8_t> is_root(N);
-  if (lfr_host_stage_export(hs, row_ptr.data(), edges, track.data(), comp.data(), is_root.data(), comp_ptr.data(),
-                            comp_nodes.data(), comp_order.data(), node_image.data(), node_feat.data()) != LFR_OK) {
-    std::fprintf(stderr, "ERROR: lfr_host_stage_export failed\n");
-    return 2;
-  }
-  lfr_host_stage_destroy(hs);
   std::printf("# graph nodes: %u\n", N);                                  // solve.cc:484
   std::printf("# graph edges: %llu\n", (unsigned long long)E);            // solve.cc:485
   if (N) {
@@ -388,7 +458,14 @@ int main(int argc, char** argv) {
     std::memset(positions, 0, 2ull * N * sizeof(double));
   }
   const Clock::time_point t_solve = Clock::now();
-  if (N) {
+  if (N && plan) {
+    int rc = lfr_plan_solve(plan, nullptr);
+    if (rc == LFR_OK) rc = lfr_plan_download(plan, nullptr, positions, nullptr);
+    if (rc != LFR_OK) {
+      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
+      return 2;
+    }
+  } else if (N) {
     lfr_problem prob;
     prob.n_nodes = N; prob.n_components = C; prob.n_edges = E;
     prob.row_ptr = row_ptr.data(); prob.edges = edges; prob.track = track.data(); prob.comp = comp.data();
@@ -412,6 +489,7 @@ int main(int argc, char** argv) {
     }
   }
   const Clock::time_point t_end = Clock::now();
+  lfr_plan_destroy(plan);
   std::printf("Solver time: %lldms\n", ms_between(t_solve, t_end));  // solve.cc:638
   std::printf("Total time: %lldms\n", ms_between(t_start, t_end));   // solve.cc:641
 

@@ -483,7 +483,6 @@ def build_problem_native(ms: MatchSet, banned_images=(), log=None) -> Problem:
     L.lfr_host_stage_export.restype = C.c_int
     L.lfr_host_stage_destroy.argtypes = [C.c_void_p]
     L.lfr_host_stage_destroy.restype = None
-    say = log if log is not None else (lambda s: None)
     skip, arrs = host_input_arrays(ms, banned_images)
     # the edge records (80 B each) are written straight into the array handed to lfr_solve
     counts = (arrs["pair_ptr"][1:] - arrs["pair_ptr"][:-1]).astype(np.int64)
@@ -514,6 +513,17 @@ def build_problem_native(ms: MatchSet, banned_images=(), log=None) -> Problem:
             raise RuntimeError("lfr_host_stage_export failed (%d)" % rc)
     finally:
         L.lfr_host_stage_destroy(h)
+    out = dict(zip(("row_ptr", "edges", "track", "comp", "is_root", "comp_ptr", "comp_nodes", "comp_order",
+                    "node_image", "node_feat"), outs))
+    return problem_from_stage(ms, skip, out, {k: getattr(sz, k) for k in HOST_SIZES_FIELDS}, "native", log)
+
+
+def problem_from_stage(ms: MatchSet, skip: np.ndarray, out: dict, sz: dict, host_stage: str, log=None) -> Problem:
+    """The Problem of a graph stage's results — `out`, the arrays of lfr_host_stage_export /
+    lfr_plan_export_graph by name (stage_outputs), `sz`, its lfr_host_sizes as a dict — with the stdout
+    lines of solve.cc:484-606.  `host_stage` names the stage in `info` ("native" or "device")."""
+    say = log if log is not None else (lambda s: None)
+    N, E, Cn = int(sz["n_nodes"]), int(sz["n_edges"]), int(sz["n_components"])
     image_fact: Dict[int, float] = {}
     for a, b, fa, fb, sk in zip(ms.pair_img1.tolist(), ms.pair_img2.tolist(), ms.pair_fact1.tolist(),
                                 ms.pair_fact2.tolist(), skip.tolist()):
@@ -521,29 +531,29 @@ def build_problem_native(ms: MatchSet, banned_images=(), log=None) -> Problem:
             continue
         image_fact.setdefault(a, fa)
         image_fact.setdefault(b, fb)
-    g = MatchGraph(n_nodes=N, node_image=node_image.astype(np.int64), node_feat=node_feat,
+    g = MatchGraph(n_nodes=N, node_image=out["node_image"].astype(np.int64), node_feat=out["node_feat"],
                    und_sim=np.zeros(0), und_n1=np.zeros(0, np.int64), und_n2=np.zeros(0, np.int64),
-                   row_ptr=row_ptr, edges=edges, image_names=ms.image_names, image_fact=image_fact,
-                   n_images=int(sz.n_images_seen))
+                   row_ptr=out["row_ptr"], edges=out["edges"], image_names=ms.image_names, image_fact=image_fact,
+                   n_images=int(sz["n_images_seen"]))
     say("# graph nodes: %d" % N)
     say("# graph edges: %d" % E)
     info: dict = {}
     if N == 0:
         z32 = np.zeros(0, dtype=np.uint32)
         return Problem(g, z32, z32, np.zeros(0, np.uint8), np.zeros(1, np.uint32), z32, z32, info)
-    say("# tracks: %d" % sz.n_tracks)
-    say("max track size: %d" % sz.max_track_size)
-    say("Graph-cut time: %dms" % int(sz.graph_cut_ms))
+    say("# tracks: %d" % sz["n_tracks"])
+    say("max track size: %d" % sz["max_track_size"])
+    say("Graph-cut time: %dms" % int(sz["graph_cut_ms"]))
     say("# components: %d" % Cn)
-    say("max component size: %d" % sz.max_component_size)
-    info.update(n_tracks=int(sz.n_tracks), n_components=Cn, max_component_size=int(sz.max_component_size),
-                tracks_ms=float(sz.tracks_ms), graph_cut_ms=float(sz.graph_cut_ms), graph_ms=float(sz.graph_ms),
-                dispatch_ms=float(sz.dispatch_ms),
-                n_meta_components=int(sz.n_meta_components),
-                n_oversized_meta_components=int(sz.n_oversized_meta_components), n_cut_groups=int(sz.n_cut_groups),
-                host_stage="native")
-    return Problem(graph=g, track=track, comp=comp, is_root=is_root, comp_ptr=comp_ptr, comp_nodes=comp_nodes,
-                   comp_order=comp_order.astype(np.int64), info=info)
+    say("max component size: %d" % sz["max_component_size"])
+    info.update(n_tracks=int(sz["n_tracks"]), n_components=Cn, max_component_size=int(sz["max_component_size"]),
+                tracks_ms=float(sz["tracks_ms"]), graph_cut_ms=float(sz["graph_cut_ms"]), graph_ms=float(sz["graph_ms"]),
+                dispatch_ms=float(sz["dispatch_ms"]),
+                n_meta_components=int(sz["n_meta_components"]),
+                n_oversized_meta_components=int(sz["n_oversized_meta_components"]), n_cut_groups=int(sz["n_cut_groups"]),
+                host_stage=host_stage)
+    return Problem(graph=g, track=out["track"], comp=out["comp"], is_root=out["is_root"], comp_ptr=out["comp_ptr"],
+                   comp_nodes=out["comp_nodes"], comp_order=out["comp_order"].astype(np.int64), info=info)
 
 
 def build_problem(ms: MatchSet, banned_images=(), log=None, native: Optional[bool] = None) -> Problem:

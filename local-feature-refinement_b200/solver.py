@@ -6,6 +6,8 @@ csrc/liblfr_b200.so) and the output assembly (solve.cc:643-679).
 """
 from __future__ import annotations
 
+import os
+import time
 from dataclasses import dataclass
 from typing import Callable, List, Optional
 
@@ -68,11 +70,57 @@ def solve_problem(p: Problem, options=None, positions: Optional[np.ndarray] = No
     return lib.solve(p, options, positions)
 
 
+class GraphStageRouteError(RuntimeError):
+    """LFR_GRAPH_STAGE asks for a route this run cannot take."""
+
+
+def graph_stage_on_device(lib, arrs: dict, n_images: int, n_devices: int = 1) -> bool:
+    """Where the graph stage of the flat lfr_host_input arrays `arrs` (graph.host_input_arrays) runs:
+    the library's size rule (lfr_graph_stage_on_device, include/lfr_graph.h), unless LFR_GRAPH_STAGE=host|device
+    forces a route (a test and measurement hook).  Forcing the device route where `lib` has no graph stage
+    on the GPU, or for more than one device, raises GraphStageRouteError: it never runs the host stage instead."""
+    force = os.environ.get("LFR_GRAPH_STAGE") or ""
+    if force == "host":
+        return False
+    if force == "device":
+        if not lib.has_graph_stage:
+            raise GraphStageRouteError("LFR_GRAPH_STAGE=device: the solve library has no graph stage on the GPU")
+        if n_devices != 1:
+            raise GraphStageRouteError("LFR_GRAPH_STAGE=device: the graph stage on the GPU drives one device (--gpus 1)")
+        return True
+    if force:
+        raise GraphStageRouteError("LFR_GRAPH_STAGE must be 'host' or 'device'")
+    return lib.graph_stage_on_device(arrs, n_images, n_devices)
+
+
 def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[[str], None]] = None,
-           solve_fn=None):
+           solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
-    may be supplied to drive a different executor (the multi-GPU path)."""
-    p = build_problem(ms, banned_images, log=log)
-    fn = solve_fn if solve_fn is not None else (lambda q: solve_problem(q, options))
-    pos, st = fn(p)
+    may be supplied to drive a different executor (the multi-GPU path; give `n_devices`).
+
+    The graph stage runs where graph_stage_on_device() says.  On the device (Plan.from_matches) the problem
+    stays in HBM and is solved there, `solve_fn` is not called, and the Problem's arrays come from
+    Plan.export_graph(); `timing["solver_ms"]` (when `timing` is given) then covers solve + download."""
+    from .capi import Plan, load_b200
+    from .graph import host_input_arrays, problem_from_stage
+    lib = load_b200()
+    skip, arrs = host_input_arrays(ms, banned_images)
+    if not graph_stage_on_device(lib, arrs, len(ms.image_names), n_devices):
+        p = build_problem(ms, banned_images, log=log)
+        fn = solve_fn if solve_fn is not None else (lambda q: solve_problem(q, options))
+        pos, st = fn(p)
+        return p, pos, st, assemble_solution(p, pos)
+    plan = Plan.from_matches(lib, arrs, options=options, n_images=len(ms.image_names))
+    try:
+        p = problem_from_stage(ms, skip, plan.export_graph(), plan.sizes, "device", log)
+        t1 = time.perf_counter()
+        if p.graph.n_nodes:
+            plan.solve()
+            pos, st = plan.download()
+        else:
+            pos, st = solve_problem(p, options)
+        if timing is not None:
+            timing["solver_ms"] = (time.perf_counter() - t1) * 1e3
+    finally:
+        plan.close()
     return p, pos, st, assemble_solution(p, pos)
