@@ -18,13 +18,17 @@ namespace graph {
 
 constexpr uint32_t kListMax = 12;  // image sets of 2..12 images: a list of image ids (lfr_host.cc kListMax)
 
-// lfr_host.cc sortable_bits: float -> uint32 whose unsigned order is the float order
+// lfr_host.cc sortable_bits: float -> uint32 whose unsigned order is the float order, -0.0 keyed as +0.0
+// (equal under the reference's tuple sort, solve.cc:489)
 __device__ __forceinline__ uint32_t sortable_bits(float f) {
-  const uint32_t u = __float_as_uint(f);
+  uint32_t u = __float_as_uint(f);
+  if (u == 0x80000000u) u = 0u;
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
-// double -> uint64 whose unsigned order is the order of the (finite) doubles
+// double -> uint64 whose unsigned order is the order of the (finite) doubles.  -0.0 would key below +0.0,
+// but the root scores it sees are sums that start at +0.0, and under round-to-nearest such a sum is never
+// -0.0 (x + -x and +0.0 + -0.0 both give +0.0)
 __device__ __forceinline__ unsigned long long sortable_bits64(double d) {
   const unsigned long long u = (unsigned long long)__double_as_longlong(d);
   return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);

@@ -100,10 +100,13 @@ struct FlatMap {
   }
 };
 
-// float -> uint32 whose unsigned order is the float order (finite values)
+// float -> uint32 whose unsigned order is the float order (finite values).  -0.0 maps to the key of
+// +0.0: the reference sorts std::tuple<double, size_t, size_t> (solve.cc:489), where the two compare
+// equal and the tie falls to (n1, n2).  Tested on the bits, so no flush-to-zero can merge a denormal in.
 inline uint32_t sortable_bits(float f) {
   uint32_t u;
   std::memcpy(&u, &f, 4);
+  if (u == 0x80000000u) u = 0u;
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
