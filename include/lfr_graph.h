@@ -40,7 +40,31 @@ int lfr_plan_create_from_matches(const lfr_host_input* in, const lfr_options* o,
                                  const double* initial_positions /* [2N] or NULL = zeros */,
                                  lfr_plan** out, lfr_host_sizes* sizes);
 
-/* Copy the stage's arrays of a plan made by lfr_plan_create_from_matches() into caller-owned arrays;
+/* One MatchingFile part for lfr_plan_create_from_wire(): its bytes and the offset of each of its
+ * matches' length prefix, as lfr_wire_walk_matches() (include/lfr_wire.h) records them. */
+typedef struct lfr_wire_part {
+  const uint8_t* buf;         /* [len] the part's bytes; may be pageable (e.g. a mapped file) */
+  uint64_t len;
+  const uint64_t* match_off;  /* [n_matches] */
+  uint64_t n_matches;
+} lfr_wire_part;
+
+/* lfr_plan_create_from_matches() from the MatchingFile bytes: the matches are decoded on the device,
+ * straight into the stage's input, and never exist on the host.  `in` carries the pair level only —
+ * n_pairs, n_matches, n_images, pair_img1/2, pair_skip, pair_ptr, built by the caller from
+ * lfr_wire_walk_matches() over the parts in order (pair_ptr global: part k's matches follow part k-1's);
+ * in->feat1 ... in->disp2 and edges_out are ignored.  The parts' n_matches must add up to in->n_matches.
+ * The bytes go up through page-locked staging.  Every match is decoded with the semantics of
+ * lfr_wire_decode_matches(), those of banned pairs included, so the result — the plan, every
+ * lfr_plan_export_graph() array and the solve — is bitwise that of lfr_plan_create_from_matches() on
+ * the host decode of the same bytes.  Errors: LFR_EINVAL with lfr_last_error() = "malformed Match
+ * message" when a match is malformed (exactly when lfr_wire_decode_matches() rejects its part), checked
+ * before the stage runs; otherwise the codes of lfr_plan_create_from_matches(). */
+int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
+                              const lfr_options* o, const double* initial_positions /* [2N] or NULL */,
+                              lfr_plan** out, lfr_host_sizes* sizes);
+
+/* Copy the stage's arrays of a plan made by lfr_plan_create_from_matches() or _from_wire() into caller-owned arrays;
  * the arguments mean what they mean in lfr_host_stage_export() (any pointer may be NULL; `edges` is a
  * device-to-host copy).  LFR_EINVAL for a plan made by lfr_plan_create(). */
 int lfr_plan_export_graph(const lfr_plan* plan, uint32_t* row_ptr /* [N+1] */, lfr_edge* edges /* [E] */,
@@ -57,6 +81,12 @@ int lfr_plan_export_graph(const lfr_plan* plan, uint32_t* row_ptr /* [N+1] */, l
  * (lfr_solve_multi() takes a host lfr_problem; plans are single-device), for NULL or malformed input and
  * for inputs the device stage refuses. */
 int lfr_graph_stage_on_device(const lfr_host_input* in, int32_t n_devices);
+
+/* On the device route, whether the matches should be decoded on the device (lfr_plan_create_from_wire)
+ * rather than on the host (lfr_wire_decode_matches + lfr_plan_create_from_matches): 1 or 0, from the
+ * match count alone (all pairs, banned ones included: every match is decoded).  0 below a threshold
+ * measured on an H100 (DESIGN.md §4).  Host code only, like lfr_graph_stage_on_device(). */
+int lfr_wire_decode_on_device(uint64_t n_matches);
 
 #ifdef __cplusplus
 }

@@ -49,6 +49,14 @@ typedef struct lfr_wire_matches {
 
 int lfr_wire_decode_matches(const uint8_t* buf, uint64_t len, lfr_wire_matches* out);
 
+/* The pair level of lfr_wire_decode_matches without decoding any match: fills pair_ptr, fact1/2 and the
+ * name offsets and lengths of `out` (feat1 ... disp2 are not touched and may be NULL), and
+ * match_off[k] = the byte offset in `buf` of match k's length prefix (the byte after its tag), for
+ * k < out->n_matches.  Same walk and same capacity rules as lfr_wire_decode_matches, so it returns
+ * LFR_EINVAL exactly when lfr_wire_scan_matches does (or the capacities are wrong); the contents of the
+ * matches are left to the decoder (lfr_plan_create_from_wire, include/lfr_graph.h). */
+int lfr_wire_walk_matches(const uint8_t* buf, uint64_t len, lfr_wire_matches* out, uint64_t* match_off);
+
 /* Encode a MatchingFile.  names are concatenated in `names`, name k =
  * names[name_off[k], name_off[k+1]).  pair_name1/2[p] index names.
  * Returns the number of bytes needed; writes only if cap is large enough. */

@@ -77,7 +77,13 @@ ABI_SYMBOLS = [
     "lfr_plan_traffic", "lfr_plan_destroy", "lfr_debug_edge_eval",
 ]
 #: the symbols include/lfr_graph.h declares
-GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_export_graph", "lfr_graph_stage_on_device"]
+GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
+                 "lfr_graph_stage_on_device", "lfr_wire_decode_on_device"]
+
+
+class LfrWirePart(C.Structure):
+    """lfr_wire_part (include/lfr_graph.h)"""
+    _fields_ = [("buf", C.c_void_p), ("len", C.c_uint64), ("match_off", C.c_void_p), ("n_matches", C.c_uint64)]
 
 
 def _ptr(a: Optional[np.ndarray]) -> Optional[int]:
@@ -132,10 +138,16 @@ class Library:
             L.lfr_plan_create_from_matches.argtypes = [C.POINTER(HostInput), C.POINTER(LfrOptions), C.c_void_p,
                                                        C.POINTER(C.c_void_p), C.POINTER(HostSizes)]
             L.lfr_plan_create_from_matches.restype = C.c_int
+            L.lfr_plan_create_from_wire.argtypes = [C.POINTER(HostInput), C.POINTER(LfrWirePart), C.c_uint32,
+                                                    C.POINTER(LfrOptions), C.c_void_p, C.POINTER(C.c_void_p),
+                                                    C.POINTER(HostSizes)]
+            L.lfr_plan_create_from_wire.restype = C.c_int
             L.lfr_plan_export_graph.argtypes = [C.c_void_p] * 11
             L.lfr_plan_export_graph.restype = C.c_int
             L.lfr_graph_stage_on_device.argtypes = [C.POINTER(HostInput), C.c_int32]
             L.lfr_graph_stage_on_device.restype = C.c_int
+            L.lfr_wire_decode_on_device.argtypes = [C.c_uint64]
+            L.lfr_wire_decode_on_device.restype = C.c_int
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -345,8 +357,58 @@ class Plan:
         self.n_nodes, self.n_components = int(sz.n_nodes), int(sz.n_components)
         return self
 
+    @classmethod
+    def from_wire(cls, lib: Library, parts, banned_images=(), options: Optional[LfrOptions] = None) -> "Plan":
+        """lfr_plan_create_from_wire (include/lfr_graph.h): the plan of from_matches() on the decode of
+        `parts` — the bytes of one MatchingFile, or of its `.part.N` pieces in order — with the matches
+        decoded on the device.  The pair level (image names in order of first appearance, banned images)
+        is walked on the host (wire.walk_matching_file).  Raises wire.ParseError where the pair walk
+        fails, and RuntimeError "... (-1): malformed Match message" where a match does not decode."""
+        from . import wire
+        if not lib.has_graph_stage:  # e.g. the CPU oracle: no device, no plans
+            raise RuntimeError("lfr: lfr_plan_create_from_wire failed (-5): %s does not provide the graph stage "
+                               "on the GPU (include/lfr_graph.h)" % lib.path)
+        names, index = [], {}
+        img1, img2, ptr, keep = [], [], [np.zeros(1, np.uint64)], []
+        wparts = (LfrWirePart * max(len(parts), 1))()
+        m0 = 0
+        for i, data in enumerate(parts):
+            a = wire.walk_matching_file(data)
+            i1, i2 = wire.intern_names(data, a, names, index)
+            img1.append(i1)
+            img2.append(i2)
+            ptr.append(a["pair_ptr"][1:] + np.uint64(m0))
+            buf = np.frombuffer(data, dtype=np.uint8)
+            keep += [buf, a["match_off"]]
+            n = int(a["match_off"].shape[0])
+            wparts[i] = LfrWirePart(buf=buf.ctypes.data if buf.size else None, len=buf.size,
+                                    match_off=a["match_off"].ctypes.data if n else None, n_matches=n)
+            m0 += n
+        cat = lambda xs: np.concatenate(xs) if xs else np.zeros(0, np.int64)  # noqa: E731
+        pair_img1, pair_img2 = cat(img1).astype(np.uint32), cat(img2).astype(np.uint32)
+        banned = set(banned_images)
+        skip = np.array([(names[x] in banned) or (names[y] in banned) for x, y in zip(pair_img1.tolist(), pair_img2.tolist())],
+                        dtype=np.uint8).reshape(-1)
+        pair_ptr = np.ascontiguousarray(np.concatenate(ptr), dtype=np.uint64)
+        arrs = dict(pair_img1=pair_img1, pair_img2=pair_img2, pair_skip=skip, pair_ptr=pair_ptr)
+        inp = HostInput(n_pairs=pair_img1.shape[0], n_matches=m0, n_images=len(names),
+                        **{k: (v.ctypes.data if v.size else None) for k, v in arrs.items()})
+        o = options if options is not None else lib.default_options()
+        self = cls.__new__(cls)
+        self.lib, self.problem, self.handle = lib, None, None
+        h = C.c_void_p()
+        sz = HostSizes()
+        lib.check(lib.lib.lfr_plan_create_from_wire(C.byref(inp), wparts, len(parts), C.byref(o), None, C.byref(h),
+                                                    C.byref(sz)), "lfr_plan_create_from_wire")
+        del keep
+        self.handle = h
+        self.sizes = {k: getattr(sz, k) for k in HOST_SIZES_FIELDS}
+        self.n_nodes, self.n_components = int(sz.n_nodes), int(sz.n_components)
+        self.image_names = names
+        return self
+
     def export_graph(self) -> dict:
-        """lfr_plan_export_graph: the stage's arrays of a plan made by from_matches(), named as in
+        """lfr_plan_export_graph: the stage's arrays of a plan made by from_matches() or from_wire(), named as in
         lfr_host_stage_export (edges: [E] EDGE_DTYPE records, copied from the device)."""
         out = stage_outputs(self.n_nodes, self.n_components, int(self.sizes["n_edges"]))
         self.lib.check(self.lib.lib.lfr_plan_export_graph(self.handle, *[(a.ctypes.data if a.size else None)

@@ -20,6 +20,7 @@
 #include "lfr_solve_tile.cuh"
 #include "lfr_solve_warp.cuh"
 #include "lfr_solve_warp2.cuh"
+#include "lfr_wire.cuh"
 
 namespace {
 
@@ -842,16 +843,30 @@ double ms_since(Clock::time_point t0) { return std::chrono::duration<double, std
 // §4): the host route is faster up to ~10 K directed edges and the device route from 200 K on; in between
 // the two trade places from run to run within their spread, and the switch sits inside that tie.
 constexpr uint64_t kDeviceGraphStageMinEdges = 32768;
+// lfr_wire_decode_on_device(): the matches from which the drop-in decodes them on the device.  On an
+// H100 80GB HBM3 (tools/gpu_wire_decode_time.py, DESIGN.md §4) lfr_plan_create_from_wire() alone beats the
+// host decode + lfr_plan_create_from_matches() from 100 K matches on, but the drop-in's host decode runs
+// while CUDA starts up: its wall time gains from 634 K matches (cfg4) on and ties at 100-137 K.
+constexpr uint64_t kDeviceDecodeMinMatches = 262144;
+// lfr_last_error() of lfr_plan_create_from_wire() on a malformed Match (include/lfr_graph.h)
+constexpr const char* kMalformedMatch = "malformed Match message";
 
-// lfr_host_stage_create() on the device, block for block (lfr_host.cc): the edge records go into
-// pl->edges, the other arrays come back to pl->graph (the schedule builder is host code and reads them).
-int build_graph_on_device(const lfr_host_input* in, lfr_plan* pl, lfr_host_sizes* S, cudaStream_t s) {
+// The graph stage's input on the device: feat1 / feat2 / sim [n_matches], disp1 / disp2 [18 n_matches],
+// match k of every pair at its global index (the order of lfr_host_input).
+struct MatchArrays {
+  TmpBuf feat1, feat2, sim, disp1, disp2;
+};
+
+// lfr_host_stage_create() on the device, block for block (lfr_host.cc), from the pair level of `in` and the
+// device-resident matches `d` (in->feat1 ... in->disp2 are not read): the edge records go into pl->edges,
+// the other arrays come back to pl->graph (the schedule builder is host code and reads them).
+int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl, lfr_host_sizes* S, cudaStream_t s) {
   using namespace lfr::graph;
   std::memset(S, 0, sizeof *S);
   auto G = std::make_unique<lfr_plan::GraphArrays>();
-  const uint64_t P = in->n_pairs, M_all = in->n_matches;
+  const uint64_t P = in->n_pairs;
   const uint32_t n_images = in->n_images;
-  TmpBuf tmp, d_img1, d_img2, d_skip, d_ptr, d_feat1, d_feat2, d_sim, d_disp1, d_disp2, d_cnt, d_off, d_seen, d_err;
+  TmpBuf tmp, d_img1, d_img2, d_skip, d_ptr, d_cnt, d_off, d_seen, d_err;
   const auto t_graph = Clock::now();
   // ---- H1: the match list -------------------------------------------------------------------------
   uint64_t M = 0;
@@ -888,17 +903,14 @@ int build_graph_on_device(const lfr_host_input* in, lfr_plan* pl, lfr_host_sizes
   TmpBuf d_kept, d_key, d_key2, d_pos, d_pos2, d_first, d_id, d_head, d_headof, d_nop;
   uint32_t N = 0;
   if (M) {
-    LFR_TRY(upload(&d_feat1, in->feat1, M_all, s));
-    LFR_TRY(upload(&d_feat2, in->feat2, M_all, s));
-    LFR_TRY(upload(&d_sim, in->sim, M_all, s));
     LFR_TRY(d_kept.reserve(8 * M));
     LFR_TRY(d_key.reserve(8 * E));
     LFR_TRY(d_key2.reserve(8 * E));
     LFR_TRY(d_pos.reserve(4 * E));
     LFR_TRY(d_pos2.reserve(4 * E));
     expand_matches_kernel<<<blocks_for(M), 256, 0, s>>>(d_off.as<uint64_t>(), P, d_img1.as<uint32_t>(), d_img2.as<uint32_t>(),
-                                                        d_ptr.as<uint64_t>(), d_feat1.as<uint32_t>(), d_feat2.as<uint32_t>(),
-                                                        d_sim.as<float>(), M, d_kept.as<uint64_t>(),
+                                                        d_ptr.as<uint64_t>(), d.feat1.as<uint32_t>(), d.feat2.as<uint32_t>(),
+                                                        d.sim.as<float>(), M, d_kept.as<uint64_t>(),
                                                         d_key.as<unsigned long long>(), d_pos.as<uint32_t>(), d_err.as<int>());
     LFR_LAUNCHED();
     int err[2];
@@ -965,17 +977,15 @@ int build_graph_on_device(const lfr_host_input* in, lfr_plan* pl, lfr_host_sizes
   }
   LFR_TRY(d_rowptr.reserve(4 * ((size_t)N + 1)));
   row_ptr_kernel<<<blocks_for(E), 256, 0, s>>>(d_ssrc.as<uint32_t>(), E, N, d_rowptr.as<uint32_t>());
-  LFR_TRY(upload(&d_disp1, in->disp1, 18 * M_all, s));
-  LFR_TRY(upload(&d_disp2, in->disp2, 18 * M_all, s));
   LFR_TRY(pl->edges.reserve(sizeof(lfr_edge) * E));
   LFR_TRY(d_cdst.reserve(4 * E));
   LFR_TRY(d_csim.reserve(4 * E));
   edge_records_kernel<<<blocks_for(E), 256, 0, s>>>(d_perm.as<uint32_t>(), E, d_kept.as<uint64_t>(), d_nop.as<uint32_t>(),
-                                                    d_sim.as<float>(), d_disp1.as<float>(), d_disp2.as<float>(),
+                                                    d.sim.as<float>(), d.disp1.as<float>(), d.disp2.as<float>(),
                                                     pl->edges.as<lfr_edge>(), d_cdst.as<uint32_t>(), d_csim.as<float>());
   LFR_LAUNCHED();
-  d_disp1.release();
-  d_disp2.release();
+  d.disp1.release();
+  d.disp2.release();
   LFR_CUDA(cudaStreamSynchronize(s));
   S->graph_ms = ms_since(t_graph);
   const auto t_tracks = Clock::now();
@@ -992,7 +1002,7 @@ int build_graph_on_device(const lfr_host_input* in, lfr_plan* pl, lfr_host_sizes
       return cub::DeviceRadixSort::SortPairs(t, nb, n2k, n2s, iota, perm1, (int)M, 0, nb1, s);
     }));
     unsigned long long *k1 = d_key.as<unsigned long long>(), *k2 = d_key2.as<unsigned long long>();
-    kruskal_keys2_kernel<<<blocks_for(M), 256, 0, s>>>(perm1, d_kept.as<uint64_t>(), d_nop.as<uint32_t>(), d_sim.as<float>(), M, nb1, k1);
+    kruskal_keys2_kernel<<<blocks_for(M), 256, 0, s>>>(perm1, d_kept.as<uint64_t>(), d_nop.as<uint32_t>(), d.sim.as<float>(), M, nb1, k1);
     LFR_LAUNCHED();
     uint32_t* ord = d_order.as<uint32_t>();
     LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
@@ -1307,6 +1317,150 @@ int build_graph_on_device(const lfr_host_input* in, lfr_plan* pl, lfr_host_sizes
   S->n_components = C;
   S->max_component_size = C ? G->comp_ptr[1] - G->comp_ptr[0] : 0;
   pl->graph = std::move(G);
+  return LFR_OK;
+}
+
+// lfr_plan_create_from_matches(): the decoded match arrays of `in` go up as they are
+int upload_matches(const lfr_host_input* in, MatchArrays& d, cudaStream_t s) {
+  const size_t M = in->n_matches;
+  LFR_TRY(upload(&d.feat1, in->feat1, M, s));
+  LFR_TRY(upload(&d.feat2, in->feat2, M, s));
+  LFR_TRY(upload(&d.sim, in->sim, M, s));
+  LFR_TRY(upload(&d.disp1, in->disp1, 18 * M, s));
+  LFR_TRY(upload(&d.disp2, in->disp2, 18 * M, s));
+  return LFR_OK;
+}
+
+// Host -> device copies of caller memory that may be pageable (a mapped file): through two page-locked
+// chunks, so that the host copy into one overlaps the DMA out of the other.
+struct Stager {
+  static constexpr size_t kChunk = 8u << 20;
+  uint8_t* h[2] = {};
+  cudaEvent_t ev[2] = {};
+  size_t chunk = 0;
+  int k = 0;
+  int init(size_t largest) {
+    chunk = std::max<size_t>(std::min(kChunk, largest), 1);
+    for (int i = 0; i < 2; ++i) {
+      LFR_CUDA(cudaHostAlloc((void**)&h[i], chunk, cudaHostAllocDefault));
+      LFR_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
+    }
+    return LFR_OK;
+  }
+  int put(void* dst, const void* src, size_t bytes, cudaStream_t s) {
+    for (size_t o = 0; o < bytes; o += chunk) {
+      const size_t b = std::min(chunk, bytes - o);
+      LFR_CUDA(cudaEventSynchronize(ev[k]));  // this chunk's previous DMA has finished
+      std::memcpy(h[k], static_cast<const uint8_t*>(src) + o, b);
+      LFR_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(dst) + o, h[k], b, cudaMemcpyHostToDevice, s));
+      LFR_CUDA(cudaEventRecord(ev[k], s));
+      k ^= 1;
+    }
+    return LFR_OK;
+  }
+  ~Stager() {
+    for (int i = 0; i < 2; ++i) {
+      if (ev[i]) {
+        cudaEventSynchronize(ev[i]);
+        cudaEventDestroy(ev[i]);
+      }
+      if (h[i]) cudaFreeHost(h[i]);
+    }
+  }
+};
+
+// {staging + copy, decode kernels} in ms of the calling thread's last lfr_plan_create_from_wire()
+thread_local double g_wire_ms[2] = {};
+
+// lfr_plan_create_from_wire(): every part's bytes and match offsets go up through the stager and every
+// Match is decoded on the device into `d` at its global index (parts in order).  LFR_EINVAL when a match
+// is malformed, before the graph stage sees anything.
+int decode_wire_on_device(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts, MatchArrays& d,
+                          cudaStream_t s) {
+  g_wire_ms[0] = g_wire_ms[1] = 0;
+  const size_t M = in->n_matches;
+  uint64_t total = 0;
+  size_t max_len = 0, max_n = 0;
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    const lfr_wire_part& pt = parts[i];
+    if ((!pt.buf && pt.len) || (!pt.match_off && pt.n_matches)) return fail(LFR_EINVAL, "NULL part buffer or match offsets");
+    total += pt.n_matches;
+    if (pt.n_matches) {
+      max_len = std::max<size_t>(max_len, pt.len);
+      max_n = std::max<size_t>(max_n, pt.n_matches);
+    }
+  }
+  if (total != M) return fail(LFR_EINVAL, "the parts' match counts do not add up to n_matches");
+  LFR_TRY(d.feat1.reserve(4 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.feat2.reserve(4 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.sim.reserve(4 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.disp1.reserve(72 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.disp2.reserve(72 * std::max<size_t>(M, 1)));
+  if (!M) return LFR_OK;
+  const auto t0 = Clock::now();
+  LFR_CUDA(cudaMemsetAsync(d.disp1.p, 0, 72 * M, s));
+  LFR_CUDA(cudaMemsetAsync(d.disp2.p, 0, 72 * M, s));
+  TmpBuf d_bytes, d_moff, d_err;
+  LFR_TRY(d_bytes.reserve(std::max<size_t>(max_len, 1)));
+  LFR_TRY(d_moff.reserve(8 * max_n));
+  LFR_TRY(d_err.reserve(4));
+  LFR_CUDA(cudaMemsetAsync(d_err.p, 0, 4, s));
+  Stager st;
+  LFR_TRY(st.init(std::max<size_t>(max_len, 8 * max_n)));
+  std::vector<cudaEvent_t> ev;
+  struct EventsFree {
+    std::vector<cudaEvent_t>& v;
+    ~EventsFree() { for (cudaEvent_t e : v) cudaEventDestroy(e); }
+  } ev_free{ev};
+  uint64_t m0 = 0;
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    const lfr_wire_part& pt = parts[i];
+    if (!pt.n_matches) continue;
+    LFR_TRY(st.put(d_bytes.p, pt.buf, pt.len, s));
+    LFR_TRY(st.put(d_moff.p, pt.match_off, 8 * pt.n_matches, s));
+    cudaEvent_t e[2];
+    for (cudaEvent_t& x : e) {
+      LFR_CUDA(cudaEventCreate(&x));
+      ev.push_back(x);
+    }
+    LFR_CUDA(cudaEventRecord(e[0], s));
+    lfr::wire::decode_matches_kernel<<<blocks_for(pt.n_matches), 256, 0, s>>>(
+        d_bytes.as<uint8_t>(), pt.len, d_moff.as<uint64_t>(), pt.n_matches, m0, d.feat1.as<uint32_t>(),
+        d.feat2.as<uint32_t>(), d.sim.as<float>(), d.disp1.as<float>(), d.disp2.as<float>(), d_err.as<int>());
+    LFR_LAUNCHED();
+    LFR_CUDA(cudaEventRecord(e[1], s));
+    m0 += pt.n_matches;
+  }
+  int err = 0;
+  LFR_TRY(fetch(&err, d_err.p, 1, s));
+  for (size_t j = 0; j < ev.size(); j += 2) {
+    float ms = 0.f;
+    LFR_CUDA(cudaEventElapsedTime(&ms, ev[j], ev[j + 1]));
+    g_wire_ms[1] += ms;
+  }
+  g_wire_ms[0] = ms_since(t0) - g_wire_ms[1];
+  if (err) return fail(LFR_EINVAL, kMalformedMatch);
+  return LFR_OK;
+}
+
+// The two entry points from matches: the stage on the device-resident `d`, then the plan.
+int create_plan_from_graph(const lfr_host_input* in, MatchArrays& d, const lfr_options& o, const double* initial_positions,
+                           lfr_plan* pl, lfr_host_sizes* S) {
+  LFR_TRY(build_graph_on_device(in, d, pl, S, 0));
+  const lfr_plan::GraphArrays& G = *pl->graph;
+  lfr_problem p;
+  p.n_nodes = S->n_nodes;
+  p.n_components = S->n_components;
+  p.n_edges = S->n_edges;
+  p.row_ptr = G.row_ptr.data();
+  p.edges = nullptr;  // already in pl->edges
+  p.track = G.track.data();
+  p.comp = G.comp.data();
+  p.is_root = G.is_root.data();
+  p.comp_ptr = G.comp_ptr.data();
+  p.comp_nodes = G.comp_nodes.data();
+  LFR_TRY(fill_plan(pl, &p, o, initial_positions, 0, false, nullptr, nullptr, /*graph_resident=*/true));
+  LFR_CUDA(cudaStreamSynchronize(0));
   return LFR_OK;
 }
 
@@ -1641,32 +1795,46 @@ int lfr_plan_create_from_matches(const lfr_host_input* in, const lfr_options* op
   lfr_plan* pl = new lfr_plan();
   pl->device = o.device;
   lfr_host_sizes S;
-  int rc = build_graph_on_device(in, pl, &S, 0);
-  if (rc == LFR_OK) {
-    const lfr_plan::GraphArrays& G = *pl->graph;
-    lfr_problem p;
-    p.n_nodes = S.n_nodes;
-    p.n_components = S.n_components;
-    p.n_edges = S.n_edges;
-    p.row_ptr = G.row_ptr.data();
-    p.edges = nullptr;  // already in pl->edges
-    p.track = G.track.data();
-    p.comp = G.comp.data();
-    p.is_root = G.is_root.data();
-    p.comp_ptr = G.comp_ptr.data();
-    p.comp_nodes = G.comp_nodes.data();
-    rc = fill_plan(pl, &p, o, initial_positions, 0, false, nullptr, nullptr, /*graph_resident=*/true);
-  }
-  if (rc == LFR_OK) {
-    cudaError_t e = cudaStreamSynchronize(0);
-    if (e != cudaSuccess) rc = fail(cuda_code(e), cudaGetErrorString(e));
-  }
+  MatchArrays d;
+  int rc = upload_matches(in, d, 0);
+  if (rc == LFR_OK) rc = create_plan_from_graph(in, d, o, initial_positions, pl, &S);
   if (rc) {
     free_plan(pl);
     return rc;
   }
   if (sizes) *sizes = S;
   *out = pl;
+  return LFR_OK;
+}
+
+int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
+                              const lfr_options* opt, const double* initial_positions, lfr_plan** out,
+                              lfr_host_sizes* sizes) {
+  if (!out) return fail(LFR_EINVAL, "out is NULL");
+  *out = nullptr;
+  if (!in) return fail(LFR_EINVAL, "input is NULL");
+  if (n_parts && !parts) return fail(LFR_EINVAL, "parts is NULL");
+  lfr_options o;
+  if (opt) o = *opt; else lfr_options_default(&o);
+  LFR_TRY(select_device(o));
+  lfr_plan* pl = new lfr_plan();
+  pl->device = o.device;
+  lfr_host_sizes S;
+  MatchArrays d;
+  int rc = decode_wire_on_device(in, parts, n_parts, d, 0);
+  if (rc == LFR_OK) rc = create_plan_from_graph(in, d, o, initial_positions, pl, &S);
+  if (rc) {
+    free_plan(pl);
+    return rc;
+  }
+  if (sizes) *sizes = S;
+  *out = pl;
+  return LFR_OK;
+}
+
+int lfr_debug_last_wire_times(double* out2) {
+  out2[0] = g_wire_ms[0];
+  out2[1] = g_wire_ms[1];
   return LFR_OK;
 }
 
@@ -1707,6 +1875,8 @@ int lfr_graph_stage_on_device(const lfr_host_input* in, int32_t n_devices) {
   }
   return e >= kDeviceGraphStageMinEdges && e < (1ull << 31) ? 1 : 0;
 }
+
+int lfr_wire_decode_on_device(uint64_t n_matches) { return n_matches >= kDeviceDecodeMinMatches ? 1 : 0; }
 
 int lfr_plan_solve(lfr_plan* pl, void* stream) {
   if (!pl) return fail(LFR_EINVAL, "plan is NULL");

@@ -6,13 +6,15 @@
 // Same flags (solve.cc:379-385, Boost.Program_options semantics and messages), same `.part.N` handling
 // (:416-424), same stdout lines (:484-485,534,549,589,591,606,638,641,670) and exit codes (0; 1 on a
 // command-line error, :397-401; -1 = 255 when the input does not parse or the output cannot be
-// written, :433-436,674-677).  The work is lfr_wire_decode_matches() (include/lfr_wire.h), the graph
-// stage and the solve, then lfr_wire_encode_solution().  The graph stage runs where
-// lfr_graph_stage_on_device() (include/lfr_graph.h) says, from the input's size:
-//   device: lfr_plan_create_from_matches(), lfr_plan_solve() + lfr_plan_download() on the plan it left
+// written, :433-436,674-677).  The work is lfr_wire_walk_matches() (include/lfr_wire.h) over the pairs,
+// the graph stage and the solve, then lfr_wire_encode_solution().  The graph stage runs where
+// lfr_graph_stage_on_device() (include/lfr_graph.h) says, from the pair level alone:
+//   device: lfr_plan_create_from_wire() on the mapped parts (the matches are decoded on the GPU) — or,
+//           below the match count lfr_wire_decode_on_device() sets, lfr_wire_decode_matches() +
+//           lfr_plan_create_from_matches() —, lfr_plan_solve() + lfr_plan_download() on the plan left
 //           in HBM, and lfr_plan_export_graph() for the node -> (image, feature) ids;
-//   host:   lfr_host_stage_create() (include/lfr_host.h) writing the edge records into page-locked
-//           memory, then lfr_solve() / lfr_solve_multi() (include/lfr.h).
+//   host:   lfr_wire_decode_matches(), lfr_host_stage_create() (include/lfr_host.h) writing the edge
+//           records into page-locked memory, then lfr_solve() / lfr_solve_multi() (include/lfr.h).
 // Both routes give the same bytes and lines.  LFR_GRAPH_STAGE=host|device forces a route (a test and
 // measurement hook).  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
@@ -41,11 +43,15 @@
 #include "../../include/lfr_wire.h"
 
 // The graph stage on the GPU is resolved weakly: the same source links against the CPU checker
-// (oracle/liblfr_ref.so), which has no plans; there the three are NULL and every input takes the host route.
+// (oracle/liblfr_ref.so), which has no plans; there they are NULL and every input takes the host route.
 extern "C" {
 int lfr_graph_stage_on_device(const lfr_host_input* in, int32_t n_devices) __attribute__((weak));
+int lfr_wire_decode_on_device(uint64_t n_matches) __attribute__((weak));
 int lfr_plan_create_from_matches(const lfr_host_input* in, const lfr_options* o, const double* initial_positions,
                                  lfr_plan** out, lfr_host_sizes* sizes) __attribute__((weak));
+int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
+                              const lfr_options* o, const double* initial_positions, lfr_plan** out,
+                              lfr_host_sizes* sizes) __attribute__((weak));
 int lfr_plan_export_graph(const lfr_plan* plan, uint32_t* row_ptr, lfr_edge* edges, uint32_t* track, uint32_t* comp,
                           uint8_t* is_root, uint32_t* comp_ptr, uint32_t* comp_nodes, uint32_t* comp_order,
                           uint32_t* node_image, uint32_t* node_feat) __attribute__((weak));
@@ -185,13 +191,23 @@ struct FileImage {
   size_t size() const { return n; }
 };
 
-// One decoded MatchingFile part, image names still as byte ranges of its buffer.
+// One MatchingFile part after the pair walk: image names as byte ranges of its buffer, the matches as
+// the offsets of their length prefixes.
 struct Part {
   FileImage buf;
   uint64_t P = 0, M = 0;
-  std::vector<uint64_t> pair_ptr, n1_off, n2_off;
-  std::vector<uint32_t> n1_len, n2_len, feat1, feat2;
-  std::vector<float> fact1, fact2, sim, disp1, disp2;
+  std::vector<uint64_t> pair_ptr, n1_off, n2_off, match_off;
+  std::vector<uint32_t> n1_len, n2_len;
+  std::vector<float> fact1, fact2;
+  lfr_wire_matches pair_level(uint32_t* feat1, uint32_t* feat2, float* sim, float* disp1, float* disp2) {
+    lfr_wire_matches w;
+    w.n_pairs = P; w.n_matches = M;
+    w.pair_ptr = pair_ptr.data(); w.fact1 = fact1.data(); w.fact2 = fact2.data();
+    w.name1_off = n1_off.data(); w.name1_len = n1_len.data();
+    w.name2_off = n2_off.data(); w.name2_len = n2_len.data();
+    w.feat1 = feat1; w.feat2 = feat2; w.sim = sim; w.disp1 = disp1; w.disp2 = disp2;
+    return w;
+  }
 };
 
 using Clock = std::chrono::steady_clock;
@@ -260,16 +276,9 @@ int main(int argc, char** argv) {
       pt.pair_ptr.resize(pt.P + 1);
       pt.n1_off.resize(pt.P); pt.n2_off.resize(pt.P); pt.n1_len.resize(pt.P); pt.n2_len.resize(pt.P);
       pt.fact1.resize(pt.P); pt.fact2.resize(pt.P);
-      pt.feat1.resize(pt.M); pt.feat2.resize(pt.M); pt.sim.resize(pt.M);
-      pt.disp1.resize(18 * pt.M); pt.disp2.resize(18 * pt.M);
-      lfr_wire_matches w;
-      w.n_pairs = pt.P; w.n_matches = pt.M;
-      w.pair_ptr = pt.pair_ptr.data(); w.fact1 = pt.fact1.data(); w.fact2 = pt.fact2.data();
-      w.name1_off = pt.n1_off.data(); w.name1_len = pt.n1_len.data();
-      w.name2_off = pt.n2_off.data(); w.name2_len = pt.n2_len.data();
-      w.feat1 = pt.feat1.data(); w.feat2 = pt.feat2.data(); w.sim = pt.sim.data();
-      w.disp1 = pt.disp1.data(); w.disp2 = pt.disp2.data();
-      ok = lfr_wire_decode_matches(pt.buf.data(), pt.buf.size(), &w) == LFR_OK;
+      pt.match_off.resize(pt.M);
+      lfr_wire_matches w = pt.pair_level(nullptr, nullptr, nullptr, nullptr, nullptr);
+      ok = lfr_wire_walk_matches(pt.buf.data(), pt.buf.size(), &w, pt.match_off.data()) == LFR_OK;
     }
     if (!ok) {
       std::fputs("Failed to parse proto object.\n", stderr);  // solve.cc:433-436
@@ -294,14 +303,6 @@ int main(int argc, char** argv) {
   std::vector<uint32_t> pair_img1(P), pair_img2(P);
   std::vector<float> pair_fact1(P), pair_fact2(P);
   std::vector<uint64_t> pair_ptr(P + 1, 0);
-  // single part: the decoded arrays are used in place; several: concatenated
-  std::vector<uint32_t> feat1_cat, feat2_cat;
-  std::vector<float> sim_cat, disp1_cat, disp2_cat;
-  const bool cat = parts.size() > 1;
-  if (cat) {
-    feat1_cat.reserve(M); feat2_cat.reserve(M); sim_cat.reserve(M);
-    disp1_cat.reserve(18 * M); disp2_cat.reserve(18 * M);
-  }
   {
     uint64_t p0 = 0, m0 = 0;
     for (Part& pt : parts) {
@@ -312,30 +313,10 @@ int main(int argc, char** argv) {
         pair_fact2[p0 + p] = pt.fact2[p];
         pair_ptr[p0 + p + 1] = m0 + pt.pair_ptr[p + 1];
       }
-      if (cat) {
-        feat1_cat.insert(feat1_cat.end(), pt.feat1.begin(), pt.feat1.end());
-        feat2_cat.insert(feat2_cat.end(), pt.feat2.begin(), pt.feat2.end());
-        sim_cat.insert(sim_cat.end(), pt.sim.begin(), pt.sim.end());
-        disp1_cat.insert(disp1_cat.end(), pt.disp1.begin(), pt.disp1.end());
-        disp2_cat.insert(disp2_cat.end(), pt.disp2.begin(), pt.disp2.end());
-      }
       p0 += pt.P;
       m0 += pt.M;
-      pt.buf.release();  // the file image (several GB at Madrid scale) is not needed past the names
-      if (cat) {
-        std::vector<uint32_t>().swap(pt.feat1);
-        std::vector<uint32_t>().swap(pt.feat2);
-        std::vector<float>().swap(pt.sim);
-        std::vector<float>().swap(pt.disp1);
-        std::vector<float>().swap(pt.disp2);
-      }
     }
   }
-  const uint32_t* feat1 = cat ? feat1_cat.data() : (parts.empty() ? nullptr : parts[0].feat1.data());
-  const uint32_t* feat2 = cat ? feat2_cat.data() : (parts.empty() ? nullptr : parts[0].feat2.data());
-  const float* sim = cat ? sim_cat.data() : (parts.empty() ? nullptr : parts[0].sim.data());
-  const float* disp1 = cat ? disp1_cat.data() : (parts.empty() ? nullptr : parts[0].disp1.data());
-  const float* disp2 = cat ? disp2_cat.data() : (parts.empty() ? nullptr : parts[0].disp2.data());
 
   // banned images (solve.cc:444-446) and the first fact seen of every image among the pairs kept
   const std::set<std::string> banned(banned_list.begin(), banned_list.end());
@@ -355,12 +336,13 @@ int main(int argc, char** argv) {
   std::memset(&in, 0, sizeof in);
   in.n_pairs = P; in.n_matches = M; in.n_images = (uint32_t)names.size();
   in.pair_img1 = pair_img1.data(); in.pair_img2 = pair_img2.data(); in.pair_skip = skip.data();
-  in.pair_ptr = pair_ptr.data(); in.feat1 = feat1; in.feat2 = feat2; in.sim = sim; in.disp1 = disp1; in.disp2 = disp2;
+  in.pair_ptr = pair_ptr.data();
 
   // ---- which graph stage: the library's size rule, or LFR_GRAPH_STAGE=host|device (a test and
   // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
   // takes the host route; forcing the device route there is an error, never a silent host run.
-  const bool have_device_stage = lfr_graph_stage_on_device && lfr_plan_create_from_matches && lfr_plan_export_graph;
+  const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
+                                 lfr_plan_create_from_wire && lfr_plan_export_graph;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -382,6 +364,27 @@ int main(int argc, char** argv) {
     }
   }
 
+  // host route, and the device route below the library's size for the decoder on the GPU: the matches of
+  // every part decoded into one set of arrays, part after part (the pair level comes out as the walk gave it)
+  const bool decode_on_device = on_device && lfr_wire_decode_on_device(M) == 1;
+  std::vector<uint32_t> feat1, feat2;
+  std::vector<float> sim, disp1, disp2;
+  if (!decode_on_device) {
+    feat1.resize(M); feat2.resize(M); sim.resize(M); disp1.resize(18 * M); disp2.resize(18 * M);
+    uint64_t m0 = 0;
+    for (Part& pt : parts) {
+      lfr_wire_matches w = pt.pair_level(feat1.data() + m0, feat2.data() + m0, sim.data() + m0, disp1.data() + 18 * m0,
+                                         disp2.data() + 18 * m0);
+      if (lfr_wire_decode_matches(pt.buf.data(), pt.buf.size(), &w) != LFR_OK) {
+        std::fputs("Failed to parse proto object.\n", stderr);  // solve.cc:433-436
+        return 255;
+      }
+      m0 += pt.M;
+      pt.buf.release();  // the file image (several GB at Madrid scale) is not needed past the decode
+    }
+    in.feat1 = feat1.data(); in.feat2 = feat2.data(); in.sim = sim.data(); in.disp1 = disp1.data(); in.disp2 = disp2.data();
+  }
+
   cuda_start.join();  // page-locked memory needs the context
   const Clock::time_point t_start = Clock::now();  // "Total time" (solve.cc:487-641): the graph work and the solve
   lfr_edge* edges = nullptr;
@@ -391,12 +394,21 @@ int main(int argc, char** argv) {
   std::vector<uint32_t> row_ptr, track, comp, comp_ptr, comp_nodes, comp_order, node_image, node_feat;
   std::vector<uint8_t> is_root;
   if (on_device) {
-    // ---- the graph stage on the GPU (include/lfr_graph.h): the problem stays in HBM for the solve and
-    // only the per-node image / feature ids come back for the SolutionFile
+    // ---- the matches decoded and the graph stage run on the GPU (include/lfr_graph.h): the problem stays
+    // in HBM for the solve and only the per-node image / feature ids come back for the SolutionFile
     lfr_options opt;
     lfr_options_default(&opt);
     opt.device = (int32_t)device;
-    const int rc = lfr_plan_create_from_matches(&in, &opt, nullptr, &plan, &sz);
+    std::vector<lfr_wire_part> wparts;
+    for (const Part& pt : parts) wparts.push_back(lfr_wire_part{pt.buf.data(), pt.buf.size(), pt.match_off.data(), pt.M});
+    const int rc = decode_on_device
+                       ? lfr_plan_create_from_wire(&in, wparts.data(), (uint32_t)wparts.size(), &opt, nullptr, &plan, &sz)
+                       : lfr_plan_create_from_matches(&in, &opt, nullptr, &plan, &sz);
+    for (Part& pt : parts) pt.buf.release();
+    if (rc == LFR_EINVAL && std::strcmp(lfr_last_error(), "malformed Match message") == 0) {
+      std::fputs("Failed to parse proto object.\n", stderr);  // solve.cc:433-436, as the host decode
+      return 255;
+    }
     if (rc == LFR_EINVAL || rc == LFR_EUNSUPPORTED) {  // the input, as the host stage would reject it
       std::fprintf(stderr, "ERROR: the host graph stage rejected the input\n");
       return 2;

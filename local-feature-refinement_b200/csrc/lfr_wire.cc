@@ -119,9 +119,10 @@ bool read_match(Reader r, lfr_wire_matches* o, uint64_t m) {
 
 // ImagePair { string image_name1 = 1; float fact1 = 2; string image_name2 = 3;
 //             float fact2 = 4; repeated Match matches = 5; }
-// count_only: match payloads are skipped by their length (their contents are validated by the decode)
+// count_only: match payloads are skipped by their length (their contents are validated by the decode);
+// match_off (header_only): the byte offset of every match's length prefix is recorded instead
 bool read_pair(Reader r, const uint8_t* base, lfr_wire_matches* o, uint64_t pair, uint64_t* m, bool count_only = false,
-               bool header_only = false) {
+               bool header_only = false, uint64_t* match_off = nullptr) {
   if (o) {
     o->fact1[pair] = o->fact2[pair] = 0.f;
     o->name1_off[pair] = o->name2_off[pair] = 0;
@@ -140,8 +141,13 @@ bool read_pair(Reader r, const uint8_t* base, lfr_wire_matches* o, uint64_t pair
     } else if (field == 2 && wt == 5) { const float f = r.f32(); if (o) o->fact1[pair] = f; }
     else if (field == 4 && wt == 5) { const float f = r.f32(); if (o) o->fact2[pair] = f; }
     else if (field == 5 && wt == 2) {
+      const uint64_t at = (uint64_t)(r.p - base);
       Reader mm = r.sub();
       if (!r.ok) return false;
+      if (match_off) {
+        if (*m >= o->n_matches) return false;
+        match_off[*m] = at;
+      }
       if (count_only || header_only) {
         ++*m;
         continue;
@@ -170,8 +176,9 @@ bool read_pair_matches(Reader r, lfr_wire_matches* o, uint64_t m, uint64_t m_end
   return r.ok && m == m_end;
 }
 
+// o == NULL: counts only.  match_off: the pair level of `o` and the match offsets only, no match decoded.
 int walk_matching_file(const uint8_t* buf, uint64_t len, lfr_wire_matches* o, uint64_t* n_pairs,
-                       uint64_t* n_matches) {
+                       uint64_t* n_matches, uint64_t* match_off = nullptr) {
   // serial walk over the pairs: header fields, match counts (match payloads skipped by length)
   Reader r{buf, buf + len};
   uint64_t pairs = 0, m = 0;
@@ -187,7 +194,8 @@ int walk_matching_file(const uint8_t* buf, uint64_t len, lfr_wire_matches* o, ui
         o->pair_ptr[pairs] = m;
         pair_payload.push_back(pr);
       }
-      if (!read_pair(pr, buf, o, pairs, &m, /*count_only=*/o == nullptr, /*header_only=*/o != nullptr)) return LFR_EINVAL;
+      if (!read_pair(pr, buf, o, pairs, &m, /*count_only=*/o == nullptr, /*header_only=*/o != nullptr, match_off))
+        return LFR_EINVAL;
       ++pairs;
     } else r.skip(wt);
   }
@@ -197,6 +205,7 @@ int walk_matching_file(const uint8_t* buf, uint64_t len, lfr_wire_matches* o, ui
   if (!o) return LFR_OK;
   if (m > o->n_matches) return LFR_EINVAL;
   o->pair_ptr[pairs] = m;
+  if (match_off) return LFR_OK;
   // the matches of every pair, pairs dealt to worker threads (a pair's matches land at pair_ptr[pair]:
   // the output does not depend on the thread count)
   unsigned n_thr = 1;
@@ -294,6 +303,15 @@ int lfr_wire_decode_matches(const uint8_t* buf, uint64_t len, lfr_wire_matches* 
   if ((!buf && len) || !out) return LFR_EINVAL;
   uint64_t np = 0, nm = 0;
   const int rc = walk_matching_file(buf, len, out, &np, &nm);
+  if (rc) return rc;
+  if (np != out->n_pairs || nm != out->n_matches) return LFR_EINVAL;
+  return LFR_OK;
+}
+
+int lfr_wire_walk_matches(const uint8_t* buf, uint64_t len, lfr_wire_matches* out, uint64_t* match_off) {
+  if ((!buf && len) || !out || (!match_off && out->n_matches)) return LFR_EINVAL;
+  uint64_t np = 0, nm = 0;
+  const int rc = walk_matching_file(buf, len, out, &np, &nm, match_off);
   if (rc) return rc;
   if (np != out->n_pairs || nm != out->n_matches) return LFR_EINVAL;
   return LFR_OK;

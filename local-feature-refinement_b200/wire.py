@@ -26,7 +26,7 @@ class WireMatches(C.Structure):
                 ("disp1", C.c_void_p), ("disp2", C.c_void_p)]
 
 
-WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_encode_matches",
+WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
                 "lfr_wire_encode_solution", "lfr_wire_decode_solution"]
 
 _bound = False
@@ -40,6 +40,8 @@ def _lib():
         L.lfr_wire_scan_matches.restype = C.c_int
         L.lfr_wire_decode_matches.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(WireMatches)]
         L.lfr_wire_decode_matches.restype = C.c_int
+        L.lfr_wire_walk_matches.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(WireMatches), C.c_void_p]
+        L.lfr_wire_walk_matches.restype = C.c_int
         L.lfr_wire_encode_matches.argtypes = [C.c_uint64] + [C.c_void_p] * 12 + [C.c_void_p, C.c_uint64]
         L.lfr_wire_encode_matches.restype = C.c_int64
         L.lfr_wire_encode_solution.argtypes = [C.c_uint64] + [C.c_void_p] * 7 + [C.c_void_p, C.c_uint64]
@@ -67,7 +69,9 @@ def matches_files(path: str) -> List[str]:
     return out
 
 
-def decode_matching_file(data: bytes) -> MatchSet:
+def _pair_level(data: bytes, with_matches: bool) -> dict:
+    """lfr_wire_decode_matches (with_matches) or lfr_wire_walk_matches on `data`: the arrays of
+    lfr_wire_matches by field name, plus `match_off` from the walk.  Raises ParseError."""
     L = _lib()
     buf = np.frombuffer(data, dtype=np.uint8)
     np_, nm = C.c_uint64(), C.c_uint64()
@@ -79,14 +83,25 @@ def decode_matching_file(data: bytes) -> MatchSet:
         pair_ptr=np.zeros(P + 1, np.uint64), fact1=np.zeros(P, np.float32), fact2=np.zeros(P, np.float32),
         name1_off=np.zeros(P, np.uint64), name1_len=np.zeros(P, np.uint32),
         name2_off=np.zeros(P, np.uint64), name2_len=np.zeros(P, np.uint32),
-        feat1=np.zeros(M, np.uint32), feat2=np.zeros(M, np.uint32), sim=np.zeros(M, np.float32),
-        disp1=np.zeros((M, 18), np.float32), disp2=np.zeros((M, 18), np.float32),
     )
+    if with_matches:
+        a.update(feat1=np.zeros(M, np.uint32), feat2=np.zeros(M, np.uint32), sim=np.zeros(M, np.float32),
+                 disp1=np.zeros((M, 18), np.float32), disp2=np.zeros((M, 18), np.float32))
     w = WireMatches(n_pairs=P, n_matches=M, **{k: v.ctypes.data for k, v in a.items()})
-    if L.lfr_wire_decode_matches(ptr, buf.size, C.byref(w)) != 0:
+    if with_matches:
+        rc = L.lfr_wire_decode_matches(ptr, buf.size, C.byref(w))
+    else:
+        a["match_off"] = np.zeros(M, np.uint64)
+        rc = L.lfr_wire_walk_matches(ptr, buf.size, C.byref(w), a["match_off"].ctypes.data)
+    if rc != 0:
         raise ParseError("Failed to parse proto object.")
-    names: List[str] = []
-    index = {}
+    return a
+
+
+def intern_names(data: bytes, a: dict, names: List[str], index: dict):
+    """Image ids of both sides of every pair of `a` (_pair_level), names numbered in order of first
+    appearance; `names` / `index` carry the numbering across the parts of one file."""
+    P = a["pair_ptr"].shape[0] - 1
     img1 = np.zeros(P, np.int64)
     img2 = np.zeros(P, np.int64)
     for p in range(P):
@@ -96,6 +111,20 @@ def decode_matching_file(data: bytes) -> MatchSet:
                 index[nm_] = len(names)
                 names.append(nm_)
             dst[p] = index[nm_]
+    return img1, img2
+
+
+def walk_matching_file(data: bytes) -> dict:
+    """The pair level of one MatchingFile and the byte offset of every match (lfr_wire_walk_matches):
+    pair_ptr, fact1, fact2, name1_off, name1_len, name2_off, name2_len, match_off.  No match is decoded;
+    raises ParseError on what lfr_wire_scan_matches rejects."""
+    return _pair_level(data, with_matches=False)
+
+
+def decode_matching_file(data: bytes) -> MatchSet:
+    a = _pair_level(data, with_matches=True)
+    names: List[str] = []
+    img1, img2 = intern_names(data, a, names, {})
     return MatchSet(image_names=names, pair_img1=img1, pair_img2=img2, pair_fact1=a["fact1"],
                     pair_fact2=a["fact2"], pair_ptr=a["pair_ptr"].astype(np.int64), feat1=a["feat1"],
                     feat2=a["feat2"], sim=a["sim"], disp1=a["disp1"], disp2=a["disp2"])
