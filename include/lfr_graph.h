@@ -73,6 +73,21 @@ int lfr_plan_export_graph(const lfr_plan* plan, uint32_t* row_ptr /* [N+1] */, l
                           uint32_t* comp_order /* [C] */, uint32_t* node_image /* [N] */,
                           uint32_t* node_feat /* [N] */);
 
+/* The SolutionFile (types.proto:30-46) of a plan made by lfr_plan_create_from_matches() or _from_wire(),
+ * encoded on the device from the plan's current positions (the last lfr_plan_solve()'s result; the
+ * initial positions before the first solve).  names / name_off / fact are indexed by image id (the ids of
+ * lfr_host_input, n_images at least its n_images), name k = names[name_off[k], name_off[k+1]).  The bytes
+ * are those of the host assembly of solve.cc:643-679 — lfr_plan_download(), images in order of their
+ * lowest node index, displacements in ascending node index, di / dj = (float) of the fp64 positions as
+ * x86 rounds them (NaN payloads included) — passed to lfr_wire_encode_solution().  Returns the bytes
+ * needed and writes them to `out` only when cap >= that (the size protocol of lfr_wire_encode_solution);
+ * *n_outside (may be NULL) = "# points with at least one coordinate > 0.5" (solve.cc:666-670), counted on
+ * the fp64 positions.  A plan with no node encodes to 0 bytes.  Negative LFR_E* on error; LFR_EINVAL for
+ * a plan made by lfr_plan_create().  The node ids stay on the device for this (8 B per node). */
+int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                 const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
+                                 uint64_t* n_outside);
+
 /* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
  * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from
  * sizes known before either stage runs — the directed edges (2 x the matches of the pairs not skipped),

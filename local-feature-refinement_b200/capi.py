@@ -78,7 +78,7 @@ ABI_SYMBOLS = [
 ]
 #: the symbols include/lfr_graph.h declares
 GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
-                 "lfr_graph_stage_on_device", "lfr_wire_decode_on_device"]
+                 "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device"]
 
 
 class LfrWirePart(C.Structure):
@@ -144,6 +144,9 @@ class Library:
             L.lfr_plan_create_from_wire.restype = C.c_int
             L.lfr_plan_export_graph.argtypes = [C.c_void_p] * 11
             L.lfr_plan_export_graph.restype = C.c_int
+            L.lfr_plan_encode_solution.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+            L.lfr_plan_encode_solution.restype = C.c_int64
             L.lfr_graph_stage_on_device.argtypes = [C.POINTER(HostInput), C.c_int32]
             L.lfr_graph_stage_on_device.restype = C.c_int
             L.lfr_wire_decode_on_device.argtypes = [C.c_uint64]
@@ -358,10 +361,11 @@ class Plan:
         return self
 
     @classmethod
-    def from_wire(cls, lib: Library, parts, banned_images=(), options: Optional[LfrOptions] = None) -> "Plan":
+    def from_wire(cls, lib: Library, parts, banned_images=(), options: Optional[LfrOptions] = None,
+                  positions: Optional[np.ndarray] = None) -> "Plan":
         """lfr_plan_create_from_wire (include/lfr_graph.h): the plan of from_matches() on the decode of
         `parts` — the bytes of one MatchingFile, or of its `.part.N` pieces in order — with the matches
-        decoded on the device.  The pair level (image names in order of first appearance, banned images)
+        decoded on the device (start point `positions`, [N, 2], or zeros).  The pair level (image names in order of first appearance, banned images)
         is walked on the host (wire.walk_matching_file).  Raises wire.ParseError where the pair walk
         fails, and RuntimeError "... (-1): malformed Match message" where a match does not decode."""
         from . import wire
@@ -394,11 +398,12 @@ class Plan:
         inp = HostInput(n_pairs=pair_img1.shape[0], n_matches=m0, n_images=len(names),
                         **{k: (v.ctypes.data if v.size else None) for k, v in arrs.items()})
         o = options if options is not None else lib.default_options()
+        init = None if positions is None else np.ascontiguousarray(positions, dtype=np.float64)
         self = cls.__new__(cls)
         self.lib, self.problem, self.handle = lib, None, None
         h = C.c_void_p()
         sz = HostSizes()
-        lib.check(lib.lib.lfr_plan_create_from_wire(C.byref(inp), wparts, len(parts), C.byref(o), None, C.byref(h),
+        lib.check(lib.lib.lfr_plan_create_from_wire(C.byref(inp), wparts, len(parts), C.byref(o), _ptr(init), C.byref(h),
                                                     C.byref(sz)), "lfr_plan_create_from_wire")
         del keep
         self.handle = h
@@ -415,6 +420,28 @@ class Plan:
                                                                           for a in out.values()]),
                        "lfr_plan_export_graph")
         return out
+
+    def encode_solution(self, image_names, image_fact, stream: int = 0):
+        """lfr_plan_encode_solution (include/lfr_graph.h): the SolutionFile of a plan made by from_matches() or
+        from_wire(), encoded on the device from its current positions.  `image_names` / `image_fact` are indexed
+        by image id, as MatchSet.image_names (the fact of an image without nodes is not read).  Returns
+        (bytes, n_outside), n_outside = "# points with at least one coordinate > 0.5"."""
+        from .wire import _names_blob
+        blob, off = _names_blob(list(image_names))
+        fact = np.ascontiguousarray(image_fact, dtype=np.float32).reshape(-1)
+        if fact.shape[0] != len(image_names):
+            raise ValueError("image_fact has %d entries for %d image names" % (fact.shape[0], len(image_names)))
+        f = self.lib.lib.lfr_plan_encode_solution
+        n_out = C.c_uint64()
+        args = (self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data, _ptr(fact))
+        need = f(*args, None, 0, C.byref(n_out))
+        if need < 0:
+            self.lib.check(int(need), "lfr_plan_encode_solution")
+        out = np.empty(max(int(need), 1), np.uint8)
+        got = f(*args, out.ctypes.data, int(need), C.byref(n_out))
+        if got != need:
+            self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution")
+        return out[:need].tobytes(), int(n_out.value)
 
     def solve(self, stream: int = 0) -> None:
         self.lib.check(self.lib.lib.lfr_plan_solve(self.handle, C.c_void_p(stream)), "lfr_plan_solve")

@@ -16,6 +16,7 @@
 #include "../../include/lfr_graph.h"
 #include "lfr_cut.h"
 #include "lfr_graph.cuh"
+#include "lfr_solution.cuh"
 #include "lfr_solve_cta.cuh"
 #include "lfr_solve_tile.cuh"
 #include "lfr_solve_warp.cuh"
@@ -221,6 +222,10 @@ struct lfr_plan {
     std::vector<uint8_t> is_root;
   };
   std::unique_ptr<GraphArrays> graph;
+  // ... and on the device, for lfr_plan_encode_solution(): the node ids (8 B per node), the image count of
+  // the input, the encoder's scratch and its output (grow-only: repeated encodes allocate nothing)
+  DevBuf node_image, node_feat, enc_scratch, enc_cub, enc_out;
+  uint32_t n_images = 0;
 
   lfr::CtaArrays cta_arrays() const {
     lfr::CtaArrays A;
@@ -282,7 +287,8 @@ void free_plan(lfr_plan* pl) {
   DevBuf* bufs[] = {&pl->row_ptr, &pl->edges, &pl->track, &pl->comp, &pl->is_root, &pl->comp_ptr, &pl->comp_nodes,
                     &pl->local_of, &pl->pos, &pl->pos_init, &pl->stats, &pl->cycles, &pl->times, &pl->lists, &pl->L_comps, &pl->L_rec, &pl->L_meta,
                     &pl->L_inlist, &pl->L_twin, &pl->L_fdst, &pl->L_bE01, &pl->L_bE23, &pl->L_fdstE, &pl->L_ell_base, &pl->L_scr, &pl->L_q, &pl->L_node, &pl->L_outptr, &pl->L_inptr, &pl->L_freeof,
-                    &pl->L_x, &pl->L_xc, &pl->L_lof, &pl->L_vec};
+                    &pl->L_x, &pl->L_xc, &pl->L_lof, &pl->L_vec, &pl->node_image, &pl->node_feat, &pl->enc_scratch,
+                    &pl->enc_cub, &pl->enc_out};
   for (DevBuf* b : bufs) b->release();
   if (pl->h_stage) cudaFreeHost(pl->h_stage);
   for (int i = 0; i < pl->n_streams; ++i) {
@@ -951,10 +957,11 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
     return LFR_OK;
   }
   if (n_images > 65535) return fail(LFR_EUNSUPPORTED, "more than 65535 images");
-  TmpBuf d_nimg, d_nfeat, d_ssrc, d_perm, d_cdst, d_csim;
-  // the six arrays fill_plan() would upload are built in the plan's own buffers and stay there
+  TmpBuf d_ssrc, d_perm, d_cdst, d_csim;
+  // the six arrays fill_plan() would upload are built in the plan's own buffers and stay there, and so do
+  // the node -> (image, feature) ids, which lfr_plan_encode_solution() reads
   DevBuf &d_rowptr = pl->row_ptr, &d_track = pl->track, &d_isroot = pl->is_root, &d_comp = pl->comp,
-         &d_cptr = pl->comp_ptr, &d_cnodes = pl->comp_nodes;
+         &d_cptr = pl->comp_ptr, &d_cnodes = pl->comp_nodes, &d_nimg = pl->node_image, &d_nfeat = pl->node_feat;
   LFR_TRY(d_nop.reserve(4 * E));
   LFR_TRY(d_nimg.reserve(4 * (size_t)N));
   LFR_TRY(d_nfeat.reserve(4 * (size_t)N));
@@ -1460,6 +1467,13 @@ int create_plan_from_graph(const lfr_host_input* in, MatchArrays& d, const lfr_o
   p.comp_ptr = G.comp_ptr.data();
   p.comp_nodes = G.comp_nodes.data();
   LFR_TRY(fill_plan(pl, &p, o, initial_positions, 0, false, nullptr, nullptr, /*graph_resident=*/true));
+  // the working positions hold the start point from creation on, so lfr_plan_download() and
+  // lfr_plan_encode_solution() see it before the first solve; that solve then skips its reset copy
+  if (pl->N) {
+    LFR_CUDA(cudaMemcpyAsync(pl->pos.p, pl->pos_init.p, sizeof(double) * 2 * (size_t)pl->N, cudaMemcpyDeviceToDevice, 0));
+    pl->pos_is_staged = true;
+  }
+  pl->n_images = in->n_images;
   LFR_CUDA(cudaStreamSynchronize(0));
   return LFR_OK;
 }
@@ -1637,6 +1651,91 @@ int download(lfr_plan* pl, cudaStream_t s, double* positions, lfr_stats* st) {
     st->n_kernel_launches = (uint32_t)pl->buckets.size() + (uint32_t)pl->cta_groups.size();
   }
   return LFR_OK;
+}
+
+// {kernels and the upload of names and facts, device-to-host copy of the bytes} in ms of the calling
+// thread's last lfr_plan_encode_solution() that wrote its output
+thread_local double g_encode_ms[2] = {};
+
+// lfr_plan_encode_solution() on a checked plan and arguments (lfr_solution.cuh): the sizing kernels, one
+// synchronisation for the total, then — when `out` has room — the writing kernels and one copy to `out`
+int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t* names, const uint64_t* name_off,
+                        const float* fact, uint8_t* out, uint64_t cap, uint64_t* n_outside) {
+  using namespace lfr::solution;
+  const uint32_t N = pl->N;
+  if (n_outside) *n_outside = 0;
+  if (!N) return 0;
+  const auto t0 = Clock::now();
+  const uint64_t name_bytes = name_off[NI];
+  // one scratch buffer carved at 256-byte boundaries: per-image arrays, the uploaded names, per-node arrays
+  size_t at = 0;
+  auto take = [&at](size_t bytes) {
+    const size_t o = at;
+    at += (bytes + 255) & ~(size_t)255;
+    return o;
+  };
+  const size_t o_first = take(4 * (size_t)NI), o_first_s = take(4 * (size_t)NI), o_iota_i = take(4 * (size_t)NI),
+               o_img_s = take(4 * (size_t)NI), o_rank = take(4 * (size_t)NI), o_img_ptr = take(4 * ((size_t)NI + 1)),
+               o_ctr = take(16), o_body = take(8 * (size_t)NI), o_isize = take(8 * ((size_t)NI + 1)),
+               o_ioff = take(8 * ((size_t)NI + 1)), o_name_off = take(8 * ((size_t)NI + 1)), o_fact = take(4 * (size_t)NI),
+               o_names = take(name_bytes), o_key = take(4 * (size_t)N), o_key_s = take(4 * (size_t)N),
+               o_iota = take(4 * (size_t)N), o_perm = take(4 * (size_t)N), o_rsize = take(8 * ((size_t)N + 1)),
+               o_noff = take(8 * ((size_t)N + 1));
+  LFR_TRY(pl->enc_scratch.reserve(at));
+  uint8_t* base = pl->enc_scratch.as<uint8_t>();
+  auto u32 = [base](size_t o) { return reinterpret_cast<uint32_t*>(base + o); };
+  auto u64 = [base](size_t o) { return reinterpret_cast<uint64_t*>(base + o); };
+  uint32_t *first = u32(o_first), *first_s = u32(o_first_s), *iota_i = u32(o_iota_i), *img_s = u32(o_img_s),
+           *rank = u32(o_rank), *img_ptr = u32(o_img_ptr), *n_present = u32(o_ctr + 8), *key = u32(o_key),
+           *key_s = u32(o_key_s), *iota = u32(o_iota), *perm = u32(o_perm);
+  uint64_t *body = u64(o_body), *isize = u64(o_isize), *ioff = u64(o_ioff), *d_name_off = u64(o_name_off),
+           *rsize = u64(o_rsize), *noff = u64(o_noff);
+  unsigned long long* d_outside = reinterpret_cast<unsigned long long*>(base + o_ctr);
+  float* d_fact = reinterpret_cast<float*>(base + o_fact);
+  uint8_t* d_names = base + o_names;
+  const uint32_t* nimg = pl->node_image.as<uint32_t>();
+  const uint32_t* nfeat = pl->node_feat.as<uint32_t>();
+  const double* pos = pl->pos.as<double>();
+
+  LFR_CUDA(cudaMemcpyAsync(d_name_off, name_off, 8 * ((size_t)NI + 1), cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemcpyAsync(d_fact, fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
+  if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, names, name_bytes, cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemsetAsync(base + o_ctr, 0, 16, s));
+  init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
+  first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {
+    return cub::DeviceRadixSort::SortPairs(t, nb, first, first_s, iota_i, img_s, (int)NI, 0, bits_for(N), s);
+  }));
+  rank_kernel<<<blocks_for(NI), 256, 0, s>>>(first_s, img_s, NI, N, rank, n_present);
+  node_key_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, rank, N, key, iota);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: ascending node index within an image
+    return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, iota, perm, (int)N, 0, bits_for(NI), s);
+  }));
+  record_size_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, N, rsize, img_ptr);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, noff, (int)N + 1, s); }));
+  image_size_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(img_s, img_ptr, noff, d_name_off, d_fact, n_present, NI, body, isize);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)NI + 1, s); }));
+  uint64_t total = 0;
+  unsigned long long outside = 0;
+  LFR_CUDA(cudaMemcpyAsync(&outside, d_outside, 8, cudaMemcpyDeviceToHost, s));
+  LFR_TRY(fetch(&total, ioff + NI, 1, s));
+  if (n_outside) *n_outside = outside;
+  if (!out || cap < total) return (int64_t)total;
+  LFR_TRY(pl->enc_out.reserve(total));
+  uint8_t* d_out = pl->enc_out.as<uint8_t>();
+  write_images_kernel<<<blocks_for(NI), 256, 0, s>>>(img_s, body, ioff, d_names, d_name_off, d_fact, n_present, d_out);
+  write_records_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, img_ptr, noff, ioff, N, d_out);
+  LFR_LAUNCHED();
+  LFR_CUDA(cudaStreamSynchronize(s));
+  g_encode_ms[0] = ms_since(t0);
+  const auto t1 = Clock::now();
+  LFR_TRY(fetch(out, d_out, total, s));
+  g_encode_ms[1] = ms_since(t1);
+  return (int64_t)total;
 }
 
 int select_device(const lfr_options& o) {
@@ -1859,6 +1958,25 @@ int lfr_plan_export_graph(const lfr_plan* pl, uint32_t* row_ptr, lfr_edge* edges
     LFR_CUDA(cudaSetDevice(pl->device));
     LFR_CUDA(cudaMemcpy(edges, pl->edges.p, sizeof(lfr_edge) * (size_t)pl->E, cudaMemcpyDeviceToHost));
   }
+  return LFR_OK;
+}
+
+int64_t lfr_plan_encode_solution(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
+                                 const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
+                                 uint64_t* n_outside) {
+  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
+  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
+  if (n_images && (!name_off || !fact)) return fail(LFR_EINVAL, "NULL image names or facts");
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
+  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  LFR_CUDA(cudaSetDevice(pl->device));
+  return encode_solution(pl, (cudaStream_t)stream, n_images, names, name_off, fact, out, cap, n_outside);
+}
+
+int lfr_debug_last_encode_times(double* out2) {
+  out2[0] = g_encode_ms[0];
+  out2[1] = g_encode_ms[1];
   return LFR_OK;
 }
 

@@ -7,14 +7,16 @@
 // (:416-424), same stdout lines (:484-485,534,549,589,591,606,638,641,670) and exit codes (0; 1 on a
 // command-line error, :397-401; -1 = 255 when the input does not parse or the output cannot be
 // written, :433-436,674-677).  The work is lfr_wire_walk_matches() (include/lfr_wire.h) over the pairs,
-// the graph stage and the solve, then lfr_wire_encode_solution().  The graph stage runs where
+// the graph stage, the solve and the SolutionFile.  The graph stage runs where
 // lfr_graph_stage_on_device() (include/lfr_graph.h) says, from the pair level alone:
 //   device: lfr_plan_create_from_wire() on the mapped parts (the matches are decoded on the GPU) — or,
 //           below the match count lfr_wire_decode_on_device() sets, lfr_wire_decode_matches() +
-//           lfr_plan_create_from_matches() —, lfr_plan_solve() + lfr_plan_download() on the plan left
-//           in HBM, and lfr_plan_export_graph() for the node -> (image, feature) ids;
+//           lfr_plan_create_from_matches() —, lfr_plan_solve() on the plan left in HBM, and
+//           lfr_plan_encode_solution() for the SolutionFile bytes (encoded on the GPU from the positions
+//           in HBM);
 //   host:   lfr_wire_decode_matches(), lfr_host_stage_create() (include/lfr_host.h) writing the edge
-//           records into page-locked memory, then lfr_solve() / lfr_solve_multi() (include/lfr.h).
+//           records into page-locked memory, then lfr_solve() / lfr_solve_multi() (include/lfr.h), the
+//           output assembly and lfr_wire_encode_solution().
 // Both routes give the same bytes and lines.  LFR_GRAPH_STAGE=host|device forces a route (a test and
 // measurement hook).  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
@@ -52,9 +54,9 @@ int lfr_plan_create_from_matches(const lfr_host_input* in, const lfr_options* o,
 int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
                               const lfr_options* o, const double* initial_positions, lfr_plan** out,
                               lfr_host_sizes* sizes) __attribute__((weak));
-int lfr_plan_export_graph(const lfr_plan* plan, uint32_t* row_ptr, lfr_edge* edges, uint32_t* track, uint32_t* comp,
-                          uint8_t* is_root, uint32_t* comp_ptr, uint32_t* comp_nodes, uint32_t* comp_order,
-                          uint32_t* node_image, uint32_t* node_feat) __attribute__((weak));
+int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                 const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
+                                 uint64_t* n_outside) __attribute__((weak));
 }
 
 namespace {
@@ -342,7 +344,7 @@ int main(int argc, char** argv) {
   // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
   // takes the host route; forcing the device route there is an error, never a silent host run.
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
-                                 lfr_plan_create_from_wire && lfr_plan_export_graph;
+                                 lfr_plan_create_from_wire && lfr_plan_encode_solution;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -395,7 +397,7 @@ int main(int argc, char** argv) {
   std::vector<uint8_t> is_root;
   if (on_device) {
     // ---- the matches decoded and the graph stage run on the GPU (include/lfr_graph.h): the problem stays
-    // in HBM for the solve and only the per-node image / feature ids come back for the SolutionFile
+    // in HBM for the solve and the SolutionFile is encoded there
     lfr_options opt;
     lfr_options_default(&opt);
     opt.device = (int32_t)device;
@@ -415,13 +417,6 @@ int main(int argc, char** argv) {
     }
     if (rc != LFR_OK) {  // no device: the host route's message, from the same device check
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
-      return 2;
-    }
-    node_image.resize(sz.n_nodes);
-    node_feat.resize(sz.n_nodes);
-    if (lfr_plan_export_graph(plan, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                              node_image.data(), node_feat.data()) != LFR_OK) {
-      std::fprintf(stderr, "ERROR: lfr_plan_export_graph failed\n");
       return 2;
     }
   } else {
@@ -461,9 +456,9 @@ int main(int argc, char** argv) {
   std::fflush(stdout);
 
   // ---- the solve (solve.cc:608-635): positions start at zero --------------------------------
-  double* positions = nullptr;
+  double* positions = nullptr;  // host route: the solve's result; the device route keeps it in HBM
   bool positions_pinned = false;
-  if (N) {
+  if (N && !plan) {
     positions = static_cast<double*>(lfr_host_alloc(2ull * N * sizeof(double)));
     positions_pinned = positions != nullptr;
     if (!positions) positions = static_cast<double*>(std::malloc(2ull * N * sizeof(double)));
@@ -472,7 +467,7 @@ int main(int argc, char** argv) {
   const Clock::time_point t_solve = Clock::now();
   if (N && plan) {
     int rc = lfr_plan_solve(plan, nullptr);
-    if (rc == LFR_OK) rc = lfr_plan_download(plan, nullptr, positions, nullptr);
+    if (rc == LFR_OK) rc = lfr_plan_download(plan, nullptr, nullptr, nullptr);  // waits for the solve, checks its error flag
     if (rc != LFR_OK) {
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
       return 2;
@@ -501,60 +496,88 @@ int main(int argc, char** argv) {
     }
   }
   const Clock::time_point t_end = Clock::now();
-  lfr_plan_destroy(plan);
   std::printf("Solver time: %lldms\n", ms_between(t_solve, t_end));  // solve.cc:638
   std::printf("Total time: %lldms\n", ms_between(t_start, t_end));   // solve.cc:641
 
   // ---- SolutionFile (solve.cc:643-679): images by first node appearance, nodes by index ------
-  std::vector<int64_t> rank(names.size(), -1);
-  std::vector<uint32_t> img_ids;
-  for (uint32_t v = 0; v < N; ++v)
-    if (rank[node_image[v]] < 0) {
-      rank[node_image[v]] = (int64_t)img_ids.size();
-      img_ids.push_back(node_image[v]);
-    }
-  const size_t I = img_ids.size();
-  std::vector<uint64_t> img_ptr(I + 1, 0);
-  for (uint32_t v = 0; v < N; ++v) ++img_ptr[(size_t)rank[node_image[v]] + 1];
-  for (size_t i = 0; i < I; ++i) img_ptr[i + 1] += img_ptr[i];
-  std::vector<uint32_t> feature_idx(N);
-  std::vector<float> di(N), dj(N);
   uint64_t n_outside = 0;
-  {
-    std::vector<uint64_t> fill(img_ptr.begin(), img_ptr.end() - 1);
-    for (uint32_t v = 0; v < N; ++v) {
-      const uint64_t k = fill[(size_t)rank[node_image[v]]]++;
-      feature_idx[k] = node_feat[v];
-      di[k] = (float)positions[2 * (size_t)v];
-      dj[k] = (float)positions[2 * (size_t)v + 1];
-      if (std::fabs(positions[2 * (size_t)v + 1]) > 0.5 || std::fabs(positions[2 * (size_t)v]) > 0.5) ++n_outside;  // solve.cc:666-669
+  int64_t need = 0;
+  uint8_t* out = nullptr;
+  bool out_pinned = false;
+  if (plan) {
+    // encoded on the GPU, names and facts indexed by image id, into page-locked memory sized by the
+    // largest encoding: a Displacement record is at most 18 bytes, an Image's header 16 plus its name field
+    std::vector<uint8_t> name_blob;
+    std::vector<uint64_t> name_off(names.size() + 1, 0);
+    uint64_t cap = 18ull * N;
+    for (size_t i = 0; i < names.size(); ++i) {
+      name_blob.insert(name_blob.end(), names[i].begin(), names[i].end());
+      name_off[i + 1] = name_blob.size();
+      cap += 16 + 11 + names[i].size();
     }
+    out = static_cast<uint8_t*>(lfr_host_alloc(cap));
+    out_pinned = out != nullptr;
+    if (!out) out = static_cast<uint8_t*>(std::malloc(cap ? cap : 1));
+    need = lfr_plan_encode_solution(plan, nullptr, (uint32_t)names.size(), name_blob.data(), name_off.data(),
+                                    image_fact.data(), out, cap, &n_outside);
+    lfr_plan_destroy(plan);
+    if (need < 0 || (uint64_t)need > cap) {
+      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", (int)need, lfr_last_error());
+      return 2;
+    }
+  } else {
+    std::vector<int64_t> rank(names.size(), -1);
+    std::vector<uint32_t> img_ids;
+    for (uint32_t v = 0; v < N; ++v)
+      if (rank[node_image[v]] < 0) {
+        rank[node_image[v]] = (int64_t)img_ids.size();
+        img_ids.push_back(node_image[v]);
+      }
+    const size_t I = img_ids.size();
+    std::vector<uint64_t> img_ptr(I + 1, 0);
+    for (uint32_t v = 0; v < N; ++v) ++img_ptr[(size_t)rank[node_image[v]] + 1];
+    for (size_t i = 0; i < I; ++i) img_ptr[i + 1] += img_ptr[i];
+    std::vector<uint32_t> feature_idx(N);
+    std::vector<float> di(N), dj(N);
+    {
+      std::vector<uint64_t> fill(img_ptr.begin(), img_ptr.end() - 1);
+      for (uint32_t v = 0; v < N; ++v) {
+        const uint64_t k = fill[(size_t)rank[node_image[v]]]++;
+        feature_idx[k] = node_feat[v];
+        di[k] = (float)positions[2 * (size_t)v];
+        dj[k] = (float)positions[2 * (size_t)v + 1];
+        if (std::fabs(positions[2 * (size_t)v + 1]) > 0.5 || std::fabs(positions[2 * (size_t)v]) > 0.5) ++n_outside;  // solve.cc:666-669
+      }
+    }
+    std::vector<uint8_t> name_blob;
+    std::vector<uint64_t> name_off(I + 1, 0);
+    std::vector<float> fact(I);
+    for (size_t i = 0; i < I; ++i) {
+      const std::string& s = names[img_ids[i]];
+      name_blob.insert(name_blob.end(), s.begin(), s.end());
+      name_off[i + 1] = name_blob.size();
+      fact[i] = image_fact[img_ids[i]];
+    }
+    if (name_blob.empty()) name_blob.push_back(0);
+    need = lfr_wire_encode_solution(I, img_ptr.data(), name_blob.data(), name_off.data(), fact.data(),
+                                    feature_idx.data(), di.data(), dj.data(), nullptr, 0);
+    out = static_cast<uint8_t*>(std::malloc((size_t)std::max<int64_t>(need, 1)));
+    if (need < 0 || lfr_wire_encode_solution(I, img_ptr.data(), name_blob.data(), name_off.data(), fact.data(),
+                                             feature_idx.data(), di.data(), dj.data(), out, (uint64_t)need) != need)
+      need = -1;
   }
   std::printf("# points with at least one coordinate > 0.5: %llu\n", (unsigned long long)n_outside);  // solve.cc:670
   std::fflush(stdout);
-  std::vector<uint8_t> name_blob;
-  std::vector<uint64_t> name_off(I + 1, 0);
-  std::vector<float> fact(I);
-  for (size_t i = 0; i < I; ++i) {
-    const std::string& s = names[img_ids[i]];
-    name_blob.insert(name_blob.end(), s.begin(), s.end());
-    name_off[i + 1] = name_blob.size();
-    fact[i] = image_fact[img_ids[i]];
-  }
-  if (name_blob.empty()) name_blob.push_back(0);
-  const int64_t need = lfr_wire_encode_solution(I, img_ptr.data(), name_blob.data(), name_off.data(), fact.data(),
-                                                feature_idx.data(), di.data(), dj.data(), nullptr, 0);
-  std::vector<uint8_t> out((size_t)std::max<int64_t>(need, 1));
-  bool written = need >= 0 && lfr_wire_encode_solution(I, img_ptr.data(), name_blob.data(), name_off.data(), fact.data(),
-                                                       feature_idx.data(), di.data(), dj.data(), out.data(), (uint64_t)need) == need;
+  bool written = need >= 0;
   if (written) {
     std::ofstream f(output_file, std::ios::binary | std::ios::trunc);
     written = f.good();
-    if (written && need) f.write(reinterpret_cast<const char*>(out.data()), need);
+    if (written && need) f.write(reinterpret_cast<const char*>(out), need);
     written = written && f.good();
   }
   if (positions_pinned) lfr_host_free(positions); else std::free(positions);
   if (edges_pinned) lfr_host_free(edges); else std::free(edges);
+  if (out_pinned) lfr_host_free(out); else std::free(out);
   if (!written) {
     std::fputs("Failed to write proto object.\n", stderr);  // solve.cc:674-677
     return 255;
