@@ -129,6 +129,7 @@ typedef struct lfr_options {
 #define LFR_DBG_PROFILE 0x10            /* per-component clock64() counters (lfr_debug_plan_cycles)            */
 #define LFR_DBG_ZERO_COPY 0x20          /* lfr_solve(): use pinned caller buffers in place, as lfr_solve_multi() does */
 #define LFR_DBG_TILE_FROM_SHIFT 8       /* bits 8..15 = n: components with more than n unknowns (n <= 32) use the two-warp tile kernel */
+#define LFR_DBG_WARP2_WARPS_SHIFT 16    /* bits 16..19 = W (1..8): warps per SM of the warp-register tier's queue kernel; 0 = the default */
 
 /* Optional per-component results, caller-owned, indexed like comp_ptr. Any
  * pointer may be NULL. */
@@ -216,7 +217,9 @@ int lfr_plan_create(const lfr_problem* p, const lfr_options* o,
 int lfr_plan_solve(lfr_plan* plan, void* stream);
 int lfr_plan_download(lfr_plan* plan, void* stream, double* positions,
                       lfr_stats* stats);
-/* number of kernels one lfr_plan_solve launches */
+/* number of kernels one lfr_plan_solve launches: one per CTA-tier size class, one (two when its
+ * members need slots of very different sizes) persistent queue launch for the register warp tier,
+ * one per remaining bucket (tile, shared-memory Cholesky, single-warp register); 1 on cfg2 */
 int lfr_plan_num_launches(const lfr_plan* plan);
 /* algorithmic bytes of the last completed solve: sum_c iters_c*(80 E_c + 36 N_c)
  * and the one-pass lower bound 80 E + 36 N over solved components (SURVEY 8d) */

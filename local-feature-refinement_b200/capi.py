@@ -24,6 +24,7 @@ LFR_OK = 0
 DBG_FORCE_SMEM_CHOLESKY, DBG_NO_TILE, DBG_NO_ZERO_COPY, DBG_PROFILE = 0x1, 0x2, 0x8, 0x10
 DBG_ZERO_COPY = 0x20
 DBG_TILE_FROM_SHIFT = 8
+DBG_WARP2_WARPS_SHIFT = 16
 TERM_NAMES = {0: "skipped", 1: "gradient_tol", 2: "parameter_tol", 3: "function_tol",
               4: "min_radius", 5: "no_convergence", 6: "failure", 7: "empty"}
 

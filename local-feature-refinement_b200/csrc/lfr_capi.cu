@@ -63,6 +63,9 @@ constexpr int kMaxSmemPerBlock = 227 * 1024;
 // Components with more unknowns than this (and <= 32) take the two-warp tile kernel <64, 32> instead of
 // the one-warp register kernel; 32 = never.  Overridden per plan by LFR_TILE_FROM_N.
 constexpr int kTileFromDefault = 32;
+// warps per SM of the warp-register tier's queue kernel (LFR_DBG_WARP2_WARPS_SHIFT overrides, up to
+// lfr::kWarp2QueueMaxWarps)
+constexpr int kWarp2QueueWarpsDefault = 8;
 constexpr int kScheduleThreadsMax = 8;  // host threads that classify the dispatch list (build_buckets)
 constexpr int kMaxStreams = 12;
 
@@ -133,6 +136,13 @@ struct CtaGroup {
   int smem_vecs = 6;  // how many of the CG arrays (p, w, r, z, y, preconditioner) live in shared memory
 };
 
+// One launch of the warp-register tier's queue kernel: `n` entries of two words at `offset` of the
+// list buffer, `warps` per CTA (one CTA per SM), each in a slot of `slot_bytes`.
+struct Warp2Group {
+  uint32_t offset = 0, n = 0;
+  int slot_bytes = 0, warps = 0;
+};
+
 struct Bucket {
   uint32_t offset = 0;  // into the bucket-list buffer
   uint32_t n = 0;
@@ -182,6 +192,11 @@ struct lfr_plan {
   unsigned long long* d_pull() const { return reinterpret_cast<unsigned long long*>(d_err() + 2); }  // {ticketed, arrived} bytes
   size_t stats_bytes() const { return 16 * (size_t)Cp + 16 * (size_t)Cp + 8 + 16; }
   std::vector<Bucket> buckets;
+  std::vector<Warp2Group> w2_groups;  // the warp-register tier's four-warp buckets, as queue launches
+  std::vector<uint32_t> w2_slots;     // build_buckets scratch
+  DevBuf queue_ctr;                   // two words per queue launch (solve_warp2_queue_kernel)
+  int n_sms = 0;
+  int num_launches() const { return (int)buckets.size() + (int)w2_groups.size() + (int)cta_groups.size(); }
   std::vector<uint32_t> comp_size;  // nodes per dispatch slot
   std::vector<uint32_t> list_host;
   // CTA tier (block-Jacobi PCG): components with more than kMaxWarpN2 unknowns, or all with linear_solver = 2
@@ -288,7 +303,7 @@ void free_plan(lfr_plan* pl) {
                     &pl->local_of, &pl->pos, &pl->pos_init, &pl->stats, &pl->cycles, &pl->times, &pl->lists, &pl->L_comps, &pl->L_rec, &pl->L_meta,
                     &pl->L_inlist, &pl->L_twin, &pl->L_fdst, &pl->L_bE01, &pl->L_bE23, &pl->L_fdstE, &pl->L_ell_base, &pl->L_scr, &pl->L_q, &pl->L_node, &pl->L_outptr, &pl->L_inptr, &pl->L_freeof,
                     &pl->L_x, &pl->L_xc, &pl->L_lof, &pl->L_vec, &pl->node_image, &pl->node_feat, &pl->enc_scratch,
-                    &pl->enc_cub, &pl->enc_out};
+                    &pl->enc_cub, &pl->enc_out, &pl->queue_ctr};
   for (DevBuf* b : bufs) b->release();
   if (pl->h_stage) cudaFreeHost(pl->h_stage);
   for (int i = 0; i < pl->n_streams; ++i) {
@@ -313,7 +328,8 @@ int upload(DevBuf* d, const T* h, size_t count, cudaStream_t s) {
 // Size-bucketed schedule: components are grouped by the shared memory one warp
 // needs for them, so small tracks run at high occupancy and the few large
 // components do not dictate the carve-up of everyone else.  Buckets are
-// launched on concurrent streams, largest components first.
+// launched on concurrent streams, largest components first; the register warp
+// tier's four-warp buckets are then merged into one persistent queue launch.
 int build_buckets(lfr_plan* pl, const lfr_problem* p) {
   // shared-memory classes of a launch (finer classes — one per "one more CTA fits an SM" boundary — mean
   // more launches for the same resident work)
@@ -531,6 +547,47 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
           emit(vi, one, start[key] + i, 1);
         }
       }
+    }
+  }
+  // The register warp tier's four-warp buckets become queue launches (solve_warp2_queue_kernel): their
+  // members in dispatch order (largest first), each entry {slot, own layout sizes}.  One launch takes
+  // every member whose own layout fits a slot at W warps per SM; the rest (if any) go to a second at
+  // as many warps as its largest member allows (>= 4: they came from four-warp buckets).  Only where
+  // some member has more than 16 unknowns: without one the per-bucket kernels run 12 warps per SM at
+  // 168 registers, which the queue kernel (255 registers for all four NREG paths) cannot (DESIGN §4).
+  pl->w2_groups.clear();
+  bool wide = false;
+  for (const Bucket& b : pl->buckets) wide = wide || (b.variant >= 24 && b.variant <= 32 && b.warps == 4);
+  std::vector<uint32_t>& q = pl->w2_slots;
+  q.clear();
+  size_t kept = 0;
+  for (const Bucket& b : pl->buckets) {
+    if (wide && b.variant >= 8 && b.variant <= 32 && b.warps == 4)
+      q.insert(q.end(), pl->list_host.begin() + b.offset, pl->list_host.begin() + b.offset + b.n);
+    else
+      pl->buckets[kept++] = b;
+  }
+  pl->buckets.resize(kept);
+  if (!q.empty()) {
+    std::sort(q.begin(), q.end());
+    const int ww = (dbg >> LFR_DBG_WARP2_WARPS_SHIFT) & 0xf;
+    const int W = ww ? std::min(ww, lfr::kWarp2QueueMaxWarps) : kWarp2QueueWarpsDefault;
+    const int cap = (kMaxSmemPerBlock / W) & ~15;
+    auto need = [&](uint32_t c) { return lfr::Warp2Layout(dim[c].e, dim[c].nc, dim[c].n2).total; };
+    for (int pass = 0; pass < 2; ++pass) {
+      Warp2Group g;
+      g.offset = (uint32_t)pl->list_host.size();
+      for (uint32_t c : q) {
+        const int b = need(c);
+        if ((b <= cap) != (pass == 0)) continue;
+        pl->list_host.push_back(c);
+        pl->list_host.push_back(lfr::warp2_queue_dims(dim[c].e, dim[c].nc, dim[c].n2));
+        g.slot_bytes = std::max(g.slot_bytes, b);
+        ++g.n;
+      }
+      if (!g.n) continue;
+      g.warps = pass == 0 ? W : std::min(W, kMaxSmemPerBlock / g.slot_bytes);
+      pl->w2_groups.push_back(g);
     }
   }
   return LFR_OK;
@@ -761,7 +818,13 @@ int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const do
     if (ps != s) LFR_CUDA(cudaEventRecord(pl->ev_edges, pl->copy_stream));
   }
   // streams for concurrent bucket launches
-  const int want = std::min<int>(kMaxStreams, std::max<int>(0, (int)pl->buckets.size() + (int)pl->cta_groups.size() - 1));
+  if (!pl->w2_groups.empty() && !pl->queue_ctr.p) {
+    // zero once: every queue launch leaves its two words at zero when it ends
+    LFR_TRY(pl->queue_ctr.reserve(2 * sizeof(uint32_t) * 2));
+    LFR_CUDA(cudaMemsetAsync(pl->queue_ctr.p, 0, pl->queue_ctr.cap, s));
+  }
+  if (!pl->w2_groups.empty() && !pl->n_sms) LFR_CUDA(cudaDeviceGetAttribute(&pl->n_sms, cudaDevAttrMultiProcessorCount, pl->device));
+  const int want = std::min<int>(kMaxStreams, std::max<int>(0, pl->num_launches() - 1));
   if (!pl->ev_fork) LFR_CUDA(cudaEventCreateWithFlags(&pl->ev_fork, cudaEventDisableTiming));
   while (pl->n_streams < want) {
     LFR_CUDA(cudaStreamCreateWithFlags(&pl->streams[pl->n_streams], cudaStreamNonBlocking));
@@ -1494,9 +1557,7 @@ int set_kernel_attrs() {
                                 kMaxSmemPerBlock));
   LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_kernel<4, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_kernel<4, 24>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_kernel<4, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_queue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 kMaxSmemPerBlock));
   LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_kernel<1, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 kMaxSmemPerBlock));
@@ -1527,7 +1588,7 @@ int launch_solve(lfr_plan* pl, cudaStream_t s) {
   const bool hbm_edges_on_copy_stream = pl->zc_edges && pl->edges_in_hbm;
   const int nb = (int)pl->buckets.size();
   const int n_cta_launches = pl->n_large ? (int)pl->cta_groups.size() : 0;
-  const int n_side = std::max(0, nb + n_cta_launches - 1);
+  const int n_side = std::max(0, nb + (int)pl->w2_groups.size() + n_cta_launches - 1);
   if (n_side > 0) LFR_CUDA(cudaEventRecord(pl->ev_fork, s));
   int side = 0;
   if (pl->n_large) {  // the CTA tier first: its components are the longest
@@ -1554,14 +1615,35 @@ int launch_solve(lfr_plan* pl, cudaStream_t s) {
       LFR_CUDA(cudaGetLastError());
     }
   }
+  // the first queue launch (or, without one, bucket 0) runs on the caller's stream, the others on side
+  // streams forked from it
+  bool on_caller = true;
+  auto next_stream = [&](cudaStream_t* bs) -> int {
+    *bs = s;
+    if (!on_caller) {
+      *bs = pl->streams[side++ % pl->n_streams];
+      LFR_CUDA(cudaStreamWaitEvent(*bs, pl->ev_fork, 0));
+    }
+    on_caller = false;
+    return LFR_OK;
+  };
+  for (size_t i = 0; i < pl->w2_groups.size(); ++i) {
+    const Warp2Group& g = pl->w2_groups[i];
+    cudaStream_t bs;
+    LFR_TRY(next_stream(&bs));
+    lfr::Warp2Queue q;
+    q.list = pl->lists.as<uint32_t>() + g.offset;
+    q.n = g.n;
+    q.slot_bytes = g.slot_bytes;
+    q.ctr = pl->queue_ctr.as<uint32_t>() + 2 * i;
+    const size_t smem = (size_t)g.slot_bytes * g.warps;
+    lfr::solve_warp2_queue_kernel<<<pl->n_sms, 32 * g.warps, smem, bs>>>(P_stage, pl->K, q);
+    LFR_CUDA(cudaGetLastError());
+  }
   for (int i = 0; i < nb; ++i) {
     const Bucket& b = pl->buckets[i];
-    // bucket 0 runs on the caller's stream, the others on side streams forked from it
-    cudaStream_t bs = s;
-    if (i > 0) {
-      bs = pl->streams[side++ % pl->n_streams];
-      LFR_CUDA(cudaStreamWaitEvent(bs, pl->ev_fork, 0));
-    }
+    cudaStream_t bs;
+    LFR_TRY(next_stream(&bs));
     lfr::WarpBucket wb;
     wb.list = pl->lists.as<uint32_t>() + b.offset;
     wb.n = b.n;
@@ -1581,15 +1663,11 @@ int launch_solve(lfr_plan* pl, cudaStream_t s) {
       lfr::solve_tile_kernel<64, 64><<<b.n, 64, smem, bs>>>(P, pl->K, wb);
     else if (b.variant == 80)
       lfr::solve_tile_kernel<128, 80><<<b.n, 128, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 8)
+    else if (b.variant == 8)  // (four-warp register buckets of a plan without a queue launch)
       lfr::solve_warp2_kernel<4, 8><<<grid, 128, smem, bs>>>(P, pl->K, wb);
     else if (b.variant == 16)
       lfr::solve_warp2_kernel<4, 16><<<grid, 128, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 24 && b.warps == 4)
-      lfr::solve_warp2_kernel<4, 24><<<grid, 128, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 32 && b.warps == 4)
-      lfr::solve_warp2_kernel<4, 32><<<grid, 128, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 32)
+    else if (b.variant == 32 && b.warps == 1)
       lfr::solve_warp2_kernel<1, 32><<<grid, 32, smem, bs>>>(P, pl->K, wb);
     else if (b.warps == 4)
       lfr::solve_warp_kernel<4><<<grid, 128, smem, bs>>>(P, pl->K, wb);
@@ -1648,7 +1726,7 @@ int download(lfr_plan* pl, cudaStream_t s, double* positions, lfr_stats* st) {
     st->total_iterations = ti;
     st->total_line_search_steps = tl;
     st->n_solved = pl->n_solved;
-    st->n_kernel_launches = (uint32_t)pl->buckets.size() + (uint32_t)pl->cta_groups.size();
+    st->n_kernel_launches = (uint32_t)pl->num_launches();
   }
   return LFR_OK;
 }
@@ -2004,7 +2082,7 @@ int lfr_plan_solve(lfr_plan* pl, void* stream) {
 
 int lfr_plan_num_launches(const lfr_plan* pl) {
   // kernels only: the device-to-device reset of `positions` is a copy, not a kernel
-  return pl ? (int)pl->buckets.size() + (int)pl->cta_groups.size() : 0;
+  return pl ? pl->num_launches() : 0;
 }
 
 int lfr_plan_download(lfr_plan* pl, void* stream, double* positions, lfr_stats* st) {
@@ -2101,6 +2179,8 @@ int lfr_debug_time_schedule(const lfr_problem* p, const lfr_options* opt, int re
     for (const Bucket& b : pl.buckets)
       std::fprintf(stderr, "bucket variant %3d  n %6u  emax %5d ncmax %4d n2max %3d  smem/warp %6d  warps %d  -> CTAs/SM by smem %d\n", b.variant,
                    b.n, b.emax, b.ncmax, b.n2max, b.smem_per_warp, b.warps, (int)(kMaxSmemPerBlock / (b.smem_per_warp * b.warps + 1024)));
+    for (const Warp2Group& g : pl.w2_groups)
+      std::fprintf(stderr, "warp2 queue  n %6u  slot %6d  warps/SM %d\n", g.n, g.slot_bytes, g.warps);
     std::fprintf(stderr, "CTA tier: %zu components\n", pl.large_slots.size());
   }
   if (digest) {  // FNV-1a over everything the launches depend on: the schedule must not depend on the thread count
@@ -2116,6 +2196,9 @@ int lfr_debug_time_schedule(const lfr_problem* p, const lfr_options* opt, int re
       mix(b.offset); mix(b.n); mix((uint64_t)b.emax); mix((uint64_t)b.ncmax); mix((uint64_t)b.n2max);
       mix((uint64_t)b.smem_per_warp); mix((uint64_t)b.warps); mix((uint64_t)b.variant);
     }
+    for (const Warp2Group& g : pl.w2_groups) {
+      mix(g.offset); mix(g.n); mix((uint64_t)g.slot_bytes); mix((uint64_t)g.warps);
+    }
     for (uint32_t c : pl.list_host) mix(c);
     for (size_t i = 0; i < pl.large_slots.size(); ++i) {
       mix(pl.large_slots[i]); mix(pl.large_cand[i]); mix(pl.large_free[i]); mix(pl.large_ell[i]);
@@ -2123,7 +2206,7 @@ int lfr_debug_time_schedule(const lfr_problem* p, const lfr_options* opt, int re
     *digest = h;
   }
   *best_us = best;
-  if (n_launches) *n_launches = (int)pl.buckets.size() + (pl.large_slots.empty() ? 0 : 1);  // (CTA tier counted once here)
+  if (n_launches) *n_launches = (int)pl.buckets.size() + (int)pl.w2_groups.size() + (pl.large_slots.empty() ? 0 : 1);  // (CTA tier counted once here)
   return LFR_OK;
 }
 

@@ -495,21 +495,15 @@ struct Warp2Tier {
   __device__ unsigned long long counter() const { return 0; }
 };
 
-// (12 resident warps per SM = 168 registers for NREG <= 16; 8 (255 registers) and 16 (128 registers)
-// are the alternatives)
-template <int WARPS, int NREG>
-__global__ void __launch_bounds__(WARPS * 32, (NREG > 16 ? 8 : 12) / WARPS)
-solve_warp2_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const uint32_t item = blockIdx.x * WARPS + wib;
-  if (item >= B.n) return;  // warps are independent: no block-level barrier anywhere
-  const uint32_t c = B.list[item];
-  unsigned char* base = smem_raw + (size_t)wib * B.smem_per_warp;
-  const Warp2Layout L(B.emax, B.ncmax, B.n2max);
+// One component on one warp, in the shared-memory slot at `base` laid out for (emax, ncmax, n2max): the
+// per-bucket kernel and the queue kernel below run exactly this.
+template <int NREG>
+__device__ __forceinline__ void warp2_solve(const DevProblem& P, const DevConsts& K, uint32_t c, unsigned char* base,
+                                            int emax, int ncmax, int n2max, int lane) {
+  const Warp2Layout L(emax, ncmax, n2max);
   Warp2Ctx C;
   C.lane = lane;
-  C.emax = B.emax;
+  C.emax = emax;
   C.ldh = L.ldh;
   C.stage = (float4*)(base + L.stage);
   C.bar = (uint64_t*)(base + L.bar);
@@ -538,7 +532,7 @@ solve_warp2_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
   // ---- component setup (solve.cc:98-143) --------------------------------------
   int Ec = 0, nf = 0;
   bool irregular = false;
-  warp_setup(C, rowstart, candptr, cnt, B.ncmax, P, K, c, lane, &Ec, &nf, &irregular);
+  warp_setup(C, rowstart, candptr, cnt, ncmax, P, K, c, lane, &Ec, &nf, &irregular);
   C.Ec = Ec;
   C.irregular = irregular;
   C.nf = nf;
@@ -546,6 +540,80 @@ solve_warp2_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
   __syncwarp();
   Warp2Tier<NREG> T{C, K, {0.0, 0.0}};
   lm_solve(T, P, K, c, prof);
+}
+
+// One bucket per launch, WARPS components per CTA: the four-warp buckets of queues without a member
+// above 16 unknowns, and the single-warp launches of the components whose slot does not fit four to a
+// CTA (12 resident warps per SM = 168 registers for NREG <= 16; 8 (255 registers) above)
+template <int WARPS, int NREG>
+__global__ void __launch_bounds__(WARPS * 32, (NREG > 16 ? 8 : 12) / WARPS)
+solve_warp2_kernel(const DevProblem P, const DevConsts K, const WarpBucket B) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const uint32_t item = blockIdx.x * WARPS + wib;
+  if (item >= B.n) return;  // warps are independent: no block-level barrier anywhere
+  warp2_solve<NREG>(P, K, B.list[item], smem_raw + (size_t)wib * B.smem_per_warp, B.emax, B.ncmax, B.n2max, lane);
+}
+
+// ---- the tier as one persistent launch ---------------------------------------------------------
+// One CTA of W warps per SM.  Every warp takes the next component from one device queue — the
+// tier's dispatch slots in dispatch order, largest first — solves it in its own shared-memory slot
+// (sized for the queue's largest member, laid out from the component's own sizes) and takes the
+// next: the longest components start first, on SMs that are not yet crowded, and a warp that
+// finishes early picks up work instead of leaving its SM share idle until a launch drains.
+struct Warp2Queue {
+  const uint32_t* list;  // 2 words per entry: dispatch slot, warp2_queue_dims()
+  uint32_t n;
+  int slot_bytes;
+  uint32_t* ctr;         // [0] next ticket, [1] warps done; the last warp to finish puts both back to 0
+};
+
+// A queue entry's layout sizes in one word: candidate out-edges (<= 65535), nodes (<= 4095), and
+// unknowns (2..32, even) as n2 / 2 - 1.
+__host__ __device__ inline uint32_t warp2_queue_dims(int emax, int ncmax, int n2max) {
+  return (uint32_t)emax | (uint32_t)ncmax << 16 | (uint32_t)(n2max / 2 - 1) << 28;
+}
+
+// At most kWarp2QueueMaxWarps warps per CTA: 255 registers cover all four NREG paths (inlined: the
+// paths as separately allocated __noinline__ functions, reading P and K through their addresses, ran
+// cfg2 about 6 % slower)
+constexpr int kWarp2QueueMaxWarps = 8;
+__global__ void __launch_bounds__(kWarp2QueueMaxWarps * 32, 1)
+solve_warp2_queue_kernel(const DevProblem P, const DevConsts K, const Warp2Queue Q) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lane = threadIdx.x & 31;
+  unsigned char* base = smem_raw + (size_t)(threadIdx.x >> 5) * Q.slot_bytes;
+  for (;;) {
+    uint32_t t = 0;
+    if (lane == 0) t = atomicAdd(Q.ctr, 1u);
+    t = __shfl_sync(kFull, t, 0);
+    if (t >= Q.n) break;
+    const uint32_t c = Q.list[2 * t], dims = Q.list[2 * t + 1];
+    const int emax = dims & 0xffff, ncmax = (dims >> 16) & 0xfff, n2max = 2 * ((int)(dims >> 28) + 1);
+    // the slot's previous component wrote it through the generic proxy; this one's records arrive by bulk copies
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+    if (n2max <= 8)
+      warp2_solve<8>(P, K, c, base, emax, ncmax, n2max, lane);
+    else if (n2max <= 16)
+      warp2_solve<16>(P, K, c, base, emax, ncmax, n2max, lane);
+    else if (n2max <= 24)
+      warp2_solve<24>(P, K, c, base, emax, ncmax, n2max, lane);
+    else
+      warp2_solve<32>(P, K, c, base, emax, ncmax, n2max, lane);
+    // the mbarrier's word is ordinary shared memory in the next component's layout
+    __syncwarp();
+    if (lane == 0) mbar_inval((uint64_t*)(base + Warp2Layout(emax, ncmax, n2max).bar));
+    __syncwarp();
+  }
+  if (lane == 0) {
+    __threadfence();
+    if (atomicAdd(Q.ctr + 1, 1u) == gridDim.x * (blockDim.x >> 5) - 1) {
+      __threadfence();  // every other warp's last ticket and its count are in before the reset
+      atomicExch(Q.ctr, 0u);
+      atomicExch(Q.ctr + 1, 0u);
+    }
+  }
 }
 
 }  // namespace lfr
