@@ -18,7 +18,6 @@
 #include "lfr_graph.cuh"
 #include "lfr_solution.cuh"
 #include "lfr_solve_cta.cuh"
-#include "lfr_solve_tile.cuh"
 #include "lfr_solve_warp.cuh"
 #include "lfr_solve_warp2.cuh"
 #include "lfr_wire.cuh"
@@ -351,7 +350,7 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
   const bool force_pcg = pl->opt.linear_solver == 2;
   auto layout_bytes = [&](int vi, int e, int nc, int n2) {
     return (vi == kV1) ? lfr::WarpLayout(e, nc, n2).total
-                       : (is_tile(vi) ? lfr::TileLayout(e, nc, n2).total : lfr::Warp2Layout(e, nc, n2).total);
+                       : lfr::RegLayout(e, nc, n2, is_tile(vi) ? 64 : 32).total;  // (one layout for both tile widths)
   };
   // This runs on the calling thread while the GPU waits for its first launch: one pass over the
   // components into flat, reused arrays (no per-call allocation once the plan is warm), then a
@@ -438,8 +437,8 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
       }
       const int e = std::max<int>(1, (int)eup);
       int vi = (n2 <= 8) ? 0 : (n2 <= 16 ? 1 : (n2 <= 24 ? 2 : (n2 <= 32 ? 3 : (n2 <= 48 ? 5 : (n2 <= 64 ? 6 : (n2 <= 80 ? 7 : kV1))))));
-      if (vi <= 3 && n2 > tile_from && lfr::TileLayout(e, (int)nc, n2).total <= kMaxSmemPerBlock) vi = 4;
-      if (vi >= 5 && is_tile(vi) && (no_tile || lfr::TileLayout(e, (int)nc, n2).total > kMaxSmemPerBlock)) vi = kV1;
+      if (vi <= 3 && n2 > tile_from && lfr::RegLayout(e, (int)nc, n2, 64).total <= kMaxSmemPerBlock) vi = 4;
+      if (vi >= 5 && is_tile(vi) && (no_tile || lfr::RegLayout(e, (int)nc, n2, 64).total > kMaxSmemPerBlock)) vi = kV1;
       if (force_v1) vi = kV1;
       int need = layout_bytes(vi, e, (int)nc, n2);
       if (need > kMaxSmemPerBlock && vi != kV1) {  // the staged records do not fit: the Cholesky warp kernel reads them from global memory
@@ -573,7 +572,7 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
     const int ww = (dbg >> LFR_DBG_WARP2_WARPS_SHIFT) & 0xf;
     const int W = ww ? std::min(ww, lfr::kWarp2QueueMaxWarps) : kWarp2QueueWarpsDefault;
     const int cap = (kMaxSmemPerBlock / W) & ~15;
-    auto need = [&](uint32_t c) { return lfr::Warp2Layout(dim[c].e, dim[c].nc, dim[c].n2).total; };
+    auto need = [&](uint32_t c) { return lfr::RegLayout(dim[c].e, dim[c].nc, dim[c].n2, 32).total; };
     for (int pass = 0; pass < 2; ++pass) {
       Warp2Group g;
       g.offset = (uint32_t)pl->list_host.size();

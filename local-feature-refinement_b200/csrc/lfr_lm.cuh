@@ -2,7 +2,7 @@
 // SURVEY A.6) with the projected Armijo line search of the bounds-constrained problem (A.7b), from
 // iteration 0 to the per-slot statistics, written once over a tier's primitives.
 //
-// A tier (Warp2Tier, TileTier, WarpTier, CtaTier: one per solve kernel) wraps its context `C` and
+// A tier (RegTier for the warp2 and tile kernels, WarpTier, CtaTier) wraps its context `C` and
 // supplies, with every thread of its warp / CTA calling each member together:
 //   kStride, kTier, kPolyWord  threads per component, the profile's tier code, the word that takes
 //                              the line search's polynomial cycles

@@ -3,7 +3,7 @@ with LFR_SCHED_DUMP: host-only, no device involved): which scenes get a queue, h
 many warps per SM, and the LFR_DBG_WARP2_WARPS_SHIFT override.
 
 The helpers below are shared with tests/test_gpu_warp2_queue.py: `warp2_layout_bytes` states the
-`Warp2Layout` of lfr_solve_warp2.cuh in Python, `with_need` builds a component whose own layout is an
+`RegLayout` of lfr_solve_warp2.cuh at 32 threads in Python, `with_need` builds a component whose own layout is an
 exact byte count, and `schedule_of` reads the dump of any problem."""
 import ctypes as C
 import re
@@ -25,7 +25,7 @@ def cap_of(w):
 
 def warp2_layout_bytes(e, nc, n2):
     """Shared-memory bytes of one warp2 slot laid out for `e` candidate out-edges, `nc` nodes and `n2`
-    unknowns: `Warp2Layout(e, nc, n2).total`, field by field."""
+    unknowns: `RegLayout(e, nc, n2, 32).total`, field by field."""
     def up16(o):
         return (o + 15) // 16 * 16
     ldh = n2 | 1
@@ -232,7 +232,7 @@ def _shape_grid(p):
 
 
 def test_layout_formula_matches_the_schedule(b200, capfd, monkeypatch, cfg4s):
-    """warp2_layout_bytes is Warp2Layout: a one-component problem's slot (queue) or smem/warp (four-warp
+    """warp2_layout_bytes is RegLayout at 32 threads: a one-component problem's slot (queue) or smem/warp (four-warp
     bucket) is the layout of its own sizes; a few components share the maximum of theirs (queue) or
     the layout of their maxima (bucket).  Every layout is a multiple of 16 bytes."""
     shapes = _shape_grid(cfg4s)
