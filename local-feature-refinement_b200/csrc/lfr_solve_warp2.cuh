@@ -512,12 +512,22 @@ __device__ __forceinline__ CandNorms reg_candidate(const RegCtx<T>& C, double al
   return nr;
 }
 
+// The register size class of a component of (at most) n2max unknowns: 8, 16, 24 or 32 for a warp
+__host__ __device__ constexpr int reg_class(int n2max) { return (n2max + 7) & ~7; }
+
 // The register tier's primitives as the driver's operations (see lfr_lm.cuh).  What the widths keep
 // apart is how they reduce: a warp sums cost, phi' and the CandNorms of the parameter test in one
 // butterfly of the candidate's evaluation; a tile reduces cost and phi' through `red` and takes each
 // norm by a sum of its own.
+// NREG is the register rows' size class, fixed at compile time (the per-bucket and tile kernels), or 0:
+// the class is the warp-uniform run-time `nreg` (the queue kernel).  Only the elimination needs a
+// compile-time row size, so with NREG = 0 lm_step branches over the four inlined reg_lm_step<8..32>
+// and one copy of everything else (setup, evaluation, assembly, line search, write-back) serves every
+// class: about a third of the instructions of four whole solves, which an SM's warps would otherwise
+// fetch from up to four places at once.
 template <int T, int NREG>
 struct RegTier {
+  static_assert(NREG > 0 || T == 32, "a run-time register class is a warp's");
   using G = Group<T>;
   static constexpr int kStride = T;
   static constexpr unsigned kTier = T == 32 ? LmProfile::kWarp2 : LmProfile::kTile;
@@ -525,6 +535,7 @@ struct RegTier {
   RegCtx<T>& C;
   const DevConsts& K;
   CandNorms nr;  // of the last candidate (warp)
+  int nreg;      // NREG == 0: reg_class() of the component
   __device__ int tid() const { return C.tid; }
   __device__ int lane() const { return C.tid & 31; }
   __device__ bool lead() const { return C.tid == 0; }
@@ -561,7 +572,16 @@ struct RegTier {
   __device__ double eval_x() { return eval<false, false>(C.x); }
   __device__ double assemble(bool first) { return reg_assemble<false>(C, first, K); }
   __device__ bool lm_step(double radius, double* model_change, double* gd, double* dmax) {
-    return reg_lm_step<NREG>(C, radius, K, model_change, gd, dmax);
+    if constexpr (NREG > 0) {
+      return reg_lm_step<NREG>(C, radius, K, model_change, gd, dmax);
+    } else {
+      switch (nreg) {
+        case 8: return reg_lm_step<8>(C, radius, K, model_change, gd, dmax);
+        case 16: return reg_lm_step<16>(C, radius, K, model_change, gd, dmax);
+        case 24: return reg_lm_step<24>(C, radius, K, model_change, gd, dmax);
+        default: return reg_lm_step<32>(C, radius, K, model_change, gd, dmax);
+      }
+    }
   }
   __device__ double trial(double alpha) {
     nr = reg_candidate(C, alpha, K);
@@ -617,8 +637,9 @@ struct RegTier {
 };
 
 // One component on T threads, in the shared memory at `base` laid out for (emax, ncmax, n2max): the
-// per-bucket kernels and the queue kernel below run exactly this.  The setup is one warp's work
-// (solve.cc:98-143); a tile's warp 0 broadcasts its three results through `hdr`.
+// per-bucket kernels and the queue kernel below run exactly this (the queue kernel with NREG = 0, the
+// register class then taken from n2max).  The setup is one warp's work (solve.cc:98-143); a tile's
+// warp 0 broadcasts its three results through `hdr`.
 template <int T, int NREG>
 __device__ __forceinline__ void reg_solve(const DevProblem& P, const DevConsts& K, uint32_t c, unsigned char* base,
                                           int emax, int ncmax, int n2max, int tid) {
@@ -646,7 +667,7 @@ __device__ __forceinline__ void reg_solve(const DevProblem& P, const DevConsts& 
   C.nf = nf;
   C.n = 2 * nf;
   if constexpr (T == 32) __syncwarp();
-  RegTier<T, NREG> Tr{C, K, {0.0, 0.0}};
+  RegTier<T, NREG> Tr{C, K, {0.0, 0.0}, reg_class(n2max)};
   lm_solve(Tr, P, K, c, prof);
 }
 
@@ -690,9 +711,10 @@ __host__ __device__ inline uint32_t warp2_queue_dims(int emax, int ncmax, int n2
   return (uint32_t)emax | (uint32_t)ncmax << 16 | (uint32_t)(n2max / 2 - 1) << 28;
 }
 
-// At most kWarp2QueueMaxWarps warps per CTA: 255 registers cover all four NREG paths (inlined: the
-// paths as separately allocated __noinline__ functions, reading P and K through their addresses, ran
-// cfg2 about 6 % slower)
+// At most kWarp2QueueMaxWarps warps per CTA: 255 registers cover all four register classes, whose
+// eliminations are inlined into the one copy of the rest of the solve (RegTier<32, 0>: four whole
+// solves, one per class, made the kernel 55 k instructions; the classes as separately allocated
+// __noinline__ functions, reading P and K through their addresses, ran cfg2 about 6 % slower)
 constexpr int kWarp2QueueMaxWarps = 8;
 __global__ void __launch_bounds__(kWarp2QueueMaxWarps * 32, 1)
 solve_warp2_queue_kernel(const DevProblem P, const DevConsts K, const Warp2Queue Q) {
@@ -709,14 +731,7 @@ solve_warp2_queue_kernel(const DevProblem P, const DevConsts K, const Warp2Queue
     // the slot's previous component wrote it through the generic proxy; this one's records arrive by bulk copies
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncwarp();
-    if (n2max <= 8)
-      reg_solve<32, 8>(P, K, c, base, emax, ncmax, n2max, lane);
-    else if (n2max <= 16)
-      reg_solve<32, 16>(P, K, c, base, emax, ncmax, n2max, lane);
-    else if (n2max <= 24)
-      reg_solve<32, 24>(P, K, c, base, emax, ncmax, n2max, lane);
-    else
-      reg_solve<32, 32>(P, K, c, base, emax, ncmax, n2max, lane);
+    reg_solve<32, 0>(P, K, c, base, emax, ncmax, n2max, lane);  // register class reg_class(n2max)
     // the mbarrier's word is ordinary shared memory in the next component's layout
     __syncwarp();
     if (lane == 0) mbar_inval((uint64_t*)(base + RegLayout(emax, ncmax, n2max, 32).bar));

@@ -1,4 +1,5 @@
-"""Per-component cycle breakdown of the solve kernels (LFR_DBG_PROFILE)."""
+"""Per-component cycle breakdown of the solve kernels (LFR_DBG_PROFILE); for the eight longest components
+also when their solve started and finished (%globaltimer, µs after the first component's start)."""
 import os
 import sys
 
@@ -26,9 +27,10 @@ e1.record()
 torch.cuda.synchronize()
 print("solve ms", e0.elapsed_time(e1), "launches", plan.num_launches())
 pos, st = plan.download()
-rec, _ = plan.profile()
+rec, tm = plan.profile()
 it = st["iterations"]
 sel = it > 0
+t0 = tm[sel, 0].min()
 tot = rec["total"][sel].astype(np.float64)
 print("components", sel.sum(), "iters sum", it.sum())
 print("cycles per component: mean %.0f  p50 %.0f  p99 %.0f  max %.0f" % (
@@ -42,4 +44,5 @@ idx = np.nonzero(sel)[0][w]
 for i in idx:
     print("  slot", i, "tier", PROFILE_TIERS.get(int(rec["tier"][i])), "nodes", int(p.comp_ptr[i + 1] - p.comp_ptr[i]),
           "iters", it[i], "ls_steps", int(rec["ls_steps"][i]), "cycles", [int(rec[k][i]) for k in names],
-          "counter", int(rec["counter"][i]), "sm", int(rec["smid"][i]))
+          "counter", int(rec["counter"][i]), "sm", int(rec["smid"][i]),
+          "start/end us %.1f %.1f" % ((int(tm[i, 0]) - int(t0)) / 1e3, (int(tm[i, 1]) - int(t0)) / 1e3))
