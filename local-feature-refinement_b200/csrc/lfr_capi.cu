@@ -65,7 +65,7 @@ constexpr int kTileFromDefault = 32;
 // warps per SM of the warp-register tier's queue kernel (LFR_DBG_WARP2_WARPS_SHIFT overrides, up to
 // lfr::kWarp2QueueMaxWarps)
 constexpr int kWarp2QueueWarpsDefault = 8;
-constexpr int kScheduleThreadsMax = 8;  // host threads that classify the dispatch list (build_buckets)
+constexpr int kScheduleThreadsMax = 8;  // host threads that classify the dispatch list (build_schedule)
 constexpr int kMaxStreams = 12;
 
 lfr::DevConsts make_consts(const lfr_options& o) {
@@ -127,29 +127,62 @@ struct DevBuf {
   T* as() const { return static_cast<T*>(p); }
 };
 
-// One launch of the CTA tier: a size class of large components (its dynamic shared memory and the
-// register cap MINB decide how many of them an SM runs at once).
-struct CtaGroup {
-  uint32_t first = 0, n = 0, max_free = 0;
-  int minb = 2;
-  int smem_vecs = 6;  // how many of the CG arrays (p, w, r, z, y, preconditioner) live in shared memory
+// The solve kernels.  The schedule builder picks one per launch; launch_solve has one launch statement each.
+enum class Kernel : uint8_t {
+  kWarp2x4_8, kWarp2x4_16, kWarp2x1_32,                // solve_warp2_kernel<WARPS, NREG>
+  kQueue,                                              // solve_warp2_queue_kernel
+  kTile64x32, kTile64x48, kTile64x64, kTile128x80,     // solve_tile_kernel<T, NREG>
+  kWarp4, kWarp1,                                      // solve_warp_kernel<WARPS> (shared-memory Cholesky)
+  kCta2, kCta3, kCta4,                                 // solve_cta_kernel<256, MINB>
+  kCount
+};
+inline bool is_cta(Kernel k) { return k >= Kernel::kCta2; }
+
+// Where a kernel reads its edge records: staged into shared memory from DevProblem::edges (the HBM copy
+// or the caller's pinned array), from the HBM copy by global index, or from the CTA tier's own arrays
+// that cta_prepare_kernel fills.
+enum class Edges : uint8_t { kStaged, kGlobal, kPrepared };
+
+struct KernelInfo {
+  const void* fn;  // for cudaFuncSetAttribute
+  int threads;     // per component; a CTA runs Launch::warps components
+  int per_cta;     // components per CTA (the queue: set per launch)
+  Edges edges;
+  int smem_max;    // dynamic shared memory to allow
+  int label;       // what LFR_SCHED_DUMP prints: a bucket's variant code, or a CTA kernel's MINB
 };
 
-// One launch of the warp-register tier's queue kernel: `n` entries of two words at `offset` of the
-// list buffer, `warps` per CTA (one CTA per SM), each in a slot of `slot_bytes`.
-struct Warp2Group {
+const KernelInfo kKernels[] = {
+    {(const void*)lfr::solve_warp2_kernel<4, 8>, 32, 4, Edges::kStaged, kMaxSmemPerBlock, 8},
+    {(const void*)lfr::solve_warp2_kernel<4, 16>, 32, 4, Edges::kStaged, kMaxSmemPerBlock, 16},
+    {(const void*)lfr::solve_warp2_kernel<1, 32>, 32, 1, Edges::kStaged, kMaxSmemPerBlock, 32},
+    {(const void*)lfr::solve_warp2_queue_kernel, 32, 0, Edges::kStaged, kMaxSmemPerBlock, 0},
+    {(const void*)lfr::solve_tile_kernel<64, 32>, 64, 1, Edges::kStaged, kMaxSmemPerBlock, 132},
+    {(const void*)lfr::solve_tile_kernel<64, 48>, 64, 1, Edges::kStaged, kMaxSmemPerBlock, 48},
+    {(const void*)lfr::solve_tile_kernel<64, 64>, 64, 1, Edges::kStaged, kMaxSmemPerBlock, 64},
+    {(const void*)lfr::solve_tile_kernel<128, 80>, 128, 1, Edges::kStaged, kMaxSmemPerBlock, 80},
+    {(const void*)lfr::solve_warp_kernel<4>, 32, 4, Edges::kGlobal, kMaxSmemPerBlock, 0},
+    {(const void*)lfr::solve_warp_kernel<1>, 32, 1, Edges::kGlobal, kMaxSmemPerBlock, 0},
+    {(const void*)lfr::solve_cta_kernel<256, 2>, 256, 1, Edges::kPrepared, 200 * 1024, 2},
+    {(const void*)lfr::solve_cta_kernel<256, 3>, 256, 1, Edges::kPrepared, 200 * 1024, 3},
+    {(const void*)lfr::solve_cta_kernel<256, 4>, 256, 1, Edges::kPrepared, 200 * 1024, 4},
+};
+static_assert(sizeof(kKernels) / sizeof(kKernels[0]) == (size_t)Kernel::kCount, "one entry per kernel");
+inline const KernelInfo& info(Kernel k) { return kKernels[(int)k]; }
+
+// One kernel launch of a solve: `n` members from `offset`, `warps` of them per CTA, each in `bytes` of
+// dynamic shared memory.
+//  - per-bucket kernels: dispatch slots in the list buffer; `bytes` is the layout of the members' maxima
+//    (emax, ncmax, n2max);
+//  - the queue: entries of two words in the list buffer, `warps` per SM, slots of `bytes`;
+//  - the CTA tier: components of L_comps, one per CTA; `bytes` holds the CG vectors of the largest
+//    (`max_free` free nodes, the first `smem_vecs` of p, w, r, z, y and the preconditioner).
+struct Launch {
+  Kernel kernel = Kernel::kCount;
   uint32_t offset = 0, n = 0;
-  int slot_bytes = 0, warps = 0;
-};
-
-struct Bucket {
-  uint32_t offset = 0;  // into the bucket-list buffer
-  uint32_t n = 0;
-  int emax = 0, ncmax = 0, n2max = 0, smem_per_warp = 0, warps = 4;
-  // 0: shared-memory Cholesky warp kernel (80 < n <= 96, and components whose staged records do not
-  // fit); 8..32: register Gauss-Jordan warp kernel (n <= variant); 132, 48, 64, 80: tile kernels
-  int variant = 0;
-  bool stages_edges() const { return variant != 0; }  // warp2 / tile tiers pull their edge records into shared memory
+  int emax = 0, ncmax = 0, n2max = 0, bytes = 0, warps = 1;
+  uint32_t max_free = 0;
+  int smem_vecs = 0;
 };
 
 int validate(const lfr_problem* p) {
@@ -190,28 +223,26 @@ struct lfr_plan {
   int* d_err() const { return reinterpret_cast<int*>(d_kept() + Cp); }
   unsigned long long* d_pull() const { return reinterpret_cast<unsigned long long*>(d_err() + 2); }  // {ticketed, arrived} bytes
   size_t stats_bytes() const { return 16 * (size_t)Cp + 16 * (size_t)Cp + 8 + 16; }
-  std::vector<Bucket> buckets;
-  std::vector<Warp2Group> w2_groups;  // the warp-register tier's four-warp buckets, as queue launches
-  std::vector<uint32_t> w2_slots;     // build_buckets scratch
+  std::vector<Launch> launches;       // in launch order: the CTA tier, the queue, the buckets
+  std::vector<uint32_t> w2_slots;     // build_schedule scratch: the queue's members
   DevBuf queue_ctr;                   // two words per queue launch (solve_warp2_queue_kernel)
   int n_sms = 0;
-  int num_launches() const { return (int)buckets.size() + (int)w2_groups.size() + (int)cta_groups.size(); }
+  int num_launches() const { return (int)launches.size(); }
   std::vector<uint32_t> comp_size;  // nodes per dispatch slot
   std::vector<uint32_t> list_host;
   // CTA tier (block-Jacobi PCG): components with more than kMaxWarpN2 unknowns, or all with linear_solver = 2
   struct SchedDim { int e, nc, n2; };
-  std::vector<uint16_t> sched_key;        // build_buckets scratch: (variant, shared-memory class) of every slot
+  std::vector<uint16_t> sched_key;        // build_schedule scratch: (route, shared-memory class) of every slot
   std::vector<SchedDim> sched_dim;
+  // the CTA tier's components by size class, in dispatch order inside a class
   std::vector<uint32_t> large_slots;
   std::vector<uint64_t> large_cand;       // candidate out-edges of each large component (row_ptr sums)
   std::vector<uint32_t> large_free;       // its non-root nodes (upper bound of the free nodes)
   std::vector<uint64_t> large_ell;        // its sliced-ELL slots (32 x the largest candidate out-degree of every 32-node slice)
   std::vector<lfr::CtaComp> L_comps_host;
-  std::vector<CtaGroup> cta_groups;
   uint32_t n_large = 0;
   DevBuf L_comps, L_rec, L_meta, L_inlist, L_twin, L_fdst, L_bE01, L_bE23, L_fdstE, L_ell_base, L_scr, L_q, L_node, L_outptr, L_inptr, L_freeof, L_x, L_xc, L_lof, L_vec;
   uint64_t L_total_free = 0;
-  uint32_t L_max_free = 0;
   uint32_t n_solved = 0;
   bool profile = false;
   // lfr_solve() zero-copy: staging tiers read the caller's pinned edge array / write the caller's
@@ -221,7 +252,6 @@ struct lfr_plan {
   const uint8_t* slot_owner = nullptr;  // lfr_solve_multi(): owner[c] of every dispatch slot, this plan solves owner == owner_id
   uint8_t owner_id = 0;
   bool edges_in_hbm = false;       // the edge array was (or is being) copied to `edges`
-  bool needs_hbm_edges = false;    // some bucket (smem-Cholesky warp tier) reads edge records from global memory by index
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_edges = nullptr;  // bulk edge copy done (only the non-staging tiers wait for it)
   cudaEvent_t ev_small = nullptr;  // fork / join of the second upload stream
@@ -324,22 +354,31 @@ int upload(DevBuf* d, const T* h, size_t count, cudaStream_t s) {
   return LFR_OK;
 }
 
-// Size-bucketed schedule: components are grouped by the shared memory one warp
-// needs for them, so small tracks run at high occupancy and the few large
-// components do not dictate the carve-up of everyone else.  Buckets are
-// launched on concurrent streams, largest components first; the register warp
-// tier's four-warp buckets are then merged into one persistent queue launch.
-int build_buckets(lfr_plan* pl, const lfr_problem* p) {
+// The solve's launch list (pl->launches).  Components are grouped by the shared memory one warp needs
+// for them, so small tracks run at high occupancy and the few large components do not dictate the
+// carve-up of everyone else.  The CTA tier launches first, one launch per size class; then the register
+// warp tier's four-warp members in persistent queue launches (where one of them has more than 16
+// unknowns), then one launch per (route, shared-memory class) bucket, largest components first.
+int build_schedule(lfr_plan* pl, const lfr_problem* p) {
   // shared-memory classes of a launch (finer classes — one per "one more CTA fits an SM" boundary — mean
   // more launches for the same resident work)
   static const int kClass[] = {2048, 3072, 4096, 6144, 8192, 12288, 16384, 24576, 32768, 57344, kMaxSmemPerBlock};
   constexpr int n_class = sizeof(kClass) / sizeof(kClass[0]);
-  // register warp kernel (8..32), register tile kernel (132 = 64 threads x NREG 32; 48, 64: 64 threads;
-  // 80: 128 threads), smem-Cholesky warp kernel (0)
-  static const int kVariant[9] = {8, 16, 24, 32, 132, 48, 64, 80, 0};
-  constexpr int kNV = 9, kV1 = 8, kKeys = kNV * n_class;
+  // the route of a component off the CTA tier: a register class (NREG 8..32), a tile kernel, or the
+  // shared-memory Cholesky warp kernel; inside a shared-memory class the last route launches first
+  enum Route { kReg8, kReg16, kReg24, kReg32, kTile32, kTile48, kTile64, kTile80, kCholesky, kRoutes };
+  // a route's kernel where four of its slots fit a CTA, and where they do not (the register classes
+  // above 16 unknowns have no four-warp kernel of their own: the queue runs them)
+  static const Kernel kFour[kRoutes] = {Kernel::kWarp2x4_8, Kernel::kWarp2x4_16, Kernel::kQueue, Kernel::kQueue,
+                                        Kernel::kTile64x32, Kernel::kTile64x48, Kernel::kTile64x64, Kernel::kTile128x80,
+                                        Kernel::kWarp4};
+  static const Kernel kOne[kRoutes] = {Kernel::kWarp2x1_32, Kernel::kWarp2x1_32, Kernel::kWarp2x1_32, Kernel::kWarp2x1_32,
+                                       Kernel::kTile64x32, Kernel::kTile64x48, Kernel::kTile64x64, Kernel::kTile128x80,
+                                       Kernel::kWarp1};
+  constexpr int kKeys = kRoutes * n_class;
   constexpr uint16_t kNoKey = 0xffff;
-  auto is_tile = [](int vi) { return vi >= 4 && vi <= 7; };
+  auto is_tile = [](int r) { return r >= kTile32 && r <= kTile80; };
+  auto fits_four = [](int bytes) { return 4 * bytes <= kMaxSmemPerBlock; };
   const int dbg = pl->opt.debug_flags;
   const bool no_tile = (dbg & LFR_DBG_NO_TILE) != 0;
   // components with more than tile_from unknowns (and <= 32) go to the two-warp tile kernel
@@ -348,19 +387,19 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
   const int tile_from = no_tile ? 32 : (tf ? tf : kTileFromDefault);
   const bool force_v1 = (dbg & LFR_DBG_FORCE_SMEM_CHOLESKY) != 0;
   const bool force_pcg = pl->opt.linear_solver == 2;
-  auto layout_bytes = [&](int vi, int e, int nc, int n2) {
-    return (vi == kV1) ? lfr::WarpLayout(e, nc, n2).total
-                       : lfr::RegLayout(e, nc, n2, is_tile(vi) ? 64 : 32).total;  // (one layout for both tile widths)
+  auto layout_bytes = [&](int r, int e, int nc, int n2) {
+    return (r == kCholesky) ? lfr::WarpLayout(e, nc, n2).total
+                            : lfr::RegLayout(e, nc, n2, is_tile(r) ? 64 : 32).total;  // (one layout for both tile widths)
   };
   // This runs on the calling thread while the GPU waits for its first launch: one pass over the
   // components into flat, reused arrays (no per-call allocation once the plan is warm), then a
-  // counting sort of the slots by (variant, shared-memory class).
+  // counting sort of the slots by (route, shared-memory class).
   const uint32_t C = p->n_components;
   pl->comp_size.resize(C);
   pl->sched_key.resize(C);
   pl->sched_dim.resize(C);
   pl->n_solved = 0;
-  pl->buckets.clear();
+  pl->launches.clear();
   pl->large_slots.clear();
   pl->large_cand.clear();
   pl->large_free.clear();
@@ -377,8 +416,9 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
   // per-slot entries of its own range and its own accumulator, so ranges run on separate threads
   // (merged in range order: the schedule does not depend on the thread count).
   struct Acc {
-    Bucket caps[kKeys];
+    lfr_plan::SchedDim caps[kKeys] = {};  // maxima of the members
     uint32_t count[kKeys] = {};
+    uint32_t fit4[kKeys] = {};            // members whose own slot fits four to a CTA
     uint32_t n_solved = 0;
     std::vector<uint32_t> large_slots, large_free;
     std::vector<uint64_t> large_cand, large_ell;
@@ -436,14 +476,14 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
         continue;
       }
       const int e = std::max<int>(1, (int)eup);
-      int vi = (n2 <= 8) ? 0 : (n2 <= 16 ? 1 : (n2 <= 24 ? 2 : (n2 <= 32 ? 3 : (n2 <= 48 ? 5 : (n2 <= 64 ? 6 : (n2 <= 80 ? 7 : kV1))))));
-      if (vi <= 3 && n2 > tile_from && lfr::RegLayout(e, (int)nc, n2, 64).total <= kMaxSmemPerBlock) vi = 4;
-      if (vi >= 5 && is_tile(vi) && (no_tile || lfr::RegLayout(e, (int)nc, n2, 64).total > kMaxSmemPerBlock)) vi = kV1;
-      if (force_v1) vi = kV1;
-      int need = layout_bytes(vi, e, (int)nc, n2);
-      if (need > kMaxSmemPerBlock && vi != kV1) {  // the staged records do not fit: the Cholesky warp kernel reads them from global memory
-        vi = kV1;
-        need = layout_bytes(vi, e, (int)nc, n2);
+      int r = (n2 <= 8) ? kReg8 : (n2 <= 16 ? kReg16 : (n2 <= 24 ? kReg24 : (n2 <= 32 ? kReg32 : (n2 <= 48 ? kTile48 : (n2 <= 64 ? kTile64 : (n2 <= 80 ? kTile80 : kCholesky))))));
+      if (r <= kReg32 && n2 > tile_from && lfr::RegLayout(e, (int)nc, n2, 64).total <= kMaxSmemPerBlock) r = kTile32;
+      if (r >= kTile48 && is_tile(r) && (no_tile || lfr::RegLayout(e, (int)nc, n2, 64).total > kMaxSmemPerBlock)) r = kCholesky;
+      if (force_v1) r = kCholesky;
+      int need = layout_bytes(r, e, (int)nc, n2);
+      if (need > kMaxSmemPerBlock && r != kCholesky) {  // the staged records do not fit: the Cholesky warp kernel reads them from global memory
+        r = kCholesky;
+        need = layout_bytes(r, e, (int)nc, n2);
       }
       if (need > kMaxSmemPerBlock) {
         // a dense, high-degree component (its per-edge scratch alone exceeds one SM's shared
@@ -453,14 +493,15 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
       }
       int k = 0;
       while (need > kClass[k]) ++k;  // need <= kClass[n_class - 1] here
-      const int key = vi * n_class + k;
+      const int key = r * n_class + k;
       key_of[c] = (uint16_t)key;
       dim[c] = lfr_plan::SchedDim{e, (int)nc, n2};
-      Bucket& cb = A.caps[key];
+      lfr_plan::SchedDim& cb = A.caps[key];
       ++A.count[key];
-      cb.emax = std::max(cb.emax, e);
-      cb.ncmax = std::max(cb.ncmax, (int)nc);
-      cb.n2max = std::max(cb.n2max, n2);
+      A.fit4[key] += fits_four(need);
+      cb.e = std::max(cb.e, e);
+      cb.nc = std::max(cb.nc, (int)nc);
+      cb.n2 = std::max(cb.n2, n2);
     }
   };
   // ranges of about equal node counts; extra threads only where their start-up pays
@@ -484,128 +525,22 @@ int build_buckets(lfr_plan* pl, const lfr_problem* p) {
     classify(cut[0], cut[1], acc[0]);
     for (std::thread& w : workers) w.join();
   }
-  Bucket caps[kKeys];
-  uint32_t count[kKeys] = {};
+  lfr_plan::SchedDim caps[kKeys] = {};
+  uint32_t count[kKeys] = {}, fit4[kKeys] = {};
   for (const Acc& A : acc) {  // range order
     if (A.rc != LFR_OK) return fail(A.rc, A.msg);
     pl->n_solved += A.n_solved;
     for (int k = 0; k < kKeys; ++k) {
       count[k] += A.count[k];
-      caps[k].emax = std::max(caps[k].emax, A.caps[k].emax);
-      caps[k].ncmax = std::max(caps[k].ncmax, A.caps[k].ncmax);
-      caps[k].n2max = std::max(caps[k].n2max, A.caps[k].n2max);
-    }
-    pl->large_slots.insert(pl->large_slots.end(), A.large_slots.begin(), A.large_slots.end());
-    pl->large_cand.insert(pl->large_cand.end(), A.large_cand.begin(), A.large_cand.end());
-    pl->large_free.insert(pl->large_free.end(), A.large_free.begin(), A.large_free.end());
-    pl->large_ell.insert(pl->large_ell.end(), A.large_ell.begin(), A.large_ell.end());
-  }
-  // emission order: largest shared-memory class first, within a class the higher tiers first
-  uint32_t start[kKeys], total = 0;
-  for (int k = n_class - 1; k >= 0; --k)
-    for (int vi = kNV - 1; vi >= 0; --vi) {
-      start[vi * n_class + k] = total;
-      total += count[vi * n_class + k];
-    }
-  pl->list_host.resize(total);
-  {
-    uint32_t fill[kKeys];
-    std::memcpy(fill, start, sizeof(fill));
-    uint32_t* list = pl->list_host.data();
-    for (uint32_t c = 0; c < C; ++c)
-      if (key_of[c] != kNoKey) list[fill[key_of[c]]++] = c;  // ascending slot index inside a bucket
-  }
-  pl->needs_hbm_edges = false;
-  auto emit = [&](int vi, const Bucket& cap, uint32_t offset, uint32_t n_mem) {
-    Bucket b = cap;
-    b.variant = kVariant[vi];
-    b.n = n_mem;
-    b.offset = offset;
-    b.smem_per_warp = layout_bytes(vi, b.emax, b.ncmax, b.n2max);
-    b.warps = (4 * b.smem_per_warp <= kMaxSmemPerBlock) ? 4 : 1;
-    if (b.variant >= 48) b.warps = 1;  // tile kernels: one component per CTA
-    if (b.warps == 1 && b.variant != 0 && b.variant < 48) b.variant = 32;  // only <1,32> is instantiated for single-warp CTAs
-    pl->buckets.push_back(b);
-    if (!b.stages_edges()) pl->needs_hbm_edges = true;  // the Cholesky warp tier reads records from HBM by global index
-  };
-  for (int k = n_class - 1; k >= 0; --k) {
-    for (int vi = kNV - 1; vi >= 0; --vi) {
-      const int key = vi * n_class + k;
-      if (!count[key]) continue;
-      const Bucket& cap = caps[key];
-      if (layout_bytes(vi, cap.emax, cap.ncmax, cap.n2max) <= kMaxSmemPerBlock) {
-        emit(vi, cap, start[key], count[key]);
-      } else {
-        // every member fits on its own but the union of their maxima does not: one launch each
-        for (uint32_t i = 0; i < count[key]; ++i) {
-          const uint32_t c = pl->list_host[start[key] + i];
-          Bucket one;
-          one.emax = dim[c].e;
-          one.ncmax = dim[c].nc;
-          one.n2max = dim[c].n2;
-          emit(vi, one, start[key] + i, 1);
-        }
-      }
+      fit4[k] += A.fit4[k];
+      caps[k].e = std::max(caps[k].e, A.caps[k].e);
+      caps[k].nc = std::max(caps[k].nc, A.caps[k].nc);
+      caps[k].n2 = std::max(caps[k].n2, A.caps[k].n2);
     }
   }
-  // The register warp tier's four-warp buckets become queue launches (solve_warp2_queue_kernel): their
-  // members in dispatch order (largest first), each entry {slot, own layout sizes}.  One launch takes
-  // every member whose own layout fits a slot at W warps per SM; the rest (if any) go to a second at
-  // as many warps as its largest member allows (>= 4: they came from four-warp buckets).  Only where
-  // some member has more than 16 unknowns: without one the per-bucket kernels run 12 warps per SM at
-  // 168 registers, which the queue kernel (255 registers for all four NREG paths) cannot (DESIGN §4).
-  pl->w2_groups.clear();
-  bool wide = false;
-  for (const Bucket& b : pl->buckets) wide = wide || (b.variant >= 24 && b.variant <= 32 && b.warps == 4);
-  std::vector<uint32_t>& q = pl->w2_slots;
-  q.clear();
-  size_t kept = 0;
-  for (const Bucket& b : pl->buckets) {
-    if (wide && b.variant >= 8 && b.variant <= 32 && b.warps == 4)
-      q.insert(q.end(), pl->list_host.begin() + b.offset, pl->list_host.begin() + b.offset + b.n);
-    else
-      pl->buckets[kept++] = b;
-  }
-  pl->buckets.resize(kept);
-  if (!q.empty()) {
-    std::sort(q.begin(), q.end());
-    const int ww = (dbg >> LFR_DBG_WARP2_WARPS_SHIFT) & 0xf;
-    const int W = ww ? std::min(ww, lfr::kWarp2QueueMaxWarps) : kWarp2QueueWarpsDefault;
-    const int cap = (kMaxSmemPerBlock / W) & ~15;
-    auto need = [&](uint32_t c) { return lfr::RegLayout(dim[c].e, dim[c].nc, dim[c].n2, 32).total; };
-    for (int pass = 0; pass < 2; ++pass) {
-      Warp2Group g;
-      g.offset = (uint32_t)pl->list_host.size();
-      for (uint32_t c : q) {
-        const int b = need(c);
-        if ((b <= cap) != (pass == 0)) continue;
-        pl->list_host.push_back(c);
-        pl->list_host.push_back(lfr::warp2_queue_dims(dim[c].e, dim[c].nc, dim[c].n2));
-        g.slot_bytes = std::max(g.slot_bytes, b);
-        ++g.n;
-      }
-      if (!g.n) continue;
-      g.warps = pass == 0 ? W : std::min(W, kMaxSmemPerBlock / g.slot_bytes);
-      pl->w2_groups.push_back(g);
-    }
-  }
-  return LFR_OK;
-}
-
-// CTA-tier components: the host only lays out per-component offsets (upper bounds: candidate edges
-// from row_ptr, non-root nodes) and sizes the HBM arrays; the kept-edge / in-edge lists, free-variable
-// numbering and twins are built on the device by cta_prepare_kernel (launched by fill_plan once the
-// edge records and local_of are in HBM).
-int prepare_large(lfr_plan* pl, const lfr_problem* p, cudaStream_t s) {
-  pl->n_large = (uint32_t)pl->large_slots.size();
-  pl->L_total_free = 0;
-  pl->L_max_free = 0;
-  pl->cta_groups.clear();
-  if (pl->n_large == 0) return LFR_OK;
-  std::vector<lfr::CtaComp>& comps = pl->L_comps_host;  // plan member: the async upload reads it
-  comps.assign(pl->n_large, lfr::CtaComp{});
-  // size classes by free nodes (upper bound): 104 bytes of CG vectors per free node in shared memory
-  // -> 1 / 2 / 4 / 8 components per SM by shared memory; registers cap it at MINB
+  // The CTA tier: one launch per size class by free nodes (upper bound), in dispatch order (largest
+  // first) inside a class.  104 bytes of CG vectors per free node in shared memory -> 1 / 2 / 4 / 8
+  // components per SM by shared memory; registers cap it at MINB.
   static const uint32_t kClassMaxFree[4] = {0xffffffffu, 1008, 504, 250};
   int minb[4] = {2, 2, 3, 4};
   if (const char* e = std::getenv("LFR_CTA_MINB")) {  // tuning hook: "2,2,3,4"
@@ -620,42 +555,154 @@ int prepare_large(lfr_plan* pl, const lfr_problem* p, cudaStream_t s) {
       for (int i = 0; i < 4; ++i) smem_vecs[i] = std::min(6, std::max(0, a[i]));
   }
   auto class_of = [&](uint32_t nfree) { return nfree > kClassMaxFree[1] ? 0 : (nfree > kClassMaxFree[2] ? 1 : (nfree > kClassMaxFree[3] ? 2 : 3)); };
-  pl->cta_groups.clear();
-  uint64_t e_off = 0, n_off = 0, f_off = 0, ell_off = 0, s_off = 0;
-  uint32_t k = 0;
   for (int cls = 0; cls < 4; ++cls) {
-    CtaGroup g;
-    g.first = k;
-    g.minb = minb[cls];
+    Launch g;
+    g.kernel = minb[cls] >= 4 ? Kernel::kCta4 : (minb[cls] == 3 ? Kernel::kCta3 : Kernel::kCta2);
+    g.offset = (uint32_t)pl->large_slots.size();
     g.smem_vecs = smem_vecs[cls];
-    for (uint32_t i = 0; i < pl->n_large; ++i) {  // dispatch order (largest first) inside a class
-      if (class_of(pl->large_free[i]) != cls) continue;
-      const uint32_t c = pl->large_slots[i];
-      const uint32_t nc = p->comp_ptr[c + 1] - p->comp_ptr[c];
-      if (pl->large_cand[i] > 0xffffffffull) return fail(LFR_EUNSUPPORTED, "component with more than 2^32 out-edges");
-      lfr::CtaComp& cc = comps[k];
-      cc.slot = c;
-      cc.Nc = nc;
-      cc.Ec = 0;  // filled on the device, with nf and regular
-      cc.nf = 0;
-      cc.regular = 0;
-      cc.e_off = e_off;
-      cc.n_off = n_off;
-      cc.f_off = f_off;
-      cc.comp_index = k;
-      cc.ell_off = ell_off;
-      cc.s_off = s_off;
-      ell_off += pl->large_ell[i];
-      s_off += (nc + 31) / 32 + 1;
-      g.max_free = std::max(g.max_free, pl->large_free[i]);
-      pl->L_max_free = std::max(pl->L_max_free, pl->large_free[i]);
-      e_off += pl->large_cand[i];
-      n_off += nc;
-      f_off += pl->large_free[i];
-      ++k;
+    for (const Acc& A : acc)
+      for (size_t i = 0; i < A.large_slots.size(); ++i) {
+        if (class_of(A.large_free[i]) != cls) continue;
+        pl->large_slots.push_back(A.large_slots[i]);
+        pl->large_cand.push_back(A.large_cand[i]);
+        pl->large_free.push_back(A.large_free[i]);
+        pl->large_ell.push_back(A.large_ell[i]);
+        g.max_free = std::max(g.max_free, A.large_free[i]);
+      }
+    g.n = (uint32_t)pl->large_slots.size() - g.offset;
+    if (!g.n) continue;
+    // the first `smem_vecs` of p, w, r, z, y (2 doubles per free node each) and the preconditioner (3)
+    const int per_node = std::min(g.smem_vecs, 5) * 2 + (g.smem_vecs >= 6 ? 3 : 0);
+    g.bytes = (int)std::min<uint64_t>(info(g.kernel).smem_max, (uint64_t)g.max_free * per_node * sizeof(double));
+    pl->launches.push_back(g);
+  }
+  // The other routes, per (route, shared-memory class) key: one launch over the union of the members'
+  // maxima or, where that overflows, one per member.  The register classes' members of four-warp
+  // launches go to the queue instead where one of them has more than 16 unknowns: without one the
+  // per-bucket kernels run 12 warps per SM at 168 registers, which the queue kernel (255 registers for
+  // all four NREG paths) cannot (DESIGN §4).
+  int bytes[kKeys];
+  uint32_t four[kKeys];  // members in four-warp launches
+  bool wide = false;
+  for (int key = 0; key < kKeys; ++key) {
+    const int r = key / n_class;
+    bytes[key] = count[key] ? layout_bytes(r, caps[key].e, caps[key].nc, caps[key].n2) : 0;
+    four[key] = bytes[key] > kMaxSmemPerBlock ? fit4[key] : (fits_four(bytes[key]) ? count[key] : 0);
+    wide = wide || ((r == kReg24 || r == kReg32) && four[key]);
+  }
+  auto queued = [&](int key) { return wide && key / n_class <= kReg32 ? four[key] : 0u; };
+  auto slot_of = [&](int key, uint32_t c) {  // a member's slot: its bucket's, or its own where that overflows
+    return bytes[key] <= kMaxSmemPerBlock ? bytes[key] : layout_bytes(key / n_class, dim[c].e, dim[c].nc, dim[c].n2);
+  };
+  // the bucket lists: largest shared-memory class first, within a class the last route first, ascending
+  // slot index inside a bucket; the queue's members in ascending slot index
+  uint32_t start[kKeys], total = 0;
+  for (int k = n_class - 1; k >= 0; --k)
+    for (int r = kRoutes - 1; r >= 0; --r) {
+      start[r * n_class + k] = total;
+      total += count[r * n_class + k] - queued(r * n_class + k);
     }
-    g.n = k - g.first;
-    if (g.n) pl->cta_groups.push_back(g);
+  pl->list_host.resize(total);
+  std::vector<uint32_t>& q = pl->w2_slots;
+  q.clear();
+  {
+    uint32_t fill[kKeys];
+    std::memcpy(fill, start, sizeof(fill));
+    uint32_t* list = pl->list_host.data();
+    for (uint32_t c = 0; c < C; ++c) {
+      const int key = key_of[c];
+      if (key == kNoKey) continue;
+      if (wide && key / n_class <= kReg32 && fits_four(slot_of(key, c)))
+        q.push_back(c);
+      else
+        list[fill[key]++] = c;
+    }
+  }
+  // The queue (solve_warp2_queue_kernel), each entry {slot, own layout sizes}: one launch takes every
+  // member whose own layout fits a slot at W warps per SM; the rest (if any) go to a second at as many
+  // warps as its largest member allows (>= 4: they fit four to a CTA).
+  if (!q.empty()) {
+    const int ww = (dbg >> LFR_DBG_WARP2_WARPS_SHIFT) & 0xf;
+    const int W = ww ? std::min(ww, lfr::kWarp2QueueMaxWarps) : kWarp2QueueWarpsDefault;
+    const int cap = (kMaxSmemPerBlock / W) & ~15;
+    for (int pass = 0; pass < 2; ++pass) {
+      Launch g;
+      g.kernel = Kernel::kQueue;
+      g.offset = (uint32_t)pl->list_host.size();
+      for (uint32_t c : q) {
+        const int b = lfr::RegLayout(dim[c].e, dim[c].nc, dim[c].n2, 32).total;
+        if ((b <= cap) != (pass == 0)) continue;
+        pl->list_host.push_back(c);
+        pl->list_host.push_back(lfr::warp2_queue_dims(dim[c].e, dim[c].nc, dim[c].n2));
+        g.bytes = std::max(g.bytes, b);
+        ++g.n;
+      }
+      if (!g.n) continue;
+      g.warps = pass == 0 ? W : std::min(W, kMaxSmemPerBlock / g.bytes);
+      pl->launches.push_back(g);
+    }
+  }
+  auto emit = [&](int r, const lfr_plan::SchedDim& d, int b, uint32_t offset, uint32_t n) {
+    Launch L;
+    L.kernel = fits_four(b) ? kFour[r] : kOne[r];
+    L.offset = offset;
+    L.n = n;
+    L.emax = d.e;
+    L.ncmax = d.nc;
+    L.n2max = d.n2;
+    L.bytes = b;
+    L.warps = info(L.kernel).per_cta;
+    pl->launches.push_back(L);
+  };
+  for (int k = n_class - 1; k >= 0; --k)
+    for (int r = kRoutes - 1; r >= 0; --r) {
+      const int key = r * n_class + k;
+      const uint32_t n = count[key] - queued(key);
+      if (!n) continue;
+      if (bytes[key] <= kMaxSmemPerBlock) {
+        emit(r, caps[key], bytes[key], start[key], n);
+      } else {  // every member fits on its own but the union of their maxima does not: one launch each
+        for (uint32_t i = 0; i < n; ++i) {
+          const uint32_t c = pl->list_host[start[key] + i];
+          emit(r, dim[c], slot_of(key, c), start[key] + i, 1);
+        }
+      }
+    }
+  return LFR_OK;
+}
+
+// CTA-tier components: the host only lays out per-component offsets (upper bounds: candidate edges
+// from row_ptr, non-root nodes), in the order of the schedule's CTA launches, and sizes the HBM arrays;
+// the kept-edge / in-edge lists, free-variable numbering and twins are built on the device by
+// cta_prepare_kernel (launched by fill_plan once the edge records and local_of are in HBM).
+int prepare_large(lfr_plan* pl, const lfr_problem* p, cudaStream_t s) {
+  pl->n_large = (uint32_t)pl->large_slots.size();
+  pl->L_total_free = 0;
+  if (pl->n_large == 0) return LFR_OK;
+  std::vector<lfr::CtaComp>& comps = pl->L_comps_host;  // plan member: the async upload reads it
+  comps.assign(pl->n_large, lfr::CtaComp{});
+  uint64_t e_off = 0, n_off = 0, f_off = 0, ell_off = 0, s_off = 0;
+  for (uint32_t k = 0; k < pl->n_large; ++k) {
+    const uint32_t c = pl->large_slots[k];
+    const uint32_t nc = p->comp_ptr[c + 1] - p->comp_ptr[c];
+    if (pl->large_cand[k] > 0xffffffffull) return fail(LFR_EUNSUPPORTED, "component with more than 2^32 out-edges");
+    lfr::CtaComp& cc = comps[k];
+    cc.slot = c;
+    cc.Nc = nc;
+    cc.Ec = 0;  // filled on the device, with nf and regular
+    cc.nf = 0;
+    cc.regular = 0;
+    cc.e_off = e_off;
+    cc.n_off = n_off;
+    cc.f_off = f_off;
+    cc.comp_index = k;
+    cc.ell_off = ell_off;
+    cc.s_off = s_off;
+    ell_off += pl->large_ell[k];
+    s_off += (nc + 31) / 32 + 1;
+    e_off += pl->large_cand[k];
+    n_off += nc;
+    f_off += pl->large_free[k];
   }
   pl->L_total_free = f_off;
   const uint64_t E1 = std::max<uint64_t>(e_off, 1), N1 = std::max<uint64_t>(n_off, 1), F1 = std::max<uint64_t>(f_off, 1);
@@ -770,8 +817,13 @@ int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const do
     pl->pos_is_staged = false;
   }
   host_mark(0);
-  LFR_TRY(build_buckets(pl, p));  // host work overlaps the copies above
+  LFR_TRY(build_schedule(pl, p));  // host work overlaps the copies above
   host_mark(1);
+  bool needs_hbm_edges = false, has_queue = false;
+  for (const Launch& L : pl->launches) {
+    needs_hbm_edges = needs_hbm_edges || info(L.kernel).edges == Edges::kGlobal;
+    has_queue = has_queue || L.kernel == Kernel::kQueue;
+  }
   // Zero-copy and the CTA tier: its preparation kernel can pull the records it keeps straight from the
   // pinned array, but SM loads over PCIe are slower than the copy engine, so that pays only while
   // those components hold less than ~0.3 of the edges
@@ -779,7 +831,7 @@ int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const do
   uint64_t cta_cand = 0;
   for (uint64_t e : pl->large_cand) cta_cand += e;
   pl->cta_from_hbm = zc_edges && 10 * cta_cand > 3 * (uint64_t)p->n_edges;
-  if (zc_edges && (pl->needs_hbm_edges || pl->cta_from_hbm)) {
+  if (zc_edges && (needs_hbm_edges || pl->cta_from_hbm)) {
     // mixed schedule: the Cholesky-warp tier reads edge records from global memory by index, so the
     // array goes to HBM after all — on its own stream, and only that tier waits for it
     if (!pl->copy_stream) LFR_CUDA(cudaStreamCreateWithFlags(&pl->copy_stream, cudaStreamNonBlocking));
@@ -817,12 +869,12 @@ int fill_plan(lfr_plan* pl, const lfr_problem* p, const lfr_options& o, const do
     if (ps != s) LFR_CUDA(cudaEventRecord(pl->ev_edges, pl->copy_stream));
   }
   // streams for concurrent bucket launches
-  if (!pl->w2_groups.empty() && !pl->queue_ctr.p) {
+  if (has_queue && !pl->queue_ctr.p) {
     // zero once: every queue launch leaves its two words at zero when it ends
     LFR_TRY(pl->queue_ctr.reserve(2 * sizeof(uint32_t) * 2));
     LFR_CUDA(cudaMemsetAsync(pl->queue_ctr.p, 0, pl->queue_ctr.cap, s));
   }
-  if (!pl->w2_groups.empty() && !pl->n_sms) LFR_CUDA(cudaDeviceGetAttribute(&pl->n_sms, cudaDevAttrMultiProcessorCount, pl->device));
+  if (has_queue && !pl->n_sms) LFR_CUDA(cudaDeviceGetAttribute(&pl->n_sms, cudaDevAttrMultiProcessorCount, pl->device));
   const int want = std::min<int>(kMaxStreams, std::max<int>(0, pl->num_launches() - 1));
   if (!pl->ev_fork) LFR_CUDA(cudaEventCreateWithFlags(&pl->ev_fork, cudaEventDisableTiming));
   while (pl->n_streams < want) {
@@ -1545,29 +1597,8 @@ int set_kernel_attrs() {
   int dev = 0;
   LFR_CUDA(cudaGetDevice(&dev));
   if (dev >= 0 && dev < 16 && done_for_device[dev]) return LFR_OK;
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_cta_kernel<256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_cta_kernel<256, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_cta_kernel<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_kernel<4, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_kernel<4, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_queue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_warp2_kernel<1, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_tile_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_tile_kernel<64, 48>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_tile_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
-  LFR_CUDA(cudaFuncSetAttribute(lfr::solve_tile_kernel<128, 80>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kMaxSmemPerBlock));
+  for (const KernelInfo& k : kKernels)
+    LFR_CUDA(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem_max));
   if (dev >= 0 && dev < 16) done_for_device[dev] = true;
   return LFR_OK;
 }
@@ -1584,94 +1615,51 @@ int launch_solve(lfr_plan* pl, cudaStream_t s) {
     P_stage.edges = pl->zc_edges;
     P_stage.pull_window = zero_copy_pull_window();
   }
-  const bool hbm_edges_on_copy_stream = pl->zc_edges && pl->edges_in_hbm;
-  const int nb = (int)pl->buckets.size();
-  const int n_cta_launches = pl->n_large ? (int)pl->cta_groups.size() : 0;
-  const int n_side = std::max(0, nb + (int)pl->w2_groups.size() + n_cta_launches - 1);
-  if (n_side > 0) LFR_CUDA(cudaEventRecord(pl->ev_fork, s));
-  int side = 0;
-  if (pl->n_large) {  // the CTA tier first: its components are the longest
-    const lfr::CtaArrays A = pl->cta_arrays();
-    for (const CtaGroup& g : pl->cta_groups) {
-      cudaStream_t bs = s;
-      if (n_side > 0) {
-        bs = pl->streams[side++ % pl->n_streams];
-        LFR_CUDA(cudaStreamWaitEvent(bs, pl->ev_fork, 0));
-      }
-      if (pl->zc_edges && pl->cta_from_hbm) LFR_CUDA(cudaStreamWaitEvent(bs, pl->ev_edges, 0));
-      // dynamic shared memory for the CG vectors of the group's largest component: the first
-      // `smem_vecs` of p, w, r, z, y (2 doubles per free node each) and the preconditioner (3)
-      const size_t per_node = (size_t)std::min(g.smem_vecs, 5) * 2 + (g.smem_vecs >= 6 ? 3 : 0);
-      const size_t cg_bytes = std::min<size_t>(200 * 1024, (size_t)g.max_free * per_node * sizeof(double));
-      const lfr::CtaComp* comps = pl->L_comps.as<lfr::CtaComp>() + g.first;
-      const unsigned smem_doubles = (unsigned)(cg_bytes / sizeof(double));
-      if (g.minb >= 4)
-        lfr::solve_cta_kernel<256, 4><<<g.n, 256, cg_bytes, bs>>>(P_hbm, pl->K, A, comps, smem_doubles);
-      else if (g.minb == 3)
-        lfr::solve_cta_kernel<256, 3><<<g.n, 256, cg_bytes, bs>>>(P_hbm, pl->K, A, comps, smem_doubles);
-      else
-        lfr::solve_cta_kernel<256, 2><<<g.n, 256, cg_bytes, bs>>>(P_hbm, pl->K, A, comps, smem_doubles);
-      LFR_CUDA(cudaGetLastError());
+  const lfr::CtaArrays A = pl->cta_arrays();
+  // The CTA tier's launches (its components are the longest) on side streams forked from the caller's,
+  // the first other launch on the caller's stream, the rest on side streams; one launch alone runs on
+  // the caller's stream.
+  const bool fork = pl->launches.size() > 1;
+  if (fork) LFR_CUDA(cudaEventRecord(pl->ev_fork, s));
+  int side = 0, n_queue = 0;
+  bool caller_busy = false;
+  for (const Launch& L : pl->launches) {
+    const KernelInfo& I = info(L.kernel);
+    cudaStream_t bs = s;
+    if (fork && (is_cta(L.kernel) || caller_busy)) {
+      bs = pl->streams[side++ % pl->n_streams];
+      LFR_CUDA(cudaStreamWaitEvent(bs, pl->ev_fork, 0));
     }
-  }
-  // the first queue launch (or, without one, bucket 0) runs on the caller's stream, the others on side
-  // streams forked from it
-  bool on_caller = true;
-  auto next_stream = [&](cudaStream_t* bs) -> int {
-    *bs = s;
-    if (!on_caller) {
-      *bs = pl->streams[side++ % pl->n_streams];
-      LFR_CUDA(cudaStreamWaitEvent(*bs, pl->ev_fork, 0));
+    caller_busy = caller_busy || !is_cta(L.kernel);
+    // with zero-copy edges, the HBM copy and the CTA tier's preparation on the copy stream (fill_plan)
+    if (pl->zc_edges && (I.edges == Edges::kGlobal ? pl->edges_in_hbm : I.edges == Edges::kPrepared && pl->cta_from_hbm))
+      LFR_CUDA(cudaStreamWaitEvent(bs, pl->ev_edges, 0));
+    const lfr::DevProblem& P = I.edges == Edges::kStaged ? P_stage : P_hbm;
+    const unsigned grid = (L.n + L.warps - 1) / L.warps, block = I.threads * L.warps;
+    const size_t smem = (size_t)L.bytes * L.warps;
+    const lfr::WarpBucket wb{pl->lists.as<uint32_t>() + L.offset, L.n, L.emax, L.ncmax, L.n2max, L.bytes};
+    const lfr::Warp2Queue q{wb.list, L.n, L.bytes, pl->queue_ctr.as<uint32_t>() + 2 * n_queue};
+    const lfr::CtaComp* comps = is_cta(L.kernel) ? pl->L_comps.as<lfr::CtaComp>() + L.offset : nullptr;
+    const unsigned smem_doubles = (unsigned)(smem / sizeof(double));
+    switch (L.kernel) {
+      case Kernel::kWarp2x4_8: lfr::solve_warp2_kernel<4, 8><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kWarp2x4_16: lfr::solve_warp2_kernel<4, 16><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kWarp2x1_32: lfr::solve_warp2_kernel<1, 32><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kQueue:  // one CTA per SM
+        lfr::solve_warp2_queue_kernel<<<pl->n_sms, block, smem, bs>>>(P, pl->K, q);
+        ++n_queue;
+        break;
+      case Kernel::kTile64x32: lfr::solve_tile_kernel<64, 32><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kTile64x48: lfr::solve_tile_kernel<64, 48><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kTile64x64: lfr::solve_tile_kernel<64, 64><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kTile128x80: lfr::solve_tile_kernel<128, 80><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kWarp4: lfr::solve_warp_kernel<4><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kWarp1: lfr::solve_warp_kernel<1><<<grid, block, smem, bs>>>(P, pl->K, wb); break;
+      case Kernel::kCta2: lfr::solve_cta_kernel<256, 2><<<grid, block, smem, bs>>>(P, pl->K, A, comps, smem_doubles); break;
+      case Kernel::kCta3: lfr::solve_cta_kernel<256, 3><<<grid, block, smem, bs>>>(P, pl->K, A, comps, smem_doubles); break;
+      case Kernel::kCta4: lfr::solve_cta_kernel<256, 4><<<grid, block, smem, bs>>>(P, pl->K, A, comps, smem_doubles); break;
+      case Kernel::kCount: break;  // (not a kernel)
     }
-    on_caller = false;
-    return LFR_OK;
-  };
-  for (size_t i = 0; i < pl->w2_groups.size(); ++i) {
-    const Warp2Group& g = pl->w2_groups[i];
-    cudaStream_t bs;
-    LFR_TRY(next_stream(&bs));
-    lfr::Warp2Queue q;
-    q.list = pl->lists.as<uint32_t>() + g.offset;
-    q.n = g.n;
-    q.slot_bytes = g.slot_bytes;
-    q.ctr = pl->queue_ctr.as<uint32_t>() + 2 * i;
-    const size_t smem = (size_t)g.slot_bytes * g.warps;
-    lfr::solve_warp2_queue_kernel<<<pl->n_sms, 32 * g.warps, smem, bs>>>(P_stage, pl->K, q);
-    LFR_CUDA(cudaGetLastError());
-  }
-  for (int i = 0; i < nb; ++i) {
-    const Bucket& b = pl->buckets[i];
-    cudaStream_t bs;
-    LFR_TRY(next_stream(&bs));
-    lfr::WarpBucket wb;
-    wb.list = pl->lists.as<uint32_t>() + b.offset;
-    wb.n = b.n;
-    wb.emax = b.emax;
-    wb.ncmax = b.ncmax;
-    wb.n2max = b.n2max;
-    wb.smem_per_warp = b.smem_per_warp;
-    const size_t smem = (size_t)b.smem_per_warp * b.warps;
-    const unsigned grid = (b.n + b.warps - 1) / b.warps;
-    const lfr::DevProblem& P = b.stages_edges() ? P_stage : P_hbm;
-    if (!b.stages_edges() && hbm_edges_on_copy_stream) LFR_CUDA(cudaStreamWaitEvent(bs, pl->ev_edges, 0));
-    if (b.variant == 132)
-      lfr::solve_tile_kernel<64, 32><<<b.n, 64, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 48)
-      lfr::solve_tile_kernel<64, 48><<<b.n, 64, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 64)
-      lfr::solve_tile_kernel<64, 64><<<b.n, 64, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 80)
-      lfr::solve_tile_kernel<128, 80><<<b.n, 128, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 8)  // (four-warp register buckets of a plan without a queue launch)
-      lfr::solve_warp2_kernel<4, 8><<<grid, 128, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 16)
-      lfr::solve_warp2_kernel<4, 16><<<grid, 128, smem, bs>>>(P, pl->K, wb);
-    else if (b.variant == 32 && b.warps == 1)
-      lfr::solve_warp2_kernel<1, 32><<<grid, 32, smem, bs>>>(P, pl->K, wb);
-    else if (b.warps == 4)
-      lfr::solve_warp_kernel<4><<<grid, 128, smem, bs>>>(P, pl->K, wb);
-    else
-      lfr::solve_warp_kernel<1><<<grid, 32, smem, bs>>>(P, pl->K, wb);
     LFR_CUDA(cudaGetLastError());
   }
   for (int k = 0; k < std::min(side, pl->n_streams); ++k) {  // join the side streams
@@ -2140,7 +2128,7 @@ int lfr_debug_last_solve_profile(int device, unsigned long long* cycles, unsigne
   return LFR_OK;
 }
 
-// host-only: best-of-`reps` time of the schedule construction (build_buckets), no device needed
+// host-only: best-of-`reps` time of the schedule construction (build_schedule), no device needed
 int lfr_debug_time_schedule(const lfr_problem* p, const lfr_options* opt, int reps, double* best_us, int* n_launches,
                             uint64_t* digest) {
   if (!p || !best_us) return fail(LFR_EINVAL, "null argument");
@@ -2153,34 +2141,22 @@ int lfr_debug_time_schedule(const lfr_problem* p, const lfr_options* opt, int re
   double best = 1e300;
   for (int r = 0; r < std::max(reps, 1); ++r) {
     const auto t0 = std::chrono::steady_clock::now();
-    LFR_TRY(build_buckets(&pl, p));
+    LFR_TRY(build_schedule(&pl, p));
     best = std::min(best, std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count());
   }
-  if (std::getenv("LFR_SCHED_SPLIT")) {  // diagnostic: the node loop alone
-    double b2 = 1e300;
-    uint64_t sink = 0;
-    for (int r = 0; r < std::max(reps, 1); ++r) {
-      const auto t0 = std::chrono::steady_clock::now();
-      for (uint32_t c = 0; c < p->n_components; ++c) {
-        uint64_t eup = 0; uint32_t nfree = 0;
-        for (uint32_t i = p->comp_ptr[c]; i < p->comp_ptr[c + 1]; ++i) {
-          const uint32_t v = p->comp_nodes[i];
-          eup += p->row_ptr[v + 1] - p->row_ptr[v];
-          nfree += p->is_root[v] ? 0 : 1;
-        }
-        sink += eup * 3 + nfree;
-      }
-      b2 = std::min(b2, std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count());
-    }
-    std::fprintf(stderr, "node loop alone %.1f us (sink %llu)\n", b2, (unsigned long long)sink);
-  }
-  if (std::getenv("LFR_SCHED_DUMP")) {
-    for (const Bucket& b : pl.buckets)
-      std::fprintf(stderr, "bucket variant %3d  n %6u  emax %5d ncmax %4d n2max %3d  smem/warp %6d  warps %d  -> CTAs/SM by smem %d\n", b.variant,
-                   b.n, b.emax, b.ncmax, b.n2max, b.smem_per_warp, b.warps, (int)(kMaxSmemPerBlock / (b.smem_per_warp * b.warps + 1024)));
-    for (const Warp2Group& g : pl.w2_groups)
-      std::fprintf(stderr, "warp2 queue  n %6u  slot %6d  warps/SM %d\n", g.n, g.slot_bytes, g.warps);
+  if (std::getenv("LFR_SCHED_DUMP")) {  // the bucket launches, the queue launches, then the CTA tier
+    for (const Launch& L : pl.launches)
+      if (L.kernel != Kernel::kQueue && !is_cta(L.kernel))
+        std::fprintf(stderr, "bucket variant %3d  n %6u  emax %5d ncmax %4d n2max %3d  smem/warp %6d  warps %d  -> CTAs/SM by smem %d\n",
+                     info(L.kernel).label, L.n, L.emax, L.ncmax, L.n2max, L.bytes, L.warps,
+                     (int)(kMaxSmemPerBlock / (L.bytes * L.warps + 1024)));
+    for (const Launch& L : pl.launches)
+      if (L.kernel == Kernel::kQueue) std::fprintf(stderr, "warp2 queue  n %6u  slot %6d  warps/SM %d\n", L.n, L.bytes, L.warps);
     std::fprintf(stderr, "CTA tier: %zu components\n", pl.large_slots.size());
+    for (const Launch& L : pl.launches)
+      if (is_cta(L.kernel))
+        std::fprintf(stderr, "cta group  n %6u  max_free %6u  minb %d  smem_vecs %d  smem %6d\n", L.n, L.max_free,
+                     info(L.kernel).label, L.smem_vecs, L.bytes);
   }
   if (digest) {  // FNV-1a over everything the launches depend on: the schedule must not depend on the thread count
     uint64_t h = 1469598103934665603ull;
@@ -2191,12 +2167,9 @@ int lfr_debug_time_schedule(const lfr_problem* p, const lfr_options* opt, int re
       }
     };
     mix(pl.n_solved);
-    for (const Bucket& b : pl.buckets) {
-      mix(b.offset); mix(b.n); mix((uint64_t)b.emax); mix((uint64_t)b.ncmax); mix((uint64_t)b.n2max);
-      mix((uint64_t)b.smem_per_warp); mix((uint64_t)b.warps); mix((uint64_t)b.variant);
-    }
-    for (const Warp2Group& g : pl.w2_groups) {
-      mix(g.offset); mix(g.n); mix((uint64_t)g.slot_bytes); mix((uint64_t)g.warps);
+    for (const Launch& L : pl.launches) {
+      mix((uint64_t)L.kernel); mix(L.offset); mix(L.n); mix((uint64_t)L.emax); mix((uint64_t)L.ncmax);
+      mix((uint64_t)L.n2max); mix((uint64_t)L.bytes); mix((uint64_t)L.warps); mix(L.max_free); mix((uint64_t)L.smem_vecs);
     }
     for (uint32_t c : pl.list_host) mix(c);
     for (size_t i = 0; i < pl.large_slots.size(); ++i) {
@@ -2205,7 +2178,7 @@ int lfr_debug_time_schedule(const lfr_problem* p, const lfr_options* opt, int re
     *digest = h;
   }
   *best_us = best;
-  if (n_launches) *n_launches = (int)pl.buckets.size() + (int)pl.w2_groups.size() + (pl.large_slots.empty() ? 0 : 1);  // (CTA tier counted once here)
+  if (n_launches) *n_launches = pl.num_launches();
   return LFR_OK;
 }
 

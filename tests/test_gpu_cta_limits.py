@@ -29,7 +29,7 @@ import pytest
 TOL_UNITS = 1e-4 / 16.0   # 1e-4 px, 1 solver unit = 16 px
 ROWS_CACHED = 4 * 256     # kCtaRowsCached x threads of solve_cta_kernel: rows beyond take the uncached loop
 MAX_CTA_NODES = 16383     # 14-bit local indices (lfr_capi.cu, to_cta_tier)
-CLASS_MAX_FREE = (0xFFFFFFFF, 1008, 504, 250)   # prepare_large's kClassMaxFree
+CLASS_MAX_FREE = (0xFFFFFFFF, 1008, 504, 250)   # build_schedule's kClassMaxFree
 SMEM_VEC_DOUBLES = 200 * 1024 // 8               # CG-vector shared memory of one CTA, in doubles
 # free-node local indices around the cached rows, the warp tiers' 12-bit limit and the 13th bit
 EDGE_INDICES = (0, 1, 255, 256, 1023, 1024, 1025, 2047, 2048, 4095, 4096, 8191, 8192)
@@ -54,7 +54,7 @@ def non_roots(p):
 
 
 def class_of(nfree):
-    """prepare_large's size class (lfr_capi.cu): 0 = more than 1008 free nodes, `<256, 2>`."""
+    """build_schedule's size class (lfr_capi.cu): 0 = more than 1008 free nodes, `<256, 2>`."""
     return 0 if nfree > CLASS_MAX_FREE[1] else (1 if nfree > CLASS_MAX_FREE[2] else (2 if nfree > CLASS_MAX_FREE[3] else 3))
 
 
@@ -380,7 +380,7 @@ def test_natural_components_take_the_cta_tier(b200, natural):
                                        ("LFR_CTA_SMEM_VECS", "3,3,3,3"), ("LFR_CTA_MINB", "4,4,4,4"),
                                        ("LFR_CTA_MINB", "2,2,2,2")])
 def test_cg_vector_placement_and_minb_are_bitwise_neutral(b200, natural, monkeypatch, var, value):
-    """prepare_large's tuning hooks, read on every call: CG vectors all in HBM (0), all but the
+    """build_schedule's tuning hooks, read on every call: CG vectors all in HBM (0), all but the
     preconditioner in shared memory (5: the layout of a component with more than 1969 free nodes, whose
     13 doubles per free node exceed 200 KB), p, w, r only (3); every size class through `<256, 4>` or
     `<256, 2>`.  Same operations at other addresses / register budgets: bitwise the default solve, on

@@ -334,8 +334,9 @@ def plan_solve(b200, p, dbg=0, times=1):
 
 def test_plan_solved_back_to_back_and_launch_counts(b200, capfd, monkeypatch, cfg2, cfg4s):
     """One plan solved three times with no download between (the ticket reset by the last warp of each
-    launch) is bitwise its first solve; lfr_stats.n_kernel_launches = Plan.num_launches() = the dump's."""
-    for name, p in (("cfg4s", cfg4s), ("cfg2", cfg2)):
+    launch) is bitwise its first solve; lfr_stats.n_kernel_launches = Plan.num_launches() = the dump's.
+    cfg5 x 0.05 adds the CTA tier, one launch per size class."""
+    for name, p in (("cfg4s", cfg4s), ("cfg2", cfg2), ("cfg5s", get_problem("cfg5", 0.05)[1])):
         plan = Plan(b200, p)
         try:
             plan.solve()

@@ -19,7 +19,7 @@ MAX_WARPS = 8          # kWarp2QueueMaxWarps (lfr_solve_warp2.cuh)
 
 
 def cap_of(w):
-    """The queue's first-launch slot cap at `w` warps per SM (build_buckets)."""
+    """The queue's first-launch slot cap at `w` warps per SM (build_schedule)."""
     return (SMEM // w) & ~15
 
 
@@ -70,6 +70,8 @@ def schedule_of(b200, capfd, monkeypatch, p, dbg=0):
     keys = ("variant", "n", "emax", "ncmax", "n2max", "smem", "warps")
     buckets = [dict(zip(keys, map(int, m))) for m in re.findall(
         r"bucket variant\s+(\d+)\s+n\s+(\d+)\s+emax\s+(\d+)\s+ncmax\s+(\d+)\s+n2max\s+(\d+)\s+smem/warp\s+(\d+)\s+warps (\d+)", err)]
+    # every launch has its line: the buckets, the queue launches and the CTA tier's size classes
+    assert nl.value == len(buckets) + len(queues) + len(re.findall(r"^cta group ", err, re.M)), err
     return nl.value, queues, buckets
 
 
@@ -81,7 +83,7 @@ def schedule(b200, capfd, monkeypatch, name, warps=0):
 
 
 def expected_queues(needs, n2s, w):
-    """The queue launches build_buckets makes of four-warp register-tier members with layouts `needs`
+    """The queue launches build_schedule makes of four-warp register-tier members with layouts `needs`
     and unknowns `n2s` at `w` warps per SM (None: no member above 16 unknowns, no queue)."""
     if max(n2s) <= 16:
         return []
@@ -176,6 +178,13 @@ def cfg4s():
     """cfg4 at a tenth of its keypoints: 199 queue members, two queue launches at 8 warps per SM."""
     from conftest import get_problem
     return get_problem("cfg4", 0.1)[1]
+
+
+@pytest.fixture(scope="module")
+def cfg5s():
+    """cfg5 at a twentieth of its keypoints: CTA-tier components in three size classes."""
+    from conftest import get_problem
+    return get_problem("cfg5", 0.05)[1]
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -318,10 +327,11 @@ def test_one_wide_member_moves_the_four_warp_buckets_into_the_queue(b200, capfd,
     assert sum(b["n"] for b in buckets if b["variant"] in (8, 16)) == int(((n2 <= 16) & (sizes_of(cfg2) >= 2)).sum())
 
 
-@pytest.mark.parametrize("scene", ["cfg2", "cfg4s"])
+@pytest.mark.parametrize("scene", ["cfg2", "cfg4s", "cfg5s"])
 def test_dispatch_order_does_not_change_the_groups(b200, capfd, monkeypatch, request, scene):
     """The ABI takes comp_ptr in any order: reversed, ascending-size and random dispatch orders give the
-    same queue launches (n, slot, warps) as the largest-first order, at 8, 5 and 1 warps per SM."""
+    same queue launches (n, slot, warps) as the largest-first order, at 8, 5 and 1 warps per SM.
+    cfg5 x 0.05 also has the CTA tier: one launch for each of its three size classes."""
     p = request.getfixturevalue(scene)
     sizes = sizes_of(p)
     orders = {"reversed": list(range(p.n_components))[::-1],
@@ -331,6 +341,7 @@ def test_dispatch_order_does_not_change_the_groups(b200, capfd, monkeypatch, req
         dbg = w << DBG_WARP2_WARPS_SHIFT
         ref = schedule_of(b200, capfd, monkeypatch, p, dbg)
         assert ref[1]
+        assert ref[0] - len(ref[1]) - len(ref[2]) == (3 if scene == "cfg5s" else 0)   # the CTA groups
         for name, order in orders.items():
             got = schedule_of(b200, capfd, monkeypatch, subset(p, order), dbg)
             assert got[0] == ref[0] and got[1] == ref[1], (name, w)
