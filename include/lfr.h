@@ -128,6 +128,7 @@ typedef struct lfr_options {
 #define LFR_DBG_NO_ZERO_COPY 0x8        /* lfr_solve_multi(): copy edges / positions through HBM even when the caller's buffers are pinned */
 #define LFR_DBG_PROFILE 0x10            /* per-component clock64() counters (lfr_debug_plan_cycles)            */
 #define LFR_DBG_ZERO_COPY 0x20          /* lfr_solve(): use pinned caller buffers in place, as lfr_solve_multi() does */
+#define LFR_DBG_DEVICE_CUT 0x40         /* lfr_plan_create_from_matches / _from_wire: cut oversized meta-components on the device (lfr_cut.cuh) */
 #define LFR_DBG_TILE_FROM_SHIFT 8       /* bits 8..15 = n: components with more than n unknowns (n <= 32) use the two-warp tile kernel */
 #define LFR_DBG_WARP2_WARPS_SHIFT 16    /* bits 16..19 = W (1..8): warps per SM of the warp-register tier's queue kernel; 0 = the default */
 

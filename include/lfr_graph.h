@@ -7,7 +7,9 @@
  * node interning, the CSR edge lists and their 80-byte records, the constrained Kruskal, track ids and
  * roots, the track meta-graph and its components, the dispatch list.  Every array is bitwise equal to
  * the host stage's.  Only the recursive 2-way cut of oversized meta-components runs on the host, on
- * the downloaded edges of those components (the same code as the host stage, lfr_cut.h).  The edge
+ * the downloaded edges of those components (the same code as the host stage, lfr_cut.h).  Its device
+ * twin (lfr_cut.cuh, the same groups, no host round trip) runs under LFR_DBG_DEVICE_CUT; it measured
+ * slower on an H100 on every workload up to cfg5, so it is not the default.  The edge
  * records never leave the device: the plan solves them in place (lfr_plan_solve / lfr_plan_download).
  *
  * `in->edges_out` is ignored.  `sizes` (may be NULL) receives every count lfr_host_stage_create()

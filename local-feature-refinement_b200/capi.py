@@ -23,6 +23,7 @@ LFR_OK = 0
 # lfr_options.debug_flags (include/lfr.h)
 DBG_FORCE_SMEM_CHOLESKY, DBG_NO_TILE, DBG_NO_ZERO_COPY, DBG_PROFILE = 0x1, 0x2, 0x8, 0x10
 DBG_ZERO_COPY = 0x20
+DBG_DEVICE_CUT = 0x40
 DBG_TILE_FROM_SHIFT = 8
 DBG_WARP2_WARPS_SHIFT = 16
 TERM_NAMES = {0: "skipped", 1: "gradient_tol", 2: "parameter_tol", 3: "function_tol",

@@ -15,6 +15,7 @@
 
 #include "../../include/lfr_graph.h"
 #include "lfr_cut.h"
+#include "lfr_cut.cuh"
 #include "lfr_graph.cuh"
 #include "lfr_solution.cuh"
 #include "lfr_solve_cta.cuh"
@@ -955,6 +956,165 @@ int components_on_device(uint32_t n, const uint32_t* a, const uint32_t* b, uint3
   return fetch(n_out, lp + n, 1, s);
 }
 
+// ---- the recursive cut on the device (lfr_cut.cuh) --------------------------------------------------
+// undirected edges of one recursion level, grouped by sub-problem (sub ascending)
+struct CutLists {
+  TmpBuf a, b, w, sub;
+  int reserve(size_t m) {
+    m = std::max<size_t>(m, 1);
+    LFR_TRY(a.reserve(4 * m));
+    LFR_TRY(b.reserve(4 * m));
+    LFR_TRY(w.reserve(8 * m));
+    LFR_TRY(sub.reserve(4 * m));
+    return LFR_OK;
+  }
+};
+
+struct SumLL {
+  __device__ __forceinline__ long long operator()(long long a, long long b) const { return a + b; }
+};
+
+// The edges idx[0..n) of `src` into `dst`, grouped by key (key_bits wide): the sub-problem of an edge is
+// the rank of its key.  `key` is overwritten.
+int group_cut_edges(uint32_t* key, const uint32_t* idx, uint32_t n, int key_bits, CutLists& src, CutLists& dst, uint32_t* n_sub,
+                    DevBuf& tmp, cudaStream_t s) {
+  TmpBuf k2, i2, head;
+  LFR_TRY(k2.reserve(4 * (size_t)n));
+  LFR_TRY(i2.reserve(4 * (size_t)n));
+  LFR_TRY(head.reserve(4 * (size_t)n));
+  uint32_t *kk = k2.as<uint32_t>(), *ii = i2.as<uint32_t>(), *h = head.as<uint32_t>();
+  LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceRadixSort::SortPairs(t, nb, key, kk, idx, ii, (int)n, 0, key_bits, s); }));
+  lfr::cut::heads_kernel<<<blocks_for(n), 256, 0, s>>>(kk, n, h);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::InclusiveSum(t, nb, h, key, (int)n, s); }));
+  lfr::cut::gather_edges_kernel<<<blocks_for(n), 256, 0, s>>>(ii, key, n, src.a.as<uint32_t>(), src.b.as<uint32_t>(), src.w.as<long long>(),
+                                                              dst.a.as<uint32_t>(), dst.b.as<uint32_t>(), dst.w.as<long long>(),
+                                                              dst.sub.as<uint32_t>());
+  LFR_LAUNCHED();
+  return fetch(n_sub, key + n - 1, 1, s);
+}
+
+// lfr_cut.h recursive_cut_all on the device, one launch set per recursion level.  E[0] holds the roots'
+// m edges (no self-loops) over nodes 0..n_nodes-1, grouped into n_sub roots; E[1] has room for m edges.
+// Every node of a root gets label[x] = label_base + (the lowest node of its group); *n_groups = groups.
+int recursive_cut_on_device(uint32_t n_nodes, CutLists (&E)[2], uint32_t m, uint32_t n_sub, const uint32_t* node_weight,
+                            uint64_t max_weight, uint32_t label_base, uint32_t* label, uint32_t* n_groups, DevBuf& tmp, cudaStream_t s) {
+  using namespace lfr::cut;
+  *n_groups = 0;
+  if (!m) return LFR_OK;
+  const size_t N = n_nodes, H = 2 * (size_t)m, NL = std::min(N, H);
+  TmpBuf beg, end, vol, vis, claim, side, sub_of, covered;                        // per node
+  TmpBuf hk, hk2, hw, hw2, uk, uw, nbr, head, hnode, hsub, lnode, lsub, lnode2, lsub2;  // per half-edge
+  TmpBuf order, pstart, pvol, pidx, pside;                                        // per node of the level
+  TmpBuf node_ptr, side_w, side_min, cont;                                        // per sub-problem
+  TmpBuf keep, key, iota, kidx, kkey, cnt;                                        // per edge
+  for (TmpBuf* b : {&beg, &end, &vis, &claim, &sub_of, &covered}) LFR_TRY(b->reserve(4 * N));
+  LFR_TRY(vol.reserve(8 * N));
+  LFR_TRY(side.reserve(N));
+  for (TmpBuf* b : {&hk, &hk2, &hw, &hw2, &uk, &uw}) LFR_TRY(b->reserve(8 * H));
+  for (TmpBuf* b : {&nbr, &head, &hnode, &hsub, &lnode, &lsub, &lnode2, &lsub2}) LFR_TRY(b->reserve(4 * H));
+  for (TmpBuf* b : {&order, &pstart, &pidx}) LFR_TRY(b->reserve(4 * NL));
+  LFR_TRY(pvol.reserve(8 * NL));
+  LFR_TRY(pside.reserve(NL));
+  LFR_TRY(node_ptr.reserve(4 * ((size_t)m + 1)));
+  LFR_TRY(side_w.reserve(16 * (size_t)m));
+  LFR_TRY(side_min.reserve(8 * (size_t)m));
+  LFR_TRY(cont.reserve(2 * (size_t)m));
+  for (TmpBuf* b : {&keep, &key, &iota, &kidx, &kkey}) LFR_TRY(b->reserve(4 * (size_t)m));
+  LFR_TRY(cnt.reserve(16));
+  LFR_CUDA(cudaMemsetAsync(vis.p, 0, 4 * N, s));
+  LFR_CUDA(cudaMemsetAsync(covered.p, 0, 4 * N, s));
+  LFR_CUDA(cudaMemsetAsync(cnt.p, 0, 16, s));
+  uint32_t* d_groups = cnt.as<uint32_t>();
+  uint32_t* d_count = d_groups + 1;
+  const int bits = bits_for(std::max<uint32_t>(n_nodes, 2) - 1);
+  int cur = 0;
+  for (uint32_t lvl = 0;; ++lvl) {
+    CutLists& C = E[cur];
+    half_edges_kernel<<<blocks_for(m), 256, 0, s>>>(C.a.as<uint32_t>(), C.b.as<uint32_t>(), C.w.as<long long>(), C.sub.as<uint32_t>(), m,
+                                                    bits, hk.as<unsigned long long>(), hw.as<long long>(), sub_of.as<uint32_t>());
+    LFR_LAUNCHED();
+    {
+      unsigned long long *k1 = hk.as<unsigned long long>(), *k2 = hk2.as<unsigned long long>(), *ku = uk.as<unsigned long long>();
+      long long *w1 = hw.as<long long>(), *w2 = hw2.as<long long>(), *wu = uw.as<long long>();
+      const int nh = (int)(2 * m);
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceRadixSort::SortPairs(t, nb, k1, k2, w1, w2, nh, 0, 2 * bits, s); }));
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+        return cub::DeviceReduce::ReduceByKey(t, nb, k2, ku, w2, wu, d_count, SumLL(), nh, s);
+      }));
+    }
+    rows_kernel<<<blocks_for(2 * (uint64_t)m), 256, 0, s>>>(uk.as<unsigned long long>(), d_count, 2 * m, bits, sub_of.as<uint32_t>(),
+                                                            nbr.as<uint32_t>(), beg.as<uint32_t>(), end.as<uint32_t>(), head.as<uint32_t>(),
+                                                            hnode.as<uint32_t>(), hsub.as<uint32_t>());
+    LFR_LAUNCHED();
+    uint32_t n_lev = 0;
+    {
+      uint32_t *h = head.as<uint32_t>(), *hn = hnode.as<uint32_t>(), *hs = hsub.as<uint32_t>(), *ln = lnode.as<uint32_t>(),
+               *ls = lsub.as<uint32_t>(), *c = d_count + 1;
+      const int nh = (int)(2 * m);
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, hn, h, ln, c, nh, s); }));
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, hs, h, ls, c, nh, s); }));
+      LFR_TRY(fetch(&n_lev, c, 1, s));
+      uint32_t *ln2 = lnode2.as<uint32_t>(), *ls2 = lsub2.as<uint32_t>();
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+        return cub::DeviceRadixSort::SortPairs(t, nb, ls, ls2, ln, ln2, (int)n_lev, 0, bits_for(std::max<uint32_t>(n_sub, 2) - 1), s);
+      }));
+    }
+    node_ptr_kernel<<<blocks_for(n_lev), 256, 0, s>>>(lsub2.as<uint32_t>(), n_lev, n_sub, node_ptr.as<uint32_t>());
+    LFR_LAUNCHED();
+    Level L;
+    L.nodes = lnode2.as<uint32_t>();
+    L.node_ptr = node_ptr.as<uint32_t>();
+    L.beg = beg.as<uint32_t>();
+    L.end = end.as<uint32_t>();
+    L.nbr = nbr.as<uint32_t>();
+    L.w = uw.as<long long>();
+    L.node_weight = node_weight;
+    L.vol = vol.as<long long>();
+    L.vis = vis.as<uint32_t>();
+    L.claim = claim.as<uint32_t>();
+    L.side = side.as<uint8_t>();
+    L.order = order.as<uint32_t>();
+    L.piece_start = pstart.as<uint32_t>();
+    L.pvol = pvol.as<long long>();
+    L.pidx = pidx.as<uint32_t>();
+    L.pside = pside.as<uint8_t>();
+    L.stamp = 2 * lvl + 1;
+    L.max_weight = max_weight;
+    L.side_w = side_w.as<long long>();
+    L.side_min = side_min.as<uint32_t>();
+    L.cont = cont.as<uint8_t>();
+    L.n_groups = d_groups;
+    cut_sub_kernel<<<n_sub, kThreads, 0, s>>>(L);
+    keep_edges_kernel<<<blocks_for(m), 256, 0, s>>>(C.a.as<uint32_t>(), C.b.as<uint32_t>(), C.sub.as<uint32_t>(), m, side.as<uint8_t>(),
+                                                    cont.as<uint8_t>(), lvl + 1, covered.as<uint32_t>(), keep.as<uint32_t>(),
+                                                    key.as<uint32_t>());
+    label_nodes_kernel<<<blocks_for(n_lev), 256, 0, s>>>(lnode2.as<uint32_t>(), lsub2.as<uint32_t>(), n_lev, side.as<uint8_t>(),
+                                                         cont.as<uint8_t>(), side_min.as<uint32_t>(), covered.as<uint32_t>(), lvl + 1,
+                                                         label_base, label, d_groups);
+    lfr::graph::iota_kernel<<<blocks_for(m), 256, 0, s>>>(iota.as<uint32_t>(), m);
+    LFR_LAUNCHED();
+    uint32_t m2 = 0;
+    {
+      uint32_t *fl = keep.as<uint32_t>(), *io = iota.as<uint32_t>(), *ki = kidx.as<uint32_t>(), *ky = key.as<uint32_t>(),
+               *kk = kkey.as<uint32_t>(), *c = d_count + 2;
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, io, fl, ki, c, (int)m, s); }));
+      LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, ky, fl, kk, c, (int)m, s); }));
+      LFR_TRY(fetch(&m2, c, 1, s));
+    }
+    if (!m2) break;
+    uint32_t n_sub2 = 0;
+    LFR_TRY(group_cut_edges(kkey.as<uint32_t>(), kidx.as<uint32_t>(), m2, bits_for(2 * (uint64_t)n_sub - 1), C, E[1 - cur], &n_sub2, tmp, s));
+    // every edge kept and one child per sub-problem: every sub-problem put all its nodes on one side (its
+    // pieces all have volume <= 0), and lfr_cut.h would cut it again forever
+    if (m2 == m && n_sub2 == n_sub) return fail(LFR_EINVAL, "recursive cut makes no progress (meta-edge weights <= 0)");
+    cur = 1 - cur;
+    m = m2;
+    n_sub = n_sub2;
+  }
+  return fetch(n_groups, d_groups, 1, s);
+}
+
 using Clock = std::chrono::steady_clock;
 double ms_since(Clock::time_point t0) { return std::chrono::duration<double, std::milli>(Clock::now() - t0).count(); }
 
@@ -980,7 +1140,12 @@ struct MatchArrays {
 // lfr_host_stage_create() on the device, block for block (lfr_host.cc), from the pair level of `in` and the
 // device-resident matches `d` (in->feat1 ... in->disp2 are not read): the edge records go into pl->edges,
 // the other arrays come back to pl->graph (the schedule builder is host code and reads them).
-int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl, lfr_host_sizes* S, cudaStream_t s) {
+// device_cut (LFR_DBG_DEVICE_CUT): oversized meta-components are cut on the device (lfr_cut.cuh, the same
+// groups) instead of by lfr_cut.h on host threads.  It is not the default: on an H100 80GB HBM3 at 700 W the
+// device cut was slower than the host cut on every workload from cfg2 to cfg5 (tools/gpu_graph_cut_time.py,
+// DESIGN.md §4), so no input size selects it.
+int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl, lfr_host_sizes* S, bool device_cut,
+                          cudaStream_t s) {
   using namespace lfr::graph;
   std::memset(S, 0, sizeof *S);
   auto G = std::make_unique<lfr_plan::GraphArrays>();
@@ -1313,7 +1478,7 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
   LFR_TRY(d_gc.reserve(4 * (size_t)T));
   LFR_CUDA(cudaMemcpyAsync(d_gc.p, d_cc.p, 4 * (size_t)T, cudaMemcpyDeviceToDevice, s));
   if (S->n_oversized_meta_components) {
-    // the undirected edges of the oversized components, in meta-edge order, go to the host cut
+    // the undirected edges of the oversized components, in meta-edge order, to the cut
     TmpBuf d_cflag, d_cidx, d_ncut, d_recs, d_gidx, d_gval;
     uint32_t n_cut = 0;
     LFR_TRY(d_cflag.reserve(4 * (size_t)n_meta));
@@ -1328,43 +1493,62 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
     LFR_LAUNCHED();
     LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceSelect::Flagged(t, nb, idx, fl, ci, cnt, (int)n_meta, s); }));
     LFR_TRY(fetch(&n_cut, cnt, 1, s));
-    LFR_TRY(d_recs.reserve(sizeof(CutRec) * std::max<size_t>(n_cut, 1)));
-    if (n_cut) {
-      cut_edges_gather_kernel<<<blocks_for(n_cut), 256, 0, s>>>(ci, n_cut, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(),
-                                                                d_wsum.as<double>(), d_cc.as<uint32_t>(), d_recs.as<CutRec>());
+    if (device_cut) {
+      // lfr_cut.cuh: the roots are the oversized components, the labels go straight into d_gc
+      CutLists E[2];
+      TmpBuf d_rkey, d_ridx;
+      LFR_TRY(E[0].reserve(n_cut));
+      LFR_TRY(E[1].reserve(n_cut));
+      LFR_TRY(d_rkey.reserve(4 * (size_t)n_cut));
+      LFR_TRY(d_ridx.reserve(4 * (size_t)n_cut));
+      lfr::cut::root_edges_kernel<<<blocks_for(n_cut), 256, 0, s>>>(ci, n_cut, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(), d_wsum.as<double>(),
+                                                                    d_cc.as<uint32_t>(), E[1].a.as<uint32_t>(), E[1].b.as<uint32_t>(),
+                                                                    E[1].w.as<long long>(), d_rkey.as<uint32_t>(), d_ridx.as<uint32_t>());
       LFR_LAUNCHED();
-    }
-    std::vector<CutRec> recs(n_cut);
-    std::vector<uint32_t> node_weight(T);
-    LFR_TRY(fetch(recs.data(), d_recs.p, n_cut, s));
-    LFR_TRY(fetch(node_weight.data(), d_nit.p, T, s));
-    // one edge list per oversized component, components ascending (lfr_host.cc's per_cc)
-    std::vector<uint32_t> comps;
-    for (const CutRec& r : recs) comps.push_back(r.comp);
-    std::sort(comps.begin(), comps.end());
-    comps.erase(std::unique(comps.begin(), comps.end()), comps.end());
-    std::vector<std::vector<lfr::CutEdge>> per_cc(comps.size());
-    for (const CutRec& r : recs) {
-      const size_t sl = (size_t)(std::lower_bound(comps.begin(), comps.end(), r.comp) - comps.begin());
-      per_cc[sl].push_back(lfr::CutEdge{r.a, r.b, lfr::cut_weight(r.wsum)});
-    }
-    std::vector<std::vector<uint32_t>> groups;
-    lfr::recursive_cut_all(std::move(per_cc), node_weight, S->n_images_seen, &groups);
-    std::vector<uint32_t> gidx, gval;
-    for (size_t g = 0; g < groups.size(); ++g)
-      for (uint32_t t : groups[g]) {
-        gidx.push_back(t);
-        gval.push_back(n_cc + (uint32_t)g);
+      uint32_t n_roots = 0;
+      LFR_TRY(group_cut_edges(d_rkey.as<uint32_t>(), d_ridx.as<uint32_t>(), n_cut, bits_for(std::max<uint32_t>(n_cc, 2) - 1), E[1], E[0],
+                              &n_roots, tmp, s));
+      LFR_TRY(recursive_cut_on_device(T, E, n_cut, n_roots, d_nit.as<uint32_t>(), S->n_images_seen, n_cc, d_gc.as<uint32_t>(),
+                                      &S->n_cut_groups, tmp, s));
+    } else {
+      LFR_TRY(d_recs.reserve(sizeof(CutRec) * std::max<size_t>(n_cut, 1)));
+      if (n_cut) {
+        cut_edges_gather_kernel<<<blocks_for(n_cut), 256, 0, s>>>(ci, n_cut, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(),
+                                                                  d_wsum.as<double>(), d_cc.as<uint32_t>(), d_recs.as<CutRec>());
+        LFR_LAUNCHED();
       }
-    S->n_cut_groups = (uint32_t)groups.size();
-    if (!gidx.empty()) {
-      LFR_TRY(upload(&d_gidx, gidx.data(), gidx.size(), s));
-      LFR_TRY(upload(&d_gval, gval.data(), gval.size(), s));
-      scatter_kernel<<<blocks_for(gidx.size()), 256, 0, s>>>(d_gidx.as<uint32_t>(), d_gval.as<uint32_t>(), (uint32_t)gidx.size(),
-                                                             d_gc.as<uint32_t>());
-      LFR_LAUNCHED();
+      std::vector<CutRec> recs(n_cut);
+      std::vector<uint32_t> node_weight(T);
+      LFR_TRY(fetch(recs.data(), d_recs.p, n_cut, s));
+      LFR_TRY(fetch(node_weight.data(), d_nit.p, T, s));
+      // one edge list per oversized component, components ascending (lfr_host.cc's per_cc)
+      std::vector<uint32_t> comps;
+      for (const CutRec& r : recs) comps.push_back(r.comp);
+      std::sort(comps.begin(), comps.end());
+      comps.erase(std::unique(comps.begin(), comps.end()), comps.end());
+      std::vector<std::vector<lfr::CutEdge>> per_cc(comps.size());
+      for (const CutRec& r : recs) {
+        const size_t sl = (size_t)(std::lower_bound(comps.begin(), comps.end(), r.comp) - comps.begin());
+        per_cc[sl].push_back(lfr::CutEdge{r.a, r.b, lfr::cut_weight(r.wsum)});
+      }
+      std::vector<std::vector<uint32_t>> groups;
+      lfr::recursive_cut_all(std::move(per_cc), node_weight, S->n_images_seen, &groups);
+      std::vector<uint32_t> gidx, gval;
+      for (size_t g = 0; g < groups.size(); ++g)
+        for (uint32_t t : groups[g]) {
+          gidx.push_back(t);
+          gval.push_back(n_cc + (uint32_t)g);
+        }
+      S->n_cut_groups = (uint32_t)groups.size();
+      if (!gidx.empty()) {
+        LFR_TRY(upload(&d_gidx, gidx.data(), gidx.size(), s));
+        LFR_TRY(upload(&d_gval, gval.data(), gval.size(), s));
+        scatter_kernel<<<blocks_for(gidx.size()), 256, 0, s>>>(d_gidx.as<uint32_t>(), d_gval.as<uint32_t>(), (uint32_t)gidx.size(),
+                                                               d_gc.as<uint32_t>());
+        LFR_LAUNCHED();
+      }
+      LFR_CUDA(cudaStreamSynchronize(s));  // the uploads above read host vectors that end with this scope
     }
-    LFR_CUDA(cudaStreamSynchronize(s));  // the uploads above read host vectors that end with this scope
   }
   LFR_TRY(d_fcc.reserve(4 * (size_t)T));
   LFR_TRY(components_on_device(T, d_ma.as<uint32_t>(), d_mb.as<uint32_t>(), n_meta, d_gc.as<uint32_t>(), d_fcc.as<uint32_t>(),
@@ -1567,7 +1751,7 @@ int decode_wire_on_device(const lfr_host_input* in, const lfr_wire_part* parts, 
 // The two entry points from matches: the stage on the device-resident `d`, then the plan.
 int create_plan_from_graph(const lfr_host_input* in, MatchArrays& d, const lfr_options& o, const double* initial_positions,
                            lfr_plan* pl, lfr_host_sizes* S) {
-  LFR_TRY(build_graph_on_device(in, d, pl, S, 0));
+  LFR_TRY(build_graph_on_device(in, d, pl, S, (o.debug_flags & LFR_DBG_DEVICE_CUT) != 0, 0));
   const lfr_plan::GraphArrays& G = *pl->graph;
   lfr_problem p;
   p.n_nodes = S->n_nodes;
@@ -2456,6 +2640,50 @@ int lfr_debug_ls_minimizer(const double* cases, uint64_t n, double* out) {
   };
   const int rc = run();
   d_i.release(); d_o.release();
+  return rc;
+}
+
+/* test hook: the device cut (lfr_cut.cuh) on one edge list, as graph.py::recursive_cut /
+   lfr_cut.h recursive_cut_all with it as the only root: group_of[x] = the lowest node of x's group, x
+   itself for a node no edge touches.  Edges (16 bytes: uint32 a, b, int64 w, lfr::CutEdge) must have
+   a, b < n and a != b (a self-loop never leaves an oversized node's sub-problem in lfr_cut.h). */
+typedef lfr::CutEdge lfr_cut_edge;
+int lfr_debug_recursive_cut(const lfr_cut_edge* edges, uint64_t m, const uint32_t* node_weight, uint64_t n, uint32_t max_weight,
+                            uint32_t* group_of) {
+  lfr_options o;
+  lfr_options_default(&o);
+  LFR_TRY(select_device(o));
+  if (m >= (1u << 30) || n >= (1u << 31)) return fail(LFR_EINVAL, "edge list too large");
+  for (uint64_t i = 0; i < m; ++i)
+    if (edges[i].a >= n || edges[i].b >= n || edges[i].a == edges[i].b) return fail(LFR_EINVAL, "cut edge out of range or a self-loop");
+  for (uint64_t x = 0; x < n; ++x) group_of[x] = (uint32_t)x;
+  if (m == 0) return LFR_OK;
+  std::vector<uint32_t> a(m), b(m), sub(m, 0);
+  std::vector<long long> w(m);
+  for (uint64_t i = 0; i < m; ++i) {
+    a[i] = edges[i].a;
+    b[i] = edges[i].b;
+    w[i] = edges[i].w;
+  }
+  CutLists E[2];
+  DevBuf d_nw, d_label, tmp;
+  uint32_t n_groups = 0;
+  auto run = [&]() -> int {
+    LFR_TRY(E[0].reserve(m));
+    LFR_TRY(E[1].reserve(m));
+    LFR_CUDA(cudaMemcpy(E[0].a.p, a.data(), 4 * m, cudaMemcpyHostToDevice));
+    LFR_CUDA(cudaMemcpy(E[0].b.p, b.data(), 4 * m, cudaMemcpyHostToDevice));
+    LFR_CUDA(cudaMemcpy(E[0].w.p, w.data(), 8 * m, cudaMemcpyHostToDevice));
+    LFR_CUDA(cudaMemcpy(E[0].sub.p, sub.data(), 4 * m, cudaMemcpyHostToDevice));
+    LFR_TRY(upload(&d_nw, node_weight, n, 0));
+    LFR_TRY(upload(&d_label, group_of, n, 0));
+    LFR_TRY(recursive_cut_on_device((uint32_t)n, E, (uint32_t)m, 1, d_nw.as<uint32_t>(), max_weight, 0, d_label.as<uint32_t>(), &n_groups,
+                                    tmp, 0));
+    LFR_CUDA(cudaMemcpy(group_of, d_label.p, 4 * n, cudaMemcpyDeviceToHost));
+    return LFR_OK;
+  };
+  const int rc = run();
+  d_nw.release(); d_label.release(); tmp.release();
   return rc;
 }
 

@@ -10,7 +10,8 @@
 // shim behind which the reference's own solve.cc is compiled as a checker
 // (oracle/ref_shims/colmap/base/graph_cut.h).  The recursive cut built on it (cut_step,
 // recursive_cut_all, at the end of this file) is shared by the host stage and the graph stage on the
-// GPU (lfr_capi.cu), so both split oversized meta-components with the same code.
+// GPU (lfr_capi.cu), so both split oversized meta-components with the same code; lfr_cut.cuh is its
+// level-parallel twin on the device, tested to give the same groups.
 //
 // Algorithm (all ties broken by ascending node id, so the result is unique):
 //   1. adjacency with parallel edges merged, neighbours ascending; vol(x) = sum of incident weights
@@ -31,6 +32,12 @@
 #include <utility>
 #include <vector>
 
+#ifdef __CUDACC__
+#define LFR_CUT_HD __host__ __device__
+#else
+#define LFR_CUT_HD
+#endif
+
 namespace lfr {
 
 struct CutEdge {
@@ -41,7 +48,7 @@ struct CutEdge {
 // The weight of an undirected meta-edge: static_cast<int>(100 * sum of similarities) (solve.cc:329).
 // Out of int range that cast is undefined in C++; here it saturates at INT_MIN / INT_MAX (truncation
 // toward zero inside), so the host stage and the graph stage on the GPU agree on every finite input.
-inline int64_t cut_weight(double sim_sum) {
+LFR_CUT_HD inline int64_t cut_weight(double sim_sum) {
   const double x = 100.0 * sim_sum;
   if (x >= 2147483647.0) return 2147483647;
   if (x <= -2147483648.0) return -2147483647 - 1;

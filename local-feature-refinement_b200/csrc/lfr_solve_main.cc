@@ -18,7 +18,7 @@
 //           records into page-locked memory, then lfr_solve() / lfr_solve_multi() (include/lfr.h), the
 //           output assembly and lfr_wire_encode_solution().
 // Both routes give the same bytes and lines.  LFR_GRAPH_STAGE=host|device forces a route (a test and
-// measurement hook).  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route).  `--n_threads` is accepted and
+// measurement hook); on the device route LFR_DEVICE_CUT=1 cuts oversized meta-components on the GPU too.  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -401,6 +401,10 @@ int main(int argc, char** argv) {
     lfr_options opt;
     lfr_options_default(&opt);
     opt.device = (int32_t)device;
+    // LFR_DEVICE_CUT=1: the recursive cut on the device too (LFR_DBG_DEVICE_CUT; a test and measurement hook)
+    if (const char* e = std::getenv("LFR_DEVICE_CUT")) {
+      if (std::strcmp(e, "1") == 0) opt.debug_flags |= LFR_DBG_DEVICE_CUT;
+    }
     std::vector<lfr_wire_part> wparts;
     for (const Part& pt : parts) wparts.push_back(lfr_wire_part{pt.buf.data(), pt.buf.size(), pt.match_off.data(), pt.M});
     const int rc = decode_on_device
