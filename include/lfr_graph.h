@@ -90,6 +90,29 @@ int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images
                                  const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
                                  uint64_t* n_outside);
 
+/* Hold images fixed in a plan made by lfr_plan_create_from_matches() or _from_wire(): every node of an
+ * image k with fixed_by_image_id[k] != 0 (ids of lfr_host_input, n_images at least its n_images) becomes
+ * constant, as a root is (solve.cc:135): it keeps its start value, gets no bounds, and a block between two
+ * constant nodes is dropped.  The mask (reference root OR node of a fixed image) is expanded on the device
+ * over the plan's node ids and the schedule is built again on it (free-node counts move components between
+ * tiers); lfr_plan_export_graph() still reports the reference's is_root.  A later call replaces the mask
+ * (an all-zero one solves as a plan never given one).  A plan never given a mask reads is_root as before and
+ * holds no mask buffer.  Synchronous on the legacy default stream.  LFR_EINVAL for a plan made by
+ * lfr_plan_create(), whose lfr_problem.is_root already says which nodes are constant. */
+int lfr_plan_fix_images(lfr_plan* plan, const uint8_t* fixed_by_image_id /* [n_images] */, uint32_t n_images);
+
+/* Start a plan made by lfr_plan_create_from_matches() or _from_wire() from a SolutionFile (types.proto:30-46):
+ * names / name_off are the scene's image names by id, as for lfr_plan_encode_solution().  The bytes are
+ * decoded on the host (lfr_wire_decode_solution), the entries keyed (image id << 32 | feature_idx) and
+ * joined to the plan's node ids on the device, with the rule of lfr_wire_join_solution()
+ * (include/lfr_wire.h), whose positions these are bit for bit.  Writes the plan's start and working
+ * positions (lfr_plan_download() and lfr_plan_encode_solution() see them before the next solve, which starts
+ * from them: free nodes are projected onto the box, constant nodes keep them).  *n_started (may be NULL) =
+ * the nodes with an entry.  Returns after the join, on `stream`.  LFR_EINVAL for malformed bytes (the plan is
+ * not changed) and for a plan made by lfr_plan_create(), which takes its start point at creation. */
+int lfr_plan_start_from_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                                 const uint8_t* names, const uint64_t* name_off, uint64_t* n_started);
+
 /* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
  * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from
  * sizes known before either stage runs — the directed edges (2 x the matches of the pairs not skipped),

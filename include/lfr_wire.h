@@ -83,6 +83,20 @@ int lfr_wire_decode_solution(const uint8_t* buf, uint64_t len, uint64_t* n_image
                              uint32_t* name_len, float* fact, uint32_t* feature_idx,
                              float* di, float* dj);
 
+/* Start positions of a scene's nodes from a SolutionFile, for refining against an earlier solution.
+ * The scene: image k is named names[name_off[k], name_off[k+1]) (ids as in lfr_host_input), node v is
+ * feature node_feat[v] of image node_image[v] (lfr_host_stage_export).  An Image message matches a scene
+ * image by its exact name bytes, and a displacement a node by its feature_idx; the last Image message with
+ * a given name wins as a whole and, within it, the last displacement of a feature (the rule of the
+ * reference's reader, reconstruction-scripts/colmap_utils.py:104-137).  positions[2v .. 2v+1] =
+ * ((double)di, (double)dj) of node v's entry, 0 for a node without one; entries of images or features not
+ * in the scene are ignored.  *n_started (may be NULL) = the nodes that have an entry.  LFR_EINVAL for
+ * bytes lfr_wire_decode_solution() rejects (positions untouched) or NULL arrays.  The device join of a
+ * plan (lfr_plan_start_from_solution, include/lfr_graph.h) gives the same bits. */
+int lfr_wire_join_solution(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                           const uint64_t* name_off, uint32_t n_nodes, const uint32_t* node_image,
+                           const uint32_t* node_feat, double* positions /* [2 n_nodes] */, uint64_t* n_started);
+
 #ifdef __cplusplus
 }
 #endif

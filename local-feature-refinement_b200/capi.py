@@ -80,7 +80,8 @@ ABI_SYMBOLS = [
 ]
 #: the symbols include/lfr_graph.h declares
 GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
-                 "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device"]
+                 "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
+                 "lfr_plan_fix_images", "lfr_plan_start_from_solution"]
 
 
 class LfrWirePart(C.Structure):
@@ -153,6 +154,11 @@ class Library:
             L.lfr_graph_stage_on_device.restype = C.c_int
             L.lfr_wire_decode_on_device.argtypes = [C.c_uint64]
             L.lfr_wire_decode_on_device.restype = C.c_int
+            L.lfr_plan_fix_images.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+            L.lfr_plan_fix_images.restype = C.c_int
+            L.lfr_plan_start_from_solution.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                                       C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+            L.lfr_plan_start_from_solution.restype = C.c_int
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -444,6 +450,29 @@ class Plan:
         if got != need:
             self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution")
         return out[:need].tobytes(), int(n_out.value)
+
+    def fix_images(self, fixed_by_image_id) -> None:
+        """lfr_plan_fix_images (include/lfr_graph.h): hold every node of the images with a non-zero entry of
+        `fixed_by_image_id` (indexed by image id, at least the plan's image count) constant in the next
+        solves, as a root is; replaces an earlier mask.  Plans made by from_matches() or from_wire() only."""
+        m = np.ascontiguousarray(fixed_by_image_id, dtype=bool).astype(np.uint8).reshape(-1)
+        self.lib.check(self.lib.lib.lfr_plan_fix_images(self.handle, m.ctypes.data if m.size else None, m.shape[0]),
+                       "lfr_plan_fix_images")
+
+    def start_from_solution(self, data: bytes, image_names, stream: int = 0) -> int:
+        """lfr_plan_start_from_solution (include/lfr_graph.h): the start point of the next solves from the
+        SolutionFile bytes `data` (the rule of wire.join_solution, joined on the device; `image_names` by image
+        id).  Returns the number of nodes that have an entry."""
+        from .wire import _names_blob
+        buf = np.frombuffer(data, dtype=np.uint8)
+        blob, off = _names_blob(list(image_names))
+        n = C.c_uint64()
+        self.lib.check(self.lib.lib.lfr_plan_start_from_solution(self.handle, C.c_void_p(stream),
+                                                                 buf.ctypes.data if buf.size else None, buf.size,
+                                                                 len(image_names), blob.ctypes.data, off.ctypes.data,
+                                                                 C.byref(n)),
+                       "lfr_plan_start_from_solution")
+        return int(n.value)
 
     def solve(self, stream: int = 0) -> None:
         self.lib.check(self.lib.lib.lfr_plan_solve(self.handle, C.c_void_p(stream)), "lfr_plan_solve")

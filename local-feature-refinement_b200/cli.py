@@ -9,7 +9,10 @@ command-line error, solve.cc:397-401; -1 = 255 when the input does not parse or
 the output cannot be written, solve.cc:433-436,674-677), so
 local-feature-evaluation/benchmark.py:100-104, eth/benchmark.py:108-112 and
 custom_demo.py:101-105 run unchanged.  `--n_threads` is accepted and ignored
-(the solve runs on the GPU).  Opt-in extras: --device, --gpus N (one process drives N GPUs), --stats_json.
+(the solve runs on the GPU).  Opt-in extras: --device, --gpus N (one process drives N GPUs), --stats_json,
+--fixed_images NAME (repeatable: the image's keypoints are held constant, as roots are) and
+--initial_solution FILE (start values from a SolutionFile instead of zeros): together they refine new
+images against an already-refined scene.
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -43,7 +46,8 @@ class _CliError(Exception):
 # (name, takes an argument, repeatable) — solve.cc:379-385 plus the opt-in extras
 _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file", True, False),
             ("n_threads", True, False), ("banned_images", True, True),
-            ("device", True, False), ("gpus", True, False), ("stats_json", True, False)]
+            ("device", True, False), ("gpus", True, False), ("stats_json", True, False),
+            ("fixed_images", True, True), ("initial_solution", True, False)]
 
 
 def _find_option(name):
@@ -116,7 +120,8 @@ def parse_args(argv):
         return argparse.Namespace(
             matches_file=vals["matches_file"], output_file=vals["output_file"],
             n_threads=_as_uint(vals, "n_threads", 8), banned_images=vals.get("banned_images", []),
-            device=_as_uint(vals, "device", 0), gpus=_as_uint(vals, "gpus", 1), stats_json=vals.get("stats_json"))
+            device=_as_uint(vals, "device", 0), gpus=_as_uint(vals, "gpus", 1), stats_json=vals.get("stats_json"),
+            fixed_images=vals.get("fixed_images", []), initial_solution=vals.get("initial_solution"))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -130,6 +135,21 @@ def main(argv=None) -> int:
     from .solver import GraphStageRouteError, refine
     from .capi import load_b200
     from .graph import refined_track_count
+
+    # the start solution is read and checked before any other work: its errors come before any output
+    start = None
+    if args.initial_solution is not None:
+        try:
+            with open(args.initial_solution, "rb") as fh:
+                start = fh.read()
+        except OSError:
+            sys.stderr.write("ERROR: cannot read the initial solution file '%s'\n" % args.initial_solution)
+            return 2
+        try:
+            wire.decode_solution(start)
+        except wire.ParseError:
+            sys.stderr.write("Failed to parse proto object.\n")
+            return 255
 
     rank = int(os.environ.get("RANK", "0"))
     say = (lambda s: print(s, flush=True)) if rank == 0 else (lambda s: None)
@@ -158,18 +178,20 @@ def main(argv=None) -> int:
     t_start = time.perf_counter()
     timing = {}
 
-    def solve_fn(p):
+    def solve_fn(p, positions=None):
         t1 = time.perf_counter()
         if "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1:
             from .dist import solve_distributed       # launched under torchrun: one rank per GPU
+            if positions is not None:
+                raise GraphStageRouteError("--initial_solution: torchrun ranks start from zeros; use --gpus N")
             pos, st = solve_distributed(p)
         elif args.gpus > 1:
             # one call drives the GPUs (lfr_solve_multi, include/lfr.h): components LPT-packed over the
             # devices, each pulling only its own edge records from the page-locked arrays
-            pos, st = lib.solve_multi(p, range(args.gpus), opts, pinned=True)
+            pos, st = lib.solve_multi(p, range(args.gpus), opts, positions=positions, pinned=True)
         else:
             from .solver import solve_problem
-            pos, st = solve_problem(p, opts)
+            pos, st = solve_problem(p, opts, positions)
         timing["solver_ms"] = (time.perf_counter() - t1) * 1e3
         return pos, st
 
@@ -178,7 +200,7 @@ def main(argv=None) -> int:
     n_devices = int(os.environ["WORLD_SIZE"]) if torchrun else max(args.gpus, 1)
     try:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
-                                 timing=timing)
+                                 timing=timing, fixed_images=args.fixed_images, initial_solution=start)
     except GraphStageRouteError as e:
         sys.stderr.write("ERROR: %s\n" % e)
         return 2

@@ -1,6 +1,7 @@
 """Build the in-tree libraries (git-ignored, but they travel to the GPU box):
 
-  liblfr_b200.so  the product: CUDA kernels + the C ABI of include/lfr.h      (nvcc, sm_90a; cross-compiles without a GPU)
+  liblfr_b200.so  the product: CUDA kernels + the C ABI of include/lfr.h      (nvcc, sm_90a; cross-compiles without a GPU;
+                  links liblfr_host.so for the wire codec)
   liblfr_host.so  CPU-only host utilities behind include/lfr_wire.h and include/lfr_host.h
                   (protobuf wire codec, host graph stage) — no CUDA dependency, so the
                   reference arm of bench.py and the tests can use them without mapping the product library
@@ -21,19 +22,24 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 OUT_EXE = os.path.join(ROOT, "multi-view-refinement", "build", "solve_native")
 INC = os.path.join("..", "..", "include")
 # build.py itself: a change of NVCC_FLAGS (e.g. the target architecture) must rebuild the library
-DEPS = SOURCES + ["build.py", "lfr_setup.cuh", "lfr_solve_warp.cuh", "lfr_solve_warp2.cuh", "lfr_solve_cta.cuh", "lfr_lm.cuh", "lfr_math.cuh", "lfr_graph.cuh", "lfr_wire.cuh", "lfr_solution.cuh", "lfr_cut.h", "lfr_cut.cuh",
-                  os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_graph.h"), os.path.join(INC, "lfr_host.h")]
-HOST_DEPS = HOST_SOURCES + ["lfr_cut.h", os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"),
+DEPS = SOURCES + ["build.py", "lfr_setup.cuh", "lfr_solve_warp.cuh", "lfr_solve_warp2.cuh", "lfr_solve_cta.cuh", "lfr_lm.cuh", "lfr_math.cuh", "lfr_graph.cuh", "lfr_wire.cuh", "lfr_solution.cuh", "lfr_cut.h", "lfr_cut.cuh", "lfr_join.h", "lfr_start.cuh",
+                  os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_graph.h"), os.path.join(INC, "lfr_host.h"),
+                  os.path.join(INC, "lfr_wire.h")]
+HOST_DEPS = HOST_SOURCES + ["lfr_cut.h", "lfr_join.h", os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"),
                             os.path.join(INC, "lfr_host.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-cudart", "shared"]
+# the product calls the wire codec of liblfr_host.so (the SolutionFile decode of lfr_plan_start_from_solution),
+# found next to it wherever the checkout is mounted
+HOST_LINK = ["-L" + HERE, "-llfr_host", "-Xlinker", "-rpath,$ORIGIN"]
 
 
 def build_variant(out: str, defines) -> str:
     """Diagnostic variant of the library (e.g. -DLFR_POLY_PROF) next to the product .so."""
+    build_host()
     cmd = [NVCC] + NVCC_FLAGS + ["-D" + d for d in defines] + ["-o", os.path.join(HERE, out)] + \
-          [os.path.join(HERE, s) for s in SOURCES]
+          [os.path.join(HERE, s) for s in SOURCES] + HOST_LINK
     subprocess.check_call(cmd)
     return os.path.join(HERE, out)
 
@@ -77,7 +83,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 def _build_cuda(force: bool = False, verbose: bool = False) -> str:
     if not force and not _stale(OUT, DEPS):
         return OUT
-    cmd = [NVCC] + NVCC_FLAGS + ["-o", OUT] + [os.path.join(HERE, s) for s in SOURCES]
+    cmd = [NVCC] + NVCC_FLAGS + ["-o", OUT] + [os.path.join(HERE, s) for s in SOURCES] + HOST_LINK
     if verbose:
         cmd.insert(1, "-Xptxas")
         cmd.insert(2, "-v")

@@ -18,7 +18,11 @@
 //           records into page-locked memory, then lfr_solve() / lfr_solve_multi() (include/lfr.h), the
 //           output assembly and lfr_wire_encode_solution().
 // Both routes give the same bytes and lines.  LFR_GRAPH_STAGE=host|device forces a route (a test and
-// measurement hook); on the device route LFR_DEVICE_CUT=1 cuts oversized meta-components on the GPU too.  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route).  `--n_threads` is accepted and
+// measurement hook); on the device route LFR_DEVICE_CUT=1 cuts oversized meta-components on the GPU too.  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route),
+// --fixed_images NAME (repeatable: every node of the image is held constant, as a root is) and
+// --initial_solution FILE (start values from a SolutionFile instead of zeros) — on the device route
+// lfr_plan_fix_images() / lfr_plan_start_from_solution(), on the host route the constant mask and
+// lfr_wire_join_solution() handed to the solve.  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -57,6 +61,9 @@ int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* par
 int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
                                  const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
                                  uint64_t* n_outside) __attribute__((weak));
+int lfr_plan_fix_images(lfr_plan* plan, const uint8_t* fixed_by_image_id, uint32_t n_images) __attribute__((weak));
+int lfr_plan_start_from_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                                 const uint8_t* names, const uint64_t* name_off, uint64_t* n_started) __attribute__((weak));
 }
 
 namespace {
@@ -80,7 +87,7 @@ struct OptionSpec {
 // solve.cc:379-385 plus the opt-in extras
 const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", true, false}, {"output_file", true, false},
                                {"n_threads", true, false},    {"banned_images", true, true}, {"device", true, false},
-                               {"gpus", true, false}};
+                               {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -101,7 +108,7 @@ const OptionSpec& find_option(const std::string& name) {
 struct Args {
   bool help = false;
   std::map<std::string, std::string> single;
-  std::vector<std::string> banned;
+  std::map<std::string, std::vector<std::string>> repeated;
 };
 
 // Boost.Program_options semantics of solve.cc:387-401: long options, `--name value` or `--name=value`,
@@ -124,7 +131,7 @@ Args parse(int argc, char** argv) {
           throw CliError{std::string("the required argument for option '--") + o.name + "' is missing"};
         }
         if (o.repeat) {
-          a.banned.push_back(v);
+          a.repeated[o.name].push_back(v);
         } else if (a.single.count(o.name)) {
           throw CliError{std::string("option '--") + o.name + "' cannot be specified more than once"};
         } else {
@@ -220,11 +227,11 @@ long long ms_between(Clock::time_point a, Clock::time_point b) {
 }  // namespace
 
 int main(int argc, char** argv) {
-  std::string matches_file, output_file;
-  std::vector<std::string> banned_list;
+  std::string matches_file, output_file, initial_solution;
+  std::vector<std::string> banned_list, fixed_list;
   uint64_t device = 0, gpus = 1;
   try {
-    const Args a = parse(argc, argv);
+    Args a = parse(argc, argv);
     if (a.help) {
       std::fputs("Patch Match graph problem solver\n\n", stdout);
       std::fputs(kUsage, stdout);
@@ -237,11 +244,29 @@ int main(int argc, char** argv) {
     (void)as_uint(a, "n_threads", 8);
     device = as_uint(a, "device", 0);
     gpus = as_uint(a, "gpus", 1);
-    banned_list = a.banned;
+    banned_list = a.repeated["banned_images"];
+    fixed_list = a.repeated["fixed_images"];
+    if (a.single.count("initial_solution")) initial_solution = a.single.at("initial_solution");
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
     return 1;
+  }
+
+  // the start solution is read and checked before any other work, so that its errors come before any output
+  FileImage start_file;
+  const bool have_start = !initial_solution.empty();
+  if (have_start) {
+    if (!start_file.open(initial_solution)) {
+      std::fprintf(stderr, "ERROR: cannot read the initial solution file '%s'\n", initial_solution.c_str());
+      return 2;
+    }
+    uint64_t ni = 0, nd = 0;
+    if (lfr_wire_decode_solution(start_file.data(), start_file.size(), &ni, &nd, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                 nullptr, nullptr) != LFR_OK) {
+      std::fputs("Failed to parse proto object.\n", stderr);  // as for the matches, solve.cc:433-436
+      return 255;
+    }
   }
 
   // A one-shot process pays for CUDA's start-up (driver initialisation over every visible GPU, context
@@ -334,6 +359,23 @@ int main(int argc, char** argv) {
     if (!have_fact[pair_img2[p]]) { have_fact[pair_img2[p]] = 1; image_fact[pair_img2[p]] = pair_fact2[p]; }
   }
 
+  // images held fixed (the same name semantics as banned images), and the names by image id as the
+  // start-point join and the encoder on the GPU take them
+  const std::set<std::string> fixed_names(fixed_list.begin(), fixed_list.end());
+  std::vector<uint8_t> fixed(names.size(), 0);
+  bool any_fixed = false;
+  for (size_t i = 0; i < names.size(); ++i)
+    if (fixed_names.count(names[i])) {
+      fixed[i] = 1;
+      any_fixed = true;
+    }
+  std::vector<uint8_t> name_blob;
+  std::vector<uint64_t> name_off(names.size() + 1, 0);
+  for (size_t i = 0; i < names.size(); ++i) {
+    name_blob.insert(name_blob.end(), names[i].begin(), names[i].end());
+    name_off[i + 1] = name_blob.size();
+  }
+
   lfr_host_input in;
   std::memset(&in, 0, sizeof in);
   in.n_pairs = P; in.n_matches = M; in.n_images = (uint32_t)names.size();
@@ -344,7 +386,8 @@ int main(int argc, char** argv) {
   // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
   // takes the host route; forcing the device route there is an error, never a silent host run.
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
-                                 lfr_plan_create_from_wire && lfr_plan_encode_solution;
+                                 lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
+                                 lfr_plan_start_from_solution;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -423,6 +466,15 @@ int main(int argc, char** argv) {
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
       return 2;
     }
+    // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
+    int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), (uint32_t)names.size()) : LFR_OK;
+    if (rc2 == LFR_OK && have_start)
+      rc2 = lfr_plan_start_from_solution(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                         name_blob.data(), name_off.data(), nullptr);
+    if (rc2 != LFR_OK) {
+      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc2, lfr_last_error());
+      return 2;
+    }
   } else {
     // ---- host graph stage (solve.cc:438-606); the edge records go straight into page-locked memory
     if (e_cap) {
@@ -459,15 +511,27 @@ int main(int argc, char** argv) {
   }
   std::fflush(stdout);
 
-  // ---- the solve (solve.cc:608-635): positions start at zero --------------------------------
+  // ---- the solve (solve.cc:608-635): positions start at zero, or from --initial_solution -----
   double* positions = nullptr;  // host route: the solve's result; the device route keeps it in HBM
   bool positions_pinned = false;
+  std::vector<uint8_t> is_const;  // host route with --fixed_images: reference roots OR nodes of fixed images
   if (N && !plan) {
     positions = static_cast<double*>(lfr_host_alloc(2ull * N * sizeof(double)));
     positions_pinned = positions != nullptr;
     if (!positions) positions = static_cast<double*>(std::malloc(2ull * N * sizeof(double)));
     std::memset(positions, 0, 2ull * N * sizeof(double));
+    if (have_start && lfr_wire_join_solution(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
+                                             name_off.data(), N, node_image.data(), node_feat.data(), positions,
+                                             nullptr) != LFR_OK) {
+      std::fprintf(stderr, "ERROR: lfr_wire_join_solution failed\n");
+      return 2;
+    }
+    if (any_fixed) {
+      is_const.resize(N);
+      for (uint32_t v = 0; v < N; ++v) is_const[v] = (is_root[v] || fixed[node_image[v]]) ? 1 : 0;
+    }
   }
+  start_file.release();
   const Clock::time_point t_solve = Clock::now();
   if (N && plan) {
     int rc = lfr_plan_solve(plan, nullptr);
@@ -480,7 +544,7 @@ int main(int argc, char** argv) {
     lfr_problem prob;
     prob.n_nodes = N; prob.n_components = C; prob.n_edges = E;
     prob.row_ptr = row_ptr.data(); prob.edges = edges; prob.track = track.data(); prob.comp = comp.data();
-    prob.is_root = is_root.data(); prob.comp_ptr = comp_ptr.data(); prob.comp_nodes = comp_nodes.data();
+    prob.is_root = any_fixed ? is_const.data() : is_root.data(); prob.comp_ptr = comp_ptr.data(); prob.comp_nodes = comp_nodes.data();
     lfr_options opt;
     lfr_options_default(&opt);
     opt.device = (int32_t)device;
@@ -511,14 +575,8 @@ int main(int argc, char** argv) {
   if (plan) {
     // encoded on the GPU, names and facts indexed by image id, into page-locked memory sized by the
     // largest encoding: a Displacement record is at most 18 bytes, an Image's header 16 plus its name field
-    std::vector<uint8_t> name_blob;
-    std::vector<uint64_t> name_off(names.size() + 1, 0);
     uint64_t cap = 18ull * N;
-    for (size_t i = 0; i < names.size(); ++i) {
-      name_blob.insert(name_blob.end(), names[i].begin(), names[i].end());
-      name_off[i + 1] = name_blob.size();
-      cap += 16 + 11 + names[i].size();
-    }
+    for (size_t i = 0; i < names.size(); ++i) cap += 16 + 11 + names[i].size();
     out = static_cast<uint8_t*>(lfr_host_alloc(cap));
     out_pinned = out != nullptr;
     if (!out) out = static_cast<uint8_t*>(std::malloc(cap ? cap : 1));
@@ -553,20 +611,20 @@ int main(int argc, char** argv) {
         if (std::fabs(positions[2 * (size_t)v + 1]) > 0.5 || std::fabs(positions[2 * (size_t)v]) > 0.5) ++n_outside;  // solve.cc:666-669
       }
     }
-    std::vector<uint8_t> name_blob;
-    std::vector<uint64_t> name_off(I + 1, 0);
+    std::vector<uint8_t> out_blob;
+    std::vector<uint64_t> out_off(I + 1, 0);
     std::vector<float> fact(I);
     for (size_t i = 0; i < I; ++i) {
       const std::string& s = names[img_ids[i]];
-      name_blob.insert(name_blob.end(), s.begin(), s.end());
-      name_off[i + 1] = name_blob.size();
+      out_blob.insert(out_blob.end(), s.begin(), s.end());
+      out_off[i + 1] = out_blob.size();
       fact[i] = image_fact[img_ids[i]];
     }
-    if (name_blob.empty()) name_blob.push_back(0);
-    need = lfr_wire_encode_solution(I, img_ptr.data(), name_blob.data(), name_off.data(), fact.data(),
+    if (out_blob.empty()) out_blob.push_back(0);
+    need = lfr_wire_encode_solution(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
                                     feature_idx.data(), di.data(), dj.data(), nullptr, 0);
     out = static_cast<uint8_t*>(std::malloc((size_t)std::max<int64_t>(need, 1)));
-    if (need < 0 || lfr_wire_encode_solution(I, img_ptr.data(), name_blob.data(), name_off.data(), fact.data(),
+    if (need < 0 || lfr_wire_encode_solution(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
                                              feature_idx.data(), di.data(), dj.data(), out, (uint64_t)need) != need)
       need = -1;
   }

@@ -27,7 +27,7 @@ class WireMatches(C.Structure):
 
 
 WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
-                "lfr_wire_encode_solution", "lfr_wire_decode_solution"]
+                "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution"]
 
 _bound = False
 
@@ -49,6 +49,9 @@ def _lib():
         L.lfr_wire_decode_solution.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
                                                C.POINTER(C.c_uint64)] + [C.c_void_p] * 7
         L.lfr_wire_decode_solution.restype = C.c_int
+        L.lfr_wire_join_solution.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+        L.lfr_wire_join_solution.restype = C.c_int
         _bound = True
     return L
 
@@ -232,3 +235,25 @@ def decode_solution(data: bytes):
         nm = data[int(noff[i]): int(noff[i]) + int(nlen[i])].decode("utf-8", errors="surrogateescape")
         out.append((nm, float(fact[i]), fi[a:b], di[a:b], dj[a:b]))
     return out
+
+
+def join_solution(data: bytes, image_names: List[str], node_image: np.ndarray, node_feat: np.ndarray):
+    """Start positions of a scene's nodes from the SolutionFile `data` (lfr_wire_join_solution,
+    include/lfr_wire.h): images matched by name bytes (`image_names` by image id), displacements by
+    feature; the last Image message with a name wins, and within it the last displacement of a feature.
+    Returns (positions [N, 2] float64, 0 where a node has no entry; number of nodes started).  Raises
+    ParseError on bytes the decoder rejects."""
+    L = _lib()
+    buf = np.frombuffer(data, dtype=np.uint8)
+    blob, off = _names_blob(list(image_names))
+    img = np.ascontiguousarray(node_image, dtype=np.uint32).reshape(-1)
+    feat = np.ascontiguousarray(node_feat, dtype=np.uint32).reshape(-1)
+    N = int(img.shape[0])
+    pos = np.zeros((N, 2), np.float64)
+    n = C.c_uint64()
+    rc = L.lfr_wire_join_solution(buf.ctypes.data if buf.size else None, buf.size, len(image_names), blob.ctypes.data,
+                                  off.ctypes.data, N, img.ctypes.data if N else None, feat.ctypes.data if N else None,
+                                  pos.ctypes.data if N else None, C.byref(n))
+    if rc != 0:
+        raise ParseError("Failed to parse proto object.")
+    return pos, int(n.value)
