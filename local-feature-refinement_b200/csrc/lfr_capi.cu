@@ -1809,6 +1809,13 @@ int launch_solve(lfr_plan* pl, cudaStream_t s) {
     LFR_CUDA(cudaMemcpyAsync(pl->pos.p, pl->pos_init.p, sizeof(double) * 2 * (size_t)pl->N,
                              cudaMemcpyDeviceToDevice, s));
   pl->pos_is_staged = false;  // a second launch on the same plan needs the reset again
+  if (pl->profile && pl->C) {
+    // the records are accumulated into (atomicAdd of cycles and of the tier word) and a component without
+    // free nodes writes none: each solve starts from zero, or the last solve's records would be mixed with
+    // every earlier one (a refixed mask moves components between tiers and to EMPTY)
+    LFR_CUDA(cudaMemsetAsync(pl->cycles.p, 0, sizeof(unsigned long long) * 8 * (size_t)pl->C, s));
+    LFR_CUDA(cudaMemsetAsync(pl->times.p, 0, sizeof(unsigned long long) * 2 * (size_t)pl->C, s));
+  }
   const lfr::DevProblem P_hbm = pl->dev();  // edges read from the HBM copy by global index
   lfr::DevProblem P_stage = P_hbm;          // edges pulled once into shared memory, possibly from the caller's pinned buffer
   if (pl->zc_edges) {

@@ -13,6 +13,8 @@ exactly the third-party API those files use:
                      mini_ceres.cc (restated Ceres 1.14 minimizer), types_pb_shim.cc (protobuf wire
                      format of types.proto), colmap shims (ThreadPool; the 2-way cut is the same
                      deterministic stand-in the product uses: Graclus is not available on either side)
+  libref_solve.so <- the same, with main() renamed (via oracle/ref_solve_shim.cc): create_and_solve_problem
+                     callable on any constant mask and start point
 
 Outputs go to oracle/_ref/ only (git-ignored, NOT gpurun-ignored: the binaries
 travel to the GPU box, where /root/reference does not exist).  Flags follow the
@@ -90,8 +92,32 @@ def build_solve(force: bool = False, optimized: bool = False) -> str:
     return out
 
 
+def build_solve_lib(force: bool = False) -> str:
+    """solve.cc's create_and_solve_problem as a C function (oracle/ref_solve_shim.cc) ->
+    oracle/_ref/libref_solve.so: the sources of build_solve() plus the shim, -O2 (no contraction, so
+    the same bits as the -O0 build; -O2 only makes the tests that call it fast enough)."""
+    out = os.path.join(OUT, "libref_solve.so")
+    if not reference_available():
+        if os.path.exists(out):
+            return out
+        raise RuntimeError("%s is missing and %s is not present" % (out, REF_SRC))
+    srcs = [os.path.join(HERE, "ref_solve_shim.cc"), os.path.join(REF_SRC, "graph.cc"),
+            os.path.join(SHIMS, "mini_ceres.cc"), os.path.join(SHIMS, "types_pb_shim.cc")]
+    include = os.path.join(HERE, "..", "include")
+    deps = srcs + [os.path.join(REF_SRC, "solve.cc"), os.path.join(REF_SRC, "cost.cc"), os.path.join(REF_SRC, "graph.h"),
+                   os.path.join(include, "lfr.h"),
+                   os.path.join(HERE, "..", "local-feature-refinement_b200", "csrc", "lfr_cut.h")] + _shim_files()
+    if not force and _newer(out, deps):
+        return out
+    os.makedirs(OUT, exist_ok=True)
+    cmd = [CXX, "-std=c++11", "-g", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-pthread",
+           "-I", SHIMS, "-I", REF_SRC, "-I", include, "-o", out] + srcs
+    subprocess.check_call(cmd)
+    return out
+
+
 def build(force: bool = False):
-    return [build_cost(force), build_solve(force), build_solve(force, optimized=True)]
+    return [build_cost(force), build_solve(force), build_solve(force, optimized=True), build_solve_lib(force)]
 
 
 if __name__ == "__main__":

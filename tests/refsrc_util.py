@@ -33,6 +33,47 @@ def load_refsrc():
     return _lib
 
 
+_solve_lib = None
+
+
+def load_refsolve():
+    """oracle/_ref/libref_solve.so: the reference's create_and_solve_problem (oracle/ref_solve_shim.cc).
+    Raises when it is neither built nor buildable: the tests that use it fail rather than skip."""
+    global _solve_lib
+    if _solve_lib is None:
+        path = _build_mod().build_solve_lib()
+        L = C.CDLL(path)
+        L.lfr_refsrc_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 7
+        L.lfr_refsrc_solve.restype = C.c_int
+        _solve_lib = L
+    return _solve_lib
+
+
+def ref_solve(p, is_const, start, n_threads=None):
+    """create_and_solve_problem on every slot of `p` (more than one node) with is_root = `is_const`
+    [n_nodes] and positions = `start` [n_nodes, 2].  Returns (positions, stats): stats holds the oracle's
+    per-slot names (iterations, termination, initial_cost, final_cost) plus ls_steps and fixed_cost per
+    slot, and the totals; initial_cost and final_cost are the Summary's, fixed cost included."""
+    from lfr_b200.capi import Library
+    L = load_refsolve()
+    s, keep = Library.marshal(p)
+    n, C_ = p.graph.n_nodes, p.n_components
+    mask = np.ascontiguousarray(is_const, np.uint8).reshape(n)
+    x0 = np.ascontiguousarray(start, np.float64).reshape(n, 2)
+    pos = np.zeros((n, 2))
+    st = dict(iterations=np.zeros(C_, np.int32), termination=np.zeros(C_, np.int32), ls_steps=np.zeros(C_, np.int32),
+              initial_cost=np.zeros(C_), final_cost=np.zeros(C_), fixed_cost=np.zeros(C_))
+    rc = L.lfr_refsrc_solve(C.addressof(s), mask.ctypes.data, x0.ctypes.data, int(n_threads or os.cpu_count() or 8),
+                            pos.ctypes.data, *[st[k].ctypes.data for k in ("iterations", "termination", "ls_steps",
+                                                                           "initial_cost", "final_cost", "fixed_cost")])
+    del keep
+    assert rc >= 0, "lfr_refsrc_solve could not match a summary to its component"
+    st["n_solved"] = rc
+    st["total_iterations"] = int(st["iterations"].sum())
+    st["total_line_search_steps"] = int(st["ls_steps"].sum())
+    return pos, st
+
+
 def ref_interpolate(L, grids, rc):
     n = grids.shape[0]
     grids = np.ascontiguousarray(grids, np.float64)
