@@ -113,6 +113,19 @@ int lfr_plan_fix_images(lfr_plan* plan, const uint8_t* fixed_by_image_id /* [n_i
 int lfr_plan_start_from_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                                  const uint8_t* names, const uint64_t* name_off, uint64_t* n_started);
 
+/* Keep what an earlier SolutionFile refined and refine everything else: lfr_plan_start_from_solution() (the
+ * same single host decode and device join, the same start and working positions bit for bit), and every
+ * node with an entry in the file (the rule of lfr_wire_join_solution_entries(), include/lfr_wire.h) becomes
+ * constant, as a node of a fixed image is.  The mask is reference root OR node of an image fixed by
+ * lfr_plan_fix_images() OR kept node; the per-image mask and the kept flags are separate inputs, so the two
+ * calls compose in either order, and the schedule is built again on the mask.  A later call replaces the
+ * kept set (an empty SolutionFile clears it); a later lfr_plan_start_from_solution() changes only the start
+ * values.  A plan never given a kept set holds no buffer for one.  *n_kept (may be NULL) = the nodes with an
+ * entry.  Synchronous on `stream`.  LFR_EINVAL for malformed bytes (the plan is not changed) and for a plan
+ * made by lfr_plan_create(). */
+int lfr_plan_keep_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                           const uint8_t* names, const uint64_t* name_off, uint64_t* n_kept);
+
 /* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
  * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from
  * sizes known before either stage runs — the directed edges (2 x the matches of the pairs not skipped),

@@ -97,6 +97,15 @@ int lfr_wire_join_solution(const uint8_t* buf, uint64_t len, uint32_t n_images, 
                            const uint64_t* name_off, uint32_t n_nodes, const uint32_t* node_image,
                            const uint32_t* node_feat, double* positions /* [2 n_nodes] */, uint64_t* n_started);
 
+/* lfr_wire_join_solution() that also says which nodes have an entry: has_entry[v] = 1 when node v's
+ * position came from the file, else 0 (the nodes lfr_plan_keep_solution(), include/lfr_graph.h, holds
+ * constant).  positions and *n_started as lfr_wire_join_solution() writes them, bit for bit.  LFR_EINVAL as
+ * there, or for a NULL has_entry with n_nodes > 0; every output is untouched then. */
+int lfr_wire_join_solution_entries(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                                   const uint64_t* name_off, uint32_t n_nodes, const uint32_t* node_image,
+                                   const uint32_t* node_feat, double* positions /* [2 n_nodes] */, uint64_t* n_started,
+                                   uint8_t* has_entry /* [n_nodes] */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -81,7 +81,7 @@ ABI_SYMBOLS = [
 #: the symbols include/lfr_graph.h declares
 GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
                  "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
-                 "lfr_plan_fix_images", "lfr_plan_start_from_solution"]
+                 "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution"]
 
 
 class LfrWirePart(C.Structure):
@@ -159,6 +159,8 @@ class Library:
             L.lfr_plan_start_from_solution.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                                                        C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
             L.lfr_plan_start_from_solution.restype = C.c_int
+            L.lfr_plan_keep_solution.argtypes = L.lfr_plan_start_from_solution.argtypes
+            L.lfr_plan_keep_solution.restype = C.c_int
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -472,6 +474,22 @@ class Plan:
                                                                  len(image_names), blob.ctypes.data, off.ctypes.data,
                                                                  C.byref(n)),
                        "lfr_plan_start_from_solution")
+        return int(n.value)
+
+    def keep_solution(self, data: bytes, image_names, stream: int = 0) -> int:
+        """lfr_plan_keep_solution (include/lfr_graph.h): start_from_solution(), and every node with an entry in
+        `data` is held constant in the next solves, as a node of a fixed image is; replaces an earlier kept
+        set (an empty file clears it) and composes with fix_images() in either order.  Returns the number of
+        nodes kept."""
+        from .wire import _names_blob
+        buf = np.frombuffer(data, dtype=np.uint8)
+        blob, off = _names_blob(list(image_names))
+        n = C.c_uint64()
+        self.lib.check(self.lib.lib.lfr_plan_keep_solution(self.handle, C.c_void_p(stream),
+                                                           buf.ctypes.data if buf.size else None, buf.size,
+                                                           len(image_names), blob.ctypes.data, off.ctypes.data,
+                                                           C.byref(n)),
+                       "lfr_plan_keep_solution")
         return int(n.value)
 
     def solve(self, stream: int = 0) -> None:

@@ -12,7 +12,8 @@ custom_demo.py:101-105 run unchanged.  `--n_threads` is accepted and ignored
 (the solve runs on the GPU).  Opt-in extras: --device, --gpus N (one process drives N GPUs), --stats_json,
 --fixed_images NAME (repeatable: the image's keypoints are held constant, as roots are) and
 --initial_solution FILE (start values from a SolutionFile instead of zeros): together they refine new
-images against an already-refined scene.
+images against an already-refined scene.  --keep_initial_solution (with --initial_solution) also holds
+every keypoint that has an entry in that file constant, and refines only the others.
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -47,7 +48,8 @@ class _CliError(Exception):
 _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file", True, False),
             ("n_threads", True, False), ("banned_images", True, True),
             ("device", True, False), ("gpus", True, False), ("stats_json", True, False),
-            ("fixed_images", True, True), ("initial_solution", True, False)]
+            ("fixed_images", True, True), ("initial_solution", True, False),
+            ("keep_initial_solution", False, False)]
 
 
 def _find_option(name):
@@ -121,7 +123,8 @@ def parse_args(argv):
             matches_file=vals["matches_file"], output_file=vals["output_file"],
             n_threads=_as_uint(vals, "n_threads", 8), banned_images=vals.get("banned_images", []),
             device=_as_uint(vals, "device", 0), gpus=_as_uint(vals, "gpus", 1), stats_json=vals.get("stats_json"),
-            fixed_images=vals.get("fixed_images", []), initial_solution=vals.get("initial_solution"))
+            fixed_images=vals.get("fixed_images", []), initial_solution=vals.get("initial_solution"),
+            keep_initial_solution=bool(vals.get("keep_initial_solution")))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -137,6 +140,9 @@ def main(argv=None) -> int:
     from .graph import refined_track_count
 
     # the start solution is read and checked before any other work: its errors come before any output
+    if args.keep_initial_solution and not args.initial_solution:
+        sys.stderr.write("ERROR: --keep_initial_solution needs --initial_solution FILE\n")
+        return 2
     start = None
     if args.initial_solution is not None:
         try:
@@ -200,7 +206,8 @@ def main(argv=None) -> int:
     n_devices = int(os.environ["WORLD_SIZE"]) if torchrun else max(args.gpus, 1)
     try:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
-                                 timing=timing, fixed_images=args.fixed_images, initial_solution=start)
+                                 timing=timing, fixed_images=args.fixed_images, initial_solution=start,
+                                 keep_initial_solution=args.keep_initial_solution)
     except GraphStageRouteError as e:
         sys.stderr.write("ERROR: %s\n" % e)
         return 2

@@ -273,10 +273,15 @@ struct lfr_plan {
   // the input, the encoder's scratch and its output (grow-only: repeated encodes allocate nothing)
   DevBuf node_image, node_feat, enc_scratch, enc_cub, enc_out;
   uint32_t n_images = 0;
-  // lfr_plan_fix_images(): the constant mask the tiers read in place of `is_root` (reference roots OR nodes
-  // of fixed images) and its host copy for the schedule builder; never allocated for a plan without one
+  // lfr_plan_fix_images() / lfr_plan_keep_solution(): the constant mask the tiers read in place of
+  // `is_root` (reference roots OR nodes of fixed images OR kept nodes) and its host copy for the schedule
+  // builder; never allocated for a plan without one.  Its two inputs are kept apart, so that each call
+  // replaces only its own: the per-image mask (empty until lfr_plan_fix_images()) and the per-node kept
+  // flags (allocated by the first lfr_plan_keep_solution())
   DevBuf const_mask;
   std::vector<uint8_t> const_host;
+  std::vector<uint8_t> fixed_host;
+  DevBuf kept;
 
   lfr::CtaArrays cta_arrays() const {
     lfr::CtaArrays A;
@@ -339,7 +344,7 @@ void free_plan(lfr_plan* pl) {
                     &pl->local_of, &pl->pos, &pl->pos_init, &pl->stats, &pl->cycles, &pl->times, &pl->lists, &pl->L_comps, &pl->L_rec, &pl->L_meta,
                     &pl->L_inlist, &pl->L_twin, &pl->L_fdst, &pl->L_bE01, &pl->L_bE23, &pl->L_fdstE, &pl->L_ell_base, &pl->L_scr, &pl->L_q, &pl->L_node, &pl->L_outptr, &pl->L_inptr, &pl->L_freeof,
                     &pl->L_x, &pl->L_xc, &pl->L_lof, &pl->L_vec, &pl->node_image, &pl->node_feat, &pl->enc_scratch,
-                    &pl->enc_cub, &pl->enc_out, &pl->queue_ctr, &pl->const_mask};
+                    &pl->enc_cub, &pl->enc_out, &pl->queue_ctr, &pl->const_mask, &pl->kept};
   for (DevBuf* b : bufs) b->release();
   if (pl->h_stage) cudaFreeHost(pl->h_stage);
   for (int i = 0; i < pl->n_streams; ++i) {
@@ -2096,6 +2101,110 @@ int solve_on_device(const lfr_problem* p, const lfr_options& o, double* position
   return LFR_OK;
 }
 
+// The constant mask of a plan made from matches (reference root OR node of a fixed image OR kept node),
+// expanded on the device over the plan's node ids, and the schedule built again on it: free-node counts
+// move components between tiers.  Synchronous on `s`.
+int build_constant_mask(lfr_plan* pl, cudaStream_t s) {
+  const lfr_plan::GraphArrays& G = *pl->graph;
+  const uint32_t N = pl->N;
+  LFR_TRY(pl->const_mask.reserve(std::max<size_t>(N, 1)));
+  if (N) {
+    const uint8_t* fixed = nullptr;
+    if (!pl->fixed_host.empty()) {
+      LFR_TRY(upload(&pl->enc_scratch, pl->fixed_host.data(), pl->fixed_host.size(), s));
+      fixed = pl->enc_scratch.as<uint8_t>();
+    }
+    lfr::start::constant_mask_kernel<<<blocks_for(N), 256, 0, s>>>(pl->is_root.as<uint8_t>(), pl->node_image.as<uint32_t>(),
+                                                                     fixed, pl->kept.p ? pl->kept.as<uint8_t>() : nullptr,
+                                                                     N, pl->const_mask.as<uint8_t>());
+    LFR_LAUNCHED();
+  }
+  pl->const_host.resize(N);
+  LFR_TRY(fetch(pl->const_host.data(), pl->const_mask.p, N, s));
+  lfr_problem p;
+  p.n_nodes = N;
+  p.n_components = pl->C;
+  p.n_edges = pl->E;
+  p.row_ptr = G.row_ptr.data();
+  p.edges = nullptr;  // in pl->edges
+  p.track = G.track.data();
+  p.comp = G.comp.data();
+  p.is_root = pl->const_host.data();
+  p.comp_ptr = G.comp_ptr.data();
+  p.comp_nodes = G.comp_nodes.data();
+  LFR_TRY(schedule_plan(pl, &p, s));
+  LFR_CUDA(cudaStreamSynchronize(s));
+  return LFR_OK;
+}
+
+// The arguments of lfr_plan_start_from_solution / lfr_plan_keep_solution checked, and the SolutionFile
+// decoded and its images resolved on the host (lfr_join.h), before either call changes the plan.
+int decode_solution_for(const lfr_plan* pl, const uint8_t* bytes, uint64_t len, uint32_t n_images, const uint8_t* names,
+                        const uint64_t* name_off, lfr::join::Decoded& d) {
+  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
+  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
+  if ((len && !bytes) || (n_images && !name_off)) return fail(LFR_EINVAL, "NULL SolutionFile bytes or image names");
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
+  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  const uint8_t no_name = 0;
+  if (lfr::join::decode(bytes, len, n_images, names ? names : &no_name, name_off, d) != LFR_OK)
+    return fail(LFR_EINVAL, "malformed SolutionFile");
+  if (d.n_disp >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "SolutionFile with 2^31 or more displacements");
+  return LFR_OK;
+}
+
+// The device join of a decoded SolutionFile against the plan's nodes: writes the start and working
+// positions, and has_entry[v] when it is not NULL.
+int join_solution(lfr_plan* pl, cudaStream_t s, const lfr::join::Decoded& d, uint8_t* has_entry, uint64_t* n_started) {
+  const uint32_t N = pl->N, D = (uint32_t)d.n_disp, I = (uint32_t)d.n_images;
+  if (n_started) *n_started = 0;
+  if (!N) return LFR_OK;
+  size_t at = 0;
+  auto take = [&at](size_t bytes) {
+    const size_t o = at;
+    at += (bytes + 255) & ~(size_t)255;
+    return o;
+  };
+  const size_t o_ctr = take(8), o_ptr = take(8 * ((size_t)I + 1)), o_id = take(4 * (size_t)I + 4), o_feat = take(4 * (size_t)D),
+               o_di = take(4 * (size_t)D), o_dj = take(4 * (size_t)D), o_key = take(8 * (size_t)D), o_key_s = take(8 * (size_t)D),
+               o_idx = take(4 * (size_t)D), o_idx_s = take(4 * (size_t)D);
+  LFR_TRY(pl->enc_scratch.reserve(at));
+  uint8_t* base = pl->enc_scratch.as<uint8_t>();
+  auto* ctr = reinterpret_cast<unsigned long long*>(base + o_ctr);
+  auto* img_ptr = reinterpret_cast<uint64_t*>(base + o_ptr);
+  auto* image_id = reinterpret_cast<uint32_t*>(base + o_id);
+  auto* feat = reinterpret_cast<uint32_t*>(base + o_feat);
+  auto* di = reinterpret_cast<float*>(base + o_di);
+  auto* dj = reinterpret_cast<float*>(base + o_dj);
+  auto* key = reinterpret_cast<unsigned long long*>(base + o_key);
+  auto* key_s = reinterpret_cast<unsigned long long*>(base + o_key_s);
+  auto* idx = reinterpret_cast<uint32_t*>(base + o_idx);
+  auto* idx_s = reinterpret_cast<uint32_t*>(base + o_idx_s);
+  LFR_CUDA(cudaMemsetAsync(ctr, 0, 8, s));
+  if (D) {
+    LFR_CUDA(cudaMemcpyAsync(img_ptr, d.img_ptr.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(image_id, d.image_id.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(feat, d.feature_idx.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(di, d.di.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(dj, d.dj.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+    lfr::start::solution_key_kernel<<<blocks_for(D), 256, 0, s>>>(img_ptr, image_id, I, feat, D, key, idx);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: equal keys stay in file order
+      return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, idx, idx_s, (int)D, 0, 64, s);
+    }));
+  }
+  lfr::start::join_kernel<<<blocks_for(N), 256, 0, s>>>(pl->node_image.as<uint32_t>(), pl->node_feat.as<uint32_t>(), N,
+                                                          key_s, idx_s, D, di, dj, pl->pos_init.as<double>(),
+                                                          pl->pos.as<double>(), ctr, has_entry);
+  LFR_LAUNCHED();
+  pl->pos_is_staged = true;  // the working positions hold the new start point (as after creation)
+  unsigned long long started = 0;
+  LFR_TRY(fetch(&started, ctr, 1, s));  // also keeps `d` alive until its copies are done
+  if (n_started) *n_started = started;
+  return LFR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2251,97 +2360,30 @@ int lfr_plan_fix_images(lfr_plan* pl, const uint8_t* fixed_by_image_id, uint32_t
   if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
   if (n_images && !fixed_by_image_id) return fail(LFR_EINVAL, "fixed_by_image_id is NULL");
   LFR_CUDA(cudaSetDevice(pl->device));
-  const lfr_plan::GraphArrays& G = *pl->graph;
-  const uint32_t N = pl->N;
-  cudaStream_t s = 0;
-  LFR_TRY(pl->const_mask.reserve(std::max<size_t>(N, 1)));
-  if (N) {
-    LFR_TRY(upload(&pl->enc_scratch, fixed_by_image_id, n_images, s));
-    lfr::start::constant_mask_kernel<<<blocks_for(N), 256, 0, s>>>(pl->is_root.as<uint8_t>(), pl->node_image.as<uint32_t>(),
-                                                                     pl->enc_scratch.as<uint8_t>(), N, pl->const_mask.as<uint8_t>());
-    LFR_LAUNCHED();
-  }
-  pl->const_host.resize(N);
-  LFR_TRY(fetch(pl->const_host.data(), pl->const_mask.p, N, s));
-  // free-node counts move components between tiers: the schedule is built again on the mask
-  lfr_problem p;
-  p.n_nodes = N;
-  p.n_components = pl->C;
-  p.n_edges = pl->E;
-  p.row_ptr = G.row_ptr.data();
-  p.edges = nullptr;  // in pl->edges
-  p.track = G.track.data();
-  p.comp = G.comp.data();
-  p.is_root = pl->const_host.data();
-  p.comp_ptr = G.comp_ptr.data();
-  p.comp_nodes = G.comp_nodes.data();
-  LFR_TRY(schedule_plan(pl, &p, s));
-  LFR_CUDA(cudaStreamSynchronize(s));
-  return LFR_OK;
+  pl->fixed_host.assign(fixed_by_image_id, fixed_by_image_id + n_images);
+  return build_constant_mask(pl, 0);
 }
 
 int lfr_plan_start_from_solution(lfr_plan* pl, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                                  const uint8_t* names, const uint64_t* name_off, uint64_t* n_started) {
-  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
-  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
-  if ((len && !bytes) || (n_images && !name_off)) return fail(LFR_EINVAL, "NULL SolutionFile bytes or image names");
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
-  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
-  // the decode and the image rule on the host (lfr_join.h), the join on the device
-  const uint8_t no_name = 0;
   lfr::join::Decoded d;
-  if (lfr::join::decode(bytes, len, n_images, names ? names : &no_name, name_off, d) != LFR_OK)
-    return fail(LFR_EINVAL, "malformed SolutionFile");
-  if (d.n_disp >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "SolutionFile with 2^31 or more displacements");
+  LFR_TRY(decode_solution_for(pl, bytes, len, n_images, names, name_off, d));
   LFR_CUDA(cudaSetDevice(pl->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  const uint32_t N = pl->N, D = (uint32_t)d.n_disp, I = (uint32_t)d.n_images;
-  if (n_started) *n_started = 0;
-  if (!N) return LFR_OK;
-  size_t at = 0;
-  auto take = [&at](size_t bytes) {
-    const size_t o = at;
-    at += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_ctr = take(8), o_ptr = take(8 * ((size_t)I + 1)), o_id = take(4 * (size_t)I + 4), o_feat = take(4 * (size_t)D),
-               o_di = take(4 * (size_t)D), o_dj = take(4 * (size_t)D), o_key = take(8 * (size_t)D), o_key_s = take(8 * (size_t)D),
-               o_idx = take(4 * (size_t)D), o_idx_s = take(4 * (size_t)D);
-  LFR_TRY(pl->enc_scratch.reserve(at));
-  uint8_t* base = pl->enc_scratch.as<uint8_t>();
-  auto* ctr = reinterpret_cast<unsigned long long*>(base + o_ctr);
-  auto* img_ptr = reinterpret_cast<uint64_t*>(base + o_ptr);
-  auto* image_id = reinterpret_cast<uint32_t*>(base + o_id);
-  auto* feat = reinterpret_cast<uint32_t*>(base + o_feat);
-  auto* di = reinterpret_cast<float*>(base + o_di);
-  auto* dj = reinterpret_cast<float*>(base + o_dj);
-  auto* key = reinterpret_cast<unsigned long long*>(base + o_key);
-  auto* key_s = reinterpret_cast<unsigned long long*>(base + o_key_s);
-  auto* idx = reinterpret_cast<uint32_t*>(base + o_idx);
-  auto* idx_s = reinterpret_cast<uint32_t*>(base + o_idx_s);
-  LFR_CUDA(cudaMemsetAsync(ctr, 0, 8, s));
-  if (D) {
-    LFR_CUDA(cudaMemcpyAsync(img_ptr, d.img_ptr.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemcpyAsync(image_id, d.image_id.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemcpyAsync(feat, d.feature_idx.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemcpyAsync(di, d.di.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemcpyAsync(dj, d.dj.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
-    lfr::start::solution_key_kernel<<<blocks_for(D), 256, 0, s>>>(img_ptr, image_id, I, feat, D, key, idx);
-    LFR_LAUNCHED();
-    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: equal keys stay in file order
-      return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, idx, idx_s, (int)D, 0, 64, s);
-    }));
+  return join_solution(pl, (cudaStream_t)stream, d, nullptr, n_started);
+}
+
+int lfr_plan_keep_solution(lfr_plan* pl, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                           const uint8_t* names, const uint64_t* name_off, uint64_t* n_kept) {
+  lfr::join::Decoded d;
+  LFR_TRY(decode_solution_for(pl, bytes, len, n_images, names, name_off, d));
+  LFR_CUDA(cudaSetDevice(pl->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (!pl->kept.p) {  // cleared, so that a join that fails before its kernel leaves no stale flags
+    LFR_TRY(pl->kept.reserve(std::max<size_t>(pl->N, 1)));
+    LFR_CUDA(cudaMemsetAsync(pl->kept.p, 0, std::max<size_t>(pl->N, 1), s));
   }
-  lfr::start::join_kernel<<<blocks_for(N), 256, 0, s>>>(pl->node_image.as<uint32_t>(), pl->node_feat.as<uint32_t>(), N,
-                                                          key_s, idx_s, D, di, dj, pl->pos_init.as<double>(),
-                                                          pl->pos.as<double>(), ctr);
-  LFR_LAUNCHED();
-  pl->pos_is_staged = true;  // the working positions hold the new start point (as after creation)
-  unsigned long long started = 0;
-  LFR_TRY(fetch(&started, ctr, 1, s));  // also keeps `d` alive until its copies are done
-  if (n_started) *n_started = started;
-  return LFR_OK;
+  LFR_TRY(join_solution(pl, s, d, pl->kept.as<uint8_t>(), n_kept));
+  return build_constant_mask(pl, s);
 }
 
 int lfr_debug_last_encode_times(double* out2) {

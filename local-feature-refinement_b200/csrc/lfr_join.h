@@ -1,6 +1,7 @@
 // lfr_join.h — the host half of a start point read from a SolutionFile (types.proto:30-46), shared by the
-// host join (lfr_wire_join_solution, lfr_wire.cc) and the device join (lfr_plan_start_from_solution,
-// lfr_capi.cu): the decode with lfr_wire_decode_solution() and the image rule.  Header-only host code.
+// host joins (lfr_wire_join_solution and _entries, lfr_wire.cc) and the device join
+// (lfr_plan_start_from_solution and lfr_plan_keep_solution, lfr_capi.cu): the decode with
+// lfr_wire_decode_solution() and the image rule, and the host joins' node loop.  Header-only host code.
 //
 // The rule is that of the reference's own reader (reconstruction-scripts/colmap_utils.py:104-137): an
 // Image message is matched to a scene image by its exact name bytes, and the last Image message with a
@@ -10,9 +11,11 @@
 #ifndef LFR_JOIN_H_
 #define LFR_JOIN_H_
 
+#include <algorithm>
 #include <cstdint>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/lfr.h"
@@ -66,6 +69,47 @@ inline int decode(const uint8_t* buf, uint64_t len, uint32_t n_images, const uin
   }
   for (uint32_t k = 0; k < n_images; ++k)
     if (winner[k] != ~0ull) d.image_id[winner[k]] = k;
+  return LFR_OK;
+}
+
+// The host join (lfr_wire_join_solution / _entries): positions[2v .. 2v+1] from node v's entry, 0 without
+// one; has_entry[v] (may be NULL) = whether it has one.  Every output is untouched when the arguments or the
+// bytes are rejected (LFR_EINVAL).
+inline int join_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                      uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, double* positions,
+                      uint8_t* has_entry, uint64_t* n_started) {
+  if ((!buf && len) || (n_images && !name_off) || (n_nodes && (!node_image || !node_feat || !positions)))
+    return LFR_EINVAL;
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return LFR_EINVAL;
+  if (n_images && name_off[n_images] && !names) return LFR_EINVAL;
+  const uint8_t no_name = 0;
+  Decoded d;
+  if (decode(buf, len, n_images, names ? names : &no_name, name_off, d) != LFR_OK) return LFR_EINVAL;
+  // (key, displacement) sorted by key, stably: the last entry of a run of equal keys is the last occurrence
+  std::vector<std::pair<uint64_t, uint64_t>> keyed;
+  keyed.reserve(d.n_disp);
+  for (uint64_t i = 0; i < d.n_images; ++i)
+    if (d.image_id[i] != kNoImage)
+      for (uint64_t k = d.img_ptr[i]; k < d.img_ptr[i + 1]; ++k) keyed.emplace_back(node_key(d.image_id[i], d.feature_idx[k]), k);
+  std::stable_sort(keyed.begin(), keyed.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  uint64_t started = 0;
+  for (uint32_t v = 0; v < n_nodes; ++v) {
+    const uint64_t key = node_key(node_image[v], node_feat[v]);
+    const auto it = std::upper_bound(keyed.begin(), keyed.end(), key,
+                                     [](uint64_t x, const std::pair<uint64_t, uint64_t>& e) { return x < e.first; });
+    double a = 0.0, b = 0.0;
+    const bool hit = it != keyed.begin() && (it - 1)->first == key;
+    if (hit) {
+      a = (double)d.di[(it - 1)->second];
+      b = (double)d.dj[(it - 1)->second];
+      ++started;
+    }
+    positions[2 * (size_t)v] = a;
+    positions[2 * (size_t)v + 1] = b;
+    if (has_entry) has_entry[v] = hit ? 1 : 0;
+  }
+  if (n_started) *n_started = started;
   return LFR_OK;
 }
 

@@ -20,9 +20,10 @@
 // Both routes give the same bytes and lines.  LFR_GRAPH_STAGE=host|device forces a route (a test and
 // measurement hook); on the device route LFR_DEVICE_CUT=1 cuts oversized meta-components on the GPU too.  Opt-in extras: --device D, --gpus N (one process drives N GPUs; host route),
 // --fixed_images NAME (repeatable: every node of the image is held constant, as a root is) and
-// --initial_solution FILE (start values from a SolutionFile instead of zeros) — on the device route
-// lfr_plan_fix_images() / lfr_plan_start_from_solution(), on the host route the constant mask and
-// lfr_wire_join_solution() handed to the solve.  `--n_threads` is accepted and
+// --initial_solution FILE (start values from a SolutionFile instead of zeros), with
+// --keep_initial_solution (every keypoint with an entry in that file is held constant too) — on the device
+// route lfr_plan_fix_images() / lfr_plan_start_from_solution() or lfr_plan_keep_solution(), on the host
+// route the constant mask and lfr_wire_join_solution() or _entries() handed to the solve.  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -64,6 +65,8 @@ int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images
 int lfr_plan_fix_images(lfr_plan* plan, const uint8_t* fixed_by_image_id, uint32_t n_images) __attribute__((weak));
 int lfr_plan_start_from_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                                  const uint8_t* names, const uint64_t* name_off, uint64_t* n_started) __attribute__((weak));
+int lfr_plan_keep_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                           const uint8_t* names, const uint64_t* name_off, uint64_t* n_kept) __attribute__((weak));
 }
 
 namespace {
@@ -87,7 +90,8 @@ struct OptionSpec {
 // solve.cc:379-385 plus the opt-in extras
 const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", true, false}, {"output_file", true, false},
                                {"n_threads", true, false},    {"banned_images", true, true}, {"device", true, false},
-                               {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false}};
+                               {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false},
+                               {"keep_initial_solution", false, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -106,7 +110,7 @@ const OptionSpec& find_option(const std::string& name) {
 }
 
 struct Args {
-  bool help = false;
+  bool help = false, keep_initial_solution = false;
   std::map<std::string, std::string> single;
   std::map<std::string, std::vector<std::string>> repeated;
 };
@@ -139,7 +143,7 @@ Args parse(int argc, char** argv) {
         }
       } else {
         if (eq != std::string::npos) throw CliError{std::string("option '--") + o.name + "' does not take any arguments"};
-        a.help = true;
+        (std::strcmp(o.name, "help") == 0 ? a.help : a.keep_initial_solution) = true;
       }
     } else if (tok.size() > 1 && tok[0] == '-') {
       throw CliError{"unrecognised option '" + tok + "'"};
@@ -230,6 +234,7 @@ int main(int argc, char** argv) {
   std::string matches_file, output_file, initial_solution;
   std::vector<std::string> banned_list, fixed_list;
   uint64_t device = 0, gpus = 1;
+  bool keep_start = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -247,6 +252,7 @@ int main(int argc, char** argv) {
     banned_list = a.repeated["banned_images"];
     fixed_list = a.repeated["fixed_images"];
     if (a.single.count("initial_solution")) initial_solution = a.single.at("initial_solution");
+    keep_start = a.keep_initial_solution;
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
@@ -256,6 +262,10 @@ int main(int argc, char** argv) {
   // the start solution is read and checked before any other work, so that its errors come before any output
   FileImage start_file;
   const bool have_start = !initial_solution.empty();
+  if (keep_start && !have_start) {
+    std::fputs("ERROR: --keep_initial_solution needs --initial_solution FILE\n", stderr);
+    return 2;
+  }
   if (have_start) {
     if (!start_file.open(initial_solution)) {
       std::fprintf(stderr, "ERROR: cannot read the initial solution file '%s'\n", initial_solution.c_str());
@@ -387,7 +397,7 @@ int main(int argc, char** argv) {
   // takes the host route; forcing the device route there is an error, never a silent host run.
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
-                                 lfr_plan_start_from_solution;
+                                 lfr_plan_start_from_solution && lfr_plan_keep_solution;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -469,8 +479,8 @@ int main(int argc, char** argv) {
     // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
     int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), (uint32_t)names.size()) : LFR_OK;
     if (rc2 == LFR_OK && have_start)
-      rc2 = lfr_plan_start_from_solution(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
-                                         name_blob.data(), name_off.data(), nullptr);
+      rc2 = (keep_start ? lfr_plan_keep_solution : lfr_plan_start_from_solution)(
+          plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(), name_off.data(), nullptr);
     if (rc2 != LFR_OK) {
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc2, lfr_last_error());
       return 2;
@@ -514,21 +524,29 @@ int main(int argc, char** argv) {
   // ---- the solve (solve.cc:608-635): positions start at zero, or from --initial_solution -----
   double* positions = nullptr;  // host route: the solve's result; the device route keeps it in HBM
   bool positions_pinned = false;
-  std::vector<uint8_t> is_const;  // host route with --fixed_images: reference roots OR nodes of fixed images
+  // host route with --fixed_images or --keep_initial_solution: reference roots OR nodes of fixed images OR
+  // nodes with an entry in the start solution
+  std::vector<uint8_t> is_const;
+  const bool any_const = any_fixed || keep_start;
   if (N && !plan) {
     positions = static_cast<double*>(lfr_host_alloc(2ull * N * sizeof(double)));
     positions_pinned = positions != nullptr;
     if (!positions) positions = static_cast<double*>(std::malloc(2ull * N * sizeof(double)));
     std::memset(positions, 0, 2ull * N * sizeof(double));
-    if (have_start && lfr_wire_join_solution(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
-                                             name_off.data(), N, node_image.data(), node_feat.data(), positions,
-                                             nullptr) != LFR_OK) {
+    std::vector<uint8_t> has_entry(keep_start ? N : 0, 0);
+    if (have_start && (keep_start ? lfr_wire_join_solution_entries(start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                                                  name_blob.data(), name_off.data(), N, node_image.data(),
+                                                                  node_feat.data(), positions, nullptr, has_entry.data())
+                                  : lfr_wire_join_solution(start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                                           name_blob.data(), name_off.data(), N, node_image.data(),
+                                                           node_feat.data(), positions, nullptr)) != LFR_OK) {
       std::fprintf(stderr, "ERROR: lfr_wire_join_solution failed\n");
       return 2;
     }
-    if (any_fixed) {
+    if (any_const) {
       is_const.resize(N);
-      for (uint32_t v = 0; v < N; ++v) is_const[v] = (is_root[v] || fixed[node_image[v]]) ? 1 : 0;
+      for (uint32_t v = 0; v < N; ++v)
+        is_const[v] = (is_root[v] || fixed[node_image[v]] || (keep_start && has_entry[v])) ? 1 : 0;
     }
   }
   start_file.release();
@@ -544,7 +562,7 @@ int main(int argc, char** argv) {
     lfr_problem prob;
     prob.n_nodes = N; prob.n_components = C; prob.n_edges = E;
     prob.row_ptr = row_ptr.data(); prob.edges = edges; prob.track = track.data(); prob.comp = comp.data();
-    prob.is_root = any_fixed ? is_const.data() : is_root.data(); prob.comp_ptr = comp_ptr.data(); prob.comp_nodes = comp_nodes.data();
+    prob.is_root = any_const ? is_const.data() : is_root.data(); prob.comp_ptr = comp_ptr.data(); prob.comp_nodes = comp_nodes.data();
     lfr_options opt;
     lfr_options_default(&opt);
     opt.device = (int32_t)device;

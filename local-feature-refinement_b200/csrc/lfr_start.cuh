@@ -1,9 +1,10 @@
-// lfr_start.cuh — fixed images and start points of a device-resident plan (lfr_plan_fix_images,
-// lfr_plan_start_from_solution; include/lfr_graph.h), over the node ids the plan keeps in HBM.
+// lfr_start.cuh — fixed images, kept solutions and start points of a device-resident plan
+// (lfr_plan_fix_images, lfr_plan_keep_solution, lfr_plan_start_from_solution; include/lfr_graph.h), over the
+// node ids the plan keeps in HBM.
 //
 // A constant node is what a root is to every tier (lfr_setup.cuh: kept at its start value, no bounds, a
-// block between two constant nodes dropped), so fixing images only widens the mask the tiers read as
-// `is_root`.  The start point is a sorted join: the SolutionFile's displacements keyed as the encoder keys
+// block between two constant nodes dropped), so fixing images and keeping a solution only widen the mask
+// the tiers read as `is_root`.  The start point is a sorted join: the SolutionFile's displacements keyed as the encoder keys
 // nodes (image id << 32 | feature, lfr_join.h), radix-sorted stably so the last of a run of equal keys is
 // the last occurrence, then one binary search per node.
 #ifndef LFR_START_CUH_
@@ -14,11 +15,13 @@
 namespace lfr {
 namespace start {
 
-// constant[v] = reference root OR node of a fixed image
+// constant[v] = reference root OR node of a fixed image OR kept node; `fixed` (per image) and `kept` (per
+// node) may each be NULL, for a plan never given that input
 __global__ void constant_mask_kernel(const uint8_t* __restrict__ is_root, const uint32_t* __restrict__ node_image,
-                                     const uint8_t* __restrict__ fixed, uint32_t N, uint8_t* __restrict__ constant) {
+                                     const uint8_t* __restrict__ fixed, const uint8_t* __restrict__ kept, uint32_t N,
+                                     uint8_t* __restrict__ constant) {
   const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v < N) constant[v] = (is_root[v] || fixed[node_image[v]]) ? 1 : 0;
+  if (v < N) constant[v] = (is_root[v] || (fixed && fixed[node_image[v]]) || (kept && kept[v])) ? 1 : 0;
 }
 
 // key of displacement d: its Image message i = the last with img_ptr[i] <= d (img_ptr[0] = 0), keyed when
@@ -38,11 +41,13 @@ __global__ void solution_key_kernel(const uint64_t* __restrict__ img_ptr, const 
   idx[d] = d;
 }
 
-// positions of node v from the last entry with its key (0 without one), into the start and working arrays
+// positions of node v from the last entry with its key (0 without one), into the start and working arrays;
+// has_entry[v] (may be NULL) = whether it has one
 __global__ void join_kernel(const uint32_t* __restrict__ node_image, const uint32_t* __restrict__ node_feat, uint32_t N,
                             const unsigned long long* __restrict__ key_s, const uint32_t* __restrict__ idx_s, uint32_t D,
                             const float* __restrict__ di, const float* __restrict__ dj, double* __restrict__ pos_init,
-                            double* __restrict__ pos, unsigned long long* __restrict__ n_started) {
+                            double* __restrict__ pos, unsigned long long* __restrict__ n_started,
+                            uint8_t* __restrict__ has_entry) {
   const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= N) return;
   const unsigned long long k = (unsigned long long)node_image[v] << 32 | node_feat[v];
@@ -52,12 +57,14 @@ __global__ void join_kernel(const uint32_t* __restrict__ node_image, const uint3
     if (key_s[mid] <= k) lo = mid + 1; else hi = mid;
   }
   double a = 0.0, b = 0.0;
-  if (lo > 0 && key_s[lo - 1] == k) {
+  const bool hit = lo > 0 && key_s[lo - 1] == k;
+  if (hit) {
     const uint32_t e = idx_s[lo - 1];
     a = (double)di[e];
     b = (double)dj[e];
     atomicAdd(n_started, 1ull);
   }
+  if (has_entry) has_entry[v] = hit ? 1 : 0;
   pos_init[2 * (size_t)v] = a;
   pos_init[2 * (size_t)v + 1] = b;
   pos[2 * (size_t)v] = a;

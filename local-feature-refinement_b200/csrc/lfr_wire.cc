@@ -445,38 +445,16 @@ int lfr_wire_decode_solution(const uint8_t* buf, uint64_t len, uint64_t* n_image
 int lfr_wire_join_solution(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
                            const uint64_t* name_off, uint32_t n_nodes, const uint32_t* node_image,
                            const uint32_t* node_feat, double* positions, uint64_t* n_started) {
-  if ((!buf && len) || (n_images && !name_off) || (n_nodes && (!node_image || !node_feat || !positions)))
-    return LFR_EINVAL;
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (name_off[k + 1] < name_off[k]) return LFR_EINVAL;
-  if (n_images && name_off[n_images] && !names) return LFR_EINVAL;
-  const uint8_t no_name = 0;
-  lfr::join::Decoded d;
-  if (lfr::join::decode(buf, len, n_images, names ? names : &no_name, name_off, d) != LFR_OK) return LFR_EINVAL;
-  // (key, displacement) sorted by key, stably: the last entry of a run of equal keys is the last occurrence
-  std::vector<std::pair<uint64_t, uint64_t>> keyed;
-  keyed.reserve(d.n_disp);
-  for (uint64_t i = 0; i < d.n_images; ++i)
-    if (d.image_id[i] != lfr::join::kNoImage)
-      for (uint64_t k = d.img_ptr[i]; k < d.img_ptr[i + 1]; ++k)
-        keyed.emplace_back(lfr::join::node_key(d.image_id[i], d.feature_idx[k]), k);
-  std::stable_sort(keyed.begin(), keyed.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-  uint64_t started = 0;
-  for (uint32_t v = 0; v < n_nodes; ++v) {
-    const uint64_t key = lfr::join::node_key(node_image[v], node_feat[v]);
-    const auto it = std::upper_bound(keyed.begin(), keyed.end(), key,
-                                     [](uint64_t x, const std::pair<uint64_t, uint64_t>& e) { return x < e.first; });
-    double a = 0.0, b = 0.0;
-    if (it != keyed.begin() && (it - 1)->first == key) {
-      a = (double)d.di[(it - 1)->second];
-      b = (double)d.dj[(it - 1)->second];
-      ++started;
-    }
-    positions[2 * (size_t)v] = a;
-    positions[2 * (size_t)v + 1] = b;
-  }
-  if (n_started) *n_started = started;
-  return LFR_OK;
+  return lfr::join::join_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions, nullptr,
+                               n_started);
+}
+
+int lfr_wire_join_solution_entries(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                                   const uint64_t* name_off, uint32_t n_nodes, const uint32_t* node_image,
+                                   const uint32_t* node_feat, double* positions, uint64_t* n_started, uint8_t* has_entry) {
+  if (n_nodes && !has_entry) return LFR_EINVAL;
+  return lfr::join::join_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions, has_entry,
+                               n_started);
 }
 
 }  // extern "C"

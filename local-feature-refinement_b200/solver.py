@@ -101,44 +101,53 @@ def fixed_image_mask(image_names: List[str], fixed_images) -> np.ndarray:
     return np.array([n in fixed for n in image_names], dtype=bool).reshape(-1)
 
 
-def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[bytes] = None):
+def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[bytes] = None,
+                     keep_initial_solution: bool = False):
     """The host route's problem initialisation with fixed images and a start solution: (the Problem to solve,
-    whose is_root is the constant mask = reference root OR node of a fixed image; start positions [N, 2] from
+    whose is_root is the constant mask = reference root OR node of a fixed image OR, with
+    `keep_initial_solution`, node with an entry in the start solution; start positions [N, 2] from
     wire.join_solution, or None for zeros)."""
     from . import wire
     g = p.graph
-    q = p
+    const = np.asarray(p.is_root) != 0
     if len(fixed_images) and g.n_nodes:
-        fixed = fixed_image_mask(g.image_names, fixed_images)
-        q = dataclasses.replace(p, is_root=((p.is_root != 0) | fixed[np.asarray(g.node_image, np.int64)]).astype(np.uint8))
+        const = const | fixed_image_mask(g.image_names, fixed_images)[np.asarray(g.node_image, np.int64)]
     start = None
     if initial_solution is not None:
-        start, _ = wire.join_solution(initial_solution, g.image_names, g.node_image, g.node_feat)
-    return q, start
+        start, _, has_entry = wire.join_solution(initial_solution, g.image_names, g.node_image, g.node_feat, entries=True)
+        if keep_initial_solution:
+            const = const | has_entry
+    if (len(fixed_images) or keep_initial_solution) and g.n_nodes:
+        return dataclasses.replace(p, is_root=const.astype(np.uint8)), start
+    return p, start
 
 
 def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[[str], None]] = None,
            solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None, fixed_images=(),
-           initial_solution: Optional[bytes] = None):
+           initial_solution: Optional[bytes] = None, keep_initial_solution: bool = False):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
     may be supplied to drive a different executor (the multi-GPU path; give `n_devices`); with a start
     solution it is called as `solve_fn(problem, positions)`.
 
     `fixed_images` (names) hold every node of those images constant, as a root is: it keeps its start value.
     `initial_solution` (SolutionFile bytes) gives the start values (wire.join_solution) instead of zeros.
-    Together they refine new images against an already-refined scene.  The returned Problem keeps the
-    reference's is_root.
+    Together they refine new images against an already-refined scene.  `keep_initial_solution` (needs
+    `initial_solution`) also holds every node with an entry in that file constant (the rule of
+    wire.join_solution), so only the keypoints it does not list are refined.  The returned Problem keeps
+    the reference's is_root.
 
     The graph stage runs where graph_stage_on_device() says.  On the device (Plan.from_matches) the problem
     stays in HBM and is solved there, `solve_fn` is not called, and the Problem's arrays come from
     Plan.export_graph(); `timing["solver_ms"]` (when `timing` is given) then covers solve + download."""
     from .capi import Plan, load_b200
     from .graph import host_input_arrays, problem_from_stage
+    if keep_initial_solution and initial_solution is None:
+        raise ValueError("keep_initial_solution needs initial_solution")
     lib = load_b200()
     skip, arrs = host_input_arrays(ms, banned_images)
     if not graph_stage_on_device(lib, arrs, len(ms.image_names), n_devices):
         p = build_problem(ms, banned_images, log=log)
-        q, start = constant_problem(p, fixed_images, initial_solution)
+        q, start = constant_problem(p, fixed_images, initial_solution, keep_initial_solution)
         fn = solve_fn if solve_fn is not None else (lambda q_, x=None: solve_problem(q_, options, x))
         pos, st = fn(q) if start is None else fn(q, start)
         return p, pos, st, assemble_solution(p, pos)
@@ -146,7 +155,9 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     try:
         if len(fixed_images) and fixed_image_mask(ms.image_names, fixed_images).any():
             plan.fix_images(fixed_image_mask(ms.image_names, fixed_images))
-        if initial_solution is not None:
+        if keep_initial_solution:
+            plan.keep_solution(initial_solution, ms.image_names)
+        elif initial_solution is not None:
             plan.start_from_solution(initial_solution, ms.image_names)
         p = problem_from_stage(ms, skip, plan.export_graph(), plan.sizes, "device", log)
         t1 = time.perf_counter()

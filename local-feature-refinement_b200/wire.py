@@ -27,7 +27,8 @@ class WireMatches(C.Structure):
 
 
 WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
-                "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution"]
+                "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution",
+                "lfr_wire_join_solution_entries"]
 
 _bound = False
 
@@ -52,6 +53,8 @@ def _lib():
         L.lfr_wire_join_solution.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
                                              C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
         L.lfr_wire_join_solution.restype = C.c_int
+        L.lfr_wire_join_solution_entries.argtypes = L.lfr_wire_join_solution.argtypes + [C.c_void_p]
+        L.lfr_wire_join_solution_entries.restype = C.c_int
         _bound = True
     return L
 
@@ -237,11 +240,13 @@ def decode_solution(data: bytes):
     return out
 
 
-def join_solution(data: bytes, image_names: List[str], node_image: np.ndarray, node_feat: np.ndarray):
+def join_solution(data: bytes, image_names: List[str], node_image: np.ndarray, node_feat: np.ndarray,
+                  entries: bool = False):
     """Start positions of a scene's nodes from the SolutionFile `data` (lfr_wire_join_solution,
     include/lfr_wire.h): images matched by name bytes (`image_names` by image id), displacements by
     feature; the last Image message with a name wins, and within it the last displacement of a feature.
-    Returns (positions [N, 2] float64, 0 where a node has no entry; number of nodes started).  Raises
+    Returns (positions [N, 2] float64, 0 where a node has no entry; number of nodes started), and with
+    `entries` also has_entry [N] bool, which nodes have an entry (lfr_wire_join_solution_entries).  Raises
     ParseError on bytes the decoder rejects."""
     L = _lib()
     buf = np.frombuffer(data, dtype=np.uint8)
@@ -251,9 +256,13 @@ def join_solution(data: bytes, image_names: List[str], node_image: np.ndarray, n
     N = int(img.shape[0])
     pos = np.zeros((N, 2), np.float64)
     n = C.c_uint64()
-    rc = L.lfr_wire_join_solution(buf.ctypes.data if buf.size else None, buf.size, len(image_names), blob.ctypes.data,
-                                  off.ctypes.data, N, img.ctypes.data if N else None, feat.ctypes.data if N else None,
-                                  pos.ctypes.data if N else None, C.byref(n))
+    args = [buf.ctypes.data if buf.size else None, buf.size, len(image_names), blob.ctypes.data, off.ctypes.data, N,
+            img.ctypes.data if N else None, feat.ctypes.data if N else None, pos.ctypes.data if N else None, C.byref(n)]
+    if entries:
+        has = np.zeros(N, np.uint8)
+        rc = L.lfr_wire_join_solution_entries(*args, has.ctypes.data if N else None)
+    else:
+        rc = L.lfr_wire_join_solution(*args)
     if rc != 0:
         raise ParseError("Failed to parse proto object.")
-    return pos, int(n.value)
+    return (pos, int(n.value), has.astype(bool)) if entries else (pos, int(n.value))
