@@ -90,6 +90,23 @@ int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images
                                  const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
                                  uint64_t* n_outside);
 
+/* lfr_plan_encode_solution() merged with an earlier SolutionFile `file`: the scene's output, each scene
+ * image followed by its carried entries, then the file's other winning Image messages — the bytes of
+ * lfr_wire_encode_solution_carried() (include/lfr_wire.h, which states the rule) on the plan's host assembly
+ * (lfr_plan_download() and the assembly lfr_plan_encode_solution() describes).  A scene image is one with at
+ * least one node; a name among names / name_off without a node (every pair banned, no match) is not one,
+ * so the file's entries for it come after the scene images, as for a name outside the scene.  The file is
+ * decoded on the host (lfr_wire_decode_solution); keying, the stable sort, the winners, the join to the
+ * nodes, the compaction and the encoding of the N node records plus the carried ones run on the device.
+ * Size protocol, `stream` and *n_outside (the scene's nodes only) as lfr_plan_encode_solution();
+ * *n_carried (may be NULL) = the carried entries.  The plan is not changed.  LFR_EINVAL for malformed bytes,
+ * repeated image names, NULL arrays and a plan made by lfr_plan_create(); LFR_EUNSUPPORTED for 2^31 or
+ * more nodes plus displacements. */
+int64_t lfr_plan_encode_solution_carried(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                         const uint64_t* name_off, const float* fact, const uint8_t* file,
+                                         uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
+                                         uint64_t* n_carried);
+
 /* Hold images fixed in a plan made by lfr_plan_create_from_matches() or _from_wire(): every node of an
  * image k with fixed_by_image_id[k] != 0 (ids of lfr_host_input, n_images at least its n_images) becomes
  * constant, as a root is (solve.cc:135): it keeps its start value, gets no bounds, and a block between two

@@ -106,6 +106,30 @@ int lfr_wire_join_solution_entries(const uint8_t* buf, uint64_t len, uint32_t n_
                                    const uint32_t* node_feat, double* positions /* [2 n_nodes] */, uint64_t* n_started,
                                    uint8_t* has_entry /* [n_nodes] */);
 
+/* lfr_wire_encode_solution() of a scene's output (the same arrays: its images in output order, each with
+ * its displacements), merged with an earlier SolutionFile `file`, so that the output holds the whole scene
+ * when only part of it was solved again.  FILE's effective content follows the rule of
+ * lfr_wire_join_solution(): the last Image message of a name wins as a whole, within it the last
+ * displacement of a feature.  A carried entry is an effective (name, feature) of FILE that the scene has
+ * no displacement for under that name (names compared by their bytes).  The output is
+ *   1. every scene image in the given order, with its name, its fact and its displacements as given, then
+ *      its carried entries in ascending feature_idx;
+ *   2. then, for every winning Image message of FILE whose name is not a scene image's, in file order, one
+ *      Image with FILE's name bytes and fact and its effective entries in ascending feature_idx (a message
+ *      with no displacement gives an Image with none).
+ * Carried di / dj keep FILE's float bits (zero bit patterns are omitted, as always).  A scene image keeps
+ * the scene's fact: FILE's displacements are taken to be in the scene's units, and are not converted.
+ * With an empty file the bytes are lfr_wire_encode_solution()'s.  Returns the bytes needed and writes them
+ * only when cap is at least that; *n_carried (may be NULL) = the carried entries, of both groups.
+ * LFR_EINVAL for bytes lfr_wire_decode_solution() rejects, repeated scene image names, NULL arrays or
+ * descending img_ptr / name_off. */
+int64_t lfr_wire_encode_solution_carried(uint64_t n_images, const uint64_t* img_ptr,
+                                         const uint8_t* names, const uint64_t* name_off,
+                                         const float* fact, const uint32_t* feature_idx,
+                                         const float* di, const float* dj,
+                                         const uint8_t* file, uint64_t file_len,
+                                         uint8_t* out, uint64_t cap, uint64_t* n_carried);
+
 #ifdef __cplusplus
 }
 #endif

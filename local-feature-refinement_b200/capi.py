@@ -81,7 +81,8 @@ ABI_SYMBOLS = [
 #: the symbols include/lfr_graph.h declares
 GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
                  "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
-                 "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution"]
+                 "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution",
+                 "lfr_plan_encode_solution_carried"]
 
 
 class LfrWirePart(C.Structure):
@@ -161,6 +162,10 @@ class Library:
             L.lfr_plan_start_from_solution.restype = C.c_int
             L.lfr_plan_keep_solution.argtypes = L.lfr_plan_start_from_solution.argtypes
             L.lfr_plan_keep_solution.restype = C.c_int
+            L.lfr_plan_encode_solution_carried.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                           C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
+                                                           C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+            L.lfr_plan_encode_solution_carried.restype = C.c_int64
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -452,6 +457,34 @@ class Plan:
         if got != need:
             self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution")
         return out[:need].tobytes(), int(n_out.value)
+
+    def encode_solution_carried(self, image_names, image_fact, carry: bytes, stream: int = 0):
+        """lfr_plan_encode_solution_carried (include/lfr_graph.h): encode_solution() merged on the device with the
+        earlier SolutionFile `carry`, as wire.encode_solution_carried() merges the host assembly.  Returns
+        (bytes, n_outside, n_carried); n_outside counts the scene's nodes only."""
+        from .wire import _names_blob
+        blob, off = _names_blob(list(image_names))
+        fact = np.ascontiguousarray(image_fact, dtype=np.float32).reshape(-1)
+        if fact.shape[0] != len(image_names):
+            raise ValueError("image_fact has %d entries for %d image names" % (fact.shape[0], len(image_names)))
+        buf = np.frombuffer(carry, dtype=np.uint8)
+        f = self.lib.lib.lfr_plan_encode_solution_carried
+        n_out, n_car = C.c_uint64(), C.c_uint64()
+        args = (self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data, _ptr(fact),
+                buf.ctypes.data if buf.size else None, buf.size)
+        # one call into a buffer of the scene's largest encoding plus the file's size (what a canonical file
+        # can add); a larger need takes a second call
+        cap = 18 * self.n_nodes + int(off[-1]) + 27 * len(image_names) + buf.size
+        out = np.empty(max(cap, 1), np.uint8)
+        need = f(*args, out.ctypes.data, cap, C.byref(n_out), C.byref(n_car))
+        if need < 0:
+            self.lib.check(int(need), "lfr_plan_encode_solution_carried")
+        if need > cap:
+            out = np.empty(int(need), np.uint8)
+            got = f(*args, out.ctypes.data, int(need), C.byref(n_out), C.byref(n_car))
+            if got != need:
+                self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution_carried")
+        return out[:need].tobytes(), int(n_out.value), int(n_car.value)
 
     def fix_images(self, fixed_by_image_id) -> None:
         """lfr_plan_fix_images (include/lfr_graph.h): hold every node of the images with a non-zero entry of

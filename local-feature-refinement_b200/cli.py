@@ -14,6 +14,8 @@ custom_demo.py:101-105 run unchanged.  `--n_threads` is accepted and ignored
 --initial_solution FILE (start values from a SolutionFile instead of zeros): together they refine new
 images against an already-refined scene.  --keep_initial_solution (with --initial_solution) also holds
 every keypoint that has an entry in that file constant, and refines only the others.
+--carry_initial_solution (with --initial_solution) writes the whole scene: the output also holds every entry
+of that file the solve does not refine (wire.encode_solution_carried), so new pairs alone can be solved.
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -49,7 +51,7 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("n_threads", True, False), ("banned_images", True, True),
             ("device", True, False), ("gpus", True, False), ("stats_json", True, False),
             ("fixed_images", True, True), ("initial_solution", True, False),
-            ("keep_initial_solution", False, False)]
+            ("keep_initial_solution", False, False), ("carry_initial_solution", False, False)]
 
 
 def _find_option(name):
@@ -124,7 +126,8 @@ def parse_args(argv):
             n_threads=_as_uint(vals, "n_threads", 8), banned_images=vals.get("banned_images", []),
             device=_as_uint(vals, "device", 0), gpus=_as_uint(vals, "gpus", 1), stats_json=vals.get("stats_json"),
             fixed_images=vals.get("fixed_images", []), initial_solution=vals.get("initial_solution"),
-            keep_initial_solution=bool(vals.get("keep_initial_solution")))
+            keep_initial_solution=bool(vals.get("keep_initial_solution")),
+            carry_initial_solution=bool(vals.get("carry_initial_solution")))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -142,6 +145,9 @@ def main(argv=None) -> int:
     # the start solution is read and checked before any other work: its errors come before any output
     if args.keep_initial_solution and not args.initial_solution:
         sys.stderr.write("ERROR: --keep_initial_solution needs --initial_solution FILE\n")
+        return 2
+    if args.carry_initial_solution and not args.initial_solution:
+        sys.stderr.write("ERROR: --carry_initial_solution needs --initial_solution FILE\n")
         return 2
     start = None
     if args.initial_solution is not None:
@@ -217,7 +223,11 @@ def main(argv=None) -> int:
     if rank != 0:
         return 0
     try:
-        data = wire.encode_solution(sol.image_names, sol.fact, sol.img_ptr, sol.feature_idx, sol.di, sol.dj)
+        if args.carry_initial_solution:
+            data, _ = wire.encode_solution_carried(sol.image_names, sol.fact, sol.img_ptr, sol.feature_idx, sol.di,
+                                                   sol.dj, start)
+        else:
+            data = wire.encode_solution(sol.image_names, sol.fact, sol.img_ptr, sol.feature_idx, sol.di, sol.dj)
         with open(args.output_file, "wb") as fh:
             fh.write(data)
     except OSError:

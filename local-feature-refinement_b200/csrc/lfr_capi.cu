@@ -11,9 +11,11 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/lfr_graph.h"
+#include "lfr_carry.cuh"
 #include "lfr_cut.h"
 #include "lfr_cut.cuh"
 #include "lfr_graph.cuh"
@@ -2205,6 +2207,162 @@ int join_solution(lfr_plan* pl, cudaStream_t s, const lfr::join::Decoded& d, uin
   return LFR_OK;
 }
 
+// lfr_plan_encode_solution_carried() on a checked plan and arguments and the decoded file (lfr_carry.cuh):
+// the scene images' ranks and the entries' join on the device, one synchronisation for the carried count,
+// the record and image sizes, one for the total, then — when `out` has room — the writing kernels and one
+// copy to `out`
+int64_t encode_solution_carried(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t* names, const uint64_t* name_off,
+                                const float* fact, const uint8_t* file, const lfr::join::Decoded& d, uint8_t* out,
+                                uint64_t cap, uint64_t* n_outside, uint64_t* n_carried) {
+  using namespace lfr::carry;
+  const uint32_t N = pl->N, D = (uint32_t)d.n_disp, I = (uint32_t)d.n_images;
+  if (n_outside) *n_outside = 0;
+  if (n_carried) *n_carried = 0;
+  // per message: its key image (the scene id of a matched winner, n_images + j for the j-th other winner,
+  // kNoImage for a message that loses to a later one of its name), and the winners' names and facts
+  std::vector<uint32_t> msg_pid(I, kNoImage);
+  std::vector<uint64_t> msg_name_off((size_t)I + 1, 0);
+  std::vector<uint8_t> msg_names;
+  uint64_t n_other = 0;
+  for (uint32_t i = 0; i < I; ++i) {
+    if (d.wins[i]) {
+      msg_pid[i] = d.image_id[i] != lfr::join::kNoImage ? d.image_id[i] : (uint32_t)(NI + n_other++);
+      msg_names.insert(msg_names.end(), file + d.name_off[i], file + d.name_off[i] + d.name_len[i]);
+    }
+    msg_name_off[(size_t)i + 1] = msg_names.size();
+  }
+  if ((uint64_t)NI + n_other >= kNoImage) return fail(LFR_EUNSUPPORTED, "too many images in the scene and the SolutionFile");
+  const uint64_t name_bytes = name_off[NI], msg_name_bytes = msg_names.size();
+  const uint32_t n_max = NI + I;  // an upper bound of the output images
+  size_t at = 0;
+  auto take = [&at](size_t bytes) {
+    const size_t o = at;
+    at += (bytes + 255) & ~(size_t)255;
+    return o;
+  };
+  // per scene image, per message, per entry, then per record (N + at most D) and per output image
+  const size_t o_ctr = take(16), o_first = take(4 * (size_t)NI), o_first_s = take(4 * (size_t)NI),
+               o_iota_i = take(4 * (size_t)NI), o_img_s = take(4 * (size_t)NI), o_rank = take(4 * (size_t)NI),
+               o_name_off = take(8 * ((size_t)NI + 1)), o_fact = take(4 * (size_t)NI), o_names = take(name_bytes),
+               o_mptr = take(8 * ((size_t)I + 1)), o_mpid = take(4 * (size_t)I + 4), o_mnoff = take(8 * ((size_t)I + 1)),
+               o_mfact = take(4 * (size_t)I + 4), o_mnames = take(msg_name_bytes), o_g2 = take(4 * ((size_t)I + 1)),
+               o_g2_off = take(4 * ((size_t)I + 1)), o_g2_msg = take(4 * (size_t)I + 4), o_feat = take(4 * (size_t)D),
+               o_di = take(4 * (size_t)D), o_dj = take(4 * (size_t)D), o_key = take(8 * (size_t)D),
+               o_key_s = take(8 * (size_t)D), o_idx = take(4 * (size_t)D), o_idx_s = take(4 * (size_t)D),
+               o_used = take(D), o_flag = take(4 * ((size_t)D + 1)), o_slot = take(4 * ((size_t)D + 1)),
+               o_ce = take(4 * (size_t)D), o_cm = take(4 * (size_t)D), o_rkey = take(4 * ((size_t)N + D)),
+               o_rkey_s = take(4 * ((size_t)N + D)), o_riota = take(4 * ((size_t)N + D)), o_perm = take(4 * ((size_t)N + D)),
+               o_rsize = take(8 * ((size_t)N + D + 1)), o_roff = take(8 * ((size_t)N + D + 1)),
+               o_iend = take(4 * ((size_t)n_max + 1)), o_body = take(8 * ((size_t)n_max + 1)),
+               o_isize = take(8 * ((size_t)n_max + 1)), o_ioff = take(8 * ((size_t)n_max + 1));
+  LFR_TRY(pl->enc_scratch.reserve(at));
+  uint8_t* base = pl->enc_scratch.as<uint8_t>();
+  auto u32 = [base](size_t o) { return reinterpret_cast<uint32_t*>(base + o); };
+  auto u64 = [base](size_t o) { return reinterpret_cast<uint64_t*>(base + o); };
+  auto f32 = [base](size_t o) { return reinterpret_cast<float*>(base + o); };
+  auto* d_outside = reinterpret_cast<unsigned long long*>(base + o_ctr);
+  uint32_t* n_present = u32(o_ctr + 8);
+  uint32_t *first = u32(o_first), *first_s = u32(o_first_s), *iota_i = u32(o_iota_i), *img_s = u32(o_img_s),
+           *rank = u32(o_rank), *mpid = u32(o_mpid), *g2 = u32(o_g2), *g2_off = u32(o_g2_off), *g2_msg = u32(o_g2_msg),
+           *feat = u32(o_feat), *idx = u32(o_idx), *idx_s = u32(o_idx_s), *flag = u32(o_flag), *slot = u32(o_slot),
+           *ce = u32(o_ce), *cm = u32(o_cm), *rkey = u32(o_rkey), *rkey_s = u32(o_rkey_s), *riota = u32(o_riota),
+           *perm = u32(o_perm), *iend = u32(o_iend);
+  uint64_t *d_name_off = u64(o_name_off), *mptr = u64(o_mptr), *mnoff = u64(o_mnoff), *rsize = u64(o_rsize),
+           *roff = u64(o_roff), *body = u64(o_body), *isize = u64(o_isize), *ioff = u64(o_ioff);
+  auto* key = reinterpret_cast<unsigned long long*>(base + o_key);
+  auto* key_s = reinterpret_cast<unsigned long long*>(base + o_key_s);
+  float *d_fact = f32(o_fact), *mfact = f32(o_mfact), *di = f32(o_di), *dj = f32(o_dj);
+  uint8_t *d_names = base + o_names, *mnames = base + o_mnames, *used = base + o_used;
+  const uint32_t* nimg = pl->node_image.as<uint32_t>();
+  const uint32_t* nfeat = pl->node_feat.as<uint32_t>();
+  const double* pos = pl->pos.as<double>();
+
+  LFR_CUDA(cudaMemsetAsync(base + o_ctr, 0, 16, s));
+  LFR_CUDA(cudaMemcpyAsync(d_name_off, name_off, 8 * ((size_t)NI + 1), cudaMemcpyHostToDevice, s));
+  if (NI) LFR_CUDA(cudaMemcpyAsync(d_fact, fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
+  if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, names, name_bytes, cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemcpyAsync(mptr, d.img_ptr.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemcpyAsync(mnoff, msg_name_off.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
+  if (I) {
+    LFR_CUDA(cudaMemcpyAsync(mpid, msg_pid.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(mfact, d.fact.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
+  }
+  if (msg_name_bytes) LFR_CUDA(cudaMemcpyAsync(mnames, msg_names.data(), msg_name_bytes, cudaMemcpyHostToDevice, s));
+  // the present scene images and their ranks, as lfr_plan_encode_solution() ranks them
+  if (NI) {
+    lfr::solution::init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
+    if (N) lfr::solution::first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, first, first_s, iota_i, img_s, (int)NI, 0, bits_for(N), s);
+    }));
+    lfr::solution::rank_kernel<<<blocks_for(NI), 256, 0, s>>>(first_s, img_s, NI, N, rank, n_present);
+    LFR_LAUNCHED();
+  }
+  // the entries: keyed, sorted stably, joined to the nodes, the carried ones compacted
+  uint32_t C = 0;
+  if (D) {
+    LFR_CUDA(cudaMemcpyAsync(feat, d.feature_idx.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(di, d.di.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(dj, d.dj.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemsetAsync(used, 0, D, s));
+    lfr::start::solution_key_kernel<<<blocks_for(D), 256, 0, s>>>(mptr, mpid, I, feat, D, key, idx);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: equal keys stay in file order
+      return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, idx, idx_s, (int)D, 0, 64, s);
+    }));
+    if (N) consume_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, nfeat, N, key_s, D, used);
+    carry_flag_kernel<<<blocks_for((uint64_t)D + 1), 256, 0, s>>>(key_s, used, D, flag);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, flag, slot, (int)D + 1, s); }));
+    carry_compact_kernel<<<blocks_for(D), 256, 0, s>>>(flag, slot, idx_s, mptr, I, D, ce, cm);
+    LFR_LAUNCHED();
+    LFR_TRY(fetch(&C, slot + D, 1, s));
+  }
+  // the other winning messages, ranked after the present scene images in file order
+  group2_flag_kernel<<<blocks_for((uint64_t)I + 1), 256, 0, s>>>(mpid, I, first, NI, N, g2);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, g2, g2_off, (int)I + 1, s); }));
+  if (I) {
+    group2_scatter_kernel<<<blocks_for(I), 256, 0, s>>>(g2, g2_off, I, g2_msg);
+    LFR_LAUNCHED();
+  }
+  // the records (nodes, then carried entries) in output order, their sizes and the images'
+  const uint32_t R = N + C;
+  if (R) {
+    record_key_kernel<<<blocks_for(R), 256, 0, s>>>(nimg, rank, N, cm, mpid, g2, g2_off, n_present, R, rkey, riota);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: nodes by index, then carried entries by feature
+      return cub::DeviceRadixSort::SortPairs(t, nb, rkey, rkey_s, riota, perm, (int)R, 0, bits_for(n_max), s);
+    }));
+  }
+  record_size_kernel<<<blocks_for((uint64_t)R + 1), 256, 0, s>>>(perm, R, N, nfeat, pos, ce, feat, di, dj, rsize);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, roff, (int)R + 1, s); }));
+  image_size_kernel<<<blocks_for((uint64_t)n_max + 1), 256, 0, s>>>(rkey_s, R, roff, n_present, g2_off, I, img_s, d_names,
+                                                                     d_name_off, d_fact, g2_msg, mnames, mnoff, mfact, n_max,
+                                                                     iend, body, isize);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)n_max + 1, s); }));
+  uint64_t total = 0;
+  unsigned long long outside = 0;
+  LFR_CUDA(cudaMemcpyAsync(&outside, d_outside, 8, cudaMemcpyDeviceToHost, s));
+  LFR_TRY(fetch(&total, ioff + n_max, 1, s));
+  if (n_outside) *n_outside = outside;
+  if (n_carried) *n_carried = C;
+  if (!out || cap < total || !total) return (int64_t)total;
+  LFR_TRY(pl->enc_out.reserve(total));
+  uint8_t* d_out = pl->enc_out.as<uint8_t>();
+  if (n_max)
+    write_images_kernel<<<blocks_for(n_max), 256, 0, s>>>(n_present, g2_off, I, img_s, d_names, d_name_off, d_fact, g2_msg,
+                                                           mnames, mnoff, mfact, body, ioff, n_max, d_out);
+  if (R)
+    write_records_kernel<<<blocks_for(R), 256, 0, s>>>(perm, rkey_s, R, N, nfeat, pos, ce, feat, di, dj, iend, roff, ioff, d_out);
+  LFR_LAUNCHED();
+  LFR_TRY(fetch(out, d_out, total, s));
+  return (int64_t)total;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2384,6 +2542,27 @@ int lfr_plan_keep_solution(lfr_plan* pl, void* stream, const uint8_t* bytes, uin
   }
   LFR_TRY(join_solution(pl, s, d, pl->kept.as<uint8_t>(), n_kept));
   return build_constant_mask(pl, s);
+}
+
+int64_t lfr_plan_encode_solution_carried(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
+                                         const uint64_t* name_off, const float* fact, const uint8_t* file,
+                                         uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
+                                         uint64_t* n_carried) {
+  lfr::join::Decoded d;
+  LFR_TRY(decode_solution_for(pl, file, file_len, n_images, names, name_off, d));
+  if (n_images && !fact) return fail(LFR_EINVAL, "NULL image facts");
+  {
+    const char* nm = names ? reinterpret_cast<const char*>(names) : "";
+    std::unordered_set<std::string> seen;
+    seen.reserve(n_images);
+    for (uint32_t k = 0; k < n_images; ++k)
+      if (!seen.emplace(nm + name_off[k], name_off[k + 1] - name_off[k]).second)
+        return fail(LFR_EINVAL, "repeated image name");
+  }
+  if ((uint64_t)pl->N + d.n_disp >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "2^31 or more nodes and displacements");
+  LFR_CUDA(cudaSetDevice(pl->device));
+  return encode_solution_carried(pl, (cudaStream_t)stream, n_images, names, name_off, fact, file, d, out, cap, n_outside,
+                                 n_carried);
 }
 
 int lfr_debug_last_encode_times(double* out2) {

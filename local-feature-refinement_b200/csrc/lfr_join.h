@@ -1,6 +1,7 @@
 // lfr_join.h — the host half of a start point read from a SolutionFile (types.proto:30-46), shared by the
-// host joins (lfr_wire_join_solution and _entries, lfr_wire.cc) and the device join
-// (lfr_plan_start_from_solution and lfr_plan_keep_solution, lfr_capi.cu): the decode with
+// host joins (lfr_wire_join_solution and _entries, lfr_wire.cc), the device join
+// (lfr_plan_start_from_solution and lfr_plan_keep_solution, lfr_capi.cu) and the carried encoders
+// (lfr_wire_encode_solution_carried, lfr_plan_encode_solution_carried): the decode with
 // lfr_wire_decode_solution() and the image rule, and the host joins' node loop.  Header-only host code.
 //
 // The rule is that of the reference's own reader (reconstruction-scripts/colmap_utils.py:104-137): an
@@ -37,6 +38,9 @@ struct Decoded {
   // per decoded Image message: the scene image id its displacements belong to, or kNoImage (a name not in
   // the scene, or a later message with the same name)
   std::vector<uint32_t> image_id;
+  // per decoded Image message: 1 when it is the last one with its name (it wins as a whole), whether or not
+  // the name is a scene image's
+  std::vector<uint8_t> wins;
 };
 
 // Decode `buf` and resolve its images against the scene's names (name k = names[name_off[k], name_off[k+1])).
@@ -61,15 +65,30 @@ inline int decode(const uint8_t* buf, uint64_t len, uint32_t n_images, const uin
   id_of.reserve(n_images);
   for (uint32_t k = 0; k < n_images; ++k)
     id_of.emplace(std::string(reinterpret_cast<const char*>(names) + name_off[k], name_off[k + 1] - name_off[k]), k);
+  std::unordered_map<std::string, uint64_t> last;  // the last Image message of each name in the file
+  last.reserve(I);
+  for (uint64_t i = 0; i < I; ++i)
+    last[std::string(reinterpret_cast<const char*>(buf) + d.name_off[i], d.name_len[i])] = i;
   d.image_id.assign(I, kNoImage);
-  std::vector<uint64_t> winner(n_images, ~0ull);  // last Image message of each scene image
-  for (uint64_t i = 0; i < I; ++i) {
-    const auto it = id_of.find(std::string(reinterpret_cast<const char*>(buf) + d.name_off[i], d.name_len[i]));
-    if (it != id_of.end()) winner[it->second] = i;
+  d.wins.assign(I, 0);
+  for (const auto& nl : last) {
+    d.wins[nl.second] = 1;
+    const auto it = id_of.find(nl.first);
+    if (it != id_of.end()) d.image_id[nl.second] = it->second;
   }
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (winner[k] != ~0ull) d.image_id[winner[k]] = k;
   return LFR_OK;
+}
+
+// The effective entries of decoded Image message i: the last displacement of each feature, in ascending
+// feature_idx (indices into d.feature_idx / di / dj).
+inline void effective_entries(const Decoded& d, uint64_t i, std::vector<uint64_t>& out) {
+  out.clear();
+  for (uint64_t k = d.img_ptr[i]; k < d.img_ptr[i + 1]; ++k) out.push_back(k);
+  std::stable_sort(out.begin(), out.end(), [&d](uint64_t a, uint64_t b) { return d.feature_idx[a] < d.feature_idx[b]; });
+  size_t w = 0;
+  for (size_t j = 0; j < out.size(); ++j)
+    if (j + 1 == out.size() || d.feature_idx[out[j + 1]] != d.feature_idx[out[j]]) out[w++] = out[j];
+  out.resize(w);
 }
 
 // The host join (lfr_wire_join_solution / _entries): positions[2v .. 2v+1] from node v's entry, 0 without

@@ -23,7 +23,10 @@
 // --initial_solution FILE (start values from a SolutionFile instead of zeros), with
 // --keep_initial_solution (every keypoint with an entry in that file is held constant too) — on the device
 // route lfr_plan_fix_images() / lfr_plan_start_from_solution() or lfr_plan_keep_solution(), on the host
-// route the constant mask and lfr_wire_join_solution() or _entries() handed to the solve.  `--n_threads` is accepted and
+// route the constant mask and lfr_wire_join_solution() or _entries() handed to the solve — and
+// --carry_initial_solution (the output also holds every entry of that file the scene does not refine:
+// lfr_plan_encode_solution_carried() on the device route, lfr_wire_encode_solution_carried() on the host
+// route's assembly).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -67,6 +70,10 @@ int lfr_plan_start_from_solution(lfr_plan* plan, void* stream, const uint8_t* by
                                  const uint8_t* names, const uint64_t* name_off, uint64_t* n_started) __attribute__((weak));
 int lfr_plan_keep_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                            const uint8_t* names, const uint64_t* name_off, uint64_t* n_kept) __attribute__((weak));
+int64_t lfr_plan_encode_solution_carried(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                         const uint64_t* name_off, const float* fact, const uint8_t* file,
+                                         uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
+                                         uint64_t* n_carried) __attribute__((weak));
 }
 
 namespace {
@@ -91,7 +98,7 @@ struct OptionSpec {
 const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", true, false}, {"output_file", true, false},
                                {"n_threads", true, false},    {"banned_images", true, true}, {"device", true, false},
                                {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false},
-                               {"keep_initial_solution", false, false}};
+                               {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -110,7 +117,7 @@ const OptionSpec& find_option(const std::string& name) {
 }
 
 struct Args {
-  bool help = false, keep_initial_solution = false;
+  bool help = false, keep_initial_solution = false, carry_initial_solution = false;
   std::map<std::string, std::string> single;
   std::map<std::string, std::vector<std::string>> repeated;
 };
@@ -143,7 +150,9 @@ Args parse(int argc, char** argv) {
         }
       } else {
         if (eq != std::string::npos) throw CliError{std::string("option '--") + o.name + "' does not take any arguments"};
-        (std::strcmp(o.name, "help") == 0 ? a.help : a.keep_initial_solution) = true;
+        (std::strcmp(o.name, "help") == 0 ? a.help
+         : std::strcmp(o.name, "keep_initial_solution") == 0 ? a.keep_initial_solution
+                                                             : a.carry_initial_solution) = true;
       }
     } else if (tok.size() > 1 && tok[0] == '-') {
       throw CliError{"unrecognised option '" + tok + "'"};
@@ -234,7 +243,7 @@ int main(int argc, char** argv) {
   std::string matches_file, output_file, initial_solution;
   std::vector<std::string> banned_list, fixed_list;
   uint64_t device = 0, gpus = 1;
-  bool keep_start = false;
+  bool keep_start = false, carry_start = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -253,6 +262,7 @@ int main(int argc, char** argv) {
     fixed_list = a.repeated["fixed_images"];
     if (a.single.count("initial_solution")) initial_solution = a.single.at("initial_solution");
     keep_start = a.keep_initial_solution;
+    carry_start = a.carry_initial_solution;
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
@@ -264,6 +274,10 @@ int main(int argc, char** argv) {
   const bool have_start = !initial_solution.empty();
   if (keep_start && !have_start) {
     std::fputs("ERROR: --keep_initial_solution needs --initial_solution FILE\n", stderr);
+    return 2;
+  }
+  if (carry_start && !have_start) {
+    std::fputs("ERROR: --carry_initial_solution needs --initial_solution FILE\n", stderr);
     return 2;
   }
   if (have_start) {
@@ -397,7 +411,7 @@ int main(int argc, char** argv) {
   // takes the host route; forcing the device route there is an error, never a silent host run.
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
-                                 lfr_plan_start_from_solution && lfr_plan_keep_solution;
+                                 lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -549,7 +563,7 @@ int main(int argc, char** argv) {
         is_const[v] = (is_root[v] || fixed[node_image[v]] || (keep_start && has_entry[v])) ? 1 : 0;
     }
   }
-  start_file.release();
+  if (!carry_start) start_file.release();  // carried into the output otherwise
   const Clock::time_point t_solve = Clock::now();
   if (N && plan) {
     int rc = lfr_plan_solve(plan, nullptr);
@@ -595,11 +609,27 @@ int main(int argc, char** argv) {
     // largest encoding: a Displacement record is at most 18 bytes, an Image's header 16 plus its name field
     uint64_t cap = 18ull * N;
     for (size_t i = 0; i < names.size(); ++i) cap += 16 + 11 + names[i].size();
+    // carried entries: a file's canonical encoding bounds what it adds; a larger need takes a second call
+    if (carry_start) cap += start_file.size();
+    auto encode = [&](uint8_t* o, uint64_t c) {
+      return carry_start ? lfr_plan_encode_solution_carried(plan, nullptr, (uint32_t)names.size(), name_blob.data(),
+                                                            name_off.data(), image_fact.data(), start_file.data(),
+                                                            start_file.size(), o, c, &n_outside, nullptr)
+                         : lfr_plan_encode_solution(plan, nullptr, (uint32_t)names.size(), name_blob.data(), name_off.data(),
+                                                    image_fact.data(), o, c, &n_outside);
+    };
     out = static_cast<uint8_t*>(lfr_host_alloc(cap));
     out_pinned = out != nullptr;
     if (!out) out = static_cast<uint8_t*>(std::malloc(cap ? cap : 1));
-    need = lfr_plan_encode_solution(plan, nullptr, (uint32_t)names.size(), name_blob.data(), name_off.data(),
-                                    image_fact.data(), out, cap, &n_outside);
+    need = encode(out, cap);
+    if (need > 0 && (uint64_t)need > cap) {
+      if (out_pinned) lfr_host_free(out); else std::free(out);
+      cap = (uint64_t)need;
+      out = static_cast<uint8_t*>(lfr_host_alloc(cap));
+      out_pinned = out != nullptr;
+      if (!out) out = static_cast<uint8_t*>(std::malloc(cap));
+      need = encode(out, cap);
+    }
     lfr_plan_destroy(plan);
     if (need < 0 || (uint64_t)need > cap) {
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", (int)need, lfr_last_error());
@@ -639,13 +669,18 @@ int main(int argc, char** argv) {
       fact[i] = image_fact[img_ids[i]];
     }
     if (out_blob.empty()) out_blob.push_back(0);
-    need = lfr_wire_encode_solution(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
-                                    feature_idx.data(), di.data(), dj.data(), nullptr, 0);
+    auto encode = [&](uint8_t* o, uint64_t c) {
+      return carry_start ? lfr_wire_encode_solution_carried(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
+                                                            feature_idx.data(), di.data(), dj.data(), start_file.data(),
+                                                            start_file.size(), o, c, nullptr)
+                         : lfr_wire_encode_solution(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
+                                                    feature_idx.data(), di.data(), dj.data(), o, c);
+    };
+    need = encode(nullptr, 0);
     out = static_cast<uint8_t*>(std::malloc((size_t)std::max<int64_t>(need, 1)));
-    if (need < 0 || lfr_wire_encode_solution(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
-                                             feature_idx.data(), di.data(), dj.data(), out, (uint64_t)need) != need)
-      need = -1;
+    if (need < 0 || encode(out, (uint64_t)need) != need) need = -1;
   }
+  start_file.release();
   std::printf("# points with at least one coordinate > 0.5: %llu\n", (unsigned long long)n_outside);  // solve.cc:670
   std::fflush(stdout);
   bool written = need >= 0;

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <thread>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/lfr.h"
@@ -455,6 +456,83 @@ int lfr_wire_join_solution_entries(const uint8_t* buf, uint64_t len, uint32_t n_
   if (n_nodes && !has_entry) return LFR_EINVAL;
   return lfr::join::join_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions, has_entry,
                                n_started);
+}
+
+int64_t lfr_wire_encode_solution_carried(uint64_t n_images, const uint64_t* img_ptr, const uint8_t* names,
+                                         const uint64_t* name_off, const float* fact, const uint32_t* feature_idx,
+                                         const float* di, const float* dj, const uint8_t* file, uint64_t file_len,
+                                         uint8_t* out, uint64_t cap, uint64_t* n_carried) {
+  if (!img_ptr || !name_off || (n_images && !fact) || (!file && file_len) || n_images >= lfr::join::kNoImage)
+    return LFR_EINVAL;
+  for (uint64_t i = 0; i < n_images; ++i)
+    if (img_ptr[i + 1] < img_ptr[i] || name_off[i + 1] < name_off[i]) return LFR_EINVAL;
+  if ((name_off[n_images] && !names) || (img_ptr[n_images] && (!feature_idx || !di || !dj))) return LFR_EINVAL;
+  const uint8_t no_name = 0;
+  const uint8_t* nm = names ? names : &no_name;
+  {
+    std::unordered_set<std::string> seen;
+    seen.reserve(n_images);
+    for (uint64_t i = 0; i < n_images; ++i)
+      if (!seen.emplace(reinterpret_cast<const char*>(nm) + name_off[i], name_off[i + 1] - name_off[i]).second)
+        return LFR_EINVAL;  // a repeated scene image name
+  }
+  lfr::join::Decoded d;
+  if (lfr::join::decode(file, file_len, (uint32_t)n_images, nm, name_off, d) != LFR_OK) return LFR_EINVAL;
+  std::vector<uint64_t> msg_of(n_images, ~0ull);  // the winning message of each scene image
+  for (uint64_t i = 0; i < d.n_images; ++i)
+    if (d.image_id[i] != lfr::join::kNoImage) msg_of[d.image_id[i]] = i;
+  // the output assembly: scene images with their displacements and then their carried entries, then the
+  // winning messages of other names in file order; one lfr_wire_encode_solution() call writes it
+  std::vector<uint64_t> o_ptr(1, 0), o_off(1, 0);
+  std::vector<uint8_t> o_names;
+  std::vector<float> o_fact, o_di, o_dj;
+  std::vector<uint32_t> o_feat;
+  std::vector<uint64_t> eff;
+  std::vector<uint32_t> scene_feats;
+  uint64_t carried = 0;
+  auto put_name = [&](const uint8_t* p, uint64_t len, float f) {
+    o_names.insert(o_names.end(), p, p + len);
+    o_off.push_back(o_names.size());
+    o_fact.push_back(f);
+  };
+  auto put_entry = [&](uint32_t f, float a, float b) {
+    o_feat.push_back(f);
+    o_di.push_back(a);
+    o_dj.push_back(b);
+  };
+  for (uint64_t i = 0; i < n_images; ++i) {
+    put_name(nm + name_off[i], name_off[i + 1] - name_off[i], fact[i]);
+    for (uint64_t k = img_ptr[i]; k < img_ptr[i + 1]; ++k) put_entry(feature_idx[k], di[k], dj[k]);
+    if (msg_of[i] != ~0ull) {
+      scene_feats.assign(feature_idx + img_ptr[i], feature_idx + img_ptr[i + 1]);
+      std::sort(scene_feats.begin(), scene_feats.end());
+      lfr::join::effective_entries(d, msg_of[i], eff);
+      for (uint64_t e : eff)
+        if (!std::binary_search(scene_feats.begin(), scene_feats.end(), d.feature_idx[e])) {
+          put_entry(d.feature_idx[e], d.di[e], d.dj[e]);
+          ++carried;
+        }
+    }
+    o_ptr.push_back(o_feat.size());
+  }
+  for (uint64_t i = 0; i < d.n_images; ++i) {
+    if (!d.wins[i] || d.image_id[i] != lfr::join::kNoImage) continue;
+    put_name(file + d.name_off[i], d.name_len[i], d.fact[i]);
+    lfr::join::effective_entries(d, i, eff);
+    for (uint64_t e : eff) put_entry(d.feature_idx[e], d.di[e], d.dj[e]);
+    carried += eff.size();
+    o_ptr.push_back(o_feat.size());
+  }
+  if (o_names.empty()) o_names.push_back(0);
+  if (o_feat.empty()) put_entry(0, 0.f, 0.f);  // a valid pointer for every array; o_ptr does not reach it
+  const uint64_t I = o_fact.size();
+  const int64_t need = lfr_wire_encode_solution(I, o_ptr.data(), o_names.data(), o_off.data(), o_fact.data(), o_feat.data(),
+                                                o_di.data(), o_dj.data(), nullptr, 0);
+  if (out && cap >= (uint64_t)need)
+    lfr_wire_encode_solution(I, o_ptr.data(), o_names.data(), o_off.data(), o_fact.data(), o_feat.data(), o_di.data(),
+                             o_dj.data(), out, cap);
+  if (n_carried) *n_carried = carried;
+  return need;
 }
 
 }  // extern "C"

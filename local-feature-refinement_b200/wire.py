@@ -28,7 +28,7 @@ class WireMatches(C.Structure):
 
 WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
                 "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution",
-                "lfr_wire_join_solution_entries"]
+                "lfr_wire_join_solution_entries", "lfr_wire_encode_solution_carried"]
 
 _bound = False
 
@@ -55,6 +55,9 @@ def _lib():
         L.lfr_wire_join_solution.restype = C.c_int
         L.lfr_wire_join_solution_entries.argtypes = L.lfr_wire_join_solution.argtypes + [C.c_void_p]
         L.lfr_wire_join_solution_entries.restype = C.c_int
+        L.lfr_wire_encode_solution_carried.argtypes = ([C.c_uint64] + [C.c_void_p] * 7 + [C.c_void_p, C.c_uint64, C.c_void_p,
+                                                        C.c_uint64, C.POINTER(C.c_uint64)])
+        L.lfr_wire_encode_solution_carried.restype = C.c_int64
         _bound = True
     return L
 
@@ -213,6 +216,33 @@ def encode_solution(image_names: List[str], fact: np.ndarray, img_ptr: np.ndarra
     got = L.lfr_wire_encode_solution(len(image_names), *ptrs, out.ctypes.data, int(need))
     assert got == need
     return out[:need].tobytes()
+
+
+def encode_solution_carried(image_names: List[str], fact: np.ndarray, img_ptr: np.ndarray, feature_idx: np.ndarray,
+                            di: np.ndarray, dj: np.ndarray, carry: bytes):
+    """encode_solution() of a scene's output merged with the earlier SolutionFile `carry`
+    (lfr_wire_encode_solution_carried, include/lfr_wire.h): each scene image gets, after its displacements,
+    the entries `carry` has for it and the scene does not (ascending feature); then come the winning Image
+    messages of `carry` whose names are not scene images, in file order.  Returns (bytes, number of carried
+    entries).  Raises ParseError on bytes the decoder rejects and ValueError on repeated image names."""
+    L = _lib()
+    blob, off = _names_blob(image_names)
+    arrs = [np.ascontiguousarray(img_ptr, np.uint64), blob, off, np.ascontiguousarray(fact, np.float32),
+            np.ascontiguousarray(feature_idx, np.uint32), np.ascontiguousarray(di, np.float32),
+            np.ascontiguousarray(dj, np.float32)]
+    ptrs = [x.ctypes.data for x in arrs]
+    buf = np.frombuffer(carry, dtype=np.uint8)
+    fptr = buf.ctypes.data if buf.size else None
+    n = C.c_uint64()
+    need = int(L.lfr_wire_encode_solution_carried(len(image_names), *ptrs, fptr, buf.size, None, 0, C.byref(n)))
+    if need < 0:
+        if len(set(image_names)) != len(image_names):
+            raise ValueError("repeated image names")
+        raise ParseError("Failed to parse proto object.")
+    out = np.zeros(max(need, 1), np.uint8)
+    got = L.lfr_wire_encode_solution_carried(len(image_names), *ptrs, fptr, buf.size, out.ctypes.data, need, C.byref(n))
+    assert got == need
+    return out[:need].tobytes(), int(n.value)
 
 
 def decode_solution(data: bytes):
