@@ -5,6 +5,9 @@
   liblfr_host.so  CPU-only host utilities behind include/lfr_wire.h and include/lfr_host.h
                   (protobuf wire codec, host graph stage) — no CUDA dependency, so the
                   reference arm of bench.py and the tests can use them without mapping the product library
+  liblfr_b200_lmstep.so
+                  the product built with -DLFR_DBG_LM_STEP: every component stops after its first LM step
+                  and reports it (csrc/lfr_lm.cuh), for tests/test_gpu_lm_step.py
   multi-view-refinement/build/solve_native
                   the native drop-in executable (lfr_solve_main.cc), linked against the two libraries
 """
@@ -15,6 +18,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "liblfr_b200.so")
 OUT_HOST = os.path.join(HERE, "liblfr_host.so")
+OUT_LM_STEP = os.path.join(HERE, "liblfr_b200_lmstep.so")
 SOURCES = ["lfr_capi.cu"]
 HOST_SOURCES = ["lfr_wire.cc", "lfr_host.cc"]
 EXE_SOURCE = "lfr_solve_main.cc"
@@ -77,7 +81,15 @@ def build(force: bool = False, verbose: bool = False) -> str:
     build_host(force)
     _build_cuda(force, verbose)
     build_exe(force)
+    build_lm_step(force)
     return OUT
+
+
+def build_lm_step(force: bool = False) -> str:
+    """The first-LM-step variant, rebuilt when the product's sources change."""
+    if force or _stale(OUT_LM_STEP, DEPS):
+        build_variant(os.path.basename(OUT_LM_STEP), ["LFR_DBG_LM_STEP"])
+    return OUT_LM_STEP
 
 
 def _build_cuda(force: bool = False, verbose: bool = False) -> str:

@@ -76,6 +76,11 @@ struct DevProblem {
 struct LmProfile {
   enum Word { kTotal = 0, kSetup, kEval, kAssemble, kSolve, kRest, kSteps, kTierWord };
   enum Tier : unsigned { kWarp2 = 1, kTile = 2, kWarp = 3, kCta = 4 };
+#ifdef LFR_DBG_LM_STEP
+  static constexpr bool kMarks = false;  // the record carries the first LM step instead (lm_solve)
+#else
+  static constexpr bool kMarks = true;
+#endif
 
   const DevProblem& P;  // the record of slot c is written when P.st_cycles is set (a kernel parameter: the
   uint32_t c;           // test costs no register), by the thread that writes the scalars
@@ -94,7 +99,7 @@ struct LmProfile {
   }
   // Charges the cycles since the last mark to word `w` (and to the total).
   __device__ __forceinline__ void tick(int w) {
-    if (!P.st_cycles) return;
+    if (!kMarks || !P.st_cycles) return;
     const long long now = clock64();
     if (lead) {
       unsigned long long* o = P.st_cycles + 8 * (size_t)c;
@@ -105,7 +110,7 @@ struct LmProfile {
     t_mark = now;
   }
   __device__ __forceinline__ void finish(unsigned ls_steps, unsigned tier, unsigned long long counter) {
-    if (!P.st_cycles) return;
+    if (!kMarks || !P.st_cycles) return;
     tick(kRest);
     if (!lead) return;
     unsigned long long* o = P.st_cycles + 8 * (size_t)c;
@@ -155,6 +160,37 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
   int iter = 0, n_invalid = 0, term = LFR_TERM_NO_CONVERGENCE;
   unsigned ls_steps = 0;
   bool success = true;
+#ifdef LFR_DBG_LM_STEP
+  // Diagnostic build (liblfr_b200_lmstep.so, csrc/build.py): the first LM step at the initial radius,
+  // then nothing else, so that tests can hold every tier's step against an exact solve of the same
+  // damped system.  dl goes to positions_out at the free coordinates (the write-back's loop: roots and
+  // constants keep their values); the scalars go to the slot's LFR_DBG_PROFILE record (a plan created
+  // with LFR_DBG_PROFILE, read by lfr_debug_plan_cycles), whose marks this build compiles out, as
+  // doubles:  0 cost at x, 1 gmax, 2 lm_step's validity (1 / 0, before the driver's model_change > 0
+  // test, except on the shared-memory Cholesky tier, whose lm_step applies that test itself and then
+  // leaves g . dl and |dl|_inf at 0 and dl unwritten), 3 model cost change, 4 g . dl, 5 |dl|_inf,
+  // 6 tier code, 7 unknowns n.
+  {
+    double mc = 0.0, gd = 0.0, dmax = 0.0;
+    const bool valid = T.lm_step(K.radius0, &mc, &gd, &dmax);
+    for (int i = T.tid(); i < C.n; i += Tier::kStride) {
+      const int l = C.lof[i >> 1];
+      P.positions_out[2 * (size_t)C.node[l] + (i & 1)] = C.dl[i];
+    }
+    if (T.lead()) {
+      P.st_iter[c] = 1;
+      P.st_term[c] = LFR_TERM_NO_CONVERGENCE;
+      P.st_cost0[c] = cost;
+      P.st_cost1[c] = cost;
+      P.st_ls[c] = 0;
+      if (P.st_cycles) {
+        const double rec[8] = {cost, gmax, valid ? 1.0 : 0.0, mc, gd, dmax, (double)Tier::kTier, (double)C.n};
+        for (int k = 0; k < 8; ++k) P.st_cycles[8 * (size_t)c + k] = (unsigned long long)__double_as_longlong(rec[k]);
+      }
+    }
+    return;
+  }
+#endif
   double x_norm = T.x_norm();
 
   // ---- trust-region loop (A.6) ---------------------------------------------------------
