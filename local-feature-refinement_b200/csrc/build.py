@@ -8,6 +8,11 @@
   liblfr_b200_lmstep.so
                   the product built with -DLFR_DBG_LM_STEP: every component stops after its first LM step
                   and reports it (csrc/lfr_lm.cuh), for tests/test_gpu_lm_step.py
+  liblfr_b200_lsprobe.so
+                  the product built with -DLFR_DBG_LS_PROBE: every component takes its first LM step, then one
+                  line-search trial, its slope and the accepted step's bookkeeping, optionally a second LM step,
+                  or the step after a rejected one, and reports them (csrc/lfr_lm.cuh), for
+                  tests/test_gpu_ls_probe.py
   multi-view-refinement/build/solve_native
                   the native drop-in executable (lfr_solve_main.cc), linked against the two libraries
 """
@@ -19,6 +24,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "liblfr_b200.so")
 OUT_HOST = os.path.join(HERE, "liblfr_host.so")
 OUT_LM_STEP = os.path.join(HERE, "liblfr_b200_lmstep.so")
+OUT_LS_PROBE = os.path.join(HERE, "liblfr_b200_lsprobe.so")
 SOURCES = ["lfr_capi.cu"]
 HOST_SOURCES = ["lfr_wire.cc", "lfr_host.cc"]
 EXE_SOURCE = "lfr_solve_main.cc"
@@ -82,6 +88,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     _build_cuda(force, verbose)
     build_exe(force)
     build_lm_step(force)
+    build_ls_probe(force)
     return OUT
 
 
@@ -90,6 +97,13 @@ def build_lm_step(force: bool = False) -> str:
     if force or _stale(OUT_LM_STEP, DEPS):
         build_variant(os.path.basename(OUT_LM_STEP), ["LFR_DBG_LM_STEP"])
     return OUT_LM_STEP
+
+
+def build_ls_probe(force: bool = False) -> str:
+    """The line-search probe variant, rebuilt when the product's sources change."""
+    if force or _stale(OUT_LS_PROBE, DEPS):
+        build_variant(os.path.basename(OUT_LS_PROBE), ["LFR_DBG_LS_PROBE"])
+    return OUT_LS_PROBE
 
 
 def _build_cuda(force: bool = False, verbose: bool = False) -> str:

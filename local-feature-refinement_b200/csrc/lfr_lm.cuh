@@ -19,6 +19,8 @@
 //   x_norm()                   |x| over the free coordinates
 //   step_norm()                |x - xc| over the free coordinates
 //   accept()                   x = xc -> the new |x|
+//   reject()                   after a rejected step: restores what the next lm_step reads of the
+//                              evaluation at x, where a trial overwrote it
 //   counter()                  the tier's own profile counter (word 7)
 // The tiers differ in how they reduce, fuse and synchronise; those choices stay inside their
 // members, so each tier's sums are the same operations, in the same order, as before the driver
@@ -76,8 +78,8 @@ struct DevProblem {
 struct LmProfile {
   enum Word { kTotal = 0, kSetup, kEval, kAssemble, kSolve, kRest, kSteps, kTierWord };
   enum Tier : unsigned { kWarp2 = 1, kTile = 2, kWarp = 3, kCta = 4 };
-#ifdef LFR_DBG_LM_STEP
-  static constexpr bool kMarks = false;  // the record carries the first LM step instead (lm_solve)
+#if defined(LFR_DBG_LM_STEP) || defined(LFR_DBG_LS_PROBE)
+  static constexpr bool kMarks = false;  // the record carries the first LM step or the probe instead (lm_solve)
 #else
   static constexpr bool kMarks = true;
 #endif
@@ -191,6 +193,66 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
     return;
   }
 #endif
+#ifdef LFR_DBG_LS_PROBE
+  // Diagnostic build (liblfr_b200_lsprobe.so, csrc/build.py): the first LM step at the initial radius,
+  // then the members the line search and the step's acceptance or rejection call, in a fixed order, so
+  // that tests can hold each value against an exact evaluation at the same point.  The mode and the step
+  // size come from line_search_sufficient_function_decrease, which only the Armijo test reads and which
+  // this build never reaches:
+  //   0 < ls_suff <= 1 (mode A, alpha = ls_suff): dl goes to positions_out at the free coordinates; then
+  //     trial(alpha), step_norm(), trial_slope(alpha), slope(), accept(), assemble(false), and the record
+  //     holds, as doubles:  0 cost by trial, 1 cost by trial_slope, 2 phi' by trial_slope, 3 phi' by
+  //     slope(), 4 |x - xc|, 5 |xc| (accept's return), 6 gmax at xc, 7 tier code.
+  //   ls_suff < 0 (mode B, alpha = -ls_suff): the same sequence, then a second lm_step at the initial
+  //     radius from xc with iteration 0's Jacobi scaling; its step dl2 goes to positions_out and the
+  //     record has the layout of the LFR_DBG_LM_STEP build: 0 cost at xc, 1 gmax at xc, 2 validity,
+  //     3 model cost change, 4 g . dl2, 5 |dl2|_inf, 6 tier code, 7 unknowns n.
+  //   ls_suff > 1 (mode C, a rejected step): trial(1) and slope() (the first contraction's samples),
+  //     then, as after a rejected step, reject() and lm_step at half the initial radius from the
+  //     unchanged x; dl2 and the record as in mode B, with the cost and gmax at x.
+  {
+    const bool second = K.ls_suff < 0.0, rejected = K.ls_suff > 1.0;
+    const double alpha = rejected ? 1.0 : fabs(K.ls_suff);
+    double mc = 0.0, gd = 0.0, dmax = 0.0;
+    bool valid = T.lm_step(K.radius0, &mc, &gd, &dmax);
+    double rec_a[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, (double)Tier::kTier};
+    double cost_b = cost, gmax_b = gmax;
+    if (rejected) {
+      T.trial(alpha);
+      T.slope();
+      T.reject();
+      valid = T.lm_step(0.5 * K.radius0, &mc, &gd, &dmax);
+    } else {
+      rec_a[0] = T.trial(alpha);
+      rec_a[4] = T.step_norm();
+      rec_a[1] = T.trial_slope(alpha, &rec_a[2]);
+      rec_a[3] = T.slope();
+      rec_a[5] = T.accept();
+      rec_a[6] = T.assemble(false);
+      cost_b = rec_a[0];
+      gmax_b = rec_a[6];
+      if (second) valid = T.lm_step(K.radius0, &mc, &gd, &dmax);
+    }
+    for (int i = T.tid(); i < C.n; i += Tier::kStride) {
+      const int l = C.lof[i >> 1];
+      P.positions_out[2 * (size_t)C.node[l] + (i & 1)] = C.dl[i];
+    }
+    if (T.lead()) {
+      P.st_iter[c] = 1;
+      P.st_term[c] = LFR_TERM_NO_CONVERGENCE;
+      P.st_cost0[c] = cost;
+      P.st_cost1[c] = cost_b;
+      P.st_ls[c] = 0;
+      if (P.st_cycles) {
+        const double rec_b[8] = {cost_b, gmax_b, valid ? 1.0 : 0.0, mc, gd, dmax, (double)Tier::kTier, (double)C.n};
+        for (int k = 0; k < 8; ++k)
+          P.st_cycles[8 * (size_t)c + k] =
+              (unsigned long long)__double_as_longlong(second || rejected ? rec_b[k] : rec_a[k]);
+      }
+    }
+    return;
+  }
+#endif
   double x_norm = T.x_norm();
 
   // ---- trust-region loop (A.6) ---------------------------------------------------------
@@ -268,6 +330,7 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
       radius = fmin(K.radius_max, radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
       nu = 2.0;
     } else {
+      T.reject();
       radius /= nu;
       nu *= 2.0;
     }

@@ -550,6 +550,11 @@ struct CtaTier {
     block_sum3(C, a2, z1, z2);
     return sqrt(a2);
   }
+  // The matrix-free product of an irregular component reads a and M of the staged evaluation, which the
+  // line search's trials overwrote: stage x's again (the block-CSR form of a regular one is assemble()'s)
+  __device__ void reject() {
+    if (!C.regular) cta_eval(C, C.x, K);
+  }
   __device__ unsigned long long counter() const { return cg_iters; }
 };
 

@@ -350,6 +350,7 @@ struct WarpTier {
     __syncwarp();
     return free_norm(C.x, nullptr);
   }
+  __device__ void reject() {}  // lm_step reads H and g, which only assemble() writes
   __device__ unsigned long long counter() const { return 0; }
 };
 

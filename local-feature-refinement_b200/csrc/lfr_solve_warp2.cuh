@@ -312,9 +312,12 @@ __device__ __forceinline__ double reg_assemble(const RegCtx<T>& C, bool first, c
       }
     }
   } else {
-    // serial path for inputs without clean edge twins: one thread accumulates every edge in order
+    // serial path for inputs without clean edge twins: one thread accumulates every edge in order.
+    // GRAD_ONLY sums into the pivot-row buffer (free outside lm_step), not g: g stays the gradient at x,
+    // which the next lm_step reads when the line search's step is rejected
+    double* const gs = GRAD_ONLY ? C.prow : C.g;
     if (C.tid == 0) {
-      for (int i = 0; i < C.n; ++i) C.g[i] = 0.0;
+      for (int i = 0; i < C.n; ++i) gs[i] = 0.0;
       for (int e = 0; e < C.Ec; ++e) {
         const uint32_t mt = C.meta[e];
         const int fs = C.freeof[mt & 0xfff], fd = C.freeof[(mt >> 12) & 0xfff];
@@ -322,8 +325,8 @@ __device__ __forceinline__ double reg_assemble(const RegCtx<T>& C, bool first, c
         const double m00 = C.scr[3 * E + e], m01 = C.scr[4 * E + e], m10 = C.scr[5 * E + e],
                      m11 = C.scr[6 * E + e];
         if (fs >= 0) {
-          C.g[2 * fs] -= a * (m00 * r0 + m10 * r1);
-          C.g[2 * fs + 1] -= a * (m01 * r0 + m11 * r1);
+          gs[2 * fs] -= a * (m00 * r0 + m10 * r1);
+          gs[2 * fs + 1] -= a * (m01 * r0 + m11 * r1);
           if (!GRAD_ONLY) {
             double* hd = C.H + (2 * fs) * ldh + 2 * fs;
             hd[0] += a * (m00 * m00 + m10 * m10);
@@ -333,8 +336,8 @@ __device__ __forceinline__ double reg_assemble(const RegCtx<T>& C, bool first, c
           }
         }
         if (fd >= 0) {
-          C.g[2 * fd] += a * r0;
-          C.g[2 * fd + 1] += a * r1;
+          gs[2 * fd] += a * r0;
+          gs[2 * fd + 1] += a * r1;
           if (!GRAD_ONLY) {
             C.H[(2 * fd) * ldh + 2 * fd] += a;
             C.H[(2 * fd + 1) * ldh + 2 * fd + 1] += a;
@@ -351,7 +354,7 @@ __device__ __forceinline__ double reg_assemble(const RegCtx<T>& C, bool first, c
     G::sync();
     for (int i = C.tid; i < C.n; i += T) {
       if (GRAD_ONLY) {
-        acc += C.g[i] * C.dl[i];
+        acc += gs[i] * C.dl[i];
       } else {
         if (first) C.S[i] = 1.0 / (1.0 + sqrt(C.H[i * ldh + i]));
         const int l = C.lof[i >> 1];
@@ -633,6 +636,7 @@ struct RegTier {
       return sqrt(G::sum(C, a2));
     }
   }
+  __device__ void reject() {}  // lm_step reads H and g, which only assemble() writes
   __device__ unsigned long long counter() const { return 0; }
 };
 
