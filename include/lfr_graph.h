@@ -135,13 +135,34 @@ int lfr_plan_start_from_solution(lfr_plan* plan, void* stream, const uint8_t* by
  * node with an entry in the file (the rule of lfr_wire_join_solution_entries(), include/lfr_wire.h) becomes
  * constant, as a node of a fixed image is.  The mask is reference root OR node of an image fixed by
  * lfr_plan_fix_images() OR kept node; the per-image mask and the kept flags are separate inputs, so the two
- * calls compose in either order, and the schedule is built again on the mask.  A later call replaces the
- * kept set (an empty SolutionFile clears it); a later lfr_plan_start_from_solution() changes only the start
+ * calls compose in either order, and the schedule is built again on the mask.  A later call, or a later
+ * lfr_plan_update_solution(), replaces the kept set (an empty SolutionFile clears it); a later lfr_plan_start_from_solution() changes only the start
  * values.  A plan never given a kept set holds no buffer for one.  *n_kept (may be NULL) = the nodes with an
  * entry.  Synchronous on `stream`.  LFR_EINVAL for malformed bytes (the plan is not changed) and for a plan
  * made by lfr_plan_create(). */
 int lfr_plan_keep_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                            const uint8_t* names, const uint64_t* name_off, uint64_t* n_kept);
+
+/* Update an earlier SolutionFile with new keypoints: solve again, from scratch, every component a keypoint
+ * without an entry in the file joins, and hold every other component at the file's values.  A component is
+ * an entry of the plan's dispatch list (lfr_problem.comp: after the cut; a component of one node counts
+ * too).  It is touched when at least one of its nodes has no entry (the rule of
+ * lfr_wire_join_solution_entries(), include/lfr_wire.h).
+ *   - a touched component's nodes start at 0 and are held only when the reference or lfr_plan_fix_images()
+ *     says so: it solves bit for bit as in a plan never given a file;
+ *   - an untouched component's nodes start at their entries and are all held: it ends LFR_TERM_EMPTY (or
+ *     SKIPPED at one node) with the file's values.
+ * The same single host decode and device join as lfr_plan_keep_solution(); one kernel marks the touched
+ * components, one writes the start and working positions and the held flags (entry AND component not
+ * touched) that the constant mask ORs in place of the kept flags, and the schedule is built again.  The held
+ * set and the kept set are one input: the last lfr_plan_keep_solution() or lfr_plan_update_solution() call
+ * wins, and an empty file clears it (every component is touched then).  It composes with
+ * lfr_plan_fix_images() in either order.  A plan never given the call allocates nothing for it.
+ * *n_held (may be NULL) = the held nodes, *n_touched (may be NULL) = the touched components; both are what
+ * lfr_wire_update_solution() counts.  Synchronous on `stream`.  LFR_EINVAL for malformed bytes (the plan is
+ * not changed) and for a plan made by lfr_plan_create(). */
+int lfr_plan_update_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                             const uint8_t* names, const uint64_t* name_off, uint64_t* n_held, uint32_t* n_touched);
 
 /* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
  * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from

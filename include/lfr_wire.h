@@ -106,6 +106,19 @@ int lfr_wire_join_solution_entries(const uint8_t* buf, uint64_t len, uint32_t n_
                                    const uint32_t* node_feat, double* positions /* [2 n_nodes] */, uint64_t* n_started,
                                    uint8_t* has_entry /* [n_nodes] */);
 
+/* The host form of lfr_plan_update_solution() (include/lfr_graph.h), bit for bit: node v is in component
+ * node_comp[v] (< n_components; lfr_problem.comp).  A component is touched when one of its nodes has no entry
+ * under the rule of lfr_wire_join_solution_entries().  held[v] = 1 when node v has an entry and its component
+ * is not touched, else 0; positions[2v .. 2v+1] = its entry when held, else 0.  The constant mask of the solve
+ * is then reference root OR node of a fixed image OR held node.  *n_held (may be NULL) = the held nodes,
+ * *n_touched (may be NULL) = the touched components.  LFR_EINVAL as lfr_wire_join_solution_entries(), or for
+ * NULL node_comp / held with n_nodes > 0 or a node_comp out of range; every output is untouched then. */
+int lfr_wire_update_solution(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                             const uint64_t* name_off, uint32_t n_nodes, const uint32_t* node_image,
+                             const uint32_t* node_feat, const uint32_t* node_comp, uint32_t n_components,
+                             double* positions /* [2 n_nodes] */, uint8_t* held /* [n_nodes] */, uint64_t* n_held,
+                             uint32_t* n_touched);
+
 /* lfr_wire_encode_solution() of a scene's output (the same arrays: its images in output order, each with
  * its displacements), merged with an earlier SolutionFile `file`, so that the output holds the whole scene
  * when only part of it was solved again.  FILE's effective content follows the rule of

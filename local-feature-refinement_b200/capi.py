@@ -82,7 +82,7 @@ ABI_SYMBOLS = [
 GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
                  "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
                  "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution",
-                 "lfr_plan_encode_solution_carried"]
+                 "lfr_plan_encode_solution_carried", "lfr_plan_update_solution"]
 
 
 class LfrWirePart(C.Structure):
@@ -162,6 +162,8 @@ class Library:
             L.lfr_plan_start_from_solution.restype = C.c_int
             L.lfr_plan_keep_solution.argtypes = L.lfr_plan_start_from_solution.argtypes
             L.lfr_plan_keep_solution.restype = C.c_int
+            L.lfr_plan_update_solution.argtypes = L.lfr_plan_start_from_solution.argtypes + [C.POINTER(C.c_uint32)]
+            L.lfr_plan_update_solution.restype = C.c_int
             L.lfr_plan_encode_solution_carried.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
                                                            C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                                            C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
@@ -524,6 +526,23 @@ class Plan:
                                                            C.byref(n)),
                        "lfr_plan_keep_solution")
         return int(n.value)
+
+    def update_solution(self, data: bytes, image_names, stream: int = 0):
+        """lfr_plan_update_solution (include/lfr_graph.h): every component with a node that has no entry in
+        `data` is touched and solves from zeros as without a file; every other component is held constant at
+        the file's values.  Replaces an earlier kept or held set (an empty file clears it) and composes with
+        fix_images() in either order.  Returns (held nodes, touched components)."""
+        from .wire import _names_blob
+        buf = np.frombuffer(data, dtype=np.uint8)
+        blob, off = _names_blob(list(image_names))
+        n = C.c_uint64()
+        t = C.c_uint32()
+        self.lib.check(self.lib.lib.lfr_plan_update_solution(self.handle, C.c_void_p(stream),
+                                                             buf.ctypes.data if buf.size else None, buf.size,
+                                                             len(image_names), blob.ctypes.data, off.ctypes.data,
+                                                             C.byref(n), C.byref(t)),
+                       "lfr_plan_update_solution")
+        return int(n.value), int(t.value)
 
     def solve(self, stream: int = 0) -> None:
         self.lib.check(self.lib.lib.lfr_plan_solve(self.handle, C.c_void_p(stream)), "lfr_plan_solve")

@@ -16,6 +16,9 @@ images against an already-refined scene.  --keep_initial_solution (with --initia
 every keypoint that has an entry in that file constant, and refines only the others.
 --carry_initial_solution (with --initial_solution) writes the whole scene: the output also holds every entry
 of that file the solve does not refine (wire.encode_solution_carried), so new pairs alone can be solved.
+--update_initial_solution (with --initial_solution, not with --keep_initial_solution) solves every component
+that a keypoint without an entry in that file joins from zeros, as a run without the file does, and holds
+every other component at the file's values (wire.update_solution, Plan.update_solution).
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -51,7 +54,8 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("n_threads", True, False), ("banned_images", True, True),
             ("device", True, False), ("gpus", True, False), ("stats_json", True, False),
             ("fixed_images", True, True), ("initial_solution", True, False),
-            ("keep_initial_solution", False, False), ("carry_initial_solution", False, False)]
+            ("keep_initial_solution", False, False), ("carry_initial_solution", False, False),
+            ("update_initial_solution", False, False)]
 
 
 def _find_option(name):
@@ -127,7 +131,8 @@ def parse_args(argv):
             device=_as_uint(vals, "device", 0), gpus=_as_uint(vals, "gpus", 1), stats_json=vals.get("stats_json"),
             fixed_images=vals.get("fixed_images", []), initial_solution=vals.get("initial_solution"),
             keep_initial_solution=bool(vals.get("keep_initial_solution")),
-            carry_initial_solution=bool(vals.get("carry_initial_solution")))
+            carry_initial_solution=bool(vals.get("carry_initial_solution")),
+            update_initial_solution=bool(vals.get("update_initial_solution")))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -148,6 +153,12 @@ def main(argv=None) -> int:
         return 2
     if args.carry_initial_solution and not args.initial_solution:
         sys.stderr.write("ERROR: --carry_initial_solution needs --initial_solution FILE\n")
+        return 2
+    if args.update_initial_solution and not args.initial_solution:
+        sys.stderr.write("ERROR: --update_initial_solution needs --initial_solution FILE\n")
+        return 2
+    if args.update_initial_solution and args.keep_initial_solution:
+        sys.stderr.write("ERROR: --update_initial_solution and --keep_initial_solution exclude each other\n")
         return 2
     start = None
     if args.initial_solution is not None:
@@ -213,7 +224,8 @@ def main(argv=None) -> int:
     try:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
                                  timing=timing, fixed_images=args.fixed_images, initial_solution=start,
-                                 keep_initial_solution=args.keep_initial_solution)
+                                 keep_initial_solution=args.keep_initial_solution,
+                                 update_initial_solution=args.update_initial_solution)
     except GraphStageRouteError as e:
         sys.stderr.write("ERROR: %s\n" % e)
         return 2

@@ -279,7 +279,8 @@ struct lfr_plan {
   // `is_root` (reference roots OR nodes of fixed images OR kept nodes) and its host copy for the schedule
   // builder; never allocated for a plan without one.  Its two inputs are kept apart, so that each call
   // replaces only its own: the per-image mask (empty until lfr_plan_fix_images()) and the per-node kept
-  // flags (allocated by the first lfr_plan_keep_solution())
+  // flags (allocated by the first lfr_plan_keep_solution() or lfr_plan_update_solution(), whose held flags
+  // they are then: the last of the two calls wins)
   DevBuf const_mask;
   std::vector<uint8_t> const_host;
   std::vector<uint8_t> fixed_host;
@@ -2541,6 +2542,38 @@ int lfr_plan_keep_solution(lfr_plan* pl, void* stream, const uint8_t* bytes, uin
     LFR_CUDA(cudaMemsetAsync(pl->kept.p, 0, std::max<size_t>(pl->N, 1), s));
   }
   LFR_TRY(join_solution(pl, s, d, pl->kept.as<uint8_t>(), n_kept));
+  return build_constant_mask(pl, s);
+}
+
+int lfr_plan_update_solution(lfr_plan* pl, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                             const uint8_t* names, const uint64_t* name_off, uint64_t* n_held, uint32_t* n_touched) {
+  lfr::join::Decoded d;
+  LFR_TRY(decode_solution_for(pl, bytes, len, n_images, names, name_off, d));
+  LFR_CUDA(cudaSetDevice(pl->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  const uint32_t N = pl->N, C = pl->C;
+  if (!pl->kept.p) {  // cleared, so that a join that fails before its kernel leaves no stale flags
+    LFR_TRY(pl->kept.reserve(std::max<size_t>(N, 1)));
+    LFR_CUDA(cudaMemsetAsync(pl->kept.p, 0, std::max<size_t>(N, 1), s));
+  }
+  // the kept flags take the join's "has entry", then the held flags in place
+  LFR_TRY(join_solution(pl, s, d, pl->kept.as<uint8_t>(), nullptr));
+  unsigned long long counts[2] = {0, 0};  // held nodes, touched components
+  if (N) {
+    TmpBuf t;  // the two counters, then one touched flag per component
+    LFR_TRY(t.reserve(16 + (size_t)C));
+    auto* ctr = t.as<unsigned long long>();
+    uint8_t* touched = t.as<uint8_t>() + 16;
+    LFR_CUDA(cudaMemsetAsync(t.p, 0, 16 + (size_t)C, s));
+    lfr::start::touch_kernel<<<blocks_for(N), 256, 0, s>>>(pl->kept.as<uint8_t>(), pl->comp.as<uint32_t>(), N, touched);
+    lfr::start::update_kernel<<<blocks_for(N), 256, 0, s>>>(pl->comp.as<uint32_t>(), touched, N, pl->kept.as<uint8_t>(),
+                                                              pl->pos_init.as<double>(), pl->pos.as<double>(), ctr);
+    lfr::start::count_touched_kernel<<<blocks_for(C), 256, 0, s>>>(touched, C, ctr + 1);
+    LFR_LAUNCHED();
+    LFR_TRY(fetch(counts, ctr, 2, s));  // before `t` is freed
+  }
+  if (n_held) *n_held = counts[0];
+  if (n_touched) *n_touched = (uint32_t)counts[1];
   return build_constant_mask(pl, s);
 }
 

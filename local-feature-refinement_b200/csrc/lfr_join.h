@@ -1,6 +1,7 @@
 // lfr_join.h — the host half of a start point read from a SolutionFile (types.proto:30-46), shared by the
-// host joins (lfr_wire_join_solution and _entries, lfr_wire.cc), the device join
-// (lfr_plan_start_from_solution and lfr_plan_keep_solution, lfr_capi.cu) and the carried encoders
+// host joins (lfr_wire_join_solution, _entries and lfr_wire_update_solution, lfr_wire.cc), the device join
+// (lfr_plan_start_from_solution, lfr_plan_keep_solution and lfr_plan_update_solution, lfr_capi.cu) and the
+// carried encoders
 // (lfr_wire_encode_solution_carried, lfr_plan_encode_solution_carried): the decode with
 // lfr_wire_decode_solution() and the image rule, and the host joins' node loop.  Header-only host code.
 //
@@ -129,6 +130,34 @@ inline int join_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const
     if (has_entry) has_entry[v] = hit ? 1 : 0;
   }
   if (n_started) *n_started = started;
+  return LFR_OK;
+}
+
+// The host update (lfr_wire_update_solution): join_nodes() with its flags, then every component with a node
+// without an entry is touched; its nodes start at 0 and are not held.  held[v] = has entry AND component not
+// touched.  Every output is untouched when the arguments or the bytes are rejected (LFR_EINVAL).
+inline int update_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                        uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, const uint32_t* node_comp,
+                        uint32_t n_components, double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched) {
+  if (n_nodes && (!node_comp || !held)) return LFR_EINVAL;
+  for (uint32_t v = 0; v < n_nodes; ++v)
+    if (node_comp[v] >= n_components) return LFR_EINVAL;
+  const int rc = join_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions, held, nullptr);
+  if (rc != LFR_OK) return rc;
+  std::vector<uint8_t> touched(n_components, 0);
+  for (uint32_t v = 0; v < n_nodes; ++v)
+    if (!held[v]) touched[node_comp[v]] = 1;
+  uint64_t nh = 0;
+  for (uint32_t v = 0; v < n_nodes; ++v) {
+    if (touched[node_comp[v]]) {
+      positions[2 * (size_t)v] = 0.0;
+      positions[2 * (size_t)v + 1] = 0.0;
+      held[v] = 0;
+    }
+    nh += held[v];
+  }
+  if (n_held) *n_held = nh;
+  if (n_touched) *n_touched = (uint32_t)std::count(touched.begin(), touched.end(), (uint8_t)1);
   return LFR_OK;
 }
 

@@ -26,7 +26,10 @@
 // route the constant mask and lfr_wire_join_solution() or _entries() handed to the solve — and
 // --carry_initial_solution (the output also holds every entry of that file the scene does not refine:
 // lfr_plan_encode_solution_carried() on the device route, lfr_wire_encode_solution_carried() on the host
-// route's assembly).  `--n_threads` is accepted and
+// route's assembly) and --update_initial_solution (every component a keypoint without an entry in that
+// file joins is solved from zeros as without the file, every other one is held at the file's values:
+// lfr_plan_update_solution() on the device route, lfr_wire_update_solution() handed to the solve on the host
+// route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -70,6 +73,9 @@ int lfr_plan_start_from_solution(lfr_plan* plan, void* stream, const uint8_t* by
                                  const uint8_t* names, const uint64_t* name_off, uint64_t* n_started) __attribute__((weak));
 int lfr_plan_keep_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                            const uint8_t* names, const uint64_t* name_off, uint64_t* n_kept) __attribute__((weak));
+int lfr_plan_update_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                             const uint8_t* names, const uint64_t* name_off, uint64_t* n_held,
+                             uint32_t* n_touched) __attribute__((weak));
 int64_t lfr_plan_encode_solution_carried(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
                                          const uint64_t* name_off, const float* fact, const uint8_t* file,
                                          uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
@@ -98,7 +104,8 @@ struct OptionSpec {
 const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", true, false}, {"output_file", true, false},
                                {"n_threads", true, false},    {"banned_images", true, true}, {"device", true, false},
                                {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false},
-                               {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false}};
+                               {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false},
+                               {"update_initial_solution", false, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -117,7 +124,7 @@ const OptionSpec& find_option(const std::string& name) {
 }
 
 struct Args {
-  bool help = false, keep_initial_solution = false, carry_initial_solution = false;
+  bool help = false, keep_initial_solution = false, carry_initial_solution = false, update_initial_solution = false;
   std::map<std::string, std::string> single;
   std::map<std::string, std::vector<std::string>> repeated;
 };
@@ -151,8 +158,9 @@ Args parse(int argc, char** argv) {
       } else {
         if (eq != std::string::npos) throw CliError{std::string("option '--") + o.name + "' does not take any arguments"};
         (std::strcmp(o.name, "help") == 0 ? a.help
-         : std::strcmp(o.name, "keep_initial_solution") == 0 ? a.keep_initial_solution
-                                                             : a.carry_initial_solution) = true;
+         : std::strcmp(o.name, "keep_initial_solution") == 0  ? a.keep_initial_solution
+         : std::strcmp(o.name, "carry_initial_solution") == 0 ? a.carry_initial_solution
+                                                              : a.update_initial_solution) = true;
       }
     } else if (tok.size() > 1 && tok[0] == '-') {
       throw CliError{"unrecognised option '" + tok + "'"};
@@ -243,7 +251,7 @@ int main(int argc, char** argv) {
   std::string matches_file, output_file, initial_solution;
   std::vector<std::string> banned_list, fixed_list;
   uint64_t device = 0, gpus = 1;
-  bool keep_start = false, carry_start = false;
+  bool keep_start = false, carry_start = false, update_start = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -263,6 +271,7 @@ int main(int argc, char** argv) {
     if (a.single.count("initial_solution")) initial_solution = a.single.at("initial_solution");
     keep_start = a.keep_initial_solution;
     carry_start = a.carry_initial_solution;
+    update_start = a.update_initial_solution;
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
@@ -278,6 +287,14 @@ int main(int argc, char** argv) {
   }
   if (carry_start && !have_start) {
     std::fputs("ERROR: --carry_initial_solution needs --initial_solution FILE\n", stderr);
+    return 2;
+  }
+  if (update_start && !have_start) {
+    std::fputs("ERROR: --update_initial_solution needs --initial_solution FILE\n", stderr);
+    return 2;
+  }
+  if (update_start && keep_start) {
+    std::fputs("ERROR: --update_initial_solution and --keep_initial_solution exclude each other\n", stderr);
     return 2;
   }
   if (have_start) {
@@ -411,7 +428,8 @@ int main(int argc, char** argv) {
   // takes the host route; forcing the device route there is an error, never a silent host run.
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
-                                 lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried;
+                                 lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
+                                 lfr_plan_update_solution;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -492,7 +510,10 @@ int main(int argc, char** argv) {
     }
     // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
     int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), (uint32_t)names.size()) : LFR_OK;
-    if (rc2 == LFR_OK && have_start)
+    if (rc2 == LFR_OK && have_start && update_start)
+      rc2 = lfr_plan_update_solution(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                     name_blob.data(), name_off.data(), nullptr, nullptr);
+    else if (rc2 == LFR_OK && have_start)
       rc2 = (keep_start ? lfr_plan_keep_solution : lfr_plan_start_from_solution)(
           plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(), name_off.data(), nullptr);
     if (rc2 != LFR_OK) {
@@ -538,17 +559,24 @@ int main(int argc, char** argv) {
   // ---- the solve (solve.cc:608-635): positions start at zero, or from --initial_solution -----
   double* positions = nullptr;  // host route: the solve's result; the device route keeps it in HBM
   bool positions_pinned = false;
-  // host route with --fixed_images or --keep_initial_solution: reference roots OR nodes of fixed images OR
-  // nodes with an entry in the start solution
+  // host route with --fixed_images, --keep_initial_solution or --update_initial_solution: reference roots OR
+  // nodes of fixed images OR nodes with an entry in the start solution (kept) or held by the update
   std::vector<uint8_t> is_const;
-  const bool any_const = any_fixed || keep_start;
+  const bool any_const = any_fixed || keep_start || update_start;
   if (N && !plan) {
     positions = static_cast<double*>(lfr_host_alloc(2ull * N * sizeof(double)));
     positions_pinned = positions != nullptr;
     if (!positions) positions = static_cast<double*>(std::malloc(2ull * N * sizeof(double)));
     std::memset(positions, 0, 2ull * N * sizeof(double));
-    std::vector<uint8_t> has_entry(keep_start ? N : 0, 0);
-    if (have_start && (keep_start ? lfr_wire_join_solution_entries(start_file.data(), start_file.size(), (uint32_t)names.size(),
+    std::vector<uint8_t> has_entry(keep_start || update_start ? N : 0, 0);
+    if (have_start && update_start) {
+      if (lfr_wire_update_solution(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
+                                   name_off.data(), N, node_image.data(), node_feat.data(), comp.data(), C, positions,
+                                   has_entry.data(), nullptr, nullptr) != LFR_OK) {
+        std::fprintf(stderr, "ERROR: lfr_wire_update_solution failed\n");
+        return 2;
+      }
+    } else if (have_start && (keep_start ? lfr_wire_join_solution_entries(start_file.data(), start_file.size(), (uint32_t)names.size(),
                                                                   name_blob.data(), name_off.data(), N, node_image.data(),
                                                                   node_feat.data(), positions, nullptr, has_entry.data())
                                   : lfr_wire_join_solution(start_file.data(), start_file.size(), (uint32_t)names.size(),
@@ -560,7 +588,7 @@ int main(int argc, char** argv) {
     if (any_const) {
       is_const.resize(N);
       for (uint32_t v = 0; v < N; ++v)
-        is_const[v] = (is_root[v] || fixed[node_image[v]] || (keep_start && has_entry[v])) ? 1 : 0;
+        is_const[v] = (is_root[v] || fixed[node_image[v]] || ((keep_start || update_start) && has_entry[v])) ? 1 : 0;
     }
   }
   if (!carry_start) start_file.release();  // carried into the output otherwise

@@ -1,6 +1,6 @@
-// lfr_start.cuh — fixed images, kept solutions and start points of a device-resident plan
-// (lfr_plan_fix_images, lfr_plan_keep_solution, lfr_plan_start_from_solution; include/lfr_graph.h), over the
-// node ids the plan keeps in HBM.
+// lfr_start.cuh — fixed images, kept and updated solutions and start points of a device-resident plan
+// (lfr_plan_fix_images, lfr_plan_keep_solution, lfr_plan_update_solution, lfr_plan_start_from_solution;
+// include/lfr_graph.h), over the node ids the plan keeps in HBM.
 //
 // A constant node is what a root is to every tier (lfr_setup.cuh: kept at its start value, no bounds, a
 // block between two constant nodes dropped), so fixing images and keeping a solution only widen the mask
@@ -69,6 +69,48 @@ __global__ void join_kernel(const uint32_t* __restrict__ node_image, const uint3
   pos_init[2 * (size_t)v + 1] = b;
   pos[2 * (size_t)v] = a;
   pos[2 * (size_t)v + 1] = b;
+}
+
+// lfr_plan_update_solution: touched[comp[v]] = 1 for every node without an entry.  Reads are coalesced; the
+// lanes of a warp that name the same component store once (the stores are idempotent across warps).
+__global__ void touch_kernel(const uint8_t* __restrict__ has_entry, const uint32_t* __restrict__ comp, uint32_t N,
+                             uint8_t* __restrict__ touched) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool miss = v < N && !has_entry[v];
+  const unsigned active = __ballot_sync(0xffffffffu, miss);
+  if (!miss) return;
+  const uint32_t c = comp[v];
+  const unsigned same = __match_any_sync(active, c);
+  if ((uint32_t)(__ffs(same) - 1) == (threadIdx.x & 31u)) touched[c] = 1;
+}
+
+// lfr_plan_update_solution after the join and touch_kernel: held[v] (has_entry in, held out) = entry AND
+// component not touched; a touched component's nodes start at 0 in the start and working arrays.
+// n_held += the held nodes.
+__global__ void update_kernel(const uint32_t* __restrict__ comp, const uint8_t* __restrict__ touched, uint32_t N,
+                              uint8_t* __restrict__ held, double* __restrict__ pos_init, double* __restrict__ pos,
+                              unsigned long long* __restrict__ n_held) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  bool h = false;
+  if (v < N) {
+    h = held[v] && !touched[comp[v]];
+    held[v] = h ? 1 : 0;
+    if (!h) {
+      pos_init[2 * (size_t)v] = 0.0;
+      pos_init[2 * (size_t)v + 1] = 0.0;
+      pos[2 * (size_t)v] = 0.0;
+      pos[2 * (size_t)v + 1] = 0.0;
+    }
+  }
+  const unsigned n = __popc(__ballot_sync(0xffffffffu, h));
+  if ((threadIdx.x & 31u) == 0 && n) atomicAdd(n_held, (unsigned long long)n);
+}
+
+// n_touched += the components with touched[c] != 0
+__global__ void count_touched_kernel(const uint8_t* __restrict__ touched, uint32_t C, unsigned long long* __restrict__ n_touched) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned n = __popc(__ballot_sync(0xffffffffu, c < C && touched[c]));
+  if ((threadIdx.x & 31u) == 0 && n) atomicAdd(n_touched, (unsigned long long)n);
 }
 
 }  // namespace start

@@ -458,6 +458,14 @@ int lfr_wire_join_solution_entries(const uint8_t* buf, uint64_t len, uint32_t n_
                                n_started);
 }
 
+int lfr_wire_update_solution(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                             const uint64_t* name_off, uint32_t n_nodes, const uint32_t* node_image,
+                             const uint32_t* node_feat, const uint32_t* node_comp, uint32_t n_components,
+                             double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched) {
+  return lfr::join::update_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, node_comp,
+                                 n_components, positions, held, n_held, n_touched);
+}
+
 int64_t lfr_wire_encode_solution_carried(uint64_t n_images, const uint64_t* img_ptr, const uint8_t* names,
                                          const uint64_t* name_off, const float* fact, const uint32_t* feature_idx,
                                          const float* di, const float* dj, const uint8_t* file, uint64_t file_len,

@@ -28,7 +28,7 @@ class WireMatches(C.Structure):
 
 WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
                 "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution",
-                "lfr_wire_join_solution_entries", "lfr_wire_encode_solution_carried"]
+                "lfr_wire_join_solution_entries", "lfr_wire_encode_solution_carried", "lfr_wire_update_solution"]
 
 _bound = False
 
@@ -58,6 +58,10 @@ def _lib():
         L.lfr_wire_encode_solution_carried.argtypes = ([C.c_uint64] + [C.c_void_p] * 7 + [C.c_void_p, C.c_uint64, C.c_void_p,
                                                         C.c_uint64, C.POINTER(C.c_uint64)])
         L.lfr_wire_encode_solution_carried.restype = C.c_int64
+        L.lfr_wire_update_solution.argtypes = ([C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32]
+                                               + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p,
+                                                                     C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)])
+        L.lfr_wire_update_solution.restype = C.c_int
         _bound = True
     return L
 
@@ -296,3 +300,32 @@ def join_solution(data: bytes, image_names: List[str], node_image: np.ndarray, n
     if rc != 0:
         raise ParseError("Failed to parse proto object.")
     return (pos, int(n.value), has.astype(bool)) if entries else (pos, int(n.value))
+
+
+def update_solution(data: bytes, image_names: List[str], node_image: np.ndarray, node_feat: np.ndarray,
+                    node_comp: np.ndarray, n_components: int):
+    """The host form of Plan.update_solution (lfr_wire_update_solution, include/lfr_wire.h): a component
+    (node_comp, lfr_problem.comp) is touched when one of its nodes has no entry in `data` under the rule of
+    join_solution.  Returns (positions [N, 2] float64: the entry of a held node, else 0; held [N] bool: entry
+    AND component not touched; number of held nodes; number of touched components).  Raises ParseError on
+    bytes the decoder rejects, ValueError on a component id out of range."""
+    L = _lib()
+    buf = np.frombuffer(data, dtype=np.uint8)
+    blob, off = _names_blob(list(image_names))
+    img = np.ascontiguousarray(node_image, dtype=np.uint32).reshape(-1)
+    feat = np.ascontiguousarray(node_feat, dtype=np.uint32).reshape(-1)
+    comp = np.ascontiguousarray(node_comp, dtype=np.uint32).reshape(-1)
+    N = int(img.shape[0])
+    if N and int(comp.max()) >= n_components:
+        raise ValueError("a component id is out of range")
+    pos = np.zeros((N, 2), np.float64)
+    held = np.zeros(N, np.uint8)
+    n = C.c_uint64()
+    t = C.c_uint32()
+    rc = L.lfr_wire_update_solution(buf.ctypes.data if buf.size else None, buf.size, len(image_names), blob.ctypes.data,
+                                    off.ctypes.data, N, img.ctypes.data if N else None, feat.ctypes.data if N else None,
+                                    comp.ctypes.data if N else None, int(n_components), pos.ctypes.data if N else None,
+                                    held.ctypes.data if N else None, C.byref(n), C.byref(t))
+    if rc != 0:
+        raise ParseError("Failed to parse proto object.")
+    return pos, held.astype(bool), int(n.value), int(t.value)
