@@ -171,7 +171,9 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
   // doubles:  0 cost at x, 1 gmax, 2 lm_step's validity (1 / 0, before the driver's model_change > 0
   // test, except on the shared-memory Cholesky tier, whose lm_step applies that test itself and then
   // leaves g . dl and |dl|_inf at 0 and dl unwritten), 3 model cost change, 4 g . dl, 5 |dl|_inf,
-  // 6 tier code, 7 unknowns n.
+  // 6 tier code + counter() x 2^-32 (on the CTA tier: the step's CG iterations; exact in a double for
+  // counts below 2^32, and its integer part is the tier code, as readers of the tier word take it),
+  // 7 unknowns n.
   {
     double mc = 0.0, gd = 0.0, dmax = 0.0;
     const bool valid = T.lm_step(K.radius0, &mc, &gd, &dmax);
@@ -186,7 +188,8 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
       P.st_cost1[c] = cost;
       P.st_ls[c] = 0;
       if (P.st_cycles) {
-        const double rec[8] = {cost, gmax, valid ? 1.0 : 0.0, mc, gd, dmax, (double)Tier::kTier, (double)C.n};
+        const double rec[8] = {cost, gmax, valid ? 1.0 : 0.0, mc, gd, dmax,
+                               (double)Tier::kTier + 0x1p-32 * (double)T.counter(), (double)C.n};
         for (int k = 0; k < 8; ++k) P.st_cycles[8 * (size_t)c + k] = (unsigned long long)__double_as_longlong(rec[k]);
       }
     }
@@ -202,11 +205,13 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
   //   0 < ls_suff <= 1 (mode A, alpha = ls_suff): dl goes to positions_out at the free coordinates; then
   //     trial(alpha), step_norm(), trial_slope(alpha), slope(), accept(), assemble(false), and the record
   //     holds, as doubles:  0 cost by trial, 1 cost by trial_slope, 2 phi' by trial_slope, 3 phi' by
-  //     slope(), 4 |x - xc|, 5 |xc| (accept's return), 6 gmax at xc, 7 tier code.
+  //     slope(), 4 |x - xc|, 5 |xc| (accept's return), 6 gmax at xc, 7 tier code + counter() x 2^-32
+  //     after the first step (on the CTA tier: its CG iterations).
   //   ls_suff < 0 (mode B, alpha = -ls_suff): the same sequence, then a second lm_step at the initial
   //     radius from xc with iteration 0's Jacobi scaling; its step dl2 goes to positions_out and the
   //     record has the layout of the LFR_DBG_LM_STEP build: 0 cost at xc, 1 gmax at xc, 2 validity,
-  //     3 model cost change, 4 g . dl2, 5 |dl2|_inf, 6 tier code, 7 unknowns n.
+  //     3 model cost change, 4 g . dl2, 5 |dl2|_inf, 6 tier code + 2^-32 x the counter()'s increase
+  //     over the second lm_step (on the CTA tier: dl2's CG iterations), 7 unknowns n.
   //   ls_suff > 1 (mode C, a rejected step): trial(1) and slope() (the first contraction's samples),
   //     then, as after a rejected step, reject() and lm_step at half the initial radius from the
   //     unchanged x; dl2 and the record as in mode B, with the cost and gmax at x.
@@ -215,7 +220,8 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
     const double alpha = rejected ? 1.0 : fabs(K.ls_suff);
     double mc = 0.0, gd = 0.0, dmax = 0.0;
     bool valid = T.lm_step(K.radius0, &mc, &gd, &dmax);
-    double rec_a[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, (double)Tier::kTier};
+    const unsigned long long count1 = T.counter();
+    double rec_a[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, (double)Tier::kTier + 0x1p-32 * (double)count1};
     double cost_b = cost, gmax_b = gmax;
     if (rejected) {
       T.trial(alpha);
@@ -244,7 +250,8 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
       P.st_cost1[c] = cost_b;
       P.st_ls[c] = 0;
       if (P.st_cycles) {
-        const double rec_b[8] = {cost_b, gmax_b, valid ? 1.0 : 0.0, mc, gd, dmax, (double)Tier::kTier, (double)C.n};
+        const double rec_b[8] = {cost_b, gmax_b, valid ? 1.0 : 0.0, mc, gd, dmax,
+                                 (double)Tier::kTier + 0x1p-32 * (double)(T.counter() - count1), (double)C.n};
         for (int k = 0; k < 8; ++k)
           P.st_cycles[8 * (size_t)c + k] =
               (unsigned long long)__double_as_longlong(second || rejected ? rec_b[k] : rec_a[k]);

@@ -498,30 +498,47 @@ double norm2(const std::vector<double>& v) {
 // Dense Cholesky solve of the SPD system A y = b (A is n x n, row-major, lower
 // part used).  Stands in for SPARSE_NORMAL_CHOLESKY (solve.cc:147): an exact
 // solve; ordering/sparsity only change round-off.
+// Row i's entries left of its first nonzero `first[i]` (its profile) stay +0 in
+// the factor, so the products with them are skipped.  In the factorisation and the
+// forward substitution they are the leading terms of each sum, which starts from an
+// entry of A or b (never -0): skipping them changes no bit.  In the back
+// substitution they are signed zeros among the terms, which can at most flip the
+// sign of an exact zero.  Long tracks and grids in natural order have a narrow
+// profile, which keeps components of thousands of nodes within reach.
 bool cholesky_solve(std::vector<double>& A, int n, const std::vector<double>& b,
                     std::vector<double>* y) {
+  std::vector<int> first(n);
+  for (int i = 0; i < n; ++i) {
+    int k = 0;
+    while (k < i && A[(size_t)i * n + k] == 0.0) ++k;
+    first[i] = k;
+  }
   for (int j = 0; j < n; ++j) {
-    double d = A[j * n + j];
-    for (int k = 0; k < j; ++k) d -= A[j * n + k] * A[j * n + k];
+    const double* Aj = &A[(size_t)j * n];
+    double d = Aj[j];
+    for (int k = first[j]; k < j; ++k) d -= Aj[k] * Aj[k];
     if (!(d > 0.0) || !std::isfinite(d)) return false;
     const double l = std::sqrt(d);
-    A[j * n + j] = l;
+    A[(size_t)j * n + j] = l;
     for (int i = j + 1; i < n; ++i) {
-      double s = A[i * n + j];
-      for (int k = 0; k < j; ++k) s -= A[i * n + k] * A[j * n + k];
-      A[i * n + j] = s / l;
+      if (first[i] > j) continue;  // L(i, j) = +0
+      double* Ai = &A[(size_t)i * n];
+      double s = Ai[j];
+      for (int k = std::max(first[i], first[j]); k < j; ++k) s -= Ai[k] * Aj[k];
+      Ai[j] = s / l;
     }
   }
   y->assign(n, 0.0);
   for (int i = 0; i < n; ++i) {
     double s = b[i];
-    for (int k = 0; k < i; ++k) s -= A[i * n + k] * (*y)[k];
-    (*y)[i] = s / A[i * n + i];
+    for (int k = first[i]; k < i; ++k) s -= A[(size_t)i * n + k] * (*y)[k];
+    (*y)[i] = s / A[(size_t)i * n + i];
   }
   for (int i = n - 1; i >= 0; --i) {
     double s = (*y)[i];
-    for (int k = i + 1; k < n; ++k) s -= A[k * n + i] * (*y)[k];
-    (*y)[i] = s / A[i * n + i];
+    for (int k = i + 1; k < n; ++k)
+      if (first[k] <= i) s -= A[(size_t)k * n + i] * (*y)[k];
+    (*y)[i] = s / A[(size_t)i * n + i];
   }
   for (int i = 0; i < n; ++i)
     if (!std::isfinite((*y)[i])) return false;

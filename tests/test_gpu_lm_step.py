@@ -4,8 +4,9 @@ damped system (tests/lm_step_ref.py).
 Whole solves against the oracle cannot see a slightly wrong step: LM corrects it in the next iteration.
 So these tests stop every component after its first step.  liblfr_b200_lmstep.so is the product built
 with -DLFR_DBG_LM_STEP (csrc/build.py): lm_solve takes iteration 0 and one lm_step at the initial radius,
-writes dl to the free nodes' positions and {cost, gmax, validity, model change, g . dl, |dl|_inf, tier,
-n} to the slot's LFR_DBG_PROFILE record, and returns.
+writes dl to the free nodes' positions and {cost, gmax, validity, model change, g . dl, |dl|_inf, tier
+(its integer part; the fraction is the tier's counter x 2^-32: CG iterations on the CTA tier), n} to the
+slot's LFR_DBG_PROFILE record, and returns.
 
 Components are built directly as lfr_problem arrays: every register class edge of the warp2 tier (in
 its per-bucket launches and in the queue kernel), the tile tier at 64 and 128 threads, the shared-memory
@@ -261,6 +262,12 @@ def lmstep():
     return lib
 
 
+def counter_of(word):
+    """The tier's counter carried by a record's tier word, tier + counter x 2^-32 (csrc/lfr_lm.cuh): the
+    step's CG iterations on the CTA tier."""
+    return int(round((word - int(word)) * 2.0 ** 32))
+
+
 def first_steps(lib, p, route, start, **opts):
     """(positions [N, 2] with dl at the free nodes, records [C, 8] as doubles) of one launch."""
     from lfr_b200 import capi
@@ -306,7 +313,7 @@ def statements(key, p, start, opts):
 
 
 def check(lib, report, key, p, start, route, opts):
-    """Runs one launch and holds every slot to the acceptance bar.  Returns the positions."""
+    """Runs one launch and holds every slot to the acceptance bar.  Returns the positions and records."""
     pos, rec = first_steps(lib, p, route, start, **opts)
     roots = p.is_root != 0
     assert np.array_equal(pos[roots], start[roots]), (key, route, "roots moved")
@@ -338,7 +345,7 @@ def check(lib, report, key, p, start, route, opts):
         w[0] = max(w[0], err / (n * st.kappa * U * norm) if norm else 0.0)
         w[1] = max(w[1], st.kappa)
         w[2] += 1
-    return pos
+    return pos, rec
 
 
 # ---------------------------------------------------------------------------------------------------
