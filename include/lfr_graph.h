@@ -164,6 +164,43 @@ int lfr_plan_keep_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, u
 int lfr_plan_update_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                              const uint8_t* names, const uint64_t* name_off, uint64_t* n_held, uint32_t* n_touched);
 
+/* lfr_plan_update_solution() that also sees every change of the matches since the earlier run: given the
+ * MatchingFile that produced the SolutionFile, it holds a component only when its problem is the problem the
+ * earlier run solved, and touches every other one.
+ *
+ * The rule.  The *earlier run* is the graph stage (solve.cc:438-606) over every pair of the earlier
+ * MatchingFile OLD, no image banned (a run that banned images is described by a file without their pairs);
+ * its cut cap is OLD's own image count.  A keypoint is identified by (exact image-name bytes, feature_idx).
+ * A component C of this plan (lfr_problem.comp, after the cut; one-node components count) is *unchanged*
+ * when the earlier run has a component C' such that
+ *   1. C' has the same keypoints as C;
+ *   2. the same keypoints are roots (the reference's is_root) in both;
+ *   3. every keypoint has the same multiset of kept out-edges in both.  An edge is kept when its kind is not
+ *      LFR_EDGE_SKIP (same track: Cauchy, same component: Tukey); it is compared on its destination keypoint,
+ *      its kind and the bits of sim and of the 18 flow floats (-0.0 is not +0.0; NaN payloads count).
+ * Skipped edges and the order of nodes and edges do not enter the rule, and the comparison is exact.  C is
+ * *held* when it is unchanged AND every one of its keypoints has an entry in the SolutionFile (the rule of
+ * lfr_wire_join_solution_entries()); every other component is *touched* and treated as
+ * lfr_plan_update_solution() treats its touched components: it starts at 0 with the constant mask root OR
+ * fixed image, and solves bit for bit as in a plan never given a file.  A held component's nodes are all
+ * constant at the file's float bits.  The touched set contains lfr_plan_update_solution()'s.
+ *
+ * `previous` is a plan made by lfr_plan_create_from_matches() or _from_wire() from OLD on the same device;
+ * it is read, not changed, and may be destroyed when the call returns.  prev_names / prev_name_off are its
+ * image names by id (prev_n_images at least its n_images), mapped to this plan's names / name_off by their
+ * bytes; names only the earlier run has get ids after this plan's.  Keys, sorts, joins and the exact compare
+ * run on the device (csrc/lfr_diff.cuh); the held flags, start positions, constant mask and schedule are
+ * lfr_plan_update_solution()'s.  *n_held, *n_touched (each may be NULL) as lfr_plan_update_solution();
+ * *n_changed (may be NULL) = the components that are not unchanged.  Synchronous on `stream`.  LFR_EINVAL as
+ * lfr_plan_update_solution(), for a `previous` not made from matches, on another device or equal to `plan`,
+ * and for malformed or repeated earlier names (the plan is not changed then); LFR_EUNSUPPORTED for 2^31 or
+ * more directed edges in the two plans together.  lfr_wire_update_solution_since() (include/lfr_host.h) is
+ * the host form, bit for bit. */
+int lfr_plan_update_solution_since(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                                   const uint8_t* names, const uint64_t* name_off, const lfr_plan* previous,
+                                   uint32_t prev_n_images, const uint8_t* prev_names, const uint64_t* prev_name_off,
+                                   uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed);
+
 /* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
  * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from
  * sizes known before either stage runs — the directed edges (2 x the matches of the pairs not skipped),

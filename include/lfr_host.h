@@ -67,6 +67,24 @@ int lfr_host_stage_export(const lfr_host_stage* hs,
 
 void lfr_host_stage_destroy(lfr_host_stage* hs);
 
+/* The host form of lfr_plan_update_solution_since() (include/lfr_graph.h, which states the rule), bit for
+ * bit: `p` is this run's problem (the reference's is_root, not a constant mask) with node ids
+ * node_image / node_feat, image names by id names / name_off (n_images); `previous` is the earlier
+ * MatchingFile's lfr_host_input (its pair_skip and edges_out are ignored: the earlier run bans no image) with
+ * its names prev_names / prev_name_off (previous->n_images).  Runs lfr_host_stage_create() on `previous`,
+ * marks the components that are not unchanged, then joins the SolutionFile `buf` as
+ * lfr_wire_update_solution() does with those components touched too: positions [2 n_nodes], held [n_nodes],
+ * *n_held and *n_touched mean what they mean there; *n_changed (may be NULL) = the components that are not
+ * unchanged.  LFR_EINVAL for malformed bytes, NULL or inconsistent arrays, or malformed or repeated earlier
+ * names; the earlier stage's codes (lfr_host_stage_create) when it rejects `previous`.  Every output is
+ * untouched on error. */
+int lfr_wire_update_solution_since(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                                   const uint64_t* name_off, const lfr_problem* p, const uint32_t* node_image,
+                                   const uint32_t* node_feat, const lfr_host_input* previous, const uint8_t* prev_names,
+                                   const uint64_t* prev_name_off, double* positions /* [2 n_nodes] */,
+                                   uint8_t* held /* [n_nodes] */, uint64_t* n_held, uint32_t* n_touched,
+                                   uint32_t* n_changed);
+
 #ifdef __cplusplus
 }
 #endif

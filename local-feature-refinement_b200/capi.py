@@ -82,7 +82,7 @@ ABI_SYMBOLS = [
 GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
                  "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
                  "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution",
-                 "lfr_plan_encode_solution_carried", "lfr_plan_update_solution"]
+                 "lfr_plan_encode_solution_carried", "lfr_plan_update_solution", "lfr_plan_update_solution_since"]
 
 
 class LfrWirePart(C.Structure):
@@ -164,6 +164,10 @@ class Library:
             L.lfr_plan_keep_solution.restype = C.c_int
             L.lfr_plan_update_solution.argtypes = L.lfr_plan_start_from_solution.argtypes + [C.POINTER(C.c_uint32)]
             L.lfr_plan_update_solution.restype = C.c_int
+            L.lfr_plan_update_solution_since.argtypes = (L.lfr_plan_start_from_solution.argtypes[:7] + [C.c_void_p, C.c_uint32] +
+                                                         [C.c_void_p] * 2 + [C.POINTER(C.c_uint64)] +
+                                                         [C.POINTER(C.c_uint32)] * 2)
+            L.lfr_plan_update_solution_since.restype = C.c_int
             L.lfr_plan_encode_solution_carried.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
                                                            C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                                            C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
@@ -361,6 +365,7 @@ class Plan:
             _, arrs = host_input_arrays(matches, banned_images)
             n_images = len(matches.image_names) if n_images is None else n_images
         inp = _host_input(arrs, n_images)
+        names = None if isinstance(matches, dict) else list(matches.image_names)
         if not lib.has_graph_stage:  # e.g. the CPU oracle: no device, no plans
             raise RuntimeError("lfr: lfr_plan_create_from_matches failed (-5): %s does not provide the graph stage "
                                "on the GPU (include/lfr_graph.h)" % lib.path)
@@ -375,6 +380,7 @@ class Plan:
         self.handle = h
         self.sizes = {k: getattr(sz, k) for k in HOST_SIZES_FIELDS}
         self.n_nodes, self.n_components = int(sz.n_nodes), int(sz.n_components)
+        self.image_names = names
         return self
 
     @classmethod
@@ -527,16 +533,32 @@ class Plan:
                        "lfr_plan_keep_solution")
         return int(n.value)
 
-    def update_solution(self, data: bytes, image_names, stream: int = 0):
+    def update_solution(self, data: bytes, image_names, stream: int = 0, previous: Optional["Plan"] = None,
+                        previous_names=None):
         """lfr_plan_update_solution (include/lfr_graph.h): every component with a node that has no entry in
         `data` is touched and solves from zeros as without a file; every other component is held constant at
         the file's values.  Replaces an earlier kept or held set (an empty file clears it) and composes with
-        fix_images() in either order.  Returns (held nodes, touched components)."""
+        fix_images() in either order.  Returns (held nodes, touched components).
+
+        With `previous`, a plan made by from_matches() or from_wire() on the MatchingFile that produced `data`
+        (every pair, no banned image), lfr_plan_update_solution_since: a component is held only when it is
+        also unchanged since that run (the rule in include/lfr_graph.h).  `previous_names` are its image names
+        by id (default: previous.image_names).  Returns (held nodes, touched components, changed components);
+        `previous` is not changed."""
         from .wire import _names_blob
         buf = np.frombuffer(data, dtype=np.uint8)
         blob, off = _names_blob(list(image_names))
         n = C.c_uint64()
         t = C.c_uint32()
+        if previous is not None:
+            pnames = list(previous.image_names if previous_names is None else previous_names)
+            pblob, poff = _names_blob(pnames)
+            ch = C.c_uint32()
+            self.lib.check(self.lib.lib.lfr_plan_update_solution_since(
+                self.handle, C.c_void_p(stream), buf.ctypes.data if buf.size else None, buf.size, len(image_names),
+                blob.ctypes.data, off.ctypes.data, previous.handle, len(pnames), pblob.ctypes.data, poff.ctypes.data,
+                C.byref(n), C.byref(t), C.byref(ch)), "lfr_plan_update_solution_since")
+            return int(n.value), int(t.value), int(ch.value)
         self.lib.check(self.lib.lib.lfr_plan_update_solution(self.handle, C.c_void_p(stream),
                                                              buf.ctypes.data if buf.size else None, buf.size,
                                                              len(image_names), blob.ctypes.data, off.ctypes.data,

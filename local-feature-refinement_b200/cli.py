@@ -19,6 +19,10 @@ of that file the solve does not refine (wire.encode_solution_carried), so new pa
 --update_initial_solution (with --initial_solution, not with --keep_initial_solution) solves every component
 that a keypoint without an entry in that file joins from zeros, as a run without the file does, and holds
 every other component at the file's values (wire.update_solution, Plan.update_solution).
+--previous_matches_file OLD.pb (with --update_initial_solution; `.part.N` pieces as for --matches_file) names
+the MatchingFile that produced the initial solution: a component is then also solved again when its problem
+is not the one OLD.pb's run solved, so banned images, new pairs between old images and changed network output
+no longer leave stale values (the rule is in include/lfr_graph.h).
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -55,7 +59,7 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("device", True, False), ("gpus", True, False), ("stats_json", True, False),
             ("fixed_images", True, True), ("initial_solution", True, False),
             ("keep_initial_solution", False, False), ("carry_initial_solution", False, False),
-            ("update_initial_solution", False, False)]
+            ("update_initial_solution", False, False), ("previous_matches_file", True, False)]
 
 
 def _find_option(name):
@@ -132,7 +136,8 @@ def parse_args(argv):
             fixed_images=vals.get("fixed_images", []), initial_solution=vals.get("initial_solution"),
             keep_initial_solution=bool(vals.get("keep_initial_solution")),
             carry_initial_solution=bool(vals.get("carry_initial_solution")),
-            update_initial_solution=bool(vals.get("update_initial_solution")))
+            update_initial_solution=bool(vals.get("update_initial_solution")),
+            previous_matches_file=vals.get("previous_matches_file"))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -160,6 +165,9 @@ def main(argv=None) -> int:
     if args.update_initial_solution and args.keep_initial_solution:
         sys.stderr.write("ERROR: --update_initial_solution and --keep_initial_solution exclude each other\n")
         return 2
+    if args.previous_matches_file is not None and not args.update_initial_solution:
+        sys.stderr.write("ERROR: --previous_matches_file needs --update_initial_solution\n")
+        return 2
     start = None
     if args.initial_solution is not None:
         try:
@@ -170,6 +178,18 @@ def main(argv=None) -> int:
             return 2
         try:
             wire.decode_solution(start)
+        except wire.ParseError:
+            sys.stderr.write("Failed to parse proto object.\n")
+            return 255
+    previous = None
+    if args.previous_matches_file is not None:
+        try:
+            if not wire.matches_files(args.previous_matches_file):
+                raise OSError(args.previous_matches_file)
+            previous = wire.read_matching_file(args.previous_matches_file)
+        except OSError:
+            sys.stderr.write("ERROR: cannot read the previous matches file '%s'\n" % args.previous_matches_file)
+            return 2
         except wire.ParseError:
             sys.stderr.write("Failed to parse proto object.\n")
             return 255
@@ -225,7 +245,7 @@ def main(argv=None) -> int:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
                                  timing=timing, fixed_images=args.fixed_images, initial_solution=start,
                                  keep_initial_solution=args.keep_initial_solution,
-                                 update_initial_solution=args.update_initial_solution)
+                                 update_initial_solution=args.update_initial_solution, previous_matches=previous)
     except GraphStageRouteError as e:
         sys.stderr.write("ERROR: %s\n" % e)
         return 2

@@ -18,6 +18,7 @@
 #include "lfr_carry.cuh"
 #include "lfr_cut.h"
 #include "lfr_cut.cuh"
+#include "lfr_diff.cuh"
 #include "lfr_graph.cuh"
 #include "lfr_solution.cuh"
 #include "lfr_solve_cta.cuh"
@@ -2364,6 +2365,115 @@ int64_t encode_solution_carried(lfr_plan* pl, cudaStream_t s, uint32_t NI, const
   return (int64_t)total;
 }
 
+// lfr_plan_update_solution() after the decode, with the touched flags seeded from changed[C] on the device
+// (NULL: none; lfr_plan_update_solution_since)
+int update_solution(lfr_plan* pl, cudaStream_t s, const lfr::join::Decoded& d, const uint8_t* changed, uint64_t* n_held,
+                    uint32_t* n_touched) {
+  const uint32_t N = pl->N, C = pl->C;
+  if (!pl->kept.p) {  // cleared, so that a join that fails before its kernel leaves no stale flags
+    LFR_TRY(pl->kept.reserve(std::max<size_t>(N, 1)));
+    LFR_CUDA(cudaMemsetAsync(pl->kept.p, 0, std::max<size_t>(N, 1), s));
+  }
+  // the kept flags take the join's "has entry", then the held flags in place
+  LFR_TRY(join_solution(pl, s, d, pl->kept.as<uint8_t>(), nullptr));
+  unsigned long long counts[2] = {0, 0};  // held nodes, touched components
+  if (N) {
+    TmpBuf t;  // the two counters, then one touched flag per component
+    LFR_TRY(t.reserve(16 + (size_t)C));
+    auto* ctr = t.as<unsigned long long>();
+    uint8_t* touched = t.as<uint8_t>() + 16;
+    LFR_CUDA(cudaMemsetAsync(t.p, 0, 16 + (size_t)C, s));
+    if (changed && C) LFR_CUDA(cudaMemcpyAsync(touched, changed, C, cudaMemcpyDeviceToDevice, s));
+    lfr::start::touch_kernel<<<blocks_for(N), 256, 0, s>>>(pl->kept.as<uint8_t>(), pl->comp.as<uint32_t>(), N, touched);
+    lfr::start::update_kernel<<<blocks_for(N), 256, 0, s>>>(pl->comp.as<uint32_t>(), touched, N, pl->kept.as<uint8_t>(),
+                                                              pl->pos_init.as<double>(), pl->pos.as<double>(), ctr);
+    lfr::start::count_touched_kernel<<<blocks_for(C), 256, 0, s>>>(touched, C, ctr + 1);
+    LFR_LAUNCHED();
+    LFR_TRY(fetch(counts, ctr, 2, s));  // before `t` is freed
+  }
+  if (n_held) *n_held = counts[0];
+  if (n_touched) *n_touched = (uint32_t)counts[1];
+  return build_constant_mask(pl, s);
+}
+
+// lfr_plan_update_solution_since(): changed[c] = 1 (device, C flags) for every component c of `pl` that fails
+// the "unchanged" test against `prev` (lfr_diff.cuh); `image_map` (host, prev's image count) gives prev's image
+// ids in pl's numbering.  *n_changed = the count.  Reads both plans, changes neither.
+int diff_components(const lfr_plan* pl, const lfr_plan* prev, const std::vector<uint32_t>& image_map, cudaStream_t s,
+                    uint8_t* changed, uint32_t* n_changed) {
+  using namespace lfr::diff;
+  const uint32_t N = pl->N, C = pl->C, M = prev->N, PC = prev->C;
+  const uint64_t E = pl->E, EB = prev->E, R = E + EB;
+  LFR_CUDA(cudaMemsetAsync(changed, 0, std::max<size_t>(C, 1), s));
+  *n_changed = 0;
+  if (!N) return LFR_OK;
+  if (R >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "2^31 or more directed edges in the two plans");
+  TmpBuf tmp, d_map, d_key, d_key_s, d_idx, d_idx_s, d_inv, d_lo, d_hi, d_size, d_psize, d_ekey, d_ekey_s, d_eval, d_eval_s, d_ctr;
+  LFR_TRY(d_map.reserve(4 * std::max<size_t>(image_map.size(), 1)));
+  for (TmpBuf* b : {&d_key, &d_key_s}) LFR_TRY(b->reserve(8 * std::max<size_t>(M, 1)));
+  for (TmpBuf* b : {&d_idx, &d_idx_s, &d_inv}) LFR_TRY(b->reserve(4 * std::max<size_t>(M, 1)));
+  for (TmpBuf* b : {&d_lo, &d_hi, &d_size}) LFR_TRY(b->reserve(4 * (size_t)C));
+  LFR_TRY(d_psize.reserve(4 * std::max<size_t>(PC, 1)));
+  for (TmpBuf* b : {&d_ekey, &d_ekey_s, &d_eval, &d_eval_s}) LFR_TRY(b->reserve(8 * std::max<size_t>(R, 1)));
+  LFR_TRY(d_ctr.reserve(8));
+  auto* key = d_key.as<unsigned long long>();
+  auto* key_s = d_key_s.as<unsigned long long>();
+  auto* lo = d_lo.as<uint32_t>();
+  auto* hi = d_hi.as<uint32_t>();
+  auto* size = d_size.as<uint32_t>();
+  auto* psize = d_psize.as<uint32_t>();
+  auto* inv = d_inv.as<uint32_t>();
+  if (!image_map.empty())
+    LFR_CUDA(cudaMemcpyAsync(d_map.p, image_map.data(), 4 * image_map.size(), cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemsetAsync(lo, 0xff, 4 * (size_t)C, s));
+  LFR_CUDA(cudaMemsetAsync(hi, 0, 4 * (size_t)C, s));
+  LFR_CUDA(cudaMemsetAsync(size, 0, 4 * (size_t)C, s));
+  LFR_CUDA(cudaMemsetAsync(psize, 0, 4 * std::max<size_t>(PC, 1), s));
+  LFR_CUDA(cudaMemsetAsync(inv, 0xff, 4 * std::max<size_t>(M, 1), s));
+  LFR_CUDA(cudaMemsetAsync(d_ctr.p, 0, 8, s));
+  if (M) {
+    prev_key_kernel<<<blocks_for(M), 256, 0, s>>>(prev->node_image.as<uint32_t>(), prev->node_feat.as<uint32_t>(), M,
+                                                  d_map.as<uint32_t>(), key, d_idx.as<uint32_t>());
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {  // keys are distinct: the mapped names are
+      return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, d_idx.as<uint32_t>(), d_idx_s.as<uint32_t>(), (int)M, 0, 64, s);
+    }));
+    size_kernel<<<blocks_for(M), 256, 0, s>>>(prev->comp.as<uint32_t>(), M, psize);
+    LFR_LAUNCHED();
+  }
+  node_kernel<<<blocks_for(N), 256, 0, s>>>(pl->node_image.as<uint32_t>(), pl->node_feat.as<uint32_t>(), pl->comp.as<uint32_t>(),
+                                            pl->is_root.as<uint8_t>(), N, key_s, d_idx_s.as<uint32_t>(), M,
+                                            prev->comp.as<uint32_t>(), prev->is_root.as<uint8_t>(), inv, lo, hi, size, changed);
+  comp_kernel<<<blocks_for(C), 256, 0, s>>>(lo, hi, size, psize, C, changed);
+  LFR_LAUNCHED();
+  const unsigned long long sentinel = (unsigned long long)N << 32;
+  auto* ekey = d_ekey.as<unsigned long long>();
+  auto* eval = d_eval.as<unsigned long long>();
+  if (E)
+    edge_key_kernel<<<blocks_for(E), 256, 0, s>>>(pl->row_ptr.as<uint32_t>(), pl->edges.as<float4>(), pl->track.as<uint32_t>(),
+                                                  pl->comp.as<uint32_t>(), N, (uint32_t)E, nullptr, 0ull, sentinel, ekey, eval);
+  if (EB)
+    edge_key_kernel<<<blocks_for(EB), 256, 0, s>>>(prev->row_ptr.as<uint32_t>(), prev->edges.as<float4>(),
+                                                   prev->track.as<uint32_t>(), prev->comp.as<uint32_t>(), M, (uint32_t)EB, inv,
+                                                   1ull, sentinel, ekey + E, eval + E);
+  LFR_LAUNCHED();
+  if (R) {
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, ekey, d_ekey_s.as<unsigned long long>(), eval,
+                                             d_eval_s.as<unsigned long long>(), (int)R, 0, 32 + bits_for(N), s);
+    }));
+    run_kernel<<<blocks_for(R), 256, 0, s>>>(d_ekey_s.as<unsigned long long>(), d_eval_s.as<unsigned long long>(), (uint32_t)R,
+                                             sentinel, pl->edges.as<uint32_t>(), prev->edges.as<uint32_t>(),
+                                             pl->comp.as<uint32_t>(), changed);
+    LFR_LAUNCHED();
+  }
+  lfr::start::count_touched_kernel<<<blocks_for(C), 256, 0, s>>>(changed, C, d_ctr.as<unsigned long long>());
+  LFR_LAUNCHED();
+  unsigned long long nc = 0;
+  LFR_TRY(fetch(&nc, d_ctr.p, 1, s));  // before the scratch is freed
+  *n_changed = (uint32_t)nc;
+  return LFR_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -2550,31 +2660,31 @@ int lfr_plan_update_solution(lfr_plan* pl, void* stream, const uint8_t* bytes, u
   lfr::join::Decoded d;
   LFR_TRY(decode_solution_for(pl, bytes, len, n_images, names, name_off, d));
   LFR_CUDA(cudaSetDevice(pl->device));
+  return update_solution(pl, (cudaStream_t)stream, d, nullptr, n_held, n_touched);
+}
+
+int lfr_plan_update_solution_since(lfr_plan* pl, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                                   const uint8_t* names, const uint64_t* name_off, const lfr_plan* previous,
+                                   uint32_t prev_n_images, const uint8_t* prev_names, const uint64_t* prev_name_off,
+                                   uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed) {
+  lfr::join::Decoded d;
+  LFR_TRY(decode_solution_for(pl, bytes, len, n_images, names, name_off, d));
+  if (!previous || !previous->graph) return fail(LFR_EINVAL, "previous plan was not made by lfr_plan_create_from_matches");
+  if (previous == pl) return fail(LFR_EINVAL, "previous plan is the plan itself");
+  if (previous->device != pl->device) return fail(LFR_EINVAL, "previous plan is on another device");
+  if (prev_n_images < previous->n_images) return fail(LFR_EINVAL, "prev_n_images is smaller than the previous plan's image count");
+  std::vector<uint32_t> image_map;
+  if (lfr::join::map_previous_images(n_images, names, name_off, prev_n_images, prev_names, prev_name_off, image_map) != LFR_OK)
+    return fail(LFR_EINVAL, "malformed or repeated previous image names");
+  LFR_CUDA(cudaSetDevice(pl->device));
   const cudaStream_t s = (cudaStream_t)stream;
-  const uint32_t N = pl->N, C = pl->C;
-  if (!pl->kept.p) {  // cleared, so that a join that fails before its kernel leaves no stale flags
-    LFR_TRY(pl->kept.reserve(std::max<size_t>(N, 1)));
-    LFR_CUDA(cudaMemsetAsync(pl->kept.p, 0, std::max<size_t>(N, 1), s));
-  }
-  // the kept flags take the join's "has entry", then the held flags in place
-  LFR_TRY(join_solution(pl, s, d, pl->kept.as<uint8_t>(), nullptr));
-  unsigned long long counts[2] = {0, 0};  // held nodes, touched components
-  if (N) {
-    TmpBuf t;  // the two counters, then one touched flag per component
-    LFR_TRY(t.reserve(16 + (size_t)C));
-    auto* ctr = t.as<unsigned long long>();
-    uint8_t* touched = t.as<uint8_t>() + 16;
-    LFR_CUDA(cudaMemsetAsync(t.p, 0, 16 + (size_t)C, s));
-    lfr::start::touch_kernel<<<blocks_for(N), 256, 0, s>>>(pl->kept.as<uint8_t>(), pl->comp.as<uint32_t>(), N, touched);
-    lfr::start::update_kernel<<<blocks_for(N), 256, 0, s>>>(pl->comp.as<uint32_t>(), touched, N, pl->kept.as<uint8_t>(),
-                                                              pl->pos_init.as<double>(), pl->pos.as<double>(), ctr);
-    lfr::start::count_touched_kernel<<<blocks_for(C), 256, 0, s>>>(touched, C, ctr + 1);
-    LFR_LAUNCHED();
-    LFR_TRY(fetch(counts, ctr, 2, s));  // before `t` is freed
-  }
-  if (n_held) *n_held = counts[0];
-  if (n_touched) *n_touched = (uint32_t)counts[1];
-  return build_constant_mask(pl, s);
+  TmpBuf changed;
+  LFR_TRY(changed.reserve(std::max<size_t>(pl->C, 1)));
+  uint32_t nc = 0;
+  LFR_TRY(diff_components(pl, previous, image_map, s, changed.as<uint8_t>(), &nc));
+  LFR_TRY(update_solution(pl, s, d, changed.as<uint8_t>(), n_held, n_touched));
+  if (n_changed) *n_changed = nc;
+  return LFR_OK;
 }
 
 int64_t lfr_plan_encode_solution_carried(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,

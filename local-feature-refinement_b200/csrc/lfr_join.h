@@ -134,17 +134,22 @@ inline int join_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const
 }
 
 // The host update (lfr_wire_update_solution): join_nodes() with its flags, then every component with a node
-// without an entry is touched; its nodes start at 0 and are not held.  held[v] = has entry AND component not
-// touched.  Every output is untouched when the arguments or the bytes are rejected (LFR_EINVAL).
+// without an entry is touched, and so is every component with changed[c] != 0 (`changed` may be NULL: none;
+// lfr_wire_update_solution_since); a touched component's nodes start at 0 and are not held.  held[v] = has
+// entry AND component not touched.  Every output is untouched when the arguments or the bytes are rejected
+// (LFR_EINVAL).
 inline int update_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
                         uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, const uint32_t* node_comp,
-                        uint32_t n_components, double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched) {
+                        uint32_t n_components, double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched,
+                        const uint8_t* changed = nullptr) {
   if (n_nodes && (!node_comp || !held)) return LFR_EINVAL;
   for (uint32_t v = 0; v < n_nodes; ++v)
     if (node_comp[v] >= n_components) return LFR_EINVAL;
   const int rc = join_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions, held, nullptr);
   if (rc != LFR_OK) return rc;
   std::vector<uint8_t> touched(n_components, 0);
+  if (changed)
+    for (uint32_t c = 0; c < n_components; ++c) touched[c] = changed[c] ? 1 : 0;
   for (uint32_t v = 0; v < n_nodes; ++v)
     if (!held[v]) touched[node_comp[v]] = 1;
   uint64_t nh = 0;
@@ -158,6 +163,36 @@ inline int update_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, con
   }
   if (n_held) *n_held = nh;
   if (n_touched) *n_touched = (uint32_t)std::count(touched.begin(), touched.end(), (uint8_t)1);
+  return LFR_OK;
+}
+
+// The earlier run's image ids in this run's numbering, by exact name bytes (lfr_wire_update_solution_since,
+// lfr_plan_update_solution_since): map[k] = the id of earlier name k among names / name_off, or, for a name
+// this run does not have, n_images + (its rank among such names).  LFR_EINVAL for NULL or descending offsets
+// and for a name repeated among the earlier names (it would give two earlier keypoints one key).
+inline int map_previous_images(uint32_t n_images, const uint8_t* names, const uint64_t* name_off, uint32_t prev_n_images,
+                               const uint8_t* prev_names, const uint64_t* prev_name_off, std::vector<uint32_t>& map) {
+  if ((n_images && !name_off) || (prev_n_images && !prev_name_off)) return LFR_EINVAL;
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return LFR_EINVAL;
+  for (uint32_t k = 0; k < prev_n_images; ++k)
+    if (prev_name_off[k + 1] < prev_name_off[k]) return LFR_EINVAL;
+  if ((n_images && name_off[n_images] && !names) || (prev_n_images && prev_name_off[prev_n_images] && !prev_names))
+    return LFR_EINVAL;
+  std::unordered_map<std::string, uint32_t> id_of;
+  id_of.reserve(n_images);
+  for (uint32_t k = 0; k < n_images; ++k)
+    id_of.emplace(std::string(reinterpret_cast<const char*>(names) + name_off[k], name_off[k + 1] - name_off[k]), k);
+  std::unordered_map<std::string, uint32_t> seen;
+  seen.reserve(prev_n_images);
+  map.assign(prev_n_images, 0);
+  uint32_t extra = 0;
+  for (uint32_t k = 0; k < prev_n_images; ++k) {
+    std::string s(reinterpret_cast<const char*>(prev_names) + prev_name_off[k], prev_name_off[k + 1] - prev_name_off[k]);
+    if (!seen.emplace(s, k).second) return LFR_EINVAL;
+    const auto it = id_of.find(s);
+    map[k] = it != id_of.end() ? it->second : n_images + extra++;
+  }
   return LFR_OK;
 }
 

@@ -29,7 +29,9 @@
 // route's assembly) and --update_initial_solution (every component a keypoint without an entry in that
 // file joins is solved from zeros as without the file, every other one is held at the file's values:
 // lfr_plan_update_solution() on the device route, lfr_wire_update_solution() handed to the solve on the host
-// route).  `--n_threads` is accepted and
+// route) and --previous_matches_file OLD.pb (with --update_initial_solution: a component is also solved again
+// when its problem is not the one OLD.pb's run solved: lfr_plan_update_solution_since() with a plan built from
+// OLD.pb on the device route, lfr_wire_update_solution_since() on the host route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -76,6 +78,10 @@ int lfr_plan_keep_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, u
 int lfr_plan_update_solution(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
                              const uint8_t* names, const uint64_t* name_off, uint64_t* n_held,
                              uint32_t* n_touched) __attribute__((weak));
+int lfr_plan_update_solution_since(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                                   const uint8_t* names, const uint64_t* name_off, const lfr_plan* previous,
+                                   uint32_t prev_n_images, const uint8_t* prev_names, const uint64_t* prev_name_off,
+                                   uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed) __attribute__((weak));
 int64_t lfr_plan_encode_solution_carried(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
                                          const uint64_t* name_off, const float* fact, const uint8_t* file,
                                          uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
@@ -105,7 +111,7 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"n_threads", true, false},    {"banned_images", true, true}, {"device", true, false},
                                {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false},
                                {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false},
-                               {"update_initial_solution", false, false}};
+                               {"update_initial_solution", false, false}, {"previous_matches_file", true, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -221,6 +227,25 @@ struct FileImage {
   size_t size() const { return n; }
 };
 
+// The earlier MatchingFile of --previous_matches_file, decoded on the host: its image names by id (in order of
+// first appearance over its parts) and the flat arrays of its lfr_host_input, no image banned.
+struct PreviousMatches {
+  std::vector<std::string> names;
+  std::vector<uint8_t> name_blob;
+  std::vector<uint64_t> name_off{0};
+  std::vector<uint32_t> pair_img1, pair_img2, feat1, feat2;
+  std::vector<uint64_t> pair_ptr{0};
+  std::vector<float> sim, disp1, disp2;
+  lfr_host_input input() const {
+    lfr_host_input in;
+    std::memset(&in, 0, sizeof in);
+    in.n_pairs = pair_img1.size(); in.n_matches = feat1.size(); in.n_images = (uint32_t)names.size();
+    in.pair_img1 = pair_img1.data(); in.pair_img2 = pair_img2.data(); in.pair_ptr = pair_ptr.data();
+    in.feat1 = feat1.data(); in.feat2 = feat2.data(); in.sim = sim.data(); in.disp1 = disp1.data(); in.disp2 = disp2.data();
+    return in;
+  }
+};
+
 // One MatchingFile part after the pair walk: image names as byte ranges of its buffer, the matches as
 // the offsets of their length prefixes.
 struct Part {
@@ -240,6 +265,56 @@ struct Part {
   }
 };
 
+// Read and decode the earlier MatchingFile `path` (or its .part.N pieces, as --matches_file): 0, 2 when no
+// file can be read, 255 when the bytes do not parse.
+int read_previous(const std::string& path, PreviousMatches& pm) {
+  std::vector<std::string> files;
+  if (file_exists(path)) {
+    files.push_back(path);
+  } else {
+    for (int k = 0;; ++k) {
+      const std::string f = path + ".part." + std::to_string(k);
+      if (!file_exists(f)) break;
+      files.push_back(f);
+    }
+  }
+  if (files.empty()) return 2;
+  std::map<std::string, uint32_t> id_of;
+  for (const std::string& f : files) {
+    Part pt;
+    if (!pt.buf.open(f)) return 2;
+    if (lfr_wire_scan_matches(pt.buf.data(), pt.buf.size(), &pt.P, &pt.M) != LFR_OK) return 255;
+    pt.pair_ptr.resize(pt.P + 1);
+    pt.n1_off.resize(pt.P); pt.n2_off.resize(pt.P); pt.n1_len.resize(pt.P); pt.n2_len.resize(pt.P);
+    pt.fact1.resize(pt.P); pt.fact2.resize(pt.P);
+    const uint64_t m0 = pm.feat1.size();
+    pm.feat1.resize(m0 + pt.M); pm.feat2.resize(m0 + pt.M); pm.sim.resize(m0 + pt.M);
+    pm.disp1.resize(18 * (m0 + pt.M)); pm.disp2.resize(18 * (m0 + pt.M));
+    lfr_wire_matches w = pt.pair_level(pm.feat1.data() + m0, pm.feat2.data() + m0, pm.sim.data() + m0,
+                                       pm.disp1.data() + 18 * m0, pm.disp2.data() + 18 * m0);
+    if (lfr_wire_decode_matches(pt.buf.data(), pt.buf.size(), &w) != LFR_OK) return 255;
+    auto intern = [&](uint64_t off, uint32_t len) {
+      std::string s(reinterpret_cast<const char*>(pt.buf.data()) + off, len);
+      const auto it = id_of.find(s);
+      if (it != id_of.end()) return it->second;
+      const uint32_t id = (uint32_t)pm.names.size();
+      id_of.emplace(s, id);
+      pm.name_blob.insert(pm.name_blob.end(), s.begin(), s.end());
+      pm.name_off.push_back(pm.name_blob.size());
+      pm.names.push_back(std::move(s));
+      return id;
+    };
+    for (uint64_t p = 0; p < pt.P; ++p) {
+      pm.pair_img1.push_back(intern(pt.n1_off[p], pt.n1_len[p]));
+      pm.pair_img2.push_back(intern(pt.n2_off[p], pt.n2_len[p]));
+      pm.pair_ptr.push_back(m0 + pt.pair_ptr[p + 1]);
+    }
+    pt.buf.release();
+  }
+  if (pm.name_blob.empty()) pm.name_blob.push_back(0);
+  return 0;
+}
+
 using Clock = std::chrono::steady_clock;
 long long ms_between(Clock::time_point a, Clock::time_point b) {
   return (long long)std::chrono::duration_cast<std::chrono::milliseconds>(b - a).count();
@@ -248,10 +323,10 @@ long long ms_between(Clock::time_point a, Clock::time_point b) {
 }  // namespace
 
 int main(int argc, char** argv) {
-  std::string matches_file, output_file, initial_solution;
+  std::string matches_file, output_file, initial_solution, previous_matches_file;
   std::vector<std::string> banned_list, fixed_list;
   uint64_t device = 0, gpus = 1;
-  bool keep_start = false, carry_start = false, update_start = false;
+  bool keep_start = false, carry_start = false, update_start = false, have_previous = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -272,6 +347,8 @@ int main(int argc, char** argv) {
     keep_start = a.keep_initial_solution;
     carry_start = a.carry_initial_solution;
     update_start = a.update_initial_solution;
+    have_previous = a.single.count("previous_matches_file") != 0;
+    if (have_previous) previous_matches_file = a.single.at("previous_matches_file");
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
@@ -297,6 +374,10 @@ int main(int argc, char** argv) {
     std::fputs("ERROR: --update_initial_solution and --keep_initial_solution exclude each other\n", stderr);
     return 2;
   }
+  if (have_previous && !update_start) {
+    std::fputs("ERROR: --previous_matches_file needs --update_initial_solution\n", stderr);
+    return 2;
+  }
   if (have_start) {
     if (!start_file.open(initial_solution)) {
       std::fprintf(stderr, "ERROR: cannot read the initial solution file '%s'\n", initial_solution.c_str());
@@ -306,6 +387,18 @@ int main(int argc, char** argv) {
     if (lfr_wire_decode_solution(start_file.data(), start_file.size(), &ni, &nd, nullptr, nullptr, nullptr, nullptr, nullptr,
                                  nullptr, nullptr) != LFR_OK) {
       std::fputs("Failed to parse proto object.\n", stderr);  // as for the matches, solve.cc:433-436
+      return 255;
+    }
+  }
+  PreviousMatches previous;
+  if (have_previous) {
+    const int rc = read_previous(previous_matches_file, previous);
+    if (rc == 2) {
+      std::fprintf(stderr, "ERROR: cannot read the previous matches file '%s'\n", previous_matches_file.c_str());
+      return 2;
+    }
+    if (rc != 0) {
+      std::fputs("Failed to parse proto object.\n", stderr);
       return 255;
     }
   }
@@ -429,7 +522,7 @@ int main(int argc, char** argv) {
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
                                  lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
-                                 lfr_plan_update_solution;
+                                 lfr_plan_update_solution && lfr_plan_update_solution_since;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -510,7 +603,17 @@ int main(int argc, char** argv) {
     }
     // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
     int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), (uint32_t)names.size()) : LFR_OK;
-    if (rc2 == LFR_OK && have_start && update_start)
+    if (rc2 == LFR_OK && have_previous) {
+      // the earlier run's graph stage on the device, for the compare only
+      const lfr_host_input pin = previous.input();
+      lfr_plan* prev_plan = nullptr;
+      rc2 = lfr_plan_create_from_matches(&pin, &opt, nullptr, &prev_plan, nullptr);
+      if (rc2 == LFR_OK)
+        rc2 = lfr_plan_update_solution_since(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                             name_blob.data(), name_off.data(), prev_plan, (uint32_t)previous.names.size(),
+                                             previous.name_blob.data(), previous.name_off.data(), nullptr, nullptr, nullptr);
+      lfr_plan_destroy(prev_plan);
+    } else if (rc2 == LFR_OK && have_start && update_start)
       rc2 = lfr_plan_update_solution(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
                                      name_blob.data(), name_off.data(), nullptr, nullptr);
     else if (rc2 == LFR_OK && have_start)
@@ -569,7 +672,20 @@ int main(int argc, char** argv) {
     if (!positions) positions = static_cast<double*>(std::malloc(2ull * N * sizeof(double)));
     std::memset(positions, 0, 2ull * N * sizeof(double));
     std::vector<uint8_t> has_entry(keep_start || update_start ? N : 0, 0);
-    if (have_start && update_start) {
+    if (have_previous) {
+      lfr_problem cur;
+      cur.n_nodes = N; cur.n_components = C; cur.n_edges = E;
+      cur.row_ptr = row_ptr.data(); cur.edges = edges; cur.track = track.data(); cur.comp = comp.data();
+      cur.is_root = is_root.data(); cur.comp_ptr = comp_ptr.data(); cur.comp_nodes = comp_nodes.data();
+      const lfr_host_input pin = previous.input();
+      if (lfr_wire_update_solution_since(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
+                                         name_off.data(), &cur, node_image.data(), node_feat.data(), &pin,
+                                         previous.name_blob.data(), previous.name_off.data(), positions, has_entry.data(),
+                                         nullptr, nullptr, nullptr) != LFR_OK) {
+        std::fprintf(stderr, "ERROR: lfr_wire_update_solution_since failed\n");
+        return 2;
+      }
+    } else if (have_start && update_start) {
       if (lfr_wire_update_solution(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
                                    name_off.data(), N, node_image.data(), node_feat.data(), comp.data(), C, positions,
                                    has_entry.data(), nullptr, nullptr) != LFR_OK) {

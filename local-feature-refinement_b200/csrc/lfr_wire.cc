@@ -2,6 +2,7 @@
 // SolutionFile) without libprotobuf.  Replaces the parse loop of
 // solve.cc:426-480 and the writer of solve.cc:643-679.  Host code only.
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <cstdlib>
 #include <cstring>
@@ -10,6 +11,7 @@
 #include <vector>
 
 #include "../../include/lfr.h"
+#include "../../include/lfr_host.h"
 #include "../../include/lfr_wire.h"
 #include "lfr_join.h"
 
@@ -464,6 +466,122 @@ int lfr_wire_update_solution(const uint8_t* buf, uint64_t len, uint32_t n_images
                              double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched) {
   return lfr::join::update_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, node_comp,
                                  n_components, positions, held, n_held, n_touched);
+}
+
+namespace {
+
+// The graph arrays the "unchanged" test reads (lfr_problem's plus the node ids)
+struct Graph {
+  uint32_t N = 0;
+  const uint32_t *row_ptr, *track, *comp, *node_image, *node_feat;
+  const uint8_t* is_root;
+  const lfr_edge* edges;
+};
+
+// kept out-edge of node v (solve.cc:105-125: same track -> Cauchy, same component -> Tukey, else skipped)
+uint32_t edge_kind(const Graph& g, uint32_t v, uint32_t w) {
+  if (g.track[v] == g.track[w]) return LFR_EDGE_CAUCHY;
+  return g.comp[v] == g.comp[w] ? LFR_EDGE_TUKEY : LFR_EDGE_SKIP;
+}
+
+// {destination in this run's node ids, kind, bits of the 18 flow floats and of sim}
+using EdgeRec = std::array<uint32_t, 21>;
+
+void kept_edges(const Graph& g, uint32_t v, const uint32_t* to_cur, std::vector<EdgeRec>& out) {
+  out.clear();
+  for (uint32_t e = g.row_ptr[v]; e < g.row_ptr[v + 1]; ++e) {
+    const uint32_t w = g.edges[e].dst, kind = edge_kind(g, v, w);
+    if (kind == LFR_EDGE_SKIP) continue;
+    EdgeRec r;
+    r[0] = to_cur ? to_cur[w] : w;
+    r[1] = kind;
+    std::memcpy(&r[2], &g.edges[e], 19 * sizeof(uint32_t));  // flow[18], sim
+    out.push_back(r);
+  }
+  std::sort(out.begin(), out.end());
+}
+
+// changed[c] = 1 for every component c of `cur` that fails the "unchanged" test against `prev`
+// (include/lfr_host.h); prev's image ids are mapped by `map`.  Returns the count.
+uint32_t changed_components(const Graph& cur, uint32_t C, const Graph& prev, uint32_t prev_C, const std::vector<uint32_t>& map,
+                            uint8_t* changed) {
+  constexpr uint32_t kNone = 0xffffffffu;
+  std::unordered_map<uint64_t, uint32_t> prev_of;
+  prev_of.reserve(prev.N);
+  for (uint32_t u = 0; u < prev.N; ++u) prev_of.emplace(lfr::join::node_key(map[prev.node_image[u]], prev.node_feat[u]), u);
+  std::vector<uint32_t> m(cur.N, kNone), inv(prev.N, kNone), pc_of(C, kNone), size(C, 0), prev_size(prev_C, 0);
+  std::fill(changed, changed + C, 0);
+  for (uint32_t v = 0; v < cur.N; ++v) {
+    const uint32_t c = cur.comp[v];
+    ++size[c];
+    const auto it = prev_of.find(lfr::join::node_key(cur.node_image[v], cur.node_feat[v]));
+    if (it == prev_of.end()) {
+      changed[c] = 1;
+      continue;
+    }
+    const uint32_t u = it->second, pc = prev.comp[u];
+    m[v] = u;
+    inv[u] = v;
+    if ((cur.is_root[v] != 0) != (prev.is_root[u] != 0)) changed[c] = 1;
+    if (pc_of[c] == kNone) pc_of[c] = pc;
+    else if (pc_of[c] != pc) changed[c] = 1;
+  }
+  for (uint32_t u = 0; u < prev.N; ++u) ++prev_size[prev.comp[u]];
+  for (uint32_t c = 0; c < C; ++c)
+    if (!changed[c] && (pc_of[c] == kNone || size[c] != prev_size[pc_of[c]])) changed[c] = 1;
+  std::vector<EdgeRec> a, b;
+  for (uint32_t v = 0; v < cur.N; ++v) {
+    if (changed[cur.comp[v]]) continue;
+    kept_edges(cur, v, nullptr, a);
+    kept_edges(prev, m[v], inv.data(), b);
+    if (a != b) changed[cur.comp[v]] = 1;
+  }
+  return (uint32_t)std::count(changed, changed + C, (uint8_t)1);
+}
+
+}  // namespace
+
+int lfr_wire_update_solution_since(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                                   const uint64_t* name_off, const lfr_problem* p, const uint32_t* node_image,
+                                   const uint32_t* node_feat, const lfr_host_input* previous, const uint8_t* prev_names,
+                                   const uint64_t* prev_name_off, double* positions, uint8_t* held, uint64_t* n_held,
+                                   uint32_t* n_touched, uint32_t* n_changed) {
+  if (!p || !previous) return LFR_EINVAL;
+  const uint32_t N = p->n_nodes, C = p->n_components;
+  if (N && (!p->row_ptr || !p->track || !p->comp || !p->is_root || !node_image || !node_feat)) return LFR_EINVAL;
+  if (N && (p->row_ptr[N] != p->n_edges || (p->n_edges && !p->edges))) return LFR_EINVAL;
+  for (uint32_t v = 0; v < N; ++v)
+    if (p->comp[v] >= C || node_image[v] >= n_images) return LFR_EINVAL;
+  for (uint64_t e = 0; e < p->n_edges; ++e)
+    if (p->edges[e].dst >= N) return LFR_EINVAL;
+  std::vector<uint32_t> map;
+  if (lfr::join::map_previous_images(n_images, names, name_off, previous->n_images, prev_names, prev_name_off, map) != LFR_OK)
+    return LFR_EINVAL;
+  // the earlier run: the graph stage over every pair of the earlier file, no image banned
+  lfr_host_input in = *previous;
+  in.pair_skip = nullptr;
+  in.edges_out = nullptr;
+  in.edges_out_capacity = 0;
+  lfr_host_stage* hs = nullptr;
+  lfr_host_sizes sz;
+  const int rc = lfr_host_stage_create(&in, &hs, &sz);
+  if (rc != LFR_OK) return rc;
+  const uint32_t M = sz.n_nodes;
+  std::vector<uint32_t> row_ptr((size_t)M + 1, 0), track(M), comp(M), node_image_b(M), node_feat_b(M);
+  std::vector<uint8_t> is_root(M);
+  std::vector<lfr_edge> edges(sz.n_edges);
+  const int rc2 = lfr_host_stage_export(hs, row_ptr.data(), edges.data(), track.data(), comp.data(), is_root.data(), nullptr,
+                                        nullptr, nullptr, node_image_b.data(), node_feat_b.data());
+  lfr_host_stage_destroy(hs);
+  if (rc2 != LFR_OK) return rc2;
+  Graph cur{N, p->row_ptr, p->track, p->comp, node_image, node_feat, p->is_root, p->edges};
+  Graph prev{M, row_ptr.data(), track.data(), comp.data(), node_image_b.data(), node_feat_b.data(), is_root.data(), edges.data()};
+  std::vector<uint8_t> changed(C, 0);
+  const uint32_t nc = changed_components(cur, C, prev, sz.n_components, map, changed.data());
+  const int rc3 = lfr::join::update_nodes(buf, len, n_images, names, name_off, N, node_image, node_feat, p->comp, C,
+                                          positions, held, n_held, n_touched, changed.data());
+  if (rc3 == LFR_OK && n_changed) *n_changed = nc;
+  return rc3;
 }
 
 int64_t lfr_wire_encode_solution_carried(uint64_t n_images, const uint64_t* img_ptr, const uint8_t* names,

@@ -102,19 +102,24 @@ def fixed_image_mask(image_names: List[str], fixed_images) -> np.ndarray:
 
 
 def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[bytes] = None,
-                     keep_initial_solution: bool = False, update_initial_solution: bool = False):
+                     keep_initial_solution: bool = False, update_initial_solution: bool = False,
+                     previous_matches: Optional[MatchSet] = None):
     """The host route's problem initialisation with fixed images and a start solution: (the Problem to solve,
     whose is_root is the constant mask = reference root OR node of a fixed image OR, with
     `keep_initial_solution`, node with an entry in the start solution OR, with `update_initial_solution`,
-    node of a component the start solution covers whole (wire.update_solution); start positions [N, 2] from
-    wire.join_solution or wire.update_solution, or None for zeros)."""
+    node of a component the start solution covers whole (wire.update_solution) and, with `previous_matches`,
+    that is unchanged since that MatchingFile's run (wire.update_solution_since); start positions [N, 2] from
+    wire.join_solution or wire.update_solution(_since), or None for zeros)."""
     from . import wire
     g = p.graph
     const = np.asarray(p.is_root) != 0
     if len(fixed_images) and g.n_nodes:
         const = const | fixed_image_mask(g.image_names, fixed_images)[np.asarray(g.node_image, np.int64)]
     start = None
-    if initial_solution is not None and update_initial_solution:
+    if initial_solution is not None and update_initial_solution and previous_matches is not None:
+        start, held, _, _, _ = wire.update_solution_since(initial_solution, p, previous_matches)
+        const = const | held
+    elif initial_solution is not None and update_initial_solution:
         start, held, _, _ = wire.update_solution(initial_solution, g.image_names, g.node_image, g.node_feat, p.comp,
                                                  p.n_components)
         const = const | held
@@ -130,7 +135,7 @@ def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[byt
 def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[[str], None]] = None,
            solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None, fixed_images=(),
            initial_solution: Optional[bytes] = None, keep_initial_solution: bool = False,
-           update_initial_solution: bool = False):
+           update_initial_solution: bool = False, previous_matches=None):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
     may be supplied to drive a different executor (the multi-GPU path; give `n_devices`); with a start
     solution it is called as `solve_fn(problem, positions)`.
@@ -142,7 +147,11 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     wire.join_solution), so only the keypoints it does not list are refined.  `update_initial_solution`
     (needs `initial_solution`, excludes `keep_initial_solution`) solves every component with a keypoint the
     file does not list from zeros, as without the file, and holds every other component at the file's
-    values (wire.update_solution, Plan.update_solution).  The returned Problem keeps the reference's is_root.
+    values (wire.update_solution, Plan.update_solution).  `previous_matches` (needs `update_initial_solution`;
+    a MatchSet or MatchingFile bytes) is the MatchingFile that produced `initial_solution`: a component is then
+    also touched when its problem is not the one that file's run solved (include/lfr_graph.h states the
+    rule; wire.update_solution_since, Plan.update_solution(previous=...)).  The returned Problem keeps the
+    reference's is_root.
 
     The graph stage runs where graph_stage_on_device() says.  On the device (Plan.from_matches) the problem
     stays in HBM and is solved there, `solve_fn` is not called, and the Problem's arrays come from
@@ -155,11 +164,17 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
         raise ValueError("update_initial_solution needs initial_solution")
     if update_initial_solution and keep_initial_solution:
         raise ValueError("update_initial_solution and keep_initial_solution exclude each other")
+    if previous_matches is not None and not update_initial_solution:
+        raise ValueError("previous_matches needs update_initial_solution")
+    if isinstance(previous_matches, (bytes, bytearray, memoryview)):
+        from .wire import decode_matching_file
+        previous_matches = decode_matching_file(bytes(previous_matches))
     lib = load_b200()
     skip, arrs = host_input_arrays(ms, banned_images)
     if not graph_stage_on_device(lib, arrs, len(ms.image_names), n_devices):
         p = build_problem(ms, banned_images, log=log)
-        q, start = constant_problem(p, fixed_images, initial_solution, keep_initial_solution, update_initial_solution)
+        q, start = constant_problem(p, fixed_images, initial_solution, keep_initial_solution, update_initial_solution,
+                                    previous_matches)
         fn = solve_fn if solve_fn is not None else (lambda q_, x=None: solve_problem(q_, options, x))
         pos, st = fn(q) if start is None else fn(q, start)
         return p, pos, st, assemble_solution(p, pos)
@@ -167,7 +182,13 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     try:
         if len(fixed_images) and fixed_image_mask(ms.image_names, fixed_images).any():
             plan.fix_images(fixed_image_mask(ms.image_names, fixed_images))
-        if update_initial_solution:
+        if update_initial_solution and previous_matches is not None:
+            prev = Plan.from_matches(lib, previous_matches, options=options)
+            try:
+                plan.update_solution(initial_solution, ms.image_names, previous=prev)
+            finally:
+                prev.close()
+        elif update_initial_solution:
             plan.update_solution(initial_solution, ms.image_names)
         elif keep_initial_solution:
             plan.keep_solution(initial_solution, ms.image_names)

@@ -28,7 +28,8 @@ class WireMatches(C.Structure):
 
 WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
                 "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution",
-                "lfr_wire_join_solution_entries", "lfr_wire_encode_solution_carried", "lfr_wire_update_solution"]
+                "lfr_wire_join_solution_entries", "lfr_wire_encode_solution_carried", "lfr_wire_update_solution",
+                "lfr_wire_update_solution_since"]
 
 _bound = False
 
@@ -62,6 +63,9 @@ def _lib():
                                                + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p,
                                                                      C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)])
         L.lfr_wire_update_solution.restype = C.c_int
+        L.lfr_wire_update_solution_since.argtypes = ([C.c_void_p, C.c_uint64, C.c_uint32] + [C.c_void_p] * 10 +
+                                                     [C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)])
+        L.lfr_wire_update_solution_since.restype = C.c_int
         _bound = True
     return L
 
@@ -329,3 +333,50 @@ def update_solution(data: bytes, image_names: List[str], node_image: np.ndarray,
     if rc != 0:
         raise ParseError("Failed to parse proto object.")
     return pos, held.astype(bool), int(n.value), int(t.value)
+
+
+def update_solution_since(data: bytes, p, previous: MatchSet):
+    """The host form of Plan.update_solution(previous=...) (lfr_wire_update_solution_since, include/lfr_host.h):
+    update_solution() on Problem `p` (its reference is_root), where a component is also touched when it is not
+    unchanged since the graph stage over every pair of `previous` (the MatchingFile that produced `data`; the
+    rule is in include/lfr_graph.h).  Returns (positions [N, 2], held [N] bool, held nodes, touched components,
+    changed components).  Raises ParseError on bytes the decoder rejects, RuntimeError when the arrays or the
+    earlier stage are rejected."""
+    from .capi import Library
+    from .graph import HostInput, host_input_arrays
+    L = _lib()
+    g = p.graph
+    s, keep = Library.marshal(p)
+    buf = np.frombuffer(data, dtype=np.uint8)
+    blob, off = _names_blob(list(g.image_names))
+    pblob, poff = _names_blob(list(previous.image_names))
+    _, arrs = host_input_arrays(previous)
+    inp = HostInput(n_pairs=previous.n_pairs, n_matches=previous.n_matches, n_images=len(previous.image_names),
+                    **{k: (v.ctypes.data if v.size else None) for k, v in arrs.items()})
+    img = np.ascontiguousarray(g.node_image, dtype=np.uint32).reshape(-1)
+    feat = np.ascontiguousarray(g.node_feat, dtype=np.uint32).reshape(-1)
+    N = int(img.shape[0])
+    pos = np.zeros((N, 2), np.float64)
+    held = np.zeros(N, np.uint8)
+    n, t, ch = C.c_uint64(), C.c_uint32(), C.c_uint32()
+    if not _solution_parses(data):  # told apart from the other refusals
+        raise ParseError("Failed to parse proto object.")
+    rc = L.lfr_wire_update_solution_since(buf.ctypes.data if buf.size else None, buf.size, len(g.image_names),
+                                          blob.ctypes.data, off.ctypes.data, C.addressof(s),
+                                          img.ctypes.data if N else None, feat.ctypes.data if N else None,
+                                          C.addressof(inp), pblob.ctypes.data, poff.ctypes.data,
+                                          pos.ctypes.data if N else None, held.ctypes.data if N else None,
+                                          C.byref(n), C.byref(t), C.byref(ch))
+    del keep, arrs
+    if rc != 0:
+        raise RuntimeError("lfr_wire_update_solution_since failed (%d)" % rc)
+    return pos, held.astype(bool), int(n.value), int(t.value), int(ch.value)
+
+
+def _solution_parses(data: bytes) -> bool:
+    """Whether the SolutionFile decoder accepts `data`."""
+    L = _lib()
+    buf = np.frombuffer(data, dtype=np.uint8)
+    ni, nd = C.c_uint64(), C.c_uint64()
+    return L.lfr_wire_decode_solution(buf.ctypes.data if buf.size else None, buf.size, C.byref(ni), C.byref(nd),
+                                      *([None] * 7)) == 0
