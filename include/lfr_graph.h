@@ -201,6 +201,58 @@ int lfr_plan_update_solution_since(lfr_plan* plan, void* stream, const uint8_t* 
                                    uint32_t prev_n_images, const uint8_t* prev_names, const uint64_t* prev_name_off,
                                    uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed);
 
+/* The problem record of a run: one 128-bit digest per component, so that a later update can ask "was this
+ * exact problem solved before?" without the earlier MatchingFile or its graph stage (about 16 bytes per
+ * component instead of the earlier run's arrays).  Each run writes the record the next one reads.
+ *
+ * The record, exactly (csrc/lfr_record.h has the code, for the host library and the kernels alike):
+ *   - S(k, m) is SipHash-2-4 (Aumasson and Bernstein) with the 16-byte key k, the message m hashed as its
+ *     little-endian bytes.  H(m) = (S(K0, m), S(K1, m)), K0 = the 16 ASCII bytes "lfr problem rec0",
+ *     K1 = "lfr problem rec1".
+ *   - The name id of an image is H(exact name bytes).  A keypoint is (name id, feature_idx).
+ *   - The node element of node v is 4 little-endian u64 words [0x4e, id(v).0, id(v).1, feat(v) | root(v) << 32],
+ *     root = the reference's is_root (not a constant mask).
+ *   - The edge element of each kept out-edge v -> w is 16 little-endian u64 words [0x45, id(v).0, id(v).1,
+ *     id(w).0, id(w).1, feat(v) | feat(w) << 32, kind | bits(sim) << 32, bits(flow[2i]) | bits(flow[2i+1]) << 32
+ *     for i = 0..8], flow in lfr_edge.flow order.  Kept and kind as the solve classifies edges: same track
+ *     gives LFR_EDGE_CAUCHY, otherwise same component LFR_EDGE_TUKEY, otherwise the edge is skipped.
+ *   - Digest(C) = (sum H(x).0, sum H(x).1) mod 2^64 over the node elements of C's nodes and the edge elements
+ *     of their kept out-edges.  It depends on neither node nor edge order, counts multiplicity, and is exact
+ *     integer arithmetic: any reduction order gives the same bits.
+ *   - The record is the 8 bytes "LFRPREC1", u64 C, then the C digests as (d0, d1) u64 pairs in ascending
+ *     (d0, d1) order: 16 + 16 C bytes.  A reader refuses any other length or magic and digests out of order.
+ * The record describes the graph stage as it ran (its banned images and its cut cap); it does not depend on
+ * fixed images, on a kept or held set or on the start point.
+ *
+ * `plan` is made from matches.  Name ids are hashed on the host from names / name_off (n_images, at least
+ * the plan's image count); elements are hashed and summed per component on the device (csrc/lfr_record.cuh)
+ * and a radix sort orders the digests.  Returns the record's size and writes it to `out` only when `cap` is
+ * at least that (lfr_plan_encode_solution's protocol); LFR_EINVAL for a plan made by lfr_plan_create() or
+ * malformed names.  Synchronous on `stream`.  The plan is not changed: a solve after the call is bitwise the
+ * same.  lfr_host_problem_record() (include/lfr_host.h) is the host form, byte for byte. */
+int64_t lfr_plan_problem_record(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                const uint64_t* name_off, uint8_t* out, uint64_t cap);
+
+/* lfr_plan_update_solution_since() against the earlier run's problem record instead of its MatchingFile.
+ * The held rule is the same with the compare replaced by digest membership: C is *unchanged* when Digest(C)
+ * appears in the record, *held* when it is unchanged and every keypoint of C has an entry in the SolutionFile;
+ * every other component is *touched* and behaves as in lfr_plan_update_solution_since().  *n_changed counts
+ * the components whose digest is absent.  The held flags, start positions, constant mask and schedule are the
+ * same code as lfr_plan_update_solution_since()'s.  Errors as lfr_plan_update_solution(), plus LFR_EINVAL for a
+ * malformed record; the plan is not changed on error.  lfr_wire_update_solution_since_record()
+ * (include/lfr_host.h) is the host form, bit for bit.
+ *
+ * Limits.  Equal digests are not exact equality: two different problems share a digest only when two different
+ * multisets of element hashes have equal sums in both lanes.  For a random function that has probability 2^-128
+ * when some multiplicity differs by an odd count, and 2^-(128-2t) when every difference is divisible by 2^t.
+ * lfr_plan_update_solution_since() stays the exact path and needs no record; it is the only option when the
+ * SolutionFile came from an older build or from the reference binary.  When the record was written by a run on
+ * OLD that banned no image, the two calls give identical results. */
+int lfr_plan_update_solution_since_record(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len,
+                                          uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                                          const uint8_t* record, uint64_t record_len, uint64_t* n_held,
+                                          uint32_t* n_touched, uint32_t* n_changed);
+
 /* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
  * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from
  * sizes known before either stage runs — the directed edges (2 x the matches of the pairs not skipped),

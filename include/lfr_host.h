@@ -85,6 +85,27 @@ int lfr_wire_update_solution_since(const uint8_t* buf, uint64_t len, uint32_t n_
                                    uint8_t* held /* [n_nodes] */, uint64_t* n_held, uint32_t* n_touched,
                                    uint32_t* n_changed);
 
+/* The host form of lfr_plan_problem_record() (include/lfr_graph.h states the record), byte for byte: the
+ * record of problem `p` with node ids node_image / node_feat and image names by id names / name_off
+ * (n_images).  `p->is_root` must be the reference's is_root (the graph stage's export), not a constant mask;
+ * comp_ptr / comp_nodes are not read.  Returns the record's size, 16 + 16 p->n_components, and writes it to
+ * `out` only when `cap` is at least that; LFR_EINVAL for NULL or inconsistent arrays.  The element hashes
+ * run on up to 8 helper threads (LFR_HOST_THREADS overrides the count); the bytes do not depend on it. */
+int64_t lfr_host_problem_record(const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat,
+                                uint32_t n_images, const uint8_t* names, const uint64_t* name_off, uint8_t* out,
+                                uint64_t cap);
+
+/* The host form of lfr_plan_update_solution_since_record() (include/lfr_graph.h), bit for bit: as
+ * lfr_wire_update_solution_since(), with the compare against the earlier run's record (record_len bytes)
+ * in place of its MatchingFile: a component is changed when its digest is not in the record.  LFR_EINVAL
+ * for malformed SolutionFile bytes, a malformed record, NULL or inconsistent arrays.  Every output is
+ * untouched on error. */
+int lfr_wire_update_solution_since_record(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                                          const uint64_t* name_off, const lfr_problem* p, const uint32_t* node_image,
+                                          const uint32_t* node_feat, const uint8_t* record, uint64_t record_len,
+                                          double* positions /* [2 n_nodes] */, uint8_t* held /* [n_nodes] */,
+                                          uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed);
+
 #ifdef __cplusplus
 }
 #endif

@@ -82,7 +82,8 @@ ABI_SYMBOLS = [
 GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "lfr_plan_export_graph",
                  "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
                  "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution",
-                 "lfr_plan_encode_solution_carried", "lfr_plan_update_solution", "lfr_plan_update_solution_since"]
+                 "lfr_plan_encode_solution_carried", "lfr_plan_update_solution", "lfr_plan_update_solution_since",
+                 "lfr_plan_problem_record", "lfr_plan_update_solution_since_record"]
 
 
 class LfrWirePart(C.Structure):
@@ -168,6 +169,13 @@ class Library:
                                                          [C.c_void_p] * 2 + [C.POINTER(C.c_uint64)] +
                                                          [C.POINTER(C.c_uint32)] * 2)
             L.lfr_plan_update_solution_since.restype = C.c_int
+            L.lfr_plan_problem_record.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_uint64]
+            L.lfr_plan_problem_record.restype = C.c_int64
+            L.lfr_plan_update_solution_since_record.argtypes = (L.lfr_plan_start_from_solution.argtypes[:7] +
+                                                                [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)] +
+                                                                [C.POINTER(C.c_uint32)] * 2)
+            L.lfr_plan_update_solution_since_record.restype = C.c_int
             L.lfr_plan_encode_solution_carried.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
                                                            C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                                            C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
@@ -533,8 +541,25 @@ class Plan:
                        "lfr_plan_keep_solution")
         return int(n.value)
 
+    def problem_record(self, image_names, stream: int = 0) -> bytes:
+        """lfr_plan_problem_record (include/lfr_graph.h, which states the record): one 128-bit digest per
+        component of this plan (made by from_matches() or from_wire()), computed on the device and sorted.
+        `image_names` by image id.  The plan is not changed."""
+        from .wire import _names_blob
+        blob, off = _names_blob(list(image_names))
+        f = self.lib.lib.lfr_plan_problem_record
+        args = (self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data)
+        need = f(*args, None, 0)
+        if need < 0:
+            self.lib.check(int(need), "lfr_plan_problem_record")
+        out = np.empty(max(int(need), 1), np.uint8)
+        got = f(*args, out.ctypes.data, int(need))
+        if got != need:
+            self.lib.check(int(got) if got < 0 else -1, "lfr_plan_problem_record")
+        return out[:need].tobytes()
+
     def update_solution(self, data: bytes, image_names, stream: int = 0, previous: Optional["Plan"] = None,
-                        previous_names=None):
+                        previous_names=None, previous_record: Optional[bytes] = None):
         """lfr_plan_update_solution (include/lfr_graph.h): every component with a node that has no entry in
         `data` is touched and solves from zeros as without a file; every other component is held constant at
         the file's values.  Replaces an earlier kept or held set (an empty file clears it) and composes with
@@ -544,12 +569,26 @@ class Plan:
         (every pair, no banned image), lfr_plan_update_solution_since: a component is held only when it is
         also unchanged since that run (the rule in include/lfr_graph.h).  `previous_names` are its image names
         by id (default: previous.image_names).  Returns (held nodes, touched components, changed components);
-        `previous` is not changed."""
+        `previous` is not changed.
+
+        With `previous_record`, the problem record (problem_record(), wire.problem_record()) of the run that
+        produced `data`, lfr_plan_update_solution_since_record: the same, with a component unchanged when its
+        digest is in the record.  Excludes `previous`."""
         from .wire import _names_blob
+        if previous is not None and previous_record is not None:
+            raise ValueError("previous and previous_record exclude each other")
         buf = np.frombuffer(data, dtype=np.uint8)
         blob, off = _names_blob(list(image_names))
         n = C.c_uint64()
         t = C.c_uint32()
+        if previous_record is not None:
+            rec = np.frombuffer(bytes(previous_record), dtype=np.uint8)
+            ch = C.c_uint32()
+            self.lib.check(self.lib.lib.lfr_plan_update_solution_since_record(
+                self.handle, C.c_void_p(stream), buf.ctypes.data if buf.size else None, buf.size, len(image_names),
+                blob.ctypes.data, off.ctypes.data, rec.ctypes.data if rec.size else None, rec.size,
+                C.byref(n), C.byref(t), C.byref(ch)), "lfr_plan_update_solution_since_record")
+            return int(n.value), int(t.value), int(ch.value)
         if previous is not None:
             pnames = list(previous.image_names if previous_names is None else previous_names)
             pblob, poff = _names_blob(pnames)

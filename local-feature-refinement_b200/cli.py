@@ -23,6 +23,11 @@ every other component at the file's values (wire.update_solution, Plan.update_so
 the MatchingFile that produced the initial solution: a component is then also solved again when its problem
 is not the one OLD.pb's run solved, so banned images, new pairs between old images and changed network output
 no longer leave stale values (the rule is in include/lfr_graph.h).
+--record_file FILE writes this run's problem record (one 128-bit digest per component, include/lfr_graph.h)
+after the SolutionFile, and --earlier_record_file FILE (with --update_initial_solution, not with
+--previous_matches_file) reads the record the run that produced the initial solution wrote, in place of its
+MatchingFile: a component is unchanged when its digest is in that record (wire.problem_record,
+Plan.problem_record, Plan.update_solution(previous_record=...)).
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -59,7 +64,8 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("device", True, False), ("gpus", True, False), ("stats_json", True, False),
             ("fixed_images", True, True), ("initial_solution", True, False),
             ("keep_initial_solution", False, False), ("carry_initial_solution", False, False),
-            ("update_initial_solution", False, False), ("previous_matches_file", True, False)]
+            ("update_initial_solution", False, False), ("previous_matches_file", True, False),
+            ("record_file", True, False), ("earlier_record_file", True, False)]
 
 
 def _find_option(name):
@@ -137,7 +143,8 @@ def parse_args(argv):
             keep_initial_solution=bool(vals.get("keep_initial_solution")),
             carry_initial_solution=bool(vals.get("carry_initial_solution")),
             update_initial_solution=bool(vals.get("update_initial_solution")),
-            previous_matches_file=vals.get("previous_matches_file"))
+            previous_matches_file=vals.get("previous_matches_file"),
+            record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -168,6 +175,12 @@ def main(argv=None) -> int:
     if args.previous_matches_file is not None and not args.update_initial_solution:
         sys.stderr.write("ERROR: --previous_matches_file needs --update_initial_solution\n")
         return 2
+    if args.earlier_record_file is not None and not args.update_initial_solution:
+        sys.stderr.write("ERROR: --earlier_record_file needs --update_initial_solution\n")
+        return 2
+    if args.earlier_record_file is not None and args.previous_matches_file is not None:
+        sys.stderr.write("ERROR: --earlier_record_file and --previous_matches_file exclude each other\n")
+        return 2
     start = None
     if args.initial_solution is not None:
         try:
@@ -193,6 +206,17 @@ def main(argv=None) -> int:
         except wire.ParseError:
             sys.stderr.write("Failed to parse proto object.\n")
             return 255
+    earlier_record = None
+    if args.earlier_record_file is not None:
+        try:
+            with open(args.earlier_record_file, "rb") as fh:
+                earlier_record = fh.read()
+        except OSError:
+            sys.stderr.write("ERROR: cannot read the earlier record file '%s'\n" % args.earlier_record_file)
+            return 2
+        if not wire.record_is_valid(earlier_record):
+            sys.stderr.write("ERROR: '%s' is not a problem record\n" % args.earlier_record_file)
+            return 2
 
     rank = int(os.environ.get("RANK", "0"))
     say = (lambda s: print(s, flush=True)) if rank == 0 else (lambda s: None)
@@ -241,11 +265,16 @@ def main(argv=None) -> int:
     # torchrun ranks and --gpus N solve a host lfr_problem: the size rule keeps them on the host route
     torchrun = "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1
     n_devices = int(os.environ["WORLD_SIZE"]) if torchrun else max(args.gpus, 1)
+    if torchrun and (args.record_file is not None or args.earlier_record_file is not None):
+        sys.stderr.write("ERROR: --record_file / --earlier_record_file: torchrun ranks do not write or read "
+                         "problem records; use --gpus N\n")
+        return 2
     try:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
                                  timing=timing, fixed_images=args.fixed_images, initial_solution=start,
                                  keep_initial_solution=args.keep_initial_solution,
-                                 update_initial_solution=args.update_initial_solution, previous_matches=previous)
+                                 update_initial_solution=args.update_initial_solution, previous_matches=previous,
+                                 previous_record=earlier_record, record_problem=args.record_file is not None)
     except GraphStageRouteError as e:
         sys.stderr.write("ERROR: %s\n" % e)
         return 2
@@ -265,6 +294,13 @@ def main(argv=None) -> int:
     except OSError:
         sys.stderr.write("Failed to write proto object.\n")
         return 255
+    if args.record_file is not None:
+        try:
+            with open(args.record_file, "wb") as fh:
+                fh.write(sol.record)
+        except OSError:
+            sys.stderr.write("ERROR: cannot write the record file '%s'\n" % args.record_file)
+            return 255
     if args.stats_json:
         n_tracks = refined_track_count(p)
         solver_s = max(timing.get("solver_ms", 0.0), 1e-9) / 1e3

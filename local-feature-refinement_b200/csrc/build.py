@@ -32,10 +32,10 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 OUT_EXE = os.path.join(ROOT, "multi-view-refinement", "build", "solve_native")
 INC = os.path.join("..", "..", "include")
 # build.py itself: a change of NVCC_FLAGS (e.g. the target architecture) must rebuild the library
-DEPS = SOURCES + ["build.py", "lfr_setup.cuh", "lfr_solve_warp.cuh", "lfr_solve_warp2.cuh", "lfr_solve_cta.cuh", "lfr_lm.cuh", "lfr_math.cuh", "lfr_graph.cuh", "lfr_wire.cuh", "lfr_solution.cuh", "lfr_carry.cuh", "lfr_diff.cuh", "lfr_cut.h", "lfr_cut.cuh", "lfr_join.h", "lfr_start.cuh",
+DEPS = SOURCES + ["build.py", "lfr_setup.cuh", "lfr_solve_warp.cuh", "lfr_solve_warp2.cuh", "lfr_solve_cta.cuh", "lfr_lm.cuh", "lfr_math.cuh", "lfr_graph.cuh", "lfr_wire.cuh", "lfr_solution.cuh", "lfr_carry.cuh", "lfr_diff.cuh", "lfr_record.h", "lfr_record.cuh", "lfr_cut.h", "lfr_cut.cuh", "lfr_join.h", "lfr_start.cuh",
                   os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_graph.h"), os.path.join(INC, "lfr_host.h"),
                   os.path.join(INC, "lfr_wire.h")]
-HOST_DEPS = HOST_SOURCES + ["lfr_cut.h", "lfr_join.h", os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"),
+HOST_DEPS = HOST_SOURCES + ["lfr_cut.h", "lfr_join.h", "lfr_record.h", os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"),
                             os.path.join(INC, "lfr_host.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -72,7 +72,7 @@ def build_exe(force: bool = False, out: str = OUT_EXE, solve_lib_dir: str = HERE
     """The native `solve`.  The product links csrc/liblfr_b200.so; tests/ link the same source against the
     CPU checker (oracle/liblfr_ref.so exports the same C ABI) to compare it with the reference binary."""
     deps = [EXE_SOURCE, os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"), os.path.join(INC, "lfr_host.h"),
-            os.path.join(INC, "lfr_graph.h")]
+            os.path.join(INC, "lfr_graph.h"), "lfr_record.h"]
     if force or _stale(out, deps) or not os.path.exists(out):
         os.makedirs(os.path.dirname(out), exist_ok=True)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-Wall", "-o", out, os.path.join(HERE, EXE_SOURCE),

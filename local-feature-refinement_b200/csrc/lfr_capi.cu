@@ -20,6 +20,7 @@
 #include "lfr_cut.cuh"
 #include "lfr_diff.cuh"
 #include "lfr_graph.cuh"
+#include "lfr_record.cuh"
 #include "lfr_solution.cuh"
 #include "lfr_solve_cta.cuh"
 #include "lfr_solve_warp.cuh"
@@ -2474,6 +2475,49 @@ int diff_components(const lfr_plan* pl, const lfr_plan* prev, const std::vector<
   *n_changed = (uint32_t)nc;
   return LFR_OK;
 }
+
+// the checks of the record calls on the image names (as lfr_plan_encode_solution's)
+int check_record_names(const lfr_plan* pl, uint32_t n_images, const uint8_t* names, const uint64_t* name_off) {
+  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
+  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
+  if (n_images && !name_off) return fail(LFR_EINVAL, "NULL image names");
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
+  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  return LFR_OK;
+}
+
+// The digest of every component of `pl` (lfr_record.cuh) into d0[C], d1[C] (device, reserved here): name ids
+// hashed on the host, elements hashed and summed on the device.  Reads the plan, changes nothing.
+int plan_digests(const lfr_plan* pl, cudaStream_t s, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                 TmpBuf& d0, TmpBuf& d1) {
+  const uint32_t N = pl->N, C = pl->C;
+  const uint64_t E = pl->E;
+  std::vector<unsigned long long> ids(2 * (size_t)std::max<uint32_t>(n_images, 1), 0);
+  for (uint32_t k = 0; k < n_images; ++k) {
+    uint64_t h0, h1;
+    lfr::record::hash_bytes(names + name_off[k], name_off[k + 1] - name_off[k], h0, h1);
+    ids[2 * (size_t)k] = h0;
+    ids[2 * (size_t)k + 1] = h1;
+  }
+  LFR_TRY(d0.reserve(8 * std::max<size_t>(C, 1)));
+  LFR_TRY(d1.reserve(8 * std::max<size_t>(C, 1)));
+  if (!C) return LFR_OK;
+  TmpBuf d_ids;
+  LFR_TRY(d_ids.reserve(8 * ids.size()));
+  LFR_CUDA(cudaMemcpyAsync(d_ids.p, ids.data(), 8 * ids.size(), cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemsetAsync(d0.p, 0, 8 * (size_t)C, s));
+  LFR_CUDA(cudaMemsetAsync(d1.p, 0, 8 * (size_t)C, s));
+  if (N + E) {
+    lfr::record::digest_kernel<<<blocks_for(N + E), 256, 0, s>>>(
+        pl->row_ptr.as<uint32_t>(), pl->edges.as<float4>(), pl->track.as<uint32_t>(), pl->comp.as<uint32_t>(),
+        pl->is_root.as<uint8_t>(), pl->node_image.as<uint32_t>(), pl->node_feat.as<uint32_t>(), d_ids.as<ulonglong2>(), N,
+        E, d0.as<unsigned long long>(), d1.as<unsigned long long>());
+    LFR_LAUNCHED();
+  }
+  LFR_CUDA(cudaStreamSynchronize(s));  // before `d_ids` is freed
+  return LFR_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -2684,6 +2728,71 @@ int lfr_plan_update_solution_since(lfr_plan* pl, void* stream, const uint8_t* by
   LFR_TRY(diff_components(pl, previous, image_map, s, changed.as<uint8_t>(), &nc));
   LFR_TRY(update_solution(pl, s, d, changed.as<uint8_t>(), n_held, n_touched));
   if (n_changed) *n_changed = nc;
+  return LFR_OK;
+}
+
+int64_t lfr_plan_problem_record(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
+                                const uint64_t* name_off, uint8_t* out, uint64_t cap) {
+  LFR_TRY(check_record_names(pl, n_images, names, name_off));
+  const uint32_t C = pl->C;
+  const uint64_t need = lfr::record::record_bytes(C);
+  if (!out || cap < need) return (int64_t)need;
+  LFR_CUDA(cudaSetDevice(pl->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  TmpBuf d0, d1, k1, v0, tmp;
+  LFR_TRY(plan_digests(pl, s, n_images, names, name_off, d0, d1));
+  std::vector<unsigned long long> h0(C), h1(C);
+  if (C) {
+    LFR_TRY(k1.reserve(8 * (size_t)C));
+    LFR_TRY(v0.reserve(8 * (size_t)C));
+    auto* a0 = d0.as<unsigned long long>();
+    auto* a1 = d1.as<unsigned long long>();
+    auto* b1 = k1.as<unsigned long long>();
+    auto* b0 = v0.as<unsigned long long>();
+    // ascending (d0, d1): by d1, then stably by d0
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceRadixSort::SortPairs(t, nb, a1, b1, a0, b0, (int)C, 0, 64, s); }));
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceRadixSort::SortPairs(t, nb, b0, a0, b1, a1, (int)C, 0, 64, s); }));
+    LFR_CUDA(cudaMemcpyAsync(h0.data(), a0, 8 * (size_t)C, cudaMemcpyDeviceToHost, s));
+    LFR_TRY(fetch(h1.data(), a1, C, s));
+  }
+  lfr::record::store_u64(out, lfr::record::kMagic);
+  lfr::record::store_u64(out + 8, C);
+  for (uint32_t c = 0; c < C; ++c) {
+    lfr::record::store_u64(out + lfr::record::kHeaderBytes + 16 * (size_t)c, h0[c]);
+    lfr::record::store_u64(out + lfr::record::kHeaderBytes + 16 * (size_t)c + 8, h1[c]);
+  }
+  return (int64_t)need;
+}
+
+int lfr_plan_update_solution_since_record(lfr_plan* pl, void* stream, const uint8_t* bytes, uint64_t len, uint32_t n_images,
+                                          const uint8_t* names, const uint64_t* name_off, const uint8_t* record,
+                                          uint64_t record_len, uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed) {
+  lfr::join::Decoded d;
+  LFR_TRY(decode_solution_for(pl, bytes, len, n_images, names, name_off, d));
+  LFR_TRY(check_record_names(pl, n_images, names, name_off));
+  uint64_t R = 0;
+  if (!lfr::record::check(record, record_len, &R)) return fail(LFR_EINVAL, "malformed problem record");
+  LFR_CUDA(cudaSetDevice(pl->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  const uint32_t C = pl->C;
+  TmpBuf d0, d1, d_rec, changed, d_ctr;
+  LFR_TRY(plan_digests(pl, s, n_images, names, name_off, d0, d1));
+  LFR_TRY(changed.reserve(std::max<size_t>(C, 1)));
+  LFR_TRY(d_rec.reserve(std::max<uint64_t>(16 * R, 16)));
+  LFR_TRY(d_ctr.reserve(8));
+  LFR_CUDA(cudaMemsetAsync(changed.p, 0, std::max<size_t>(C, 1), s));
+  LFR_CUDA(cudaMemsetAsync(d_ctr.p, 0, 8, s));
+  unsigned long long nc = 0;
+  if (C) {
+    if (R) LFR_CUDA(cudaMemcpyAsync(d_rec.p, record + lfr::record::kHeaderBytes, 16 * R, cudaMemcpyHostToDevice, s));
+    lfr::record::lookup_kernel<<<blocks_for(C), 256, 0, s>>>(d0.as<unsigned long long>(), d1.as<unsigned long long>(), C,
+                                                             d_rec.as<ulonglong2>(), R, changed.as<uint8_t>());
+    lfr::start::count_touched_kernel<<<blocks_for(C), 256, 0, s>>>(changed.as<uint8_t>(), C, d_ctr.as<unsigned long long>());
+    LFR_LAUNCHED();
+    LFR_TRY(fetch(&nc, d_ctr.p, 1, s));  // also orders the record's upload before the caller's buffer may go
+  }
+  LFR_TRY(update_solution(pl, s, d, changed.as<uint8_t>(), n_held, n_touched));
+  if (n_changed) *n_changed = (uint32_t)nc;
   return LFR_OK;
 }
 

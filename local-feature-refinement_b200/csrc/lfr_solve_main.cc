@@ -31,7 +31,11 @@
 // lfr_plan_update_solution() on the device route, lfr_wire_update_solution() handed to the solve on the host
 // route) and --previous_matches_file OLD.pb (with --update_initial_solution: a component is also solved again
 // when its problem is not the one OLD.pb's run solved: lfr_plan_update_solution_since() with a plan built from
-// OLD.pb on the device route, lfr_wire_update_solution_since() on the host route).  `--n_threads` is accepted and
+// OLD.pb on the device route, lfr_wire_update_solution_since() on the host route) and --record_file FILE (after
+// the SolutionFile, this run's problem record: lfr_plan_problem_record() on the device route,
+// lfr_host_problem_record() on the host route, the same bytes) and --earlier_record_file FILE (with
+// --update_initial_solution, in place of --previous_matches_file: the record the earlier run wrote;
+// lfr_plan_update_solution_since_record() / lfr_wire_update_solution_since_record()).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -56,6 +60,7 @@
 #include "../../include/lfr_graph.h"
 #include "../../include/lfr_host.h"
 #include "../../include/lfr_wire.h"
+#include "lfr_record.h"
 
 // The graph stage on the GPU is resolved weakly: the same source links against the CPU checker
 // (oracle/liblfr_ref.so), which has no plans; there they are NULL and every input takes the host route.
@@ -82,6 +87,12 @@ int lfr_plan_update_solution_since(lfr_plan* plan, void* stream, const uint8_t* 
                                    const uint8_t* names, const uint64_t* name_off, const lfr_plan* previous,
                                    uint32_t prev_n_images, const uint8_t* prev_names, const uint64_t* prev_name_off,
                                    uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed) __attribute__((weak));
+int64_t lfr_plan_problem_record(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                const uint64_t* name_off, uint8_t* out, uint64_t cap) __attribute__((weak));
+int lfr_plan_update_solution_since_record(lfr_plan* plan, void* stream, const uint8_t* bytes, uint64_t len,
+                                          uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                                          const uint8_t* record, uint64_t record_len, uint64_t* n_held,
+                                          uint32_t* n_touched, uint32_t* n_changed) __attribute__((weak));
 int64_t lfr_plan_encode_solution_carried(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
                                          const uint64_t* name_off, const float* fact, const uint8_t* file,
                                          uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
@@ -111,7 +122,8 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"n_threads", true, false},    {"banned_images", true, true}, {"device", true, false},
                                {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false},
                                {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false},
-                               {"update_initial_solution", false, false}, {"previous_matches_file", true, false}};
+                               {"update_initial_solution", false, false}, {"previous_matches_file", true, false},
+                               {"record_file", true, false},  {"earlier_record_file", true, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -323,10 +335,11 @@ long long ms_between(Clock::time_point a, Clock::time_point b) {
 }  // namespace
 
 int main(int argc, char** argv) {
-  std::string matches_file, output_file, initial_solution, previous_matches_file;
+  std::string matches_file, output_file, initial_solution, previous_matches_file, record_file, earlier_record_file;
   std::vector<std::string> banned_list, fixed_list;
   uint64_t device = 0, gpus = 1;
-  bool keep_start = false, carry_start = false, update_start = false, have_previous = false;
+  bool keep_start = false, carry_start = false, update_start = false, have_previous = false, have_record = false,
+       have_earlier = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -349,6 +362,10 @@ int main(int argc, char** argv) {
     update_start = a.update_initial_solution;
     have_previous = a.single.count("previous_matches_file") != 0;
     if (have_previous) previous_matches_file = a.single.at("previous_matches_file");
+    have_record = a.single.count("record_file") != 0;
+    if (have_record) record_file = a.single.at("record_file");
+    have_earlier = a.single.count("earlier_record_file") != 0;
+    if (have_earlier) earlier_record_file = a.single.at("earlier_record_file");
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
@@ -378,6 +395,14 @@ int main(int argc, char** argv) {
     std::fputs("ERROR: --previous_matches_file needs --update_initial_solution\n", stderr);
     return 2;
   }
+  if (have_earlier && !update_start) {
+    std::fputs("ERROR: --earlier_record_file needs --update_initial_solution\n", stderr);
+    return 2;
+  }
+  if (have_earlier && have_previous) {
+    std::fputs("ERROR: --earlier_record_file and --previous_matches_file exclude each other\n", stderr);
+    return 2;
+  }
   if (have_start) {
     if (!start_file.open(initial_solution)) {
       std::fprintf(stderr, "ERROR: cannot read the initial solution file '%s'\n", initial_solution.c_str());
@@ -400,6 +425,20 @@ int main(int argc, char** argv) {
     if (rc != 0) {
       std::fputs("Failed to parse proto object.\n", stderr);
       return 255;
+    }
+  }
+  std::vector<uint8_t> earlier_record;
+  if (have_earlier) {
+    FileImage f;
+    if (!f.open(earlier_record_file)) {
+      std::fprintf(stderr, "ERROR: cannot read the earlier record file '%s'\n", earlier_record_file.c_str());
+      return 2;
+    }
+    earlier_record.assign(f.data(), f.data() + f.size());
+    f.release();
+    if (!lfr::record::check(earlier_record.data(), earlier_record.size(), nullptr)) {
+      std::fprintf(stderr, "ERROR: '%s' is not a problem record\n", earlier_record_file.c_str());
+      return 2;
     }
   }
 
@@ -522,7 +561,8 @@ int main(int argc, char** argv) {
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
                                  lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
-                                 lfr_plan_update_solution && lfr_plan_update_solution_since;
+                                 lfr_plan_update_solution && lfr_plan_update_solution_since && lfr_plan_problem_record &&
+                                 lfr_plan_update_solution_since_record;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -603,7 +643,11 @@ int main(int argc, char** argv) {
     }
     // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
     int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), (uint32_t)names.size()) : LFR_OK;
-    if (rc2 == LFR_OK && have_previous) {
+    if (rc2 == LFR_OK && have_earlier) {
+      rc2 = lfr_plan_update_solution_since_record(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                                  name_blob.data(), name_off.data(), earlier_record.data(),
+                                                  earlier_record.size(), nullptr, nullptr, nullptr);
+    } else if (rc2 == LFR_OK && have_previous) {
       // the earlier run's graph stage on the device, for the compare only
       const lfr_host_input pin = previous.input();
       lfr_plan* prev_plan = nullptr;
@@ -648,6 +692,14 @@ int main(int argc, char** argv) {
   }
   const uint32_t N = sz.n_nodes, C = sz.n_components;
   const uint64_t E = sz.n_edges;
+  // the host route's problem with the reference's is_root (the update since an earlier run and the record read it)
+  auto host_problem = [&] {
+    lfr_problem p;
+    p.n_nodes = N; p.n_components = C; p.n_edges = E;
+    p.row_ptr = row_ptr.data(); p.edges = edges; p.track = track.data(); p.comp = comp.data();
+    p.is_root = is_root.data(); p.comp_ptr = comp_ptr.data(); p.comp_nodes = comp_nodes.data();
+    return p;
+  };
   std::printf("# graph nodes: %u\n", N);                                  // solve.cc:484
   std::printf("# graph edges: %llu\n", (unsigned long long)E);            // solve.cc:485
   if (N) {
@@ -672,11 +724,17 @@ int main(int argc, char** argv) {
     if (!positions) positions = static_cast<double*>(std::malloc(2ull * N * sizeof(double)));
     std::memset(positions, 0, 2ull * N * sizeof(double));
     std::vector<uint8_t> has_entry(keep_start || update_start ? N : 0, 0);
-    if (have_previous) {
-      lfr_problem cur;
-      cur.n_nodes = N; cur.n_components = C; cur.n_edges = E;
-      cur.row_ptr = row_ptr.data(); cur.edges = edges; cur.track = track.data(); cur.comp = comp.data();
-      cur.is_root = is_root.data(); cur.comp_ptr = comp_ptr.data(); cur.comp_nodes = comp_nodes.data();
+    if (have_earlier) {
+      const lfr_problem cur = host_problem();
+      if (lfr_wire_update_solution_since_record(start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                                name_blob.data(), name_off.data(), &cur, node_image.data(), node_feat.data(),
+                                                earlier_record.data(), earlier_record.size(), positions, has_entry.data(),
+                                                nullptr, nullptr, nullptr) != LFR_OK) {
+        std::fprintf(stderr, "ERROR: lfr_wire_update_solution_since_record failed\n");
+        return 2;
+      }
+    } else if (have_previous) {
+      const lfr_problem cur = host_problem();
       const lfr_host_input pin = previous.input();
       if (lfr_wire_update_solution_since(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
                                          name_off.data(), &cur, node_image.data(), node_feat.data(), &pin,
@@ -742,6 +800,32 @@ int main(int argc, char** argv) {
   const Clock::time_point t_end = Clock::now();
   std::printf("Solver time: %lldms\n", ms_between(t_solve, t_end));  // solve.cc:638
   std::printf("Total time: %lldms\n", ms_between(t_start, t_end));   // solve.cc:641
+
+  // ---- --record_file: this run's problem record (include/lfr_graph.h), from the reference roots
+  std::vector<uint8_t> record_out;
+  if (have_record) {
+    int64_t got = -1;
+    if (plan) {
+      const int64_t need_r = lfr_plan_problem_record(plan, nullptr, (uint32_t)names.size(), name_blob.data(),
+                                                     name_off.data(), nullptr, 0);
+      record_out.resize(need_r > 0 ? (size_t)need_r : 0);
+      got = need_r < 0 ? need_r
+                       : lfr_plan_problem_record(plan, nullptr, (uint32_t)names.size(), name_blob.data(), name_off.data(),
+                                                 record_out.data(), record_out.size());
+    } else {
+      const lfr_problem cur = host_problem();
+      const int64_t need_r = lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), (uint32_t)names.size(),
+                                                     name_blob.data(), name_off.data(), nullptr, 0);
+      record_out.resize(need_r > 0 ? (size_t)need_r : 0);
+      got = need_r < 0 ? need_r
+                       : lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), (uint32_t)names.size(),
+                                                 name_blob.data(), name_off.data(), record_out.data(), record_out.size());
+    }
+    if (got < 0 || (uint64_t)got != record_out.size()) {
+      std::fprintf(stderr, "ERROR: the problem record failed (%d): %s\n", (int)got, lfr_last_error());
+      return 2;
+    }
+  }
 
   // ---- SolutionFile (solve.cc:643-679): images by first node appearance, nodes by index ------
   uint64_t n_outside = 0;
@@ -840,6 +924,14 @@ int main(int argc, char** argv) {
   if (!written) {
     std::fputs("Failed to write proto object.\n", stderr);  // solve.cc:674-677
     return 255;
+  }
+  if (have_record) {
+    std::ofstream f(record_file, std::ios::binary | std::ios::trunc);
+    if (f.good()) f.write(reinterpret_cast<const char*>(record_out.data()), (std::streamsize)record_out.size());
+    if (!f.good()) {
+      std::fprintf(stderr, "ERROR: cannot write the record file '%s'\n", record_file.c_str());
+      return 255;
+    }
   }
   return 0;
 }

@@ -14,6 +14,7 @@
 #include "../../include/lfr_host.h"
 #include "../../include/lfr_wire.h"
 #include "lfr_join.h"
+#include "lfr_record.h"
 
 namespace {
 
@@ -582,6 +583,137 @@ int lfr_wire_update_solution_since(const uint8_t* buf, uint64_t len, uint32_t n_
                                           positions, held, n_held, n_touched, changed.data());
   if (rc3 == LFR_OK && n_changed) *n_changed = nc;
   return rc3;
+}
+
+namespace {
+
+using Digest = std::pair<uint64_t, uint64_t>;
+
+// The checks of lfr_host_problem_record(): a problem whose arrays are consistent, node ids within the names
+bool record_input_ok(const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat, uint32_t n_images,
+                     const uint8_t* names, const uint64_t* name_off) {
+  if (!p) return false;
+  const uint32_t N = p->n_nodes, C = p->n_components;
+  if (N && (!p->row_ptr || !p->track || !p->comp || !p->is_root || !node_image || !node_feat)) return false;
+  if (N && (p->row_ptr[0] != 0 || p->row_ptr[N] != p->n_edges || (p->n_edges && !p->edges))) return false;
+  if (!N && p->n_edges) return false;
+  for (uint32_t v = 0; v < N; ++v)
+    if (p->comp[v] >= C || node_image[v] >= n_images || p->row_ptr[v + 1] < p->row_ptr[v]) return false;
+  for (uint64_t e = 0; e < p->n_edges; ++e)
+    if (p->edges[e].dst >= N) return false;
+  if (n_images && !name_off) return false;
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return false;
+  return !(n_images && name_off[n_images] && !names);
+}
+
+// digest[c] of every component c of `p` (include/lfr_graph.h; lfr_record.h has the elements).  Components
+// are dealt to helper threads in blocks; each digest is one thread's exact sum, so the result does not
+// depend on the thread count (LFR_HOST_THREADS overrides it).
+std::vector<Digest> component_digests(const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat,
+                                      uint32_t n_images, const uint8_t* names, const uint64_t* name_off) {
+  namespace rec = lfr::record;
+  const uint32_t N = p->n_nodes, C = p->n_components;
+  std::vector<Digest> id(n_images);
+  for (uint32_t k = 0; k < n_images; ++k)
+    rec::hash_bytes(names + name_off[k], name_off[k + 1] - name_off[k], id[k].first, id[k].second);
+  std::vector<uint32_t> start((size_t)C + 1, 0), order(N);  // nodes by component
+  for (uint32_t v = 0; v < N; ++v) ++start[p->comp[v] + 1];
+  for (uint32_t c = 0; c < C; ++c) start[c + 1] += start[c];
+  {
+    std::vector<uint32_t> fill(start.begin(), start.end() - 1);
+    for (uint32_t v = 0; v < N; ++v) order[fill[p->comp[v]]++] = v;
+  }
+  std::vector<Digest> digest(C, Digest(0, 0));
+  auto one = [&](uint32_t c) {
+    uint64_t s0 = 0, s1 = 0, h0, h1;
+    for (uint32_t k = start[c]; k < start[c + 1]; ++k) {
+      const uint32_t v = order[k];
+      const Digest& iv = id[node_image[v]];
+      rec::node_element(iv.first, iv.second, node_feat[v], p->is_root[v] != 0, h0, h1);
+      s0 += h0;
+      s1 += h1;
+      for (uint32_t e = p->row_ptr[v]; e < p->row_ptr[v + 1]; ++e) {
+        const lfr_edge& r = p->edges[e];
+        const uint32_t w = r.dst, kind = rec::edge_kind(p->track[v], p->track[w], p->comp[v], p->comp[w]);
+        if (kind == LFR_EDGE_SKIP) continue;
+        uint32_t words[19];
+        std::memcpy(words, &r, sizeof words);  // flow[18], sim
+        const Digest& iw = id[node_image[w]];
+        rec::edge_element(iv.first, iv.second, iw.first, iw.second, node_feat[v], node_feat[w], kind, words, h0, h1);
+        s0 += h0;
+        s1 += h1;
+      }
+    }
+    digest[c] = Digest(s0, s1);
+  };
+  unsigned n_thr = 1;
+  if ((uint64_t)N + p->n_edges >= (1u << 16)) {
+    const unsigned hw = std::thread::hardware_concurrency();
+    n_thr = std::min(8u, hw ? hw : 1u);
+  }
+  if (const char* e = std::getenv("LFR_HOST_THREADS")) n_thr = (unsigned)std::max(1, std::min(64, std::atoi(e)));
+  constexpr uint32_t kBlock = 64;
+  std::atomic<uint32_t> next{0};
+  auto work = [&] {
+    for (;;) {
+      const uint32_t b = next.fetch_add(1);
+      if ((uint64_t)b * kBlock >= C) return;
+      for (uint32_t c = b * kBlock; c < std::min<uint64_t>(C, (uint64_t)(b + 1) * kBlock); ++c) one(c);
+    }
+  };
+  std::vector<std::thread> helpers;
+  for (unsigned t = 1; t < n_thr; ++t) helpers.emplace_back(work);
+  work();
+  for (std::thread& h : helpers) h.join();
+  return digest;
+}
+
+}  // namespace
+
+int64_t lfr_host_problem_record(const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat,
+                                uint32_t n_images, const uint8_t* names, const uint64_t* name_off, uint8_t* out,
+                                uint64_t cap) {
+  namespace rec = lfr::record;
+  if (!record_input_ok(p, node_image, node_feat, n_images, names, name_off)) return LFR_EINVAL;
+  const uint64_t need = rec::record_bytes(p->n_components);
+  if (!out || cap < need) return (int64_t)need;
+  std::vector<Digest> d = component_digests(p, node_image, node_feat, n_images, names, name_off);
+  std::sort(d.begin(), d.end());
+  rec::store_u64(out, rec::kMagic);
+  rec::store_u64(out + 8, d.size());
+  for (size_t c = 0; c < d.size(); ++c) {
+    rec::store_u64(out + rec::kHeaderBytes + 16 * c, d[c].first);
+    rec::store_u64(out + rec::kHeaderBytes + 16 * c + 8, d[c].second);
+  }
+  return (int64_t)need;
+}
+
+int lfr_wire_update_solution_since_record(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names,
+                                          const uint64_t* name_off, const lfr_problem* p, const uint32_t* node_image,
+                                          const uint32_t* node_feat, const uint8_t* record, uint64_t record_len,
+                                          double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched,
+                                          uint32_t* n_changed) {
+  namespace rec = lfr::record;
+  if (!record_input_ok(p, node_image, node_feat, n_images, names, name_off)) return LFR_EINVAL;
+  uint64_t R = 0;
+  if (!rec::check(record, record_len, &R)) return LFR_EINVAL;
+  const uint32_t C = p->n_components;
+  const std::vector<Digest> d = component_digests(p, node_image, node_feat, n_images, names, name_off);
+  std::vector<Digest> earlier(R);
+  for (uint64_t k = 0; k < R; ++k)
+    earlier[k] = Digest(rec::load_u64(record + rec::kHeaderBytes + 16 * k), rec::load_u64(record + rec::kHeaderBytes + 16 * k + 8));
+  std::vector<uint8_t> changed(C, 0);
+  uint32_t nc = 0;
+  for (uint32_t c = 0; c < C; ++c)
+    if (!std::binary_search(earlier.begin(), earlier.end(), d[c])) {
+      changed[c] = 1;
+      ++nc;
+    }
+  const int rc = lfr::join::update_nodes(buf, len, n_images, names, name_off, p->n_nodes, node_image, node_feat, p->comp, C,
+                                         positions, held, n_held, n_touched, changed.data());
+  if (rc == LFR_OK && n_changed) *n_changed = nc;
+  return rc;
 }
 
 int64_t lfr_wire_encode_solution_carried(uint64_t n_images, const uint64_t* img_ptr, const uint8_t* names,

@@ -29,6 +29,7 @@ class Solution:
     di: np.ndarray            # [N] float32 (row displacement, positions[node][0])
     dj: np.ndarray            # [N] float32 (col displacement, positions[node][1])
     n_outside: int            # "# points with at least one coordinate > 0.5" (solve.cc:666-670)
+    record: Optional[bytes] = None  # the run's problem record (include/lfr_graph.h), with refine(record_problem=True)
 
 
 def assemble_solution(p: Problem, positions: np.ndarray) -> Solution:
@@ -103,20 +104,24 @@ def fixed_image_mask(image_names: List[str], fixed_images) -> np.ndarray:
 
 def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[bytes] = None,
                      keep_initial_solution: bool = False, update_initial_solution: bool = False,
-                     previous_matches: Optional[MatchSet] = None):
+                     previous_matches: Optional[MatchSet] = None, previous_record: Optional[bytes] = None):
     """The host route's problem initialisation with fixed images and a start solution: (the Problem to solve,
     whose is_root is the constant mask = reference root OR node of a fixed image OR, with
     `keep_initial_solution`, node with an entry in the start solution OR, with `update_initial_solution`,
     node of a component the start solution covers whole (wire.update_solution) and, with `previous_matches`,
-    that is unchanged since that MatchingFile's run (wire.update_solution_since); start positions [N, 2] from
-    wire.join_solution or wire.update_solution(_since), or None for zeros)."""
+    that is unchanged since that MatchingFile's run (wire.update_solution_since) or, with `previous_record`,
+    whose digest is in that run's problem record (wire.update_solution_since_record); start positions [N, 2]
+    from wire.join_solution or wire.update_solution(_since(_record)), or None for zeros)."""
     from . import wire
     g = p.graph
     const = np.asarray(p.is_root) != 0
     if len(fixed_images) and g.n_nodes:
         const = const | fixed_image_mask(g.image_names, fixed_images)[np.asarray(g.node_image, np.int64)]
     start = None
-    if initial_solution is not None and update_initial_solution and previous_matches is not None:
+    if initial_solution is not None and update_initial_solution and previous_record is not None:
+        start, held, _, _, _ = wire.update_solution_since_record(initial_solution, p, previous_record)
+        const = const | held
+    elif initial_solution is not None and update_initial_solution and previous_matches is not None:
         start, held, _, _, _ = wire.update_solution_since(initial_solution, p, previous_matches)
         const = const | held
     elif initial_solution is not None and update_initial_solution:
@@ -135,7 +140,8 @@ def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[byt
 def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[[str], None]] = None,
            solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None, fixed_images=(),
            initial_solution: Optional[bytes] = None, keep_initial_solution: bool = False,
-           update_initial_solution: bool = False, previous_matches=None):
+           update_initial_solution: bool = False, previous_matches=None, previous_record: Optional[bytes] = None,
+           record_problem: bool = False):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
     may be supplied to drive a different executor (the multi-GPU path; give `n_devices`); with a start
     solution it is called as `solve_fn(problem, positions)`.
@@ -150,8 +156,12 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     values (wire.update_solution, Plan.update_solution).  `previous_matches` (needs `update_initial_solution`;
     a MatchSet or MatchingFile bytes) is the MatchingFile that produced `initial_solution`: a component is then
     also touched when its problem is not the one that file's run solved (include/lfr_graph.h states the
-    rule; wire.update_solution_since, Plan.update_solution(previous=...)).  The returned Problem keeps the
-    reference's is_root.
+    rule; wire.update_solution_since, Plan.update_solution(previous=...)).  `previous_record` (needs
+    `update_initial_solution`, excludes `previous_matches`) is that run's problem record instead: a component is
+    unchanged when its digest is in the record (wire.update_solution_since_record,
+    Plan.update_solution(previous_record=...)).  With `record_problem` the returned Solution's `record` is this
+    run's problem record (wire.problem_record on the host route, Plan.problem_record on the device route; the
+    same bytes), for the next update.  The returned Problem keeps the reference's is_root.
 
     The graph stage runs where graph_stage_on_device() says.  On the device (Plan.from_matches) the problem
     stays in HBM and is solved there, `solve_fn` is not called, and the Problem's arrays come from
@@ -166,6 +176,15 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
         raise ValueError("update_initial_solution and keep_initial_solution exclude each other")
     if previous_matches is not None and not update_initial_solution:
         raise ValueError("previous_matches needs update_initial_solution")
+    if previous_record is not None and not update_initial_solution:
+        raise ValueError("previous_record needs update_initial_solution")
+    if previous_record is not None and previous_matches is not None:
+        raise ValueError("previous_record and previous_matches exclude each other")
+    if previous_record is not None:
+        from .wire import record_is_valid
+        previous_record = bytes(previous_record)
+        if not record_is_valid(previous_record):
+            raise ValueError("malformed problem record")
     if isinstance(previous_matches, (bytes, bytearray, memoryview)):
         from .wire import decode_matching_file
         previous_matches = decode_matching_file(bytes(previous_matches))
@@ -174,15 +193,21 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     if not graph_stage_on_device(lib, arrs, len(ms.image_names), n_devices):
         p = build_problem(ms, banned_images, log=log)
         q, start = constant_problem(p, fixed_images, initial_solution, keep_initial_solution, update_initial_solution,
-                                    previous_matches)
+                                    previous_matches, previous_record)
         fn = solve_fn if solve_fn is not None else (lambda q_, x=None: solve_problem(q_, options, x))
         pos, st = fn(q) if start is None else fn(q, start)
-        return p, pos, st, assemble_solution(p, pos)
+        sol = assemble_solution(p, pos)
+        if record_problem:
+            from .wire import problem_record
+            sol.record = problem_record(p, ms.image_names)
+        return p, pos, st, sol
     plan = Plan.from_matches(lib, arrs, options=options, n_images=len(ms.image_names))
     try:
         if len(fixed_images) and fixed_image_mask(ms.image_names, fixed_images).any():
             plan.fix_images(fixed_image_mask(ms.image_names, fixed_images))
-        if update_initial_solution and previous_matches is not None:
+        if update_initial_solution and previous_record is not None:
+            plan.update_solution(initial_solution, ms.image_names, previous_record=previous_record)
+        elif update_initial_solution and previous_matches is not None:
             prev = Plan.from_matches(lib, previous_matches, options=options)
             try:
                 plan.update_solution(initial_solution, ms.image_names, previous=prev)
@@ -203,6 +228,9 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
             pos, st = solve_problem(p, options)
         if timing is not None:
             timing["solver_ms"] = (time.perf_counter() - t1) * 1e3
+        record = plan.problem_record(ms.image_names) if record_problem else None
     finally:
         plan.close()
-    return p, pos, st, assemble_solution(p, pos)
+    sol = assemble_solution(p, pos)
+    sol.record = record
+    return p, pos, st, sol

@@ -29,7 +29,7 @@ class WireMatches(C.Structure):
 WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
                 "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution",
                 "lfr_wire_join_solution_entries", "lfr_wire_encode_solution_carried", "lfr_wire_update_solution",
-                "lfr_wire_update_solution_since"]
+                "lfr_wire_update_solution_since", "lfr_host_problem_record", "lfr_wire_update_solution_since_record"]
 
 _bound = False
 
@@ -66,6 +66,12 @@ def _lib():
         L.lfr_wire_update_solution_since.argtypes = ([C.c_void_p, C.c_uint64, C.c_uint32] + [C.c_void_p] * 10 +
                                                      [C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)])
         L.lfr_wire_update_solution_since.restype = C.c_int
+        L.lfr_host_problem_record.argtypes = [C.c_void_p] * 3 + [C.c_uint32] + [C.c_void_p] * 3 + [C.c_uint64]
+        L.lfr_host_problem_record.restype = C.c_int64
+        L.lfr_wire_update_solution_since_record.argtypes = ([C.c_void_p, C.c_uint64, C.c_uint32] + [C.c_void_p] * 6 +
+                                                            [C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64),
+                                                             C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)])
+        L.lfr_wire_update_solution_since_record.restype = C.c_int
         _bound = True
     return L
 
@@ -380,3 +386,80 @@ def _solution_parses(data: bytes) -> bool:
     ni, nd = C.c_uint64(), C.c_uint64()
     return L.lfr_wire_decode_solution(buf.ctypes.data if buf.size else None, buf.size, C.byref(ni), C.byref(nd),
                                       *([None] * 7)) == 0
+
+
+RECORD_MAGIC = b"LFRPREC1"
+
+
+def record_is_valid(record: bytes) -> bool:
+    """Whether `record` is a well-formed problem record (include/lfr_graph.h): the magic "LFRPREC1", the length
+    16 + 16 C for its count C, and the C digests in ascending (d0, d1) order."""
+    if len(record) < 16 or record[:8] != RECORD_MAGIC:
+        return False
+    n = int.from_bytes(record[8:16], "little")
+    if len(record) != 16 + 16 * n:
+        return False
+    d = np.frombuffer(record, dtype="<u8", offset=16).reshape(-1, 2)
+    if n < 2:
+        return True
+    a0, a1, b0, b1 = d[:-1, 0], d[:-1, 1], d[1:, 0], d[1:, 1]
+    return bool(np.all((b0 > a0) | ((b0 == a0) & (b1 >= a1))))
+
+
+def _record_args(p, image_names):
+    from .capi import Library
+    g = p.graph
+    s, keep = Library.marshal(p)
+    blob, off = _names_blob(list(g.image_names if image_names is None else image_names))
+    img = np.ascontiguousarray(g.node_image, dtype=np.uint32).reshape(-1)
+    feat = np.ascontiguousarray(g.node_feat, dtype=np.uint32).reshape(-1)
+    return s, keep, blob, off, img, feat
+
+
+def problem_record(p, image_names=None) -> bytes:
+    """The problem record of Problem `p` on the host (lfr_host_problem_record, include/lfr_host.h; the record is
+    stated in include/lfr_graph.h), byte for byte Plan.problem_record().  `p.is_root` must be the reference's
+    is_root, as build_problem() leaves it.  `image_names` by image id (default: p.graph.image_names)."""
+    L = _lib()
+    s, keep, blob, off, img, feat = _record_args(p, image_names)
+    N = int(img.shape[0])
+    args = (C.addressof(s), img.ctypes.data if N else None, feat.ctypes.data if N else None, len(off) - 1,
+            blob.ctypes.data, off.ctypes.data)
+    need = L.lfr_host_problem_record(*args, None, 0)
+    if need < 0:
+        raise RuntimeError("lfr_host_problem_record failed (%d)" % need)
+    out = np.empty(max(int(need), 1), np.uint8)
+    got = L.lfr_host_problem_record(*args, out.ctypes.data, int(need))
+    del keep
+    if got != need:
+        raise RuntimeError("lfr_host_problem_record failed (%d)" % got)
+    return out[:need].tobytes()
+
+
+def update_solution_since_record(data: bytes, p, record: bytes):
+    """The host form of Plan.update_solution(previous_record=...) (lfr_wire_update_solution_since_record,
+    include/lfr_host.h): update_solution_since() with the earlier run's problem record in place of its
+    MatchingFile.  Returns (positions [N, 2], held [N] bool, held nodes, touched components, changed
+    components).  Raises ParseError on SolutionFile bytes the decoder rejects, ValueError on a malformed
+    record, RuntimeError when the arrays are rejected."""
+    L = _lib()
+    if not record_is_valid(bytes(record)):
+        raise ValueError("malformed problem record")
+    if not _solution_parses(data):
+        raise ParseError("Failed to parse proto object.")
+    s, keep, blob, off, img, feat = _record_args(p, None)
+    buf = np.frombuffer(data, dtype=np.uint8)
+    rec = np.frombuffer(bytes(record), dtype=np.uint8)
+    N = int(img.shape[0])
+    pos = np.zeros((N, 2), np.float64)
+    held = np.zeros(N, np.uint8)
+    n, t, ch = C.c_uint64(), C.c_uint32(), C.c_uint32()
+    rc = L.lfr_wire_update_solution_since_record(buf.ctypes.data if buf.size else None, buf.size, len(off) - 1,
+                                                 blob.ctypes.data, off.ctypes.data, C.addressof(s),
+                                                 img.ctypes.data if N else None, feat.ctypes.data if N else None,
+                                                 rec.ctypes.data, rec.size, pos.ctypes.data if N else None,
+                                                 held.ctypes.data if N else None, C.byref(n), C.byref(t), C.byref(ch))
+    del keep
+    if rc != 0:
+        raise RuntimeError("lfr_wire_update_solution_since_record failed (%d)" % rc)
+    return pos, held.astype(bool), int(n.value), int(t.value), int(ch.value)
