@@ -90,6 +90,14 @@ int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images
                                  const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
                                  uint64_t* n_outside);
 
+/* lfr_plan_encode_solution() restricted to the images k with written[k] != 0 (--query_images writes the query
+ * images only): the other images get no Image message, and the bytes are those of the full encoding with
+ * their Image messages left out.  *n_outside still counts every node.  Same size protocol and errors, and
+ * LFR_EINVAL for a NULL `written`. */
+int64_t lfr_plan_encode_solution_images(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                        const uint64_t* name_off, const float* fact, const uint8_t* written, uint8_t* out,
+                                        uint64_t cap, uint64_t* n_outside);
+
 /* lfr_plan_encode_solution() merged with an earlier SolutionFile `file`: the scene's output, each scene
  * image followed by its carried entries, then the file's other winning Image messages — the bytes of
  * lfr_wire_encode_solution_carried() (include/lfr_wire.h, which states the rule) on the plan's host assembly

@@ -359,7 +359,8 @@ class Plan:
                      positions: Optional[np.ndarray] = None, n_images: Optional[int] = None) -> "Plan":
         """lfr_plan_create_from_matches (include/lfr_graph.h): the graph stage runs on the device and the
         problem stays there.  `matches` is a MatchSet or a dict of the flat lfr_host_input arrays
-        (pair_img1, pair_img2, pair_skip, pair_ptr, feat1, feat2, sim, disp1, disp2; n_images required).
+        (pair_img1, pair_img2, pair_skip, pair_ptr, feat1, feat2, sim, disp1, disp2, optionally image_group;
+        n_images required).
         `self.sizes` is the lfr_host_sizes of the stage as a dict."""
         if isinstance(matches, dict):
             arrs = {k: np.ascontiguousarray(v, dtype=dt) for k, (v, dt) in
@@ -369,6 +370,8 @@ class Plan:
                                                          ("disp1", np.float32), ("disp2", np.float32)))}
             if n_images is None:
                 raise ValueError("n_images is required with flat arrays")
+            if matches.get("image_group") is not None:   # sub-scenes (MatchSet.query_subscenes)
+                arrs["image_group"] = np.ascontiguousarray(matches["image_group"], dtype=np.uint32)
         else:
             _, arrs = host_input_arrays(matches, banned_images)
             n_images = len(matches.image_names) if n_images is None else n_images

@@ -28,6 +28,9 @@ after the SolutionFile, and --earlier_record_file FILE (with --update_initial_so
 --previous_matches_file) reads the record the run that produced the initial solution wrote, in place of its
 MatchingFile: a component is unchanged when its digest is in that record (wire.problem_record,
 Plan.problem_record, Plan.update_solution(previous_record=...)).
+--query_images NAME (repeatable) localizes many queries in one run: a pair that names one query image belongs
+to that query's sub-scene, a pair that names none is not solved, and each query is refined as a run on its
+sub-scene's pairs alone refines it (solver.refine(query_images=...)).  Only query images are written.
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -65,7 +68,7 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("fixed_images", True, True), ("initial_solution", True, False),
             ("keep_initial_solution", False, False), ("carry_initial_solution", False, False),
             ("update_initial_solution", False, False), ("previous_matches_file", True, False),
-            ("record_file", True, False), ("earlier_record_file", True, False)]
+            ("record_file", True, False), ("earlier_record_file", True, False), ("query_images", True, True)]
 
 
 def _find_option(name):
@@ -144,7 +147,8 @@ def parse_args(argv):
             carry_initial_solution=bool(vals.get("carry_initial_solution")),
             update_initial_solution=bool(vals.get("update_initial_solution")),
             previous_matches_file=vals.get("previous_matches_file"),
-            record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"))
+            record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"),
+            query_images=vals.get("query_images"))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -181,6 +185,15 @@ def main(argv=None) -> int:
     if args.earlier_record_file is not None and args.previous_matches_file is not None:
         sys.stderr.write("ERROR: --earlier_record_file and --previous_matches_file exclude each other\n")
         return 2
+    if args.query_images is not None:
+        for on, opt in ((args.update_initial_solution, "--update_initial_solution"),
+                        (args.previous_matches_file is not None, "--previous_matches_file"),
+                        (args.record_file is not None, "--record_file"),
+                        (args.earlier_record_file is not None, "--earlier_record_file"),
+                        (args.carry_initial_solution, "--carry_initial_solution")):
+            if on:
+                sys.stderr.write("ERROR: --query_images and %s exclude each other\n" % opt)
+                return 2
     start = None
     if args.initial_solution is not None:
         try:
@@ -269,13 +282,22 @@ def main(argv=None) -> int:
         sys.stderr.write("ERROR: --record_file / --earlier_record_file: torchrun ranks do not write or read "
                          "problem records; use --gpus N\n")
         return 2
+    if torchrun and args.query_images is not None:
+        sys.stderr.write("ERROR: --query_images: torchrun ranks do not localize queries; use --gpus N\n")
+        return 2
     try:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
                                  timing=timing, fixed_images=args.fixed_images, initial_solution=start,
                                  keep_initial_solution=args.keep_initial_solution,
                                  update_initial_solution=args.update_initial_solution, previous_matches=previous,
-                                 previous_record=earlier_record, record_problem=args.record_file is not None)
+                                 previous_record=earlier_record, record_problem=args.record_file is not None,
+                                 query_images=args.query_images)
     except GraphStageRouteError as e:
+        sys.stderr.write("ERROR: %s\n" % e)
+        return 2
+    except ValueError as e:   # --query_images: a pair that names two query images, or too many images
+        if args.query_images is None:
+            raise
         sys.stderr.write("ERROR: %s\n" % e)
         return 2
     say("Solver time: %dms" % int(timing.get("solver_ms", 0.0)))                       # solve.cc:638

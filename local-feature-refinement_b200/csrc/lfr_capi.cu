@@ -1023,8 +1023,10 @@ int group_cut_edges(uint32_t* key, const uint32_t* idx, uint32_t n, int key_bits
 // lfr_cut.h recursive_cut_all on the device, one launch set per recursion level.  E[0] holds the roots'
 // m edges (no self-loops) over nodes 0..n_nodes-1, grouped into n_sub roots; E[1] has room for m edges.
 // Every node of a root gets label[x] = label_base + (the lowest node of its group); *n_groups = groups.
+// node_cap (device, may be NULL): a per-node max_weight, the same for every node of a root (sub-scenes).
 int recursive_cut_on_device(uint32_t n_nodes, CutLists (&E)[2], uint32_t m, uint32_t n_sub, const uint32_t* node_weight,
-                            uint64_t max_weight, uint32_t label_base, uint32_t* label, uint32_t* n_groups, DevBuf& tmp, cudaStream_t s) {
+                            uint64_t max_weight, uint32_t label_base, uint32_t* label, uint32_t* n_groups, DevBuf& tmp, cudaStream_t s,
+                            const uint32_t* node_cap = nullptr) {
   using namespace lfr::cut;
   *n_groups = 0;
   if (!m) return LFR_OK;
@@ -1107,6 +1109,7 @@ int recursive_cut_on_device(uint32_t n_nodes, CutLists (&E)[2], uint32_t m, uint
     L.pside = pside.as<uint8_t>();
     L.stamp = 2 * lvl + 1;
     L.max_weight = max_weight;
+    L.node_cap = node_cap;
     L.side_w = side_w.as<long long>();
     L.side_min = side_min.as<uint32_t>();
     L.cont = cont.as<uint8_t>();
@@ -1177,6 +1180,22 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
   auto G = std::make_unique<lfr_plan::GraphArrays>();
   const uint64_t P = in->n_pairs;
   const uint32_t n_images = in->n_images;
+  // sub-scenes (lfr_host_input::image_group): each image's index inside its sub-scene and the set width, as
+  // lfr_host.cc has them; the cut cap of each image's sub-scene once the seen images are known
+  const uint32_t* group = in->image_group;
+  std::vector<uint32_t> local_image, image_cap;
+  uint32_t set_width = n_images, n_groups = 0;
+  if (group) {
+    for (uint32_t i = 0; i < n_images; ++i) n_groups = std::max(n_groups, group[i] + 1);
+    std::vector<uint32_t> n_in_group(n_groups, 0);
+    local_image.resize(n_images);
+    for (uint32_t i = 0; i < n_images; ++i) local_image[i] = n_in_group[group[i]]++;
+    set_width = n_groups ? *std::max_element(n_in_group.begin(), n_in_group.end()) : 0;
+    for (uint64_t p = 0; p < in->n_pairs; ++p)  // a pair spans two sub-scenes: the host stage's LFR_EINVAL
+      if (!(in->pair_skip && in->pair_skip[p]) && in->pair_img1[p] < n_images && in->pair_img2[p] < n_images &&
+          group[in->pair_img1[p]] != group[in->pair_img2[p]])
+        return fail(LFR_EINVAL, "a pair spans two sub-scenes");
+  }
   TmpBuf tmp, d_img1, d_img2, d_skip, d_ptr, d_cnt, d_off, d_seen, d_err;
   const auto t_graph = Clock::now();
   // ---- H1: the match list -------------------------------------------------------------------------
@@ -1208,6 +1227,12 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
     std::vector<uint8_t> seen(n_images);
     LFR_TRY(fetch(seen.data(), d_seen.p, n_images, s));
     for (uint8_t v : seen) S->n_images_seen += v;
+    if (group) {
+      std::vector<uint32_t> group_seen(n_groups, 0);
+      for (uint32_t i = 0; i < n_images; ++i) group_seen[group[i]] += seen[i];
+      image_cap.resize(n_images);
+      for (uint32_t i = 0; i < n_images; ++i) image_cap[i] = group_seen[group[i]];
+    }
   }
   if (2 * M >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "more than 2^31 - 1 directed edges");
   const uint64_t E = 2 * M;
@@ -1323,8 +1348,8 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
   }
   UfState U;
   std::memset(&U, 0, sizeof U);
-  U.small_sets = n_images <= 64;
-  U.W = (n_images + 63) / 64;
+  U.small_sets = set_width <= 64;
+  U.W = (set_width + 63) / 64;
   LFR_TRY(d_parent.reserve(4 * (size_t)N));
   LFR_TRY(d_size.reserve(4 * (size_t)N));
   LFR_TRY(d_res.reserve(4 * (size_t)N));
@@ -1332,6 +1357,14 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
   U.size = d_size.as<uint32_t>();
   U.res = d_res.as<uint32_t>();
   U.node_image = d_nimg.as<uint32_t>();
+  TmpBuf d_local, d_nloc;
+  if (group) {  // the sets index images inside their sub-scene
+    LFR_TRY(upload(&d_local, local_image.data(), n_images, s));
+    LFR_TRY(d_nloc.reserve(4 * (size_t)N));
+    gather_kernel<<<blocks_for(N), 256, 0, s>>>(d_nimg.as<uint32_t>(), d_local.as<uint32_t>(), N, d_nloc.as<uint32_t>());
+    LFR_LAUNCHED();
+    U.node_image = d_nloc.as<uint32_t>();
+  }
   if (U.small_sets) {
     LFR_TRY(d_mask.reserve(8 * (size_t)N));
     U.mask = d_mask.as<unsigned long long>();
@@ -1494,7 +1527,19 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
   LFR_TRY(d_big.reserve(4 * (size_t)n_cc));
   LFR_CUDA(cudaMemsetAsync(d_ccn.p, 0, 8 * (size_t)n_cc, s));
   cc_weight_kernel<<<blocks_for(T), 256, 0, s>>>(d_cc.as<uint32_t>(), d_nit.as<uint32_t>(), T, d_ccn.as<unsigned long long>());
-  oversized_kernel<<<blocks_for(n_cc), 256, 0, s>>>(d_ccn.as<unsigned long long>(), n_cc, S->n_images_seen, d_big.as<uint32_t>());
+  // sub-scenes: the cap of every meta-component and of each of its tracks
+  TmpBuf d_icap, d_cccap, d_tcap;
+  if (group) {
+    LFR_TRY(upload(&d_icap, image_cap.data(), n_images, s));
+    LFR_TRY(d_cccap.reserve(4 * (size_t)n_cc));
+    LFR_TRY(d_tcap.reserve(4 * (size_t)T));
+    cc_cap_kernel<<<blocks_for(N), 256, 0, s>>>(d_nimg.as<uint32_t>(), d_track.as<uint32_t>(), d_cc.as<uint32_t>(),
+                                                 d_icap.as<uint32_t>(), N, d_cccap.as<uint32_t>());
+    gather_kernel<<<blocks_for(T), 256, 0, s>>>(d_cc.as<uint32_t>(), d_cccap.as<uint32_t>(), T, d_tcap.as<uint32_t>());
+    LFR_LAUNCHED();
+  }
+  oversized_kernel<<<blocks_for(n_cc), 256, 0, s>>>(d_ccn.as<unsigned long long>(), n_cc, S->n_images_seen,
+                                                    group ? d_cccap.as<uint32_t>() : nullptr, d_big.as<uint32_t>());
   LFR_LAUNCHED();
   {
     uint32_t *big = d_big.as<uint32_t>(), *out = d_red.as<uint32_t>();
@@ -1535,7 +1580,7 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
       LFR_TRY(group_cut_edges(d_rkey.as<uint32_t>(), d_ridx.as<uint32_t>(), n_cut, bits_for(std::max<uint32_t>(n_cc, 2) - 1), E[1], E[0],
                               &n_roots, tmp, s));
       LFR_TRY(recursive_cut_on_device(T, E, n_cut, n_roots, d_nit.as<uint32_t>(), S->n_images_seen, n_cc, d_gc.as<uint32_t>(),
-                                      &S->n_cut_groups, tmp, s));
+                                      &S->n_cut_groups, tmp, s, group ? d_tcap.as<uint32_t>() : nullptr));
     } else {
       LFR_TRY(d_recs.reserve(sizeof(CutRec) * std::max<size_t>(n_cut, 1)));
       if (n_cut) {
@@ -1557,8 +1602,10 @@ int build_graph_on_device(const lfr_host_input* in, MatchArrays& d, lfr_plan* pl
         const size_t sl = (size_t)(std::lower_bound(comps.begin(), comps.end(), r.comp) - comps.begin());
         per_cc[sl].push_back(lfr::CutEdge{r.a, r.b, lfr::cut_weight(r.wsum)});
       }
+      std::vector<uint32_t> track_cap(group ? T : 0);
+      if (group) LFR_TRY(fetch(track_cap.data(), d_tcap.p, T, s));
       std::vector<std::vector<uint32_t>> groups;
-      lfr::recursive_cut_all(std::move(per_cc), node_weight, S->n_images_seen, &groups);
+      lfr::recursive_cut_all(std::move(per_cc), node_weight, S->n_images_seen, &groups, group ? track_cap.data() : nullptr);
       std::vector<uint32_t> gidx, gval;
       for (size_t g = 0; g < groups.size(); ++g)
         for (uint32_t t : groups[g]) {
@@ -1942,7 +1989,7 @@ thread_local double g_encode_ms[2] = {};
 // lfr_plan_encode_solution() on a checked plan and arguments (lfr_solution.cuh): the sizing kernels, one
 // synchronisation for the total, then — when `out` has room — the writing kernels and one copy to `out`
 int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t* names, const uint64_t* name_off,
-                        const float* fact, uint8_t* out, uint64_t cap, uint64_t* n_outside) {
+                        const float* fact, uint8_t* out, uint64_t cap, uint64_t* n_outside, const uint8_t* written = nullptr) {
   using namespace lfr::solution;
   const uint32_t N = pl->N;
   if (n_outside) *n_outside = 0;
@@ -1962,13 +2009,13 @@ int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t
                o_ioff = take(8 * ((size_t)NI + 1)), o_name_off = take(8 * ((size_t)NI + 1)), o_fact = take(4 * (size_t)NI),
                o_names = take(name_bytes), o_key = take(4 * (size_t)N), o_key_s = take(4 * (size_t)N),
                o_iota = take(4 * (size_t)N), o_perm = take(4 * (size_t)N), o_rsize = take(8 * ((size_t)N + 1)),
-               o_noff = take(8 * ((size_t)N + 1));
+               o_noff = take(8 * ((size_t)N + 1)), o_written = take(written ? NI : 0);
   LFR_TRY(pl->enc_scratch.reserve(at));
   uint8_t* base = pl->enc_scratch.as<uint8_t>();
   auto u32 = [base](size_t o) { return reinterpret_cast<uint32_t*>(base + o); };
   auto u64 = [base](size_t o) { return reinterpret_cast<uint64_t*>(base + o); };
   uint32_t *first = u32(o_first), *first_s = u32(o_first_s), *iota_i = u32(o_iota_i), *img_s = u32(o_img_s),
-           *rank = u32(o_rank), *img_ptr = u32(o_img_ptr), *n_present = u32(o_ctr + 8), *key = u32(o_key),
+           *rank = u32(o_rank), *img_ptr = u32(o_img_ptr), *n_present = u32(o_ctr + 8), *n_written = u32(o_ctr + 12), *key = u32(o_key),
            *key_s = u32(o_key_s), *iota = u32(o_iota), *perm = u32(o_perm);
   uint64_t *body = u64(o_body), *isize = u64(o_isize), *ioff = u64(o_ioff), *d_name_off = u64(o_name_off),
            *rsize = u64(o_rsize), *noff = u64(o_noff);
@@ -1983,21 +2030,30 @@ int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t
   LFR_CUDA(cudaMemcpyAsync(d_fact, fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
   if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, names, name_bytes, cudaMemcpyHostToDevice, s));
   LFR_CUDA(cudaMemsetAsync(base + o_ctr, 0, 16, s));
+  const uint8_t* d_written = written ? base + o_written : nullptr;
+  if (written) LFR_CUDA(cudaMemcpyAsync(base + o_written, written, NI, cudaMemcpyHostToDevice, s));
   init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
-  first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside);
+  first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside, d_written);
   LFR_LAUNCHED();
   LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {
     return cub::DeviceRadixSort::SortPairs(t, nb, first, first_s, iota_i, img_s, (int)NI, 0, bits_for(N), s);
   }));
   rank_kernel<<<blocks_for(NI), 256, 0, s>>>(first_s, img_s, NI, N, rank, n_present);
-  node_key_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, rank, N, key, iota);
+  node_key_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, rank, N, key, iota, d_written, NI, n_written);
   LFR_LAUNCHED();
   LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: ascending node index within an image
     return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, iota, perm, (int)N, 0, bits_for(NI), s);
   }));
-  record_size_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, N, rsize, img_ptr);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, noff, (int)N + 1, s); }));
+  // the written nodes lead the sorted order; the others get no record
+  uint32_t NW = N;
+  if (written) LFR_TRY(fetch(&NW, n_written, 1, s));
+  if (NW) {
+    record_size_kernel<<<blocks_for(NW), 256, 0, s>>>(perm, key_s, nfeat, pos, NW, rsize, img_ptr);
+    LFR_LAUNCHED();
+  } else {
+    LFR_CUDA(cudaMemsetAsync(rsize, 0, 8, s));
+  }
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, noff, (int)NW + 1, s); }));
   image_size_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(img_s, img_ptr, noff, d_name_off, d_fact, n_present, NI, body, isize);
   LFR_LAUNCHED();
   LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)NI + 1, s); }));
@@ -2010,7 +2066,7 @@ int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t
   LFR_TRY(pl->enc_out.reserve(total));
   uint8_t* d_out = pl->enc_out.as<uint8_t>();
   write_images_kernel<<<blocks_for(NI), 256, 0, s>>>(img_s, body, ioff, d_names, d_name_off, d_fact, n_present, d_out);
-  write_records_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, img_ptr, noff, ioff, N, d_out);
+  if (NW) write_records_kernel<<<blocks_for(NW), 256, 0, s>>>(perm, key_s, nfeat, pos, img_ptr, noff, ioff, NW, d_out);
   LFR_LAUNCHED();
   LFR_CUDA(cudaStreamSynchronize(s));
   g_encode_ms[0] = ms_since(t0);
@@ -2199,7 +2255,17 @@ int join_solution(lfr_plan* pl, cudaStream_t s, const lfr::join::Decoded& d, uin
       return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, idx, idx_s, (int)D, 0, 64, s);
     }));
   }
-  lfr::start::join_kernel<<<blocks_for(N), 256, 0, s>>>(pl->node_image.as<uint32_t>(), pl->node_feat.as<uint32_t>(), N,
+  // image ids that share a name join through the lowest of them (lfr_join.h): the nodes keyed by that id
+  const uint32_t* node_image = pl->node_image.as<uint32_t>();
+  TmpBuf d_canon, d_nkey;
+  if (!d.canon.empty()) {
+    LFR_TRY(upload(&d_canon, d.canon.data(), d.canon.size(), s));
+    LFR_TRY(d_nkey.reserve(4 * (size_t)N));
+    lfr::graph::gather_kernel<<<blocks_for(N), 256, 0, s>>>(node_image, d_canon.as<uint32_t>(), N, d_nkey.as<uint32_t>());
+    LFR_LAUNCHED();
+    node_image = d_nkey.as<uint32_t>();
+  }
+  lfr::start::join_kernel<<<blocks_for(N), 256, 0, s>>>(node_image, pl->node_feat.as<uint32_t>(), N,
                                                           key_s, idx_s, D, di, dj, pl->pos_init.as<double>(),
                                                           pl->pos.as<double>(), ctr, has_entry);
   LFR_LAUNCHED();
@@ -2294,7 +2360,7 @@ int64_t encode_solution_carried(lfr_plan* pl, cudaStream_t s, uint32_t NI, const
   // the present scene images and their ranks, as lfr_plan_encode_solution() ranks them
   if (NI) {
     lfr::solution::init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
-    if (N) lfr::solution::first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside);
+    if (N) lfr::solution::first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside, nullptr);
     LFR_LAUNCHED();
     LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {
       return cub::DeviceRadixSort::SortPairs(t, nb, first, first_s, iota_i, img_s, (int)NI, 0, bits_for(N), s);
@@ -2666,6 +2732,20 @@ int64_t lfr_plan_encode_solution(lfr_plan* pl, void* stream, uint32_t n_images, 
   if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
   LFR_CUDA(cudaSetDevice(pl->device));
   return encode_solution(pl, (cudaStream_t)stream, n_images, names, name_off, fact, out, cap, n_outside);
+}
+
+int64_t lfr_plan_encode_solution_images(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
+                                        const uint64_t* name_off, const float* fact, const uint8_t* written, uint8_t* out,
+                                        uint64_t cap, uint64_t* n_outside) {
+  if (!written) return fail(LFR_EINVAL, "written is NULL");
+  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
+  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
+  if (n_images && (!name_off || !fact)) return fail(LFR_EINVAL, "NULL image names or facts");
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
+  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  LFR_CUDA(cudaSetDevice(pl->device));
+  return encode_solution(pl, (cudaStream_t)stream, n_images, names, name_off, fact, out, cap, n_outside, written);
 }
 
 int lfr_plan_fix_images(lfr_plan* pl, const uint8_t* fixed_by_image_id, uint32_t n_images) {

@@ -49,6 +49,7 @@ struct Level {
   uint8_t* pside;            // [n_level_nodes]
   uint32_t stamp;            // two stamps per level: stamp (pieces), stamp + 1 (second BFS)
   uint64_t max_weight;
+  const uint32_t* node_cap;  // may be NULL: max_weight per node, the same for a sub-problem's nodes (sub-scenes)
   long long* side_w;         // [2 n_sub] node weight of each side
   uint32_t* side_min;        // [2 n_sub] lowest node of each side
   uint8_t* cont;             // [2 n_sub] 1: the side is cut again (over max_weight, not two nodes)
@@ -292,7 +293,7 @@ __global__ void __launch_bounds__(kThreads) cut_sub_kernel(Level L) {
   }
   __syncthreads();
   if (tid < 2) {
-    const bool over = sh.sw[tid] > L.max_weight;
+    const bool over = sh.sw[tid] > (L.node_cap ? (uint64_t)L.node_cap[nodes[0]] : L.max_weight);
     L.side_w[2 * k + tid] = (long long)sh.sw[tid];
     L.side_min[2 * k + tid] = sh.smin[tid];
     L.cont[2 * k + tid] = (sh.scnt[tid] && over && n != 2) ? 1 : 0;

@@ -205,9 +205,12 @@ inline void cut_release(CutWorkspace& W) {
 // nodes become singleton groups, solve.cc:240-246).  The 2-way cut itself is lfr_cut.h.
 // One step: cut `edges`, emit the finished groups, return the edge lists of the two sides that
 // have to be cut again (empty when done).  A pure function of `edges` (in their order).
+// `cap_of_node` (may be NULL): a per-node max_weight in place of `max_weight`; every node of one meta-component
+// must have the same cap (the image count of its sub-scene, lfr_host_input::image_group).
 inline void cut_step(const std::vector<CutEdge>& edges, const std::vector<uint32_t>& node_weight, uint32_t max_weight,
               CutWorkspace& W, std::vector<uint8_t>& covered, std::vector<std::vector<uint32_t>>* groups,
-              std::vector<CutEdge> (&sub)[2]) {
+              std::vector<CutEdge> (&sub)[2], const uint32_t* cap_of_node = nullptr) {
+  if (cap_of_node) max_weight = cap_of_node[edges[0].a];
   // a third of all sub-problems are two tracks joined by (parallel) edges: whatever their weights, each
   // side of the cut is one node with no edge inside — two singleton groups (solve.cc:205-211 / :240-246)
   {
@@ -258,7 +261,8 @@ inline void cut_step(const std::vector<CutEdge>& edges, const std::vector<uint32
 // depend on the order in which the sub-problems are processed (each cut is a function of its own edge
 // list only), so the work list is shared by a few threads; only membership is used afterwards.
 inline void recursive_cut_all(std::vector<std::vector<CutEdge>> roots, const std::vector<uint32_t>& node_weight,
-                       uint32_t max_weight, std::vector<std::vector<uint32_t>>* groups) {
+                       uint32_t max_weight, std::vector<std::vector<uint32_t>>* groups,
+                       const uint32_t* cap_of_node = nullptr) {
   uint64_t total_edges = 0;
   for (const auto& r : roots) total_edges += r.size();
   unsigned n_thr = 1;
@@ -276,7 +280,7 @@ inline void recursive_cut_all(std::vector<std::vector<CutEdge>> roots, const std
     while (!work.empty()) {
       const std::vector<CutEdge> edges = std::move(work.back());
       work.pop_back();
-      cut_step(edges, node_weight, max_weight, W, covered, groups, sub);
+      cut_step(edges, node_weight, max_weight, W, covered, groups, sub, cap_of_node);
       if (!sub[1].empty()) work.push_back(std::move(sub[1]));
       if (!sub[0].empty()) work.push_back(std::move(sub[0]));
     }
@@ -305,7 +309,7 @@ inline void recursive_cut_all(std::vector<std::vector<CutEdge>> roots, const std
       while (!mine.empty()) {
         const std::vector<CutEdge> edges = std::move(mine.back());
         mine.pop_back();
-        cut_step(edges, node_weight, max_weight, W, covered, &found[t], sub);
+        cut_step(edges, node_weight, max_weight, W, covered, &found[t], sub, cap_of_node);
         for (int sd = 1; sd >= 0; --sd) {
           if (sub[sd].empty()) continue;
           if (sub[sd].size() >= kShare) {

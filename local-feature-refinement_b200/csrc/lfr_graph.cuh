@@ -458,9 +458,11 @@ __global__ void cc_weight_kernel(const uint32_t* cc, const uint32_t* nodes_in_tr
   if (t < T) atomicAdd(&cc_nodes[cc[t]], (unsigned long long)nodes_in_track[t]);
 }
 
-__global__ void oversized_kernel(const unsigned long long* cc_nodes, uint32_t n_cc, uint32_t max_nodes, uint32_t* big) {
+// cap (may be NULL: max_nodes for all): the cut cap of each meta-component (sub-scenes, lfr_host_input::image_group)
+__global__ void oversized_kernel(const unsigned long long* cc_nodes, uint32_t n_cc, uint32_t max_nodes, const uint32_t* cap,
+                                 uint32_t* big) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < n_cc) big[c] = cc_nodes[c] > max_nodes ? 1u : 0u;
+  if (c < n_cc) big[c] = cc_nodes[c] > (cap ? cap[c] : max_nodes) ? 1u : 0u;
 }
 
 // undirected meta-edges (ma < mb) of oversized components, weight int(100 * sum) (solve.cc:327-330)
@@ -486,6 +488,14 @@ __global__ void cut_edges_gather_kernel(const uint32_t* idx, uint32_t n, const u
 __global__ void scatter_kernel(const uint32_t* idx, const uint32_t* val, uint32_t n, uint32_t* dst) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[idx[i]] = val[i];
+}
+
+// sub-scenes: cc_cap[meta-component of node v] = the image count of v's sub-scene (every node of a
+// meta-component writes the same value)
+__global__ void cc_cap_kernel(const uint32_t* node_image, const uint32_t* track, const uint32_t* cc, const uint32_t* image_cap,
+                              uint32_t n, uint32_t* cc_cap) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v < n) cc_cap[cc[track[v]]] = image_cap[node_image[v]];
 }
 
 __global__ void gather_kernel(const uint32_t* idx, const uint32_t* src, uint32_t n, uint32_t* dst) {

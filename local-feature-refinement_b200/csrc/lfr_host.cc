@@ -196,6 +196,17 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
   std::vector<uint64_t> kept_matches;  // indices of matches of non-skipped pairs, in order
   std::vector<uint32_t> m_img1, m_img2;
   std::vector<uint8_t> seen_img(in->n_images, 0);
+  // sub-scenes (image_group): each image's index inside its sub-scene, the width of a union-find image set
+  const uint32_t* group = in->image_group;
+  std::vector<uint32_t> local_image(group ? in->n_images : 0);
+  uint32_t set_width = in->n_images;
+  uint32_t n_groups = 0;
+  if (group) {
+    for (uint32_t i = 0; i < in->n_images; ++i) n_groups = std::max(n_groups, group[i] + 1);
+    std::vector<uint32_t> n_in_group(n_groups, 0);
+    for (uint32_t i = 0; i < in->n_images; ++i) local_image[i] = n_in_group[group[i]]++;
+    set_width = n_groups ? *std::max_element(n_in_group.begin(), n_in_group.end()) : 0;
+  }
   {
     uint64_t n_kept = 0;
     for (uint64_t p = 0; p < in->n_pairs; ++p)
@@ -212,6 +223,10 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
       delete hs;
       return LFR_EINVAL;
     }
+    if (group && group[in->pair_img1[p]] != group[in->pair_img2[p]]) {  // a pair spans two sub-scenes
+      delete hs;
+      return LFR_EINVAL;
+    }
     seen_img[in->pair_img1[p]] = 1;
     seen_img[in->pair_img2[p]] = 1;
     for (uint64_t m = in->pair_ptr[p]; m < in->pair_ptr[p + 1]; ++m) {
@@ -225,6 +240,8 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
     }
   }
   for (uint8_t v : seen_img) S.n_images_seen += v;
+  std::vector<uint32_t> group_seen(n_groups, 0);  // solve.cc:448-451's images_set.size() of each sub-scene
+  for (uint32_t i = 0; group && i < in->n_images; ++i) group_seen[group[i]] += seen_img[i];
   const double t_g0 = ms_since(t_graph);
   const uint64_t M = kept_matches.size();
   std::vector<uint32_t> n1(M), n2(M);
@@ -365,20 +382,22 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
     delete hs;
     return LFR_EUNSUPPORTED;
   }
-  const bool small_sets = in->n_images <= 64;  // image set of a union-find root as one 64-bit mask
+  // the image of node v as the sets below index it: inside its sub-scene (a union never spans two)
+  auto set_image = [&](uint32_t v) -> uint32_t { return group ? local_image[hs->node_image[v]] : hs->node_image[v]; };
+  const bool small_sets = set_width <= 64;  // image set of a union-find root as one 64-bit mask
   std::vector<uint64_t> mask(small_sets ? N : 0);
   // more than 64 images: a root's image set is {its own image} while it is a singleton (no storage),
-  // a short sorted list up to kListMax entries, then a bitset of n_images bits from a pool
-  const uint32_t W = (in->n_images + 63) / 64;
+  // a short sorted list up to kListMax entries, then a bitset of set_width bits from a pool
+  const uint32_t W = (set_width + 63) / 64;
   constexpr uint32_t kListMax = 12;
   std::vector<uint16_t> lists;                               // kListMax entries per slot
   std::vector<uint64_t> bitsets;                             // W words per slot
   std::vector<int32_t> free_lists;
   if (small_sets)
-    for (uint32_t v = 0; v < N; ++v) mask[v] = 1ull << hs->node_image[v];
+    for (uint32_t v = 0; v < N; ++v) mask[v] = 1ull << set_image(v);
   auto set_has = [&](uint32_t r, uint16_t img) -> bool {
     const uint32_t sz = uf[r].size;
-    if (sz == 1) return (uint16_t)hs->node_image[r] == img;
+    if (sz == 1) return (uint16_t)set_image(r) == img;
     if (sz <= kListMax) {
       const uint16_t* l = &lists[(size_t)uf[r].slot * kListMax];
       for (uint32_t i = 0; i < sz; ++i)
@@ -391,7 +410,7 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
   auto for_each_image = [&](uint32_t r, auto&& fn) {
     const uint32_t sz = uf[r].size;
     if (sz == 1) {
-      fn((uint16_t)hs->node_image[r]);
+      fn((uint16_t)set_image(r));
     } else if (sz <= kListMax) {
       const uint16_t* l = &lists[(size_t)uf[r].slot * kListMax];
       for (uint32_t i = 0; i < sz; ++i) fn(l[i]);
@@ -426,7 +445,7 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
           sl = (int32_t)(lists.size() / kListMax);
           lists.resize(lists.size() + kListMax);
         }
-        lists[(size_t)sl * kListMax] = (uint16_t)hs->node_image[dst];
+        lists[(size_t)sl * kListMax] = (uint16_t)set_image(dst);
         uf[dst].slot = sl;
       }
       uint16_t* l = &lists[(size_t)uf[dst].slot * kListMax];
@@ -601,10 +620,16 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
   std::vector<uint32_t> gc(cc);
   uint32_t next_label = n_cc;
   const uint32_t max_nodes = S.n_images_seen;
+  // with sub-scenes, the cap of a meta-component (and of each of its tracks) is its sub-scene's image count
+  std::vector<uint32_t> cc_cap(group ? n_cc : 0), track_cap(group ? T : 0);
+  if (group) {
+    for (uint32_t v = 0; v < N; ++v) cc_cap[cc[hs->track[v]]] = group_seen[group[hs->node_image[v]]];
+    for (uint32_t t = 0; t < T; ++t) track_cap[t] = cc_cap[cc[t]];
+  }
   std::vector<std::vector<lfr::CutEdge>> per_cc;
   std::vector<int32_t> big_slot(n_cc, -1);
   for (uint32_t c = 0; c < n_cc; ++c)
-    if (cc_nodes[c] > max_nodes) {
+    if (cc_nodes[c] > (group ? cc_cap[c] : max_nodes)) {
       big_slot[c] = (int32_t)per_cc.size();
       per_cc.emplace_back();
     }
@@ -617,7 +642,7 @@ int lfr_host_stage_create(const lfr_host_input* in, lfr_host_stage** out, lfr_ho
       per_cc[s].push_back(lfr::CutEdge{ma[i], mb[i], lfr::cut_weight(wsum[i])});  // static_cast<int>(100 * it.second), solve.cc:329
     }
     std::vector<std::vector<uint32_t>> groups;
-    lfr::recursive_cut_all(std::move(per_cc), nodes_in_track, max_nodes, &groups);
+    lfr::recursive_cut_all(std::move(per_cc), nodes_in_track, max_nodes, &groups, group ? track_cap.data() : nullptr);
     for (const auto& g : groups) {  // labels only say "same group": their order is irrelevant
       for (uint32_t t : g) gc[t] = next_label;
       ++next_label;

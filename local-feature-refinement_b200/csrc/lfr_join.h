@@ -9,7 +9,9 @@
 // Image message is matched to a scene image by its exact name bytes, and the last Image message with a
 // given name wins as a whole; within it, the last displacement of a feature wins.  Each displacement of a
 // winning message gets the key (image id << 32 | feature_idx), as the encoder keys its nodes; every other
-// displacement gets kNoKey, which no node has (image ids are < 2^32 - 1).
+// displacement gets kNoKey, which no node has (image ids are < 2^32 - 1).  Scene image ids that share a name
+// (--query_images gives a database image one id per sub-scene) all join the entries of that name: a node of
+// image k is keyed with the lowest id of k's name (Decoded::canon).
 #ifndef LFR_JOIN_H_
 #define LFR_JOIN_H_
 
@@ -42,6 +44,9 @@ struct Decoded {
   // per decoded Image message: 1 when it is the last one with its name (it wins as a whole), whether or not
   // the name is a scene image's
   std::vector<uint8_t> wins;
+  // per scene image id: the lowest id with the same name, the image whose entries it joins; empty when every
+  // scene name is distinct (then each id is its own)
+  std::vector<uint32_t> canon;
 };
 
 // Decode `buf` and resolve its images against the scene's names (name k = names[name_off[k], name_off[k+1])).
@@ -64,8 +69,16 @@ inline int decode(const uint8_t* buf, uint64_t len, uint32_t n_images, const uin
     return LFR_EINVAL;
   std::unordered_map<std::string, uint32_t> id_of;
   id_of.reserve(n_images);
-  for (uint32_t k = 0; k < n_images; ++k)
-    id_of.emplace(std::string(reinterpret_cast<const char*>(names) + name_off[k], name_off[k + 1] - name_off[k]), k);
+  d.canon.clear();
+  for (uint32_t k = 0; k < n_images; ++k) {
+    const auto it =
+        id_of.emplace(std::string(reinterpret_cast<const char*>(names) + name_off[k], name_off[k + 1] - name_off[k]), k);
+    if (!it.second && d.canon.empty()) {
+      d.canon.resize(n_images);
+      for (uint32_t j = 0; j < n_images; ++j) d.canon[j] = j;
+    }
+    if (!d.canon.empty()) d.canon[k] = it.first->second;
+  }
   std::unordered_map<std::string, uint64_t> last;  // the last Image message of each name in the file
   last.reserve(I);
   for (uint64_t i = 0; i < I; ++i)
@@ -115,7 +128,7 @@ inline int join_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const
   std::stable_sort(keyed.begin(), keyed.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
   uint64_t started = 0;
   for (uint32_t v = 0; v < n_nodes; ++v) {
-    const uint64_t key = node_key(node_image[v], node_feat[v]);
+    const uint64_t key = node_key(d.canon.empty() ? node_image[v] : d.canon[node_image[v]], node_feat[v]);
     const auto it = std::upper_bound(keyed.begin(), keyed.end(), key,
                                      [](uint64_t x, const std::pair<uint64_t, uint64_t>& e) { return x < e.first; });
     double a = 0.0, b = 0.0;

@@ -11,6 +11,8 @@
 //   (exclusive scan of the record sizes -> node_off)
 //   image_size_kernel   body and record size of each image  (exclusive scan -> img_off; img_off[end] = total)
 //   write_images_kernel / write_records_kernel   the bytes, one thread per image / per node
+// With `written` (lfr_plan_encode_solution_images, --query_images) an image without the flag is absent: its
+// nodes count towards "> 0.5" but sort after every written node and get no record.
 #pragma once
 
 #include <cstdint>
@@ -73,7 +75,7 @@ __global__ void init_images_kernel(uint32_t* first, uint32_t* iota, uint32_t n_i
 // first[img] = min node index over the image's nodes (one atomic per run of equal images in a warp, from
 // its lowest lane, which holds the run's lowest node); *n_outside += |pos| > 0.5 on either coordinate
 __global__ void first_node_kernel(const uint32_t* node_image, const double* pos, uint32_t n, uint32_t* first,
-                                  unsigned long long* n_outside) {
+                                  unsigned long long* n_outside, const uint8_t* written) {
   const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
   const bool live = v < n;
   const unsigned mask = __ballot_sync(0xffffffffu, live);
@@ -81,7 +83,7 @@ __global__ void first_node_kernel(const uint32_t* node_image, const double* pos,
   if (live) {
     const uint32_t img = node_image[v];
     const unsigned peers = __match_any_sync(mask, img);
-    if ((threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) atomicMin(first + img, v);
+    if ((threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1) && (!written || written[img])) atomicMin(first + img, v);
     outside = fabs(pos[2 * (size_t)v + 1]) > 0.5 || fabs(pos[2 * (size_t)v]) > 0.5;  // solve.cc:666-669
   }
   const int c = __syncthreads_count(outside);
@@ -97,12 +99,22 @@ __global__ void rank_kernel(const uint32_t* first_sorted, const uint32_t* img_so
   if (r + 1 == n_images || first_sorted[r + 1] >= n_nodes) *n_present = r + 1;
 }
 
+// key[v] = rank of v's image, or n_images (after every written image) for a node of an absent image;
+// *n_written (with `written`) = the nodes of written images
 __global__ void node_key_kernel(const uint32_t* node_image, const uint32_t* rank, uint32_t n, uint32_t* key,
-                                uint32_t* iota) {
+                                uint32_t* iota, const uint8_t* written, uint32_t n_images, uint32_t* n_written) {
   const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n) return;
-  key[v] = rank[node_image[v]];
-  iota[v] = v;
+  bool w = false;
+  if (v < n) {
+    const uint32_t img = node_image[v];
+    w = !written || written[img];
+    key[v] = w ? rank[img] : n_images;
+    iota[v] = v;
+  }
+  if (written) {
+    const int c = __syncthreads_count(w);
+    if (threadIdx.x == 0 && c) atomicAdd(n_written, (uint32_t)c);
+  }
 }
 
 // output slot k holds node perm[k] of the image of rank key_sorted[k]: its record's size (tag, 1-byte length —

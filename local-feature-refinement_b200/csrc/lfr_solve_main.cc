@@ -35,7 +35,10 @@
 // the SolutionFile, this run's problem record: lfr_plan_problem_record() on the device route,
 // lfr_host_problem_record() on the host route, the same bytes) and --earlier_record_file FILE (with
 // --update_initial_solution, in place of --previous_matches_file: the record the earlier run wrote;
-// lfr_plan_update_solution_since_record() / lfr_wire_update_solution_since_record()).  `--n_threads` is accepted and
+// lfr_plan_update_solution_since_record() / lfr_wire_update_solution_since_record()) and --query_images NAME
+// (repeatable: each query's pairs become a sub-scene with its own ids for the database images, the graph stage
+// takes the sub-scene of every id, lfr_host_input::image_group, and only query images are written:
+// lfr_plan_encode_solution_images() on the device route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -93,6 +96,9 @@ int lfr_plan_update_solution_since_record(lfr_plan* plan, void* stream, const ui
                                           uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
                                           const uint8_t* record, uint64_t record_len, uint64_t* n_held,
                                           uint32_t* n_touched, uint32_t* n_changed) __attribute__((weak));
+int64_t lfr_plan_encode_solution_images(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                        const uint64_t* name_off, const float* fact, const uint8_t* written, uint8_t* out,
+                                        uint64_t cap, uint64_t* n_outside) __attribute__((weak));
 int64_t lfr_plan_encode_solution_carried(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
                                          const uint64_t* name_off, const float* fact, const uint8_t* file,
                                          uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
@@ -123,7 +129,8 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"gpus", true, false},         {"fixed_images", true, true},  {"initial_solution", true, false},
                                {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false},
                                {"update_initial_solution", false, false}, {"previous_matches_file", true, false},
-                               {"record_file", true, false},  {"earlier_record_file", true, false}};
+                               {"record_file", true, false},  {"earlier_record_file", true, false},
+                               {"query_images", true, true}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -336,10 +343,10 @@ long long ms_between(Clock::time_point a, Clock::time_point b) {
 
 int main(int argc, char** argv) {
   std::string matches_file, output_file, initial_solution, previous_matches_file, record_file, earlier_record_file;
-  std::vector<std::string> banned_list, fixed_list;
+  std::vector<std::string> banned_list, fixed_list, query_list;
   uint64_t device = 0, gpus = 1;
   bool keep_start = false, carry_start = false, update_start = false, have_previous = false, have_record = false,
-       have_earlier = false;
+       have_earlier = false, have_query = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -356,6 +363,8 @@ int main(int argc, char** argv) {
     gpus = as_uint(a, "gpus", 1);
     banned_list = a.repeated["banned_images"];
     fixed_list = a.repeated["fixed_images"];
+    have_query = a.repeated.count("query_images") != 0;
+    query_list = a.repeated["query_images"];
     if (a.single.count("initial_solution")) initial_solution = a.single.at("initial_solution");
     keep_start = a.keep_initial_solution;
     carry_start = a.carry_initial_solution;
@@ -402,6 +411,16 @@ int main(int argc, char** argv) {
   if (have_earlier && have_previous) {
     std::fputs("ERROR: --earlier_record_file and --previous_matches_file exclude each other\n", stderr);
     return 2;
+  }
+  if (have_query) {  // each query is refined against the scene as it stands; the incremental modes update one scene
+    for (const auto& o : {std::make_pair(update_start, "--update_initial_solution"),
+                          std::make_pair(have_previous, "--previous_matches_file"), std::make_pair(have_record, "--record_file"),
+                          std::make_pair(have_earlier, "--earlier_record_file"),
+                          std::make_pair(carry_start, "--carry_initial_solution")})
+      if (o.first) {
+        std::fprintf(stderr, "ERROR: --query_images and %s exclude each other\n", o.second);
+        return 2;
+      }
   }
   if (have_start) {
     if (!start_file.open(initial_solution)) {
@@ -518,14 +537,61 @@ int main(int argc, char** argv) {
     }
   }
 
-  // banned images (solve.cc:444-446) and the first fact seen of every image among the pairs kept
+  // banned images (solve.cc:444-446)
   const std::set<std::string> banned(banned_list.begin(), banned_list.end());
   std::vector<uint8_t> skip(P, 0);
-  std::vector<float> image_fact(names.size(), 0.f);
-  std::vector<uint8_t> have_fact(names.size(), 0);
+  for (uint64_t p = 0; p < P; ++p)
+    skip[p] = (banned.count(names[pair_img1[p]]) || banned.count(names[pair_img2[p]])) ? 1 : 0;
+
+  // --query_images: a kept pair that names one query image belongs to that query's sub-scene, and its images
+  // get that sub-scene's ids, in order of first appearance; a pair that names none is not solved.  The graph
+  // stage then gives every sub-scene what a run on its pairs alone gives (lfr_host_input::image_group).
+  // orig_of: the original image id (and name) of every stage image id; the identity without queries.
+  std::vector<uint8_t> is_query(names.size(), 0);
+  std::vector<uint32_t> orig_of, image_group;
+  if (have_query) {
+    const std::set<std::string> queries(query_list.begin(), query_list.end());
+    for (size_t i = 0; i < names.size(); ++i) is_query[i] = queries.count(names[i]) ? 1 : 0;
+    std::map<std::pair<uint32_t, uint32_t>, uint32_t> sub_id;  // (query image, image) -> stage image id
+    auto sub = [&](uint32_t q, uint32_t img) {
+      const auto it = sub_id.emplace(std::make_pair(q, img), (uint32_t)orig_of.size());
+      if (it.second) {
+        orig_of.push_back(img);
+        image_group.push_back(q);
+      }
+      return it.first->second;
+    };
+    for (uint64_t p = 0; p < P; ++p) {
+      const uint32_t a = pair_img1[p], b = pair_img2[p];
+      if (!skip[p] && is_query[a] && is_query[b]) {
+        std::fprintf(stderr, "ERROR: the pair '%s' - '%s' names two query images\n", names[a].c_str(), names[b].c_str());
+        return 2;
+      }
+      if (skip[p] || !(is_query[a] || is_query[b])) {
+        skip[p] = 1;
+        pair_img1[p] = pair_img2[p] = 0;  // never read: skipped pairs name no image of the stage
+        continue;
+      }
+      const uint32_t q = is_query[a] ? a : b;
+      pair_img1[p] = sub(q, a);
+      pair_img2[p] = sub(q, b);
+    }
+    if (orig_of.size() > 65535) {
+      std::fprintf(stderr, "ERROR: --query_images: the sub-scenes hold %zu images, more than 65535; split the query list "
+                           "over several runs\n", orig_of.size());
+      return 2;
+    }
+  } else {
+    orig_of.resize(names.size());
+    for (uint32_t i = 0; i < (uint32_t)names.size(); ++i) orig_of[i] = i;
+  }
+  const uint32_t n_ids = (uint32_t)orig_of.size();  // image ids of the graph stage's input
+
+  // the first fact seen of every image among the pairs kept
+  std::vector<float> image_fact(n_ids, 0.f);
+  std::vector<uint8_t> have_fact(n_ids, 0);
   uint64_t e_cap = 0;
   for (uint64_t p = 0; p < P; ++p) {
-    skip[p] = (banned.count(names[pair_img1[p]]) || banned.count(names[pair_img2[p]])) ? 1 : 0;
     if (skip[p]) continue;
     e_cap += 2 * (pair_ptr[p + 1] - pair_ptr[p]);
     if (!have_fact[pair_img1[p]]) { have_fact[pair_img1[p]] = 1; image_fact[pair_img1[p]] = pair_fact1[p]; }
@@ -533,27 +599,32 @@ int main(int argc, char** argv) {
   }
 
   // images held fixed (the same name semantics as banned images), and the names by image id as the
-  // start-point join and the encoder on the GPU take them
+  // start-point join and the encoder on the GPU take them (ids of the graph stage: with --query_images a
+  // database image's name repeats once per sub-scene, and the joins give every copy the same entries)
   const std::set<std::string> fixed_names(fixed_list.begin(), fixed_list.end());
-  std::vector<uint8_t> fixed(names.size(), 0);
+  std::vector<uint8_t> fixed(n_ids, 0), image_written(n_ids, 0);
   bool any_fixed = false;
-  for (size_t i = 0; i < names.size(); ++i)
-    if (fixed_names.count(names[i])) {
+  for (uint32_t i = 0; i < n_ids; ++i) {
+    image_written[i] = !have_query || is_query[orig_of[i]];
+    if (fixed_names.count(names[orig_of[i]])) {
       fixed[i] = 1;
       any_fixed = true;
     }
+  }
   std::vector<uint8_t> name_blob;
-  std::vector<uint64_t> name_off(names.size() + 1, 0);
-  for (size_t i = 0; i < names.size(); ++i) {
-    name_blob.insert(name_blob.end(), names[i].begin(), names[i].end());
+  std::vector<uint64_t> name_off(n_ids + 1, 0);
+  for (uint32_t i = 0; i < n_ids; ++i) {
+    const std::string& nm = names[orig_of[i]];
+    name_blob.insert(name_blob.end(), nm.begin(), nm.end());
     name_off[i + 1] = name_blob.size();
   }
 
   lfr_host_input in;
   std::memset(&in, 0, sizeof in);
-  in.n_pairs = P; in.n_matches = M; in.n_images = (uint32_t)names.size();
+  in.n_pairs = P; in.n_matches = M; in.n_images = n_ids;
   in.pair_img1 = pair_img1.data(); in.pair_img2 = pair_img2.data(); in.pair_skip = skip.data();
   in.pair_ptr = pair_ptr.data();
+  in.image_group = have_query ? image_group.data() : nullptr;
 
   // ---- which graph stage: the library's size rule, or LFR_GRAPH_STAGE=host|device (a test and
   // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
@@ -562,7 +633,7 @@ int main(int argc, char** argv) {
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
                                  lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
                                  lfr_plan_update_solution && lfr_plan_update_solution_since && lfr_plan_problem_record &&
-                                 lfr_plan_update_solution_since_record;
+                                 lfr_plan_update_solution_since_record && lfr_plan_encode_solution_images;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -642,9 +713,9 @@ int main(int argc, char** argv) {
       return 2;
     }
     // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
-    int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), (uint32_t)names.size()) : LFR_OK;
+    int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), n_ids) : LFR_OK;
     if (rc2 == LFR_OK && have_earlier) {
-      rc2 = lfr_plan_update_solution_since_record(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
+      rc2 = lfr_plan_update_solution_since_record(plan, nullptr, start_file.data(), start_file.size(), n_ids,
                                                   name_blob.data(), name_off.data(), earlier_record.data(),
                                                   earlier_record.size(), nullptr, nullptr, nullptr);
     } else if (rc2 == LFR_OK && have_previous) {
@@ -653,16 +724,16 @@ int main(int argc, char** argv) {
       lfr_plan* prev_plan = nullptr;
       rc2 = lfr_plan_create_from_matches(&pin, &opt, nullptr, &prev_plan, nullptr);
       if (rc2 == LFR_OK)
-        rc2 = lfr_plan_update_solution_since(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
+        rc2 = lfr_plan_update_solution_since(plan, nullptr, start_file.data(), start_file.size(), n_ids,
                                              name_blob.data(), name_off.data(), prev_plan, (uint32_t)previous.names.size(),
                                              previous.name_blob.data(), previous.name_off.data(), nullptr, nullptr, nullptr);
       lfr_plan_destroy(prev_plan);
     } else if (rc2 == LFR_OK && have_start && update_start)
-      rc2 = lfr_plan_update_solution(plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(),
+      rc2 = lfr_plan_update_solution(plan, nullptr, start_file.data(), start_file.size(), n_ids,
                                      name_blob.data(), name_off.data(), nullptr, nullptr);
     else if (rc2 == LFR_OK && have_start)
       rc2 = (keep_start ? lfr_plan_keep_solution : lfr_plan_start_from_solution)(
-          plan, nullptr, start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(), name_off.data(), nullptr);
+          plan, nullptr, start_file.data(), start_file.size(), n_ids, name_blob.data(), name_off.data(), nullptr);
     if (rc2 != LFR_OK) {
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc2, lfr_last_error());
       return 2;
@@ -726,7 +797,7 @@ int main(int argc, char** argv) {
     std::vector<uint8_t> has_entry(keep_start || update_start ? N : 0, 0);
     if (have_earlier) {
       const lfr_problem cur = host_problem();
-      if (lfr_wire_update_solution_since_record(start_file.data(), start_file.size(), (uint32_t)names.size(),
+      if (lfr_wire_update_solution_since_record(start_file.data(), start_file.size(), n_ids,
                                                 name_blob.data(), name_off.data(), &cur, node_image.data(), node_feat.data(),
                                                 earlier_record.data(), earlier_record.size(), positions, has_entry.data(),
                                                 nullptr, nullptr, nullptr) != LFR_OK) {
@@ -736,7 +807,7 @@ int main(int argc, char** argv) {
     } else if (have_previous) {
       const lfr_problem cur = host_problem();
       const lfr_host_input pin = previous.input();
-      if (lfr_wire_update_solution_since(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
+      if (lfr_wire_update_solution_since(start_file.data(), start_file.size(), n_ids, name_blob.data(),
                                          name_off.data(), &cur, node_image.data(), node_feat.data(), &pin,
                                          previous.name_blob.data(), previous.name_off.data(), positions, has_entry.data(),
                                          nullptr, nullptr, nullptr) != LFR_OK) {
@@ -744,16 +815,16 @@ int main(int argc, char** argv) {
         return 2;
       }
     } else if (have_start && update_start) {
-      if (lfr_wire_update_solution(start_file.data(), start_file.size(), (uint32_t)names.size(), name_blob.data(),
+      if (lfr_wire_update_solution(start_file.data(), start_file.size(), n_ids, name_blob.data(),
                                    name_off.data(), N, node_image.data(), node_feat.data(), comp.data(), C, positions,
                                    has_entry.data(), nullptr, nullptr) != LFR_OK) {
         std::fprintf(stderr, "ERROR: lfr_wire_update_solution failed\n");
         return 2;
       }
-    } else if (have_start && (keep_start ? lfr_wire_join_solution_entries(start_file.data(), start_file.size(), (uint32_t)names.size(),
+    } else if (have_start && (keep_start ? lfr_wire_join_solution_entries(start_file.data(), start_file.size(), n_ids,
                                                                   name_blob.data(), name_off.data(), N, node_image.data(),
                                                                   node_feat.data(), positions, nullptr, has_entry.data())
-                                  : lfr_wire_join_solution(start_file.data(), start_file.size(), (uint32_t)names.size(),
+                                  : lfr_wire_join_solution(start_file.data(), start_file.size(), n_ids,
                                                            name_blob.data(), name_off.data(), N, node_image.data(),
                                                            node_feat.data(), positions, nullptr)) != LFR_OK) {
       std::fprintf(stderr, "ERROR: lfr_wire_join_solution failed\n");
@@ -806,19 +877,19 @@ int main(int argc, char** argv) {
   if (have_record) {
     int64_t got = -1;
     if (plan) {
-      const int64_t need_r = lfr_plan_problem_record(plan, nullptr, (uint32_t)names.size(), name_blob.data(),
+      const int64_t need_r = lfr_plan_problem_record(plan, nullptr, n_ids, name_blob.data(),
                                                      name_off.data(), nullptr, 0);
       record_out.resize(need_r > 0 ? (size_t)need_r : 0);
       got = need_r < 0 ? need_r
-                       : lfr_plan_problem_record(plan, nullptr, (uint32_t)names.size(), name_blob.data(), name_off.data(),
+                       : lfr_plan_problem_record(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
                                                  record_out.data(), record_out.size());
     } else {
       const lfr_problem cur = host_problem();
-      const int64_t need_r = lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), (uint32_t)names.size(),
+      const int64_t need_r = lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), n_ids,
                                                      name_blob.data(), name_off.data(), nullptr, 0);
       record_out.resize(need_r > 0 ? (size_t)need_r : 0);
       got = need_r < 0 ? need_r
-                       : lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), (uint32_t)names.size(),
+                       : lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), n_ids,
                                                  name_blob.data(), name_off.data(), record_out.data(), record_out.size());
     }
     if (got < 0 || (uint64_t)got != record_out.size()) {
@@ -836,14 +907,16 @@ int main(int argc, char** argv) {
     // encoded on the GPU, names and facts indexed by image id, into page-locked memory sized by the
     // largest encoding: a Displacement record is at most 18 bytes, an Image's header 16 plus its name field
     uint64_t cap = 18ull * N;
-    for (size_t i = 0; i < names.size(); ++i) cap += 16 + 11 + names[i].size();
+    cap += 27ull * n_ids + name_blob.size();
     // carried entries: a file's canonical encoding bounds what it adds; a larger need takes a second call
     if (carry_start) cap += start_file.size();
     auto encode = [&](uint8_t* o, uint64_t c) {
-      return carry_start ? lfr_plan_encode_solution_carried(plan, nullptr, (uint32_t)names.size(), name_blob.data(),
+      return carry_start ? lfr_plan_encode_solution_carried(plan, nullptr, n_ids, name_blob.data(),
                                                             name_off.data(), image_fact.data(), start_file.data(),
                                                             start_file.size(), o, c, &n_outside, nullptr)
-                         : lfr_plan_encode_solution(plan, nullptr, (uint32_t)names.size(), name_blob.data(), name_off.data(),
+                         : have_query ? lfr_plan_encode_solution_images(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
+                                                                        image_fact.data(), image_written.data(), o, c, &n_outside)
+                         : lfr_plan_encode_solution(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
                                                     image_fact.data(), o, c, &n_outside);
     };
     out = static_cast<uint8_t*>(lfr_host_alloc(cap));
@@ -864,34 +937,42 @@ int main(int argc, char** argv) {
       return 2;
     }
   } else {
-    std::vector<int64_t> rank(names.size(), -1);
+    // with --query_images only the query images are written (a database image's keypoints have one value
+    // per query): rank -2 marks the images left out; every node still counts towards n_outside
+    std::vector<int64_t> rank(n_ids, -1);
     std::vector<uint32_t> img_ids;
     for (uint32_t v = 0; v < N; ++v)
-      if (rank[node_image[v]] < 0) {
+      if (rank[node_image[v]] == -1) {
+        if (!image_written[node_image[v]]) {
+          rank[node_image[v]] = -2;
+          continue;
+        }
         rank[node_image[v]] = (int64_t)img_ids.size();
         img_ids.push_back(node_image[v]);
       }
     const size_t I = img_ids.size();
     std::vector<uint64_t> img_ptr(I + 1, 0);
-    for (uint32_t v = 0; v < N; ++v) ++img_ptr[(size_t)rank[node_image[v]] + 1];
+    for (uint32_t v = 0; v < N; ++v)
+      if (rank[node_image[v]] >= 0) ++img_ptr[(size_t)rank[node_image[v]] + 1];
     for (size_t i = 0; i < I; ++i) img_ptr[i + 1] += img_ptr[i];
-    std::vector<uint32_t> feature_idx(N);
-    std::vector<float> di(N), dj(N);
+    std::vector<uint32_t> feature_idx(img_ptr[I]);
+    std::vector<float> di(img_ptr[I]), dj(img_ptr[I]);
     {
       std::vector<uint64_t> fill(img_ptr.begin(), img_ptr.end() - 1);
       for (uint32_t v = 0; v < N; ++v) {
+        if (std::fabs(positions[2 * (size_t)v + 1]) > 0.5 || std::fabs(positions[2 * (size_t)v]) > 0.5) ++n_outside;  // solve.cc:666-669
+        if (rank[node_image[v]] < 0) continue;
         const uint64_t k = fill[(size_t)rank[node_image[v]]]++;
         feature_idx[k] = node_feat[v];
         di[k] = (float)positions[2 * (size_t)v];
         dj[k] = (float)positions[2 * (size_t)v + 1];
-        if (std::fabs(positions[2 * (size_t)v + 1]) > 0.5 || std::fabs(positions[2 * (size_t)v]) > 0.5) ++n_outside;  // solve.cc:666-669
       }
     }
     std::vector<uint8_t> out_blob;
     std::vector<uint64_t> out_off(I + 1, 0);
     std::vector<float> fact(I);
     for (size_t i = 0; i < I; ++i) {
-      const std::string& s = names[img_ids[i]];
+      const std::string& s = names[orig_of[img_ids[i]]];
       out_blob.insert(out_blob.end(), s.begin(), s.end());
       out_off[i + 1] = out_blob.size();
       fact[i] = image_fact[img_ids[i]];

@@ -112,15 +112,17 @@ def build_graph(ms: MatchSet, banned_images=()) -> MatchGraph:
     )
 
 
-def compute_tracks(g: MatchGraph) -> np.ndarray:
+def compute_tracks(g: MatchGraph, set_image: Optional[np.ndarray] = None) -> np.ndarray:
     """H2 — maximum spanning forest with the "one node per image" constraint
-    (solve.cc:489-541).  Returns track_idx[N]."""
+    (solve.cc:489-541).  Returns track_idx[N].  `set_image` [n_images] (sub-scenes): the index the image
+    sets use for each image id, its index inside its sub-scene."""
     N = g.n_nodes
     # std::sort + std::reverse on (sim, n1, n2)  (solve.cc:489-490)
     order = np.lexsort((g.und_n2, g.und_n1, g.und_sim))[::-1]
     parent = [-1] * N
     # image set of each union-find root as a Python-int bitset
-    imgs = [1 << int(i) for i in g.node_image.tolist()]
+    key = g.node_image if set_image is None else np.asarray(set_image)[g.node_image]
+    imgs = [1 << int(i) for i in key.tolist()]
     size = [1] * N
     a1 = g.und_n1[order].tolist()
     a2 = g.und_n2[order].tolist()
@@ -328,8 +330,9 @@ def recursive_cut(edge_a, edge_b, edge_w, node_weight, max_weight) -> List[List[
 
 
 def separate_meta_graph(g: MatchGraph, track: np.ndarray, max_nodes: int,
-                        stats: Optional[dict] = None) -> np.ndarray:
-    """H4 — solve.cc:252-373.  Returns component_idx[N]."""
+                        stats: Optional[dict] = None, node_cap: Optional[np.ndarray] = None) -> np.ndarray:
+    """H4 — solve.cc:252-373.  Returns component_idx[N].  `node_cap` [N] (sub-scenes): the cut cap of each
+    node's meta-component in place of `max_nodes`, its sub-scene's image count."""
     N = g.n_nodes
     T = int(track.max()) + 1 if N else 0
     nodes_in_track = np.bincount(track, minlength=T)
@@ -347,7 +350,10 @@ def separate_meta_graph(g: MatchGraph, track: np.ndarray, max_nodes: int,
     cc_nodes = np.bincount(cc, weights=nodes_in_track, minlength=n_cc).astype(np.int64)
     gc = cc.copy()                 # gc_component_idx_container: start from the CC label
     next_label = n_cc
-    big = np.nonzero(cc_nodes > max_nodes)[0]
+    cap = np.full(n_cc, max_nodes, dtype=np.int64)
+    if node_cap is not None:
+        cap[cc[track]] = node_cap
+    big = np.nonzero(cc_nodes > cap)[0]
     n_cut_groups = 0
     if big.shape[0]:
         und = ma < mb              # undirected edge list, weight int(100 * sum sim) (solve.cc:327-330)
@@ -357,7 +363,7 @@ def separate_meta_graph(g: MatchGraph, track: np.ndarray, max_nodes: int,
         nw = nodes_in_track.tolist()
         for c in big.tolist():
             sel = ucc == c
-            groups = recursive_cut(ua[sel].tolist(), ub[sel].tolist(), uw[sel].tolist(), nw, max_nodes)
+            groups = recursive_cut(ua[sel].tolist(), ub[sel].tolist(), uw[sel].tolist(), nw, int(cap[c]))
             for grp in groups:
                 gc[np.array(grp, dtype=np.int64)] = next_label
                 next_label += 1
@@ -396,7 +402,7 @@ class HostInput(C.Structure):
                 ("pair_img1", C.c_void_p), ("pair_img2", C.c_void_p), ("pair_skip", C.c_void_p),
                 ("pair_ptr", C.c_void_p), ("feat1", C.c_void_p), ("feat2", C.c_void_p), ("sim", C.c_void_p),
                 ("disp1", C.c_void_p), ("disp2", C.c_void_p), ("edges_out", C.c_void_p),
-                ("edges_out_capacity", C.c_uint64)]
+                ("edges_out_capacity", C.c_uint64), ("image_group", C.c_void_p)]
 
 
 class HostSizes(C.Structure):
@@ -409,8 +415,9 @@ class HostSizes(C.Structure):
                 ("dispatch_ms", C.c_double)]
 
 
-def host_input_arrays(ms: MatchSet, banned_images=()):
-    """The flat arrays of lfr_host_input for `ms`: (pair_skip, dict of contiguous arrays by field name)."""
+def host_input_arrays(ms: MatchSet, banned_images=(), image_group=None):
+    """The flat arrays of lfr_host_input for `ms`: (pair_skip, dict of contiguous arrays by field name).
+    `image_group` (MatchSet.query_subscenes) adds the sub-scene of every image id."""
     banned = set(banned_images)
     skip = np.array([(ms.image_names[a] in banned) or (ms.image_names[b] in banned)
                      for a, b in zip(ms.pair_img1.tolist(), ms.pair_img2.tolist())], dtype=np.uint8) \
@@ -421,6 +428,8 @@ def host_input_arrays(ms: MatchSet, banned_images=()):
         feat1=np.ascontiguousarray(ms.feat1, dtype=np.uint32), feat2=np.ascontiguousarray(ms.feat2, dtype=np.uint32),
         sim=np.ascontiguousarray(ms.sim, dtype=np.float32), disp1=np.ascontiguousarray(ms.disp1, dtype=np.float32),
         disp2=np.ascontiguousarray(ms.disp2, dtype=np.float32))
+    if image_group is not None:
+        arrs["image_group"] = np.ascontiguousarray(image_group, dtype=np.uint32)
     return skip, arrs
 
 
@@ -472,7 +481,7 @@ def host_stage_export(arrs: dict, n_images: int):
     return 0, out, {k: getattr(sz, k) for k in HOST_SIZES_FIELDS}
 
 
-def build_problem_native(ms: MatchSet, banned_images=(), log=None) -> Problem:
+def build_problem_native(ms: MatchSet, banned_images=(), log=None, image_group=None) -> Problem:
     """solve.cc:405-606 through the native host stage (csrc/lfr_host.cc, include/lfr_host.h)."""
     from .capi import load_host
 
@@ -483,7 +492,7 @@ def build_problem_native(ms: MatchSet, banned_images=(), log=None) -> Problem:
     L.lfr_host_stage_export.restype = C.c_int
     L.lfr_host_stage_destroy.argtypes = [C.c_void_p]
     L.lfr_host_stage_destroy.restype = None
-    skip, arrs = host_input_arrays(ms, banned_images)
+    skip, arrs = host_input_arrays(ms, banned_images, image_group)
     # the edge records (80 B each) are written straight into the array handed to lfr_solve
     counts = (arrs["pair_ptr"][1:] - arrs["pair_ptr"][:-1]).astype(np.int64)
     e_cap = 2 * int(counts[skip == 0].sum()) if ms.n_pairs else 0
@@ -556,17 +565,31 @@ def problem_from_stage(ms: MatchSet, skip: np.ndarray, out: dict, sz: dict, host
                    comp_nodes=out["comp_nodes"], comp_order=out["comp_order"].astype(np.int64), info=info)
 
 
-def build_problem(ms: MatchSet, banned_images=(), log=None, native: Optional[bool] = None) -> Problem:
+def build_problem(ms: MatchSet, banned_images=(), log=None, native: Optional[bool] = None,
+                  image_group: Optional[np.ndarray] = None) -> Problem:
     """solve.cc:405-606 end to end.  Uses the native host stage (csrc/lfr_host.cc)
     unless native=False or LFR_HOST_PYTHON=1 selects the numpy implementation below
-    (the two are tested to agree exactly)."""
+    (the two are tested to agree exactly).  `image_group` [n_images]: the sub-scene of every image id
+    (MatchSet.query_subscenes; lfr_host_input::image_group)."""
     import os
     import time
     if native is None:
         native = not os.environ.get("LFR_HOST_PYTHON")
     if native:
-        return build_problem_native(ms, banned_images, log)
+        return build_problem_native(ms, banned_images, log, image_group)
     g = build_graph(ms, banned_images)
+    set_image = node_cap = None
+    if image_group is not None:
+        grp = np.asarray(image_group, dtype=np.int64)
+        set_image = np.zeros(grp.shape[0], dtype=np.int64)      # index inside the sub-scene
+        for k in range(int(grp.max()) + 1 if grp.size else 0):
+            ids = np.nonzero(grp == k)[0]
+            set_image[ids] = np.arange(ids.shape[0])
+        kept = ms.without_images(banned_images)
+        seen = np.zeros(grp.shape[0], dtype=bool)               # images_set of each sub-scene
+        seen[kept.pair_img1] = True
+        seen[kept.pair_img2] = True
+        group_seen = np.bincount(grp[seen], minlength=int(grp.max()) + 1 if grp.size else 0)
     say = log if log is not None else (lambda s: None)
     say("# graph nodes: %d" % g.n_nodes)                       # solve.cc:484
     say("# graph edges: %d" % (2 * g.und_n1.shape[0]))         # solve.cc:485
@@ -575,13 +598,15 @@ def build_problem(ms: MatchSet, banned_images=(), log=None, native: Optional[boo
         z32 = np.zeros(0, dtype=np.uint32)
         return Problem(g, z32, z32, np.zeros(0, np.uint8), np.zeros(1, np.uint32), z32, z32, info)
     t0 = time.perf_counter()
-    track = compute_tracks(g)
+    track = compute_tracks(g, set_image)
     n_tracks = int(track.max()) + 1
     say("# tracks: %d" % n_tracks)                             # solve.cc:534
     say("max track size: %d" % int(np.bincount(track).max()))  # solve.cc:549
     is_root = select_roots(g, track)
     t1 = time.perf_counter()
-    comp = separate_meta_graph(g, track, g.n_images, info)
+    if image_group is not None:
+        node_cap = group_seen[grp[g.node_image]]
+    comp = separate_meta_graph(g, track, g.n_images, info, node_cap)
     t2 = time.perf_counter()
     say("Graph-cut time: %dms" % int((t2 - t1) * 1e3))         # solve.cc:589
     n_comp = int(comp.max()) + 1

@@ -108,6 +108,40 @@ class MatchSet:
             disp1=self.disp1[sel], disp2=self.disp2[sel], meta=dict(self.meta),
         )
 
+    def query_subscenes(self, query_images, banned_images=()):
+        """--query_images: (the pairs of every query's sub-scene as one MatchSet, image_group).
+        After the banned images are dropped, a pair that names one query image belongs to that query's
+        sub-scene and a pair that names none is dropped; each sub-scene gets its own id for every image it
+        holds, in order of first appearance, so the sub-scenes share no node.  image_names of the result
+        repeat a database image's name once per sub-scene; image_group[id] is the sub-scene (the query's
+        image id in `self`).  Raises ValueError for a pair that names two queries."""
+        queries = set(query_images)
+        ms = self.without_images(banned_images)
+        is_q = [n in queries for n in ms.image_names]
+        keep, img1, img2, group, orig_of, ids = [], [], [], [], [], {}
+
+        def sub(q, i):
+            if (q, i) not in ids:
+                ids[(q, i)] = len(orig_of)
+                orig_of.append(i)
+                group.append(q)
+            return ids[(q, i)]
+
+        for p, (a, b) in enumerate(zip(ms.pair_img1.tolist(), ms.pair_img2.tolist())):
+            if is_q[a] and is_q[b]:
+                raise ValueError("the pair '%s' - '%s' names two query images" % (ms.image_names[a], ms.image_names[b]))
+            if not (is_q[a] or is_q[b]):
+                continue
+            q = a if is_q[a] else b
+            keep.append(p)
+            img1.append(sub(q, a))
+            img2.append(sub(q, b))
+        out = ms.select_pairs(np.array(keep, dtype=np.int64))
+        out.image_names = [ms.image_names[i] for i in orig_of]
+        out.pair_img1 = np.array(img1, dtype=np.int64)
+        out.pair_img2 = np.array(img2, dtype=np.int64)
+        return out, np.array(group, dtype=np.uint32)
+
     @staticmethod
     def concatenate(parts: List["MatchSet"]) -> "MatchSet":
         """Concatenate the `.part.N` files of one matching file (solve.cc:416-424):

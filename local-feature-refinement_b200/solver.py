@@ -32,7 +32,9 @@ class Solution:
     record: Optional[bytes] = None  # the run's problem record (include/lfr_graph.h), with refine(record_problem=True)
 
 
-def assemble_solution(p: Problem, positions: np.ndarray) -> Solution:
+def assemble_solution(p: Problem, positions: np.ndarray, written: Optional[np.ndarray] = None) -> Solution:
+    """`written` [n_images] bool (--query_images): only these images get an Image message; every node still
+    counts towards n_outside."""
     g = p.graph
     N = g.n_nodes
     if N == 0:
@@ -41,15 +43,19 @@ def assemble_solution(p: Problem, positions: np.ndarray) -> Solution:
     img_ids, first = np.unique(g.node_image, return_index=True)
     order = np.argsort(first, kind="stable")
     img_ids = img_ids[order]                      # images by first node appearance
+    pos = np.asarray(positions, dtype=np.float64).reshape(N, 2)
+    n_out = int(np.count_nonzero((np.abs(pos[:, 1]) > 0.5) | (np.abs(pos[:, 0]) > 0.5)))
+    nodes = np.arange(N)
+    if written is not None:
+        img_ids = img_ids[np.asarray(written, dtype=bool)[img_ids]]
+        nodes = np.nonzero(np.asarray(written, dtype=bool)[g.node_image])[0]
     rank = np.full(int(g.node_image.max()) + 1, -1, dtype=np.int64)
     rank[img_ids] = np.arange(img_ids.shape[0])
-    node_rank = rank[g.node_image]
-    perm = np.argsort(node_rank, kind="stable")   # nodes grouped by image, ascending node index
+    node_rank = rank[g.node_image[nodes]]
+    perm = nodes[np.argsort(node_rank, kind="stable")]   # nodes grouped by image, ascending node index
     counts = np.bincount(node_rank, minlength=img_ids.shape[0])
     img_ptr = np.zeros(img_ids.shape[0] + 1, dtype=np.uint64)
     np.cumsum(counts, out=img_ptr[1:])
-    pos = np.asarray(positions, dtype=np.float64).reshape(N, 2)
-    n_out = int(np.count_nonzero((np.abs(pos[:, 1]) > 0.5) | (np.abs(pos[:, 0]) > 0.5)))
     return Solution(
         image_names=[g.image_names[i] for i in img_ids.tolist()],
         fact=np.array([g.image_fact[i] for i in img_ids.tolist()], dtype=np.float32),
@@ -141,7 +147,7 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
            solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None, fixed_images=(),
            initial_solution: Optional[bytes] = None, keep_initial_solution: bool = False,
            update_initial_solution: bool = False, previous_matches=None, previous_record: Optional[bytes] = None,
-           record_problem: bool = False):
+           record_problem: bool = False, query_images=None):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
     may be supplied to drive a different executor (the multi-GPU path; give `n_devices`); with a start
     solution it is called as `solve_fn(problem, positions)`.
@@ -165,7 +171,13 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
 
     The graph stage runs where graph_stage_on_device() says.  On the device (Plan.from_matches) the problem
     stays in HBM and is solved there, `solve_fn` is not called, and the Problem's arrays come from
-    Plan.export_graph(); `timing["solver_ms"]` (when `timing` is given) then covers solve + download."""
+    Plan.export_graph(); `timing["solver_ms"]` (when `timing` is given) then covers solve + download.
+
+    `query_images` (names; names not in `ms` are ignored) localizes many queries in one run: every query is
+    refined against the rest of the scene on its own (MatchSet.query_subscenes), and each query's Image
+    message is the one a run on its sub-scene's pairs alone writes.  Only query images are written.  It
+    excludes update_initial_solution, previous_matches, previous_record and record_problem (ValueError); a
+    pair that names two query images, or sub-scenes of more than 65535 images in all, raise ValueError too."""
     from .capi import Plan, load_b200
     from .graph import host_input_arrays, problem_from_stage
     if keep_initial_solution and initial_solution is None:
@@ -185,18 +197,34 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
         previous_record = bytes(previous_record)
         if not record_is_valid(previous_record):
             raise ValueError("malformed problem record")
+    if query_images is not None:
+        for on, what in ((update_initial_solution, "update_initial_solution"), (previous_matches is not None, "previous_matches"),
+                         (previous_record is not None, "previous_record"), (record_problem, "record_problem")):
+            if on:
+                raise ValueError("query_images and %s exclude each other" % what)
+        # one scene of disjoint sub-scenes: database images get one id per sub-scene (their names repeat, and
+        # the joins and the fixed mask, which go by name, give every copy the same values)
+        ms, image_group = ms.query_subscenes(query_images, banned_images)
+        banned_images = ()
+        if len(ms.image_names) > 65535:
+            raise ValueError("query_images: the sub-scenes hold %d images, more than 65535; split the query list over "
+                             "several runs" % len(ms.image_names))
+        queries = set(query_images)
+        written = np.array([n in queries for n in ms.image_names], dtype=bool)
+    else:
+        image_group = written = None
     if isinstance(previous_matches, (bytes, bytearray, memoryview)):
         from .wire import decode_matching_file
         previous_matches = decode_matching_file(bytes(previous_matches))
     lib = load_b200()
-    skip, arrs = host_input_arrays(ms, banned_images)
+    skip, arrs = host_input_arrays(ms, banned_images, image_group)
     if not graph_stage_on_device(lib, arrs, len(ms.image_names), n_devices):
-        p = build_problem(ms, banned_images, log=log)
+        p = build_problem(ms, banned_images, log=log, image_group=image_group)
         q, start = constant_problem(p, fixed_images, initial_solution, keep_initial_solution, update_initial_solution,
                                     previous_matches, previous_record)
         fn = solve_fn if solve_fn is not None else (lambda q_, x=None: solve_problem(q_, options, x))
         pos, st = fn(q) if start is None else fn(q, start)
-        sol = assemble_solution(p, pos)
+        sol = assemble_solution(p, pos, written)
         if record_problem:
             from .wire import problem_record
             sol.record = problem_record(p, ms.image_names)
@@ -231,6 +259,6 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
         record = plan.problem_record(ms.image_names) if record_problem else None
     finally:
         plan.close()
-    sol = assemble_solution(p, pos)
+    sol = assemble_solution(p, pos, written)
     sol.record = record
     return p, pos, st, sol
