@@ -298,7 +298,8 @@ def main(argv=None) -> int:
     except ValueError as e:   # --query_images: a pair that names two query images, or too many images
         if args.query_images is None:
             raise
-        sys.stderr.write("ERROR: %s\n" % e)
+        msg = str(e)   # refine() names its argument, the command line its option (lfr_solve_main.cc's line)
+        sys.stderr.write("ERROR: %s\n" % ("--" + msg if msg.startswith("query_images:") else msg))
         return 2
     say("Solver time: %dms" % int(timing.get("solver_ms", 0.0)))                       # solve.cc:638
     say("Total time: %dms" % int((time.perf_counter() - t_start) * 1e3))               # solve.cc:641

@@ -239,11 +239,12 @@ def test_cuts_run_with_the_sub_scene_cap(scene):
     assert n_cut > 0
 
 
-def test_stage_with_groups_equals_the_per_group_stages(scene):
+def assert_stages_agree_by_sub_scene(batch, queries, banned, grouped=None):
     """The C++ and numpy stages on the grouped input give, sub-scene by sub-scene, the arrays of the stage on that
-    sub-scene's pairs alone, under the renumbering that keeps relative order."""
-    d, db, batch, queries, banned = scene
-    sub, group = batch.query_subscenes(queries, [banned])
+    sub-scene's pairs alone, under the renumbering that keeps relative order.  `grouped` (sub MatchSet, image_group)
+    replaces batch.query_subscenes(queries, [banned]) as the grouped input: the same sub-scenes, their images
+    numbered otherwise."""
+    sub, group = grouped if grouped is not None else batch.query_subscenes(queries, [banned])
     _, arrs = host_input_arrays(sub, (), group)
     rc, out, sz = host_stage_export(arrs, len(sub.image_names))
     assert rc == 0
@@ -277,6 +278,12 @@ def test_stage_with_groups_equals_the_per_group_stages(scene):
         eb = np.concatenate([out["edges"][rb[v]:rb[v + 1]] for v in nodes.tolist()])
         assert np.array_equal(remap[eb["dst"].astype(np.int64)], o["edges"]["dst"].astype(np.int64))
         assert eb["flow"].tobytes() == o["edges"]["flow"].tobytes() and eb["sim"].tobytes() == o["edges"]["sim"].tobytes()
+    return out, sz
+
+
+def test_stage_with_groups_equals_the_per_group_stages(scene):
+    d, db, batch, queries, banned = scene
+    assert_stages_agree_by_sub_scene(batch, queries, banned)
 
 
 @pytest.mark.parametrize("mode", sorted(MODES))
