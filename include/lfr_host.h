@@ -45,12 +45,13 @@ typedef struct lfr_host_input {
   lfr_edge* edges_out;
   uint64_t edges_out_capacity;  /* in records                                     */
   /* optional: [n_images] the sub-scene of every image id, or NULL: the whole input is one scene.  With
-   * sub-scenes (--query_images) every non-skipped pair joins two images of one sub-scene (LFR_EINVAL
-   * otherwise), the cut cap of a meta-component is the number of images its sub-scene's non-skipped pairs
-   * name (n_images_seen of that sub-scene alone), and a union-find image set indexes images inside their
-   * sub-scene, so its storage follows the largest sub-scene, not n_images.  Each sub-scene then gets the
-   * arrays a stage on its pairs alone gives, under a renumbering that keeps their relative order.  The
-   * graph stage on the GPU does not take sub-scenes (lfr_graph_stage_on_device() says host for them). */
+   * sub-scenes (--query_images, one query or with --joint_queries a group of queries each) every
+   * non-skipped pair joins two images of one sub-scene (LFR_EINVAL otherwise), the cut cap of a
+   * meta-component is the number of images its sub-scene's non-skipped pairs name (n_images_seen of that
+   * sub-scene alone), and a union-find image set indexes images inside their sub-scene, so its storage
+   * follows the largest sub-scene, not n_images.  Each sub-scene then gets the arrays a stage on its pairs
+   * alone gives, under a renumbering that keeps their relative order.  The graph stage on the GPU
+   * (lfr_plan_create_from_matches(), lfr_plan_create_from_wire()) takes sub-scenes as this stage does. */
   const uint32_t* image_group;
 } lfr_host_input;
 

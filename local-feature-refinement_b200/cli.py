@@ -31,6 +31,9 @@ Plan.problem_record, Plan.update_solution(previous_record=...)).
 --query_images NAME (repeatable) localizes many queries in one run: a pair that names one query image belongs
 to that query's sub-scene, a pair that names none is not solved, and each query is refined as a run on its
 sub-scene's pairs alone refines it (solver.refine(query_images=...)).  Only query images are written.
+--joint_queries (with --query_images) refines queries that a kept pair names together, such as the frames of a
+sequence or the cameras of a rig, in one sub-scene: each query is refined as a run on its group's pairs alone
+refines it (solver.refine(joint_queries=True)).
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -68,7 +71,8 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("fixed_images", True, True), ("initial_solution", True, False),
             ("keep_initial_solution", False, False), ("carry_initial_solution", False, False),
             ("update_initial_solution", False, False), ("previous_matches_file", True, False),
-            ("record_file", True, False), ("earlier_record_file", True, False), ("query_images", True, True)]
+            ("record_file", True, False), ("earlier_record_file", True, False), ("query_images", True, True),
+            ("joint_queries", False, False)]
 
 
 def _find_option(name):
@@ -148,7 +152,7 @@ def parse_args(argv):
             update_initial_solution=bool(vals.get("update_initial_solution")),
             previous_matches_file=vals.get("previous_matches_file"),
             record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"),
-            query_images=vals.get("query_images"))
+            query_images=vals.get("query_images"), joint_queries=bool(vals.get("joint_queries")))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -194,6 +198,9 @@ def main(argv=None) -> int:
             if on:
                 sys.stderr.write("ERROR: --query_images and %s exclude each other\n" % opt)
                 return 2
+    if args.joint_queries and args.query_images is None:
+        sys.stderr.write("ERROR: --joint_queries needs --query_images\n")
+        return 2
     start = None
     if args.initial_solution is not None:
         try:
@@ -291,7 +298,7 @@ def main(argv=None) -> int:
                                  keep_initial_solution=args.keep_initial_solution,
                                  update_initial_solution=args.update_initial_solution, previous_matches=previous,
                                  previous_record=earlier_record, record_problem=args.record_file is not None,
-                                 query_images=args.query_images)
+                                 query_images=args.query_images, joint_queries=args.joint_queries)
     except GraphStageRouteError as e:
         sys.stderr.write("ERROR: %s\n" % e)
         return 2

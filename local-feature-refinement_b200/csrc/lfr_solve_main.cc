@@ -38,7 +38,8 @@
 // lfr_plan_update_solution_since_record() / lfr_wire_update_solution_since_record()) and --query_images NAME
 // (repeatable: each query's pairs become a sub-scene with its own ids for the database images, the graph stage
 // takes the sub-scene of every id, lfr_host_input::image_group, and only query images are written:
-// lfr_plan_encode_solution_images() on the device route).  `--n_threads` is accepted and
+// lfr_plan_encode_solution_images() on the device route) and --joint_queries (with --query_images: queries
+// that a kept pair names together share one sub-scene, so sequences and rigs are refined jointly).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <chrono>
@@ -130,7 +131,7 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false},
                                {"update_initial_solution", false, false}, {"previous_matches_file", true, false},
                                {"record_file", true, false},  {"earlier_record_file", true, false},
-                               {"query_images", true, true}};
+                               {"query_images", true, true},  {"joint_queries", false, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -149,7 +150,8 @@ const OptionSpec& find_option(const std::string& name) {
 }
 
 struct Args {
-  bool help = false, keep_initial_solution = false, carry_initial_solution = false, update_initial_solution = false;
+  bool help = false, keep_initial_solution = false, carry_initial_solution = false, update_initial_solution = false,
+       joint_queries = false;
   std::map<std::string, std::string> single;
   std::map<std::string, std::vector<std::string>> repeated;
 };
@@ -185,6 +187,7 @@ Args parse(int argc, char** argv) {
         (std::strcmp(o.name, "help") == 0 ? a.help
          : std::strcmp(o.name, "keep_initial_solution") == 0  ? a.keep_initial_solution
          : std::strcmp(o.name, "carry_initial_solution") == 0 ? a.carry_initial_solution
+         : std::strcmp(o.name, "joint_queries") == 0          ? a.joint_queries
                                                               : a.update_initial_solution) = true;
       }
     } else if (tok.size() > 1 && tok[0] == '-') {
@@ -346,7 +349,7 @@ int main(int argc, char** argv) {
   std::vector<std::string> banned_list, fixed_list, query_list;
   uint64_t device = 0, gpus = 1;
   bool keep_start = false, carry_start = false, update_start = false, have_previous = false, have_record = false,
-       have_earlier = false, have_query = false;
+       have_earlier = false, have_query = false, joint = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -365,6 +368,7 @@ int main(int argc, char** argv) {
     fixed_list = a.repeated["fixed_images"];
     have_query = a.repeated.count("query_images") != 0;
     query_list = a.repeated["query_images"];
+    joint = a.joint_queries;
     if (a.single.count("initial_solution")) initial_solution = a.single.at("initial_solution");
     keep_start = a.keep_initial_solution;
     carry_start = a.carry_initial_solution;
@@ -421,6 +425,10 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "ERROR: --query_images and %s exclude each other\n", o.second);
         return 2;
       }
+  }
+  if (joint && !have_query) {
+    std::fputs("ERROR: --joint_queries needs --query_images\n", stderr);
+    return 2;
   }
   if (have_start) {
     if (!start_file.open(initial_solution)) {
@@ -543,38 +551,54 @@ int main(int argc, char** argv) {
   for (uint64_t p = 0; p < P; ++p)
     skip[p] = (banned.count(names[pair_img1[p]]) || banned.count(names[pair_img2[p]])) ? 1 : 0;
 
-  // --query_images: a kept pair that names one query image belongs to that query's sub-scene, and its images
-  // get that sub-scene's ids, in order of first appearance; a pair that names none is not solved.  The graph
-  // stage then gives every sub-scene what a run on its pairs alone gives (lfr_host_input::image_group).
+  // --query_images: a kept pair that names a query image belongs to that query's group's sub-scene, and its
+  // images get that sub-scene's ids, in order of first appearance; a pair that names none is not solved.  A
+  // group is one query, or with --joint_queries a connected component of the queries under the kept pairs
+  // that name two of them (with or without matches).  The graph stage then gives every sub-scene what a run
+  // on its pairs alone gives (lfr_host_input::image_group).
   // orig_of: the original image id (and name) of every stage image id; the identity without queries.
   std::vector<uint8_t> is_query(names.size(), 0);
   std::vector<uint32_t> orig_of, image_group;
   if (have_query) {
     const std::set<std::string> queries(query_list.begin(), query_list.end());
     for (size_t i = 0; i < names.size(); ++i) is_query[i] = queries.count(names[i]) ? 1 : 0;
-    std::map<std::pair<uint32_t, uint32_t>, uint32_t> sub_id;  // (query image, image) -> stage image id
-    auto sub = [&](uint32_t q, uint32_t img) {
-      const auto it = sub_id.emplace(std::make_pair(q, img), (uint32_t)orig_of.size());
+    // the group of every query image: a union-find whose root is the group's lowest image id, its label.  It
+    // runs over all pairs before any id is handed out, since a later pair can merge two groups that hold ids.
+    std::vector<uint32_t> group_of(names.size());
+    for (uint32_t i = 0; i < (uint32_t)names.size(); ++i) group_of[i] = i;
+    auto find = [&](uint32_t x) {
+      while (group_of[x] != x) x = group_of[x] = group_of[group_of[x]];
+      return x;
+    };
+    for (uint64_t p = 0; p < P; ++p) {
+      const uint32_t a = pair_img1[p], b = pair_img2[p];
+      if (skip[p] || !is_query[a] || !is_query[b]) continue;
+      if (!joint) {
+        std::fprintf(stderr, "ERROR: the pair '%s' - '%s' names two query images\n", names[a].c_str(), names[b].c_str());
+        return 2;
+      }
+      const uint32_t ra = find(a), rb = find(b);
+      group_of[std::max(ra, rb)] = std::min(ra, rb);
+    }
+    std::map<std::pair<uint32_t, uint32_t>, uint32_t> sub_id;  // (group, image) -> stage image id
+    auto sub = [&](uint32_t g, uint32_t img) {
+      const auto it = sub_id.emplace(std::make_pair(g, img), (uint32_t)orig_of.size());
       if (it.second) {
         orig_of.push_back(img);
-        image_group.push_back(q);
+        image_group.push_back(g);
       }
       return it.first->second;
     };
     for (uint64_t p = 0; p < P; ++p) {
       const uint32_t a = pair_img1[p], b = pair_img2[p];
-      if (!skip[p] && is_query[a] && is_query[b]) {
-        std::fprintf(stderr, "ERROR: the pair '%s' - '%s' names two query images\n", names[a].c_str(), names[b].c_str());
-        return 2;
-      }
       if (skip[p] || !(is_query[a] || is_query[b])) {
         skip[p] = 1;
         pair_img1[p] = pair_img2[p] = 0;  // never read: skipped pairs name no image of the stage
         continue;
       }
-      const uint32_t q = is_query[a] ? a : b;
-      pair_img1[p] = sub(q, a);
-      pair_img2[p] = sub(q, b);
+      const uint32_t g = find(is_query[a] ? a : b);
+      pair_img1[p] = sub(g, a);
+      pair_img2[p] = sub(g, b);
     }
     if (orig_of.size() > 65535) {
       std::fprintf(stderr, "ERROR: --query_images: the sub-scenes hold %zu images, more than 65535; split the query list "

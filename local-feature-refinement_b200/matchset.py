@@ -108,34 +108,51 @@ class MatchSet:
             disp1=self.disp1[sel], disp2=self.disp2[sel], meta=dict(self.meta),
         )
 
-    def query_subscenes(self, query_images, banned_images=()):
-        """--query_images: (the pairs of every query's sub-scene as one MatchSet, image_group).
-        After the banned images are dropped, a pair that names one query image belongs to that query's
-        sub-scene and a pair that names none is dropped; each sub-scene gets its own id for every image it
-        holds, in order of first appearance, so the sub-scenes share no node.  image_names of the result
-        repeat a database image's name once per sub-scene; image_group[id] is the sub-scene (the query's
-        image id in `self`).  Raises ValueError for a pair that names two queries."""
+    def query_subscenes(self, query_images, banned_images=(), joint=False):
+        """--query_images: (the pairs of every query group's sub-scene as one MatchSet, image_group).
+        A group is one query; with `joint` (--joint_queries) it is a connected component of the queries under
+        the kept pairs that name two of them, with or without matches.  After the banned images are dropped,
+        a pair that names a query image belongs to that query's group's sub-scene and a pair that names none
+        is dropped; each sub-scene gets its own id for every image it holds, in order of first appearance, so
+        the sub-scenes share no node.  image_names of the result repeat a database image's name once per
+        sub-scene; image_group[id] is the sub-scene (the group's lowest query image id in `self`).  Without
+        `joint`, raises ValueError for a pair that names two queries."""
         queries = set(query_images)
         ms = self.without_images(banned_images)
         is_q = [n in queries for n in ms.image_names]
+        pairs = list(zip(ms.pair_img1.tolist(), ms.pair_img2.tolist()))
+        # the group of every query image: a union-find rooted at the group's lowest image id, run over all
+        # pairs before any id is handed out (a later pair can merge two groups that already hold ids)
+        group_of = list(range(len(ms.image_names)))
+
+        def find(x):
+            while group_of[x] != x:
+                group_of[x] = group_of[group_of[x]]
+                x = group_of[x]
+            return x
+
+        for a, b in pairs:
+            if is_q[a] and is_q[b]:
+                if not joint:
+                    raise ValueError("the pair '%s' - '%s' names two query images" % (ms.image_names[a], ms.image_names[b]))
+                ra, rb = find(a), find(b)
+                group_of[max(ra, rb)] = min(ra, rb)
         keep, img1, img2, group, orig_of, ids = [], [], [], [], [], {}
 
-        def sub(q, i):
-            if (q, i) not in ids:
-                ids[(q, i)] = len(orig_of)
+        def sub(g, i):
+            if (g, i) not in ids:
+                ids[(g, i)] = len(orig_of)
                 orig_of.append(i)
-                group.append(q)
-            return ids[(q, i)]
+                group.append(g)
+            return ids[(g, i)]
 
-        for p, (a, b) in enumerate(zip(ms.pair_img1.tolist(), ms.pair_img2.tolist())):
-            if is_q[a] and is_q[b]:
-                raise ValueError("the pair '%s' - '%s' names two query images" % (ms.image_names[a], ms.image_names[b]))
+        for p, (a, b) in enumerate(pairs):
             if not (is_q[a] or is_q[b]):
                 continue
-            q = a if is_q[a] else b
+            g = find(a if is_q[a] else b)
             keep.append(p)
-            img1.append(sub(q, a))
-            img2.append(sub(q, b))
+            img1.append(sub(g, a))
+            img2.append(sub(g, b))
         out = ms.select_pairs(np.array(keep, dtype=np.int64))
         out.image_names = [ms.image_names[i] for i in orig_of]
         out.pair_img1 = np.array(img1, dtype=np.int64)

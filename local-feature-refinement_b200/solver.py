@@ -147,7 +147,7 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
            solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None, fixed_images=(),
            initial_solution: Optional[bytes] = None, keep_initial_solution: bool = False,
            update_initial_solution: bool = False, previous_matches=None, previous_record: Optional[bytes] = None,
-           record_problem: bool = False, query_images=None):
+           record_problem: bool = False, query_images=None, joint_queries: bool = False):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
     may be supplied to drive a different executor (the multi-GPU path; give `n_devices`); with a start
     solution it is called as `solve_fn(problem, positions)`.
@@ -177,7 +177,10 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     refined against the rest of the scene on its own (MatchSet.query_subscenes), and each query's Image
     message is the one a run on its sub-scene's pairs alone writes.  Only query images are written.  It
     excludes update_initial_solution, previous_matches, previous_record and record_problem (ValueError); a
-    pair that names two query images, or sub-scenes of more than 65535 images in all, raise ValueError too."""
+    pair that names two query images, or sub-scenes of more than 65535 images in all, raise ValueError too.
+    `joint_queries` (needs `query_images`) refines queries that a kept pair names together (sequences, rigs) in
+    one sub-scene: a group is a connected component of the queries under such pairs, and each query's Image
+    message is the one a run on its group's pairs alone writes."""
     from .capi import Plan, load_b200
     from .graph import host_input_arrays, problem_from_stage
     if keep_initial_solution and initial_solution is None:
@@ -197,6 +200,8 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
         previous_record = bytes(previous_record)
         if not record_is_valid(previous_record):
             raise ValueError("malformed problem record")
+    if joint_queries and query_images is None:
+        raise ValueError("joint_queries needs query_images")
     if query_images is not None:
         for on, what in ((update_initial_solution, "update_initial_solution"), (previous_matches is not None, "previous_matches"),
                          (previous_record is not None, "previous_record"), (record_problem, "record_problem")):
@@ -204,7 +209,7 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
                 raise ValueError("query_images and %s exclude each other" % what)
         # one scene of disjoint sub-scenes: database images get one id per sub-scene (their names repeat, and
         # the joins and the fixed mask, which go by name, give every copy the same values)
-        ms, image_group = ms.query_subscenes(query_images, banned_images)
+        ms, image_group = ms.query_subscenes(query_images, banned_images, joint=joint_queries)
         banned_images = ()
         if len(ms.image_names) > 65535:
             raise ValueError("query_images: the sub-scenes hold %d images, more than 65535; split the query list over "

@@ -100,9 +100,10 @@ def pair_list(cfg: SynthConfig, rng: np.random.Generator) -> List[Tuple[int, int
     raise ValueError(cfg.pairs)
 
 
-def generate(cfg, scale: float = 1.0, seed: int | None = None) -> MatchSet:
+def generate(cfg, scale: float = 1.0, seed: int | None = None, pairs=None) -> MatchSet:
     """Build the MatchSet of a config (name, alias or SynthConfig).  `scale`
-    multiplies keypoints per image (for quick tests)."""
+    multiplies keypoints per image (for quick tests).  `pairs` ([(a, b)], a != b) replaces the
+    config's pair list."""
     if isinstance(cfg, str):
         cfg = CONFIGS[ALIASES.get(cfg, cfg)]
     rng = np.random.default_rng(cfg.seed if seed is None else seed)
@@ -128,7 +129,7 @@ def generate(cfg, scale: float = 1.0, seed: int | None = None) -> MatchSet:
     # keypoint localisation error of each observation, units of 16 px
     terr = [rng.uniform(-0.3, 0.3, size=(o.shape[0], 2)) for o in obs]
 
-    pairs = pair_list(cfg, rng)
+    pairs = pair_list(cfg, rng) if pairs is None else [(int(a), int(b)) for a, b in pairs]
     f1s, f2s, sims, d1s, d2s, ptr = [], [], [], [], [], [0]
     n_out = int(round(cfg.outlier_frac * K))
     for (a, b) in pairs:
