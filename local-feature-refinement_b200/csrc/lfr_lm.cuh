@@ -15,6 +15,9 @@
 //   trial(alpha)               xc = P(x + alpha dl) and the cost there
 //   trial_slope(alpha, &dphi)  the same plus phi'(alpha) = grad f(xc) . dl (only read if the cost is finite)
 //   slope()                    phi' at the candidate of the last trial()
+//   restore_full_step()        after a failed line search: the candidate of the last trial() and its
+//                              cost again, as that call left them (trial_slope() has replaced them since)
+//   kSkipFailingContraction    whether a line search stops before a contraction that cannot pass
 //   scale_step(s)              dl *= s
 //   x_norm()                   |x| over the free coordinates
 //   step_norm()                |x - xc| over the free coordinates
@@ -300,6 +303,16 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
         ++ls_steps;
         if (ls_iter >= K.max_ls_iter) break;
         prof.tick(LmProfile::kRest);
+        // The contraction picks its step between max_contraction and min_contraction x current.x (a root
+        // of the interpolant may land past the upper end by the rounding of t -> x, hence the margin): when
+        // even the longest step is below the minimum step size, the search fails whatever the polynomial
+        // says, and the polynomial is not worth computing.  Only the warp2 queue kernel, whose slowest
+        // components end in such searches, tests this: the per-bucket warp kernels (168 registers) measured
+        // slower with the test than without it, and the other tiers keep their code as it was.
+        if constexpr (Tier::kSkipFailingContraction) {
+          const double longest = fmax(K.ls_min_contraction, K.ls_max_contraction) * current.x;
+          if (longest > 0.0 && longest * dmax * (1.0 + 0x1p-30) < K.ls_min_step) break;
+        }
         const double step = ls_next_step(initial, previous, current, K, T.lane());
         prof.tick(Tier::kPolyWord);
         if (step * dmax < K.ls_min_step) break;
@@ -316,8 +329,8 @@ __device__ __forceinline__ void lm_solve(Tier& T, const DevProblem& P, const Dev
       }
       if (ls_ok) {
         T.scale_step(current.x);
-      } else {  // line search failed: delta unchanged, candidate = P(x + delta)
-        cost_c = T.trial(1.0);
+      } else {  // line search failed: delta unchanged, candidate = P(x + delta), the search's first trial
+        cost_c = T.restore_full_step();
         c_valid = isfinite(cost_c);
       }
     }

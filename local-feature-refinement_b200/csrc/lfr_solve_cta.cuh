@@ -495,6 +495,7 @@ struct CtaTier {
   static constexpr int kStride = NT;
   static constexpr unsigned kTier = LmProfile::kCta;
   static constexpr int kPolyWord = LmProfile::kRest;
+  static constexpr bool kSkipFailingContraction = false;  // see lm_solve
   CtaCtx& C;
   const DevConsts& K;
   unsigned cg_iters;
@@ -516,6 +517,7 @@ struct CtaTier {
     return cost;
   }
   __device__ double slope() { return cta_assemble<true>(C, false, K); }
+  __device__ double restore_full_step() { return trial(1.0); }
   __device__ void scale_step(double s) {
     for (int i = C.tid; i < C.n; i += NT) C.dl[i] *= s;
     __syncthreads();

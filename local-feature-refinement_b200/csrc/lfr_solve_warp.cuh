@@ -300,6 +300,7 @@ struct WarpTier {
   static constexpr int kStride = 32;
   static constexpr unsigned kTier = LmProfile::kWarp;
   static constexpr int kPolyWord = LmProfile::kTierWord;
+  static constexpr bool kSkipFailingContraction = false;  // see lm_solve
   WarpCtx& C;
   const DevConsts& K;
   __device__ int tid() const { return C.lane; }
@@ -328,6 +329,7 @@ struct WarpTier {
     return cost;
   }
   __device__ double slope() { return staged_grad_dot(C); }
+  __device__ double restore_full_step() { return trial(1.0); }
   __device__ void scale_step(double s) {
     for (int i = C.lane; i < C.n; i += 32) C.dl[i] *= s;
     __syncwarp();

@@ -539,6 +539,16 @@ struct RegTier {
   const DevConsts& K;
   CandNorms nr;  // of the last candidate (warp)
   int nreg;      // NREG == 0: reg_class() of the component
+  // The queue kernel keeps the last trial()'s cost and norms: a failed line search takes them back
+  // instead of evaluating the full step again, and restages its evaluation only if the step is accepted.
+  // The tiles (which sum the norms from xc) and the per-bucket warp kernels evaluate the full step again:
+  // at 168 registers for 12 warps per SM the kept values spill, which measured slower on cfg3, whose
+  // searches do not fail.
+  static constexpr bool kKeepFullStep = T == 32 && NREG == 0;
+  static constexpr bool kSkipFailingContraction = kKeepFullStep;  // see lm_solve
+  double cost_full = 0.0;
+  CandNorms nr_full{0.0, 0.0};
+  bool restored = false;  // xc and the staged evaluation are a trial_slope()'s, not the restored step's
   __device__ int tid() const { return C.tid; }
   __device__ int lane() const { return C.tid & 31; }
   __device__ bool lead() const { return C.tid == 0; }
@@ -588,13 +598,28 @@ struct RegTier {
   }
   __device__ double trial(double alpha) {
     nr = reg_candidate(C, alpha, K);
-    return eval<false, true>(C.xc);
+    const double cost = eval<false, true>(C.xc);
+    if constexpr (kKeepFullStep) {
+      cost_full = cost;
+      nr_full = nr;
+      restored = false;
+    }
+    return cost;
   }
   __device__ double trial_slope(double alpha, double* dphi) {
     nr = reg_candidate(C, alpha, K);
     return eval<true, true>(C.xc, dphi);
   }
   __device__ double slope() { return reg_assemble<true>(C, false, K); }
+  __device__ double restore_full_step() {
+    if constexpr (kKeepFullStep) {
+      nr = nr_full;
+      restored = true;
+      return cost_full;
+    } else {
+      return trial(1.0);
+    }
+  }
   __device__ void scale_step(double s) {
     for (int i = C.tid; i < C.n; i += T) C.dl[i] *= s;
     G::sync();
@@ -623,6 +648,11 @@ struct RegTier {
   }
   __device__ double accept() {
     if constexpr (T == 32) {
+      if (kKeepFullStep && restored) {  // the same candidate and staged evaluation as the restored trial(1.0) made
+        reg_candidate(C, 1.0, K);
+        eval<false, false>(C.xc);
+        restored = false;
+      }
       for (int i = C.tid; i < 2 * C.Nc; i += T) C.x[i] = C.xc[i];
       __syncwarp();
       return sqrt(nr.xn2);

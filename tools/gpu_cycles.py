@@ -1,4 +1,4 @@
-"""Per-component cycle breakdown of the solve kernels (LFR_DBG_PROFILE); for the eight longest components
+"""Per-component cycle breakdown of the solve kernels (LFR_DBG_PROFILE); for the ten longest components
 also when their solve started and finished (%globaltimer, µs after the first component's start)."""
 import os
 import sys
@@ -39,7 +39,7 @@ names = ["total", "setup", "eval", "assemble", "solve", "rest"]
 for k in names:
     print("  %-9s sum %.3e  share %.1f%%  per-iter %.0f" % (
         k, rec[k][sel].sum(), 100.0 * rec[k][sel].sum() / tot.sum(), rec[k][sel].sum() / max(1, it[sel].sum())))
-w = np.argsort(-tot)[:8]
+w = np.argsort(-tot)[:10]
 idx = np.nonzero(sel)[0][w]
 for i in idx:
     print("  slot", i, "tier", PROFILE_TIERS.get(int(rec["tier"][i])), "nodes", int(p.comp_ptr[i + 1] - p.comp_ptr[i]),
