@@ -278,14 +278,18 @@ __device__ __noinline__ int real_roots_in(const double* c, int n, double lo, dou
 // back with lfr_debug_poly_prof().  [0] coefficients [1] first evaluations
 // [2] grid classification (or quadratic) [3] extremum cells (or cubic level)
 // [4] root solves (or quartic level) [5] final evaluations
-// [6] quintic calls [7] cubic calls [8] Newton iterations [9] bracket_root calls
-// [10] whole cubic-interpolant call
+// [6] quintic calls [7] cubic calls [8] Horner evaluations of the polishes
+// [9] polished roots [10] whole cubic-interpolant call
+// The clock is read only at stage boundaries, and a polish adds its Horner count
+// once, after its loop, so the counters do not lengthen the loop they count.
 __device__ unsigned long long g_poly_prof[16];
 #define LFR_PP_TICK(k) do { const long long n__ = clock64(); if (lane == 0) atomicAdd(&g_poly_prof[k], (unsigned long long)(n__ - pp_t)); pp_t = n__; } while (0)
 #define LFR_PP_COUNT(k) atomicAdd(&g_poly_prof[k], 1ull)
+#define LFR_PP_ADD(k, n) atomicAdd(&g_poly_prof[k], (unsigned long long)(n))
 #else
 #define LFR_PP_TICK(k) do {} while (0)
 #define LFR_PP_COUNT(k) do {} while (0)
+#define LFR_PP_ADD(k, n) do {} while (0)
 #endif
 
 // ---- fixed-degree variants ----------------------------------------------------
@@ -315,15 +319,15 @@ __device__ __forceinline__ double poly_eval_n(const double (&p)[N], double x) {
 }
 
 template <int N>
-__device__ __forceinline__ double bracket_root_n(const double (&q)[N], double a, double b, double fa, double fb) {
+__device__ __forceinline__ double bracket_root_loop(const double (&q)[N], double a, double b, double fa, double fb,
+                                                    int& nh) {
   if (fa == 0.0) return a;
   if (fb == 0.0) return b;
   double xl = fa < 0.0 ? a : b, xh = fa < 0.0 ? b : a;
   double x = a - fa * newton_quotient(b - a, fb - fa);
   if (!(x > fmin(a, b) && x < fmax(a, b))) x = 0.5 * (a + b);
-  LFR_PP_COUNT(9);
   for (int it = 0; it < 100; ++it) {
-    LFR_PP_COUNT(8);
+    ++nh;
     double f, df;
     horner2_n<N>(q, x, &f, &df);
     if (f == 0.0) return x;
@@ -339,6 +343,74 @@ __device__ __forceinline__ double bracket_root_n(const double (&q)[N], double a,
     x = xn;
     if (fabs(dx) <= 1e-8 * fabs(x)) return x;
   }
+  return x;
+}
+
+template <int N>
+__device__ __forceinline__ double bracket_root_n(const double (&q)[N], double a, double b, double fa, double fb) {
+  int nh = 0;  // Horner evaluations (diagnostic build only)
+  const double r = bracket_root_loop<N>(q, a, b, fa, fb, nh);
+  LFR_PP_ADD(8, nh);
+  LFR_PP_COUNT(9);
+  return r;
+}
+
+// f / df in double precision: the MUFU.RCP64H seed of 1 / df (about 23 bits), one
+// FMA refinement (about 46 bits) and the product.  Newton keeps its quadratic
+// convergence down to the last bits, without the 2^-24 floor of newton_quotient,
+// at a chain much shorter than a division's.  A zero or denormal df gives a
+// non-finite quotient, which the caller's bracket test turns into a bisection.
+__device__ __forceinline__ double newton_quotient64(double f, double df) {
+  double r;
+  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(df));
+  r = fma(r, fma(-df, r, 1.0), r);
+  return f * r;
+}
+
+// One Halley step for a root of f from s = 0, with f(s) = f0 + f1 s + f2 s^2 + ... (the
+// Taylor expansion the grid point already holds): the offset of the start; error O(s^3).
+__device__ __forceinline__ double halley_offset(double f0, double f1, double f2) {
+  double r;  // a zero or out-of-range denominator gives an infinite or zero offset: no start
+  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(fma(f1, f1, -f2 * f0)));
+  return -(f0 * f1) * r;
+}
+
+// One real root of q inside the bracket [a, b] of a grid cell (f(a), f(b) of opposite sign, q
+// monotone there), from the start x0 that the Taylor expansion at a cell end gives (the
+// regula-falsi point if x0 is not strictly inside).  Then bracket_root_n's safeguarded Newton
+// with the double-precision quotient: from a start within ~w^3 of the root (w = the cell width)
+// one step lands within the last bits and the next one meets the stopping rule.
+template <int N>
+__device__ __forceinline__ double cell_root_n(const double (&q)[N], double x0, double a, double b, double fa,
+                                              double fb) {
+  if (fa == 0.0) return a;
+  if (fb == 0.0) return b;
+  int nh = 0;  // Horner evaluations (diagnostic build only)
+  double xl = fa < 0.0 ? a : b, xh = fa < 0.0 ? b : a;
+  double x = x0;
+  if (!(x > fmin(a, b) && x < fmax(a, b))) {
+    x = a - fa * newton_quotient(b - a, fb - fa);
+    if (!(x > fmin(a, b) && x < fmax(a, b))) x = 0.5 * (a + b);
+  }
+  for (int it = 0; it < 100; ++it) {
+    ++nh;
+    double f, df;
+    horner2_n<N>(q, x, &f, &df);
+    if (f == 0.0) break;
+    if (f < 0.0) xl = x; else xh = x;
+    double dx = newton_quotient64(f, df);
+    double xn = x - dx;
+    if (xn == x) break;
+    if (!(xn >= fmin(xl, xh) && xn <= fmax(xl, xh))) {
+      xn = 0.5 * (xl + xh);
+      dx = x - xn;
+    }
+    if (xn == x) break;
+    x = xn;
+    if (fabs(dx) <= 1e-8 * fabs(x)) break;
+  }
+  LFR_PP_ADD(8, nh);
+  LFR_PP_COUNT(9);
   return x;
 }
 
@@ -432,8 +504,9 @@ __device__ __forceinline__ int quartic_roots_in(const double (&q)[5], double lo,
 //   D = 3, D' = 0         has exactly one (monotone),
 // and every other case (two extrema inside one cell, an exact zero on the grid,
 // non-finite values) goes to the derivative recursion, which stays the reference.
-// Every root is polished by the same safeguarded Newton as before, from a bracket
-// 31x tighter, so both routes return the same roots up to the last bits.
+// Every root is polished by a safeguarded Newton inside its cell (cell_root_n), started
+// from a Halley step on the Taylor expansion the grid point already holds, so both
+// routes return the same roots up to the last bits.
 __device__ __forceinline__ int quartic_roots_grid(const double (&q)[5], double lo, double hi, double (&out)[4],
                                                   int lane, long long& pp_t) {
   const double w = (hi - lo) * (1.0 / 31.0);
@@ -461,13 +534,17 @@ __device__ __forceinline__ int quartic_roots_grid(const double (&q)[5], double l
   }
   if (__any_sync(0xffffffffu, bad || kind == 3)) return quartic_roots_in(q, lo, hi, out, lane, pp_t);
   LFR_PP_TICK(2);
-  // cells with one extremum of q: find it, look at the sign of q there
+  // The polishes start from one Halley step on the Taylor expansion at t: for the root of q on
+  // (a4, a3, a2), for the extremum on q' = a3 + 2 a2 s + 3 a1 s^2 + 4 a0 s^3.  The root's start
+  // waits in e, which a cell with one extremum overwrites with the extremum: there e ends both
+  // brackets, and their (rare) roots start from the regula-falsi point.
   int nl = kind == 1 ? 1 : 0;
-  double xb = tn, fb = qn, e = 0.0, qe = 0.0;
+  double xb = tn, fb = qn, e = t + halley_offset(a4, a3, a2), qe = 0.0;
+  // cells with one extremum of q: find it, look at the sign of q there
   if (__any_sync(0xffffffffu, kind == 2)) {
     if (kind == 2) {
       const double d3[4] = {4.0 * q[0], 3.0 * q[1], 2.0 * q[2], q[3]};
-      e = bracket_root_n<4>(d3, t, tn, a3, dqn);
+      e = cell_root_n<4>(d3, t + halley_offset(a3, 2.0 * a2, 3.0 * a1), t, tn, a3, dqn);
       qe = poly_eval_n<5>(q, e);
       if (qe != 0.0 && ((qe < 0.0) != (a4 < 0.0))) {  // q crosses zero on both sides of e
         nl = 2;
@@ -478,9 +555,9 @@ __device__ __forceinline__ int quartic_roots_grid(const double (&q)[5], double l
   }
   LFR_PP_TICK(3);
   double ra = 0.0, rb = 0.0;
-  if (nl >= 1) ra = bracket_root_n<5>(q, t, xb, a4, fb);
+  if (nl >= 1) ra = cell_root_n<5>(q, e, t, xb, a4, fb);
   if (__any_sync(0xffffffffu, nl == 2)) {
-    if (nl == 2) rb = bracket_root_n<5>(q, e, tn, qe, qn);
+    if (nl == 2) rb = cell_root_n<5>(q, e, e, tn, qe, qn);
   }
   // gather in ascending order (cells are ordered, ra < rb inside a cell)
   unsigned m1 = __ballot_sync(0xffffffffu, nl >= 1);

@@ -27,10 +27,10 @@ torch.cuda.synchronize()
 lib.lib.lfr_debug_poly_prof(out.ctypes.data, 1)
 names = ["coefficients", "first evals", "grid classify", "extremum cells", "root solves", "final evals"]
 nq, nc = int(out[6]), int(out[7])
-print("quintic calls", nq, "cubic calls", nc, "newton iterations", int(out[8]), "bracket_root calls", int(out[9]))
+print("quintic calls", nq, "cubic calls", nc, "Horner evaluations", int(out[8]), "polished roots", int(out[9]))
 for i, nm in enumerate(names):
     print("  %-14s %8.0f cycles / quintic call" % (nm, out[i] / max(nq, 1)))
 print("  quintic total  %8.0f" % (out[:6].sum() / max(nq, 1)))
 print("  cubic call     %8.0f cycles / call" % (out[10] / max(nc, 1)))
 if out[9]:
-    print("  newton iterations per bracketed root %.2f" % (out[8] / out[9]))
+    print("  Horner evaluations per polished root %.2f" % (out[8] / out[9]))
