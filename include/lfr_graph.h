@@ -98,6 +98,19 @@ int64_t lfr_plan_encode_solution_images(lfr_plan* plan, void* stream, uint32_t n
                                         const uint64_t* name_off, const float* fact, const uint8_t* written, uint8_t* out,
                                         uint64_t cap, uint64_t* n_outside);
 
+/* The SolutionFiles of a batch of scenes (--additional_scenes) in one device pass: image k belongs to group
+ * group_of_image[k] (< n_groups).  Group g's bytes are out[group_off[g], group_off[g+1]), equal to
+ * lfr_plan_encode_solution_images() with written = the images of group g, and n_outside[g] counts the nodes of
+ * group g's images only.  A group with no node encodes to 0 bytes.  group_off [n_groups + 1] and n_outside
+ * [n_groups] are filled on every successful call; the return value is the total, group_off[n_groups], and the
+ * bytes are written only when cap >= that (the size protocol of lfr_plan_encode_solution).  The groups are
+ * encoded together, not one after the other: a thousand groups cost one encode.  LFR_EINVAL as
+ * lfr_plan_encode_solution(), or for NULL group_of_image / group_off / n_outside or a group id >= n_groups. */
+int64_t lfr_plan_encode_solution_groups(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                        const uint64_t* name_off, const float* fact, const uint32_t* group_of_image,
+                                        uint32_t n_groups, uint8_t* out, uint64_t cap, uint64_t* group_off /* [n_groups+1] */,
+                                        uint64_t* n_outside /* [n_groups] */);
+
 /* lfr_plan_encode_solution() merged with an earlier SolutionFile `file`: the scene's output, each scene
  * image followed by its carried entries, then the file's other winning Image messages — the bytes of
  * lfr_wire_encode_solution_carried() (include/lfr_wire.h, which states the rule) on the plan's host assembly

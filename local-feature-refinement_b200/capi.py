@@ -83,7 +83,7 @@ GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "l
                  "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
                  "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution",
                  "lfr_plan_encode_solution_carried", "lfr_plan_update_solution", "lfr_plan_update_solution_since",
-                 "lfr_plan_problem_record", "lfr_plan_update_solution_since_record"]
+                 "lfr_plan_problem_record", "lfr_plan_update_solution_since_record", "lfr_plan_encode_solution_groups"]
 
 
 class LfrWirePart(C.Structure):
@@ -180,6 +180,10 @@ class Library:
                                                            C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                                            C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
             L.lfr_plan_encode_solution_carried.restype = C.c_int64
+            L.lfr_plan_encode_solution_groups.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                          C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64,
+                                                          C.c_void_p, C.c_void_p]
+            L.lfr_plan_encode_solution_groups.restype = C.c_int64
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -476,6 +480,31 @@ class Plan:
         if got != need:
             self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution")
         return out[:need].tobytes(), int(n_out.value)
+
+    def encode_solution_groups(self, image_names, image_fact, image_group, n_groups: int, stream: int = 0):
+        """lfr_plan_encode_solution_groups (include/lfr_graph.h): one SolutionFile per image group, encoded on the
+        device in one pass.  `image_group[id]` < n_groups is the group of image id.  Returns ([bytes of every
+        group], [n_outside of every group])."""
+        from .wire import _names_blob
+        blob, off = _names_blob(list(image_names))
+        fact = np.ascontiguousarray(image_fact, dtype=np.float32).reshape(-1)
+        group = np.ascontiguousarray(image_group, dtype=np.uint32).reshape(-1)
+        if fact.shape[0] != len(image_names) or group.shape[0] != len(image_names):
+            raise ValueError("image_fact / image_group do not have one entry per image name")
+        goff = np.zeros(n_groups + 1, np.uint64)
+        n_out = np.zeros(max(n_groups, 1), np.uint64)
+        f = self.lib.lib.lfr_plan_encode_solution_groups
+        args = (self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data, _ptr(fact),
+                _ptr(group), n_groups)
+        need = f(*args, None, 0, goff.ctypes.data, n_out.ctypes.data)
+        if need < 0:
+            self.lib.check(int(need), "lfr_plan_encode_solution_groups")
+        out = np.empty(max(int(need), 1), np.uint8)
+        got = f(*args, out.ctypes.data, int(need), goff.ctypes.data, n_out.ctypes.data)
+        if got != need:
+            self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution_groups")
+        data = out[:need].tobytes()
+        return [data[int(goff[g]):int(goff[g + 1])] for g in range(n_groups)], [int(x) for x in n_out[:n_groups]]
 
     def encode_solution_carried(self, image_names, image_fact, carry: bytes, stream: int = 0):
         """lfr_plan_encode_solution_carried (include/lfr_graph.h): encode_solution() merged on the device with the

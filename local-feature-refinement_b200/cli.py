@@ -34,6 +34,9 @@ sub-scene's pairs alone refines it (solver.refine(query_images=...)).  Only quer
 --joint_queries (with --query_images) refines queries that a kept pair names together, such as the frames of a
 sequence or the cameras of a rig, in one sub-scene: each query is refined as a run on its group's pairs alone
 refines it (solver.refine(joint_queries=True)).
+--additional_scenes FILE (lines `MATCHES_FILE<TAB>OUTPUT_FILE`) refines many scenes in one run: the scene of
+--matches_file / --output_file and every listed one, each output file byte for byte what that scene's own run
+writes (solver.refine_scenes).
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -72,7 +75,7 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("keep_initial_solution", False, False), ("carry_initial_solution", False, False),
             ("update_initial_solution", False, False), ("previous_matches_file", True, False),
             ("record_file", True, False), ("earlier_record_file", True, False), ("query_images", True, True),
-            ("joint_queries", False, False)]
+            ("joint_queries", False, False), ("additional_scenes", True, False)]
 
 
 def _find_option(name):
@@ -152,11 +155,70 @@ def parse_args(argv):
             update_initial_solution=bool(vals.get("update_initial_solution")),
             previous_matches_file=vals.get("previous_matches_file"),
             record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"),
-            query_images=vals.get("query_images"), joint_queries=bool(vals.get("joint_queries")))
+            query_images=vals.get("query_images"), joint_queries=bool(vals.get("joint_queries")),
+            additional_scenes=vals.get("additional_scenes"))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
         raise SystemExit(1)
+
+
+def read_scene_list(path, matches_file, output_file):
+    """--additional_scenes FILE: [(matches file, output file)] of scene 0 (--matches_file / --output_file) and
+    of every line `MATCHES_FILE<TAB>OUTPUT_FILE` (raw bytes; the last newline optional), or the bytes of the one
+    ERROR line for an unreadable file, a malformed line or two scenes with the same output path (lfr_solve_main.cc
+    writes the same lines)."""
+    try:
+        with open(path, "rb") as fh:
+            text = fh.read()
+    except OSError:
+        return b"ERROR: cannot read the scene list file '%s'\n" % os.fsencode(path)
+    scenes = [(os.fsencode(matches_file), os.fsencode(output_file))]
+    lines = text.split(b"\n")
+    if lines[-1] == b"":
+        lines.pop()
+    for k, line in enumerate(lines, 1):
+        why = ("it is empty" if not line else "it has no TAB" if b"\t" not in line
+               else "it has more than one TAB" if line.count(b"\t") > 1
+               else "its matches file is empty" if line.startswith(b"\t")
+               else "its output file is empty" if line.endswith(b"\t")
+               else "it holds a NUL byte" if b"\0" in line else None)
+        if why:
+            return b"ERROR: --additional_scenes: line %d is not MATCHES_FILE<TAB>OUTPUT_FILE: %s\n" % (k, why.encode())
+        scenes.append(tuple(line.split(b"\t")))
+    seen = set()
+    for _, o in scenes:
+        if o in seen:
+            return b"ERROR: --additional_scenes: two scenes write '%s'\n" % o
+        seen.add(o)
+    return [(os.fsdecode(m), os.fsdecode(o)) for m, o in scenes]
+
+
+def _run_scenes(args, scenes, ms, opts, say, solve_fn, n_devices, timing, t_start) -> int:
+    """--additional_scenes after the scenes were read: one refine_scenes() run, the stdout lines once, then the
+    output files in scene order."""
+    from .solver import GraphStageRouteError, refine_scenes
+    sols = []
+    try:
+        data = refine_scenes([m for m, _ in scenes], args.banned_images, opts, log=say, solve_fn=solve_fn,
+                             n_devices=n_devices, timing=timing, solutions=sols)
+    except GraphStageRouteError as e:
+        sys.stderr.write("ERROR: %s\n" % e)
+        return 2
+    except ValueError as e:   # more than 65535 image ids
+        sys.stderr.write("ERROR: --%s\n" % e)
+        return 2
+    say("Solver time: %dms" % int(timing.get("solver_ms", 0.0)))                       # solve.cc:638
+    say("Total time: %dms" % int((time.perf_counter() - t_start) * 1e3))               # solve.cc:641
+    say("# points with at least one coordinate > 0.5: %d" % sum(s.n_outside for s in sols))   # solve.cc:670
+    try:
+        for (_, out), d in zip(scenes, data):
+            with open(out, "wb") as fh:
+                fh.write(d)
+    except OSError:
+        sys.stderr.write("Failed to write proto object.\n")
+        return 255
+    return 0
 
 
 def main(argv=None) -> int:
@@ -201,6 +263,25 @@ def main(argv=None) -> int:
     if args.joint_queries and args.query_images is None:
         sys.stderr.write("ERROR: --joint_queries needs --query_images\n")
         return 2
+    scenes = None
+    if args.additional_scenes is not None:
+        for on, opt in ((bool(args.fixed_images), "--fixed_images"), (args.initial_solution is not None, "--initial_solution"),
+                        (args.keep_initial_solution, "--keep_initial_solution"),
+                        (args.carry_initial_solution, "--carry_initial_solution"),
+                        (args.update_initial_solution, "--update_initial_solution"),
+                        (args.previous_matches_file is not None, "--previous_matches_file"),
+                        (args.record_file is not None, "--record_file"),
+                        (args.earlier_record_file is not None, "--earlier_record_file"),
+                        (args.query_images is not None, "--query_images"), (args.joint_queries, "--joint_queries")):
+            if on:
+                sys.stderr.write("ERROR: --additional_scenes and %s exclude each other\n" % opt)
+                return 2
+        scenes = read_scene_list(args.additional_scenes, args.matches_file, args.output_file)
+        if isinstance(scenes, bytes):
+            sys.stderr.flush()
+            sys.stderr.buffer.write(scenes)
+            sys.stderr.buffer.flush()
+            return 2
     start = None
     if args.initial_solution is not None:
         try:
@@ -252,13 +333,17 @@ def main(argv=None) -> int:
     except wire.ParseError:
         sys.stderr.write("Failed to parse proto object.\n")
         return 255
+    from .matchset import MatchSet
     if ms is None:
-        from .matchset import MatchSet
-        import numpy as np
-        ms = MatchSet([], np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32),
-                      np.zeros(0, np.float32), np.zeros(1, np.int64), np.zeros(0, np.uint32),
-                      np.zeros(0, np.uint32), np.zeros(0, np.float32), np.zeros((0, 18), np.float32),
-                      np.zeros((0, 18), np.float32))
+        ms = MatchSet.empty()
+    if scenes is not None:
+        # every scene's input is read before any output is written
+        try:
+            scenes = [(ms, scenes[0][1])] + [(wire.read_matching_file(m) if wire.matches_files(m) else MatchSet.empty(), o)
+                                             for m, o in scenes[1:]]
+        except wire.ParseError:
+            sys.stderr.write("Failed to parse proto object.\n")
+            return 255
 
     lib = load_b200()   # fails loudly when the CUDA library is missing
     opts = lib.default_options(device=args.device, n_threads=args.n_threads)
@@ -292,6 +377,11 @@ def main(argv=None) -> int:
     if torchrun and args.query_images is not None:
         sys.stderr.write("ERROR: --query_images: torchrun ranks do not localize queries; use --gpus N\n")
         return 2
+    if torchrun and scenes is not None:
+        sys.stderr.write("ERROR: --additional_scenes: torchrun ranks do not refine scene batches; use --gpus N\n")
+        return 2
+    if scenes is not None:
+        return _run_scenes(args, scenes, ms, opts, say, solve_fn, n_devices, timing, t_start)
     try:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
                                  timing=timing, fixed_images=args.fixed_images, initial_solution=start,

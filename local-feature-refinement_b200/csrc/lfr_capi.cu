@@ -2076,6 +2076,98 @@ int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t
   return (int64_t)total;
 }
 
+// lfr_plan_encode_solution_groups() on a checked plan and arguments (lfr_solution.cuh): encode_solution()'s
+// kernels on the images ranked by (group, first node), so that the groups' SolutionFiles are consecutive
+// ranges of one output; the group offsets and counts come back with the total
+int64_t encode_solution_groups(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t* names, const uint64_t* name_off,
+                               const float* fact, const uint32_t* group_of_image, uint32_t G, uint8_t* out, uint64_t cap,
+                               uint64_t* group_off, uint64_t* n_outside) {
+  using namespace lfr::solution;
+  const uint32_t N = pl->N;
+  if (!N) {
+    std::memset(group_off, 0, 8 * ((size_t)G + 1));
+    std::memset(n_outside, 0, 8 * (size_t)G);
+    return 0;
+  }
+  const uint64_t name_bytes = name_off[NI];
+  size_t at = 0;
+  auto take = [&at](size_t bytes) {
+    const size_t o = at;
+    at += (bytes + 255) & ~(size_t)255;
+    return o;
+  };
+  const size_t o_first = take(4 * (size_t)NI), o_key = take(8 * (size_t)NI), o_key_s = take(8 * (size_t)NI),
+               o_iota_i = take(4 * (size_t)NI), o_img_s = take(4 * (size_t)NI), o_present = take(4 * ((size_t)NI + 1)),
+               o_dense = take(4 * ((size_t)NI + 1)), o_rank = take(4 * (size_t)NI), o_img_d = take(4 * (size_t)NI),
+               o_img_ptr = take(4 * ((size_t)NI + 1)), o_ctr = take(16), o_body = take(8 * (size_t)NI),
+               o_isize = take(8 * ((size_t)NI + 1)), o_ioff = take(8 * ((size_t)NI + 1)),
+               o_name_off = take(8 * ((size_t)NI + 1)), o_fact = take(4 * (size_t)NI), o_names = take(name_bytes),
+               o_group = take(4 * (size_t)NI), o_gcount = take(4 * ((size_t)G + 1)), o_grank = take(4 * ((size_t)G + 1)),
+               o_goff = take(8 * ((size_t)G + 1)), o_gout = take(8 * (size_t)G), o_nkey = take(4 * (size_t)N),
+               o_nkey_s = take(4 * (size_t)N), o_iota = take(4 * (size_t)N), o_perm = take(4 * (size_t)N),
+               o_rsize = take(8 * ((size_t)N + 1)), o_noff = take(8 * ((size_t)N + 1));
+  LFR_TRY(pl->enc_scratch.reserve(at));
+  uint8_t* base = pl->enc_scratch.as<uint8_t>();
+  auto u32 = [base](size_t o) { return reinterpret_cast<uint32_t*>(base + o); };
+  auto u64 = [base](size_t o) { return reinterpret_cast<uint64_t*>(base + o); };
+  auto ull = [base](size_t o) { return reinterpret_cast<unsigned long long*>(base + o); };
+  uint32_t *first = u32(o_first), *iota_i = u32(o_iota_i), *img_s = u32(o_img_s), *present = u32(o_present),
+           *dense = u32(o_dense), *rank = u32(o_rank), *img_d = u32(o_img_d), *img_ptr = u32(o_img_ptr),
+           *n_present = u32(o_ctr), *d_group = u32(o_group), *gcount = u32(o_gcount), *grank = u32(o_grank),
+           *key = u32(o_nkey), *key_s = u32(o_nkey_s), *iota = u32(o_iota), *perm = u32(o_perm);
+  uint64_t *body = u64(o_body), *isize = u64(o_isize), *ioff = u64(o_ioff), *d_name_off = u64(o_name_off),
+           *goff = u64(o_goff), *rsize = u64(o_rsize), *noff = u64(o_noff);
+  unsigned long long *ikey = ull(o_key), *ikey_s = ull(o_key_s), *gout = ull(o_gout);
+  float* d_fact = reinterpret_cast<float*>(base + o_fact);
+  uint8_t* d_names = base + o_names;
+  const uint32_t* nimg = pl->node_image.as<uint32_t>();
+  const uint32_t* nfeat = pl->node_feat.as<uint32_t>();
+  const double* pos = pl->pos.as<double>();
+
+  LFR_CUDA(cudaMemcpyAsync(d_name_off, name_off, 8 * ((size_t)NI + 1), cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemcpyAsync(d_fact, fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
+  if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, names, name_bytes, cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemcpyAsync(d_group, group_of_image, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
+  LFR_CUDA(cudaMemsetAsync(gcount, 0, 4 * ((size_t)G + 1), s));
+  if (G) LFR_CUDA(cudaMemsetAsync(gout, 0, 8 * (size_t)G, s));
+  init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
+  group_first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, d_group, first, gout);
+  group_key_kernel<<<blocks_for(NI), 256, 0, s>>>(first, d_group, NI, ikey);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // by group, then by first node
+    return cub::DeviceRadixSort::SortPairs(t, nb, ikey, ikey_s, iota_i, img_s, (int)NI, 0, 32 + bits_for(G), s);
+  }));
+  group_present_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(ikey_s, NI, N, present, gcount);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, present, dense, (int)NI + 1, s); }));
+  group_rank_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(img_s, present, dense, NI, rank, img_d, n_present);
+  node_key_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, rank, N, key, iota, nullptr, NI, nullptr);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: ascending node index within an image
+    return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, iota, perm, (int)N, 0, bits_for(NI), s);
+  }));
+  record_size_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, N, rsize, img_ptr);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, noff, (int)N + 1, s); }));
+  image_size_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(img_d, img_ptr, noff, d_name_off, d_fact, n_present, NI, body, isize);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)NI + 1, s); }));
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, gcount, grank, (int)G + 1, s); }));
+  group_off_kernel<<<blocks_for((uint64_t)G + 1), 256, 0, s>>>(grank, ioff, G, goff);
+  LFR_LAUNCHED();
+  if (G) LFR_CUDA(cudaMemcpyAsync(n_outside, gout, 8 * (size_t)G, cudaMemcpyDeviceToHost, s));
+  LFR_TRY(fetch(group_off, goff, (size_t)G + 1, s));
+  const uint64_t total = group_off[G];
+  if (!out || cap < total) return (int64_t)total;
+  LFR_TRY(pl->enc_out.reserve(total));
+  uint8_t* d_out = pl->enc_out.as<uint8_t>();
+  write_images_kernel<<<blocks_for(NI), 256, 0, s>>>(img_d, body, ioff, d_names, d_name_off, d_fact, n_present, d_out);
+  write_records_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, img_ptr, noff, ioff, N, d_out);
+  LFR_LAUNCHED();
+  LFR_TRY(fetch(out, d_out, total, s));
+  return (int64_t)total;
+}
+
 int select_device(const lfr_options& o) {
   int n_dev = 0;
   LFR_CUDA(cudaGetDeviceCount(&n_dev));
@@ -2746,6 +2838,24 @@ int64_t lfr_plan_encode_solution_images(lfr_plan* pl, void* stream, uint32_t n_i
   if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
   LFR_CUDA(cudaSetDevice(pl->device));
   return encode_solution(pl, (cudaStream_t)stream, n_images, names, name_off, fact, out, cap, n_outside, written);
+}
+
+int64_t lfr_plan_encode_solution_groups(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
+                                        const uint64_t* name_off, const float* fact, const uint32_t* group_of_image,
+                                        uint32_t n_groups, uint8_t* out, uint64_t cap, uint64_t* group_off,
+                                        uint64_t* n_outside) {
+  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
+  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
+  if (n_images && (!name_off || !fact || !group_of_image)) return fail(LFR_EINVAL, "NULL image names, facts or groups");
+  if (!group_off || (n_groups && !n_outside)) return fail(LFR_EINVAL, "NULL group_off or n_outside");
+  for (uint32_t k = 0; k < n_images; ++k) {
+    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
+    if (group_of_image[k] >= n_groups) return fail(LFR_EINVAL, "an image's group is not below n_groups");
+  }
+  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  LFR_CUDA(cudaSetDevice(pl->device));
+  return encode_solution_groups(pl, (cudaStream_t)stream, n_images, names, name_off, fact, group_of_image, n_groups, out,
+                                cap, group_off, n_outside);
 }
 
 int lfr_plan_fix_images(lfr_plan* pl, const uint8_t* fixed_by_image_id, uint32_t n_images) {

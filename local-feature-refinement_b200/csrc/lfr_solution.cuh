@@ -13,6 +13,16 @@
 //   write_images_kernel / write_records_kernel   the bytes, one thread per image / per node
 // With `written` (lfr_plan_encode_solution_images, --query_images) an image without the flag is absent: its
 // nodes count towards "> 0.5" but sort after every written node and get no record.
+//
+// lfr_plan_encode_solution_groups (--additional_scenes) writes one SolutionFile per image group in the same
+// pass: the images are sorted once by (group, first node) and ranked densely over the present ones, so every
+// later kernel above runs unchanged and group g's bytes are one contiguous range of the output:
+//   group_first_node_kernel   first[img]; the "> 0.5" count of every group
+//   group_key_kernel          key[img] = group << 32 | first[img]  (sort -> img_s, by group then first node)
+//   group_present_kernel      present[r] of the sorted images, present images per group
+//   (exclusive scan of present -> dense ranks)  group_rank_kernel: rank, the present images in order
+//   (node_key .. write_records as above; exclusive scan of the per-group counts -> first rank of each group)
+//   group_off_kernel          group_off[g] = byte offset of the group's first image
 #pragma once
 
 #include <cstdint>
@@ -197,6 +207,57 @@ __global__ void write_records_kernel(const uint32_t* perm, const uint32_t* key_s
     *p++ = kTagDj;
     put_fixed32(p, dj);
   }
+}
+
+// first_node_kernel without `written`, the "> 0.5" count kept per group (one atomic per run of equal groups
+// in a warp)
+__global__ void group_first_node_kernel(const uint32_t* node_image, const double* pos, uint32_t n, const uint32_t* group,
+                                        uint32_t* first, unsigned long long* n_outside) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = v < n;
+  const unsigned mask = __ballot_sync(0xffffffffu, live);
+  if (!live) return;
+  const uint32_t img = node_image[v];
+  const unsigned peers = __match_any_sync(mask, img);
+  if ((threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) atomicMin(first + img, v);
+  const bool outside = fabs(pos[2 * (size_t)v + 1]) > 0.5 || fabs(pos[2 * (size_t)v]) > 0.5;  // solve.cc:666-669
+  const uint32_t g = group[img];
+  const unsigned same = __match_any_sync(mask, g), out = __ballot_sync(mask, outside) & same;
+  if ((threadIdx.x & 31) == (unsigned)(__ffs(same) - 1) && out) atomicAdd(n_outside + g, (unsigned long long)__popc(out));
+}
+
+// an image without a node keeps first = n_nodes and sorts after its group's present images
+__global__ void group_key_kernel(const uint32_t* first, const uint32_t* group, uint32_t n_images, unsigned long long* key) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_images) key[i] = (unsigned long long)group[i] << 32 | first[i];
+}
+
+// present[r] of the sorted images (present[n_images] = 0, so that the exclusive scan ends on their count) and
+// the present images of every group
+__global__ void group_present_kernel(const unsigned long long* key_sorted, uint32_t n_images, uint32_t n_nodes,
+                                     uint32_t* present, uint32_t* group_count) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r > n_images) return;
+  const bool p = r < n_images && (uint32_t)key_sorted[r] < n_nodes;
+  present[r] = p;
+  if (p) atomicAdd(group_count + (uint32_t)(key_sorted[r] >> 32), 1u);
+}
+
+// rank[img] and img_dense[rank] of every present image, ranks dense in (group, first node) order; *n_present
+__global__ void group_rank_kernel(const uint32_t* img_sorted, const uint32_t* present, const uint32_t* dense,
+                                  uint32_t n_images, uint32_t* rank, uint32_t* img_dense, uint32_t* n_present) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0) *n_present = dense[n_images];
+  if (r >= n_images || !present[r]) return;
+  rank[img_sorted[r]] = dense[r];
+  img_dense[dense[r]] = img_sorted[r];
+}
+
+// group_off[g] = the byte offset of group g's first present image (its rank group_rank[g]); past the last
+// present image the scan of the image sizes holds the total
+__global__ void group_off_kernel(const uint32_t* group_rank, const uint64_t* img_off, uint32_t n_groups, uint64_t* group_off) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g <= n_groups) group_off[g] = img_off[group_rank[g]];
 }
 
 }  // namespace solution

@@ -39,9 +39,13 @@
 // (repeatable: each query's pairs become a sub-scene with its own ids for the database images, the graph stage
 // takes the sub-scene of every id, lfr_host_input::image_group, and only query images are written:
 // lfr_plan_encode_solution_images() on the device route) and --joint_queries (with --query_images: queries
-// that a kept pair names together share one sub-scene, so sequences and rigs are refined jointly).  `--n_threads` is accepted and
+// that a kept pair names together share one sub-scene, so sequences and rigs are refined jointly) and
+// --additional_scenes FILE (lines `MATCHES_FILE<TAB>OUTPUT_FILE`: every listed scene is one more sub-scene of the
+// same run, and each scene's output file holds what its own run writes: lfr_plan_encode_solution_groups() on
+// the device route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdint>
@@ -104,6 +108,10 @@ int64_t lfr_plan_encode_solution_carried(lfr_plan* plan, void* stream, uint32_t 
                                          const uint64_t* name_off, const float* fact, const uint8_t* file,
                                          uint64_t file_len, uint8_t* out, uint64_t cap, uint64_t* n_outside,
                                          uint64_t* n_carried) __attribute__((weak));
+int64_t lfr_plan_encode_solution_groups(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                        const uint64_t* name_off, const float* fact, const uint32_t* group_of_image,
+                                        uint32_t n_groups, uint8_t* out, uint64_t cap, uint64_t* group_off,
+                                        uint64_t* n_outside) __attribute__((weak));
 }
 
 namespace {
@@ -131,7 +139,8 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"keep_initial_solution", false, false}, {"carry_initial_solution", false, false},
                                {"update_initial_solution", false, false}, {"previous_matches_file", true, false},
                                {"record_file", true, false},  {"earlier_record_file", true, false},
-                               {"query_images", true, true},  {"joint_queries", false, false}};
+                               {"query_images", true, true},  {"joint_queries", false, false},
+                               {"additional_scenes", true, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -337,6 +346,46 @@ int read_previous(const std::string& path, PreviousMatches& pm) {
   return 0;
 }
 
+// The --additional_scenes list: one `MATCHES_FILE<TAB>OUTPUT_FILE` per line (raw bytes; the last newline is
+// optional), appended to `scenes`.  0, or 2 after one ERROR line for an unreadable file, a malformed line or
+// two scenes (the first one included) with the same output path.
+int read_scene_list(const std::string& path, std::vector<std::pair<std::string, std::string>>& scenes) {
+  FileImage f;
+  if (!f.open(path)) {
+    std::fprintf(stderr, "ERROR: cannot read the scene list file '%s'\n", path.c_str());
+    return 2;
+  }
+  const std::string text(reinterpret_cast<const char*>(f.data()), f.size());
+  f.release();
+  size_t line = 0;
+  for (size_t at = 0; at < text.size();) {
+    ++line;
+    const size_t end = std::min(text.find('\n', at), text.size());
+    const std::string l = text.substr(at, end - at);
+    at = end + 1;
+    const size_t tab = l.find('\t');
+    const char* why = l.empty()                                  ? "it is empty"
+                      : tab == std::string::npos                 ? "it has no TAB"
+                      : l.find('\t', tab + 1) != std::string::npos ? "it has more than one TAB"
+                      : tab == 0                                 ? "its matches file is empty"
+                      : tab + 1 == l.size()                      ? "its output file is empty"
+                      : l.find('\0') != std::string::npos        ? "it holds a NUL byte"
+                                                                 : nullptr;
+    if (why) {
+      std::fprintf(stderr, "ERROR: --additional_scenes: line %zu is not MATCHES_FILE<TAB>OUTPUT_FILE: %s\n", line, why);
+      return 2;
+    }
+    scenes.emplace_back(l.substr(0, tab), l.substr(tab + 1));
+  }
+  std::set<std::string> outputs;
+  for (const auto& sc : scenes)
+    if (!outputs.insert(sc.second).second) {
+      std::fprintf(stderr, "ERROR: --additional_scenes: two scenes write '%s'\n", sc.second.c_str());
+      return 2;
+    }
+  return 0;
+}
+
 using Clock = std::chrono::steady_clock;
 long long ms_between(Clock::time_point a, Clock::time_point b) {
   return (long long)std::chrono::duration_cast<std::chrono::milliseconds>(b - a).count();
@@ -345,11 +394,12 @@ long long ms_between(Clock::time_point a, Clock::time_point b) {
 }  // namespace
 
 int main(int argc, char** argv) {
-  std::string matches_file, output_file, initial_solution, previous_matches_file, record_file, earlier_record_file;
+  std::string matches_file, output_file, initial_solution, previous_matches_file, record_file, earlier_record_file,
+      scene_list;
   std::vector<std::string> banned_list, fixed_list, query_list;
   uint64_t device = 0, gpus = 1;
   bool keep_start = false, carry_start = false, update_start = false, have_previous = false, have_record = false,
-       have_earlier = false, have_query = false, joint = false;
+       have_earlier = false, have_query = false, joint = false, have_scenes = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -379,6 +429,8 @@ int main(int argc, char** argv) {
     if (have_record) record_file = a.single.at("record_file");
     have_earlier = a.single.count("earlier_record_file") != 0;
     if (have_earlier) earlier_record_file = a.single.at("earlier_record_file");
+    have_scenes = a.single.count("additional_scenes") != 0;
+    if (have_scenes) scene_list = a.single.at("additional_scenes");
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
@@ -430,6 +482,25 @@ int main(int argc, char** argv) {
     std::fputs("ERROR: --joint_queries needs --query_images\n", stderr);
     return 2;
   }
+  // --additional_scenes: the scene of --matches_file / --output_file is scene 0, the listed ones follow; each
+  // scene's output is what its own run writes (the same command with that scene's two files alone)
+  std::vector<std::pair<std::string, std::string>> scenes{{matches_file, output_file}};
+  if (have_scenes) {  // the start solution, the fixed images and the incremental modes belong to one scene
+    for (const auto& o : {std::make_pair(!fixed_list.empty(), "--fixed_images"), std::make_pair(have_start, "--initial_solution"),
+                          std::make_pair(keep_start, "--keep_initial_solution"),
+                          std::make_pair(carry_start, "--carry_initial_solution"),
+                          std::make_pair(update_start, "--update_initial_solution"),
+                          std::make_pair(have_previous, "--previous_matches_file"), std::make_pair(have_record, "--record_file"),
+                          std::make_pair(have_earlier, "--earlier_record_file"), std::make_pair(have_query, "--query_images"),
+                          std::make_pair(joint, "--joint_queries")})
+      if (o.first) {
+        std::fprintf(stderr, "ERROR: --additional_scenes and %s exclude each other\n", o.second);
+        return 2;
+      }
+    const int rc = read_scene_list(scene_list, scenes);
+    if (rc) return rc;
+  }
+  const uint32_t S = (uint32_t)scenes.size();
   if (have_start) {
     if (!start_file.open(initial_solution)) {
       std::fprintf(stderr, "ERROR: cannot read the initial solution file '%s'\n", initial_solution.c_str());
@@ -483,15 +554,21 @@ int main(int argc, char** argv) {
     ~Joiner() { if (t.joinable()) t.join(); }
   } join_on_exit{cuda_start};
 
-  // ---- solve.cc:412-481: the file, or its .part.N pieces ------------------------------------
+  // ---- solve.cc:412-481: the file, or its .part.N pieces, of every scene -----------------------
   std::vector<std::string> files;
-  if (file_exists(matches_file)) {
-    files.push_back(matches_file);
-  } else {
-    for (int k = 0;; ++k) {
-      const std::string f = matches_file + ".part." + std::to_string(k);
-      if (!file_exists(f)) break;
-      files.push_back(f);
+  std::vector<uint32_t> part_scene;
+  for (uint32_t sc = 0; sc < S; ++sc) {
+    const std::string& mf = scenes[sc].first;
+    if (file_exists(mf)) {
+      files.push_back(mf);
+      part_scene.push_back(sc);
+    } else {
+      for (int k = 0;; ++k) {
+        const std::string f = mf + ".part." + std::to_string(k);
+        if (!file_exists(f)) break;
+        files.push_back(f);
+        part_scene.push_back(sc);
+      }
     }
   }
   std::vector<Part> parts(files.size());
@@ -513,7 +590,8 @@ int main(int argc, char** argv) {
     }
   }
 
-  // image names -> ids in order of first appearance over all parts; the pairs of all parts in order
+  // image names -> ids in order of first appearance over all parts; the pairs of all parts in order, and the
+  // scene of every pair
   std::vector<std::string> names;
   std::map<std::string, uint32_t> id_of;
   auto intern = [&](const Part& pt, uint64_t off, uint32_t len) {
@@ -530,10 +608,13 @@ int main(int argc, char** argv) {
   std::vector<uint32_t> pair_img1(P), pair_img2(P);
   std::vector<float> pair_fact1(P), pair_fact2(P);
   std::vector<uint64_t> pair_ptr(P + 1, 0);
+  std::vector<uint32_t> pair_scene(P);
   {
     uint64_t p0 = 0, m0 = 0;
-    for (Part& pt : parts) {
+    for (size_t i = 0; i < parts.size(); ++i) {
+      Part& pt = parts[i];
       for (uint64_t p = 0; p < pt.P; ++p) {
+        pair_scene[p0 + p] = part_scene[i];
         pair_img1[p0 + p] = intern(pt, pt.n1_off[p], pt.n1_len[p]);
         pair_img2[p0 + p] = intern(pt, pt.n2_off[p], pt.n2_len[p]);
         pair_fact1[p0 + p] = pt.fact1[p];
@@ -555,11 +636,13 @@ int main(int argc, char** argv) {
   // images get that sub-scene's ids, in order of first appearance; a pair that names none is not solved.  A
   // group is one query, or with --joint_queries a connected component of the queries under the kept pairs
   // that name two of them (with or without matches).  The graph stage then gives every sub-scene what a run
-  // on its pairs alone gives (lfr_host_input::image_group).
-  // orig_of: the original image id (and name) of every stage image id; the identity without queries.
+  // on its pairs alone gives (lfr_host_input::image_group).  --additional_scenes: the same rule with every
+  // kept pair in its scene's sub-scene, labelled by the scene index, so that scenes that share image names
+  // share no node and each meta-component is cut at its own scene's image count.
+  // orig_of: the original image id (and name) of every stage image id; the identity without sub-scenes.
   std::vector<uint8_t> is_query(names.size(), 0);
   std::vector<uint32_t> orig_of, image_group;
-  if (have_query) {
+  if (have_query || have_scenes) {
     const std::set<std::string> queries(query_list.begin(), query_list.end());
     for (size_t i = 0; i < names.size(); ++i) is_query[i] = queries.count(names[i]) ? 1 : 0;
     // the group of every query image: a union-find whose root is the group's lowest image id, its label.  It
@@ -570,7 +653,7 @@ int main(int argc, char** argv) {
       while (group_of[x] != x) x = group_of[x] = group_of[group_of[x]];
       return x;
     };
-    for (uint64_t p = 0; p < P; ++p) {
+    for (uint64_t p = 0; have_query && p < P; ++p) {
       const uint32_t a = pair_img1[p], b = pair_img2[p];
       if (skip[p] || !is_query[a] || !is_query[b]) continue;
       if (!joint) {
@@ -591,18 +674,22 @@ int main(int argc, char** argv) {
     };
     for (uint64_t p = 0; p < P; ++p) {
       const uint32_t a = pair_img1[p], b = pair_img2[p];
-      if (skip[p] || !(is_query[a] || is_query[b])) {
+      if (skip[p] || (have_query && !(is_query[a] || is_query[b]))) {
         skip[p] = 1;
         pair_img1[p] = pair_img2[p] = 0;  // never read: skipped pairs name no image of the stage
         continue;
       }
-      const uint32_t g = find(is_query[a] ? a : b);
+      const uint32_t g = have_query ? find(is_query[a] ? a : b) : pair_scene[p];
       pair_img1[p] = sub(g, a);
       pair_img2[p] = sub(g, b);
     }
     if (orig_of.size() > 65535) {
-      std::fprintf(stderr, "ERROR: --query_images: the sub-scenes hold %zu images, more than 65535; split the query list "
-                           "over several runs\n", orig_of.size());
+      if (have_query)
+        std::fprintf(stderr, "ERROR: --query_images: the sub-scenes hold %zu images, more than 65535; split the query list "
+                             "over several runs\n", orig_of.size());
+      else
+        std::fprintf(stderr, "ERROR: --additional_scenes: the scenes hold %zu images, more than 65535; split the scene list "
+                             "over several runs\n", orig_of.size());
       return 2;
     }
   } else {
@@ -648,7 +735,7 @@ int main(int argc, char** argv) {
   in.n_pairs = P; in.n_matches = M; in.n_images = n_ids;
   in.pair_img1 = pair_img1.data(); in.pair_img2 = pair_img2.data(); in.pair_skip = skip.data();
   in.pair_ptr = pair_ptr.data();
-  in.image_group = have_query ? image_group.data() : nullptr;
+  in.image_group = have_query || have_scenes ? image_group.data() : nullptr;
 
   // ---- which graph stage: the library's size rule, or LFR_GRAPH_STAGE=host|device (a test and
   // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
@@ -657,7 +744,8 @@ int main(int argc, char** argv) {
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
                                  lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
                                  lfr_plan_update_solution && lfr_plan_update_solution_since && lfr_plan_problem_record &&
-                                 lfr_plan_update_solution_since_record && lfr_plan_encode_solution_images;
+                                 lfr_plan_update_solution_since_record && lfr_plan_encode_solution_images &&
+                                 lfr_plan_encode_solution_groups;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -927,6 +1015,8 @@ int main(int argc, char** argv) {
   int64_t need = 0;
   uint8_t* out = nullptr;
   bool out_pinned = false;
+  // scene sc's SolutionFile is out[scene_off[sc], scene_off[sc + 1])
+  std::vector<uint64_t> scene_off(S + 1, 0), scene_outside(S, 0);
   if (plan) {
     // encoded on the GPU, names and facts indexed by image id, into page-locked memory sized by the
     // largest encoding: a Displacement record is at most 18 bytes, an Image's header 16 plus its name field
@@ -940,6 +1030,9 @@ int main(int argc, char** argv) {
                                                             start_file.size(), o, c, &n_outside, nullptr)
                          : have_query ? lfr_plan_encode_solution_images(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
                                                                         image_fact.data(), image_written.data(), o, c, &n_outside)
+                         : have_scenes ? lfr_plan_encode_solution_groups(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
+                                                                         image_fact.data(), image_group.data(), S, o, c,
+                                                                         scene_off.data(), scene_outside.data())
                          : lfr_plan_encode_solution(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
                                                     image_fact.data(), o, c, &n_outside);
     };
@@ -960,6 +1053,10 @@ int main(int argc, char** argv) {
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", (int)need, lfr_last_error());
       return 2;
     }
+    if (have_scenes)
+      for (uint64_t c : scene_outside) n_outside += c;
+    else
+      scene_off[1] = (uint64_t)need;
   } else {
     // with --query_images only the query images are written (a database image's keypoints have one value
     // per query): rank -2 marks the images left out; every node still counts towards n_outside
@@ -974,6 +1071,19 @@ int main(int argc, char** argv) {
         rank[node_image[v]] = (int64_t)img_ids.size();
         img_ids.push_back(node_image[v]);
       }
+    // with --additional_scenes the images go scene after scene, each scene's in the order above
+    std::vector<size_t> scene_img(S + 1, 0);
+    if (have_scenes) {
+      std::stable_sort(img_ids.begin(), img_ids.end(),
+                       [&](uint32_t x, uint32_t y) { return image_group[x] < image_group[y]; });
+      for (size_t i = 0; i < img_ids.size(); ++i) {
+        rank[img_ids[i]] = (int64_t)i;
+        ++scene_img[image_group[img_ids[i]] + 1];
+      }
+      for (uint32_t sc = 0; sc < S; ++sc) scene_img[sc + 1] += scene_img[sc];
+    } else {
+      scene_img[1] = img_ids.size();
+    }
     const size_t I = img_ids.size();
     std::vector<uint64_t> img_ptr(I + 1, 0);
     for (uint32_t v = 0; v < N; ++v)
@@ -1002,25 +1112,34 @@ int main(int argc, char** argv) {
       fact[i] = image_fact[img_ids[i]];
     }
     if (out_blob.empty()) out_blob.push_back(0);
-    auto encode = [&](uint8_t* o, uint64_t c) {
-      return carry_start ? lfr_wire_encode_solution_carried(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
-                                                            feature_idx.data(), di.data(), dj.data(), start_file.data(),
-                                                            start_file.size(), o, c, nullptr)
-                         : lfr_wire_encode_solution(I, img_ptr.data(), out_blob.data(), out_off.data(), fact.data(),
-                                                    feature_idx.data(), di.data(), dj.data(), o, c);
+    // the images [a, b) of the output order: one scene's SolutionFile
+    auto encode = [&](size_t a, size_t b, uint8_t* o, uint64_t c) {
+      return carry_start ? lfr_wire_encode_solution_carried(b - a, img_ptr.data() + a, out_blob.data(), out_off.data() + a,
+                                                            fact.data() + a, feature_idx.data(), di.data(), dj.data(),
+                                                            start_file.data(), start_file.size(), o, c, nullptr)
+                         : lfr_wire_encode_solution(b - a, img_ptr.data() + a, out_blob.data(), out_off.data() + a,
+                                                    fact.data() + a, feature_idx.data(), di.data(), dj.data(), o, c);
     };
-    need = encode(nullptr, 0);
+    for (uint32_t sc = 0; sc < S && need >= 0; ++sc) {
+      const int64_t n = encode(scene_img[sc], scene_img[sc + 1], nullptr, 0);
+      need = n < 0 ? -1 : need + n;
+      scene_off[sc + 1] = (uint64_t)need;
+    }
     out = static_cast<uint8_t*>(std::malloc((size_t)std::max<int64_t>(need, 1)));
-    if (need < 0 || encode(out, (uint64_t)need) != need) need = -1;
+    for (uint32_t sc = 0; sc < S && need >= 0; ++sc) {
+      const uint64_t n = scene_off[sc + 1] - scene_off[sc];
+      if (encode(scene_img[sc], scene_img[sc + 1], out + scene_off[sc], n) != (int64_t)n) need = -1;
+    }
   }
   start_file.release();
   std::printf("# points with at least one coordinate > 0.5: %llu\n", (unsigned long long)n_outside);  // solve.cc:670
   std::fflush(stdout);
   bool written = need >= 0;
-  if (written) {
-    std::ofstream f(output_file, std::ios::binary | std::ios::trunc);
+  for (uint32_t sc = 0; written && sc < S; ++sc) {  // in scene order; the first failure ends the run
+    std::ofstream f(scenes[sc].second, std::ios::binary | std::ios::trunc);
     written = f.good();
-    if (written && need) f.write(reinterpret_cast<const char*>(out), need);
+    const uint64_t n = scene_off[sc + 1] - scene_off[sc];
+    if (written && n) f.write(reinterpret_cast<const char*>(out + scene_off[sc]), (std::streamsize)n);
     written = written && f.good();
   }
   if (positions_pinned) lfr_host_free(positions); else std::free(positions);

@@ -137,27 +137,38 @@ class MatchSet:
                     raise ValueError("the pair '%s' - '%s' names two query images" % (ms.image_names[a], ms.image_names[b]))
                 ra, rb = find(a), find(b)
                 group_of[max(ra, rb)] = min(ra, rb)
-        keep, img1, img2, group, orig_of, ids = [], [], [], [], [], {}
+        keep = [p for p, (a, b) in enumerate(pairs) if is_q[a] or is_q[b]]
+        return _sub_scenes(ms, keep, [find(a if is_q[a] else b) for a, b in (pairs[p] for p in keep)])
 
-        def sub(g, i):
-            if (g, i) not in ids:
-                ids[(g, i)] = len(orig_of)
-                orig_of.append(i)
-                group.append(g)
-            return ids[(g, i)]
+    @staticmethod
+    def join_scenes(scenes: List["MatchSet"], banned_images=()):
+        """--additional_scenes: (the kept pairs of all `scenes` as one MatchSet, image_group).  Scene s's pairs
+        follow scene s-1's; the banned images (by name) are dropped from every scene; each scene gets its own
+        id for every image it holds, in order of first appearance, by query_subscenes' rule with the scene
+        index as the label, so scenes that reuse image names share no node and each sub-scene is what a run on
+        that scene alone stages."""
+        kept = [s.without_images(banned_images) for s in scenes] + [MatchSet.empty()]
+        names, label, ptr, base, m0 = [], [], [np.zeros(1, np.int64)], 0, 0
+        for k, s in enumerate(kept):
+            names += s.image_names
+            label += [k] * s.n_pairs
+            ptr.append(s.pair_ptr[1:].astype(np.int64) + m0)
+            m0 += s.n_matches
+        offs = np.cumsum([0] + [len(s.image_names) for s in kept])
+        cat = lambda f, dt: np.concatenate([getattr(s, f) for s in kept]).astype(dt)
+        flat = MatchSet(names, np.concatenate([s.pair_img1.astype(np.int64) + o for s, o in zip(kept, offs)]),
+                        np.concatenate([s.pair_img2.astype(np.int64) + o for s, o in zip(kept, offs)]),
+                        cat("pair_fact1", np.float32), cat("pair_fact2", np.float32), np.concatenate(ptr),
+                        cat("feat1", np.uint32), cat("feat2", np.uint32), cat("sim", np.float32),
+                        cat("disp1", np.float32).reshape(-1, 18), cat("disp2", np.float32).reshape(-1, 18))
+        return _sub_scenes(flat, list(range(flat.n_pairs)), label)
 
-        for p, (a, b) in enumerate(pairs):
-            if not (is_q[a] or is_q[b]):
-                continue
-            g = find(a if is_q[a] else b)
-            keep.append(p)
-            img1.append(sub(g, a))
-            img2.append(sub(g, b))
-        out = ms.select_pairs(np.array(keep, dtype=np.int64))
-        out.image_names = [ms.image_names[i] for i in orig_of]
-        out.pair_img1 = np.array(img1, dtype=np.int64)
-        out.pair_img2 = np.array(img2, dtype=np.int64)
-        return out, np.array(group, dtype=np.uint32)
+    @staticmethod
+    def empty() -> "MatchSet":
+        """A MatchingFile with no pair: what the reference reads when the matches file is missing."""
+        return MatchSet([], np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32),
+                        np.zeros(0, np.float32), np.zeros(1, np.int64), np.zeros(0, np.uint32), np.zeros(0, np.uint32),
+                        np.zeros(0, np.float32), np.zeros((0, 18), np.float32), np.zeros((0, 18), np.float32))
 
     @staticmethod
     def concatenate(parts: List["MatchSet"]) -> "MatchSet":
@@ -206,3 +217,26 @@ class MatchSet:
             disp2=(np.concatenate([ms.disp2 for ms in parts]) if parts else np.zeros((0, 18), np.float32)),
             meta=dict(parts[0].meta) if parts else {},
         )
+
+
+def _sub_scenes(ms: MatchSet, keep, label):
+    """The pairs `keep` of `ms` (in order), pair keep[k] in the sub-scene labelled label[k]: every sub-scene
+    gets its own id for each image it holds, in order of first appearance.  Returns (the MatchSet, whose
+    image_names repeat a name once per sub-scene that holds it, image_group[id] = the label)."""
+    img1, img2, group, orig_of, ids = [], [], [], [], {}
+
+    def sub(g, i):
+        if (g, i) not in ids:
+            ids[(g, i)] = len(orig_of)
+            orig_of.append(i)
+            group.append(g)
+        return ids[(g, i)]
+
+    for p, g in zip(keep, label):
+        img1.append(sub(g, int(ms.pair_img1[p])))
+        img2.append(sub(g, int(ms.pair_img2[p])))
+    out = ms.select_pairs(np.array(keep, dtype=np.int64))
+    out.image_names = [ms.image_names[i] for i in orig_of]
+    out.pair_img1 = np.array(img1, dtype=np.int64)
+    out.pair_img2 = np.array(img2, dtype=np.int64)
+    return out, np.array(group, dtype=np.uint32)

@@ -67,6 +67,44 @@ def assemble_solution(p: Problem, positions: np.ndarray, written: Optional[np.nd
     )
 
 
+def assemble_scene_solutions(p: Problem, positions: np.ndarray, image_group: np.ndarray, n_groups: int) -> List[Solution]:
+    """--additional_scenes: the Solution of every group g < n_groups (image_group[id] = the group of image id),
+    each equal to assemble_solution(p, positions, written=image_group == g) with n_outside counted on the
+    group's own nodes; one sort of the images by (group, first node) for all groups."""
+    g = p.graph
+    N = g.n_nodes
+    empty = Solution([], np.zeros(0, np.float32), np.zeros(1, np.uint64), np.zeros(0, np.uint32),
+                     np.zeros(0, np.float32), np.zeros(0, np.float32), 0)
+    if N == 0:
+        return [dataclasses.replace(empty) for _ in range(n_groups)]
+    image_group = np.asarray(image_group, dtype=np.int64)
+    img_ids, first = np.unique(g.node_image, return_index=True)
+    order = np.lexsort((first, image_group[img_ids]))
+    img_ids = img_ids[order]                      # by group, then by first node appearance
+    pos = np.asarray(positions, dtype=np.float64).reshape(N, 2)
+    node_group = image_group[g.node_image]
+    outside = (np.abs(pos[:, 1]) > 0.5) | (np.abs(pos[:, 0]) > 0.5)
+    n_out = np.bincount(node_group[outside], minlength=n_groups)
+    rank = np.full(int(g.node_image.max()) + 1, -1, dtype=np.int64)
+    rank[img_ids] = np.arange(img_ids.shape[0])
+    node_rank = rank[g.node_image]
+    perm = np.argsort(node_rank, kind="stable")   # nodes by image in output order, ascending node index
+    node_ptr = np.zeros(img_ids.shape[0] + 1, dtype=np.int64)
+    np.cumsum(np.bincount(node_rank, minlength=img_ids.shape[0]), out=node_ptr[1:])
+    img_bound = np.searchsorted(image_group[img_ids], np.arange(n_groups + 1))
+    feat, di, dj = g.node_feat[perm].astype(np.uint32), pos[perm, 0].astype(np.float32), pos[perm, 1].astype(np.float32)
+    out = []
+    for k in range(n_groups):
+        a, b = int(img_bound[k]), int(img_bound[k + 1])
+        lo, hi = int(node_ptr[a]), int(node_ptr[b])
+        ids = img_ids[a:b].tolist()
+        out.append(Solution(image_names=[g.image_names[i] for i in ids],
+                            fact=np.array([g.image_fact[i] for i in ids], dtype=np.float32),
+                            img_ptr=(node_ptr[a:b + 1] - lo).astype(np.uint64), feature_idx=feat[lo:hi], di=di[lo:hi],
+                            dj=dj[lo:hi], n_outside=int(n_out[k])))
+    return out
+
+
 def solve_problem(p: Problem, options=None, positions: Optional[np.ndarray] = None):
     """One lfr_solve call on the CUDA library.  Returns (positions [N,2], stats)."""
     from .capi import load_b200
@@ -147,7 +185,8 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
            solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None, fixed_images=(),
            initial_solution: Optional[bytes] = None, keep_initial_solution: bool = False,
            update_initial_solution: bool = False, previous_matches=None, previous_record: Optional[bytes] = None,
-           record_problem: bool = False, query_images=None, joint_queries: bool = False):
+           record_problem: bool = False, query_images=None, joint_queries: bool = False,
+           image_group: Optional[np.ndarray] = None):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
     may be supplied to drive a different executor (the multi-GPU path; give `n_devices`); with a start
     solution it is called as `solve_fn(problem, positions)`.
@@ -180,7 +219,10 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     pair that names two query images, or sub-scenes of more than 65535 images in all, raise ValueError too.
     `joint_queries` (needs `query_images`) refines queries that a kept pair names together (sequences, rigs) in
     one sub-scene: a group is a connected component of the queries under such pairs, and each query's Image
-    message is the one a run on its group's pairs alone writes."""
+    message is the one a run on its group's pairs alone writes.
+
+    `image_group` ([n_images], MatchSet.join_scenes) stages every group of ids as a scene of its own, as
+    refine_scenes() does; it excludes query_images (ValueError)."""
     from .capi import Plan, load_b200
     from .graph import host_input_arrays, problem_from_stage
     if keep_initial_solution and initial_solution is None:
@@ -202,6 +244,8 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
             raise ValueError("malformed problem record")
     if joint_queries and query_images is None:
         raise ValueError("joint_queries needs query_images")
+    if image_group is not None and query_images is not None:
+        raise ValueError("image_group and query_images exclude each other")
     if query_images is not None:
         for on, what in ((update_initial_solution, "update_initial_solution"), (previous_matches is not None, "previous_matches"),
                          (previous_record is not None, "previous_record"), (record_problem, "record_problem")):
@@ -217,7 +261,7 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
         queries = set(query_images)
         written = np.array([n in queries for n in ms.image_names], dtype=bool)
     else:
-        image_group = written = None
+        written = None
     if isinstance(previous_matches, (bytes, bytearray, memoryview)):
         from .wire import decode_matching_file
         previous_matches = decode_matching_file(bytes(previous_matches))
@@ -267,3 +311,26 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     sol = assemble_solution(p, pos, written)
     sol.record = record
     return p, pos, st, sol
+
+
+def refine_scenes(match_sets: List[MatchSet], banned_images=(), options=None, log: Optional[Callable[[str], None]] = None,
+                  solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None,
+                  solutions: Optional[list] = None) -> List[bytes]:
+    """--additional_scenes: refine many scenes in one run and return one SolutionFile per scene, each byte for
+    byte what refine() + wire.encode_solution write for that scene alone with the same `banned_images` (names,
+    applied to every scene).  The scenes are one ordinary run (MatchSet.join_scenes: every scene a sub-scene
+    with its own image ids), so its route, `log` lines and statistics are those of the whole batch: the counts
+    are the sums over the scenes' own runs and the maxima their maxima.  `solutions`, when given, receives
+    every scene's Solution (its n_outside is the scene's own count).  More than 65535 image ids over all
+    scenes raise ValueError."""
+    from .wire import encode_solution
+    ms, image_group = MatchSet.join_scenes(match_sets, banned_images)
+    if len(ms.image_names) > 65535:
+        raise ValueError("additional_scenes: the scenes hold %d images, more than 65535; split the scene list over "
+                         "several runs" % len(ms.image_names))
+    p, pos, _, _ = refine(ms, (), options, log=log, solve_fn=solve_fn, n_devices=n_devices, timing=timing,
+                          image_group=image_group)
+    sols = assemble_scene_solutions(p, pos, image_group, len(match_sets))
+    if solutions is not None:
+        solutions.extend(sols)
+    return [encode_solution(s.image_names, s.fact, s.img_ptr, s.feature_idx, s.di, s.dj) for s in sols]
