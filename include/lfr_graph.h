@@ -66,6 +66,24 @@ int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* par
                               const lfr_options* o, const double* initial_positions /* [2N] or NULL */,
                               lfr_plan** out, lfr_host_sizes* sizes);
 
+/* lfr_plan_create_from_wire() for a batch whose pairs are listed out of one MatchingFile (--listed_pairs): the
+ * file's matches are decoded once on the device, in file order, and the batch's match arrays are then built
+ * there from the entry list.  Entry k (k < in->n_pairs) is the file's pair pair_src[k] (< n_src_pairs); entries
+ * may repeat and reorder pairs.  src_pair_ptr [n_src_pairs + 1] is the file's pair level from
+ * lfr_wire_walk_matches() over the parts in order (global match offsets, as in->pair_ptr of
+ * lfr_plan_create_from_wire()); the parts' n_matches add up to src_pair_ptr[n_src_pairs].  `in` carries the
+ * batch's pair level: entry k's images and sub-scene (pair_img1/2, pair_skip, image_group) and pair_ptr, which
+ * must be the exclusive scan of the entries' match counts (in->n_matches its total).  The expand is a scan of
+ * those counts on the device and a gather that copies each match's feature indices, similarity and two
+ * 18-float grids to its entry, bit for bit, so the result is bitwise lfr_plan_create_from_matches() on the
+ * host decode of the file with every entry's matches copied into place.  Errors: those of
+ * lfr_plan_create_from_wire(), and LFR_EINVAL for NULL arrays, a source pair out of range, a decreasing
+ * src_pair_ptr or a pair_ptr that is not that scan. */
+int lfr_plan_create_from_wire_listed(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
+                                     const uint64_t* src_pair_ptr, uint64_t n_src_pairs, const uint64_t* pair_src,
+                                     const lfr_options* o, const double* initial_positions /* [2N] or NULL */,
+                                     lfr_plan** out, lfr_host_sizes* sizes);
+
 /* Copy the stage's arrays of a plan made by lfr_plan_create_from_matches() or _from_wire() into caller-owned arrays;
  * the arguments mean what they mean in lfr_host_stage_export() (any pointer may be NULL; `edges` is a
  * device-to-host copy).  LFR_EINVAL for a plan made by lfr_plan_create(). */

@@ -83,7 +83,8 @@ GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "l
                  "lfr_plan_encode_solution", "lfr_graph_stage_on_device", "lfr_wire_decode_on_device",
                  "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution",
                  "lfr_plan_encode_solution_carried", "lfr_plan_update_solution", "lfr_plan_update_solution_since",
-                 "lfr_plan_problem_record", "lfr_plan_update_solution_since_record", "lfr_plan_encode_solution_groups"]
+                 "lfr_plan_problem_record", "lfr_plan_update_solution_since_record", "lfr_plan_encode_solution_groups",
+                 "lfr_plan_create_from_wire_listed"]
 
 
 class LfrWirePart(C.Structure):
@@ -147,6 +148,10 @@ class Library:
                                                     C.POINTER(LfrOptions), C.c_void_p, C.POINTER(C.c_void_p),
                                                     C.POINTER(HostSizes)]
             L.lfr_plan_create_from_wire.restype = C.c_int
+            L.lfr_plan_create_from_wire_listed.argtypes = [C.POINTER(HostInput), C.POINTER(LfrWirePart), C.c_uint32,
+                                                           C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(LfrOptions),
+                                                           C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(HostSizes)]
+            L.lfr_plan_create_from_wire_listed.restype = C.c_int
             L.lfr_plan_export_graph.argtypes = [C.c_void_p] * 11
             L.lfr_plan_export_graph.restype = C.c_int
             L.lfr_plan_encode_solution.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -448,6 +453,81 @@ class Plan:
         self.sizes = {k: getattr(sz, k) for k in HOST_SIZES_FIELDS}
         self.n_nodes, self.n_components = int(sz.n_nodes), int(sz.n_components)
         self.image_names = names
+        return self
+
+    @classmethod
+    def from_wire_listed(cls, lib: Library, parts, match_lists, banned_images=(), options: Optional[LfrOptions] = None,
+                         positions: Optional[np.ndarray] = None) -> "Plan":
+        """lfr_plan_create_from_wire_listed (include/lfr_graph.h): the plan of from_matches() on the batch of
+        solver.refine_lists() — MatchSet.join_scenes() of every list's pairs, the banned images dropped — built
+        from the bytes of one MatchingFile (`parts`, as for from_wire()) decoded once on the device and expanded
+        there into the lists' pairs.  `match_lists` as in refine_lists(): (name1, name2) lines, or None for every
+        pair of the file.  `self.image_names` and `self.image_group` are the batch's names and list labels by
+        image id.  Raises matchset.UnheldPairError for a line whose pair the file does not hold."""
+        from . import wire
+        from .matchset import MatchSet, sub_scene_ids
+        if not lib.has_graph_stage:  # e.g. the CPU oracle: no device, no plans
+            raise RuntimeError("lfr: lfr_plan_create_from_wire_listed failed (-5): %s does not provide the graph "
+                               "stage on the GPU (include/lfr_graph.h)" % lib.path)
+        names, index = [], {}
+        img1, img2, ptr, keep = [], [], [np.zeros(1, np.uint64)], []
+        wparts = (LfrWirePart * max(len(parts), 1))()
+        m0 = 0
+        for i, data in enumerate(parts):
+            a = wire.walk_matching_file(data)
+            i1, i2 = wire.intern_names(data, a, names, index)
+            img1.append(i1)
+            img2.append(i2)
+            ptr.append(a["pair_ptr"][1:] + np.uint64(m0))
+            buf = np.frombuffer(data, dtype=np.uint8)
+            keep += [buf, a["match_off"]]
+            n = int(a["match_off"].shape[0])
+            wparts[i] = LfrWirePart(buf=buf.ctypes.data if buf.size else None, len=buf.size,
+                                    match_off=a["match_off"].ctypes.data if n else None, n_matches=n)
+            m0 += n
+        cat = lambda xs: np.concatenate(xs) if xs else np.zeros(0, np.int64)  # noqa: E731
+        file_img1, file_img2 = cat(img1).astype(np.int64), cat(img2).astype(np.int64)
+        src_ptr = np.ascontiguousarray(np.concatenate(ptr), dtype=np.uint64)
+        P = file_img1.shape[0]
+        z = np.zeros(P, np.float32)
+        pairs = MatchSet(names, file_img1, file_img2, z, z, src_ptr.astype(np.int64), np.zeros(0, np.uint32),
+                         np.zeros(0, np.uint32), np.zeros(0, np.float32), np.zeros((0, 18), np.float32),
+                         np.zeros((0, 18), np.float32))
+        banned = set(banned_images)
+        kept = np.array([names[x] not in banned and names[y] not in banned for x, y in
+                         zip(file_img1.tolist(), file_img2.tolist())], dtype=bool).reshape(-1)
+        src, label = [], []
+        for k, lines in enumerate(match_lists):
+            idx = np.arange(P) if lines is None else pairs.listed_pair_index(lines)
+            idx = idx[kept[idx]]
+            src.append(idx)
+            label += [k] * idx.shape[0]
+        pair_src = np.ascontiguousarray(cat(src), dtype=np.uint64)
+        e1, e2, orig_of, group = sub_scene_ids(file_img1[pair_src.astype(np.int64)], file_img2[pair_src.astype(np.int64)],
+                                               label)
+        counts = (src_ptr[1:] - src_ptr[:-1])[pair_src.astype(np.int64)]
+        pair_ptr = np.zeros(pair_src.shape[0] + 1, np.uint64)
+        np.cumsum(counts, out=pair_ptr[1:])
+        arrs = dict(pair_img1=e1.astype(np.uint32), pair_img2=e2.astype(np.uint32),
+                    pair_skip=np.zeros(pair_src.shape[0], np.uint8), pair_ptr=pair_ptr, image_group=group)
+        inp = HostInput(n_pairs=pair_src.shape[0], n_matches=int(pair_ptr[-1]), n_images=len(orig_of),
+                        **{k: (v.ctypes.data if v.size else None) for k, v in arrs.items()})
+        o = options if options is not None else lib.default_options()
+        init = None if positions is None else np.ascontiguousarray(positions, dtype=np.float64)
+        self = cls.__new__(cls)
+        self.lib, self.problem, self.handle = lib, None, None
+        h = C.c_void_p()
+        sz = HostSizes()
+        lib.check(lib.lib.lfr_plan_create_from_wire_listed(C.byref(inp), wparts, len(parts), src_ptr.ctypes.data, P,
+                                                           _ptr(pair_src) if pair_src.size else None, C.byref(o),
+                                                           _ptr(init), C.byref(h), C.byref(sz)),
+                  "lfr_plan_create_from_wire_listed")
+        del keep
+        self.handle = h
+        self.sizes = {k: getattr(sz, k) for k in HOST_SIZES_FIELDS}
+        self.n_nodes, self.n_components = int(sz.n_nodes), int(sz.n_components)
+        self.image_names = [names[i] for i in orig_of]
+        self.image_group = group
         return self
 
     def export_graph(self) -> dict:

@@ -37,6 +37,9 @@ refines it (solver.refine(joint_queries=True)).
 --additional_scenes FILE (lines `MATCHES_FILE<TAB>OUTPUT_FILE`) refines many scenes in one run: the scene of
 --matches_file / --output_file and every listed one, each output file byte for byte what that scene's own run
 writes (solver.refine_scenes).
+--listed_pairs FILE (lines `MATCH_LIST<TAB>OUTPUT_FILE`) refines the pairs of many match lists (`NAME1 NAME2` per
+line, as compute_match_graph.py reads them) out of --matches_file in one run: each output file byte for byte
+what the run on a MatchingFile of that list's pairs in line order writes (solver.refine_lists).
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -75,7 +78,8 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("keep_initial_solution", False, False), ("carry_initial_solution", False, False),
             ("update_initial_solution", False, False), ("previous_matches_file", True, False),
             ("record_file", True, False), ("earlier_record_file", True, False), ("query_images", True, True),
-            ("joint_queries", False, False), ("additional_scenes", True, False)]
+            ("joint_queries", False, False), ("additional_scenes", True, False),
+            ("listed_pairs", True, False)]
 
 
 def _find_option(name):
@@ -156,7 +160,7 @@ def parse_args(argv):
             previous_matches_file=vals.get("previous_matches_file"),
             record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"),
             query_images=vals.get("query_images"), joint_queries=bool(vals.get("joint_queries")),
-            additional_scenes=vals.get("additional_scenes"))
+            additional_scenes=vals.get("additional_scenes"), listed_pairs=vals.get("listed_pairs"))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -192,6 +196,94 @@ def read_scene_list(path, matches_file, output_file):
             return b"ERROR: --additional_scenes: two scenes write '%s'\n" % o
         seen.add(o)
     return [(os.fsdecode(m), os.fsdecode(o)) for m, o in scenes]
+
+
+def read_pair_lists(path, output_file):
+    """--listed_pairs FILE: [(match list path or None, output file, [(name1, name2)] or None)], list 0 being every
+    pair of --matches_file written to `output_file`, or the bytes of the one ERROR line for an unreadable file,
+    a malformed line, two lists with the same output path, an unreadable match list or a malformed line of one
+    (lfr_solve_main.cc writes the same lines, in the same order).  A match list's line is split as
+    compute_match_graph.py:97 splits it: the newline stripped, split on single spaces, exactly two fields."""
+    try:
+        with open(path, "rb") as fh:
+            text = fh.read()
+    except OSError:
+        return b"ERROR: cannot read the pair list file '%s'\n" % os.fsencode(path)
+    lists = [(None, os.fsencode(output_file))]
+    lines = text.split(b"\n")
+    if lines[-1] == b"":
+        lines.pop()
+    for k, line in enumerate(lines, 1):
+        why = ("it is empty" if not line else "it has no TAB" if b"\t" not in line
+               else "it has more than one TAB" if line.count(b"\t") > 1
+               else "its match list is empty" if line.startswith(b"\t")
+               else "its output file is empty" if line.endswith(b"\t")
+               else "it holds a NUL byte" if b"\0" in line else None)
+        if why:
+            return b"ERROR: --listed_pairs: line %d is not MATCH_LIST<TAB>OUTPUT_FILE: %s\n" % (k, why.encode())
+        lists.append(tuple(line.split(b"\t")))
+    seen = set()
+    for _, o in lists:
+        if o in seen:
+            return b"ERROR: --listed_pairs: two lists write '%s'\n" % o
+        seen.add(o)
+    out = [(None, output_file, None)]
+    for k, (m, o) in enumerate(lists[1:], 1):
+        try:
+            with open(m, "rb") as fh:
+                t = fh.read()
+        except OSError:
+            return b"ERROR: --listed_pairs: line %d: cannot read the match list '%s'\n" % (k, m)
+        rows = t.split(b"\n")
+        if rows[-1] == b"":
+            rows.pop()
+        pairs = []
+        for j, row in enumerate(rows, 1):
+            f = row.split(b" ")
+            if len(f) != 2:
+                return (b"ERROR: --listed_pairs: line %d of the match list '%s' is not NAME1 NAME2: it has %d fields\n"
+                        % (j, m, len(f)))
+            pairs.append(tuple(x.decode("utf-8", errors="surrogateescape") for x in f))
+        out.append((os.fsdecode(m), os.fsdecode(o), pairs))
+    return out
+
+
+def _run_lists(args, lists, ms, opts, say, solve_fn, n_devices, timing, t_start) -> int:
+    """--listed_pairs after the lists were read: one refine_lists() run, the stdout lines once, then the output
+    files in list order."""
+    from .matchset import UnheldPairError
+    from .solver import GraphStageRouteError, refine_lists
+    sols = []
+    try:
+        data = refine_lists(ms, [pairs for _, _, pairs in lists], args.banned_images, opts, log=say, solve_fn=solve_fn,
+                            n_devices=n_devices, timing=timing, solutions=sols)
+    except UnheldPairError as e:
+        enc = lambda x: x.encode("utf-8", errors="surrogateescape")  # noqa: E731
+        msg = b"ERROR: --listed_pairs: line %d of the match list '%s': the matches file holds no pair '%s' '%s'" % (
+            e.line, os.fsencode(lists[e.list][0]), enc(e.name1), enc(e.name2))
+        if e.reverse:
+            msg += b"; it holds only '%s' '%s'" % (enc(e.name2), enc(e.name1))
+        sys.stderr.flush()
+        sys.stderr.buffer.write(msg + b"\n")
+        sys.stderr.buffer.flush()
+        return 2
+    except GraphStageRouteError as e:
+        sys.stderr.write("ERROR: %s\n" % e)
+        return 2
+    except ValueError as e:   # more than 65535 image ids
+        sys.stderr.write("ERROR: --%s\n" % e)
+        return 2
+    say("Solver time: %dms" % int(timing.get("solver_ms", 0.0)))                       # solve.cc:638
+    say("Total time: %dms" % int((time.perf_counter() - t_start) * 1e3))               # solve.cc:641
+    say("# points with at least one coordinate > 0.5: %d" % sum(s.n_outside for s in sols))   # solve.cc:670
+    try:
+        for (_, out, _), d in zip(lists, data):
+            with open(out, "wb") as fh:
+                fh.write(d)
+    except OSError:
+        sys.stderr.write("Failed to write proto object.\n")
+        return 255
+    return 0
 
 
 def _run_scenes(args, scenes, ms, opts, say, solve_fn, n_devices, timing, t_start) -> int:
@@ -263,6 +355,26 @@ def main(argv=None) -> int:
     if args.joint_queries and args.query_images is None:
         sys.stderr.write("ERROR: --joint_queries needs --query_images\n")
         return 2
+    lists = None
+    if args.listed_pairs is not None:   # as --additional_scenes, whose batches it excludes too
+        for on, opt in ((bool(args.fixed_images), "--fixed_images"), (args.initial_solution is not None, "--initial_solution"),
+                        (args.keep_initial_solution, "--keep_initial_solution"),
+                        (args.carry_initial_solution, "--carry_initial_solution"),
+                        (args.update_initial_solution, "--update_initial_solution"),
+                        (args.previous_matches_file is not None, "--previous_matches_file"),
+                        (args.record_file is not None, "--record_file"),
+                        (args.earlier_record_file is not None, "--earlier_record_file"),
+                        (args.query_images is not None, "--query_images"), (args.joint_queries, "--joint_queries"),
+                        (args.additional_scenes is not None, "--additional_scenes")):
+            if on:
+                sys.stderr.write("ERROR: --listed_pairs and %s exclude each other\n" % opt)
+                return 2
+        lists = read_pair_lists(args.listed_pairs, args.output_file)
+        if isinstance(lists, bytes):
+            sys.stderr.flush()
+            sys.stderr.buffer.write(lists)
+            sys.stderr.buffer.flush()
+            return 2
     scenes = None
     if args.additional_scenes is not None:
         for on, opt in ((bool(args.fixed_images), "--fixed_images"), (args.initial_solution is not None, "--initial_solution"),
@@ -380,6 +492,11 @@ def main(argv=None) -> int:
     if torchrun and scenes is not None:
         sys.stderr.write("ERROR: --additional_scenes: torchrun ranks do not refine scene batches; use --gpus N\n")
         return 2
+    if torchrun and lists is not None:
+        sys.stderr.write("ERROR: --listed_pairs: torchrun ranks do not refine list batches; use --gpus N\n")
+        return 2
+    if lists is not None:
+        return _run_lists(args, lists, ms, opts, say, solve_fn, n_devices, timing, t_start)
     if scenes is not None:
         return _run_scenes(args, scenes, ms, opts, say, solve_fn, n_devices, timing, t_start)
     try:

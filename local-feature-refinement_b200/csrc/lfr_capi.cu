@@ -1821,6 +1821,37 @@ int decode_wire_on_device(const lfr_host_input* in, const lfr_wire_part* parts, 
   return LFR_OK;
 }
 
+// lfr_plan_create_from_wire_listed(): the batch's match arrays `d` (M matches) from the file's, `src`, decoded
+// once in file order.  A scan of the entries' match counts gives each entry's first match; one block per
+// entry then copies its source pair's matches there, bit for bit.
+int expand_listed_on_device(const uint64_t* src_pair_ptr, uint64_t n_src, const uint64_t* pair_src, uint64_t n,
+                            uint64_t M, const MatchArrays& src, MatchArrays& d, cudaStream_t s) {
+  LFR_TRY(d.feat1.reserve(4 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.feat2.reserve(4 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.sim.reserve(4 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.disp1.reserve(72 * std::max<size_t>(M, 1)));
+  LFR_TRY(d.disp2.reserve(72 * std::max<size_t>(M, 1)));
+  if (!M) return LFR_OK;
+  TmpBuf d_sptr, d_psrc, d_cnt, d_dst, tmp;
+  LFR_TRY(upload(&d_sptr, src_pair_ptr, n_src + 1, s));
+  LFR_TRY(upload(&d_psrc, pair_src, n, s));
+  LFR_TRY(d_cnt.reserve(8 * (n + 1)));
+  LFR_TRY(d_dst.reserve(8 * (n + 1)));
+  uint64_t* cnt = d_cnt.as<uint64_t>();
+  uint64_t* dst = d_dst.as<uint64_t>();
+  lfr::wire::listed_counts_kernel<<<blocks_for(n + 1), 256, 0, s>>>(d_sptr.as<uint64_t>(), d_psrc.as<uint64_t>(), n, cnt);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, cnt, dst, (int)n + 1, s); }));
+  const unsigned grid = (unsigned)std::min<uint64_t>(n, 1u << 30);
+  lfr::wire::listed_gather_kernel<<<grid, 256, 0, s>>>(
+      d_sptr.as<uint64_t>(), d_psrc.as<uint64_t>(), dst, n, src.feat1.as<uint32_t>(), src.feat2.as<uint32_t>(),
+      src.sim.as<uint32_t>(), src.disp1.as<uint2>(), src.disp2.as<uint2>(), d.feat1.as<uint32_t>(),
+      d.feat2.as<uint32_t>(), d.sim.as<uint32_t>(), d.disp1.as<uint2>(), d.disp2.as<uint2>());
+  LFR_LAUNCHED();
+  LFR_CUDA(cudaStreamSynchronize(s));  // before the scratch buffers and `src` are freed
+  return LFR_OK;
+}
+
 // The two entry points from matches: the stage on the device-resident `d`, then the plan.
 int create_plan_from_graph(const lfr_host_input* in, MatchArrays& d, const lfr_options& o, const double* initial_positions,
                            lfr_plan* pl, lfr_host_sizes* S) {
@@ -2773,6 +2804,55 @@ int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* par
   lfr_host_sizes S;
   MatchArrays d;
   int rc = decode_wire_on_device(in, parts, n_parts, d, 0);
+  if (rc == LFR_OK) rc = create_plan_from_graph(in, d, o, initial_positions, pl, &S);
+  if (rc) {
+    free_plan(pl);
+    return rc;
+  }
+  if (sizes) *sizes = S;
+  *out = pl;
+  return LFR_OK;
+}
+
+int lfr_plan_create_from_wire_listed(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
+                                     const uint64_t* src_pair_ptr, uint64_t n_src_pairs, const uint64_t* pair_src,
+                                     const lfr_options* opt, const double* initial_positions, lfr_plan** out,
+                                     lfr_host_sizes* sizes) {
+  if (!out) return fail(LFR_EINVAL, "out is NULL");
+  *out = nullptr;
+  if (!in) return fail(LFR_EINVAL, "input is NULL");
+  if (n_parts && !parts) return fail(LFR_EINVAL, "parts is NULL");
+  if (!src_pair_ptr || (in->n_pairs && (!pair_src || !in->pair_ptr)))
+    return fail(LFR_EINVAL, "NULL src_pair_ptr, pair_src or pair_ptr");
+  // the entries against the file's pair level: every source pair exists, and in->pair_ptr is the scan of
+  // the entries' match counts (the stage reads it on the host; the expand computes it on the device)
+  if (src_pair_ptr[0] != 0) return fail(LFR_EINVAL, "src_pair_ptr[0] is not 0");
+  for (uint64_t p = 0; p < n_src_pairs; ++p)
+    if (src_pair_ptr[p + 1] < src_pair_ptr[p]) return fail(LFR_EINVAL, "src_pair_ptr decreases");
+  if (in->n_pairs && in->pair_ptr[0] != 0) return fail(LFR_EINVAL, "pair_ptr[0] is not 0");
+  for (uint64_t k = 0; k < in->n_pairs; ++k) {
+    if (pair_src[k] >= n_src_pairs) return fail(LFR_EINVAL, "a listed pair's source is out of range");
+    if (in->pair_ptr[k + 1] - in->pair_ptr[k] != src_pair_ptr[pair_src[k] + 1] - src_pair_ptr[pair_src[k]])
+      return fail(LFR_EINVAL, "pair_ptr is not the scan of the listed pairs' match counts");
+  }
+  if ((in->n_pairs ? in->pair_ptr[in->n_pairs] : 0) != in->n_matches)
+    return fail(LFR_EINVAL, "pair_ptr does not end at n_matches");
+  if (in->n_matches && in->n_pairs + 1 > (uint64_t)INT32_MAX) return fail(LFR_EUNSUPPORTED, "2^31 or more listed pairs");
+  lfr_options o;
+  if (opt) o = *opt; else lfr_options_default(&o);
+  LFR_TRY(select_device(o));
+  lfr_plan* pl = new lfr_plan();
+  pl->device = o.device;
+  lfr_host_sizes S;
+  MatchArrays d;
+  int rc;
+  {
+    lfr_host_input file_in = *in;  // the decoder sees the file's matches
+    file_in.n_matches = src_pair_ptr[n_src_pairs];
+    MatchArrays src;
+    rc = decode_wire_on_device(&file_in, parts, n_parts, src, 0);
+    if (rc == LFR_OK) rc = expand_listed_on_device(src_pair_ptr, n_src_pairs, pair_src, in->n_pairs, in->n_matches, src, d, 0);
+  }
   if (rc == LFR_OK) rc = create_plan_from_graph(in, d, o, initial_positions, pl, &S);
   if (rc) {
     free_plan(pl);

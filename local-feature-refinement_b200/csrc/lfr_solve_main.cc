@@ -42,7 +42,10 @@
 // that a kept pair names together share one sub-scene, so sequences and rigs are refined jointly) and
 // --additional_scenes FILE (lines `MATCHES_FILE<TAB>OUTPUT_FILE`: every listed scene is one more sub-scene of the
 // same run, and each scene's output file holds what its own run writes: lfr_plan_encode_solution_groups() on
-// the device route).  `--n_threads` is accepted and
+// the device route) and --listed_pairs FILE (lines `MATCH_LIST<TAB>OUTPUT_FILE`: the pairs of every match list,
+// one `NAME1 NAME2` per line, are taken out of --matches_file, and each list's output file holds what the run on
+// a MatchingFile of those pairs in line order writes: lfr_plan_create_from_wire_listed() expands the file's
+// matches, decoded once, on the device route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <algorithm>
@@ -58,6 +61,7 @@
 #include <set>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include <sys/mman.h>
@@ -80,6 +84,10 @@ int lfr_plan_create_from_matches(const lfr_host_input* in, const lfr_options* o,
 int lfr_plan_create_from_wire(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
                               const lfr_options* o, const double* initial_positions, lfr_plan** out,
                               lfr_host_sizes* sizes) __attribute__((weak));
+int lfr_plan_create_from_wire_listed(const lfr_host_input* in, const lfr_wire_part* parts, uint32_t n_parts,
+                                     const uint64_t* src_pair_ptr, uint64_t n_src_pairs, const uint64_t* pair_src,
+                                     const lfr_options* o, const double* initial_positions, lfr_plan** out,
+                                     lfr_host_sizes* sizes) __attribute__((weak));
 int64_t lfr_plan_encode_solution(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
                                  const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
                                  uint64_t* n_outside) __attribute__((weak));
@@ -140,7 +148,7 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"update_initial_solution", false, false}, {"previous_matches_file", true, false},
                                {"record_file", true, false},  {"earlier_record_file", true, false},
                                {"query_images", true, true},  {"joint_queries", false, false},
-                               {"additional_scenes", true, false}};
+                               {"additional_scenes", true, false}, {"listed_pairs", true, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -386,6 +394,84 @@ int read_scene_list(const std::string& path, std::vector<std::pair<std::string, 
   return 0;
 }
 
+// One --listed_pairs entry: a match list's path, its output file and its lines (NAME1, NAME2); `all` is list 0,
+// every pair of --matches_file in file order.
+struct PairList {
+  std::string path, output;
+  std::vector<std::pair<std::string, std::string>> lines;
+  bool all = false;
+};
+
+// The --listed_pairs file: one `MATCH_LIST<TAB>OUTPUT_FILE` per line (the rules of read_scene_list), appended to
+// `lists` after list 0, then every match list read and split as compute_match_graph.py:97 splits it (the
+// newline stripped, single spaces; exactly two fields).  0, or 2 after one ERROR line for an unreadable file, a
+// malformed line, two lists (the first one included) with the same output path, an unreadable match list or a
+// malformed line of one, in that order.
+int read_pair_lists(const std::string& path, std::vector<PairList>& lists) {
+  FileImage f;
+  if (!f.open(path)) {
+    std::fprintf(stderr, "ERROR: cannot read the pair list file '%s'\n", path.c_str());
+    return 2;
+  }
+  const std::string text(reinterpret_cast<const char*>(f.data()), f.size());
+  f.release();
+  size_t line = 0;
+  for (size_t at = 0; at < text.size();) {
+    ++line;
+    const size_t end = std::min(text.find('\n', at), text.size());
+    const std::string l = text.substr(at, end - at);
+    at = end + 1;
+    const size_t tab = l.find('\t');
+    const char* why = l.empty()                                  ? "it is empty"
+                      : tab == std::string::npos                 ? "it has no TAB"
+                      : l.find('\t', tab + 1) != std::string::npos ? "it has more than one TAB"
+                      : tab == 0                                 ? "its match list is empty"
+                      : tab + 1 == l.size()                      ? "its output file is empty"
+                      : l.find('\0') != std::string::npos        ? "it holds a NUL byte"
+                                                                 : nullptr;
+    if (why) {
+      std::fprintf(stderr, "ERROR: --listed_pairs: line %zu is not MATCH_LIST<TAB>OUTPUT_FILE: %s\n", line, why);
+      return 2;
+    }
+    PairList pl;
+    pl.path = l.substr(0, tab);
+    pl.output = l.substr(tab + 1);
+    lists.push_back(std::move(pl));
+  }
+  std::set<std::string> outputs;
+  for (const PairList& pl : lists)
+    if (!outputs.insert(pl.output).second) {
+      std::fprintf(stderr, "ERROR: --listed_pairs: two lists write '%s'\n", pl.output.c_str());
+      return 2;
+    }
+  for (size_t i = 1; i < lists.size(); ++i) {
+    PairList& pl = lists[i];
+    FileImage g;
+    if (!g.open(pl.path)) {
+      std::fprintf(stderr, "ERROR: --listed_pairs: line %zu: cannot read the match list '%s'\n", i, pl.path.c_str());
+      return 2;
+    }
+    const std::string t(reinterpret_cast<const char*>(g.data()), g.size());
+    g.release();
+    size_t j = 0;
+    for (size_t at = 0; at < t.size();) {
+      ++j;
+      const size_t end = std::min(t.find('\n', at), t.size());
+      const std::string l = t.substr(at, end - at);
+      at = end + 1;
+      const size_t fields = 1 + (size_t)std::count(l.begin(), l.end(), ' ');
+      if (fields != 2) {
+        std::fprintf(stderr, "ERROR: --listed_pairs: line %zu of the match list '%s' is not NAME1 NAME2: it has %zu fields\n",
+                     j, pl.path.c_str(), fields);
+        return 2;
+      }
+      const size_t sp = l.find(' ');
+      pl.lines.emplace_back(l.substr(0, sp), l.substr(sp + 1));
+    }
+  }
+  return 0;
+}
+
 using Clock = std::chrono::steady_clock;
 long long ms_between(Clock::time_point a, Clock::time_point b) {
   return (long long)std::chrono::duration_cast<std::chrono::milliseconds>(b - a).count();
@@ -395,11 +481,12 @@ long long ms_between(Clock::time_point a, Clock::time_point b) {
 
 int main(int argc, char** argv) {
   std::string matches_file, output_file, initial_solution, previous_matches_file, record_file, earlier_record_file,
-      scene_list;
+      scene_list, list_file;
   std::vector<std::string> banned_list, fixed_list, query_list;
   uint64_t device = 0, gpus = 1;
   bool keep_start = false, carry_start = false, update_start = false, have_previous = false, have_record = false,
-       have_earlier = false, have_query = false, joint = false, have_scenes = false;
+       have_earlier = false, have_query = false, joint = false, have_scenes = false,
+       have_lists = false;
   try {
     Args a = parse(argc, argv);
     if (a.help) {
@@ -431,6 +518,8 @@ int main(int argc, char** argv) {
     if (have_earlier) earlier_record_file = a.single.at("earlier_record_file");
     have_scenes = a.single.count("additional_scenes") != 0;
     if (have_scenes) scene_list = a.single.at("additional_scenes");
+    have_lists = a.single.count("listed_pairs") != 0;
+    if (have_lists) list_file = a.single.at("listed_pairs");
   } catch (const CliError& e) {  // solve.cc:397-401
     std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
     std::fputs(kUsage, stderr);
@@ -482,6 +571,27 @@ int main(int argc, char** argv) {
     std::fputs("ERROR: --joint_queries needs --query_images\n", stderr);
     return 2;
   }
+  // --listed_pairs: list 0 is every pair of --matches_file, written to --output_file; the listed match lists
+  // follow.  Each list's output is what its own run writes: the same command on a MatchingFile that holds the
+  // file's pair for every line of the list, in line order.
+  std::vector<PairList> lists(1);
+  lists[0].output = output_file;
+  lists[0].all = true;
+  if (have_lists) {  // as --additional_scenes, whose batches it excludes too
+    for (const auto& o : {std::make_pair(!fixed_list.empty(), "--fixed_images"), std::make_pair(have_start, "--initial_solution"),
+                          std::make_pair(keep_start, "--keep_initial_solution"),
+                          std::make_pair(carry_start, "--carry_initial_solution"),
+                          std::make_pair(update_start, "--update_initial_solution"),
+                          std::make_pair(have_previous, "--previous_matches_file"), std::make_pair(have_record, "--record_file"),
+                          std::make_pair(have_earlier, "--earlier_record_file"), std::make_pair(have_query, "--query_images"),
+                          std::make_pair(joint, "--joint_queries"), std::make_pair(have_scenes, "--additional_scenes")})
+      if (o.first) {
+        std::fprintf(stderr, "ERROR: --listed_pairs and %s exclude each other\n", o.second);
+        return 2;
+      }
+    const int rc = read_pair_lists(list_file, lists);
+    if (rc) return rc;
+  }
   // --additional_scenes: the scene of --matches_file / --output_file is scene 0, the listed ones follow; each
   // scene's output is what its own run writes (the same command with that scene's two files alone)
   std::vector<std::pair<std::string, std::string>> scenes{{matches_file, output_file}};
@@ -500,7 +610,7 @@ int main(int argc, char** argv) {
     const int rc = read_scene_list(scene_list, scenes);
     if (rc) return rc;
   }
-  const uint32_t S = (uint32_t)scenes.size();
+  uint32_t S = (uint32_t)scenes.size();  // the batch's members: scenes, or with --listed_pairs the lists
   if (have_start) {
     if (!start_file.open(initial_solution)) {
       std::fprintf(stderr, "ERROR: cannot read the initial solution file '%s'\n", initial_solution.c_str());
@@ -626,6 +736,65 @@ int main(int argc, char** argv) {
     }
   }
 
+  // --listed_pairs: the batch's pairs are the lists' lines, list after list, each the first pair of the file
+  // with exactly those two names (one map over the pairs, names as bytes); every pair of the file for list 0.
+  // pair_src is the file's pair behind each of them, whose matches are copied to it after the decode.
+  const uint64_t M_file = M;  // the matches the decode reads: the file's
+  std::vector<uint64_t> pair_src, file_pair_ptr;
+  if (have_lists) {
+    std::unordered_map<uint64_t, uint64_t> first;  // image1 << 32 | image2 -> the first pair
+    for (uint64_t p = 0; p < P; ++p) first.emplace((uint64_t)pair_img1[p] << 32 | pair_img2[p], p);
+    std::vector<uint32_t> list_of;
+    for (size_t l = 0; l < lists.size(); ++l) {
+      if (lists[l].all) {
+        for (uint64_t p = 0; p < P; ++p) {
+          pair_src.push_back(p);
+          list_of.push_back((uint32_t)l);
+        }
+        continue;
+      }
+      for (size_t j = 0; j < lists[l].lines.size(); ++j) {
+        const std::string& n1 = lists[l].lines[j].first;
+        const std::string& n2 = lists[l].lines[j].second;
+        const auto i1 = id_of.find(n1), i2 = id_of.find(n2);
+        auto hit = first.end();
+        bool reverse = false;
+        if (i1 != id_of.end() && i2 != id_of.end()) {
+          hit = first.find((uint64_t)i1->second << 32 | i2->second);
+          reverse = first.count((uint64_t)i2->second << 32 | i1->second) != 0;
+        }
+        if (hit == first.end()) {
+          std::fprintf(stderr, "ERROR: --listed_pairs: line %zu of the match list '%s': the matches file holds no pair '%s' '%s'",
+                       j + 1, lists[l].path.c_str(), n1.c_str(), n2.c_str());
+          if (reverse) std::fprintf(stderr, "; it holds only '%s' '%s'", n2.c_str(), n1.c_str());
+          std::fputs("\n", stderr);
+          return 2;
+        }
+        pair_src.push_back(hit->second);
+        list_of.push_back((uint32_t)l);
+      }
+    }
+    const uint64_t Q = pair_src.size();
+    std::vector<uint32_t> img1(Q), img2(Q);
+    std::vector<float> f1(Q), f2(Q);
+    std::vector<uint64_t> ptr(Q + 1, 0);
+    for (uint64_t k = 0; k < Q; ++k) {
+      const uint64_t p = pair_src[k];
+      img1[k] = pair_img1[p]; img2[k] = pair_img2[p]; f1[k] = pair_fact1[p]; f2[k] = pair_fact2[p];
+      ptr[k + 1] = ptr[k] + (pair_ptr[p + 1] - pair_ptr[p]);
+    }
+    pair_img1.swap(img1); pair_img2.swap(img2); pair_fact1.swap(f1); pair_fact2.swap(f2);
+    file_pair_ptr.swap(pair_ptr);
+    pair_ptr.swap(ptr);
+    pair_scene.swap(list_of);
+    P = Q;
+    M = pair_ptr[Q];
+    scenes.clear();  // from here on the batch's members are the lists
+    for (const PairList& pl : lists) scenes.emplace_back(pl.path, pl.output);
+    S = (uint32_t)scenes.size();
+  }
+  const bool batched = have_scenes || have_lists;
+
   // banned images (solve.cc:444-446)
   const std::set<std::string> banned(banned_list.begin(), banned_list.end());
   std::vector<uint8_t> skip(P, 0);
@@ -638,11 +807,12 @@ int main(int argc, char** argv) {
   // that name two of them (with or without matches).  The graph stage then gives every sub-scene what a run
   // on its pairs alone gives (lfr_host_input::image_group).  --additional_scenes: the same rule with every
   // kept pair in its scene's sub-scene, labelled by the scene index, so that scenes that share image names
-  // share no node and each meta-component is cut at its own scene's image count.
+  // share no node and each meta-component is cut at its own scene's image count.  --listed_pairs: the same with
+  // the list index as the label, so a pair listed by two lists is a node set of each.
   // orig_of: the original image id (and name) of every stage image id; the identity without sub-scenes.
   std::vector<uint8_t> is_query(names.size(), 0);
   std::vector<uint32_t> orig_of, image_group;
-  if (have_query || have_scenes) {
+  if (have_query || batched) {
     const std::set<std::string> queries(query_list.begin(), query_list.end());
     for (size_t i = 0; i < names.size(); ++i) is_query[i] = queries.count(names[i]) ? 1 : 0;
     // the group of every query image: a union-find whose root is the group's lowest image id, its label.  It
@@ -686,6 +856,9 @@ int main(int argc, char** argv) {
     if (orig_of.size() > 65535) {
       if (have_query)
         std::fprintf(stderr, "ERROR: --query_images: the sub-scenes hold %zu images, more than 65535; split the query list "
+                             "over several runs\n", orig_of.size());
+      else if (have_lists)
+        std::fprintf(stderr, "ERROR: --listed_pairs: the lists hold %zu images, more than 65535; split the pair list "
                              "over several runs\n", orig_of.size());
       else
         std::fprintf(stderr, "ERROR: --additional_scenes: the scenes hold %zu images, more than 65535; split the scene list "
@@ -735,7 +908,7 @@ int main(int argc, char** argv) {
   in.n_pairs = P; in.n_matches = M; in.n_images = n_ids;
   in.pair_img1 = pair_img1.data(); in.pair_img2 = pair_img2.data(); in.pair_skip = skip.data();
   in.pair_ptr = pair_ptr.data();
-  in.image_group = have_query || have_scenes ? image_group.data() : nullptr;
+  in.image_group = have_query || batched ? image_group.data() : nullptr;
 
   // ---- which graph stage: the library's size rule, or LFR_GRAPH_STAGE=host|device (a test and
   // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
@@ -745,7 +918,7 @@ int main(int argc, char** argv) {
                                  lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
                                  lfr_plan_update_solution && lfr_plan_update_solution_since && lfr_plan_problem_record &&
                                  lfr_plan_update_solution_since_record && lfr_plan_encode_solution_images &&
-                                 lfr_plan_encode_solution_groups;
+                                 lfr_plan_encode_solution_groups && lfr_plan_create_from_wire_listed;
   bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (force && *force) {
@@ -768,12 +941,14 @@ int main(int argc, char** argv) {
   }
 
   // host route, and the device route below the library's size for the decoder on the GPU: the matches of
-  // every part decoded into one set of arrays, part after part (the pair level comes out as the walk gave it)
-  const bool decode_on_device = on_device && lfr_wire_decode_on_device(M) == 1;
+  // every part decoded into one set of arrays, part after part (the pair level comes out as the walk gave it).
+  // With --listed_pairs the file is decoded once and every listed pair's matches are then copied into place;
+  // the decoder's threshold sees the file's match count.
+  const bool decode_on_device = on_device && lfr_wire_decode_on_device(M_file) == 1;
   std::vector<uint32_t> feat1, feat2;
   std::vector<float> sim, disp1, disp2;
   if (!decode_on_device) {
-    feat1.resize(M); feat2.resize(M); sim.resize(M); disp1.resize(18 * M); disp2.resize(18 * M);
+    feat1.resize(M_file); feat2.resize(M_file); sim.resize(M_file); disp1.resize(18 * M_file); disp2.resize(18 * M_file);
     uint64_t m0 = 0;
     for (Part& pt : parts) {
       lfr_wire_matches w = pt.pair_level(feat1.data() + m0, feat2.data() + m0, sim.data() + m0, disp1.data() + 18 * m0,
@@ -784,6 +959,19 @@ int main(int argc, char** argv) {
       }
       m0 += pt.M;
       pt.buf.release();  // the file image (several GB at Madrid scale) is not needed past the decode
+    }
+    if (have_lists) {
+      std::vector<uint32_t> e1(M), e2(M);
+      std::vector<float> es(M), ed1(18 * M), ed2(18 * M);
+      for (uint64_t k = 0; k < P; ++k) {
+        const uint64_t a = file_pair_ptr[pair_src[k]], c = pair_ptr[k + 1] - pair_ptr[k], b = pair_ptr[k];
+        std::copy_n(feat1.begin() + a, c, e1.begin() + b);
+        std::copy_n(feat2.begin() + a, c, e2.begin() + b);
+        std::copy_n(sim.begin() + a, c, es.begin() + b);
+        std::copy_n(disp1.begin() + 18 * a, 18 * c, ed1.begin() + 18 * b);
+        std::copy_n(disp2.begin() + 18 * a, 18 * c, ed2.begin() + 18 * b);
+      }
+      feat1.swap(e1); feat2.swap(e2); sim.swap(es); disp1.swap(ed1); disp2.swap(ed2);
     }
     in.feat1 = feat1.data(); in.feat2 = feat2.data(); in.sim = sim.data(); in.disp1 = disp1.data(); in.disp2 = disp2.data();
   }
@@ -808,7 +996,10 @@ int main(int argc, char** argv) {
     }
     std::vector<lfr_wire_part> wparts;
     for (const Part& pt : parts) wparts.push_back(lfr_wire_part{pt.buf.data(), pt.buf.size(), pt.match_off.data(), pt.M});
-    const int rc = decode_on_device
+    const int rc = decode_on_device && have_lists
+                       ? lfr_plan_create_from_wire_listed(&in, wparts.data(), (uint32_t)wparts.size(), file_pair_ptr.data(),
+                                                          file_pair_ptr.size() - 1, pair_src.data(), &opt, nullptr, &plan, &sz)
+                   : decode_on_device
                        ? lfr_plan_create_from_wire(&in, wparts.data(), (uint32_t)wparts.size(), &opt, nullptr, &plan, &sz)
                        : lfr_plan_create_from_matches(&in, &opt, nullptr, &plan, &sz);
     for (Part& pt : parts) pt.buf.release();
@@ -1030,7 +1221,7 @@ int main(int argc, char** argv) {
                                                             start_file.size(), o, c, &n_outside, nullptr)
                          : have_query ? lfr_plan_encode_solution_images(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
                                                                         image_fact.data(), image_written.data(), o, c, &n_outside)
-                         : have_scenes ? lfr_plan_encode_solution_groups(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
+                         : batched ? lfr_plan_encode_solution_groups(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
                                                                          image_fact.data(), image_group.data(), S, o, c,
                                                                          scene_off.data(), scene_outside.data())
                          : lfr_plan_encode_solution(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
@@ -1053,7 +1244,7 @@ int main(int argc, char** argv) {
       std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", (int)need, lfr_last_error());
       return 2;
     }
-    if (have_scenes)
+    if (batched)
       for (uint64_t c : scene_outside) n_outside += c;
     else
       scene_off[1] = (uint64_t)need;
@@ -1071,9 +1262,9 @@ int main(int argc, char** argv) {
         rank[node_image[v]] = (int64_t)img_ids.size();
         img_ids.push_back(node_image[v]);
       }
-    // with --additional_scenes the images go scene after scene, each scene's in the order above
+    // with --additional_scenes (--listed_pairs) the images go scene (list) after scene, each one's in the order above
     std::vector<size_t> scene_img(S + 1, 0);
-    if (have_scenes) {
+    if (batched) {
       std::stable_sort(img_ids.begin(), img_ids.end(),
                        [&](uint32_t x, uint32_t y) { return image_group[x] < image_group[y]; });
       for (size_t i = 0; i < img_ids.size(); ++i) {

@@ -119,5 +119,43 @@ __global__ void __launch_bounds__(256) decode_matches_kernel(const uint8_t* __re
   if (!r.ok || !read_match(mm, m0 + i, feat1, feat2, sim, disp1, disp2)) *err = 1;
 }
 
+// Listed pairs (lfr_plan_create_from_wire_listed): entry k of the batch holds the matches of the file's pair
+// pair_src[k], decoded once in file order.  cnt[k] = that pair's match count for k < n, cnt[n] = 0, so an
+// exclusive scan of cnt[0..n] gives every entry's first match and the total.
+__global__ void __launch_bounds__(256) listed_counts_kernel(const uint64_t* __restrict__ src_ptr,
+                                                            const uint64_t* __restrict__ pair_src, uint64_t n,
+                                                            uint64_t* __restrict__ cnt) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k > n) return;
+  cnt[k] = k < n ? src_ptr[pair_src[k] + 1] - src_ptr[pair_src[k]] : 0;
+}
+
+// One block per entry: its source pair's matches are copied to dst_ptr[k].. as raw words (feature indices,
+// the similarity's bits and the two 18-float grids as 9 eight-byte words each), so the copy is bit for bit.
+// Both ranges are contiguous, so consecutive threads touch consecutive words.
+__global__ void __launch_bounds__(256) listed_gather_kernel(const uint64_t* __restrict__ src_ptr,
+                                                            const uint64_t* __restrict__ pair_src,
+                                                            const uint64_t* __restrict__ dst_ptr, uint64_t n,
+                                                            const uint32_t* __restrict__ s_feat1,
+                                                            const uint32_t* __restrict__ s_feat2,
+                                                            const uint32_t* __restrict__ s_sim,
+                                                            const uint2* __restrict__ s_disp1,
+                                                            const uint2* __restrict__ s_disp2, uint32_t* __restrict__ feat1,
+                                                            uint32_t* __restrict__ feat2, uint32_t* __restrict__ sim,
+                                                            uint2* __restrict__ disp1, uint2* __restrict__ disp2) {
+  for (uint64_t k = blockIdx.x; k < n; k += gridDim.x) {
+    const uint64_t a = src_ptr[pair_src[k]], c = src_ptr[pair_src[k] + 1] - a, b = dst_ptr[k];
+    for (uint64_t i = threadIdx.x; i < c; i += blockDim.x) {
+      feat1[b + i] = s_feat1[a + i];
+      feat2[b + i] = s_feat2[a + i];
+      sim[b + i] = s_sim[a + i];
+    }
+    for (uint64_t i = threadIdx.x; i < 9 * c; i += blockDim.x) {
+      disp1[9 * b + i] = s_disp1[9 * a + i];
+      disp2[9 * b + i] = s_disp2[9 * a + i];
+    }
+  }
+}
+
 }  // namespace wire
 }  // namespace lfr

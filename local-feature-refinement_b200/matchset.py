@@ -140,6 +140,28 @@ class MatchSet:
         keep = [p for p, (a, b) in enumerate(pairs) if is_q[a] or is_q[b]]
         return _sub_scenes(ms, keep, [find(a if is_q[a] else b) for a, b in (pairs[p] for p in keep)])
 
+    def listed_pair_index(self, lines) -> np.ndarray:
+        """--listed_pairs: the index of the pair that each line (name1, name2) of a match list names, in line
+        order: the first pair whose image_name1 is name1 and image_name2 is name2 exactly.  A repeated line
+        gives its pair again.  Raises UnheldPairError for the first line whose pair the set does not hold (a
+        pair held only the other way round is not that pair: the network computes each direction on its own
+        crops)."""
+        first = {}
+        for p, (a, b) in enumerate(zip(self.pair_img1.tolist(), self.pair_img2.tolist())):
+            first.setdefault((self.image_names[a], self.image_names[b]), p)
+        idx = []
+        for k, (n1, n2) in enumerate(lines, 1):
+            p = first.get((n1, n2))
+            if p is None:
+                raise UnheldPairError(k, n1, n2, (n2, n1) in first)
+            idx.append(p)
+        return np.array(idx, dtype=np.int64)
+
+    def select_listed_pairs(self, lines) -> "MatchSet":
+        """The MatchingFile a run of the two-view network over the match list `lines` ((name1, name2) per line)
+        writes, taken from this superset: one pair per line, in line order (listed_pair_index)."""
+        return self.select_pairs(self.listed_pair_index(lines))
+
     @staticmethod
     def join_scenes(scenes: List["MatchSet"], banned_images=()):
         """--additional_scenes: (the kept pairs of all `scenes` as one MatchSet, image_group).  Scene s's pairs
@@ -219,10 +241,33 @@ class MatchSet:
         )
 
 
+class UnheldPairError(ValueError):
+    """A match-list line whose pair the MatchingFile does not hold: `line` counts from 1; `reverse` says whether
+    the file holds the pair the other way round."""
+
+    def __init__(self, line: int, name1: str, name2: str, reverse: bool):
+        super().__init__("line %d: the matches file holds no pair '%s' '%s'%s"
+                         % (line, name1, name2, "; it holds only '%s' '%s'" % (name2, name1) if reverse else ""))
+        self.line, self.name1, self.name2, self.reverse = line, name1, name2, reverse
+
+
 def _sub_scenes(ms: MatchSet, keep, label):
     """The pairs `keep` of `ms` (in order), pair keep[k] in the sub-scene labelled label[k]: every sub-scene
     gets its own id for each image it holds, in order of first appearance.  Returns (the MatchSet, whose
     image_names repeat a name once per sub-scene that holds it, image_group[id] = the label)."""
+    keep = np.array(keep, dtype=np.int64)
+    img1, img2, orig_of, group = sub_scene_ids(ms.pair_img1[keep], ms.pair_img2[keep], label)
+    out = ms.select_pairs(keep)
+    out.image_names = [ms.image_names[i] for i in orig_of]
+    out.pair_img1 = img1
+    out.pair_img2 = img2
+    return out, group
+
+
+def sub_scene_ids(pair_img1, pair_img2, label):
+    """The id rule of _sub_scenes on the pair level alone: pair k in the sub-scene label[k] gets, on each side,
+    that sub-scene's id for the image, handed out in order of first appearance.  Returns (pair_img1, pair_img2,
+    orig_of: the original image of every id, image_group: the label of every id)."""
     img1, img2, group, orig_of, ids = [], [], [], [], {}
 
     def sub(g, i):
@@ -232,11 +277,7 @@ def _sub_scenes(ms: MatchSet, keep, label):
             group.append(g)
         return ids[(g, i)]
 
-    for p, g in zip(keep, label):
-        img1.append(sub(g, int(ms.pair_img1[p])))
-        img2.append(sub(g, int(ms.pair_img2[p])))
-    out = ms.select_pairs(np.array(keep, dtype=np.int64))
-    out.image_names = [ms.image_names[i] for i in orig_of]
-    out.pair_img1 = np.array(img1, dtype=np.int64)
-    out.pair_img2 = np.array(img2, dtype=np.int64)
-    return out, np.array(group, dtype=np.uint32)
+    for a, b, g in zip(np.asarray(pair_img1).tolist(), np.asarray(pair_img2).tolist(), list(label)):
+        img1.append(sub(g, a))
+        img2.append(sub(g, b))
+    return (np.array(img1, dtype=np.int64), np.array(img2, dtype=np.int64), orig_of, np.array(group, dtype=np.uint32))

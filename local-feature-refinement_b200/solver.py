@@ -323,14 +323,43 @@ def refine_scenes(match_sets: List[MatchSet], banned_images=(), options=None, lo
     are the sums over the scenes' own runs and the maxima their maxima.  `solutions`, when given, receives
     every scene's Solution (its n_outside is the scene's own count).  More than 65535 image ids over all
     scenes raise ValueError."""
+    return _refine_batch(match_sets, banned_images, options, log, solve_fn, n_devices, timing, solutions,
+                         "additional_scenes: the scenes hold %d images, more than 65535; split the scene list over "
+                         "several runs")
+
+
+def _refine_batch(match_sets, banned_images, options, log, solve_fn, n_devices, timing, solutions, too_many: str):
+    """refine_scenes() and refine_lists(): `too_many` % n_ids is the ValueError past 65535 image ids."""
     from .wire import encode_solution
     ms, image_group = MatchSet.join_scenes(match_sets, banned_images)
     if len(ms.image_names) > 65535:
-        raise ValueError("additional_scenes: the scenes hold %d images, more than 65535; split the scene list over "
-                         "several runs" % len(ms.image_names))
+        raise ValueError(too_many % len(ms.image_names))
     p, pos, _, _ = refine(ms, (), options, log=log, solve_fn=solve_fn, n_devices=n_devices, timing=timing,
                           image_group=image_group)
     sols = assemble_scene_solutions(p, pos, image_group, len(match_sets))
     if solutions is not None:
         solutions.extend(sols)
     return [encode_solution(s.image_names, s.fact, s.img_ptr, s.feature_idx, s.di, s.dj) for s in sols]
+
+
+def refine_lists(ms: MatchSet, match_lists, banned_images=(), options=None, log: Optional[Callable[[str], None]] = None,
+                 solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None,
+                 solutions: Optional[list] = None) -> List[bytes]:
+    """--listed_pairs: refine the pairs of many match lists out of one superset MatchingFile `ms` and return one
+    SolutionFile per list.  A list is a sequence of (name1, name2) lines, or None for every pair of `ms` in file
+    order.  List L's bytes are those of refine() + wire.encode_solution on the MatchingFile that holds one pair
+    per line of L in line order (MatchSet.select_listed_pairs: the first pair of `ms` with exactly those two
+    names), with the same `banned_images`.  The lists run as one scene batch (refine_scenes' code), so the
+    stdout lines and `solutions` are those of a scene batch.  A line whose pair `ms` does not hold raises
+    matchset.UnheldPairError (its `list` attribute is the list's index); more than 65535 image ids over all
+    lists raise ValueError."""
+    from .matchset import UnheldPairError
+    sets = []
+    for k, lines in enumerate(match_lists):
+        try:
+            sets.append(ms if lines is None else ms.select_listed_pairs(lines))
+        except UnheldPairError as e:
+            e.list = k
+            raise
+    return _refine_batch(sets, banned_images, options, log, solve_fn, n_devices, timing, solutions,
+                         "listed_pairs: the lists hold %d images, more than 65535; split the pair list over several runs")
