@@ -167,8 +167,9 @@ __device__ __forceinline__ double newton_quotient(double f, double df) {
 // One real root of q inside the bracket [a, b] (f(a), f(b) of opposite sign, q monotone there):
 // Newton's iteration started from the regula-falsi point of the bracket (the ends' values are
 // known, and the brackets are narrow: one grid cell or one monotone segment), kept inside the
-// shrinking bracket by a bisection step whenever Newton would leave it.  Stops after a step of
-// relative size <= 1e-8 (quadratic convergence: the error is then ~1e-16).  The oracle's fast
+// shrinking bracket by a bisection step whenever Newton would leave it.  Stops after a Newton step of
+// relative size <= 1e-8 (quadratic convergence: the error is then ~1e-16); a bisection step that short
+// only says the bracket is narrow, not that its midpoint is the root, so the iteration goes on.  The oracle's fast
 // formulation runs the same operations.
 __device__ __forceinline__ double bracket_root(const double* q, int nq, double a, double b, double fa, double fb) {
   if (fa == 0.0) return a;
@@ -186,7 +187,7 @@ __device__ __forceinline__ double bracket_root(const double* q, int nq, double a
     if (xn == x) return x;  // converged to the last bit (checked before the bracket test: x itself is one end of the bracket)
     if (!(xn >= fmin(xl, xh) && xn <= fmax(xl, xh))) {  // Newton leaves the bracket (or is not finite): bisect
       xn = 0.5 * (xl + xh);
-      dx = x - xn;
+      dx = __longlong_as_double(0x7ff8000000000000ll);  // NaN: no stop after a bisection step
     }
     if (xn == x) return x;
     x = xn;
@@ -337,7 +338,7 @@ __device__ __forceinline__ double bracket_root_loop(const double (&q)[N], double
     if (xn == x) return x;  // converged to the last bit (checked before the bracket test: x itself is one end of the bracket)
     if (!(xn >= fmin(xl, xh) && xn <= fmax(xl, xh))) {
       xn = 0.5 * (xl + xh);
-      dx = x - xn;
+      dx = __longlong_as_double(0x7ff8000000000000ll);  // NaN: no stop after a bisection step
     }
     if (xn == x) return x;
     x = xn;
@@ -403,7 +404,7 @@ __device__ __forceinline__ double cell_root_n(const double (&q)[N], double x0, d
     if (xn == x) break;
     if (!(xn >= fmin(xl, xh) && xn <= fmax(xl, xh))) {
       xn = 0.5 * (xl + xh);
-      dx = x - xn;
+      dx = __longlong_as_double(0x7ff8000000000000ll);  // NaN: no stop after a bisection step
     }
     if (xn == x) break;
     x = xn;

@@ -215,7 +215,7 @@ double newton_quotient(double f, double df) {
 
 // One real root of q inside the bracket [a, b] (opposite signs at the ends, q monotone there):
 // Newton from the regula-falsi point, bisection whenever a step would leave the shrinking bracket;
-// stops after a step of relative size <= 1e-8 (quadratic convergence: error ~1e-16 afterwards; the
+// stops after a Newton step of relative size <= 1e-8 (quadratic convergence: error ~1e-16 afterwards; the
 // 6e-8 relative error of newton_quotient only adds 6e-8 * 1e-8).  Same operations as
 // csrc/lfr_math.cuh::bracket_root.
 double bracket_root(const double* q, int nq, double a, double b, double fa, double fb) {
@@ -234,7 +234,7 @@ double bracket_root(const double* q, int nq, double a, double b, double fa, doub
     if (xn == x) return x;  // converged to the last bit (checked before the bracket test: x itself is one end of the bracket)
     if (!(xn >= std::fmin(xl, xh) && xn <= std::fmax(xl, xh))) {
       xn = 0.5 * (xl + xh);
-      dx = x - xn;
+      dx = std::numeric_limits<double>::quiet_NaN();  // no stop after a bisection step
     }
     if (xn == x) return x;
     x = xn;
