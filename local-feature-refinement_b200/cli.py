@@ -167,66 +167,98 @@ def parse_args(argv):
         raise SystemExit(1)
 
 
-def read_scene_list(path, matches_file, output_file):
-    """--additional_scenes FILE: [(matches file, output file)] of scene 0 (--matches_file / --output_file) and
-    of every line `MATCHES_FILE<TAB>OUTPUT_FILE` (raw bytes; the last newline optional), or the bytes of the one
-    ERROR line for an unreadable file, a malformed line or two scenes with the same output path (lfr_solve_main.cc
-    writes the same lines)."""
+# The rules between the opt-in options, in order: with two conflicts, the first rule that fires writes the message
+# (lfr_solve_main.cc has the same table).  (option, "needs" or "excludes", the others)
+_ONE_SCENE = ["--fixed_images", "--initial_solution", "--keep_initial_solution", "--carry_initial_solution",
+              "--update_initial_solution", "--previous_matches_file", "--record_file", "--earlier_record_file",
+              "--query_images", "--joint_queries"]   # a batch's scenes or lists exclude what belongs to one scene
+_RULES = [("--keep_initial_solution", "needs", ["--initial_solution"]),
+          ("--carry_initial_solution", "needs", ["--initial_solution"]),
+          ("--update_initial_solution", "needs", ["--initial_solution"]),
+          ("--update_initial_solution", "excludes", ["--keep_initial_solution"]),
+          ("--previous_matches_file", "needs", ["--update_initial_solution"]),
+          ("--earlier_record_file", "needs", ["--update_initial_solution"]),
+          ("--earlier_record_file", "excludes", ["--previous_matches_file"]),
+          # each query is refined against the scene as it stands; the incremental modes update one scene
+          ("--query_images", "excludes", ["--update_initial_solution", "--previous_matches_file", "--record_file",
+                                          "--earlier_record_file", "--carry_initial_solution"]),
+          ("--joint_queries", "needs", ["--query_images"]),
+          ("--listed_pairs", "excludes", _ONE_SCENE + ["--additional_scenes"]),
+          ("--additional_scenes", "excludes", _ONE_SCENE)]
+
+
+def _broken_rule(args):
+    """The ERROR line of the first rule in _RULES the command line breaks, or None.  An option is given when the
+    command line names it; a needed option must also have a value (an empty --initial_solution names no file)."""
+    value = lambda opt: getattr(args, opt[2:])  # noqa: E731
+    given = lambda opt: value(opt) not in (None, False, [])  # noqa: E731
+    for opt, kind, others in _RULES:
+        for other in (others if given(opt) else ()):
+            if kind == "needs" and not value(other):
+                return "ERROR: %s needs %s%s\n" % (opt, other, " FILE" if other == "--initial_solution" else "")
+            if kind == "excludes" and given(other):
+                return "ERROR: %s and %s exclude each other\n" % (opt, other)
+    return None
+
+
+def _lines(data):
+    """The lines of `data`; the last newline is optional."""
+    lines = data.split(b"\n")
+    if lines[-1] == b"":
+        lines.pop()
+    return lines
+
+
+# the nouns of the two list files: (option, file, first column, what an empty first column is, rows)
+_SCENE_LIST = (b"--additional_scenes", b"scene list", b"MATCHES_FILE", b"its matches file is empty", b"scenes")
+_PAIR_LIST = (b"--listed_pairs", b"pair list", b"MATCH_LIST", b"its match list is empty", b"lists")
+
+
+def _read_tab_list(path, kind, row0):
+    """The list file of --additional_scenes or --listed_pairs (`kind`): [row0] and a (first, output) row of bytes for
+    every line `FIRST<TAB>OUTPUT_FILE` (raw bytes; the last newline optional), or the bytes of the one ERROR line
+    for an unreadable file, a malformed line or two rows with the same output path (lfr_solve_main.cc writes the
+    same lines)."""
+    option, noun, first, first_empty, rows_noun = kind
     try:
         with open(path, "rb") as fh:
             text = fh.read()
     except OSError:
-        return b"ERROR: cannot read the scene list file '%s'\n" % os.fsencode(path)
-    scenes = [(os.fsencode(matches_file), os.fsencode(output_file))]
-    lines = text.split(b"\n")
-    if lines[-1] == b"":
-        lines.pop()
-    for k, line in enumerate(lines, 1):
-        why = ("it is empty" if not line else "it has no TAB" if b"\t" not in line
-               else "it has more than one TAB" if line.count(b"\t") > 1
-               else "its matches file is empty" if line.startswith(b"\t")
-               else "its output file is empty" if line.endswith(b"\t")
-               else "it holds a NUL byte" if b"\0" in line else None)
+        return b"ERROR: cannot read the %s file '%s'\n" % (noun, os.fsencode(path))
+    rows = [row0]
+    for k, line in enumerate(_lines(text), 1):
+        why = (b"it is empty" if not line else b"it has no TAB" if b"\t" not in line
+               else b"it has more than one TAB" if line.count(b"\t") > 1
+               else first_empty if line.startswith(b"\t")
+               else b"its output file is empty" if line.endswith(b"\t")
+               else b"it holds a NUL byte" if b"\0" in line else None)
         if why:
-            return b"ERROR: --additional_scenes: line %d is not MATCHES_FILE<TAB>OUTPUT_FILE: %s\n" % (k, why.encode())
-        scenes.append(tuple(line.split(b"\t")))
+            return b"ERROR: %s: line %d is not %s<TAB>OUTPUT_FILE: %s\n" % (option, k, first, why)
+        rows.append(tuple(line.split(b"\t")))
     seen = set()
-    for _, o in scenes:
+    for _, o in rows:
         if o in seen:
-            return b"ERROR: --additional_scenes: two scenes write '%s'\n" % o
+            return b"ERROR: %s: two %s write '%s'\n" % (option, rows_noun, o)
         seen.add(o)
-    return [(os.fsdecode(m), os.fsdecode(o)) for m, o in scenes]
+    return rows
+
+
+def read_scene_list(path, matches_file, output_file):
+    """--additional_scenes FILE: [(matches file, output file)] of scene 0 (--matches_file / --output_file) and
+    of every line `MATCHES_FILE<TAB>OUTPUT_FILE`, or the bytes of the one ERROR line (_read_tab_list)."""
+    scenes = _read_tab_list(path, _SCENE_LIST, (os.fsencode(matches_file), os.fsencode(output_file)))
+    return scenes if isinstance(scenes, bytes) else [(os.fsdecode(m), os.fsdecode(o)) for m, o in scenes]
 
 
 def read_pair_lists(path, output_file):
     """--listed_pairs FILE: [(match list path or None, output file, [(name1, name2)] or None)], list 0 being every
-    pair of --matches_file written to `output_file`, or the bytes of the one ERROR line for an unreadable file,
-    a malformed line, two lists with the same output path, an unreadable match list or a malformed line of one
-    (lfr_solve_main.cc writes the same lines, in the same order).  A match list's line is split as
-    compute_match_graph.py:97 splits it: the newline stripped, split on single spaces, exactly two fields."""
-    try:
-        with open(path, "rb") as fh:
-            text = fh.read()
-    except OSError:
-        return b"ERROR: cannot read the pair list file '%s'\n" % os.fsencode(path)
-    lists = [(None, os.fsencode(output_file))]
-    lines = text.split(b"\n")
-    if lines[-1] == b"":
-        lines.pop()
-    for k, line in enumerate(lines, 1):
-        why = ("it is empty" if not line else "it has no TAB" if b"\t" not in line
-               else "it has more than one TAB" if line.count(b"\t") > 1
-               else "its match list is empty" if line.startswith(b"\t")
-               else "its output file is empty" if line.endswith(b"\t")
-               else "it holds a NUL byte" if b"\0" in line else None)
-        if why:
-            return b"ERROR: --listed_pairs: line %d is not MATCH_LIST<TAB>OUTPUT_FILE: %s\n" % (k, why.encode())
-        lists.append(tuple(line.split(b"\t")))
-    seen = set()
-    for _, o in lists:
-        if o in seen:
-            return b"ERROR: --listed_pairs: two lists write '%s'\n" % o
-        seen.add(o)
+    pair of --matches_file written to `output_file`, or the bytes of the one ERROR line for what _read_tab_list
+    refuses, an unreadable match list or a malformed line of one (lfr_solve_main.cc writes the same lines, in the
+    same order).  A match list's line is split as compute_match_graph.py:97 splits it: the newline stripped, split
+    on single spaces, exactly two fields."""
+    lists = _read_tab_list(path, _PAIR_LIST, (None, os.fsencode(output_file)))
+    if isinstance(lists, bytes):
+        return lists
     out = [(None, output_file, None)]
     for k, (m, o) in enumerate(lists[1:], 1):
         try:
@@ -234,11 +266,8 @@ def read_pair_lists(path, output_file):
                 t = fh.read()
         except OSError:
             return b"ERROR: --listed_pairs: line %d: cannot read the match list '%s'\n" % (k, m)
-        rows = t.split(b"\n")
-        if rows[-1] == b"":
-            rows.pop()
         pairs = []
-        for j, row in enumerate(rows, 1):
+        for j, row in enumerate(_lines(t), 1):
             f = row.split(b" ")
             if len(f) != 2:
                 return (b"ERROR: --listed_pairs: line %d of the match list '%s' is not NAME1 NAME2: it has %d fields\n"
@@ -248,19 +277,20 @@ def read_pair_lists(path, output_file):
     return out
 
 
-def _run_lists(args, lists, ms, opts, say, solve_fn, n_devices, timing, t_start) -> int:
-    """--listed_pairs after the lists were read: one refine_lists() run, the stdout lines once, then the output
-    files in list order."""
+def _run_batch(refine_batch, inputs, rows, args, opts, say, solve_fn, n_devices, timing, t_start) -> int:
+    """--additional_scenes or --listed_pairs after the rows (scenes or lists, each with its output file second) were
+    read: one refine_batch(*inputs, ...) run (refine_scenes or refine_lists), the stdout lines once, then the output
+    files in row order."""
     from .matchset import UnheldPairError
-    from .solver import GraphStageRouteError, refine_lists
+    from .solver import GraphStageRouteError
     sols = []
     try:
-        data = refine_lists(ms, [pairs for _, _, pairs in lists], args.banned_images, opts, log=say, solve_fn=solve_fn,
-                            n_devices=n_devices, timing=timing, solutions=sols)
-    except UnheldPairError as e:
+        data = refine_batch(*inputs, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
+                            timing=timing, solutions=sols)
+    except UnheldPairError as e:   # --listed_pairs: a list line whose pair the file does not hold
         enc = lambda x: x.encode("utf-8", errors="surrogateescape")  # noqa: E731
         msg = b"ERROR: --listed_pairs: line %d of the match list '%s': the matches file holds no pair '%s' '%s'" % (
-            e.line, os.fsencode(lists[e.list][0]), enc(e.name1), enc(e.name2))
+            e.line, os.fsencode(rows[e.list][0]), enc(e.name1), enc(e.name2))
         if e.reverse:
             msg += b"; it holds only '%s' '%s'" % (enc(e.name2), enc(e.name1))
         sys.stderr.flush()
@@ -277,35 +307,8 @@ def _run_lists(args, lists, ms, opts, say, solve_fn, n_devices, timing, t_start)
     say("Total time: %dms" % int((time.perf_counter() - t_start) * 1e3))               # solve.cc:641
     say("# points with at least one coordinate > 0.5: %d" % sum(s.n_outside for s in sols))   # solve.cc:670
     try:
-        for (_, out, _), d in zip(lists, data):
-            with open(out, "wb") as fh:
-                fh.write(d)
-    except OSError:
-        sys.stderr.write("Failed to write proto object.\n")
-        return 255
-    return 0
-
-
-def _run_scenes(args, scenes, ms, opts, say, solve_fn, n_devices, timing, t_start) -> int:
-    """--additional_scenes after the scenes were read: one refine_scenes() run, the stdout lines once, then the
-    output files in scene order."""
-    from .solver import GraphStageRouteError, refine_scenes
-    sols = []
-    try:
-        data = refine_scenes([m for m, _ in scenes], args.banned_images, opts, log=say, solve_fn=solve_fn,
-                             n_devices=n_devices, timing=timing, solutions=sols)
-    except GraphStageRouteError as e:
-        sys.stderr.write("ERROR: %s\n" % e)
-        return 2
-    except ValueError as e:   # more than 65535 image ids
-        sys.stderr.write("ERROR: --%s\n" % e)
-        return 2
-    say("Solver time: %dms" % int(timing.get("solver_ms", 0.0)))                       # solve.cc:638
-    say("Total time: %dms" % int((time.perf_counter() - t_start) * 1e3))               # solve.cc:641
-    say("# points with at least one coordinate > 0.5: %d" % sum(s.n_outside for s in sols))   # solve.cc:670
-    try:
-        for (_, out), d in zip(scenes, data):
-            with open(out, "wb") as fh:
+        for row, d in zip(rows, data):
+            with open(row[1], "wb") as fh:
                 fh.write(d)
     except OSError:
         sys.stderr.write("Failed to write proto object.\n")
@@ -317,58 +320,18 @@ def main(argv=None) -> int:
     args = parse_args(sys.argv[1:] if argv is None else argv)
 
     from . import wire
-    from .solver import GraphStageRouteError, refine
+    from .solver import GraphStageRouteError, refine, refine_lists, refine_scenes
+
     from .capi import load_b200
     from .graph import refined_track_count
 
-    # the start solution is read and checked before any other work: its errors come before any output
-    if args.keep_initial_solution and not args.initial_solution:
-        sys.stderr.write("ERROR: --keep_initial_solution needs --initial_solution FILE\n")
-        return 2
-    if args.carry_initial_solution and not args.initial_solution:
-        sys.stderr.write("ERROR: --carry_initial_solution needs --initial_solution FILE\n")
-        return 2
-    if args.update_initial_solution and not args.initial_solution:
-        sys.stderr.write("ERROR: --update_initial_solution needs --initial_solution FILE\n")
-        return 2
-    if args.update_initial_solution and args.keep_initial_solution:
-        sys.stderr.write("ERROR: --update_initial_solution and --keep_initial_solution exclude each other\n")
-        return 2
-    if args.previous_matches_file is not None and not args.update_initial_solution:
-        sys.stderr.write("ERROR: --previous_matches_file needs --update_initial_solution\n")
-        return 2
-    if args.earlier_record_file is not None and not args.update_initial_solution:
-        sys.stderr.write("ERROR: --earlier_record_file needs --update_initial_solution\n")
-        return 2
-    if args.earlier_record_file is not None and args.previous_matches_file is not None:
-        sys.stderr.write("ERROR: --earlier_record_file and --previous_matches_file exclude each other\n")
-        return 2
-    if args.query_images is not None:
-        for on, opt in ((args.update_initial_solution, "--update_initial_solution"),
-                        (args.previous_matches_file is not None, "--previous_matches_file"),
-                        (args.record_file is not None, "--record_file"),
-                        (args.earlier_record_file is not None, "--earlier_record_file"),
-                        (args.carry_initial_solution, "--carry_initial_solution")):
-            if on:
-                sys.stderr.write("ERROR: --query_images and %s exclude each other\n" % opt)
-                return 2
-    if args.joint_queries and args.query_images is None:
-        sys.stderr.write("ERROR: --joint_queries needs --query_images\n")
+    # the rules, then the start solution read and checked before any other work: their errors come before any output
+    broken = _broken_rule(args)
+    if broken:
+        sys.stderr.write(broken)
         return 2
     lists = None
-    if args.listed_pairs is not None:   # as --additional_scenes, whose batches it excludes too
-        for on, opt in ((bool(args.fixed_images), "--fixed_images"), (args.initial_solution is not None, "--initial_solution"),
-                        (args.keep_initial_solution, "--keep_initial_solution"),
-                        (args.carry_initial_solution, "--carry_initial_solution"),
-                        (args.update_initial_solution, "--update_initial_solution"),
-                        (args.previous_matches_file is not None, "--previous_matches_file"),
-                        (args.record_file is not None, "--record_file"),
-                        (args.earlier_record_file is not None, "--earlier_record_file"),
-                        (args.query_images is not None, "--query_images"), (args.joint_queries, "--joint_queries"),
-                        (args.additional_scenes is not None, "--additional_scenes")):
-            if on:
-                sys.stderr.write("ERROR: --listed_pairs and %s exclude each other\n" % opt)
-                return 2
+    if args.listed_pairs is not None:
         lists = read_pair_lists(args.listed_pairs, args.output_file)
         if isinstance(lists, bytes):
             sys.stderr.flush()
@@ -377,17 +340,6 @@ def main(argv=None) -> int:
             return 2
     scenes = None
     if args.additional_scenes is not None:
-        for on, opt in ((bool(args.fixed_images), "--fixed_images"), (args.initial_solution is not None, "--initial_solution"),
-                        (args.keep_initial_solution, "--keep_initial_solution"),
-                        (args.carry_initial_solution, "--carry_initial_solution"),
-                        (args.update_initial_solution, "--update_initial_solution"),
-                        (args.previous_matches_file is not None, "--previous_matches_file"),
-                        (args.record_file is not None, "--record_file"),
-                        (args.earlier_record_file is not None, "--earlier_record_file"),
-                        (args.query_images is not None, "--query_images"), (args.joint_queries, "--joint_queries")):
-            if on:
-                sys.stderr.write("ERROR: --additional_scenes and %s exclude each other\n" % opt)
-                return 2
         scenes = read_scene_list(args.additional_scenes, args.matches_file, args.output_file)
         if isinstance(scenes, bytes):
             sys.stderr.flush()
@@ -482,23 +434,19 @@ def main(argv=None) -> int:
     # torchrun ranks and --gpus N solve a host lfr_problem: the size rule keeps them on the host route
     torchrun = "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1
     n_devices = int(os.environ["WORLD_SIZE"]) if torchrun else max(args.gpus, 1)
-    if torchrun and (args.record_file is not None or args.earlier_record_file is not None):
-        sys.stderr.write("ERROR: --record_file / --earlier_record_file: torchrun ranks do not write or read "
-                         "problem records; use --gpus N\n")
-        return 2
-    if torchrun and args.query_images is not None:
-        sys.stderr.write("ERROR: --query_images: torchrun ranks do not localize queries; use --gpus N\n")
-        return 2
-    if torchrun and scenes is not None:
-        sys.stderr.write("ERROR: --additional_scenes: torchrun ranks do not refine scene batches; use --gpus N\n")
-        return 2
-    if torchrun and lists is not None:
-        sys.stderr.write("ERROR: --listed_pairs: torchrun ranks do not refine list batches; use --gpus N\n")
-        return 2
+    for on, msg in ((args.record_file is not None or args.earlier_record_file is not None,
+                     "--record_file / --earlier_record_file: torchrun ranks do not write or read problem records"),
+                    (args.query_images is not None, "--query_images: torchrun ranks do not localize queries"),
+                    (scenes is not None, "--additional_scenes: torchrun ranks do not refine scene batches"),
+                    (lists is not None, "--listed_pairs: torchrun ranks do not refine list batches")):
+        if torchrun and on:
+            sys.stderr.write("ERROR: %s; use --gpus N\n" % msg)
+            return 2
+    batch = (args, opts, say, solve_fn, n_devices, timing, t_start)
     if lists is not None:
-        return _run_lists(args, lists, ms, opts, say, solve_fn, n_devices, timing, t_start)
+        return _run_batch(refine_lists, (ms, [pairs for _, _, pairs in lists]), lists, *batch)
     if scenes is not None:
-        return _run_scenes(args, scenes, ms, opts, say, solve_fn, n_devices, timing, t_start)
+        return _run_batch(refine_scenes, ([m for m, _ in scenes],), scenes, *batch)
     try:
         p, pos, st, sol = refine(ms, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
                                  timing=timing, fixed_images=args.fixed_images, initial_solution=start,

@@ -51,6 +51,7 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <cstdarg>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -58,6 +59,8 @@
 #include <fcntl.h>
 #include <fstream>
 #include <map>
+#include <memory>
+#include <optional>
 #include <set>
 #include <string>
 #include <thread>
@@ -136,6 +139,19 @@ struct CliError {
   std::string msg;
 };
 
+// The end of the run with exit code `code`; its message is on stderr already
+struct Exit {
+  int code;
+};
+
+[[noreturn]] __attribute__((format(printf, 2, 3))) void fail(int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  std::vfprintf(stderr, fmt, ap);
+  va_end(ap);
+  throw Exit{code};
+}
+
 struct OptionSpec {
   const char* name;
   bool takes, repeat;
@@ -166,17 +182,22 @@ const OptionSpec& find_option(const std::string& name) {
   throw CliError{"unrecognised option '--" + name + "'"};
 }
 
-struct Args {
+// The command line.  An absent single option is nullopt, except --initial_solution, which is empty when absent.
+struct Options {
   bool help = false, keep_initial_solution = false, carry_initial_solution = false, update_initial_solution = false,
        joint_queries = false;
-  std::map<std::string, std::string> single;
-  std::map<std::string, std::vector<std::string>> repeated;
+  std::string matches_file, output_file, initial_solution;
+  std::optional<std::string> previous_matches_file, record_file, earlier_record_file, additional_scenes, listed_pairs;
+  std::vector<std::string> banned_images, fixed_images, query_images;
+  uint64_t device = 0, gpus = 1;
 };
 
 // Boost.Program_options semantics of solve.cc:387-401: long options, `--name value` or `--name=value`,
 // no positional arguments, Boost's error messages
-Args parse(int argc, char** argv) {
-  Args a;
+Options parse(int argc, char** argv) {
+  std::map<std::string, std::string> single;
+  std::map<std::string, std::vector<std::string>> repeated;
+  std::set<std::string> flags;
   for (int i = 1; i < argc;) {
     const std::string tok = argv[i++];
     if (tok.size() > 2 && tok.compare(0, 2, "--") == 0) {
@@ -193,19 +214,15 @@ Args parse(int argc, char** argv) {
           throw CliError{std::string("the required argument for option '--") + o.name + "' is missing"};
         }
         if (o.repeat) {
-          a.repeated[o.name].push_back(v);
-        } else if (a.single.count(o.name)) {
+          repeated[o.name].push_back(v);
+        } else if (single.count(o.name)) {
           throw CliError{std::string("option '--") + o.name + "' cannot be specified more than once"};
         } else {
-          a.single[o.name] = v;
+          single[o.name] = v;
         }
       } else {
         if (eq != std::string::npos) throw CliError{std::string("option '--") + o.name + "' does not take any arguments"};
-        (std::strcmp(o.name, "help") == 0 ? a.help
-         : std::strcmp(o.name, "keep_initial_solution") == 0  ? a.keep_initial_solution
-         : std::strcmp(o.name, "carry_initial_solution") == 0 ? a.carry_initial_solution
-         : std::strcmp(o.name, "joint_queries") == 0          ? a.joint_queries
-                                                              : a.update_initial_solution) = true;
+        flags.insert(o.name);
       }
     } else if (tok.size() > 1 && tok[0] == '-') {
       throw CliError{"unrecognised option '" + tok + "'"};
@@ -213,22 +230,135 @@ Args parse(int argc, char** argv) {
       throw CliError{"too many positional options have been specified on the command line"};
     }
   }
-  return a;
+  Options o;
+  o.help = flags.count("help") != 0;
+  if (o.help) return o;
+  for (const char* req : {"matches_file", "output_file"})  // po::notify: required options, in declaration order
+    if (!single.count(req)) throw CliError{std::string("the option '--") + req + "' is required but missing"};
+  auto as_uint = [&](const char* name, uint64_t dflt) {  // lexical_cast<size_t>
+    const auto it = single.find(name);
+    if (it == single.end()) return dflt;
+    const std::string& v = it->second;
+    bool digits = !v.empty();
+    for (char c : v) digits = digits && c >= '0' && c <= '9';
+    if (!digits) throw CliError{"the argument ('" + v + "') for option '--" + name + "' is invalid"};
+    return (uint64_t)std::strtoull(v.c_str(), nullptr, 10);
+  };
+  (void)as_uint("n_threads", 8);
+  o.device = as_uint("device", 0);
+  o.gpus = as_uint("gpus", 1);
+  auto given = [&](const char* name) {
+    const auto it = single.find(name);
+    return it == single.end() ? std::optional<std::string>() : it->second;
+  };
+  o.matches_file = single.at("matches_file");
+  o.output_file = single.at("output_file");
+  o.initial_solution = given("initial_solution").value_or("");
+  o.previous_matches_file = given("previous_matches_file");
+  o.record_file = given("record_file");
+  o.earlier_record_file = given("earlier_record_file");
+  o.additional_scenes = given("additional_scenes");
+  o.listed_pairs = given("listed_pairs");
+  o.banned_images = repeated["banned_images"];
+  o.fixed_images = repeated["fixed_images"];
+  o.query_images = repeated["query_images"];
+  o.keep_initial_solution = flags.count("keep_initial_solution") != 0;
+  o.carry_initial_solution = flags.count("carry_initial_solution") != 0;
+  o.update_initial_solution = flags.count("update_initial_solution") != 0;
+  o.joint_queries = flags.count("joint_queries") != 0;
+  return o;
 }
 
-uint64_t as_uint(const Args& a, const char* name, uint64_t dflt) {  // lexical_cast<size_t>
-  const auto it = a.single.find(name);
-  if (it == a.single.end()) return dflt;
-  const std::string& v = it->second;
-  bool digits = !v.empty();
-  for (char c : v) digits = digits && c >= '0' && c <= '9';
-  if (!digits) throw CliError{"the argument ('" + v + "') for option '--" + name + "' is invalid"};
-  return std::strtoull(v.c_str(), nullptr, 10);
+// The opt-in options the rules between options speak of
+enum Opt { kFixed, kStart, kKeep, kCarry, kUpdate, kPrevious, kRecord, kEarlier, kQuery, kJoint, kScenes, kLists, kNumOpts };
+const char* const kOptName[kNumOpts] = {"--fixed_images",          "--initial_solution",    "--keep_initial_solution",
+                                        "--carry_initial_solution", "--update_initial_solution", "--previous_matches_file",
+                                        "--record_file",           "--earlier_record_file", "--query_images",
+                                        "--joint_queries",         "--additional_scenes",   "--listed_pairs"};
+
+// `opt` needs `others[0]`, or excludes each of `others`
+struct Rule {
+  Opt opt;
+  bool needs;
+  std::vector<Opt> others;
+};
+// The start solution, the fixed images, the incremental modes and the queries belong to one scene: a batch
+// (--additional_scenes, --listed_pairs) excludes them
+const std::vector<Opt> kOneScene = {kFixed, kStart, kKeep, kCarry, kUpdate, kPrevious, kRecord, kEarlier, kQuery, kJoint};
+// In order: with two conflicts, the first rule that fires writes the message.
+const std::vector<Rule> kRules = {
+    {kKeep, true, {kStart}},
+    {kCarry, true, {kStart}},
+    {kUpdate, true, {kStart}},
+    {kUpdate, false, {kKeep}},
+    {kPrevious, true, {kUpdate}},
+    {kEarlier, true, {kUpdate}},
+    {kEarlier, false, {kPrevious}},
+    // each query is refined against the scene as it stands; the incremental modes update one scene
+    {kQuery, false, {kUpdate, kPrevious, kRecord, kEarlier, kCarry}},
+    {kJoint, true, {kQuery}},
+    {kLists, false, [] { std::vector<Opt> v = kOneScene; v.push_back(kScenes); return v; }()},
+    {kScenes, false, kOneScene},
+};
+
+// Exits 2 after the ERROR line of the first rule the command line breaks
+void check_rules(const Options& o) {
+  const bool set[kNumOpts] = {!o.fixed_images.empty(),       !o.initial_solution.empty(), o.keep_initial_solution,
+                              o.carry_initial_solution,      o.update_initial_solution,   o.previous_matches_file.has_value(),
+                              o.record_file.has_value(),     o.earlier_record_file.has_value(), !o.query_images.empty(),
+                              o.joint_queries,               o.additional_scenes.has_value(), o.listed_pairs.has_value()};
+  for (const Rule& r : kRules) {
+    if (!set[r.opt]) continue;
+    for (const Opt b : r.others) {
+      if (r.needs && !set[b]) fail(2, "ERROR: %s needs %s%s\n", kOptName[r.opt], kOptName[b], b == kStart ? " FILE" : "");
+      if (!r.needs && set[b]) fail(2, "ERROR: %s and %s exclude each other\n", kOptName[r.opt], kOptName[b]);
+    }
+  }
+}
+
+// How the solve starts (solve.cc:608-612): from zeros, or from --initial_solution joined, kept, or updated (alone,
+// since --previous_matches_file, since --earlier_record_file)
+enum class Start { kZeros, kJoin, kKeep, kUpdate, kUpdateSinceMatches, kUpdateSinceRecord };
+
+Start start_mode(const Options& o) {
+  if (o.initial_solution.empty()) return Start::kZeros;
+  if (o.earlier_record_file) return Start::kUpdateSinceRecord;
+  if (o.previous_matches_file) return Start::kUpdateSinceMatches;
+  if (o.update_initial_solution) return Start::kUpdate;
+  return o.keep_initial_solution ? Start::kKeep : Start::kJoin;
+}
+
+// keep and the updates hold the nodes with an entry in the start solution constant
+bool holds_entries(Start s) { return s != Start::kZeros && s != Start::kJoin; }
+
+// The sub-scenes of the graph stage (lfr_host_input::image_group), with the nouns of the "more than 65535" message
+struct Labelling {
+  enum Kind { kNone, kQueries, kScenes, kLists } kind;
+  const char *option, *members, *list;
+  bool batched() const { return kind == kScenes || kind == kLists; }
+};
+
+Labelling labelling(const Options& o) {
+  if (!o.query_images.empty()) return {Labelling::kQueries, "--query_images", "sub-scenes", "query list"};
+  if (o.listed_pairs) return {Labelling::kLists, "--listed_pairs", "lists", "pair list"};
+  if (o.additional_scenes) return {Labelling::kScenes, "--additional_scenes", "scenes", "scene list"};
+  return {Labelling::kNone, nullptr, nullptr, nullptr};
 }
 
 bool file_exists(const std::string& path) {
   std::ifstream f(path, std::ios::binary);
   return f.good();
+}
+
+// solve.cc:416-424: the file `path`, or else its pieces `path`.part.0, .part.1, ... up to the first one missing
+std::vector<std::string> matching_files(const std::string& path) {
+  if (file_exists(path)) return {path};
+  std::vector<std::string> files;
+  for (int k = 0;; ++k) {
+    std::string f = path + ".part." + std::to_string(k);
+    if (!file_exists(f)) return files;
+    files.push_back(std::move(f));
+  }
 }
 
 // A file mapped read-only (a Madrid-scale MatchingFile is several GB: no second copy of it in memory).
@@ -266,6 +396,129 @@ struct FileImage {
   size_t size() const { return n; }
 };
 
+// The bytes of the file `path` into `text`; false when it cannot be read
+bool read_file(const std::string& path, std::string& text) {
+  FileImage f;
+  if (!f.open(path)) return false;
+  text.assign(reinterpret_cast<const char*>(f.data()), f.size());
+  f.release();
+  return true;
+}
+
+// The lines of `text`, split at '\n'; the last newline is optional
+std::vector<std::string> lines_of(const std::string& text) {
+  std::vector<std::string> lines;
+  for (size_t at = 0; at < text.size();) {
+    const size_t end = std::min(text.find('\n', at), text.size());
+    lines.push_back(text.substr(at, end - at));
+    at = end + 1;
+  }
+  return lines;
+}
+
+// One MatchingFile part after the pair walk: image names as byte ranges of its buffer, the matches as
+// the offsets of their length prefixes.
+struct Part {
+  FileImage buf;
+  uint64_t P = 0, M = 0;
+  std::vector<uint64_t> pair_ptr, n1_off, n2_off, match_off;
+  std::vector<uint32_t> n1_len, n2_len;
+  std::vector<float> fact1, fact2;
+  // Map `path`, count its pairs and matches and size the pair-level arrays: 0, 2 when the file cannot be mapped,
+  // 255 when its bytes do not parse
+  int open(const std::string& path) {
+    if (!buf.open(path)) return 2;
+    if (lfr_wire_scan_matches(buf.data(), buf.size(), &P, &M) != LFR_OK) return 255;
+    pair_ptr.resize(P + 1);
+    n1_off.resize(P); n2_off.resize(P); n1_len.resize(P); n2_len.resize(P);
+    fact1.resize(P); fact2.resize(P);
+    return 0;
+  }
+  lfr_wire_matches pair_level(uint32_t* feat1, uint32_t* feat2, float* sim, float* disp1, float* disp2) {
+    lfr_wire_matches w;
+    w.n_pairs = P; w.n_matches = M;
+    w.pair_ptr = pair_ptr.data(); w.fact1 = fact1.data(); w.fact2 = fact2.data();
+    w.name1_off = n1_off.data(); w.name1_len = n1_len.data();
+    w.name2_off = n2_off.data(); w.name2_len = n2_len.data();
+    w.feat1 = feat1; w.feat2 = feat2; w.sim = sim; w.disp1 = disp1; w.disp2 = disp2;
+    return w;
+  }
+};
+
+// Image names -> ids in order of first appearance
+struct NameTable {
+  std::vector<std::string> names;
+  std::map<std::string, uint32_t> id_of;
+  uint32_t intern(const Part& pt, uint64_t off, uint32_t len) {
+    std::string s(reinterpret_cast<const char*>(pt.buf.data()) + off, len);
+    const auto it = id_of.find(s);
+    if (it != id_of.end()) return it->second;
+    const uint32_t id = (uint32_t)names.size();
+    id_of.emplace(s, id);
+    names.push_back(std::move(s));
+    return id;
+  }
+};
+
+using StringPairs = std::vector<std::pair<std::string, std::string>>;
+
+// The nouns of a TAB-separated list file
+struct TabList {
+  const char *option, *file, *first, *first_empty, *rows;
+};
+const TabList kSceneList = {"--additional_scenes", "scene list", "MATCHES_FILE", "its matches file is empty", "scenes"};
+const TabList kPairList = {"--listed_pairs", "pair list", "MATCH_LIST", "its match list is empty", "lists"};
+
+// The list file of --additional_scenes or --listed_pairs: one `FIRST<TAB>OUTPUT_FILE` per line (raw bytes; the
+// last newline is optional), appended to `rows`.  Exits 2 after one ERROR line for an unreadable file, a malformed
+// line or two rows (those in `rows` before included) with the same output path.
+void read_tab_list(const TabList& kind, const std::string& path, StringPairs& rows) {
+  std::string text;
+  if (!read_file(path, text)) fail(2, "ERROR: cannot read the %s file '%s'\n", kind.file, path.c_str());
+  const std::vector<std::string> lines = lines_of(text);
+  for (size_t k = 0; k < lines.size(); ++k) {
+    const std::string& l = lines[k];
+    const size_t tab = l.find('\t');
+    const char* why = l.empty()                                  ? "it is empty"
+                      : tab == std::string::npos                 ? "it has no TAB"
+                      : l.find('\t', tab + 1) != std::string::npos ? "it has more than one TAB"
+                      : tab == 0                                 ? kind.first_empty
+                      : tab + 1 == l.size()                      ? "its output file is empty"
+                      : l.find('\0') != std::string::npos        ? "it holds a NUL byte"
+                                                                 : nullptr;
+    if (why) fail(2, "ERROR: %s: line %zu is not %s<TAB>OUTPUT_FILE: %s\n", kind.option, k + 1, kind.first, why);
+    rows.emplace_back(l.substr(0, tab), l.substr(tab + 1));
+  }
+  std::set<std::string> outputs;
+  for (const auto& r : rows)
+    if (!outputs.insert(r.second).second) fail(2, "ERROR: %s: two %s write '%s'\n", kind.option, kind.rows, r.second.c_str());
+}
+
+// The --listed_pairs file: one match list per line (read_tab_list, appended to `rows` after list 0, every pair of
+// --matches_file), every match list read and split as compute_match_graph.py:97 splits it (the newline stripped,
+// single spaces; exactly two fields).  The lines (NAME1, NAME2) of every list, none for list 0.  Exits 2 after one
+// ERROR line for what read_tab_list refuses, an unreadable match list or a malformed line of one, in that order.
+std::vector<StringPairs> read_pair_lists(const std::string& path, StringPairs& rows) {
+  read_tab_list(kPairList, path, rows);
+  std::vector<StringPairs> lists(rows.size());
+  for (size_t i = 1; i < rows.size(); ++i) {
+    const std::string& list = rows[i].first;
+    std::string text;
+    if (!read_file(list, text)) fail(2, "ERROR: --listed_pairs: line %zu: cannot read the match list '%s'\n", i, list.c_str());
+    const std::vector<std::string> lines = lines_of(text);
+    for (size_t j = 0; j < lines.size(); ++j) {
+      const std::string& l = lines[j];
+      const size_t fields = 1 + (size_t)std::count(l.begin(), l.end(), ' ');
+      if (fields != 2)
+        fail(2, "ERROR: --listed_pairs: line %zu of the match list '%s' is not NAME1 NAME2: it has %zu fields\n", j + 1,
+             list.c_str(), fields);
+      const size_t sp = l.find(' ');
+      lists[i].emplace_back(l.substr(0, sp), l.substr(sp + 1));
+    }
+  }
+  return lists;
+}
+
 // The earlier MatchingFile of --previous_matches_file, decoded on the host: its image names by id (in order of
 // first appearance over its parts) and the flat arrays of its lfr_host_input, no image banned.
 struct PreviousMatches {
@@ -285,521 +538,206 @@ struct PreviousMatches {
   }
 };
 
-// One MatchingFile part after the pair walk: image names as byte ranges of its buffer, the matches as
-// the offsets of their length prefixes.
-struct Part {
-  FileImage buf;
-  uint64_t P = 0, M = 0;
-  std::vector<uint64_t> pair_ptr, n1_off, n2_off, match_off;
-  std::vector<uint32_t> n1_len, n2_len;
-  std::vector<float> fact1, fact2;
-  lfr_wire_matches pair_level(uint32_t* feat1, uint32_t* feat2, float* sim, float* disp1, float* disp2) {
-    lfr_wire_matches w;
-    w.n_pairs = P; w.n_matches = M;
-    w.pair_ptr = pair_ptr.data(); w.fact1 = fact1.data(); w.fact2 = fact2.data();
-    w.name1_off = n1_off.data(); w.name1_len = n1_len.data();
-    w.name2_off = n2_off.data(); w.name2_len = n2_len.data();
-    w.feat1 = feat1; w.feat2 = feat2; w.sim = sim; w.disp1 = disp1; w.disp2 = disp2;
-    return w;
-  }
-};
-
 // Read and decode the earlier MatchingFile `path` (or its .part.N pieces, as --matches_file): 0, 2 when no
 // file can be read, 255 when the bytes do not parse.
 int read_previous(const std::string& path, PreviousMatches& pm) {
-  std::vector<std::string> files;
-  if (file_exists(path)) {
-    files.push_back(path);
-  } else {
-    for (int k = 0;; ++k) {
-      const std::string f = path + ".part." + std::to_string(k);
-      if (!file_exists(f)) break;
-      files.push_back(f);
-    }
-  }
+  const std::vector<std::string> files = matching_files(path);
   if (files.empty()) return 2;
-  std::map<std::string, uint32_t> id_of;
+  NameTable names;
   for (const std::string& f : files) {
     Part pt;
-    if (!pt.buf.open(f)) return 2;
-    if (lfr_wire_scan_matches(pt.buf.data(), pt.buf.size(), &pt.P, &pt.M) != LFR_OK) return 255;
-    pt.pair_ptr.resize(pt.P + 1);
-    pt.n1_off.resize(pt.P); pt.n2_off.resize(pt.P); pt.n1_len.resize(pt.P); pt.n2_len.resize(pt.P);
-    pt.fact1.resize(pt.P); pt.fact2.resize(pt.P);
+    if (const int rc = pt.open(f)) return rc;
     const uint64_t m0 = pm.feat1.size();
     pm.feat1.resize(m0 + pt.M); pm.feat2.resize(m0 + pt.M); pm.sim.resize(m0 + pt.M);
     pm.disp1.resize(18 * (m0 + pt.M)); pm.disp2.resize(18 * (m0 + pt.M));
     lfr_wire_matches w = pt.pair_level(pm.feat1.data() + m0, pm.feat2.data() + m0, pm.sim.data() + m0,
                                        pm.disp1.data() + 18 * m0, pm.disp2.data() + 18 * m0);
     if (lfr_wire_decode_matches(pt.buf.data(), pt.buf.size(), &w) != LFR_OK) return 255;
-    auto intern = [&](uint64_t off, uint32_t len) {
-      std::string s(reinterpret_cast<const char*>(pt.buf.data()) + off, len);
-      const auto it = id_of.find(s);
-      if (it != id_of.end()) return it->second;
-      const uint32_t id = (uint32_t)pm.names.size();
-      id_of.emplace(s, id);
-      pm.name_blob.insert(pm.name_blob.end(), s.begin(), s.end());
-      pm.name_off.push_back(pm.name_blob.size());
-      pm.names.push_back(std::move(s));
-      return id;
-    };
     for (uint64_t p = 0; p < pt.P; ++p) {
-      pm.pair_img1.push_back(intern(pt.n1_off[p], pt.n1_len[p]));
-      pm.pair_img2.push_back(intern(pt.n2_off[p], pt.n2_len[p]));
+      pm.pair_img1.push_back(names.intern(pt, pt.n1_off[p], pt.n1_len[p]));
+      pm.pair_img2.push_back(names.intern(pt, pt.n2_off[p], pt.n2_len[p]));
       pm.pair_ptr.push_back(m0 + pt.pair_ptr[p + 1]);
     }
     pt.buf.release();
+  }
+  pm.names = std::move(names.names);
+  for (const std::string& s : pm.names) {
+    pm.name_blob.insert(pm.name_blob.end(), s.begin(), s.end());
+    pm.name_off.push_back(pm.name_blob.size());
   }
   if (pm.name_blob.empty()) pm.name_blob.push_back(0);
   return 0;
 }
 
-// The --additional_scenes list: one `MATCHES_FILE<TAB>OUTPUT_FILE` per line (raw bytes; the last newline is
-// optional), appended to `scenes`.  0, or 2 after one ERROR line for an unreadable file, a malformed line or
-// two scenes (the first one included) with the same output path.
-int read_scene_list(const std::string& path, std::vector<std::pair<std::string, std::string>>& scenes) {
-  FileImage f;
-  if (!f.open(path)) {
-    std::fprintf(stderr, "ERROR: cannot read the scene list file '%s'\n", path.c_str());
-    return 2;
-  }
-  const std::string text(reinterpret_cast<const char*>(f.data()), f.size());
-  f.release();
-  size_t line = 0;
-  for (size_t at = 0; at < text.size();) {
-    ++line;
-    const size_t end = std::min(text.find('\n', at), text.size());
-    const std::string l = text.substr(at, end - at);
-    at = end + 1;
-    const size_t tab = l.find('\t');
-    const char* why = l.empty()                                  ? "it is empty"
-                      : tab == std::string::npos                 ? "it has no TAB"
-                      : l.find('\t', tab + 1) != std::string::npos ? "it has more than one TAB"
-                      : tab == 0                                 ? "its matches file is empty"
-                      : tab + 1 == l.size()                      ? "its output file is empty"
-                      : l.find('\0') != std::string::npos        ? "it holds a NUL byte"
-                                                                 : nullptr;
-    if (why) {
-      std::fprintf(stderr, "ERROR: --additional_scenes: line %zu is not MATCHES_FILE<TAB>OUTPUT_FILE: %s\n", line, why);
-      return 2;
-    }
-    scenes.emplace_back(l.substr(0, tab), l.substr(tab + 1));
-  }
-  std::set<std::string> outputs;
-  for (const auto& sc : scenes)
-    if (!outputs.insert(sc.second).second) {
-      std::fprintf(stderr, "ERROR: --additional_scenes: two scenes write '%s'\n", sc.second.c_str());
-      return 2;
-    }
-  return 0;
-}
-
-// One --listed_pairs entry: a match list's path, its output file and its lines (NAME1, NAME2); `all` is list 0,
-// every pair of --matches_file in file order.
-struct PairList {
-  std::string path, output;
-  std::vector<std::pair<std::string, std::string>> lines;
-  bool all = false;
+// What the start point reads besides the MatchingFiles: the start solution (mapped while the run needs it), the
+// earlier MatchingFile and the earlier record
+struct StartInputs {
+  FileImage file;
+  PreviousMatches previous;
+  std::vector<uint8_t> earlier_record;
 };
 
-// The --listed_pairs file: one `MATCH_LIST<TAB>OUTPUT_FILE` per line (the rules of read_scene_list), appended to
-// `lists` after list 0, then every match list read and split as compute_match_graph.py:97 splits it (the
-// newline stripped, single spaces; exactly two fields).  0, or 2 after one ERROR line for an unreadable file, a
-// malformed line, two lists (the first one included) with the same output path, an unreadable match list or a
-// malformed line of one, in that order.
-int read_pair_lists(const std::string& path, std::vector<PairList>& lists) {
-  FileImage f;
-  if (!f.open(path)) {
-    std::fprintf(stderr, "ERROR: cannot read the pair list file '%s'\n", path.c_str());
-    return 2;
-  }
-  const std::string text(reinterpret_cast<const char*>(f.data()), f.size());
-  f.release();
-  size_t line = 0;
-  for (size_t at = 0; at < text.size();) {
-    ++line;
-    const size_t end = std::min(text.find('\n', at), text.size());
-    const std::string l = text.substr(at, end - at);
-    at = end + 1;
-    const size_t tab = l.find('\t');
-    const char* why = l.empty()                                  ? "it is empty"
-                      : tab == std::string::npos                 ? "it has no TAB"
-                      : l.find('\t', tab + 1) != std::string::npos ? "it has more than one TAB"
-                      : tab == 0                                 ? "its match list is empty"
-                      : tab + 1 == l.size()                      ? "its output file is empty"
-                      : l.find('\0') != std::string::npos        ? "it holds a NUL byte"
-                                                                 : nullptr;
-    if (why) {
-      std::fprintf(stderr, "ERROR: --listed_pairs: line %zu is not MATCH_LIST<TAB>OUTPUT_FILE: %s\n", line, why);
-      return 2;
-    }
-    PairList pl;
-    pl.path = l.substr(0, tab);
-    pl.output = l.substr(tab + 1);
-    lists.push_back(std::move(pl));
-  }
-  std::set<std::string> outputs;
-  for (const PairList& pl : lists)
-    if (!outputs.insert(pl.output).second) {
-      std::fprintf(stderr, "ERROR: --listed_pairs: two lists write '%s'\n", pl.output.c_str());
-      return 2;
-    }
-  for (size_t i = 1; i < lists.size(); ++i) {
-    PairList& pl = lists[i];
-    FileImage g;
-    if (!g.open(pl.path)) {
-      std::fprintf(stderr, "ERROR: --listed_pairs: line %zu: cannot read the match list '%s'\n", i, pl.path.c_str());
-      return 2;
-    }
-    const std::string t(reinterpret_cast<const char*>(g.data()), g.size());
-    g.release();
-    size_t j = 0;
-    for (size_t at = 0; at < t.size();) {
-      ++j;
-      const size_t end = std::min(t.find('\n', at), t.size());
-      const std::string l = t.substr(at, end - at);
-      at = end + 1;
-      const size_t fields = 1 + (size_t)std::count(l.begin(), l.end(), ' ');
-      if (fields != 2) {
-        std::fprintf(stderr, "ERROR: --listed_pairs: line %zu of the match list '%s' is not NAME1 NAME2: it has %zu fields\n",
-                     j, pl.path.c_str(), fields);
-        return 2;
-      }
-      const size_t sp = l.find(' ');
-      pl.lines.emplace_back(l.substr(0, sp), l.substr(sp + 1));
-    }
-  }
-  return 0;
-}
-
-using Clock = std::chrono::steady_clock;
-long long ms_between(Clock::time_point a, Clock::time_point b) {
-  return (long long)std::chrono::duration_cast<std::chrono::milliseconds>(b - a).count();
-}
-
-}  // namespace
-
-int main(int argc, char** argv) {
-  std::string matches_file, output_file, initial_solution, previous_matches_file, record_file, earlier_record_file,
-      scene_list, list_file;
-  std::vector<std::string> banned_list, fixed_list, query_list;
-  uint64_t device = 0, gpus = 1;
-  bool keep_start = false, carry_start = false, update_start = false, have_previous = false, have_record = false,
-       have_earlier = false, have_query = false, joint = false, have_scenes = false,
-       have_lists = false;
-  try {
-    Args a = parse(argc, argv);
-    if (a.help) {
-      std::fputs("Patch Match graph problem solver\n\n", stdout);
-      std::fputs(kUsage, stdout);
-      return 0;
-    }
-    for (const char* req : {"matches_file", "output_file"})  // po::notify: required options, in declaration order
-      if (!a.single.count(req)) throw CliError{std::string("the option '--") + req + "' is required but missing"};
-    matches_file = a.single.at("matches_file");
-    output_file = a.single.at("output_file");
-    (void)as_uint(a, "n_threads", 8);
-    device = as_uint(a, "device", 0);
-    gpus = as_uint(a, "gpus", 1);
-    banned_list = a.repeated["banned_images"];
-    fixed_list = a.repeated["fixed_images"];
-    have_query = a.repeated.count("query_images") != 0;
-    query_list = a.repeated["query_images"];
-    joint = a.joint_queries;
-    if (a.single.count("initial_solution")) initial_solution = a.single.at("initial_solution");
-    keep_start = a.keep_initial_solution;
-    carry_start = a.carry_initial_solution;
-    update_start = a.update_initial_solution;
-    have_previous = a.single.count("previous_matches_file") != 0;
-    if (have_previous) previous_matches_file = a.single.at("previous_matches_file");
-    have_record = a.single.count("record_file") != 0;
-    if (have_record) record_file = a.single.at("record_file");
-    have_earlier = a.single.count("earlier_record_file") != 0;
-    if (have_earlier) earlier_record_file = a.single.at("earlier_record_file");
-    have_scenes = a.single.count("additional_scenes") != 0;
-    if (have_scenes) scene_list = a.single.at("additional_scenes");
-    have_lists = a.single.count("listed_pairs") != 0;
-    if (have_lists) list_file = a.single.at("listed_pairs");
-  } catch (const CliError& e) {  // solve.cc:397-401
-    std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
-    std::fputs(kUsage, stderr);
-    return 1;
-  }
-
-  // the start solution is read and checked before any other work, so that its errors come before any output
-  FileImage start_file;
-  const bool have_start = !initial_solution.empty();
-  if (keep_start && !have_start) {
-    std::fputs("ERROR: --keep_initial_solution needs --initial_solution FILE\n", stderr);
-    return 2;
-  }
-  if (carry_start && !have_start) {
-    std::fputs("ERROR: --carry_initial_solution needs --initial_solution FILE\n", stderr);
-    return 2;
-  }
-  if (update_start && !have_start) {
-    std::fputs("ERROR: --update_initial_solution needs --initial_solution FILE\n", stderr);
-    return 2;
-  }
-  if (update_start && keep_start) {
-    std::fputs("ERROR: --update_initial_solution and --keep_initial_solution exclude each other\n", stderr);
-    return 2;
-  }
-  if (have_previous && !update_start) {
-    std::fputs("ERROR: --previous_matches_file needs --update_initial_solution\n", stderr);
-    return 2;
-  }
-  if (have_earlier && !update_start) {
-    std::fputs("ERROR: --earlier_record_file needs --update_initial_solution\n", stderr);
-    return 2;
-  }
-  if (have_earlier && have_previous) {
-    std::fputs("ERROR: --earlier_record_file and --previous_matches_file exclude each other\n", stderr);
-    return 2;
-  }
-  if (have_query) {  // each query is refined against the scene as it stands; the incremental modes update one scene
-    for (const auto& o : {std::make_pair(update_start, "--update_initial_solution"),
-                          std::make_pair(have_previous, "--previous_matches_file"), std::make_pair(have_record, "--record_file"),
-                          std::make_pair(have_earlier, "--earlier_record_file"),
-                          std::make_pair(carry_start, "--carry_initial_solution")})
-      if (o.first) {
-        std::fprintf(stderr, "ERROR: --query_images and %s exclude each other\n", o.second);
-        return 2;
-      }
-  }
-  if (joint && !have_query) {
-    std::fputs("ERROR: --joint_queries needs --query_images\n", stderr);
-    return 2;
-  }
-  // --listed_pairs: list 0 is every pair of --matches_file, written to --output_file; the listed match lists
-  // follow.  Each list's output is what its own run writes: the same command on a MatchingFile that holds the
-  // file's pair for every line of the list, in line order.
-  std::vector<PairList> lists(1);
-  lists[0].output = output_file;
-  lists[0].all = true;
-  if (have_lists) {  // as --additional_scenes, whose batches it excludes too
-    for (const auto& o : {std::make_pair(!fixed_list.empty(), "--fixed_images"), std::make_pair(have_start, "--initial_solution"),
-                          std::make_pair(keep_start, "--keep_initial_solution"),
-                          std::make_pair(carry_start, "--carry_initial_solution"),
-                          std::make_pair(update_start, "--update_initial_solution"),
-                          std::make_pair(have_previous, "--previous_matches_file"), std::make_pair(have_record, "--record_file"),
-                          std::make_pair(have_earlier, "--earlier_record_file"), std::make_pair(have_query, "--query_images"),
-                          std::make_pair(joint, "--joint_queries"), std::make_pair(have_scenes, "--additional_scenes")})
-      if (o.first) {
-        std::fprintf(stderr, "ERROR: --listed_pairs and %s exclude each other\n", o.second);
-        return 2;
-      }
-    const int rc = read_pair_lists(list_file, lists);
-    if (rc) return rc;
-  }
-  // --additional_scenes: the scene of --matches_file / --output_file is scene 0, the listed ones follow; each
-  // scene's output is what its own run writes (the same command with that scene's two files alone)
-  std::vector<std::pair<std::string, std::string>> scenes{{matches_file, output_file}};
-  if (have_scenes) {  // the start solution, the fixed images and the incremental modes belong to one scene
-    for (const auto& o : {std::make_pair(!fixed_list.empty(), "--fixed_images"), std::make_pair(have_start, "--initial_solution"),
-                          std::make_pair(keep_start, "--keep_initial_solution"),
-                          std::make_pair(carry_start, "--carry_initial_solution"),
-                          std::make_pair(update_start, "--update_initial_solution"),
-                          std::make_pair(have_previous, "--previous_matches_file"), std::make_pair(have_record, "--record_file"),
-                          std::make_pair(have_earlier, "--earlier_record_file"), std::make_pair(have_query, "--query_images"),
-                          std::make_pair(joint, "--joint_queries")})
-      if (o.first) {
-        std::fprintf(stderr, "ERROR: --additional_scenes and %s exclude each other\n", o.second);
-        return 2;
-      }
-    const int rc = read_scene_list(scene_list, scenes);
-    if (rc) return rc;
-  }
-  uint32_t S = (uint32_t)scenes.size();  // the batch's members: scenes, or with --listed_pairs the lists
-  if (have_start) {
-    if (!start_file.open(initial_solution)) {
-      std::fprintf(stderr, "ERROR: cannot read the initial solution file '%s'\n", initial_solution.c_str());
-      return 2;
-    }
+// Read and check the start inputs before any other work, so that their errors come before any output
+void read_start_inputs(const Options& o, StartInputs& si) {
+  if (!o.initial_solution.empty()) {
+    if (!si.file.open(o.initial_solution))
+      fail(2, "ERROR: cannot read the initial solution file '%s'\n", o.initial_solution.c_str());
     uint64_t ni = 0, nd = 0;
-    if (lfr_wire_decode_solution(start_file.data(), start_file.size(), &ni, &nd, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                 nullptr, nullptr) != LFR_OK) {
-      std::fputs("Failed to parse proto object.\n", stderr);  // as for the matches, solve.cc:433-436
-      return 255;
-    }
+    if (lfr_wire_decode_solution(si.file.data(), si.file.size(), &ni, &nd, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                 nullptr, nullptr) != LFR_OK)
+      fail(255, "Failed to parse proto object.\n");  // as for the matches, solve.cc:433-436
   }
-  PreviousMatches previous;
-  if (have_previous) {
-    const int rc = read_previous(previous_matches_file, previous);
-    if (rc == 2) {
-      std::fprintf(stderr, "ERROR: cannot read the previous matches file '%s'\n", previous_matches_file.c_str());
-      return 2;
-    }
-    if (rc != 0) {
-      std::fputs("Failed to parse proto object.\n", stderr);
-      return 255;
-    }
+  if (o.previous_matches_file) {
+    const int rc = read_previous(*o.previous_matches_file, si.previous);
+    if (rc == 2) fail(2, "ERROR: cannot read the previous matches file '%s'\n", o.previous_matches_file->c_str());
+    if (rc != 0) fail(255, "Failed to parse proto object.\n");
   }
-  std::vector<uint8_t> earlier_record;
-  if (have_earlier) {
-    FileImage f;
-    if (!f.open(earlier_record_file)) {
-      std::fprintf(stderr, "ERROR: cannot read the earlier record file '%s'\n", earlier_record_file.c_str());
-      return 2;
-    }
-    earlier_record.assign(f.data(), f.data() + f.size());
-    f.release();
-    if (!lfr::record::check(earlier_record.data(), earlier_record.size(), nullptr)) {
-      std::fprintf(stderr, "ERROR: '%s' is not a problem record\n", earlier_record_file.c_str());
-      return 2;
-    }
+  if (o.earlier_record_file) {
+    const std::string& path = *o.earlier_record_file;
+    std::string text;
+    if (!read_file(path, text)) fail(2, "ERROR: cannot read the earlier record file '%s'\n", path.c_str());
+    si.earlier_record.assign(text.begin(), text.end());
+    if (!lfr::record::check(si.earlier_record.data(), si.earlier_record.size(), nullptr))
+      fail(2, "ERROR: '%s' is not a problem record\n", path.c_str());
   }
+}
 
-  // A one-shot process pays for CUDA's start-up (driver initialisation over every visible GPU, context
-  // creation: 0.4-0.8 s on an 8-GPU box) more than for all of its work on a Fountain-scale scene.  Two
-  // measures: only the device that will be used is made visible (unless the caller already chose),
-  // and the start-up runs on a helper thread while the input is read, decoded and turned into a graph.
-  if (gpus <= 1 && !std::getenv("CUDA_VISIBLE_DEVICES")) {
-    setenv("CUDA_VISIBLE_DEVICES", std::to_string(device).c_str(), 1);
-    device = 0;
-  }
-  std::thread cuda_start([] { lfr_host_free(lfr_host_alloc(64)); });
-  struct Joiner {
-    std::thread& t;
-    ~Joiner() { if (t.joinable()) t.join(); }
-  } join_on_exit{cuda_start};
+// The pairs of all parts in order, with the batch member (scene) of every pair; image ids in order of first
+// appearance over all parts.  With --listed_pairs, select_listed_pairs() makes them the lists' pairs.
+struct Pairs {
+  std::vector<Part> parts;
+  NameTable names;
+  uint64_t P = 0, M = 0, M_file = 0;  // M_file: the matches the decode reads, the file's
+  std::vector<uint32_t> img1, img2, member;
+  std::vector<float> fact1, fact2;
+  std::vector<uint64_t> ptr;
+  std::vector<uint64_t> src, file_ptr;  // --listed_pairs alone: the file's pair behind every pair, the file's pair_ptr
+};
 
-  // ---- solve.cc:412-481: the file, or its .part.N pieces, of every scene -----------------------
+// solve.cc:412-481: the parts of every scene's MatchingFile mapped and walked.  Exits 255 when one does not parse.
+Pairs read_pairs(const StringPairs& scenes) {
+  Pairs ps;
   std::vector<std::string> files;
-  std::vector<uint32_t> part_scene;
-  for (uint32_t sc = 0; sc < S; ++sc) {
-    const std::string& mf = scenes[sc].first;
-    if (file_exists(mf)) {
-      files.push_back(mf);
-      part_scene.push_back(sc);
-    } else {
-      for (int k = 0;; ++k) {
-        const std::string f = mf + ".part." + std::to_string(k);
-        if (!file_exists(f)) break;
-        files.push_back(f);
-        part_scene.push_back(sc);
-      }
+  std::vector<uint32_t> part_member;
+  for (uint32_t sc = 0; sc < scenes.size(); ++sc)
+    for (const std::string& f : matching_files(scenes[sc].first)) {
+      files.push_back(f);
+      part_member.push_back(sc);
     }
-  }
-  std::vector<Part> parts(files.size());
+  ps.parts.resize(files.size());
   for (size_t i = 0; i < files.size(); ++i) {
-    Part& pt = parts[i];
-    bool ok = pt.buf.open(files[i]);
-    if (ok) ok = lfr_wire_scan_matches(pt.buf.data(), pt.buf.size(), &pt.P, &pt.M) == LFR_OK;
+    Part& pt = ps.parts[i];
+    bool ok = pt.open(files[i]) == 0;
     if (ok) {
-      pt.pair_ptr.resize(pt.P + 1);
-      pt.n1_off.resize(pt.P); pt.n2_off.resize(pt.P); pt.n1_len.resize(pt.P); pt.n2_len.resize(pt.P);
-      pt.fact1.resize(pt.P); pt.fact2.resize(pt.P);
       pt.match_off.resize(pt.M);
       lfr_wire_matches w = pt.pair_level(nullptr, nullptr, nullptr, nullptr, nullptr);
       ok = lfr_wire_walk_matches(pt.buf.data(), pt.buf.size(), &w, pt.match_off.data()) == LFR_OK;
     }
-    if (!ok) {
-      std::fputs("Failed to parse proto object.\n", stderr);  // solve.cc:433-436
-      return 255;
-    }
+    if (!ok) fail(255, "Failed to parse proto object.\n");  // solve.cc:433-436
   }
-
-  // image names -> ids in order of first appearance over all parts; the pairs of all parts in order, and the
-  // scene of every pair
-  std::vector<std::string> names;
-  std::map<std::string, uint32_t> id_of;
-  auto intern = [&](const Part& pt, uint64_t off, uint32_t len) {
-    std::string s(reinterpret_cast<const char*>(pt.buf.data()) + off, len);
-    const auto it = id_of.find(s);
-    if (it != id_of.end()) return it->second;
-    const uint32_t id = (uint32_t)names.size();
-    id_of.emplace(s, id);
-    names.push_back(std::move(s));
-    return id;
-  };
-  uint64_t P = 0, M = 0;
-  for (const Part& pt : parts) { P += pt.P; M += pt.M; }
-  std::vector<uint32_t> pair_img1(P), pair_img2(P);
-  std::vector<float> pair_fact1(P), pair_fact2(P);
-  std::vector<uint64_t> pair_ptr(P + 1, 0);
-  std::vector<uint32_t> pair_scene(P);
-  {
-    uint64_t p0 = 0, m0 = 0;
-    for (size_t i = 0; i < parts.size(); ++i) {
-      Part& pt = parts[i];
-      for (uint64_t p = 0; p < pt.P; ++p) {
-        pair_scene[p0 + p] = part_scene[i];
-        pair_img1[p0 + p] = intern(pt, pt.n1_off[p], pt.n1_len[p]);
-        pair_img2[p0 + p] = intern(pt, pt.n2_off[p], pt.n2_len[p]);
-        pair_fact1[p0 + p] = pt.fact1[p];
-        pair_fact2[p0 + p] = pt.fact2[p];
-        pair_ptr[p0 + p + 1] = m0 + pt.pair_ptr[p + 1];
-      }
-      p0 += pt.P;
-      m0 += pt.M;
+  for (const Part& pt : ps.parts) { ps.P += pt.P; ps.M += pt.M; }
+  ps.M_file = ps.M;
+  ps.img1.resize(ps.P); ps.img2.resize(ps.P); ps.member.resize(ps.P);
+  ps.fact1.resize(ps.P); ps.fact2.resize(ps.P);
+  ps.ptr.assign(ps.P + 1, 0);
+  uint64_t p0 = 0, m0 = 0;
+  for (size_t i = 0; i < ps.parts.size(); ++i) {
+    const Part& pt = ps.parts[i];
+    for (uint64_t p = 0; p < pt.P; ++p) {
+      ps.member[p0 + p] = part_member[i];
+      ps.img1[p0 + p] = ps.names.intern(pt, pt.n1_off[p], pt.n1_len[p]);
+      ps.img2[p0 + p] = ps.names.intern(pt, pt.n2_off[p], pt.n2_len[p]);
+      ps.fact1[p0 + p] = pt.fact1[p];
+      ps.fact2[p0 + p] = pt.fact2[p];
+      ps.ptr[p0 + p + 1] = m0 + pt.pair_ptr[p + 1];
     }
+    p0 += pt.P;
+    m0 += pt.M;
   }
+  return ps;
+}
 
-  // --listed_pairs: the batch's pairs are the lists' lines, list after list, each the first pair of the file
-  // with exactly those two names (one map over the pairs, names as bytes); every pair of the file for list 0.
-  // pair_src is the file's pair behind each of them, whose matches are copied to it after the decode.
-  const uint64_t M_file = M;  // the matches the decode reads: the file's
-  std::vector<uint64_t> pair_src, file_pair_ptr;
-  if (have_lists) {
-    std::unordered_map<uint64_t, uint64_t> first;  // image1 << 32 | image2 -> the first pair
-    for (uint64_t p = 0; p < P; ++p) first.emplace((uint64_t)pair_img1[p] << 32 | pair_img2[p], p);
-    std::vector<uint32_t> list_of;
-    for (size_t l = 0; l < lists.size(); ++l) {
-      if (lists[l].all) {
-        for (uint64_t p = 0; p < P; ++p) {
-          pair_src.push_back(p);
-          list_of.push_back((uint32_t)l);
-        }
-        continue;
-      }
-      for (size_t j = 0; j < lists[l].lines.size(); ++j) {
-        const std::string& n1 = lists[l].lines[j].first;
-        const std::string& n2 = lists[l].lines[j].second;
-        const auto i1 = id_of.find(n1), i2 = id_of.find(n2);
-        auto hit = first.end();
-        bool reverse = false;
-        if (i1 != id_of.end() && i2 != id_of.end()) {
-          hit = first.find((uint64_t)i1->second << 32 | i2->second);
-          reverse = first.count((uint64_t)i2->second << 32 | i1->second) != 0;
-        }
-        if (hit == first.end()) {
-          std::fprintf(stderr, "ERROR: --listed_pairs: line %zu of the match list '%s': the matches file holds no pair '%s' '%s'",
-                       j + 1, lists[l].path.c_str(), n1.c_str(), n2.c_str());
-          if (reverse) std::fprintf(stderr, "; it holds only '%s' '%s'", n2.c_str(), n1.c_str());
-          std::fputs("\n", stderr);
-          return 2;
-        }
-        pair_src.push_back(hit->second);
+// --listed_pairs: the batch's pairs are the lists' lines, list after list, each the first pair of the file
+// with exactly those two names (one map over the pairs, names as bytes); every pair of the file for list 0.
+// `rows` holds every list's path first.
+// ps.src is the file's pair behind each of them, whose matches are copied to it after the decode.  Exits 2 after
+// one ERROR line for a line whose pair the file does not hold.
+void select_listed_pairs(Pairs& ps, const StringPairs& rows, const std::vector<StringPairs>& lists) {
+  std::unordered_map<uint64_t, uint64_t> first;  // image1 << 32 | image2 -> the first pair
+  for (uint64_t p = 0; p < ps.P; ++p) first.emplace((uint64_t)ps.img1[p] << 32 | ps.img2[p], p);
+  const auto& id_of = ps.names.id_of;
+  std::vector<uint32_t> list_of;
+  for (size_t l = 0; l < lists.size(); ++l) {
+    if (l == 0) {
+      for (uint64_t p = 0; p < ps.P; ++p) {
+        ps.src.push_back(p);
         list_of.push_back((uint32_t)l);
       }
+      continue;
     }
-    const uint64_t Q = pair_src.size();
-    std::vector<uint32_t> img1(Q), img2(Q);
-    std::vector<float> f1(Q), f2(Q);
-    std::vector<uint64_t> ptr(Q + 1, 0);
-    for (uint64_t k = 0; k < Q; ++k) {
-      const uint64_t p = pair_src[k];
-      img1[k] = pair_img1[p]; img2[k] = pair_img2[p]; f1[k] = pair_fact1[p]; f2[k] = pair_fact2[p];
-      ptr[k + 1] = ptr[k] + (pair_ptr[p + 1] - pair_ptr[p]);
+    for (size_t j = 0; j < lists[l].size(); ++j) {
+      const std::string& n1 = lists[l][j].first;
+      const std::string& n2 = lists[l][j].second;
+      const auto i1 = id_of.find(n1), i2 = id_of.find(n2);
+      auto hit = first.end();
+      bool reverse = false;
+      if (i1 != id_of.end() && i2 != id_of.end()) {
+        hit = first.find((uint64_t)i1->second << 32 | i2->second);
+        reverse = first.count((uint64_t)i2->second << 32 | i1->second) != 0;
+      }
+      if (hit == first.end()) {
+        std::fprintf(stderr, "ERROR: --listed_pairs: line %zu of the match list '%s': the matches file holds no pair '%s' '%s'",
+                     j + 1, rows[l].first.c_str(), n1.c_str(), n2.c_str());
+        if (reverse) std::fprintf(stderr, "; it holds only '%s' '%s'", n2.c_str(), n1.c_str());
+        fail(2, "\n");
+      }
+      ps.src.push_back(hit->second);
+      list_of.push_back((uint32_t)l);
     }
-    pair_img1.swap(img1); pair_img2.swap(img2); pair_fact1.swap(f1); pair_fact2.swap(f2);
-    file_pair_ptr.swap(pair_ptr);
-    pair_ptr.swap(ptr);
-    pair_scene.swap(list_of);
-    P = Q;
-    M = pair_ptr[Q];
-    scenes.clear();  // from here on the batch's members are the lists
-    for (const PairList& pl : lists) scenes.emplace_back(pl.path, pl.output);
-    S = (uint32_t)scenes.size();
   }
-  const bool batched = have_scenes || have_lists;
+  const uint64_t Q = ps.src.size();
+  std::vector<uint32_t> img1(Q), img2(Q);
+  std::vector<float> f1(Q), f2(Q);
+  std::vector<uint64_t> ptr(Q + 1, 0);
+  for (uint64_t k = 0; k < Q; ++k) {
+    const uint64_t p = ps.src[k];
+    img1[k] = ps.img1[p]; img2[k] = ps.img2[p]; f1[k] = ps.fact1[p]; f2[k] = ps.fact2[p];
+    ptr[k + 1] = ptr[k] + (ps.ptr[p + 1] - ps.ptr[p]);
+  }
+  ps.img1.swap(img1); ps.img2.swap(img2); ps.fact1.swap(f1); ps.fact2.swap(f2);
+  ps.file_ptr.swap(ps.ptr);
+  ps.ptr.swap(ptr);
+  ps.member.swap(list_of);
+  ps.P = Q;
+  ps.M = ps.ptr[Q];
+}
 
+// The graph stage's input, and everything indexed by its image ids: the original ids, or with sub-scenes one id
+// per (sub-scene, image) in order of first appearance
+struct Staged {
+  lfr_host_input in;
+  std::vector<uint8_t> skip;
+  std::vector<uint32_t> orig_of, image_group;  // the original image id and the sub-scene of every id
+  std::vector<float> image_fact;
+  std::vector<uint8_t> fixed, written;
+  bool any_fixed = false;
+  std::vector<uint8_t> name_blob;
+  std::vector<uint64_t> name_off;
+  uint64_t e_cap = 0;  // the edge records of the pairs kept
+  uint32_t n_ids() const { return (uint32_t)orig_of.size(); }
+};
+
+// The pairs as the graph stage takes them (their image ids become stage ids).  Exits 2 after one ERROR line for a
+// pair that names two query images without --joint_queries, or for more than 65535 stage ids.
+Staged stage(Pairs& ps, const Options& o, const Labelling& lab) {
+  Staged st;
+  const std::vector<std::string>& names = ps.names.names;
+  const bool queries = lab.kind == Labelling::kQueries;
+  const uint64_t P = ps.P;
   // banned images (solve.cc:444-446)
-  const std::set<std::string> banned(banned_list.begin(), banned_list.end());
-  std::vector<uint8_t> skip(P, 0);
-  for (uint64_t p = 0; p < P; ++p)
-    skip[p] = (banned.count(names[pair_img1[p]]) || banned.count(names[pair_img2[p]])) ? 1 : 0;
+  const std::set<std::string> banned(o.banned_images.begin(), o.banned_images.end());
+  st.skip.assign(P, 0);
+  for (uint64_t p = 0; p < P; ++p) st.skip[p] = (banned.count(names[ps.img1[p]]) || banned.count(names[ps.img2[p]])) ? 1 : 0;
 
   // --query_images: a kept pair that names a query image belongs to that query's group's sub-scene, and its
   // images get that sub-scene's ids, in order of first appearance; a pair that names none is not solved.  A
@@ -809,12 +747,10 @@ int main(int argc, char** argv) {
   // kept pair in its scene's sub-scene, labelled by the scene index, so that scenes that share image names
   // share no node and each meta-component is cut at its own scene's image count.  --listed_pairs: the same with
   // the list index as the label, so a pair listed by two lists is a node set of each.
-  // orig_of: the original image id (and name) of every stage image id; the identity without sub-scenes.
   std::vector<uint8_t> is_query(names.size(), 0);
-  std::vector<uint32_t> orig_of, image_group;
-  if (have_query || batched) {
-    const std::set<std::string> queries(query_list.begin(), query_list.end());
-    for (size_t i = 0; i < names.size(); ++i) is_query[i] = queries.count(names[i]) ? 1 : 0;
+  if (lab.kind != Labelling::kNone) {
+    const std::set<std::string> query_names(o.query_images.begin(), o.query_images.end());
+    for (size_t i = 0; i < names.size(); ++i) is_query[i] = query_names.count(names[i]) ? 1 : 0;
     // the group of every query image: a union-find whose root is the group's lowest image id, its label.  It
     // runs over all pairs before any id is handed out, since a later pair can merge two groups that hold ids.
     std::vector<uint32_t> group_of(names.size());
@@ -823,530 +759,579 @@ int main(int argc, char** argv) {
       while (group_of[x] != x) x = group_of[x] = group_of[group_of[x]];
       return x;
     };
-    for (uint64_t p = 0; have_query && p < P; ++p) {
-      const uint32_t a = pair_img1[p], b = pair_img2[p];
-      if (skip[p] || !is_query[a] || !is_query[b]) continue;
-      if (!joint) {
-        std::fprintf(stderr, "ERROR: the pair '%s' - '%s' names two query images\n", names[a].c_str(), names[b].c_str());
-        return 2;
-      }
+    for (uint64_t p = 0; queries && p < P; ++p) {
+      const uint32_t a = ps.img1[p], b = ps.img2[p];
+      if (st.skip[p] || !is_query[a] || !is_query[b]) continue;
+      if (!o.joint_queries) fail(2, "ERROR: the pair '%s' - '%s' names two query images\n", names[a].c_str(), names[b].c_str());
       const uint32_t ra = find(a), rb = find(b);
       group_of[std::max(ra, rb)] = std::min(ra, rb);
     }
     std::map<std::pair<uint32_t, uint32_t>, uint32_t> sub_id;  // (group, image) -> stage image id
     auto sub = [&](uint32_t g, uint32_t img) {
-      const auto it = sub_id.emplace(std::make_pair(g, img), (uint32_t)orig_of.size());
+      const auto it = sub_id.emplace(std::make_pair(g, img), (uint32_t)st.orig_of.size());
       if (it.second) {
-        orig_of.push_back(img);
-        image_group.push_back(g);
+        st.orig_of.push_back(img);
+        st.image_group.push_back(g);
       }
       return it.first->second;
     };
     for (uint64_t p = 0; p < P; ++p) {
-      const uint32_t a = pair_img1[p], b = pair_img2[p];
-      if (skip[p] || (have_query && !(is_query[a] || is_query[b]))) {
-        skip[p] = 1;
-        pair_img1[p] = pair_img2[p] = 0;  // never read: skipped pairs name no image of the stage
+      const uint32_t a = ps.img1[p], b = ps.img2[p];
+      if (st.skip[p] || (queries && !(is_query[a] || is_query[b]))) {
+        st.skip[p] = 1;
+        ps.img1[p] = ps.img2[p] = 0;  // never read: skipped pairs name no image of the stage
         continue;
       }
-      const uint32_t g = have_query ? find(is_query[a] ? a : b) : pair_scene[p];
-      pair_img1[p] = sub(g, a);
-      pair_img2[p] = sub(g, b);
+      const uint32_t g = queries ? find(is_query[a] ? a : b) : ps.member[p];
+      ps.img1[p] = sub(g, a);
+      ps.img2[p] = sub(g, b);
     }
-    if (orig_of.size() > 65535) {
-      if (have_query)
-        std::fprintf(stderr, "ERROR: --query_images: the sub-scenes hold %zu images, more than 65535; split the query list "
-                             "over several runs\n", orig_of.size());
-      else if (have_lists)
-        std::fprintf(stderr, "ERROR: --listed_pairs: the lists hold %zu images, more than 65535; split the pair list "
-                             "over several runs\n", orig_of.size());
-      else
-        std::fprintf(stderr, "ERROR: --additional_scenes: the scenes hold %zu images, more than 65535; split the scene list "
-                             "over several runs\n", orig_of.size());
-      return 2;
-    }
+    if (st.orig_of.size() > 65535)
+      fail(2, "ERROR: %s: the %s hold %zu images, more than 65535; split the %s over several runs\n", lab.option,
+           lab.members, st.orig_of.size(), lab.list);
   } else {
-    orig_of.resize(names.size());
-    for (uint32_t i = 0; i < (uint32_t)names.size(); ++i) orig_of[i] = i;
+    st.orig_of.resize(names.size());
+    for (uint32_t i = 0; i < (uint32_t)names.size(); ++i) st.orig_of[i] = i;
   }
-  const uint32_t n_ids = (uint32_t)orig_of.size();  // image ids of the graph stage's input
+  const uint32_t n_ids = st.n_ids();
 
   // the first fact seen of every image among the pairs kept
-  std::vector<float> image_fact(n_ids, 0.f);
+  st.image_fact.assign(n_ids, 0.f);
   std::vector<uint8_t> have_fact(n_ids, 0);
-  uint64_t e_cap = 0;
   for (uint64_t p = 0; p < P; ++p) {
-    if (skip[p]) continue;
-    e_cap += 2 * (pair_ptr[p + 1] - pair_ptr[p]);
-    if (!have_fact[pair_img1[p]]) { have_fact[pair_img1[p]] = 1; image_fact[pair_img1[p]] = pair_fact1[p]; }
-    if (!have_fact[pair_img2[p]]) { have_fact[pair_img2[p]] = 1; image_fact[pair_img2[p]] = pair_fact2[p]; }
+    if (st.skip[p]) continue;
+    st.e_cap += 2 * (ps.ptr[p + 1] - ps.ptr[p]);
+    if (!have_fact[ps.img1[p]]) { have_fact[ps.img1[p]] = 1; st.image_fact[ps.img1[p]] = ps.fact1[p]; }
+    if (!have_fact[ps.img2[p]]) { have_fact[ps.img2[p]] = 1; st.image_fact[ps.img2[p]] = ps.fact2[p]; }
   }
 
   // images held fixed (the same name semantics as banned images), and the names by image id as the
   // start-point join and the encoder on the GPU take them (ids of the graph stage: with --query_images a
   // database image's name repeats once per sub-scene, and the joins give every copy the same entries)
-  const std::set<std::string> fixed_names(fixed_list.begin(), fixed_list.end());
-  std::vector<uint8_t> fixed(n_ids, 0), image_written(n_ids, 0);
-  bool any_fixed = false;
+  const std::set<std::string> fixed_names(o.fixed_images.begin(), o.fixed_images.end());
+  st.fixed.assign(n_ids, 0);
+  st.written.assign(n_ids, 0);
   for (uint32_t i = 0; i < n_ids; ++i) {
-    image_written[i] = !have_query || is_query[orig_of[i]];
-    if (fixed_names.count(names[orig_of[i]])) {
-      fixed[i] = 1;
-      any_fixed = true;
+    st.written[i] = !queries || is_query[st.orig_of[i]];
+    if (fixed_names.count(names[st.orig_of[i]])) {
+      st.fixed[i] = 1;
+      st.any_fixed = true;
     }
   }
-  std::vector<uint8_t> name_blob;
-  std::vector<uint64_t> name_off(n_ids + 1, 0);
+  st.name_off.assign(n_ids + 1, 0);
   for (uint32_t i = 0; i < n_ids; ++i) {
-    const std::string& nm = names[orig_of[i]];
-    name_blob.insert(name_blob.end(), nm.begin(), nm.end());
-    name_off[i + 1] = name_blob.size();
+    const std::string& nm = names[st.orig_of[i]];
+    st.name_blob.insert(st.name_blob.end(), nm.begin(), nm.end());
+    st.name_off[i + 1] = st.name_blob.size();
   }
 
-  lfr_host_input in;
-  std::memset(&in, 0, sizeof in);
-  in.n_pairs = P; in.n_matches = M; in.n_images = n_ids;
-  in.pair_img1 = pair_img1.data(); in.pair_img2 = pair_img2.data(); in.pair_skip = skip.data();
-  in.pair_ptr = pair_ptr.data();
-  in.image_group = have_query || batched ? image_group.data() : nullptr;
+  std::memset(&st.in, 0, sizeof st.in);
+  st.in.n_pairs = P; st.in.n_matches = ps.M; st.in.n_images = n_ids;
+  st.in.pair_img1 = ps.img1.data(); st.in.pair_img2 = ps.img2.data(); st.in.pair_skip = st.skip.data();
+  st.in.pair_ptr = ps.ptr.data();
+  st.in.image_group = lab.kind != Labelling::kNone ? st.image_group.data() : nullptr;
+  return st;
+}
 
-  // ---- which graph stage: the library's size rule, or LFR_GRAPH_STAGE=host|device (a test and
-  // measurement hook, not a product option).  A library without the stage on the GPU — the CPU checker —
-  // takes the host route; forcing the device route there is an error, never a silent host run.
+// Which graph stage: the library's size rule, or LFR_GRAPH_STAGE=host|device (a test and measurement hook, not a
+// product option).  A library without the stage on the GPU — the CPU checker — takes the host route; forcing the
+// device route there is an error, never a silent host run.
+bool device_route(const lfr_host_input& in, uint64_t gpus) {
   const bool have_device_stage = lfr_graph_stage_on_device && lfr_wire_decode_on_device && lfr_plan_create_from_matches &&
                                  lfr_plan_create_from_wire && lfr_plan_encode_solution && lfr_plan_fix_images &&
                                  lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
                                  lfr_plan_update_solution && lfr_plan_update_solution_since && lfr_plan_problem_record &&
                                  lfr_plan_update_solution_since_record && lfr_plan_encode_solution_images &&
                                  lfr_plan_encode_solution_groups && lfr_plan_create_from_wire_listed;
-  bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
+  const bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
-  if (force && *force) {
-    if (std::strcmp(force, "host") == 0) {
-      on_device = false;
-    } else if (std::strcmp(force, "device") == 0) {
-      if (!have_device_stage) {
-        std::fprintf(stderr, "ERROR: LFR_GRAPH_STAGE=device: the solve library has no graph stage on the GPU\n");
-        return 2;
-      }
-      if (gpus > 1) {
-        std::fprintf(stderr, "ERROR: LFR_GRAPH_STAGE=device: the graph stage on the GPU drives one device (--gpus 1)\n");
-        return 2;
-      }
-      on_device = true;
-    } else {
-      std::fprintf(stderr, "ERROR: LFR_GRAPH_STAGE must be 'host' or 'device'\n");
-      return 2;
-    }
-  }
+  if (!force || !*force) return on_device;
+  if (std::strcmp(force, "host") == 0) return false;
+  if (std::strcmp(force, "device") != 0) fail(2, "ERROR: LFR_GRAPH_STAGE must be 'host' or 'device'\n");
+  if (!have_device_stage) fail(2, "ERROR: LFR_GRAPH_STAGE=device: the solve library has no graph stage on the GPU\n");
+  if (gpus > 1) fail(2, "ERROR: LFR_GRAPH_STAGE=device: the graph stage on the GPU drives one device (--gpus 1)\n");
+  return true;
+}
 
-  // host route, and the device route below the library's size for the decoder on the GPU: the matches of
-  // every part decoded into one set of arrays, part after part (the pair level comes out as the walk gave it).
-  // With --listed_pairs the file is decoded once and every listed pair's matches are then copied into place;
-  // the decoder's threshold sees the file's match count.
-  const bool decode_on_device = on_device && lfr_wire_decode_on_device(M_file) == 1;
+// The decoded matches of every pair
+struct Matches {
   std::vector<uint32_t> feat1, feat2;
   std::vector<float> sim, disp1, disp2;
-  if (!decode_on_device) {
-    feat1.resize(M_file); feat2.resize(M_file); sim.resize(M_file); disp1.resize(18 * M_file); disp2.resize(18 * M_file);
-    uint64_t m0 = 0;
-    for (Part& pt : parts) {
-      lfr_wire_matches w = pt.pair_level(feat1.data() + m0, feat2.data() + m0, sim.data() + m0, disp1.data() + 18 * m0,
-                                         disp2.data() + 18 * m0);
-      if (lfr_wire_decode_matches(pt.buf.data(), pt.buf.size(), &w) != LFR_OK) {
-        std::fputs("Failed to parse proto object.\n", stderr);  // solve.cc:433-436
-        return 255;
-      }
-      m0 += pt.M;
-      pt.buf.release();  // the file image (several GB at Madrid scale) is not needed past the decode
-    }
-    if (have_lists) {
-      std::vector<uint32_t> e1(M), e2(M);
-      std::vector<float> es(M), ed1(18 * M), ed2(18 * M);
-      for (uint64_t k = 0; k < P; ++k) {
-        const uint64_t a = file_pair_ptr[pair_src[k]], c = pair_ptr[k + 1] - pair_ptr[k], b = pair_ptr[k];
-        std::copy_n(feat1.begin() + a, c, e1.begin() + b);
-        std::copy_n(feat2.begin() + a, c, e2.begin() + b);
-        std::copy_n(sim.begin() + a, c, es.begin() + b);
-        std::copy_n(disp1.begin() + 18 * a, 18 * c, ed1.begin() + 18 * b);
-        std::copy_n(disp2.begin() + 18 * a, 18 * c, ed2.begin() + 18 * b);
-      }
-      feat1.swap(e1); feat2.swap(e2); sim.swap(es); disp1.swap(ed1); disp2.swap(ed2);
-    }
-    in.feat1 = feat1.data(); in.feat2 = feat2.data(); in.sim = sim.data(); in.disp1 = disp1.data(); in.disp2 = disp2.data();
-  }
+};
 
-  cuda_start.join();  // page-locked memory needs the context
-  const Clock::time_point t_start = Clock::now();  // "Total time" (solve.cc:487-641): the graph work and the solve
-  lfr_edge* edges = nullptr;
-  bool edges_pinned = false;
-  lfr_plan* plan = nullptr;
-  lfr_host_sizes sz;
-  std::vector<uint32_t> row_ptr, track, comp, comp_ptr, comp_nodes, comp_order, node_image, node_feat;
-  std::vector<uint8_t> is_root;
-  if (on_device) {
-    // ---- the matches decoded and the graph stage run on the GPU (include/lfr_graph.h): the problem stays
-    // in HBM for the solve and the SolutionFile is encoded there
-    lfr_options opt;
-    lfr_options_default(&opt);
-    opt.device = (int32_t)device;
-    // LFR_DEVICE_CUT=1: the recursive cut on the device too (LFR_DBG_DEVICE_CUT; a test and measurement hook)
-    if (const char* e = std::getenv("LFR_DEVICE_CUT")) {
-      if (std::strcmp(e, "1") == 0) opt.debug_flags |= LFR_DBG_DEVICE_CUT;
-    }
-    std::vector<lfr_wire_part> wparts;
-    for (const Part& pt : parts) wparts.push_back(lfr_wire_part{pt.buf.data(), pt.buf.size(), pt.match_off.data(), pt.M});
-    const int rc = decode_on_device && have_lists
-                       ? lfr_plan_create_from_wire_listed(&in, wparts.data(), (uint32_t)wparts.size(), file_pair_ptr.data(),
-                                                          file_pair_ptr.size() - 1, pair_src.data(), &opt, nullptr, &plan, &sz)
-                   : decode_on_device
-                       ? lfr_plan_create_from_wire(&in, wparts.data(), (uint32_t)wparts.size(), &opt, nullptr, &plan, &sz)
-                       : lfr_plan_create_from_matches(&in, &opt, nullptr, &plan, &sz);
-    for (Part& pt : parts) pt.buf.release();
-    if (rc == LFR_EINVAL && std::strcmp(lfr_last_error(), "malformed Match message") == 0) {
-      std::fputs("Failed to parse proto object.\n", stderr);  // solve.cc:433-436, as the host decode
-      return 255;
-    }
-    if (rc == LFR_EINVAL || rc == LFR_EUNSUPPORTED) {  // the input, as the host stage would reject it
-      std::fprintf(stderr, "ERROR: the host graph stage rejected the input\n");
-      return 2;
-    }
-    if (rc != LFR_OK) {  // no device: the host route's message, from the same device check
-      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
-      return 2;
-    }
-    // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
-    int rc2 = any_fixed ? lfr_plan_fix_images(plan, fixed.data(), n_ids) : LFR_OK;
-    if (rc2 == LFR_OK && have_earlier) {
-      rc2 = lfr_plan_update_solution_since_record(plan, nullptr, start_file.data(), start_file.size(), n_ids,
-                                                  name_blob.data(), name_off.data(), earlier_record.data(),
-                                                  earlier_record.size(), nullptr, nullptr, nullptr);
-    } else if (rc2 == LFR_OK && have_previous) {
-      // the earlier run's graph stage on the device, for the compare only
-      const lfr_host_input pin = previous.input();
-      lfr_plan* prev_plan = nullptr;
-      rc2 = lfr_plan_create_from_matches(&pin, &opt, nullptr, &prev_plan, nullptr);
-      if (rc2 == LFR_OK)
-        rc2 = lfr_plan_update_solution_since(plan, nullptr, start_file.data(), start_file.size(), n_ids,
-                                             name_blob.data(), name_off.data(), prev_plan, (uint32_t)previous.names.size(),
-                                             previous.name_blob.data(), previous.name_off.data(), nullptr, nullptr, nullptr);
-      lfr_plan_destroy(prev_plan);
-    } else if (rc2 == LFR_OK && have_start && update_start)
-      rc2 = lfr_plan_update_solution(plan, nullptr, start_file.data(), start_file.size(), n_ids,
-                                     name_blob.data(), name_off.data(), nullptr, nullptr);
-    else if (rc2 == LFR_OK && have_start)
-      rc2 = (keep_start ? lfr_plan_keep_solution : lfr_plan_start_from_solution)(
-          plan, nullptr, start_file.data(), start_file.size(), n_ids, name_blob.data(), name_off.data(), nullptr);
-    if (rc2 != LFR_OK) {
-      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc2, lfr_last_error());
-      return 2;
-    }
-  } else {
-    // ---- host graph stage (solve.cc:438-606); the edge records go straight into page-locked memory
-    if (e_cap) {
-      edges = static_cast<lfr_edge*>(lfr_host_alloc(e_cap * sizeof(lfr_edge)));
-      edges_pinned = edges != nullptr;
-      if (!edges) edges = static_cast<lfr_edge*>(std::malloc(e_cap * sizeof(lfr_edge)));
-    }
-    in.edges_out = edges; in.edges_out_capacity = e_cap;
-    lfr_host_stage* hs = nullptr;
-    if (lfr_host_stage_create(&in, &hs, &sz) != LFR_OK) {
-      std::fprintf(stderr, "ERROR: the host graph stage rejected the input\n");
-      return 2;
-    }
-    const uint32_t n = sz.n_nodes, c = sz.n_components;
-    row_ptr.assign((size_t)n + 1, 0); track.resize(n); comp.resize(n); comp_ptr.assign((size_t)c + 1, 0);
-    comp_nodes.resize(n); comp_order.resize(c); node_image.resize(n); node_feat.resize(n); is_root.resize(n);
-    if (lfr_host_stage_export(hs, row_ptr.data(), edges, track.data(), comp.data(), is_root.data(), comp_ptr.data(),
-                              comp_nodes.data(), comp_order.data(), node_image.data(), node_feat.data()) != LFR_OK) {
-      std::fprintf(stderr, "ERROR: lfr_host_stage_export failed\n");
-      return 2;
-    }
-    lfr_host_stage_destroy(hs);
+// Host route, and the device route below the library's size for the decoder on the GPU: the matches of every part
+// decoded into one set of arrays, part after part (the pair level comes out as the walk gave it), each part's
+// mapping released after its decode.  With --listed_pairs the file is decoded once and every listed pair's matches
+// are then copied into place.  Exits 255 when a part does not parse.
+void decode_on_host(Pairs& ps, Matches& m, lfr_host_input& in) {
+  const uint64_t M = ps.M_file;
+  m.feat1.resize(M); m.feat2.resize(M); m.sim.resize(M); m.disp1.resize(18 * M); m.disp2.resize(18 * M);
+  uint64_t m0 = 0;
+  for (Part& pt : ps.parts) {
+    lfr_wire_matches w = pt.pair_level(m.feat1.data() + m0, m.feat2.data() + m0, m.sim.data() + m0,
+                                       m.disp1.data() + 18 * m0, m.disp2.data() + 18 * m0);
+    if (lfr_wire_decode_matches(pt.buf.data(), pt.buf.size(), &w) != LFR_OK)
+      fail(255, "Failed to parse proto object.\n");  // solve.cc:433-436
+    m0 += pt.M;
+    pt.buf.release();  // the file image (several GB at Madrid scale) is not needed past the decode
   }
-  const uint32_t N = sz.n_nodes, C = sz.n_components;
-  const uint64_t E = sz.n_edges;
-  // the host route's problem with the reference's is_root (the update since an earlier run and the record read it)
-  auto host_problem = [&] {
-    lfr_problem p;
-    p.n_nodes = N; p.n_components = C; p.n_edges = E;
-    p.row_ptr = row_ptr.data(); p.edges = edges; p.track = track.data(); p.comp = comp.data();
-    p.is_root = is_root.data(); p.comp_ptr = comp_ptr.data(); p.comp_nodes = comp_nodes.data();
-    return p;
-  };
-  std::printf("# graph nodes: %u\n", N);                                  // solve.cc:484
-  std::printf("# graph edges: %llu\n", (unsigned long long)E);            // solve.cc:485
-  if (N) {
+  if (!ps.file_ptr.empty()) {  // --listed_pairs
+    Matches e;
+    e.feat1.resize(ps.M); e.feat2.resize(ps.M); e.sim.resize(ps.M); e.disp1.resize(18 * ps.M); e.disp2.resize(18 * ps.M);
+    for (uint64_t k = 0; k < ps.P; ++k) {
+      const uint64_t a = ps.file_ptr[ps.src[k]], c = ps.ptr[k + 1] - ps.ptr[k], b = ps.ptr[k];
+      std::copy_n(m.feat1.begin() + a, c, e.feat1.begin() + b);
+      std::copy_n(m.feat2.begin() + a, c, e.feat2.begin() + b);
+      std::copy_n(m.sim.begin() + a, c, e.sim.begin() + b);
+      std::copy_n(m.disp1.begin() + 18 * a, 18 * c, e.disp1.begin() + 18 * b);
+      std::copy_n(m.disp2.begin() + 18 * a, 18 * c, e.disp2.begin() + 18 * b);
+    }
+    m = std::move(e);
+  }
+  in.feat1 = m.feat1.data(); in.feat2 = m.feat2.data(); in.sim = m.sim.data(); in.disp1 = m.disp1.data(); in.disp2 = m.disp2.data();
+}
+
+// Host memory that is page-locked when lfr_host_alloc() gives it (the copies to and from the GPU run at full
+// speed) and malloc'ed otherwise, or malloc'ed alone when not `page_locked`; freed the matching way.
+struct HostFree {
+  bool pinned = false;
+  void operator()(void* p) const { pinned ? lfr_host_free(p) : std::free(p); }
+};
+template <class T>
+using HostArray = std::unique_ptr<T[], HostFree>;
+template <class T>
+HostArray<T> host_array(size_t n, bool page_locked = true) {
+  if (void* p = page_locked ? lfr_host_alloc(n * sizeof(T)) : nullptr) return HostArray<T>(static_cast<T*>(p), HostFree{true});
+  return HostArray<T>(static_cast<T*>(std::malloc(n ? n * sizeof(T) : 1)), HostFree{false});
+}
+
+struct PlanDestroy {
+  void operator()(lfr_plan* p) const { lfr_plan_destroy(p); }
+};
+using PlanPtr = std::unique_ptr<lfr_plan, PlanDestroy>;
+
+// --record_file: this run's problem record (include/lfr_graph.h), from the reference roots, by a size-then-fill
+// call `fill(out, cap)`.  Exits 2 when it fails.
+template <class Fill>
+void problem_record(std::vector<uint8_t>& record, Fill fill) {
+  const int64_t need = fill(nullptr, 0);
+  record.resize(need > 0 ? (size_t)need : 0);
+  const int64_t got = need < 0 ? need : fill(record.data(), record.size());
+  if (got < 0 || (uint64_t)got != record.size())
+    fail(2, "ERROR: the problem record failed (%d): %s\n", (int)got, lfr_last_error());
+}
+
+using Clock = std::chrono::steady_clock;
+
+void print_sizes(const lfr_host_sizes& sz) {
+  std::printf("# graph nodes: %u\n", sz.n_nodes);                          // solve.cc:484
+  std::printf("# graph edges: %llu\n", (unsigned long long)sz.n_edges);    // solve.cc:485
+  if (sz.n_nodes) {
     std::printf("# tracks: %u\n", sz.n_tracks);                           // solve.cc:534
     std::printf("max track size: %u\n", sz.max_track_size);               // solve.cc:549
     std::printf("Graph-cut time: %lldms\n", (long long)sz.graph_cut_ms);  // solve.cc:589
-    std::printf("# components: %u\n", C);                                 // solve.cc:591
+    std::printf("# components: %u\n", sz.n_components);                  // solve.cc:591
     std::printf("max component size: %u\n", sz.max_component_size);       // solve.cc:606
   }
   std::fflush(stdout);
+}
+
+// "Solver time" from `t_solve` and "Total time" (solve.cc:487-641: the graph work and the solve) from `t_start`
+void print_times(Clock::time_point t_start, Clock::time_point t_solve) {
+  const Clock::time_point t_end = Clock::now();
+  auto ms = [](Clock::duration d) { return (long long)std::chrono::duration_cast<std::chrono::milliseconds>(d).count(); };
+  std::printf("Solver time: %lldms\n", ms(t_end - t_solve));  // solve.cc:638
+  std::printf("Total time: %lldms\n", ms(t_end - t_start));   // solve.cc:641
+}
+
+// What a route gives: the SolutionFile of every output k, bytes[off[k], off[k + 1]), the count of
+// solve.cc:666-669 and the problem record
+struct Result {
+  HostArray<uint8_t> bytes;
+  std::vector<uint64_t> off;
+  uint64_t n_outside = 0;
+  std::vector<uint8_t> record;
+  bool encoded = true;  // false: the host route's encoder failed, which solve.cc:674-677 reports as a write failure
+};
+
+// The device route: the graph stage on the GPU (include/lfr_graph.h), from the mapped parts or from `in`'s decoded
+// matches; the problem stays in HBM for the solve and the SolutionFile is encoded there.
+Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps, const Staged& st, StartInputs& si,
+                  size_t n_out, bool decode_on_device, Clock::time_point t_start) {
+  lfr_options opt;
+  lfr_options_default(&opt);
+  opt.device = (int32_t)o.device;
+  // LFR_DEVICE_CUT=1: the recursive cut on the device too (LFR_DBG_DEVICE_CUT; a test and measurement hook)
+  if (const char* e = std::getenv("LFR_DEVICE_CUT")) {
+    if (std::strcmp(e, "1") == 0) opt.debug_flags |= LFR_DBG_DEVICE_CUT;
+  }
+  std::vector<lfr_wire_part> wparts;
+  for (const Part& pt : ps.parts) wparts.push_back(lfr_wire_part{pt.buf.data(), pt.buf.size(), pt.match_off.data(), pt.M});
+  lfr_plan* created = nullptr;
+  lfr_host_sizes sz;
+  const int rc = decode_on_device && lab.kind == Labelling::kLists
+                     ? lfr_plan_create_from_wire_listed(&st.in, wparts.data(), (uint32_t)wparts.size(), ps.file_ptr.data(),
+                                                        ps.file_ptr.size() - 1, ps.src.data(), &opt, nullptr, &created, &sz)
+                 : decode_on_device
+                     ? lfr_plan_create_from_wire(&st.in, wparts.data(), (uint32_t)wparts.size(), &opt, nullptr, &created, &sz)
+                     : lfr_plan_create_from_matches(&st.in, &opt, nullptr, &created, &sz);
+  PlanPtr plan(created);
+  for (Part& pt : ps.parts) pt.buf.release();
+  if (rc == LFR_EINVAL && std::strcmp(lfr_last_error(), "malformed Match message") == 0)
+    fail(255, "Failed to parse proto object.\n");  // solve.cc:433-436, as the host decode
+  if (rc == LFR_EINVAL || rc == LFR_EUNSUPPORTED)  // the input, as the host stage would reject it
+    fail(2, "ERROR: the host graph stage rejected the input\n");
+  if (rc != LFR_OK)  // no device: the host route's message, from the same device check
+    fail(2, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
+
+  // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
+  const uint32_t n_ids = st.n_ids();
+  const uint8_t* names = st.name_blob.data();
+  const uint64_t* name_off = st.name_off.data();
+  const uint8_t* file = si.file.data();
+  const uint64_t file_len = si.file.size();
+  int rc2 = st.any_fixed ? lfr_plan_fix_images(plan.get(), st.fixed.data(), n_ids) : LFR_OK;
+  if (rc2 == LFR_OK && start == Start::kUpdateSinceRecord) {
+    rc2 = lfr_plan_update_solution_since_record(plan.get(), nullptr, file, file_len, n_ids, names, name_off,
+                                                si.earlier_record.data(), si.earlier_record.size(), nullptr, nullptr,
+                                                nullptr);
+  } else if (rc2 == LFR_OK && start == Start::kUpdateSinceMatches) {
+    // the earlier run's graph stage on the device, for the compare only
+    const PreviousMatches& pm = si.previous;
+    const lfr_host_input pin = pm.input();
+    lfr_plan* created_prev = nullptr;
+    rc2 = lfr_plan_create_from_matches(&pin, &opt, nullptr, &created_prev, nullptr);
+    const PlanPtr prev(created_prev);
+    if (rc2 == LFR_OK)
+      rc2 = lfr_plan_update_solution_since(plan.get(), nullptr, file, file_len, n_ids, names, name_off, prev.get(),
+                                           (uint32_t)pm.names.size(), pm.name_blob.data(), pm.name_off.data(), nullptr,
+                                           nullptr, nullptr);
+  } else if (rc2 == LFR_OK && start == Start::kUpdate) {
+    rc2 = lfr_plan_update_solution(plan.get(), nullptr, file, file_len, n_ids, names, name_off, nullptr, nullptr);
+  } else if (rc2 == LFR_OK && start != Start::kZeros) {
+    rc2 = (start == Start::kKeep ? lfr_plan_keep_solution : lfr_plan_start_from_solution)(
+        plan.get(), nullptr, file, file_len, n_ids, names, name_off, nullptr);
+  }
+  if (rc2 != LFR_OK) fail(2, "ERROR: the solve failed (%d): %s\n", rc2, lfr_last_error());
+  print_sizes(sz);
+
+  if (!o.carry_initial_solution) si.file.release();  // carried into the output otherwise
+  const Clock::time_point t_solve = Clock::now();
+  if (sz.n_nodes) {
+    int rc3 = lfr_plan_solve(plan.get(), nullptr);
+    if (rc3 == LFR_OK) rc3 = lfr_plan_download(plan.get(), nullptr, nullptr, nullptr);  // waits for the solve, checks its error flag
+    if (rc3 != LFR_OK) fail(2, "ERROR: the solve failed (%d): %s\n", rc3, lfr_last_error());
+  }
+  print_times(t_start, t_solve);
+
+  Result r;
+  if (o.record_file)
+    problem_record(r.record, [&](uint8_t* out, uint64_t cap) {
+      return lfr_plan_problem_record(plan.get(), nullptr, n_ids, names, name_off, out, cap);
+    });
+
+  // ---- SolutionFile (solve.cc:643-679), encoded on the GPU, names and facts indexed by image id, into
+  // page-locked memory sized by the largest encoding: a Displacement record is at most 18 bytes, an Image's
+  // header 16 plus its name field
+  uint64_t cap = 18ull * sz.n_nodes;
+  cap += 27ull * n_ids + st.name_blob.size();
+  // carried entries: a file's canonical encoding bounds what it adds; a larger need takes a second call
+  if (o.carry_initial_solution) cap += si.file.size();
+  r.off.assign(n_out + 1, 0);
+  std::vector<uint64_t> outside(n_out, 0);
+  const float* fact = st.image_fact.data();
+  auto encode = [&](uint8_t* out, uint64_t c) {
+    return o.carry_initial_solution
+               ? lfr_plan_encode_solution_carried(plan.get(), nullptr, n_ids, names, name_off, fact, si.file.data(),
+                                                  si.file.size(), out, c, &r.n_outside, nullptr)
+           : lab.kind == Labelling::kQueries
+               ? lfr_plan_encode_solution_images(plan.get(), nullptr, n_ids, names, name_off, fact, st.written.data(),
+                                                 out, c, &r.n_outside)
+           : lab.batched()
+               ? lfr_plan_encode_solution_groups(plan.get(), nullptr, n_ids, names, name_off, fact, st.image_group.data(),
+                                                 (uint32_t)n_out, out, c, r.off.data(), outside.data())
+               : lfr_plan_encode_solution(plan.get(), nullptr, n_ids, names, name_off, fact, out, c, &r.n_outside);
+  };
+  r.bytes = host_array<uint8_t>(cap);
+  int64_t need = encode(r.bytes.get(), cap);
+  if (need > 0 && (uint64_t)need > cap) {
+    r.bytes.reset();
+    cap = (uint64_t)need;
+    r.bytes = host_array<uint8_t>(cap);
+    need = encode(r.bytes.get(), cap);
+  }
+  plan.reset();
+  if (need < 0 || (uint64_t)need > cap) fail(2, "ERROR: the solve failed (%d): %s\n", (int)need, lfr_last_error());
+  if (lab.batched())
+    for (uint64_t c : outside) r.n_outside += c;
+  else
+    r.off[1] = (uint64_t)need;
+  return r;
+}
+
+// The host route: the host graph stage (solve.cc:438-606) writing the edge records straight into page-locked
+// memory, the start point joined on the host, lfr_solve() / lfr_solve_multi() and the output assembly.
+Result run_host(const Options& o, Start start, const Labelling& lab, const Pairs& ps, Staged& st, StartInputs& si,
+                size_t n_out, Clock::time_point t_start) {
+  const HostArray<lfr_edge> edges_buf = st.e_cap ? host_array<lfr_edge>(st.e_cap) : nullptr;
+  lfr_edge* edges = edges_buf.get();
+  st.in.edges_out = edges; st.in.edges_out_capacity = st.e_cap;
+  lfr_host_stage* hs = nullptr;
+  lfr_host_sizes sz;
+  if (lfr_host_stage_create(&st.in, &hs, &sz) != LFR_OK) fail(2, "ERROR: the host graph stage rejected the input\n");
+  const uint32_t N = sz.n_nodes, C = sz.n_components;
+  std::vector<uint32_t> row_ptr((size_t)N + 1, 0), track(N), comp(N), comp_ptr((size_t)C + 1, 0), comp_nodes(N),
+      comp_order(C), node_image(N), node_feat(N);
+  std::vector<uint8_t> is_root(N);
+  const int rc = lfr_host_stage_export(hs, row_ptr.data(), edges, track.data(), comp.data(), is_root.data(),
+                                       comp_ptr.data(), comp_nodes.data(), comp_order.data(), node_image.data(),
+                                       node_feat.data());
+  lfr_host_stage_destroy(hs);
+  if (rc != LFR_OK) fail(2, "ERROR: lfr_host_stage_export failed\n");
+  // the problem with the reference's is_root (the update since an earlier run and the record read it)
+  lfr_problem prob;
+  prob.n_nodes = N; prob.n_components = C; prob.n_edges = sz.n_edges;
+  prob.row_ptr = row_ptr.data(); prob.edges = edges; prob.track = track.data(); prob.comp = comp.data();
+  prob.is_root = is_root.data(); prob.comp_ptr = comp_ptr.data(); prob.comp_nodes = comp_nodes.data();
+  print_sizes(sz);
 
   // ---- the solve (solve.cc:608-635): positions start at zero, or from --initial_solution -----
-  double* positions = nullptr;  // host route: the solve's result; the device route keeps it in HBM
-  bool positions_pinned = false;
-  // host route with --fixed_images, --keep_initial_solution or --update_initial_solution: reference roots OR
-  // nodes of fixed images OR nodes with an entry in the start solution (kept) or held by the update
+  const uint32_t n_ids = st.n_ids();
+  const uint8_t* names = st.name_blob.data();
+  const uint64_t* name_off = st.name_off.data();
+  const uint8_t* file = si.file.data();
+  const uint64_t file_len = si.file.size();
+  HostArray<double> positions_buf;
+  double* positions = nullptr;
+  // with --fixed_images, --keep_initial_solution or an update: reference roots OR nodes of fixed images OR nodes
+  // with an entry in the start solution (kept) or held by the update
   std::vector<uint8_t> is_const;
-  const bool any_const = any_fixed || keep_start || update_start;
-  if (N && !plan) {
-    positions = static_cast<double*>(lfr_host_alloc(2ull * N * sizeof(double)));
-    positions_pinned = positions != nullptr;
-    if (!positions) positions = static_cast<double*>(std::malloc(2ull * N * sizeof(double)));
+  const bool any_const = st.any_fixed || holds_entries(start);
+  if (N) {
+    positions_buf = host_array<double>(2ull * N);
+    positions = positions_buf.get();
     std::memset(positions, 0, 2ull * N * sizeof(double));
-    std::vector<uint8_t> has_entry(keep_start || update_start ? N : 0, 0);
-    if (have_earlier) {
-      const lfr_problem cur = host_problem();
-      if (lfr_wire_update_solution_since_record(start_file.data(), start_file.size(), n_ids,
-                                                name_blob.data(), name_off.data(), &cur, node_image.data(), node_feat.data(),
-                                                earlier_record.data(), earlier_record.size(), positions, has_entry.data(),
-                                                nullptr, nullptr, nullptr) != LFR_OK) {
-        std::fprintf(stderr, "ERROR: lfr_wire_update_solution_since_record failed\n");
-        return 2;
-      }
-    } else if (have_previous) {
-      const lfr_problem cur = host_problem();
-      const lfr_host_input pin = previous.input();
-      if (lfr_wire_update_solution_since(start_file.data(), start_file.size(), n_ids, name_blob.data(),
-                                         name_off.data(), &cur, node_image.data(), node_feat.data(), &pin,
-                                         previous.name_blob.data(), previous.name_off.data(), positions, has_entry.data(),
-                                         nullptr, nullptr, nullptr) != LFR_OK) {
-        std::fprintf(stderr, "ERROR: lfr_wire_update_solution_since failed\n");
-        return 2;
-      }
-    } else if (have_start && update_start) {
-      if (lfr_wire_update_solution(start_file.data(), start_file.size(), n_ids, name_blob.data(),
-                                   name_off.data(), N, node_image.data(), node_feat.data(), comp.data(), C, positions,
-                                   has_entry.data(), nullptr, nullptr) != LFR_OK) {
-        std::fprintf(stderr, "ERROR: lfr_wire_update_solution failed\n");
-        return 2;
-      }
-    } else if (have_start && (keep_start ? lfr_wire_join_solution_entries(start_file.data(), start_file.size(), n_ids,
-                                                                  name_blob.data(), name_off.data(), N, node_image.data(),
-                                                                  node_feat.data(), positions, nullptr, has_entry.data())
-                                  : lfr_wire_join_solution(start_file.data(), start_file.size(), n_ids,
-                                                           name_blob.data(), name_off.data(), N, node_image.data(),
-                                                           node_feat.data(), positions, nullptr)) != LFR_OK) {
-      std::fprintf(stderr, "ERROR: lfr_wire_join_solution failed\n");
-      return 2;
+    std::vector<uint8_t> has_entry(holds_entries(start) ? N : 0, 0);
+    if (start == Start::kUpdateSinceRecord) {
+      if (lfr_wire_update_solution_since_record(file, file_len, n_ids, names, name_off, &prob, node_image.data(),
+                                                node_feat.data(), si.earlier_record.data(), si.earlier_record.size(),
+                                                positions, has_entry.data(), nullptr, nullptr, nullptr) != LFR_OK)
+        fail(2, "ERROR: lfr_wire_update_solution_since_record failed\n");
+    } else if (start == Start::kUpdateSinceMatches) {
+      const lfr_host_input pin = si.previous.input();
+      if (lfr_wire_update_solution_since(file, file_len, n_ids, names, name_off, &prob, node_image.data(),
+                                         node_feat.data(), &pin, si.previous.name_blob.data(), si.previous.name_off.data(),
+                                         positions, has_entry.data(), nullptr, nullptr, nullptr) != LFR_OK)
+        fail(2, "ERROR: lfr_wire_update_solution_since failed\n");
+    } else if (start == Start::kUpdate) {
+      if (lfr_wire_update_solution(file, file_len, n_ids, names, name_off, N, node_image.data(), node_feat.data(),
+                                   comp.data(), C, positions, has_entry.data(), nullptr, nullptr) != LFR_OK)
+        fail(2, "ERROR: lfr_wire_update_solution failed\n");
+    } else if (start != Start::kZeros &&
+               (start == Start::kKeep
+                    ? lfr_wire_join_solution_entries(file, file_len, n_ids, names, name_off, N, node_image.data(),
+                                                     node_feat.data(), positions, nullptr, has_entry.data())
+                    : lfr_wire_join_solution(file, file_len, n_ids, names, name_off, N, node_image.data(),
+                                             node_feat.data(), positions, nullptr)) != LFR_OK) {
+      fail(2, "ERROR: lfr_wire_join_solution failed\n");
     }
     if (any_const) {
       is_const.resize(N);
       for (uint32_t v = 0; v < N; ++v)
-        is_const[v] = (is_root[v] || fixed[node_image[v]] || ((keep_start || update_start) && has_entry[v])) ? 1 : 0;
+        is_const[v] = (is_root[v] || st.fixed[node_image[v]] || (holds_entries(start) && has_entry[v])) ? 1 : 0;
     }
   }
-  if (!carry_start) start_file.release();  // carried into the output otherwise
+  if (!o.carry_initial_solution) si.file.release();  // carried into the output otherwise
   const Clock::time_point t_solve = Clock::now();
-  if (N && plan) {
-    int rc = lfr_plan_solve(plan, nullptr);
-    if (rc == LFR_OK) rc = lfr_plan_download(plan, nullptr, nullptr, nullptr);  // waits for the solve, checks its error flag
-    if (rc != LFR_OK) {
-      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
-      return 2;
-    }
-  } else if (N) {
-    lfr_problem prob;
-    prob.n_nodes = N; prob.n_components = C; prob.n_edges = E;
-    prob.row_ptr = row_ptr.data(); prob.edges = edges; prob.track = track.data(); prob.comp = comp.data();
-    prob.is_root = any_const ? is_const.data() : is_root.data(); prob.comp_ptr = comp_ptr.data(); prob.comp_nodes = comp_nodes.data();
+  if (N) {
+    lfr_problem solve_prob = prob;
+    if (any_const) solve_prob.is_root = is_const.data();
     lfr_options opt;
     lfr_options_default(&opt);
-    opt.device = (int32_t)device;
-    lfr_stats st;
-    std::memset(&st, 0, sizeof st);
-    int rc;
-    if (gpus > 1) {
-      std::vector<int32_t> devs((size_t)gpus);
+    opt.device = (int32_t)o.device;
+    lfr_stats stats;
+    std::memset(&stats, 0, sizeof stats);
+    int rc3;
+    if (o.gpus > 1) {
+      std::vector<int32_t> devs((size_t)o.gpus);
       for (size_t i = 0; i < devs.size(); ++i) devs[i] = (int32_t)i;
-      rc = lfr_solve_multi(&prob, &opt, devs.data(), (int32_t)devs.size(), positions, &st, nullptr);
+      rc3 = lfr_solve_multi(&solve_prob, &opt, devs.data(), (int32_t)devs.size(), positions, &stats, nullptr);
     } else {
-      rc = lfr_solve(&prob, &opt, positions, &st);
+      rc3 = lfr_solve(&solve_prob, &opt, positions, &stats);
     }
-    if (rc != LFR_OK) {  // no CPU fallback: without a CUDA device this is where the program stops
-      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
-      return 2;
-    }
+    if (rc3 != LFR_OK)  // no CPU fallback: without a CUDA device this is where the program stops
+      fail(2, "ERROR: the solve failed (%d): %s\n", rc3, lfr_last_error());
   }
-  const Clock::time_point t_end = Clock::now();
-  std::printf("Solver time: %lldms\n", ms_between(t_solve, t_end));  // solve.cc:638
-  std::printf("Total time: %lldms\n", ms_between(t_start, t_end));   // solve.cc:641
+  print_times(t_start, t_solve);
 
-  // ---- --record_file: this run's problem record (include/lfr_graph.h), from the reference roots
-  std::vector<uint8_t> record_out;
-  if (have_record) {
-    int64_t got = -1;
-    if (plan) {
-      const int64_t need_r = lfr_plan_problem_record(plan, nullptr, n_ids, name_blob.data(),
-                                                     name_off.data(), nullptr, 0);
-      record_out.resize(need_r > 0 ? (size_t)need_r : 0);
-      got = need_r < 0 ? need_r
-                       : lfr_plan_problem_record(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
-                                                 record_out.data(), record_out.size());
-    } else {
-      const lfr_problem cur = host_problem();
-      const int64_t need_r = lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), n_ids,
-                                                     name_blob.data(), name_off.data(), nullptr, 0);
-      record_out.resize(need_r > 0 ? (size_t)need_r : 0);
-      got = need_r < 0 ? need_r
-                       : lfr_host_problem_record(&cur, node_image.data(), node_feat.data(), n_ids,
-                                                 name_blob.data(), name_off.data(), record_out.data(), record_out.size());
-    }
-    if (got < 0 || (uint64_t)got != record_out.size()) {
-      std::fprintf(stderr, "ERROR: the problem record failed (%d): %s\n", (int)got, lfr_last_error());
-      return 2;
-    }
-  }
+  Result r;
+  if (o.record_file)
+    problem_record(r.record, [&](uint8_t* out, uint64_t cap) {
+      return lfr_host_problem_record(&prob, node_image.data(), node_feat.data(), n_ids, names, name_off, out, cap);
+    });
 
-  // ---- SolutionFile (solve.cc:643-679): images by first node appearance, nodes by index ------
-  uint64_t n_outside = 0;
-  int64_t need = 0;
-  uint8_t* out = nullptr;
-  bool out_pinned = false;
-  // scene sc's SolutionFile is out[scene_off[sc], scene_off[sc + 1])
-  std::vector<uint64_t> scene_off(S + 1, 0), scene_outside(S, 0);
-  if (plan) {
-    // encoded on the GPU, names and facts indexed by image id, into page-locked memory sized by the
-    // largest encoding: a Displacement record is at most 18 bytes, an Image's header 16 plus its name field
-    uint64_t cap = 18ull * N;
-    cap += 27ull * n_ids + name_blob.size();
-    // carried entries: a file's canonical encoding bounds what it adds; a larger need takes a second call
-    if (carry_start) cap += start_file.size();
-    auto encode = [&](uint8_t* o, uint64_t c) {
-      return carry_start ? lfr_plan_encode_solution_carried(plan, nullptr, n_ids, name_blob.data(),
-                                                            name_off.data(), image_fact.data(), start_file.data(),
-                                                            start_file.size(), o, c, &n_outside, nullptr)
-                         : have_query ? lfr_plan_encode_solution_images(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
-                                                                        image_fact.data(), image_written.data(), o, c, &n_outside)
-                         : batched ? lfr_plan_encode_solution_groups(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
-                                                                         image_fact.data(), image_group.data(), S, o, c,
-                                                                         scene_off.data(), scene_outside.data())
-                         : lfr_plan_encode_solution(plan, nullptr, n_ids, name_blob.data(), name_off.data(),
-                                                    image_fact.data(), o, c, &n_outside);
-    };
-    out = static_cast<uint8_t*>(lfr_host_alloc(cap));
-    out_pinned = out != nullptr;
-    if (!out) out = static_cast<uint8_t*>(std::malloc(cap ? cap : 1));
-    need = encode(out, cap);
-    if (need > 0 && (uint64_t)need > cap) {
-      if (out_pinned) lfr_host_free(out); else std::free(out);
-      cap = (uint64_t)need;
-      out = static_cast<uint8_t*>(lfr_host_alloc(cap));
-      out_pinned = out != nullptr;
-      if (!out) out = static_cast<uint8_t*>(std::malloc(cap));
-      need = encode(out, cap);
+  // ---- SolutionFile (solve.cc:643-679): images by first node appearance, nodes by index.  With --query_images
+  // only the query images are written (a database image's keypoints have one value per query): rank -2 marks the
+  // images left out; every node still counts towards n_outside
+  std::vector<int64_t> rank(n_ids, -1);
+  std::vector<uint32_t> img_ids;
+  for (uint32_t v = 0; v < N; ++v)
+    if (rank[node_image[v]] == -1) {
+      if (!st.written[node_image[v]]) {
+        rank[node_image[v]] = -2;
+        continue;
+      }
+      rank[node_image[v]] = (int64_t)img_ids.size();
+      img_ids.push_back(node_image[v]);
     }
-    lfr_plan_destroy(plan);
-    if (need < 0 || (uint64_t)need > cap) {
-      std::fprintf(stderr, "ERROR: the solve failed (%d): %s\n", (int)need, lfr_last_error());
-      return 2;
+  // with --additional_scenes (--listed_pairs) the images go scene (list) after scene, each one's in the order above
+  std::vector<size_t> out_img(n_out + 1, 0);
+  if (lab.batched()) {
+    std::stable_sort(img_ids.begin(), img_ids.end(),
+                     [&](uint32_t x, uint32_t y) { return st.image_group[x] < st.image_group[y]; });
+    for (size_t i = 0; i < img_ids.size(); ++i) {
+      rank[img_ids[i]] = (int64_t)i;
+      ++out_img[st.image_group[img_ids[i]] + 1];
     }
-    if (batched)
-      for (uint64_t c : scene_outside) n_outside += c;
-    else
-      scene_off[1] = (uint64_t)need;
+    for (size_t k = 0; k < n_out; ++k) out_img[k + 1] += out_img[k];
   } else {
-    // with --query_images only the query images are written (a database image's keypoints have one value
-    // per query): rank -2 marks the images left out; every node still counts towards n_outside
-    std::vector<int64_t> rank(n_ids, -1);
-    std::vector<uint32_t> img_ids;
-    for (uint32_t v = 0; v < N; ++v)
-      if (rank[node_image[v]] == -1) {
-        if (!image_written[node_image[v]]) {
-          rank[node_image[v]] = -2;
-          continue;
-        }
-        rank[node_image[v]] = (int64_t)img_ids.size();
-        img_ids.push_back(node_image[v]);
-      }
-    // with --additional_scenes (--listed_pairs) the images go scene (list) after scene, each one's in the order above
-    std::vector<size_t> scene_img(S + 1, 0);
-    if (batched) {
-      std::stable_sort(img_ids.begin(), img_ids.end(),
-                       [&](uint32_t x, uint32_t y) { return image_group[x] < image_group[y]; });
-      for (size_t i = 0; i < img_ids.size(); ++i) {
-        rank[img_ids[i]] = (int64_t)i;
-        ++scene_img[image_group[img_ids[i]] + 1];
-      }
-      for (uint32_t sc = 0; sc < S; ++sc) scene_img[sc + 1] += scene_img[sc];
-    } else {
-      scene_img[1] = img_ids.size();
-    }
-    const size_t I = img_ids.size();
-    std::vector<uint64_t> img_ptr(I + 1, 0);
-    for (uint32_t v = 0; v < N; ++v)
-      if (rank[node_image[v]] >= 0) ++img_ptr[(size_t)rank[node_image[v]] + 1];
-    for (size_t i = 0; i < I; ++i) img_ptr[i + 1] += img_ptr[i];
-    std::vector<uint32_t> feature_idx(img_ptr[I]);
-    std::vector<float> di(img_ptr[I]), dj(img_ptr[I]);
-    {
-      std::vector<uint64_t> fill(img_ptr.begin(), img_ptr.end() - 1);
-      for (uint32_t v = 0; v < N; ++v) {
-        if (std::fabs(positions[2 * (size_t)v + 1]) > 0.5 || std::fabs(positions[2 * (size_t)v]) > 0.5) ++n_outside;  // solve.cc:666-669
-        if (rank[node_image[v]] < 0) continue;
-        const uint64_t k = fill[(size_t)rank[node_image[v]]]++;
-        feature_idx[k] = node_feat[v];
-        di[k] = (float)positions[2 * (size_t)v];
-        dj[k] = (float)positions[2 * (size_t)v + 1];
-      }
-    }
-    std::vector<uint8_t> out_blob;
-    std::vector<uint64_t> out_off(I + 1, 0);
-    std::vector<float> fact(I);
-    for (size_t i = 0; i < I; ++i) {
-      const std::string& s = names[orig_of[img_ids[i]]];
-      out_blob.insert(out_blob.end(), s.begin(), s.end());
-      out_off[i + 1] = out_blob.size();
-      fact[i] = image_fact[img_ids[i]];
-    }
-    if (out_blob.empty()) out_blob.push_back(0);
-    // the images [a, b) of the output order: one scene's SolutionFile
-    auto encode = [&](size_t a, size_t b, uint8_t* o, uint64_t c) {
-      return carry_start ? lfr_wire_encode_solution_carried(b - a, img_ptr.data() + a, out_blob.data(), out_off.data() + a,
-                                                            fact.data() + a, feature_idx.data(), di.data(), dj.data(),
-                                                            start_file.data(), start_file.size(), o, c, nullptr)
-                         : lfr_wire_encode_solution(b - a, img_ptr.data() + a, out_blob.data(), out_off.data() + a,
-                                                    fact.data() + a, feature_idx.data(), di.data(), dj.data(), o, c);
-    };
-    for (uint32_t sc = 0; sc < S && need >= 0; ++sc) {
-      const int64_t n = encode(scene_img[sc], scene_img[sc + 1], nullptr, 0);
-      need = n < 0 ? -1 : need + n;
-      scene_off[sc + 1] = (uint64_t)need;
-    }
-    out = static_cast<uint8_t*>(std::malloc((size_t)std::max<int64_t>(need, 1)));
-    for (uint32_t sc = 0; sc < S && need >= 0; ++sc) {
-      const uint64_t n = scene_off[sc + 1] - scene_off[sc];
-      if (encode(scene_img[sc], scene_img[sc + 1], out + scene_off[sc], n) != (int64_t)n) need = -1;
+    out_img[1] = img_ids.size();
+  }
+  const size_t I = img_ids.size();
+  std::vector<uint64_t> img_ptr(I + 1, 0);
+  for (uint32_t v = 0; v < N; ++v)
+    if (rank[node_image[v]] >= 0) ++img_ptr[(size_t)rank[node_image[v]] + 1];
+  for (size_t i = 0; i < I; ++i) img_ptr[i + 1] += img_ptr[i];
+  std::vector<uint32_t> feature_idx(img_ptr[I]);
+  std::vector<float> di(img_ptr[I]), dj(img_ptr[I]);
+  {
+    std::vector<uint64_t> fill(img_ptr.begin(), img_ptr.end() - 1);
+    for (uint32_t v = 0; v < N; ++v) {
+      if (std::fabs(positions[2 * (size_t)v + 1]) > 0.5 || std::fabs(positions[2 * (size_t)v]) > 0.5) ++r.n_outside;  // solve.cc:666-669
+      if (rank[node_image[v]] < 0) continue;
+      const uint64_t k = fill[(size_t)rank[node_image[v]]]++;
+      feature_idx[k] = node_feat[v];
+      di[k] = (float)positions[2 * (size_t)v];
+      dj[k] = (float)positions[2 * (size_t)v + 1];
     }
   }
-  start_file.release();
-  std::printf("# points with at least one coordinate > 0.5: %llu\n", (unsigned long long)n_outside);  // solve.cc:670
+  std::vector<uint8_t> out_blob;
+  std::vector<uint64_t> out_off(I + 1, 0);
+  std::vector<float> fact(I);
+  for (size_t i = 0; i < I; ++i) {
+    const std::string& s = ps.names.names[st.orig_of[img_ids[i]]];
+    out_blob.insert(out_blob.end(), s.begin(), s.end());
+    out_off[i + 1] = out_blob.size();
+    fact[i] = st.image_fact[img_ids[i]];
+  }
+  if (out_blob.empty()) out_blob.push_back(0);
+  // the images [a, b) of the output order: one output's SolutionFile
+  auto encode = [&](size_t a, size_t b, uint8_t* out, uint64_t c) {
+    return o.carry_initial_solution
+               ? lfr_wire_encode_solution_carried(b - a, img_ptr.data() + a, out_blob.data(), out_off.data() + a,
+                                                  fact.data() + a, feature_idx.data(), di.data(), dj.data(),
+                                                  si.file.data(), si.file.size(), out, c, nullptr)
+               : lfr_wire_encode_solution(b - a, img_ptr.data() + a, out_blob.data(), out_off.data() + a,
+                                          fact.data() + a, feature_idx.data(), di.data(), dj.data(), out, c);
+  };
+  r.off.assign(n_out + 1, 0);
+  int64_t need = 0;
+  for (size_t k = 0; k < n_out && need >= 0; ++k) {
+    const int64_t n = encode(out_img[k], out_img[k + 1], nullptr, 0);
+    need = n < 0 ? -1 : need + n;
+    r.off[k + 1] = (uint64_t)need;
+  }
+  r.bytes = host_array<uint8_t>((size_t)std::max<int64_t>(need, 1), false);
+  for (size_t k = 0; k < n_out && need >= 0; ++k) {
+    const uint64_t n = r.off[k + 1] - r.off[k];
+    if (encode(out_img[k], out_img[k + 1], r.bytes.get() + r.off[k], n) != (int64_t)n) need = -1;
+  }
+  r.encoded = need >= 0;
+  return r;
+}
+
+int run(int argc, char** argv) {
+  Options o;
+  try {
+    o = parse(argc, argv);
+  } catch (const CliError& e) {  // solve.cc:397-401
+    std::fprintf(stderr, "ERROR: %s\n\n", e.msg.c_str());
+    std::fputs(kUsage, stderr);
+    return 1;
+  }
+  if (o.help) {
+    std::fputs("Patch Match graph problem solver\n\n", stdout);
+    std::fputs(kUsage, stdout);
+    return 0;
+  }
+  check_rules(o);
+  const Start start = start_mode(o);
+  const Labelling lab = labelling(o);
+
+  // the batch's rows, each with its output file second: scene 0 / list 0 is --matches_file / --output_file, then
+  // with --additional_scenes every listed scene (each scene's output is what its own run writes: the same command
+  // with that scene's two files alone), or with --listed_pairs every listed match list (its output is what the same
+  // command writes on a MatchingFile that holds the file's pair for every line of the list, in line order)
+  StringPairs rows{{o.matches_file, o.output_file}};
+  std::vector<StringPairs> lists;
+  if (o.listed_pairs) lists = read_pair_lists(*o.listed_pairs, rows);
+  if (o.additional_scenes) read_tab_list(kSceneList, *o.additional_scenes, rows);
+  StartInputs si;
+  read_start_inputs(o, si);
+
+  // A one-shot process pays for CUDA's start-up (driver initialisation over every visible GPU, context
+  // creation: 0.4-0.8 s on an 8-GPU box) more than for all of its work on a Fountain-scale scene.  Two
+  // measures: only the device that will be used is made visible (unless the caller already chose),
+  // and the start-up runs on a helper thread while the input is read, decoded and turned into a graph.
+  if (o.gpus <= 1 && !std::getenv("CUDA_VISIBLE_DEVICES")) {
+    setenv("CUDA_VISIBLE_DEVICES", std::to_string(o.device).c_str(), 1);
+    o.device = 0;
+  }
+  std::thread cuda_start([] { lfr_host_free(lfr_host_alloc(64)); });
+  struct Joiner {
+    std::thread& t;
+    ~Joiner() { if (t.joinable()) t.join(); }
+  } join_on_exit{cuda_start};
+
+  Pairs ps = read_pairs(o.listed_pairs ? StringPairs{rows[0]} : rows);  // the lists' pairs are --matches_file's
+  if (o.listed_pairs) select_listed_pairs(ps, rows, lists);
+  Staged st = stage(ps, o, lab);
+  const bool on_device = device_route(st.in, o.gpus);
+  // the decoder's threshold sees the file's match count
+  const bool decode_on_device = on_device && lfr_wire_decode_on_device(ps.M_file) == 1;
+  Matches matches;
+  if (!decode_on_device) decode_on_host(ps, matches, st.in);
+
+  cuda_start.join();  // page-locked memory needs the context
+  const Clock::time_point t_start = Clock::now();
+  Result r = on_device ? run_device(o, start, lab, ps, st, si, rows.size(), decode_on_device, t_start)
+                       : run_host(o, start, lab, ps, st, si, rows.size(), t_start);
+  si.file.release();
+  std::printf("# points with at least one coordinate > 0.5: %llu\n", (unsigned long long)r.n_outside);  // solve.cc:670
   std::fflush(stdout);
-  bool written = need >= 0;
-  for (uint32_t sc = 0; written && sc < S; ++sc) {  // in scene order; the first failure ends the run
-    std::ofstream f(scenes[sc].second, std::ios::binary | std::ios::trunc);
+  bool written = r.encoded;
+  for (size_t k = 0; written && k < rows.size(); ++k) {  // in row order; the first failure ends the run
+    std::ofstream f(rows[k].second, std::ios::binary | std::ios::trunc);
     written = f.good();
-    const uint64_t n = scene_off[sc + 1] - scene_off[sc];
-    if (written && n) f.write(reinterpret_cast<const char*>(out + scene_off[sc]), (std::streamsize)n);
+    const uint64_t n = r.off[k + 1] - r.off[k];
+    if (written && n) f.write(reinterpret_cast<const char*>(r.bytes.get() + r.off[k]), (std::streamsize)n);
     written = written && f.good();
   }
-  if (positions_pinned) lfr_host_free(positions); else std::free(positions);
-  if (edges_pinned) lfr_host_free(edges); else std::free(edges);
-  if (out_pinned) lfr_host_free(out); else std::free(out);
-  if (!written) {
-    std::fputs("Failed to write proto object.\n", stderr);  // solve.cc:674-677
-    return 255;
-  }
-  if (have_record) {
-    std::ofstream f(record_file, std::ios::binary | std::ios::trunc);
-    if (f.good()) f.write(reinterpret_cast<const char*>(record_out.data()), (std::streamsize)record_out.size());
-    if (!f.good()) {
-      std::fprintf(stderr, "ERROR: cannot write the record file '%s'\n", record_file.c_str());
-      return 255;
-    }
+  if (!written) fail(255, "Failed to write proto object.\n");  // solve.cc:674-677
+  if (o.record_file) {
+    std::ofstream f(*o.record_file, std::ios::binary | std::ios::trunc);
+    if (f.good()) f.write(reinterpret_cast<const char*>(r.record.data()), (std::streamsize)r.record.size());
+    if (!f.good()) fail(255, "ERROR: cannot write the record file '%s'\n", o.record_file->c_str());
   }
   return 0;
+}
+
+}  // namespace
+
+int main(int argc, char** argv) {
+  try {
+    return run(argc, argv);
+  } catch (const Exit& e) {
+    return e.code;
+  }
 }
