@@ -539,6 +539,22 @@ class Plan:
                        "lfr_plan_export_graph")
         return out
 
+    def _encode(self, name, args, outs, cap=0):
+        """The size protocol of the lfr_plan_encode_solution* calls: name(*args, out, cap, *outs) into a buffer of
+        `cap` bytes (none when 0), and once more into a buffer of the returned size when that is larger.
+        Returns the bytes."""
+        f = getattr(self.lib.lib, name)
+        out = np.empty(max(cap, 1), np.uint8)
+        need = f(*args, out.ctypes.data if cap else None, cap, *outs)
+        if need < 0:
+            self.lib.check(int(need), name)
+        if need > cap:
+            out = np.empty(int(need), np.uint8)
+            got = f(*args, out.ctypes.data, int(need), *outs)
+            if got != need:
+                self.lib.check(int(got) if got < 0 else -1, name)
+        return out[:need].tobytes()
+
     def encode_solution(self, image_names, image_fact, stream: int = 0):
         """lfr_plan_encode_solution (include/lfr_graph.h): the SolutionFile of a plan made by from_matches() or
         from_wire(), encoded on the device from its current positions.  `image_names` / `image_fact` are indexed
@@ -549,17 +565,11 @@ class Plan:
         fact = np.ascontiguousarray(image_fact, dtype=np.float32).reshape(-1)
         if fact.shape[0] != len(image_names):
             raise ValueError("image_fact has %d entries for %d image names" % (fact.shape[0], len(image_names)))
-        f = self.lib.lib.lfr_plan_encode_solution
         n_out = C.c_uint64()
-        args = (self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data, _ptr(fact))
-        need = f(*args, None, 0, C.byref(n_out))
-        if need < 0:
-            self.lib.check(int(need), "lfr_plan_encode_solution")
-        out = np.empty(max(int(need), 1), np.uint8)
-        got = f(*args, out.ctypes.data, int(need), C.byref(n_out))
-        if got != need:
-            self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution")
-        return out[:need].tobytes(), int(n_out.value)
+        data = self._encode("lfr_plan_encode_solution", (self.handle, C.c_void_p(stream), len(image_names),
+                                                         blob.ctypes.data, off.ctypes.data, _ptr(fact)),
+                            (C.byref(n_out),))
+        return data, int(n_out.value)
 
     def encode_solution_groups(self, image_names, image_fact, image_group, n_groups: int, stream: int = 0):
         """lfr_plan_encode_solution_groups (include/lfr_graph.h): one SolutionFile per image group, encoded on the
@@ -573,17 +583,10 @@ class Plan:
             raise ValueError("image_fact / image_group do not have one entry per image name")
         goff = np.zeros(n_groups + 1, np.uint64)
         n_out = np.zeros(max(n_groups, 1), np.uint64)
-        f = self.lib.lib.lfr_plan_encode_solution_groups
-        args = (self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data, _ptr(fact),
-                _ptr(group), n_groups)
-        need = f(*args, None, 0, goff.ctypes.data, n_out.ctypes.data)
-        if need < 0:
-            self.lib.check(int(need), "lfr_plan_encode_solution_groups")
-        out = np.empty(max(int(need), 1), np.uint8)
-        got = f(*args, out.ctypes.data, int(need), goff.ctypes.data, n_out.ctypes.data)
-        if got != need:
-            self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution_groups")
-        data = out[:need].tobytes()
+        data = self._encode("lfr_plan_encode_solution_groups", (self.handle, C.c_void_p(stream), len(image_names),
+                                                                blob.ctypes.data, off.ctypes.data, _ptr(fact),
+                                                                _ptr(group), n_groups),
+                            (goff.ctypes.data, n_out.ctypes.data))
         return [data[int(goff[g]):int(goff[g + 1])] for g in range(n_groups)], [int(x) for x in n_out[:n_groups]]
 
     def encode_solution_carried(self, image_names, image_fact, carry: bytes, stream: int = 0):
@@ -596,23 +599,15 @@ class Plan:
         if fact.shape[0] != len(image_names):
             raise ValueError("image_fact has %d entries for %d image names" % (fact.shape[0], len(image_names)))
         buf = np.frombuffer(carry, dtype=np.uint8)
-        f = self.lib.lib.lfr_plan_encode_solution_carried
         n_out, n_car = C.c_uint64(), C.c_uint64()
-        args = (self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data, _ptr(fact),
-                buf.ctypes.data if buf.size else None, buf.size)
         # one call into a buffer of the scene's largest encoding plus the file's size (what a canonical file
         # can add); a larger need takes a second call
         cap = 18 * self.n_nodes + int(off[-1]) + 27 * len(image_names) + buf.size
-        out = np.empty(max(cap, 1), np.uint8)
-        need = f(*args, out.ctypes.data, cap, C.byref(n_out), C.byref(n_car))
-        if need < 0:
-            self.lib.check(int(need), "lfr_plan_encode_solution_carried")
-        if need > cap:
-            out = np.empty(int(need), np.uint8)
-            got = f(*args, out.ctypes.data, int(need), C.byref(n_out), C.byref(n_car))
-            if got != need:
-                self.lib.check(int(got) if got < 0 else -1, "lfr_plan_encode_solution_carried")
-        return out[:need].tobytes(), int(n_out.value), int(n_car.value)
+        data = self._encode("lfr_plan_encode_solution_carried", (self.handle, C.c_void_p(stream), len(image_names),
+                                                                 blob.ctypes.data, off.ctypes.data, _ptr(fact),
+                                                                 buf.ctypes.data if buf.size else None, buf.size),
+                            (C.byref(n_out), C.byref(n_car)), cap)
+        return data, int(n_out.value), int(n_car.value)
 
     def fix_images(self, fixed_by_image_id) -> None:
         """lfr_plan_fix_images (include/lfr_graph.h): hold every node of the images with a non-zero entry of

@@ -32,7 +32,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 OUT_EXE = os.path.join(ROOT, "multi-view-refinement", "build", "solve_native")
 INC = os.path.join("..", "..", "include")
 # build.py itself: a change of NVCC_FLAGS (e.g. the target architecture) must rebuild the library
-DEPS = SOURCES + ["build.py", "lfr_setup.cuh", "lfr_solve_warp.cuh", "lfr_solve_warp2.cuh", "lfr_solve_cta.cuh", "lfr_lm.cuh", "lfr_math.cuh", "lfr_graph.cuh", "lfr_wire.cuh", "lfr_solution.cuh", "lfr_carry.cuh", "lfr_diff.cuh", "lfr_record.h", "lfr_record.cuh", "lfr_cut.h", "lfr_cut.cuh", "lfr_join.h", "lfr_start.cuh",
+DEPS = SOURCES + ["build.py", "lfr_setup.cuh", "lfr_solve_warp.cuh", "lfr_solve_warp2.cuh", "lfr_solve_cta.cuh", "lfr_lm.cuh", "lfr_math.cuh", "lfr_graph.cuh", "lfr_wire.cuh", "lfr_solution.cuh", "lfr_diff.cuh", "lfr_record.h", "lfr_record.cuh", "lfr_cut.h", "lfr_cut.cuh", "lfr_join.h", "lfr_start.cuh",
                   os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_graph.h"), os.path.join(INC, "lfr_host.h"),
                   os.path.join(INC, "lfr_wire.h")]
 HOST_DEPS = HOST_SOURCES + ["lfr_cut.h", "lfr_join.h", "lfr_record.h", os.path.join(INC, "lfr.h"), os.path.join(INC, "lfr_wire.h"),

@@ -3,6 +3,7 @@
 // launches, and result download.  No CPU fallback: every entry point that
 // computes fails with LFR_ENODEV / LFR_ECUDA when no device is usable.
 #include <algorithm>
+#include <cassert>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -15,7 +16,6 @@
 #include <vector>
 
 #include "../../include/lfr_graph.h"
-#include "lfr_carry.cuh"
 #include "lfr_cut.h"
 #include "lfr_cut.cuh"
 #include "lfr_diff.cuh"
@@ -2014,90 +2014,237 @@ int download(lfr_plan* pl, cudaStream_t s, double* positions, lfr_stats* st) {
 }
 
 // {kernels and the upload of names and facts, device-to-host copy of the bytes} in ms of the calling
-// thread's last lfr_plan_encode_solution() that wrote its output
+// thread's last lfr_plan_encode_solution* call that wrote its output
 thread_local double g_encode_ms[2] = {};
 
-// lfr_plan_encode_solution() on a checked plan and arguments (lfr_solution.cuh): the sizing kernels, one
-// synchronisation for the total, then — when `out` has room — the writing kernels and one copy to `out`
-int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t* names, const uint64_t* name_off,
-                        const float* fact, uint8_t* out, uint64_t cap, uint64_t* n_outside, const uint8_t* written = nullptr) {
-  using namespace lfr::solution;
-  const uint32_t N = pl->N;
-  if (n_outside) *n_outside = 0;
-  if (!N) return 0;
-  const auto t0 = Clock::now();
-  const uint64_t name_bytes = name_off[NI];
-  // one scratch buffer carved at 256-byte boundaries: per-image arrays, the uploaded names, per-node arrays
+// Device arrays carved out of one buffer at 256-byte boundaries: `lay` takes every array in turn with
+// take<T>(count); it runs once to size the buffer and once more to place the arrays in it.
+struct Carve {
+  uintptr_t base = 0;
   size_t at = 0;
-  auto take = [&at](size_t bytes) {
-    const size_t o = at;
-    at += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_first = take(4 * (size_t)NI), o_first_s = take(4 * (size_t)NI), o_iota_i = take(4 * (size_t)NI),
-               o_img_s = take(4 * (size_t)NI), o_rank = take(4 * (size_t)NI), o_img_ptr = take(4 * ((size_t)NI + 1)),
-               o_ctr = take(16), o_body = take(8 * (size_t)NI), o_isize = take(8 * ((size_t)NI + 1)),
-               o_ioff = take(8 * ((size_t)NI + 1)), o_name_off = take(8 * ((size_t)NI + 1)), o_fact = take(4 * (size_t)NI),
-               o_names = take(name_bytes), o_key = take(4 * (size_t)N), o_key_s = take(4 * (size_t)N),
-               o_iota = take(4 * (size_t)N), o_perm = take(4 * (size_t)N), o_rsize = take(8 * ((size_t)N + 1)),
-               o_noff = take(8 * ((size_t)N + 1)), o_written = take(written ? NI : 0);
-  LFR_TRY(pl->enc_scratch.reserve(at));
-  uint8_t* base = pl->enc_scratch.as<uint8_t>();
-  auto u32 = [base](size_t o) { return reinterpret_cast<uint32_t*>(base + o); };
-  auto u64 = [base](size_t o) { return reinterpret_cast<uint64_t*>(base + o); };
-  uint32_t *first = u32(o_first), *first_s = u32(o_first_s), *iota_i = u32(o_iota_i), *img_s = u32(o_img_s),
-           *rank = u32(o_rank), *img_ptr = u32(o_img_ptr), *n_present = u32(o_ctr + 8), *n_written = u32(o_ctr + 12), *key = u32(o_key),
-           *key_s = u32(o_key_s), *iota = u32(o_iota), *perm = u32(o_perm);
-  uint64_t *body = u64(o_body), *isize = u64(o_isize), *ioff = u64(o_ioff), *d_name_off = u64(o_name_off),
-           *rsize = u64(o_rsize), *noff = u64(o_noff);
-  unsigned long long* d_outside = reinterpret_cast<unsigned long long*>(base + o_ctr);
-  float* d_fact = reinterpret_cast<float*>(base + o_fact);
-  uint8_t* d_names = base + o_names;
+  template <typename T>
+  T* take(size_t count) {
+    T* p = reinterpret_cast<T*>(base + at);
+    at += (sizeof(T) * count + 255) & ~(size_t)255;
+    return p;
+  }
+};
+
+template <typename F>
+int carve(DevBuf& buf, F&& lay) {
+  Carve c;
+  lay(c);
+  LFR_TRY(buf.reserve(c.at));
+  c = Carve{reinterpret_cast<uintptr_t>(buf.p), 0};
+  lay(c);
+  return LFR_OK;
+}
+
+// The checks of every call that reads the scene's image names, in this order: a plan made from matches,
+// n_images, the caller's NULL arguments (`missing`: the message for the one found, or NULL), ascending
+// name_off (and, with `group`, every image's group below G) and names.
+int check_names(const lfr_plan* pl, uint32_t n_images, const uint8_t* names, const uint64_t* name_off, const char* missing,
+                const uint32_t* group = nullptr, uint32_t G = 0) {
+  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
+  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
+  if (missing) return fail(LFR_EINVAL, missing);
+  for (uint32_t k = 0; k < n_images; ++k) {
+    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
+    if (group && group[k] >= G) return fail(LFR_EINVAL, "an image's group is not below n_groups");
+  }
+  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  return LFR_OK;
+}
+
+// What an lfr_plan_encode_solution* call encodes: the scene's image names and facts; optionally a group per
+// image (one of G; G or more: the image is not written); optionally an earlier SolutionFile to carry, its
+// bytes and their decode (G = 1 only).
+struct EncodeInput {
+  uint32_t n_images;
+  const uint8_t* names;
+  const uint64_t* name_off;
+  const float* fact;
+  const uint32_t* group = nullptr;
+  uint32_t G = 1;
+  const uint8_t* file = nullptr;
+  const lfr::join::Decoded* decoded = nullptr;
+};
+
+// Every lfr_plan_encode_solution* call on a checked plan and input (lfr_solution.cuh): the sizing kernels
+// (with a file, one synchronisation for the carried count among them), one synchronisation for the sizes,
+// then, when `out` has room, the writing kernels, one synchronisation and one copy to `out`.  Host outputs:
+// group_off[0..G], n_outside[0..G] (slot G: the images not written) and *n_carried.
+int64_t encode_solution(lfr_plan* pl, cudaStream_t s, const EncodeInput& in, uint8_t* out, uint64_t cap,
+                        uint64_t* group_off, uint64_t* n_outside, uint64_t* n_carried) {
+  using namespace lfr::solution;
+  const lfr::join::Decoded* d = in.decoded;
+  assert(!d || in.G == 1);  // no call carries a file into several groups
+  const uint32_t N = pl->N, NI = in.n_images, G = in.G;
+  const uint32_t D = d ? (uint32_t)d->n_disp : 0, I = d ? (uint32_t)d->n_images : 0;
+  std::fill(group_off, group_off + G + 1, 0);
+  std::fill(n_outside, n_outside + G + 1, 0);
+  *n_carried = 0;
+  if (!N && !d) return 0;
+  const auto t0 = Clock::now();
+  // per message of the file: its key image (the scene id of a matched winner, NI + j for the j-th other
+  // winner, kNoImage for a message that loses to a later one of its name), and the winners' names
+  std::vector<uint32_t> msg_pid(I, kNoImage);
+  std::vector<uint64_t> msg_name_off((size_t)I + 1, 0);
+  std::vector<uint8_t> msg_names;
+  uint64_t n_other = 0;
+  for (uint32_t i = 0; i < I; ++i) {
+    if (d->wins[i]) {
+      msg_pid[i] = d->image_id[i] != lfr::join::kNoImage ? d->image_id[i] : (uint32_t)(NI + n_other++);
+      msg_names.insert(msg_names.end(), in.file + d->name_off[i], in.file + d->name_off[i] + d->name_len[i]);
+    }
+    msg_name_off[(size_t)i + 1] = msg_names.size();
+  }
+  if ((uint64_t)NI + n_other >= kNoImage) return fail(LFR_EUNSUPPORTED, "too many images in the scene and the SolutionFile");
+  const uint64_t name_bytes = in.name_off[NI];
+  const uint32_t n_max = NI + I;  // an upper bound of the output images
+  // an image's key: group << shift | its first node; an absent image's sorts after every group's images
+  const int shift = bits_for(N);
+  const unsigned long long absent = (unsigned long long)G << shift | N;
+
+  unsigned long long *d_outside, *key, *key_s, *ekey, *ekey_s;
+  uint32_t *n_present, *iota_i, *img_s, *rank, *d_group, *mpid, *g2, *g2_off, *g2_msg, *feat, *idx, *idx_s, *flag, *slot,
+      *ce, *cm, *rkey, *rkey_s, *riota, *perm, *img_ptr;
+  uint64_t *d_name_off, *mptr, *mnoff, *rsize, *roff, *body, *isize, *ioff, *goff;
+  float *d_fact, *mfact, *di, *dj;
+  uint8_t *d_names, *mnames, *used;
+  // per scene image, per message, per entry, per record (N + at most D) and per output image
+  LFR_TRY(carve(pl->enc_scratch, [&](Carve& c) {
+    d_outside = c.take<unsigned long long>((size_t)G + 2);  // then n_present and n_out
+    key = c.take<unsigned long long>(NI);
+    key_s = c.take<unsigned long long>(NI);
+    iota_i = c.take<uint32_t>(NI);
+    img_s = c.take<uint32_t>(NI);
+    rank = c.take<uint32_t>(NI);
+    d_name_off = c.take<uint64_t>((size_t)NI + 1);
+    d_fact = c.take<float>(NI);
+    d_names = c.take<uint8_t>(name_bytes);
+    d_group = c.take<uint32_t>(in.group ? NI : 0);
+    mptr = c.take<uint64_t>((size_t)I + 1);
+    mpid = c.take<uint32_t>(I);
+    mnoff = c.take<uint64_t>((size_t)I + 1);
+    mfact = c.take<float>(I);
+    mnames = c.take<uint8_t>(msg_names.size());
+    g2 = c.take<uint32_t>((size_t)I + 1);
+    g2_off = c.take<uint32_t>((size_t)I + 1);
+    g2_msg = c.take<uint32_t>(I);
+    feat = c.take<uint32_t>(D);
+    di = c.take<float>(D);
+    dj = c.take<float>(D);
+    ekey = c.take<unsigned long long>(D);
+    ekey_s = c.take<unsigned long long>(D);
+    idx = c.take<uint32_t>(D);
+    idx_s = c.take<uint32_t>(D);
+    used = c.take<uint8_t>(D);
+    flag = c.take<uint32_t>((size_t)D + 1);
+    slot = c.take<uint32_t>((size_t)D + 1);
+    ce = c.take<uint32_t>(D);
+    cm = c.take<uint32_t>(D);
+    rkey = c.take<uint32_t>((size_t)N + D);
+    rkey_s = c.take<uint32_t>((size_t)N + D);
+    riota = c.take<uint32_t>((size_t)N + D);
+    perm = c.take<uint32_t>((size_t)N + D);
+    rsize = c.take<uint64_t>((size_t)N + D + 1);
+    roff = c.take<uint64_t>((size_t)N + D + 1);
+    img_ptr = c.take<uint32_t>((size_t)n_max + 1);
+    body = c.take<uint64_t>(n_max);
+    isize = c.take<uint64_t>((size_t)n_max + 1);
+    ioff = c.take<uint64_t>((size_t)n_max + 1);
+    goff = c.take<uint64_t>((size_t)G + 1);
+  }));
+  n_present = reinterpret_cast<uint32_t*>(d_outside + G + 1);
+  uint32_t* n_out = d ? n_present + 1 : n_present;  // the output images: the present ones, then the file's others
+  if (!in.group) d_group = nullptr;
   const uint32_t* nimg = pl->node_image.as<uint32_t>();
-  const uint32_t* nfeat = pl->node_feat.as<uint32_t>();
   const double* pos = pl->pos.as<double>();
 
-  LFR_CUDA(cudaMemcpyAsync(d_name_off, name_off, 8 * ((size_t)NI + 1), cudaMemcpyHostToDevice, s));
-  LFR_CUDA(cudaMemcpyAsync(d_fact, fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
-  if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, names, name_bytes, cudaMemcpyHostToDevice, s));
-  LFR_CUDA(cudaMemsetAsync(base + o_ctr, 0, 16, s));
-  const uint8_t* d_written = written ? base + o_written : nullptr;
-  if (written) LFR_CUDA(cudaMemcpyAsync(base + o_written, written, NI, cudaMemcpyHostToDevice, s));
-  init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
-  first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside, d_written);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {
-    return cub::DeviceRadixSort::SortPairs(t, nb, first, first_s, iota_i, img_s, (int)NI, 0, bits_for(N), s);
-  }));
-  rank_kernel<<<blocks_for(NI), 256, 0, s>>>(first_s, img_s, NI, N, rank, n_present);
-  node_key_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, rank, N, key, iota, d_written, NI, n_written);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: ascending node index within an image
-    return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, iota, perm, (int)N, 0, bits_for(NI), s);
-  }));
-  // the written nodes lead the sorted order; the others get no record
-  uint32_t NW = N;
-  if (written) LFR_TRY(fetch(&NW, n_written, 1, s));
-  if (NW) {
-    record_size_kernel<<<blocks_for(NW), 256, 0, s>>>(perm, key_s, nfeat, pos, NW, rsize, img_ptr);
+  LFR_CUDA(cudaMemsetAsync(d_outside, 0, 8 * ((size_t)G + 2), s));
+  LFR_CUDA(cudaMemcpyAsync(d_name_off, in.name_off, 8 * ((size_t)NI + 1), cudaMemcpyHostToDevice, s));
+  if (NI) LFR_CUDA(cudaMemcpyAsync(d_fact, in.fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
+  if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, in.names, name_bytes, cudaMemcpyHostToDevice, s));
+  if (d_group && NI) LFR_CUDA(cudaMemcpyAsync(d_group, in.group, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
+  // the present images, ranked by (group, first node)
+  if (NI) {
+    init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(key, iota_i, NI, absent);
+    if (N) first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, d_group, G, shift, key, d_outside);
     LFR_LAUNCHED();
-  } else {
-    LFR_CUDA(cudaMemsetAsync(rsize, 0, 8, s));
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, iota_i, img_s, (int)NI, 0, shift + bits_for(G), s);
+    }));
+    rank_kernel<<<blocks_for(NI), 256, 0, s>>>(key_s, img_s, NI, absent, rank, n_present);
+    LFR_LAUNCHED();
   }
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, noff, (int)NW + 1, s); }));
-  image_size_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(img_s, img_ptr, noff, d_name_off, d_fact, n_present, NI, body, isize);
+  // the file's entries: keyed, sorted stably, joined to the nodes, the carried ones compacted; its other
+  // winning messages ranked after the present scene images in file order
+  uint32_t C = 0;
+  if (d) {
+    LFR_CUDA(cudaMemcpyAsync(mptr, d->img_ptr.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
+    LFR_CUDA(cudaMemcpyAsync(mnoff, msg_name_off.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
+    if (I) {
+      LFR_CUDA(cudaMemcpyAsync(mpid, msg_pid.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
+      LFR_CUDA(cudaMemcpyAsync(mfact, d->fact.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
+    }
+    if (!msg_names.empty()) LFR_CUDA(cudaMemcpyAsync(mnames, msg_names.data(), msg_names.size(), cudaMemcpyHostToDevice, s));
+    if (D) {
+      LFR_CUDA(cudaMemcpyAsync(feat, d->feature_idx.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+      LFR_CUDA(cudaMemcpyAsync(di, d->di.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+      LFR_CUDA(cudaMemcpyAsync(dj, d->dj.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
+      LFR_CUDA(cudaMemsetAsync(used, 0, D, s));
+      lfr::start::solution_key_kernel<<<blocks_for(D), 256, 0, s>>>(mptr, mpid, I, feat, D, ekey, idx);
+      LFR_LAUNCHED();
+      LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: equal keys stay in file order
+        return cub::DeviceRadixSort::SortPairs(t, nb, ekey, ekey_s, idx, idx_s, (int)D, 0, 64, s);
+      }));
+      if (N) consume_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pl->node_feat.as<uint32_t>(), N, ekey_s, D, used);
+      carry_flag_kernel<<<blocks_for((uint64_t)D + 1), 256, 0, s>>>(ekey_s, used, D, flag);
+      LFR_LAUNCHED();
+      LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, flag, slot, (int)D + 1, s); }));
+      carry_compact_kernel<<<blocks_for(D), 256, 0, s>>>(flag, slot, idx_s, mptr, I, D, ce, cm);
+      LFR_LAUNCHED();
+      LFR_TRY(fetch(&C, slot + D, 1, s));
+    }
+    group2_flag_kernel<<<blocks_for((uint64_t)I + 1), 256, 0, s>>>(mpid, I, key, NI, absent, g2);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, g2, g2_off, (int)I + 1, s); }));
+    group2_scatter_kernel<<<blocks_for((uint64_t)I + 1), 256, 0, s>>>(g2, g2_off, I, n_present, g2_msg, n_out);
+    LFR_LAUNCHED();
+  }
+  // the records (nodes, then carried entries) in output order, their sizes and the images'
+  const uint32_t R = N + C;
+  const Records rec{N, pl->node_feat.as<uint32_t>(), pos, ce, feat, di, dj};
+  const Headers hdr{n_present, img_s, d_names, d_name_off, d_fact, g2_msg, mnames, mnoff, mfact};
+  if (R) {
+    record_key_kernel<<<blocks_for(R), 256, 0, s>>>(nimg, d_group, G, rank, N, cm, mpid, g2, g2_off, n_present, R, n_max,
+                                                     rkey, riota);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: nodes by index, then carried entries by feature
+      return cub::DeviceRadixSort::SortPairs(t, nb, rkey, rkey_s, riota, perm, (int)R, 0, bits_for(n_max), s);
+    }));
+  }
+  record_size_kernel<<<blocks_for((uint64_t)R + 1), 256, 0, s>>>(perm, rkey_s, R, rec, n_out, rsize, img_ptr);
   LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)NI + 1, s); }));
-  uint64_t total = 0;
-  unsigned long long outside = 0;
-  LFR_CUDA(cudaMemcpyAsync(&outside, d_outside, 8, cudaMemcpyDeviceToHost, s));
-  LFR_TRY(fetch(&total, ioff + NI, 1, s));
-  if (n_outside) *n_outside = outside;
-  if (!out || cap < total) return (int64_t)total;
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, roff, (int)R + 1, s); }));
+  image_size_kernel<<<blocks_for((uint64_t)n_max + 1), 256, 0, s>>>(hdr, img_ptr, roff, n_out, n_max, body, isize);
+  LFR_LAUNCHED();
+  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)n_max + 1, s); }));
+  // one group: {0, the total}
+  if (G > 1) {
+    group_off_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(key_s, NI, shift, G, ioff, goff);
+    LFR_LAUNCHED();
+  }
+  LFR_CUDA(cudaMemcpyAsync(n_outside, d_outside, 8 * ((size_t)G + 1), cudaMemcpyDeviceToHost, s));
+  LFR_TRY(G > 1 ? fetch(group_off, goff, (size_t)G + 1, s) : fetch(group_off + 1, ioff + n_max, 1, s));
+  const uint64_t total = group_off[G];
+  *n_carried = C;
+  if (!out || cap < total || !total) return (int64_t)total;
   LFR_TRY(pl->enc_out.reserve(total));
   uint8_t* d_out = pl->enc_out.as<uint8_t>();
-  write_images_kernel<<<blocks_for(NI), 256, 0, s>>>(img_s, body, ioff, d_names, d_name_off, d_fact, n_present, d_out);
-  if (NW) write_records_kernel<<<blocks_for(NW), 256, 0, s>>>(perm, key_s, nfeat, pos, img_ptr, noff, ioff, NW, d_out);
+  if (n_max) write_images_kernel<<<blocks_for(n_max), 256, 0, s>>>(hdr, body, ioff, n_out, n_max, d_out);
+  if (R) write_records_kernel<<<blocks_for(R), 256, 0, s>>>(perm, rkey_s, R, rec, img_ptr, roff, ioff, n_out, d_out);
   LFR_LAUNCHED();
   LFR_CUDA(cudaStreamSynchronize(s));
   g_encode_ms[0] = ms_since(t0);
@@ -2107,96 +2254,14 @@ int64_t encode_solution(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t
   return (int64_t)total;
 }
 
-// lfr_plan_encode_solution_groups() on a checked plan and arguments (lfr_solution.cuh): encode_solution()'s
-// kernels on the images ranked by (group, first node), so that the groups' SolutionFiles are consecutive
-// ranges of one output; the group offsets and counts come back with the total
-int64_t encode_solution_groups(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t* names, const uint64_t* name_off,
-                               const float* fact, const uint32_t* group_of_image, uint32_t G, uint8_t* out, uint64_t cap,
-                               uint64_t* group_off, uint64_t* n_outside) {
-  using namespace lfr::solution;
-  const uint32_t N = pl->N;
-  if (!N) {
-    std::memset(group_off, 0, 8 * ((size_t)G + 1));
-    std::memset(n_outside, 0, 8 * (size_t)G);
-    return 0;
-  }
-  const uint64_t name_bytes = name_off[NI];
-  size_t at = 0;
-  auto take = [&at](size_t bytes) {
-    const size_t o = at;
-    at += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_first = take(4 * (size_t)NI), o_key = take(8 * (size_t)NI), o_key_s = take(8 * (size_t)NI),
-               o_iota_i = take(4 * (size_t)NI), o_img_s = take(4 * (size_t)NI), o_present = take(4 * ((size_t)NI + 1)),
-               o_dense = take(4 * ((size_t)NI + 1)), o_rank = take(4 * (size_t)NI), o_img_d = take(4 * (size_t)NI),
-               o_img_ptr = take(4 * ((size_t)NI + 1)), o_ctr = take(16), o_body = take(8 * (size_t)NI),
-               o_isize = take(8 * ((size_t)NI + 1)), o_ioff = take(8 * ((size_t)NI + 1)),
-               o_name_off = take(8 * ((size_t)NI + 1)), o_fact = take(4 * (size_t)NI), o_names = take(name_bytes),
-               o_group = take(4 * (size_t)NI), o_gcount = take(4 * ((size_t)G + 1)), o_grank = take(4 * ((size_t)G + 1)),
-               o_goff = take(8 * ((size_t)G + 1)), o_gout = take(8 * (size_t)G), o_nkey = take(4 * (size_t)N),
-               o_nkey_s = take(4 * (size_t)N), o_iota = take(4 * (size_t)N), o_perm = take(4 * (size_t)N),
-               o_rsize = take(8 * ((size_t)N + 1)), o_noff = take(8 * ((size_t)N + 1));
-  LFR_TRY(pl->enc_scratch.reserve(at));
-  uint8_t* base = pl->enc_scratch.as<uint8_t>();
-  auto u32 = [base](size_t o) { return reinterpret_cast<uint32_t*>(base + o); };
-  auto u64 = [base](size_t o) { return reinterpret_cast<uint64_t*>(base + o); };
-  auto ull = [base](size_t o) { return reinterpret_cast<unsigned long long*>(base + o); };
-  uint32_t *first = u32(o_first), *iota_i = u32(o_iota_i), *img_s = u32(o_img_s), *present = u32(o_present),
-           *dense = u32(o_dense), *rank = u32(o_rank), *img_d = u32(o_img_d), *img_ptr = u32(o_img_ptr),
-           *n_present = u32(o_ctr), *d_group = u32(o_group), *gcount = u32(o_gcount), *grank = u32(o_grank),
-           *key = u32(o_nkey), *key_s = u32(o_nkey_s), *iota = u32(o_iota), *perm = u32(o_perm);
-  uint64_t *body = u64(o_body), *isize = u64(o_isize), *ioff = u64(o_ioff), *d_name_off = u64(o_name_off),
-           *goff = u64(o_goff), *rsize = u64(o_rsize), *noff = u64(o_noff);
-  unsigned long long *ikey = ull(o_key), *ikey_s = ull(o_key_s), *gout = ull(o_gout);
-  float* d_fact = reinterpret_cast<float*>(base + o_fact);
-  uint8_t* d_names = base + o_names;
-  const uint32_t* nimg = pl->node_image.as<uint32_t>();
-  const uint32_t* nfeat = pl->node_feat.as<uint32_t>();
-  const double* pos = pl->pos.as<double>();
-
-  LFR_CUDA(cudaMemcpyAsync(d_name_off, name_off, 8 * ((size_t)NI + 1), cudaMemcpyHostToDevice, s));
-  LFR_CUDA(cudaMemcpyAsync(d_fact, fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
-  if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, names, name_bytes, cudaMemcpyHostToDevice, s));
-  LFR_CUDA(cudaMemcpyAsync(d_group, group_of_image, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
-  LFR_CUDA(cudaMemsetAsync(gcount, 0, 4 * ((size_t)G + 1), s));
-  if (G) LFR_CUDA(cudaMemsetAsync(gout, 0, 8 * (size_t)G, s));
-  init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
-  group_first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, d_group, first, gout);
-  group_key_kernel<<<blocks_for(NI), 256, 0, s>>>(first, d_group, NI, ikey);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // by group, then by first node
-    return cub::DeviceRadixSort::SortPairs(t, nb, ikey, ikey_s, iota_i, img_s, (int)NI, 0, 32 + bits_for(G), s);
-  }));
-  group_present_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(ikey_s, NI, N, present, gcount);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, present, dense, (int)NI + 1, s); }));
-  group_rank_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(img_s, present, dense, NI, rank, img_d, n_present);
-  node_key_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, rank, N, key, iota, nullptr, NI, nullptr);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: ascending node index within an image
-    return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, iota, perm, (int)N, 0, bits_for(NI), s);
-  }));
-  record_size_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, N, rsize, img_ptr);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, noff, (int)N + 1, s); }));
-  image_size_kernel<<<blocks_for((uint64_t)NI + 1), 256, 0, s>>>(img_d, img_ptr, noff, d_name_off, d_fact, n_present, NI, body, isize);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)NI + 1, s); }));
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, gcount, grank, (int)G + 1, s); }));
-  group_off_kernel<<<blocks_for((uint64_t)G + 1), 256, 0, s>>>(grank, ioff, G, goff);
-  LFR_LAUNCHED();
-  if (G) LFR_CUDA(cudaMemcpyAsync(n_outside, gout, 8 * (size_t)G, cudaMemcpyDeviceToHost, s));
-  LFR_TRY(fetch(group_off, goff, (size_t)G + 1, s));
-  const uint64_t total = group_off[G];
-  if (!out || cap < total) return (int64_t)total;
-  LFR_TRY(pl->enc_out.reserve(total));
-  uint8_t* d_out = pl->enc_out.as<uint8_t>();
-  write_images_kernel<<<blocks_for(NI), 256, 0, s>>>(img_d, body, ioff, d_names, d_name_off, d_fact, n_present, d_out);
-  write_records_kernel<<<blocks_for(N), 256, 0, s>>>(perm, key_s, nfeat, pos, img_ptr, noff, ioff, N, d_out);
-  LFR_LAUNCHED();
-  LFR_TRY(fetch(out, d_out, total, s));
-  return (int64_t)total;
+// encode_solution() for the calls with one output: its "> 0.5" count summed over the slots
+int64_t encode_one(lfr_plan* pl, void* stream, const EncodeInput& in, uint8_t* out, uint64_t cap, uint64_t* n_outside,
+                   uint64_t* n_carried = nullptr) {
+  uint64_t group_off[2], outside[2], carried;
+  const int64_t total = encode_solution(pl, (cudaStream_t)stream, in, out, cap, group_off, outside, &carried);
+  if (n_outside) *n_outside = outside[0] + outside[1];
+  if (n_carried) *n_carried = carried;
+  return total;
 }
 
 int select_device(const lfr_options& o) {
@@ -2325,12 +2390,8 @@ int build_constant_mask(lfr_plan* pl, cudaStream_t s) {
 // decoded and its images resolved on the host (lfr_join.h), before either call changes the plan.
 int decode_solution_for(const lfr_plan* pl, const uint8_t* bytes, uint64_t len, uint32_t n_images, const uint8_t* names,
                         const uint64_t* name_off, lfr::join::Decoded& d) {
-  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
-  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
-  if ((len && !bytes) || (n_images && !name_off)) return fail(LFR_EINVAL, "NULL SolutionFile bytes or image names");
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
-  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  LFR_TRY(check_names(pl, n_images, names, name_off,
+                      (len && !bytes) || (n_images && !name_off) ? "NULL SolutionFile bytes or image names" : nullptr));
   const uint8_t no_name = 0;
   if (lfr::join::decode(bytes, len, n_images, names ? names : &no_name, name_off, d) != LFR_OK)
     return fail(LFR_EINVAL, "malformed SolutionFile");
@@ -2344,27 +2405,22 @@ int join_solution(lfr_plan* pl, cudaStream_t s, const lfr::join::Decoded& d, uin
   const uint32_t N = pl->N, D = (uint32_t)d.n_disp, I = (uint32_t)d.n_images;
   if (n_started) *n_started = 0;
   if (!N) return LFR_OK;
-  size_t at = 0;
-  auto take = [&at](size_t bytes) {
-    const size_t o = at;
-    at += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_ctr = take(8), o_ptr = take(8 * ((size_t)I + 1)), o_id = take(4 * (size_t)I + 4), o_feat = take(4 * (size_t)D),
-               o_di = take(4 * (size_t)D), o_dj = take(4 * (size_t)D), o_key = take(8 * (size_t)D), o_key_s = take(8 * (size_t)D),
-               o_idx = take(4 * (size_t)D), o_idx_s = take(4 * (size_t)D);
-  LFR_TRY(pl->enc_scratch.reserve(at));
-  uint8_t* base = pl->enc_scratch.as<uint8_t>();
-  auto* ctr = reinterpret_cast<unsigned long long*>(base + o_ctr);
-  auto* img_ptr = reinterpret_cast<uint64_t*>(base + o_ptr);
-  auto* image_id = reinterpret_cast<uint32_t*>(base + o_id);
-  auto* feat = reinterpret_cast<uint32_t*>(base + o_feat);
-  auto* di = reinterpret_cast<float*>(base + o_di);
-  auto* dj = reinterpret_cast<float*>(base + o_dj);
-  auto* key = reinterpret_cast<unsigned long long*>(base + o_key);
-  auto* key_s = reinterpret_cast<unsigned long long*>(base + o_key_s);
-  auto* idx = reinterpret_cast<uint32_t*>(base + o_idx);
-  auto* idx_s = reinterpret_cast<uint32_t*>(base + o_idx_s);
+  unsigned long long *ctr, *key, *key_s;
+  uint64_t* img_ptr;
+  uint32_t *image_id, *feat, *idx, *idx_s;
+  float *di, *dj;
+  LFR_TRY(carve(pl->enc_scratch, [&](Carve& c) {
+    ctr = c.take<unsigned long long>(1);
+    img_ptr = c.take<uint64_t>((size_t)I + 1);
+    image_id = c.take<uint32_t>((size_t)I + 1);
+    feat = c.take<uint32_t>(D);
+    di = c.take<float>(D);
+    dj = c.take<float>(D);
+    key = c.take<unsigned long long>(D);
+    key_s = c.take<unsigned long long>(D);
+    idx = c.take<uint32_t>(D);
+    idx_s = c.take<uint32_t>(D);
+  }));
   LFR_CUDA(cudaMemsetAsync(ctr, 0, 8, s));
   if (D) {
     LFR_CUDA(cudaMemcpyAsync(img_ptr, d.img_ptr.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
@@ -2397,162 +2453,6 @@ int join_solution(lfr_plan* pl, cudaStream_t s, const lfr::join::Decoded& d, uin
   LFR_TRY(fetch(&started, ctr, 1, s));  // also keeps `d` alive until its copies are done
   if (n_started) *n_started = started;
   return LFR_OK;
-}
-
-// lfr_plan_encode_solution_carried() on a checked plan and arguments and the decoded file (lfr_carry.cuh):
-// the scene images' ranks and the entries' join on the device, one synchronisation for the carried count,
-// the record and image sizes, one for the total, then — when `out` has room — the writing kernels and one
-// copy to `out`
-int64_t encode_solution_carried(lfr_plan* pl, cudaStream_t s, uint32_t NI, const uint8_t* names, const uint64_t* name_off,
-                                const float* fact, const uint8_t* file, const lfr::join::Decoded& d, uint8_t* out,
-                                uint64_t cap, uint64_t* n_outside, uint64_t* n_carried) {
-  using namespace lfr::carry;
-  const uint32_t N = pl->N, D = (uint32_t)d.n_disp, I = (uint32_t)d.n_images;
-  if (n_outside) *n_outside = 0;
-  if (n_carried) *n_carried = 0;
-  // per message: its key image (the scene id of a matched winner, n_images + j for the j-th other winner,
-  // kNoImage for a message that loses to a later one of its name), and the winners' names and facts
-  std::vector<uint32_t> msg_pid(I, kNoImage);
-  std::vector<uint64_t> msg_name_off((size_t)I + 1, 0);
-  std::vector<uint8_t> msg_names;
-  uint64_t n_other = 0;
-  for (uint32_t i = 0; i < I; ++i) {
-    if (d.wins[i]) {
-      msg_pid[i] = d.image_id[i] != lfr::join::kNoImage ? d.image_id[i] : (uint32_t)(NI + n_other++);
-      msg_names.insert(msg_names.end(), file + d.name_off[i], file + d.name_off[i] + d.name_len[i]);
-    }
-    msg_name_off[(size_t)i + 1] = msg_names.size();
-  }
-  if ((uint64_t)NI + n_other >= kNoImage) return fail(LFR_EUNSUPPORTED, "too many images in the scene and the SolutionFile");
-  const uint64_t name_bytes = name_off[NI], msg_name_bytes = msg_names.size();
-  const uint32_t n_max = NI + I;  // an upper bound of the output images
-  size_t at = 0;
-  auto take = [&at](size_t bytes) {
-    const size_t o = at;
-    at += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  // per scene image, per message, per entry, then per record (N + at most D) and per output image
-  const size_t o_ctr = take(16), o_first = take(4 * (size_t)NI), o_first_s = take(4 * (size_t)NI),
-               o_iota_i = take(4 * (size_t)NI), o_img_s = take(4 * (size_t)NI), o_rank = take(4 * (size_t)NI),
-               o_name_off = take(8 * ((size_t)NI + 1)), o_fact = take(4 * (size_t)NI), o_names = take(name_bytes),
-               o_mptr = take(8 * ((size_t)I + 1)), o_mpid = take(4 * (size_t)I + 4), o_mnoff = take(8 * ((size_t)I + 1)),
-               o_mfact = take(4 * (size_t)I + 4), o_mnames = take(msg_name_bytes), o_g2 = take(4 * ((size_t)I + 1)),
-               o_g2_off = take(4 * ((size_t)I + 1)), o_g2_msg = take(4 * (size_t)I + 4), o_feat = take(4 * (size_t)D),
-               o_di = take(4 * (size_t)D), o_dj = take(4 * (size_t)D), o_key = take(8 * (size_t)D),
-               o_key_s = take(8 * (size_t)D), o_idx = take(4 * (size_t)D), o_idx_s = take(4 * (size_t)D),
-               o_used = take(D), o_flag = take(4 * ((size_t)D + 1)), o_slot = take(4 * ((size_t)D + 1)),
-               o_ce = take(4 * (size_t)D), o_cm = take(4 * (size_t)D), o_rkey = take(4 * ((size_t)N + D)),
-               o_rkey_s = take(4 * ((size_t)N + D)), o_riota = take(4 * ((size_t)N + D)), o_perm = take(4 * ((size_t)N + D)),
-               o_rsize = take(8 * ((size_t)N + D + 1)), o_roff = take(8 * ((size_t)N + D + 1)),
-               o_iend = take(4 * ((size_t)n_max + 1)), o_body = take(8 * ((size_t)n_max + 1)),
-               o_isize = take(8 * ((size_t)n_max + 1)), o_ioff = take(8 * ((size_t)n_max + 1));
-  LFR_TRY(pl->enc_scratch.reserve(at));
-  uint8_t* base = pl->enc_scratch.as<uint8_t>();
-  auto u32 = [base](size_t o) { return reinterpret_cast<uint32_t*>(base + o); };
-  auto u64 = [base](size_t o) { return reinterpret_cast<uint64_t*>(base + o); };
-  auto f32 = [base](size_t o) { return reinterpret_cast<float*>(base + o); };
-  auto* d_outside = reinterpret_cast<unsigned long long*>(base + o_ctr);
-  uint32_t* n_present = u32(o_ctr + 8);
-  uint32_t *first = u32(o_first), *first_s = u32(o_first_s), *iota_i = u32(o_iota_i), *img_s = u32(o_img_s),
-           *rank = u32(o_rank), *mpid = u32(o_mpid), *g2 = u32(o_g2), *g2_off = u32(o_g2_off), *g2_msg = u32(o_g2_msg),
-           *feat = u32(o_feat), *idx = u32(o_idx), *idx_s = u32(o_idx_s), *flag = u32(o_flag), *slot = u32(o_slot),
-           *ce = u32(o_ce), *cm = u32(o_cm), *rkey = u32(o_rkey), *rkey_s = u32(o_rkey_s), *riota = u32(o_riota),
-           *perm = u32(o_perm), *iend = u32(o_iend);
-  uint64_t *d_name_off = u64(o_name_off), *mptr = u64(o_mptr), *mnoff = u64(o_mnoff), *rsize = u64(o_rsize),
-           *roff = u64(o_roff), *body = u64(o_body), *isize = u64(o_isize), *ioff = u64(o_ioff);
-  auto* key = reinterpret_cast<unsigned long long*>(base + o_key);
-  auto* key_s = reinterpret_cast<unsigned long long*>(base + o_key_s);
-  float *d_fact = f32(o_fact), *mfact = f32(o_mfact), *di = f32(o_di), *dj = f32(o_dj);
-  uint8_t *d_names = base + o_names, *mnames = base + o_mnames, *used = base + o_used;
-  const uint32_t* nimg = pl->node_image.as<uint32_t>();
-  const uint32_t* nfeat = pl->node_feat.as<uint32_t>();
-  const double* pos = pl->pos.as<double>();
-
-  LFR_CUDA(cudaMemsetAsync(base + o_ctr, 0, 16, s));
-  LFR_CUDA(cudaMemcpyAsync(d_name_off, name_off, 8 * ((size_t)NI + 1), cudaMemcpyHostToDevice, s));
-  if (NI) LFR_CUDA(cudaMemcpyAsync(d_fact, fact, 4 * (size_t)NI, cudaMemcpyHostToDevice, s));
-  if (name_bytes) LFR_CUDA(cudaMemcpyAsync(d_names, names, name_bytes, cudaMemcpyHostToDevice, s));
-  LFR_CUDA(cudaMemcpyAsync(mptr, d.img_ptr.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
-  LFR_CUDA(cudaMemcpyAsync(mnoff, msg_name_off.data(), 8 * ((size_t)I + 1), cudaMemcpyHostToDevice, s));
-  if (I) {
-    LFR_CUDA(cudaMemcpyAsync(mpid, msg_pid.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemcpyAsync(mfact, d.fact.data(), 4 * (size_t)I, cudaMemcpyHostToDevice, s));
-  }
-  if (msg_name_bytes) LFR_CUDA(cudaMemcpyAsync(mnames, msg_names.data(), msg_name_bytes, cudaMemcpyHostToDevice, s));
-  // the present scene images and their ranks, as lfr_plan_encode_solution() ranks them
-  if (NI) {
-    lfr::solution::init_images_kernel<<<blocks_for(NI), 256, 0, s>>>(first, iota_i, NI, N);
-    if (N) lfr::solution::first_node_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, pos, N, first, d_outside, nullptr);
-    LFR_LAUNCHED();
-    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {
-      return cub::DeviceRadixSort::SortPairs(t, nb, first, first_s, iota_i, img_s, (int)NI, 0, bits_for(N), s);
-    }));
-    lfr::solution::rank_kernel<<<blocks_for(NI), 256, 0, s>>>(first_s, img_s, NI, N, rank, n_present);
-    LFR_LAUNCHED();
-  }
-  // the entries: keyed, sorted stably, joined to the nodes, the carried ones compacted
-  uint32_t C = 0;
-  if (D) {
-    LFR_CUDA(cudaMemcpyAsync(feat, d.feature_idx.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemcpyAsync(di, d.di.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemcpyAsync(dj, d.dj.data(), 4 * (size_t)D, cudaMemcpyHostToDevice, s));
-    LFR_CUDA(cudaMemsetAsync(used, 0, D, s));
-    lfr::start::solution_key_kernel<<<blocks_for(D), 256, 0, s>>>(mptr, mpid, I, feat, D, key, idx);
-    LFR_LAUNCHED();
-    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: equal keys stay in file order
-      return cub::DeviceRadixSort::SortPairs(t, nb, key, key_s, idx, idx_s, (int)D, 0, 64, s);
-    }));
-    if (N) consume_kernel<<<blocks_for(N), 256, 0, s>>>(nimg, nfeat, N, key_s, D, used);
-    carry_flag_kernel<<<blocks_for((uint64_t)D + 1), 256, 0, s>>>(key_s, used, D, flag);
-    LFR_LAUNCHED();
-    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, flag, slot, (int)D + 1, s); }));
-    carry_compact_kernel<<<blocks_for(D), 256, 0, s>>>(flag, slot, idx_s, mptr, I, D, ce, cm);
-    LFR_LAUNCHED();
-    LFR_TRY(fetch(&C, slot + D, 1, s));
-  }
-  // the other winning messages, ranked after the present scene images in file order
-  group2_flag_kernel<<<blocks_for((uint64_t)I + 1), 256, 0, s>>>(mpid, I, first, NI, N, g2);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, g2, g2_off, (int)I + 1, s); }));
-  if (I) {
-    group2_scatter_kernel<<<blocks_for(I), 256, 0, s>>>(g2, g2_off, I, g2_msg);
-    LFR_LAUNCHED();
-  }
-  // the records (nodes, then carried entries) in output order, their sizes and the images'
-  const uint32_t R = N + C;
-  if (R) {
-    record_key_kernel<<<blocks_for(R), 256, 0, s>>>(nimg, rank, N, cm, mpid, g2, g2_off, n_present, R, rkey, riota);
-    LFR_LAUNCHED();
-    LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) {  // stable: nodes by index, then carried entries by feature
-      return cub::DeviceRadixSort::SortPairs(t, nb, rkey, rkey_s, riota, perm, (int)R, 0, bits_for(n_max), s);
-    }));
-  }
-  record_size_kernel<<<blocks_for((uint64_t)R + 1), 256, 0, s>>>(perm, R, N, nfeat, pos, ce, feat, di, dj, rsize);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, rsize, roff, (int)R + 1, s); }));
-  image_size_kernel<<<blocks_for((uint64_t)n_max + 1), 256, 0, s>>>(rkey_s, R, roff, n_present, g2_off, I, img_s, d_names,
-                                                                     d_name_off, d_fact, g2_msg, mnames, mnoff, mfact, n_max,
-                                                                     iend, body, isize);
-  LFR_LAUNCHED();
-  LFR_TRY(cub_run(pl->enc_cub, [&](void* t, size_t& nb) { return cub::DeviceScan::ExclusiveSum(t, nb, isize, ioff, (int)n_max + 1, s); }));
-  uint64_t total = 0;
-  unsigned long long outside = 0;
-  LFR_CUDA(cudaMemcpyAsync(&outside, d_outside, 8, cudaMemcpyDeviceToHost, s));
-  LFR_TRY(fetch(&total, ioff + n_max, 1, s));
-  if (n_outside) *n_outside = outside;
-  if (n_carried) *n_carried = C;
-  if (!out || cap < total || !total) return (int64_t)total;
-  LFR_TRY(pl->enc_out.reserve(total));
-  uint8_t* d_out = pl->enc_out.as<uint8_t>();
-  if (n_max)
-    write_images_kernel<<<blocks_for(n_max), 256, 0, s>>>(n_present, g2_off, I, img_s, d_names, d_name_off, d_fact, g2_msg,
-                                                           mnames, mnoff, mfact, body, ioff, n_max, d_out);
-  if (R)
-    write_records_kernel<<<blocks_for(R), 256, 0, s>>>(perm, rkey_s, R, N, nfeat, pos, ce, feat, di, dj, iend, roff, ioff, d_out);
-  LFR_LAUNCHED();
-  LFR_TRY(fetch(out, d_out, total, s));
-  return (int64_t)total;
 }
 
 // lfr_plan_update_solution() after the decode, with the touched flags seeded from changed[C] on the device
@@ -2662,17 +2562,6 @@ int diff_components(const lfr_plan* pl, const lfr_plan* prev, const std::vector<
   unsigned long long nc = 0;
   LFR_TRY(fetch(&nc, d_ctr.p, 1, s));  // before the scratch is freed
   *n_changed = (uint32_t)nc;
-  return LFR_OK;
-}
-
-// the checks of the record calls on the image names (as lfr_plan_encode_solution's)
-int check_record_names(const lfr_plan* pl, uint32_t n_images, const uint8_t* names, const uint64_t* name_off) {
-  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
-  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
-  if (n_images && !name_off) return fail(LFR_EINVAL, "NULL image names");
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
-  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
   return LFR_OK;
 }
 
@@ -2896,46 +2785,38 @@ int lfr_plan_export_graph(const lfr_plan* pl, uint32_t* row_ptr, lfr_edge* edges
 int64_t lfr_plan_encode_solution(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
                                  const uint64_t* name_off, const float* fact, uint8_t* out, uint64_t cap,
                                  uint64_t* n_outside) {
-  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
-  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
-  if (n_images && (!name_off || !fact)) return fail(LFR_EINVAL, "NULL image names or facts");
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
-  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  LFR_TRY(check_names(pl, n_images, names, name_off, n_images && (!name_off || !fact) ? "NULL image names or facts" : nullptr));
   LFR_CUDA(cudaSetDevice(pl->device));
-  return encode_solution(pl, (cudaStream_t)stream, n_images, names, name_off, fact, out, cap, n_outside);
+  return encode_one(pl, stream, EncodeInput{n_images, names, name_off, fact}, out, cap, n_outside);
 }
 
 int64_t lfr_plan_encode_solution_images(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
                                         const uint64_t* name_off, const float* fact, const uint8_t* written, uint8_t* out,
                                         uint64_t cap, uint64_t* n_outside) {
   if (!written) return fail(LFR_EINVAL, "written is NULL");
-  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
-  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
-  if (n_images && (!name_off || !fact)) return fail(LFR_EINVAL, "NULL image names or facts");
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
-  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  LFR_TRY(check_names(pl, n_images, names, name_off, n_images && (!name_off || !fact) ? "NULL image names or facts" : nullptr));
   LFR_CUDA(cudaSetDevice(pl->device));
-  return encode_solution(pl, (cudaStream_t)stream, n_images, names, name_off, fact, out, cap, n_outside, written);
+  std::vector<uint32_t> group(n_images);  // one group; an image without the flag is in none
+  for (uint32_t k = 0; k < n_images; ++k) group[k] = written[k] ? 0 : 1;
+  return encode_one(pl, stream, EncodeInput{n_images, names, name_off, fact, group.data(), 1}, out, cap, n_outside);
 }
 
 int64_t lfr_plan_encode_solution_groups(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
                                         const uint64_t* name_off, const float* fact, const uint32_t* group_of_image,
                                         uint32_t n_groups, uint8_t* out, uint64_t cap, uint64_t* group_off,
                                         uint64_t* n_outside) {
-  if (!pl || !pl->graph) return fail(LFR_EINVAL, "plan was not made by lfr_plan_create_from_matches");
-  if (n_images < pl->n_images) return fail(LFR_EINVAL, "n_images is smaller than the plan's image count");
-  if (n_images && (!name_off || !fact || !group_of_image)) return fail(LFR_EINVAL, "NULL image names, facts or groups");
-  if (!group_off || (n_groups && !n_outside)) return fail(LFR_EINVAL, "NULL group_off or n_outside");
-  for (uint32_t k = 0; k < n_images; ++k) {
-    if (name_off[k + 1] < name_off[k]) return fail(LFR_EINVAL, "name_off is not ascending");
-    if (group_of_image[k] >= n_groups) return fail(LFR_EINVAL, "an image's group is not below n_groups");
-  }
-  if (n_images && name_off[n_images] && !names) return fail(LFR_EINVAL, "names is NULL");
+  const char* missing = n_images && (!name_off || !fact || !group_of_image) ? "NULL image names, facts or groups"
+                        : !group_off || (n_groups && !n_outside)           ? "NULL group_off or n_outside"
+                                                                           : nullptr;
+  LFR_TRY(check_names(pl, n_images, names, name_off, missing, group_of_image, n_groups));
   LFR_CUDA(cudaSetDevice(pl->device));
-  return encode_solution_groups(pl, (cudaStream_t)stream, n_images, names, name_off, fact, group_of_image, n_groups, out,
-                                cap, group_off, n_outside);
+  std::vector<uint64_t> outside((size_t)n_groups + 1);
+  uint64_t carried;
+  const int64_t total = encode_solution(pl, (cudaStream_t)stream,
+                                        EncodeInput{n_images, names, name_off, fact, group_of_image, n_groups}, out, cap,
+                                        group_off, outside.data(), &carried);
+  std::copy(outside.begin(), outside.end() - 1, n_outside);
+  return total;
 }
 
 int lfr_plan_fix_images(lfr_plan* pl, const uint8_t* fixed_by_image_id, uint32_t n_images) {
@@ -3003,7 +2884,7 @@ int lfr_plan_update_solution_since(lfr_plan* pl, void* stream, const uint8_t* by
 
 int64_t lfr_plan_problem_record(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
                                 const uint64_t* name_off, uint8_t* out, uint64_t cap) {
-  LFR_TRY(check_record_names(pl, n_images, names, name_off));
+  LFR_TRY(check_names(pl, n_images, names, name_off, n_images && !name_off ? "NULL image names" : nullptr));
   const uint32_t C = pl->C;
   const uint64_t need = lfr::record::record_bytes(C);
   if (!out || cap < need) return (int64_t)need;
@@ -3039,7 +2920,7 @@ int lfr_plan_update_solution_since_record(lfr_plan* pl, void* stream, const uint
                                           uint64_t record_len, uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed) {
   lfr::join::Decoded d;
   LFR_TRY(decode_solution_for(pl, bytes, len, n_images, names, name_off, d));
-  LFR_TRY(check_record_names(pl, n_images, names, name_off));
+  LFR_TRY(check_names(pl, n_images, names, name_off, n_images && !name_off ? "NULL image names" : nullptr));
   uint64_t R = 0;
   if (!lfr::record::check(record, record_len, &R)) return fail(LFR_EINVAL, "malformed problem record");
   LFR_CUDA(cudaSetDevice(pl->device));
@@ -3083,8 +2964,8 @@ int64_t lfr_plan_encode_solution_carried(lfr_plan* pl, void* stream, uint32_t n_
   }
   if ((uint64_t)pl->N + d.n_disp >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "2^31 or more nodes and displacements");
   LFR_CUDA(cudaSetDevice(pl->device));
-  return encode_solution_carried(pl, (cudaStream_t)stream, n_images, names, name_off, fact, file, d, out, cap, n_outside,
-                                 n_carried);
+  return encode_one(pl, stream, EncodeInput{n_images, names, name_off, fact, nullptr, 1, file, &d}, out, cap, n_outside,
+                    n_carried);
 }
 
 int lfr_debug_last_encode_times(double* out2) {

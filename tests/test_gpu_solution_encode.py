@@ -60,11 +60,32 @@ def host_encoding(plan, names, fact):
 
 
 def assert_same_encoding(plan, names, fact):
+    """The plain encoder against the host path; the masked, grouped and carried encoders, on the inputs that make
+    them the plain one (every image written, one group of every image, an empty file), against the plain one."""
     got = plan.encode_solution(names, fact)
     want = host_encoding(plan, names, fact)
     assert got[1] == want[1]
     assert got[0] == want[0]
-    return got[0]
+    data, n_outside = got
+    blob, off = wire._names_blob(list(names))
+    fact32 = np.ascontiguousarray(fact, np.float32)
+    args = (plan.handle, None, len(names), blob.ctypes.data, off.ctypes.data, fact32.ctypes.data)
+    buf = np.empty(max(len(data), 1), np.uint8)
+    f = plan.lib.lib.lfr_plan_encode_solution_images
+    f.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                  C.c_uint64, C.POINTER(C.c_uint64)]
+    f.restype = C.c_int64
+    n = C.c_uint64(7)
+    written = np.ones(max(len(names), 1), np.uint8)
+    assert f(*args, written.ctypes.data, buf.ctypes.data, buf.size, C.byref(n)) == len(data)
+    assert buf[:len(data)].tobytes() == data and n.value == n_outside
+    group = np.zeros(max(len(names), 1), np.uint32)
+    goff, outside = np.full(2, 7, np.uint64), np.full(1, 7, np.uint64)
+    assert plan.lib.lib.lfr_plan_encode_solution_groups(*args, group.ctypes.data, 1, buf.ctypes.data, buf.size,
+                                                        goff.ctypes.data, outside.ctypes.data) == len(data)
+    assert buf[:len(data)].tobytes() == data and goff.tolist() == [0, len(data)] and outside.tolist() == [n_outside]
+    assert plan.encode_solution_carried(names, fact, b"") == (data, n_outside, 0)
+    return data
 
 
 def plans(b200, parts, banned=(), positions=None):
