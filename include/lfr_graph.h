@@ -292,6 +292,41 @@ int lfr_plan_update_solution_since_record(lfr_plan* plan, void* stream, const ui
                                           const uint8_t* record, uint64_t record_len, uint64_t* n_held,
                                           uint32_t* n_touched, uint32_t* n_changed);
 
+/* Many scenes of one plan, each updated as its own run: image id k belongs to scene group_of_image[k] < n_groups
+ * (as for lfr_plan_encode_solution_groups; every component lies in one scene).  Scene g's SolutionFile is files[g]
+ * (file_len[g] bytes), decoded on the host against scene g's image ids alone, since scenes reuse image names; a
+ * NULL file has no entry, so every component of the scene is touched and solves bit for bit as from zeros.  With
+ * records[g] (record_len[g] bytes) scene g follows lfr_plan_update_solution_since_record() against that record,
+ * looked up within the scene alone (one kernel binary-searches scene g's slice of all the records); a NULL record
+ * gives scene g the rule of lfr_plan_update_solution().  `files` or `records` may be NULL for none at all.
+ * Every scene's entries are keyed by scene image id and joined in one pass, and the touch, update and schedule
+ * steps are those of lfr_plan_update_solution(): the kernel launches, CUB calls and copies do not grow with
+ * n_groups.  *n_held and *n_touched are sums over the scenes; *n_changed counts the changed components of the
+ * scenes with a record.  With n_groups == 1 the call is lfr_plan_update_solution() (NULL record) or
+ * lfr_plan_update_solution_since_record(), bit for bit.  Errors as those calls, plus LFR_EINVAL for a group out of
+ * range; the plan is not changed on error.  lfr_wire_update_solution_groups() (include/lfr_host.h) is the host
+ * form, bit for bit. */
+int lfr_plan_update_solution_groups(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                    const uint64_t* name_off, const uint32_t* group_of_image, uint32_t n_groups,
+                                    const uint8_t* const* files, const uint64_t* file_len, const uint8_t* const* records,
+                                    const uint64_t* record_len, uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed);
+
+/* The problem record of every scene of a plan (scenes as for lfr_plan_update_solution_groups): scene g's is
+ * out[group_off[g], group_off[g + 1]), byte for byte lfr_plan_problem_record() of a plan of scene g alone.  The
+ * digests are computed once on the device, ordered by (scene, d0, d1) with three stable radix sorts, and every
+ * header and digest is written in one device pass and copied out once; nothing grows with n_groups but the offsets.
+ * group_off[0..n_groups] is always filled; the records are written when `cap` holds them all
+ * (lfr_plan_encode_solution_groups' protocol).  Returns the total size, or the errors of lfr_plan_problem_record()
+ * and LFR_EINVAL for a group out of range or a NULL group_off.  The plan is not changed.
+ * lfr_host_problem_record_groups() (include/lfr_host.h) is the host form, byte for byte. */
+int64_t lfr_plan_problem_record_groups(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                       const uint64_t* name_off, const uint32_t* group_of_image, uint32_t n_groups,
+                                       uint8_t* out, uint64_t cap, uint64_t* group_off);
+
+/* A test hook: the calling thread's device operations since the last reset, {kernel launch sites checked, CUB
+ * calls, synchronising copies to the host}, into out3 (may be NULL); reset != 0 zeroes them. */
+int lfr_debug_device_ops(unsigned long long* out3, int reset);
+
 /* Whether a solve of `in` on `n_devices` devices should run its graph stage on the device
  * (lfr_plan_create_from_matches) rather than on the host (lfr_host_stage_create): 1 or 0.  Decided from
  * sizes known before either stage runs — the directed edges (2 x the matches of the pairs not skipped),

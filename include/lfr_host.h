@@ -115,6 +115,32 @@ int lfr_wire_update_solution_since_record(const uint8_t* buf, uint64_t len, uint
                                           double* positions /* [2 n_nodes] */, uint8_t* held /* [n_nodes] */,
                                           uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed);
 
+/* The host form of lfr_plan_update_solution_groups() (include/lfr_graph.h), bit for bit: many scenes of one run,
+ * image id k in scene group_of_image[k] < n_groups, each updated from its own SolutionFile (files[g], file_len[g]
+ * bytes, decoded against scene g's image ids alone; NULL: no entry, so every component of the scene is touched)
+ * and, where records[g] is not NULL, against its own earlier record (record_len[g] bytes; a component of scene g
+ * is changed when its digest is not in records[g]).  `files` or `records` may be NULL for none at all.
+ * *n_changed counts the changed components of the scenes with a record.  LFR_EINVAL for a SolutionFile that does
+ * not parse, a malformed record, a group out of range, a component whose nodes span two scenes, NULL or
+ * inconsistent arrays.  Every output is untouched on error. */
+int lfr_wire_update_solution_groups(uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                                    const uint32_t* group_of_image, uint32_t n_groups, const uint8_t* const* files,
+                                    const uint64_t* file_len, const uint8_t* const* records, const uint64_t* record_len,
+                                    const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat,
+                                    double* positions /* [2 n_nodes] */, uint8_t* held /* [n_nodes] */,
+                                    uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed);
+
+/* The host form of lfr_plan_problem_record_groups() (include/lfr_graph.h), the same bytes: the problem record of
+ * every scene g < n_groups of `p` (image id k in scene group_of_image[k]), each what lfr_host_problem_record()
+ * writes for the scene's own run, back to back; scene g's is out[group_off[g], group_off[g + 1]).
+ * group_off[0..n_groups] is always filled; the records are written when `cap` holds them all.  Returns the total
+ * size, or LFR_EINVAL as lfr_host_problem_record() and for a group out of range or a component whose nodes span
+ * two scenes. */
+int64_t lfr_host_problem_record_groups(const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat,
+                                       uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                                       const uint32_t* group_of_image, uint32_t n_groups, uint8_t* out, uint64_t cap,
+                                       uint64_t* group_off);
+
 #ifdef __cplusplus
 }
 #endif

@@ -84,7 +84,8 @@ GRAPH_SYMBOLS = ["lfr_plan_create_from_matches", "lfr_plan_create_from_wire", "l
                  "lfr_plan_fix_images", "lfr_plan_start_from_solution", "lfr_plan_keep_solution",
                  "lfr_plan_encode_solution_carried", "lfr_plan_update_solution", "lfr_plan_update_solution_since",
                  "lfr_plan_problem_record", "lfr_plan_update_solution_since_record", "lfr_plan_encode_solution_groups",
-                 "lfr_plan_create_from_wire_listed"]
+                 "lfr_plan_create_from_wire_listed", "lfr_plan_update_solution_groups", "lfr_plan_problem_record_groups",
+                 "lfr_debug_device_ops"]
 
 
 class LfrWirePart(C.Structure):
@@ -189,6 +190,15 @@ class Library:
                                                           C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64,
                                                           C.c_void_p, C.c_void_p]
             L.lfr_plan_encode_solution_groups.restype = C.c_int64
+            L.lfr_plan_update_solution_groups.argtypes = ([C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                           C.c_void_p, C.c_uint32] + [C.c_void_p] * 4 +
+                                                          [C.POINTER(C.c_uint64)] + [C.POINTER(C.c_uint32)] * 2)
+            L.lfr_plan_update_solution_groups.restype = C.c_int
+            L.lfr_plan_problem_record_groups.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                         C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
+            L.lfr_plan_problem_record_groups.restype = C.c_int64
+            L.lfr_debug_device_ops.argtypes = [C.c_void_p, C.c_int]
+            L.lfr_debug_device_ops.restype = C.c_int
         if L.lfr_abi_version() != 1:
             raise RuntimeError("lfr: ABI version mismatch in %s" % path)
 
@@ -711,6 +721,51 @@ class Plan:
                                                              C.byref(n), C.byref(t)),
                        "lfr_plan_update_solution")
         return int(n.value), int(t.value)
+
+    def update_solution_groups(self, solutions, image_names, image_group, records=None, stream: int = 0):
+        """lfr_plan_update_solution_groups (include/lfr_graph.h): every scene g of this plan (image id k in scene
+        image_group[k]) updated as its own run from solutions[g] (SolutionFile bytes, decoded against scene g's
+        image ids alone; None: no entry, so every component of the scene is touched) and, where records[g] is not
+        None, against that earlier problem record (looked up within the scene), else by update_solution()'s
+        plain rule.  One join and one lookup for all scenes.  Returns (held nodes, touched components, changed
+        components), sums over the scenes."""
+        from .wire import _names_blob, group_arrays
+        G = len(solutions)
+        records = [None] * G if records is None else list(records)
+        blob, off = _names_blob(list(image_names))
+        group = np.ascontiguousarray(image_group, dtype=np.uint32).reshape(-1)
+        if group.shape[0] != len(image_names) or len(records) != G:
+            raise ValueError("image_group needs one entry per image name and records one per scene")
+        fptr, flen, fkeep = group_arrays(solutions)
+        rptr, rlen, rkeep = group_arrays(records)
+        n, t, ch = C.c_uint64(), C.c_uint32(), C.c_uint32()
+        self.lib.check(self.lib.lib.lfr_plan_update_solution_groups(
+            self.handle, C.c_void_p(stream), len(image_names), blob.ctypes.data, off.ctypes.data,
+            group.ctypes.data if group.size else None, G, fptr, flen.ctypes.data, rptr, rlen.ctypes.data, C.byref(n),
+            C.byref(t), C.byref(ch)), "lfr_plan_update_solution_groups")
+        del fkeep, rkeep
+        return int(n.value), int(t.value), int(ch.value)
+
+    def problem_record_groups(self, image_names, image_group, n_groups: int, stream: int = 0):
+        """lfr_plan_problem_record_groups (include/lfr_graph.h): the problem record of every scene g < n_groups of this
+        plan (image id k in scene image_group[k]), each byte for byte problem_record() of a plan of the scene alone,
+        computed, ordered and written on the device in one pass.  Returns [bytes of every scene]."""
+        from .wire import _names_blob
+        blob, off = _names_blob(list(image_names))
+        group = np.ascontiguousarray(image_group, dtype=np.uint32).reshape(-1)
+        if group.shape[0] != len(image_names):
+            raise ValueError("image_group needs one entry per image name")
+        goff = np.zeros(n_groups + 1, np.uint64)
+        cap = 16 * (n_groups + self.n_components)
+        out = np.empty(max(cap, 1), np.uint8)
+        got = self.lib.lib.lfr_plan_problem_record_groups(self.handle, C.c_void_p(stream), len(image_names),
+                                                          blob.ctypes.data, off.ctypes.data,
+                                                          group.ctypes.data if group.size else None, n_groups,
+                                                          out.ctypes.data, cap, goff.ctypes.data)
+        if got != cap:
+            self.lib.check(int(got) if got < 0 else -1, "lfr_plan_problem_record_groups")
+        data = out[:cap].tobytes()
+        return [data[int(goff[g]):int(goff[g + 1])] for g in range(n_groups)]
 
     def solve(self, stream: int = 0) -> None:
         self.lib.check(self.lib.lib.lfr_plan_solve(self.handle, C.c_void_p(stream)), "lfr_plan_solve")

@@ -40,6 +40,11 @@ writes (solver.refine_scenes).
 --listed_pairs FILE (lines `MATCH_LIST<TAB>OUTPUT_FILE`) refines the pairs of many match lists (`NAME1 NAME2` per
 line, as compute_match_graph.py reads them) out of --matches_file in one run: each output file byte for byte
 what the run on a MatchingFile of that list's pairs in line order writes (solver.refine_lists).
+--versioned_scenes FILE (lines `MATCHES_FILE<TAB>OUTPUT_FILE<TAB>INITIAL_SOLUTION<TAB>EARLIER_RECORD<TAB>RECORD_FILE`,
+the last three fields may be empty) updates many scenes in one run: a scene with an initial solution is updated
+from it (and against its earlier record) as --update_initial_solution updates it alone, one without solves from
+zeros, and each output and record file is byte for byte what that scene's own run writes (solver.refine_scenes with
+initial_solutions, previous_records and record_problem).  Scene 0's start comes from the ordinary flags.
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -79,7 +84,7 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("update_initial_solution", False, False), ("previous_matches_file", True, False),
             ("record_file", True, False), ("earlier_record_file", True, False), ("query_images", True, True),
             ("joint_queries", False, False), ("additional_scenes", True, False),
-            ("listed_pairs", True, False)]
+            ("listed_pairs", True, False), ("versioned_scenes", True, False)]
 
 
 def _find_option(name):
@@ -160,7 +165,8 @@ def parse_args(argv):
             previous_matches_file=vals.get("previous_matches_file"),
             record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"),
             query_images=vals.get("query_images"), joint_queries=bool(vals.get("joint_queries")),
-            additional_scenes=vals.get("additional_scenes"), listed_pairs=vals.get("listed_pairs"))
+            additional_scenes=vals.get("additional_scenes"), listed_pairs=vals.get("listed_pairs"),
+            versioned_scenes=vals.get("versioned_scenes"))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -184,7 +190,11 @@ _RULES = [("--keep_initial_solution", "needs", ["--initial_solution"]),
                                           "--earlier_record_file", "--carry_initial_solution"]),
           ("--joint_queries", "needs", ["--query_images"]),
           ("--listed_pairs", "excludes", _ONE_SCENE + ["--additional_scenes"]),
-          ("--additional_scenes", "excludes", _ONE_SCENE)]
+          ("--additional_scenes", "excludes", _ONE_SCENE),
+          # every scene of --versioned_scenes starts from its own solution and record, scene 0 from the ordinary flags
+          ("--versioned_scenes", "excludes", ["--fixed_images", "--keep_initial_solution", "--carry_initial_solution",
+                                              "--previous_matches_file", "--query_images", "--joint_queries",
+                                              "--additional_scenes", "--listed_pairs"])]
 
 
 def _broken_rule(args):
@@ -198,6 +208,9 @@ def _broken_rule(args):
                 return "ERROR: %s needs %s%s\n" % (opt, other, " FILE" if other == "--initial_solution" else "")
             if kind == "excludes" and given(other):
                 return "ERROR: %s and %s exclude each other\n" % (opt, other)
+    # a batch's scenes are updated or solved from zeros: a start point alone belongs to one scene
+    if given("--versioned_scenes") and args.initial_solution and not args.update_initial_solution:
+        return "ERROR: --versioned_scenes: --initial_solution needs --update_initial_solution\n"
     return None
 
 
@@ -250,6 +263,69 @@ def read_scene_list(path, matches_file, output_file):
     return scenes if isinstance(scenes, bytes) else [(os.fsdecode(m), os.fsdecode(o)) for m, o in scenes]
 
 
+_VERSIONED_LINE = b"MATCHES_FILE<TAB>OUTPUT_FILE<TAB>INITIAL_SOLUTION<TAB>EARLIER_RECORD<TAB>RECORD_FILE"
+
+
+def read_versioned_list(path, row0):
+    """--versioned_scenes FILE: [row0] and a (matches, output, initial solution, earlier record, record file) row of
+    bytes (empty: none; a record file is None when the scene writes none, so scene 0's is None without
+    --record_file and its path, empty or not, with it) for every line, or the bytes of the one ERROR line for an unreadable file, a malformed line or
+    a file that two outputs or records would write (lfr_solve_main.cc writes the same lines)."""
+    try:
+        with open(path, "rb") as fh:
+            text = fh.read()
+    except OSError:
+        return b"ERROR: cannot read the scene list file '%s'\n" % os.fsencode(path)
+    rows = [row0]
+    for k, line in enumerate(_lines(text), 1):
+        f = line.split(b"\t")
+        why = (b"it is empty" if not line else b"it has fewer than four TABs" if len(f) < 5
+               else b"it has more than four TABs" if len(f) > 5
+               else b"its matches file is empty" if not f[0]
+               else b"its output file is empty" if not f[1]
+               else b"it holds a NUL byte" if b"\0" in line
+               else b"it has an earlier record but no initial solution" if f[3] and not f[2] else None)
+        if why:
+            return b"ERROR: --versioned_scenes: line %d is not %s: %s\n" % (k, _VERSIONED_LINE, why)
+        rows.append(tuple(f[:4]) + (f[4] or None,))
+    seen = set()
+    for row in rows:
+        for w in (row[1], row[4]):
+            if w and w in seen:
+                return b"ERROR: --versioned_scenes: two files written are '%s'\n" % w
+            seen.add(w)
+    return rows
+
+
+def read_versioned_starts(rows, start, earlier_record):
+    """Every scene's (initial solution bytes or None, earlier record bytes or None) of the read_versioned_list() rows,
+    scene 0's being `start` and `earlier_record`, or the bytes of the one ERROR line naming the list's line."""
+    from . import wire
+    out = [(start, earlier_record)]
+    for k, (_, _, init, earlier, _) in enumerate(rows[1:], 1):
+        sol = rec = None
+        if init:
+            try:
+                with open(init, "rb") as fh:
+                    sol = fh.read()
+            except OSError:
+                return b"ERROR: --versioned_scenes: line %d: cannot read the initial solution file '%s'\n" % (k, init)
+            try:
+                wire.decode_solution(sol)
+            except wire.ParseError:
+                return b"ERROR: --versioned_scenes: line %d: the initial solution file '%s' does not parse\n" % (k, init)
+        if earlier:
+            try:
+                with open(earlier, "rb") as fh:
+                    rec = fh.read()
+            except OSError:
+                return b"ERROR: --versioned_scenes: line %d: cannot read the earlier record file '%s'\n" % (k, earlier)
+            if not wire.record_is_valid(rec):
+                return b"ERROR: --versioned_scenes: line %d: '%s' is not a problem record\n" % (k, earlier)
+        out.append((sol, rec))
+    return out
+
+
 def read_pair_lists(path, output_file):
     """--listed_pairs FILE: [(match list path or None, output file, [(name1, name2)] or None)], list 0 being every
     pair of --matches_file written to `output_file`, or the bytes of the one ERROR line for what _read_tab_list
@@ -277,16 +353,22 @@ def read_pair_lists(path, output_file):
     return out
 
 
-def _run_batch(refine_batch, inputs, rows, args, opts, say, solve_fn, n_devices, timing, t_start) -> int:
-    """--additional_scenes or --listed_pairs after the rows (scenes or lists, each with its output file second) were
-    read: one refine_batch(*inputs, ...) run (refine_scenes or refine_lists), the stdout lines once, then the output
-    files in row order."""
+def _run_batch(refine_batch, inputs, rows, args, opts, say, solve_fn, n_devices, timing, t_start, starts=None) -> int:
+    """--additional_scenes, --listed_pairs or --versioned_scenes after the rows (scenes or lists, each with its output
+    file second; with --versioned_scenes its record file fifth) were read: one refine_batch(*inputs, ...) run
+    (refine_scenes or refine_lists; `starts`: every scene's (initial solution, earlier record)), the stdout lines
+    once, then the output files in row order and the record files in row order."""
     from .matchset import UnheldPairError
     from .solver import GraphStageRouteError
     sols = []
+    extra = {}
+    records = [None if r[4] is None else os.fsdecode(r[4]) for r in rows] if starts is not None else []
+    if starts is not None:
+        extra = dict(initial_solutions=[s for s, _ in starts], previous_records=[r for _, r in starts],
+                     record_problem=any(r is not None for r in records))
     try:
         data = refine_batch(*inputs, args.banned_images, opts, log=say, solve_fn=solve_fn, n_devices=n_devices,
-                            timing=timing, solutions=sols)
+                            timing=timing, solutions=sols, **extra)
     except UnheldPairError as e:   # --listed_pairs: a list line whose pair the file does not hold
         enc = lambda x: x.encode("utf-8", errors="surrogateescape")  # noqa: E731
         msg = b"ERROR: --listed_pairs: line %d of the match list '%s': the matches file holds no pair '%s' '%s'" % (
@@ -313,6 +395,15 @@ def _run_batch(refine_batch, inputs, rows, args, opts, say, solve_fn, n_devices,
     except OSError:
         sys.stderr.write("Failed to write proto object.\n")
         return 255
+    for path, sol in zip(records, sols):
+        if path is None:
+            continue
+        try:
+            with open(path, "wb") as fh:
+                fh.write(sol.record)
+        except OSError:
+            sys.stderr.write("ERROR: cannot write the record file '%s'\n" % path)
+            return 255
     return 0
 
 
@@ -344,6 +435,18 @@ def main(argv=None) -> int:
         if isinstance(scenes, bytes):
             sys.stderr.flush()
             sys.stderr.buffer.write(scenes)
+            sys.stderr.buffer.flush()
+            return 2
+    versioned = None
+    if args.versioned_scenes is not None:
+        enc = lambda x: b"" if x is None else os.fsencode(x)  # noqa: E731
+        versioned = read_versioned_list(args.versioned_scenes, (enc(args.matches_file), enc(args.output_file),
+                                                                enc(args.initial_solution), enc(args.earlier_record_file),
+                                                                None if args.record_file is None
+                                                                else os.fsencode(args.record_file)))
+        if isinstance(versioned, bytes):
+            sys.stderr.flush()
+            sys.stderr.buffer.write(versioned)
             sys.stderr.buffer.flush()
             return 2
     start = None
@@ -382,6 +485,15 @@ def main(argv=None) -> int:
         if not wire.record_is_valid(earlier_record):
             sys.stderr.write("ERROR: '%s' is not a problem record\n" % args.earlier_record_file)
             return 2
+    starts = None
+    if versioned is not None:
+        starts = read_versioned_starts(versioned, start, earlier_record)
+        if isinstance(starts, bytes):
+            sys.stderr.flush()
+            sys.stderr.buffer.write(starts)
+            sys.stderr.buffer.flush()
+            return 2
+        scenes = [(os.fsdecode(r[0]), os.fsdecode(r[1])) for r in versioned]
 
     rank = int(os.environ.get("RANK", "0"))
     say = (lambda s: print(s, flush=True)) if rank == 0 else (lambda s: None)
@@ -437,14 +549,17 @@ def main(argv=None) -> int:
     for on, msg in ((args.record_file is not None or args.earlier_record_file is not None,
                      "--record_file / --earlier_record_file: torchrun ranks do not write or read problem records"),
                     (args.query_images is not None, "--query_images: torchrun ranks do not localize queries"),
-                    (scenes is not None, "--additional_scenes: torchrun ranks do not refine scene batches"),
-                    (lists is not None, "--listed_pairs: torchrun ranks do not refine list batches")):
+                    (args.additional_scenes is not None, "--additional_scenes: torchrun ranks do not refine scene batches"),
+                    (lists is not None, "--listed_pairs: torchrun ranks do not refine list batches"),
+                    (versioned is not None, "--versioned_scenes: torchrun ranks do not refine scene batches")):
         if torchrun and on:
             sys.stderr.write("ERROR: %s; use --gpus N\n" % msg)
             return 2
     batch = (args, opts, say, solve_fn, n_devices, timing, t_start)
     if lists is not None:
         return _run_batch(refine_lists, (ms, [pairs for _, _, pairs in lists]), lists, *batch)
+    if versioned is not None:
+        return _run_batch(refine_scenes, ([m for m, _ in scenes],), versioned, *batch, starts=starts)
     if scenes is not None:
         return _run_batch(refine_scenes, ([m for m, _ in scenes],), scenes, *batch)
     try:

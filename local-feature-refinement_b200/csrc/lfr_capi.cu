@@ -941,9 +941,14 @@ struct MaxOp {
   __device__ __forceinline__ uint32_t operator()(uint32_t a, uint32_t b) const { return a > b ? a : b; }
 };
 
+// The calling thread's device operations since lfr_debug_device_ops() last reset them: {kernel launch sites checked,
+// CUB calls, synchronising copies to the host} (a test hook: a call's count must not grow with its input's groups)
+thread_local unsigned long long g_device_ops[3] = {};
+
 // one CUB device call: size query, temporary storage, run
 template <typename F>
 int cub_run(DevBuf& tmp, F&& f) {
+  ++g_device_ops[1];
   size_t bytes = 0;
   LFR_CUDA(f(static_cast<void*>(nullptr), bytes));
   LFR_TRY(tmp.reserve(std::max<size_t>(bytes, 1)));
@@ -954,12 +959,17 @@ int cub_run(DevBuf& tmp, F&& f) {
 template <typename T>
 int fetch(T* h, const void* d, size_t count, cudaStream_t s) {
   if (!count) return LFR_OK;
+  ++g_device_ops[2];
   LFR_CUDA(cudaMemcpyAsync(h, d, count * sizeof(T), cudaMemcpyDeviceToHost, s));
   LFR_CUDA(cudaStreamSynchronize(s));
   return LFR_OK;
 }
 
-#define LFR_LAUNCHED() LFR_CUDA(cudaGetLastError())
+#define LFR_LAUNCHED()  \
+  do {                   \
+    ++g_device_ops[0];   \
+    LFR_CUDA(cudaGetLastError()); \
+  } while (0)
 
 // Connected components of 0..n-1 over the edges (a[i], b[i]) (only those inside one group of `gc`
 // when given), labelled in order of their lowest member: label[n], returns the count in *n_out.
@@ -2596,6 +2606,21 @@ int plan_digests(const lfr_plan* pl, cudaStream_t s, uint32_t n_images, const ui
   LFR_CUDA(cudaStreamSynchronize(s));  // before `d_ids` is freed
   return LFR_OK;
 }
+
+// The group of every component of `pl` into cgroup[C] (device, reserved here), from the caller's group of every
+// image (uploaded into d_group, reserved here)
+int component_groups(const lfr_plan* pl, cudaStream_t s, uint32_t n_images, const uint32_t* group_of_image, TmpBuf& d_group,
+                     TmpBuf& cgroup) {
+  const uint32_t N = pl->N, C = pl->C;
+  LFR_TRY(upload(&d_group, group_of_image, n_images, s));
+  LFR_TRY(cgroup.reserve(4 * std::max<size_t>(C, 1)));
+  if (N) {
+    lfr::record::component_group_kernel<<<blocks_for(N), 256, 0, s>>>(pl->comp.as<uint32_t>(), pl->node_image.as<uint32_t>(),
+                                                                      d_group.as<uint32_t>(), N, cgroup.as<uint32_t>());
+    LFR_LAUNCHED();
+  }
+  return LFR_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -2944,6 +2969,122 @@ int lfr_plan_update_solution_since_record(lfr_plan* pl, void* stream, const uint
   }
   LFR_TRY(update_solution(pl, s, d, changed.as<uint8_t>(), n_held, n_touched));
   if (n_changed) *n_changed = (uint32_t)nc;
+  return LFR_OK;
+}
+
+int lfr_plan_update_solution_groups(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
+                                    const uint64_t* name_off, const uint32_t* group_of_image, uint32_t n_groups,
+                                    const uint8_t* const* files, const uint64_t* file_len, const uint8_t* const* records,
+                                    const uint64_t* record_len, uint64_t* n_held, uint32_t* n_touched, uint32_t* n_changed) {
+  const uint32_t G = n_groups;
+  const char* missing = n_images && (!name_off || !group_of_image)                        ? "NULL image names or groups"
+                        : G && ((files && !file_len) || (records && !record_len))           ? "NULL file_len or record_len"
+                                                                                            : nullptr;
+  LFR_TRY(check_names(pl, n_images, names, name_off, missing, group_of_image, G));
+  // every record checked, and every scene's digests back to back: scene g's in [rec_off[g], rec_off[g + 1])
+  std::vector<uint64_t> rec_off((size_t)G + 1, 0);
+  std::vector<uint8_t> has_rec(std::max<uint32_t>(G, 1), 0), rec_bytes;
+  for (uint32_t g = 0; g < G; ++g) {
+    uint64_t R = 0;
+    if (records && records[g]) {
+      if (!lfr::record::check(records[g], record_len[g], &R)) return fail(LFR_EINVAL, "malformed problem record");
+      has_rec[g] = 1;
+      rec_bytes.insert(rec_bytes.end(), records[g] + lfr::record::kHeaderBytes, records[g] + record_len[g]);
+    }
+    rec_off[g + 1] = rec_off[g] + R;
+  }
+  const bool any_rec = std::find(has_rec.begin(), has_rec.end(), (uint8_t)1) != has_rec.end();
+  lfr::join::Decoded d;
+  const uint8_t no_name = 0;
+  if (lfr::join::decode_groups(G, files, file_len, n_images, names ? names : &no_name, name_off, group_of_image, d) != LFR_OK)
+    return fail(LFR_EINVAL, "malformed SolutionFile");
+  if (d.n_disp >= (1ull << 31)) return fail(LFR_EUNSUPPORTED, "SolutionFiles with 2^31 or more displacements");
+  LFR_CUDA(cudaSetDevice(pl->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  const uint32_t C = pl->C;
+  TmpBuf d0, d1, d_group, cgroup, d_rec, d_rec_off, d_has, changed, d_ctr;
+  unsigned long long nc = 0;
+  if (any_rec && C) {
+    // the digests, each component's scene, and one lookup of every component in its own scene's record
+    LFR_TRY(plan_digests(pl, s, n_images, names, name_off, d0, d1));
+    LFR_TRY(component_groups(pl, s, n_images, group_of_image, d_group, cgroup));
+    LFR_TRY(upload(&d_rec, rec_bytes.data(), rec_bytes.size(), s));
+    LFR_TRY(upload(&d_rec_off, rec_off.data(), rec_off.size(), s));
+    LFR_TRY(upload(&d_has, has_rec.data(), has_rec.size(), s));
+    LFR_TRY(changed.reserve(C));
+    LFR_TRY(d_ctr.reserve(8));
+    LFR_CUDA(cudaMemsetAsync(d_ctr.p, 0, 8, s));
+    lfr::record::group_lookup_kernel<<<blocks_for(C), 256, 0, s>>>(
+        d0.as<unsigned long long>(), d1.as<unsigned long long>(), cgroup.as<uint32_t>(), C, d_rec.as<ulonglong2>(),
+        d_rec_off.as<uint64_t>(), d_has.as<uint8_t>(), changed.as<uint8_t>());
+    lfr::start::count_touched_kernel<<<blocks_for(C), 256, 0, s>>>(changed.as<uint8_t>(), C, d_ctr.as<unsigned long long>());
+    LFR_LAUNCHED();
+    LFR_TRY(fetch(&nc, d_ctr.p, 1, s));  // also orders the uploads before the host vectors go
+  }
+  LFR_TRY(update_solution(pl, s, d, any_rec && C ? changed.as<uint8_t>() : nullptr, n_held, n_touched));
+  if (n_changed) *n_changed = (uint32_t)nc;
+  return LFR_OK;
+}
+
+int64_t lfr_plan_problem_record_groups(lfr_plan* pl, void* stream, uint32_t n_images, const uint8_t* names,
+                                       const uint64_t* name_off, const uint32_t* group_of_image, uint32_t n_groups,
+                                       uint8_t* out, uint64_t cap, uint64_t* group_off) {
+  const uint32_t G = n_groups;
+  const char* missing = n_images && (!name_off || !group_of_image) ? "NULL image names or groups"
+                        : !group_off                                 ? "NULL group_off"
+                                                                     : nullptr;
+  LFR_TRY(check_names(pl, n_images, names, name_off, missing, group_of_image, G));
+  LFR_CUDA(cudaSetDevice(pl->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  const uint32_t C = pl->C;
+  TmpBuf d0, d1, d_group, cgroup, iota, k1, i1, k0, k0s, i2, kg, kgs, i3, goff, tmp;
+  // the digests and each component's scene; then (group, d0, d1) order by three stable radix sorts of an index:
+  // by d1, by d0, by group
+  LFR_TRY(plan_digests(pl, s, n_images, names, name_off, d0, d1));
+  LFR_TRY(component_groups(pl, s, n_images, group_of_image, d_group, cgroup));
+  for (TmpBuf* b : {&iota, &i1, &i2, &kg, &kgs, &i3}) LFR_TRY(b->reserve(4 * std::max<size_t>(C, 1)));
+  for (TmpBuf* b : {&k1, &k0, &k0s}) LFR_TRY(b->reserve(8 * std::max<size_t>(C, 1)));
+  LFR_TRY(goff.reserve(8 * ((size_t)G + 1)));
+  const auto* a0 = d0.as<unsigned long long>();
+  const auto* a1 = d1.as<unsigned long long>();
+  if (C) {
+    lfr::graph::iota_kernel<<<blocks_for(C), 256, 0, s>>>(iota.as<uint32_t>(), C);
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, a1, k1.as<unsigned long long>(), iota.as<uint32_t>(), i1.as<uint32_t>(),
+                                             (int)C, 0, 64, s);
+    }));
+    lfr::record::gather_u64_kernel<<<blocks_for(C), 256, 0, s>>>(a0, i1.as<uint32_t>(), C, k0.as<unsigned long long>());
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, k0.as<unsigned long long>(), k0s.as<unsigned long long>(), i1.as<uint32_t>(),
+                                             i2.as<uint32_t>(), (int)C, 0, 64, s);
+    }));
+    lfr::record::gather_u32_kernel<<<blocks_for(C), 256, 0, s>>>(cgroup.as<uint32_t>(), i2.as<uint32_t>(), C, kg.as<uint32_t>());
+    LFR_LAUNCHED();
+    LFR_TRY(cub_run(tmp, [&](void* t, size_t& nb) {
+      return cub::DeviceRadixSort::SortPairs(t, nb, kg.as<uint32_t>(), kgs.as<uint32_t>(), i2.as<uint32_t>(), i3.as<uint32_t>(),
+                                             (int)C, 0, bits_for(G), s);
+    }));
+  }
+  lfr::record::record_group_off_kernel<<<blocks_for((uint64_t)G + 1), 256, 0, s>>>(kgs.as<uint32_t>(), C, G, goff.as<uint64_t>());
+  LFR_LAUNCHED();
+  LFR_TRY(fetch(group_off, goff.p, (size_t)G + 1, s));
+  const uint64_t total = group_off[G];
+  if (!out || cap < total || !total) return (int64_t)total;
+  LFR_TRY(pl->enc_out.reserve(total));
+  lfr::record::record_write_kernel<<<blocks_for((uint64_t)C + G), 256, 0, s>>>(a0, a1, i3.as<uint32_t>(), kgs.as<uint32_t>(), C, G,
+                                                                                goff.as<uint64_t>(), pl->enc_out.as<uint8_t>());
+  LFR_LAUNCHED();
+  LFR_TRY(fetch(out, pl->enc_out.p, total, s));
+  return (int64_t)total;
+}
+
+int lfr_debug_device_ops(unsigned long long* out3, int reset) {
+  for (int k = 0; k < 3; ++k) {
+    if (out3) out3[k] = g_device_ops[k];
+    if (reset) g_device_ops[k] = 0;
+  }
   return LFR_OK;
 }
 

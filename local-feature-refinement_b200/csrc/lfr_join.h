@@ -105,20 +105,10 @@ inline void effective_entries(const Decoded& d, uint64_t i, std::vector<uint64_t
   out.resize(w);
 }
 
-// The host join (lfr_wire_join_solution / _entries): positions[2v .. 2v+1] from node v's entry, 0 without
-// one; has_entry[v] (may be NULL) = whether it has one.  Every output is untouched when the arguments or the
-// bytes are rejected (LFR_EINVAL).
-inline int join_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
-                      uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, double* positions,
-                      uint8_t* has_entry, uint64_t* n_started) {
-  if ((!buf && len) || (n_images && !name_off) || (n_nodes && (!node_image || !node_feat || !positions)))
-    return LFR_EINVAL;
-  for (uint32_t k = 0; k < n_images; ++k)
-    if (name_off[k + 1] < name_off[k]) return LFR_EINVAL;
-  if (n_images && name_off[n_images] && !names) return LFR_EINVAL;
-  const uint8_t no_name = 0;
-  Decoded d;
-  if (decode(buf, len, n_images, names ? names : &no_name, name_off, d) != LFR_OK) return LFR_EINVAL;
+// The host join of a decoded file: positions[2v .. 2v+1] from node v's entry, 0 without one; has_entry[v] (may be
+// NULL) = whether it has one
+inline void join_decoded(const Decoded& d, uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat,
+                         double* positions, uint8_t* has_entry, uint64_t* n_started) {
   // (key, displacement) sorted by key, stably: the last entry of a run of equal keys is the last occurrence
   std::vector<std::pair<uint64_t, uint64_t>> keyed;
   keyed.reserve(d.n_disp);
@@ -143,23 +133,35 @@ inline int join_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const
     if (has_entry) has_entry[v] = hit ? 1 : 0;
   }
   if (n_started) *n_started = started;
+}
+
+// The checks of every host join on the scene's names: NULL arguments, descending name_off
+inline bool names_ok(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                     uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, const double* positions) {
+  if ((!buf && len) || (n_images && !name_off) || (n_nodes && (!node_image || !node_feat || !positions))) return false;
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (name_off[k + 1] < name_off[k]) return false;
+  return !(n_images && name_off[n_images] && !names);
+}
+
+// The host join (lfr_wire_join_solution / _entries): join_decoded() of `buf`.  Every output is untouched when the
+// arguments or the bytes are rejected (LFR_EINVAL).
+inline int join_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                      uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, double* positions,
+                      uint8_t* has_entry, uint64_t* n_started) {
+  if (!names_ok(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions)) return LFR_EINVAL;
+  const uint8_t no_name = 0;
+  Decoded d;
+  if (decode(buf, len, n_images, names ? names : &no_name, name_off, d) != LFR_OK) return LFR_EINVAL;
+  join_decoded(d, n_nodes, node_image, node_feat, positions, has_entry, n_started);
   return LFR_OK;
 }
 
-// The host update (lfr_wire_update_solution): join_nodes() with its flags, then every component with a node
-// without an entry is touched, and so is every component with changed[c] != 0 (`changed` may be NULL: none;
-// lfr_wire_update_solution_since); a touched component's nodes start at 0 and are not held.  held[v] = has
-// entry AND component not touched.  Every output is untouched when the arguments or the bytes are rejected
-// (LFR_EINVAL).
-inline int update_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
-                        uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, const uint32_t* node_comp,
-                        uint32_t n_components, double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched,
-                        const uint8_t* changed = nullptr) {
-  if (n_nodes && (!node_comp || !held)) return LFR_EINVAL;
-  for (uint32_t v = 0; v < n_nodes; ++v)
-    if (node_comp[v] >= n_components) return LFR_EINVAL;
-  const int rc = join_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions, held, nullptr);
-  if (rc != LFR_OK) return rc;
+// The touch rule after a join whose has-entry flags are in `held`: every component with a node without an entry
+// is touched, and so is every component with changed[c] != 0 (`changed` may be NULL: none); a touched component's
+// nodes start at 0 and are not held.  held[v] = has entry AND component not touched.
+inline void touch_components(uint32_t n_nodes, const uint32_t* node_comp, uint32_t n_components, double* positions,
+                             uint8_t* held, uint64_t* n_held, uint32_t* n_touched, const uint8_t* changed) {
   std::vector<uint8_t> touched(n_components, 0);
   if (changed)
     for (uint32_t c = 0; c < n_components; ++c) touched[c] = changed[c] ? 1 : 0;
@@ -176,6 +178,76 @@ inline int update_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, con
   }
   if (n_held) *n_held = nh;
   if (n_touched) *n_touched = (uint32_t)std::count(touched.begin(), touched.end(), (uint8_t)1);
+}
+
+// The host update (lfr_wire_update_solution): join_nodes() with its flags, then touch_components() (`changed`:
+// lfr_wire_update_solution_since).  Every output is untouched when the arguments or the bytes are rejected
+// (LFR_EINVAL).
+inline int update_nodes(const uint8_t* buf, uint64_t len, uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                        uint32_t n_nodes, const uint32_t* node_image, const uint32_t* node_feat, const uint32_t* node_comp,
+                        uint32_t n_components, double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched,
+                        const uint8_t* changed = nullptr) {
+  if (n_nodes && (!node_comp || !held)) return LFR_EINVAL;
+  for (uint32_t v = 0; v < n_nodes; ++v)
+    if (node_comp[v] >= n_components) return LFR_EINVAL;
+  const int rc = join_nodes(buf, len, n_images, names, name_off, n_nodes, node_image, node_feat, positions, held, nullptr);
+  if (rc != LFR_OK) return rc;
+  touch_components(n_nodes, node_comp, n_components, positions, held, n_held, n_touched, changed);
+  return LFR_OK;
+}
+
+// The SolutionFiles of many scenes in one run (lfr_plan_update_solution_groups, lfr_wire_update_solution_groups):
+// file g (files[g], file_len[g] bytes; NULL: no entries) is decoded and resolved against group g's image ids alone
+// (group_of_image[id] < G), since scenes reuse image names, and the decodes are concatenated into `d` with every
+// winning message keyed by its scene image id.  The keys of different groups differ, so one join of `d` gives every
+// node its own scene's entry.  LFR_EINVAL, with *bad_group = g, when file g does not parse.
+inline int decode_groups(uint32_t G, const uint8_t* const* files, const uint64_t* file_len, uint32_t n_images,
+                         const uint8_t* names, const uint64_t* name_off, const uint32_t* group_of_image, Decoded& d,
+                         uint32_t* bad_group = nullptr) {
+  std::vector<uint32_t> start((size_t)G + 1, 0), ids(n_images);  // the ids of every group, ascending
+  for (uint32_t k = 0; k < n_images; ++k) ++start[group_of_image[k] + 1];
+  for (uint32_t g = 0; g < G; ++g) start[g + 1] += start[g];
+  {
+    std::vector<uint32_t> fill(start.begin(), start.end() - 1);
+    for (uint32_t k = 0; k < n_images; ++k) ids[fill[group_of_image[k]]++] = k;
+  }
+  d = Decoded();
+  d.img_ptr.assign(1, 0);
+  std::vector<uint8_t> blob;
+  std::vector<uint64_t> off;
+  const uint8_t no_name = 0;
+  for (uint32_t g = 0; g < G; ++g) {
+    if (!files || !files[g]) continue;
+    const uint32_t a = start[g], n = start[g + 1] - a;
+    blob.clear();
+    off.assign(1, 0);
+    for (uint32_t j = 0; j < n; ++j) {
+      const uint32_t k = ids[a + j];
+      blob.insert(blob.end(), names + name_off[k], names + name_off[k + 1]);
+      off.push_back(blob.size());
+    }
+    Decoded dg;
+    if (decode(files[g], file_len[g], n, blob.empty() ? &no_name : blob.data(), off.data(), dg) != LFR_OK) {
+      if (bad_group) *bad_group = g;
+      return LFR_EINVAL;
+    }
+    if (!dg.canon.empty()) {  // names repeated within the group: each id joins through its group's lowest
+      if (d.canon.empty()) {
+        d.canon.resize(n_images);
+        for (uint32_t k = 0; k < n_images; ++k) d.canon[k] = k;
+      }
+      for (uint32_t j = 0; j < n; ++j) d.canon[ids[a + j]] = ids[a + dg.canon[j]];
+    }
+    for (uint64_t i = 0; i < dg.n_images; ++i) {
+      d.image_id.push_back(dg.image_id[i] == kNoImage ? kNoImage : ids[a + dg.image_id[i]]);
+      d.img_ptr.push_back(d.n_disp + dg.img_ptr[i + 1]);
+    }
+    d.feature_idx.insert(d.feature_idx.end(), dg.feature_idx.begin(), dg.feature_idx.end());
+    d.di.insert(d.di.end(), dg.di.begin(), dg.di.end());
+    d.dj.insert(d.dj.end(), dg.dj.begin(), dg.dj.end());
+    d.n_images += dg.n_images;
+    d.n_disp += dg.n_disp;
+  }
   return LFR_OK;
 }
 

@@ -9,6 +9,9 @@
 //                   the order of the atomics does not matter.
 //   two stable radix sorts (by d1, then by d0) order the digests; lookup_kernel marks the components
 //   whose digest an earlier record lacks (binary search).
+//   Many scenes of one plan: component_group_kernel gives every component its scene, group_lookup_kernel searches
+//   only that scene's slice of the concatenated records, and record_group_off_kernel / record_write_kernel lay out
+//   every scene's record after a third stable radix pass by scene.
 #pragma once
 
 #include <cstdint>
@@ -99,6 +102,82 @@ __global__ void lookup_kernel(const unsigned long long* __restrict__ d0, const u
     if (m.x < a || (m.x == a && m.y < b)) lo = mid + 1; else hi = mid;
   }
   changed[c] = (lo < R && rec[lo].x == a && rec[lo].y == b) ? 0 : 1;
+}
+
+// ---- many scenes in one plan (lfr_plan_update_solution_groups, lfr_plan_problem_record_groups) --------------
+// A component lies in one scene: cgroup[comp[v]] = the group of v's image (the stores of one component agree).
+__global__ void component_group_kernel(const uint32_t* __restrict__ comp, const uint32_t* __restrict__ node_image,
+                                       const uint32_t* __restrict__ group_of_image, uint32_t N, uint32_t* __restrict__ cgroup) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v < N) cgroup[comp[v]] = group_of_image[node_image[v]];
+}
+
+// lookup_kernel within each component's own scene: rec holds every scene's earlier digests back to back, scene g's
+// in [rec_off[g], rec_off[g + 1]), ascending.  A component of a scene without a record (has_rec[g] == 0) is not
+// changed: the plain update rule.
+__global__ void group_lookup_kernel(const unsigned long long* __restrict__ d0, const unsigned long long* __restrict__ d1,
+                                    const uint32_t* __restrict__ cgroup, uint32_t C, const ulonglong2* __restrict__ rec,
+                                    const uint64_t* __restrict__ rec_off, const uint8_t* __restrict__ has_rec,
+                                    uint8_t* __restrict__ changed) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const uint32_t g = cgroup[c];
+  if (!has_rec[g]) {
+    changed[c] = 0;
+    return;
+  }
+  const unsigned long long a = d0[c], b = d1[c];
+  const uint64_t R = rec_off[g + 1];
+  uint64_t lo = rec_off[g], hi = R;  // the first earlier digest of the scene >= (a, b)
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) / 2;
+    const ulonglong2 m = rec[mid];
+    if (m.x < a || (m.x == a && m.y < b)) lo = mid + 1; else hi = mid;
+  }
+  changed[c] = (lo < R && rec[lo].x == a && rec[lo].y == b) ? 0 : 1;
+}
+
+// out[i] = src[idx[i]]
+__global__ void gather_u64_kernel(const unsigned long long* __restrict__ src, const uint32_t* __restrict__ idx, uint32_t n,
+                                  unsigned long long* __restrict__ out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = src[idx[i]];
+}
+
+// out[i] = src[idx[i]]
+__global__ void gather_u32_kernel(const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx, uint32_t n,
+                                  uint32_t* __restrict__ out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = src[idx[i]];
+}
+
+// goff[g] (g <= G) = the byte offset of scene g's record: 16 per record header and per digest before it; `gs` = the
+// C component groups in ascending order
+__global__ void record_group_off_kernel(const uint32_t* __restrict__ gs, uint32_t C, uint32_t G, uint64_t* __restrict__ goff) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g > G) return;
+  uint32_t lo = 0, hi = C;  // the first component of a group >= g
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) / 2;
+    if (gs[mid] < g) lo = mid + 1; else hi = mid;
+  }
+  goff[g] = kHeaderBytes * (uint64_t)g + 16 * (uint64_t)lo;
+}
+
+// Every scene's record into `out`: thread i < C writes the i-th digest in (group, d0, d1) order (component
+// perm[i], of group gs[i]) after the headers of groups 0..gs[i]; thread C + g writes scene g's header.
+__global__ void record_write_kernel(const unsigned long long* __restrict__ d0, const unsigned long long* __restrict__ d1,
+                                    const uint32_t* __restrict__ perm, const uint32_t* __restrict__ gs, uint32_t C, uint32_t G,
+                                    const uint64_t* __restrict__ goff, uint8_t* __restrict__ out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < C) {
+    const uint32_t c = perm[i];
+    *reinterpret_cast<ulonglong2*>(out + kHeaderBytes * ((uint64_t)gs[i] + 1) + 16 * (uint64_t)i) = make_ulonglong2(d0[c], d1[c]);
+  } else if (i < C + G) {
+    const uint32_t g = i - C;
+    const uint64_t n = (goff[g + 1] - goff[g]) / 16 - 1;
+    *reinterpret_cast<ulonglong2*>(out + goff[g]) = make_ulonglong2(kMagic, n);
+  }
 }
 
 }  // namespace record

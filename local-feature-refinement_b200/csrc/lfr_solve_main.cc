@@ -45,7 +45,11 @@
 // the device route) and --listed_pairs FILE (lines `MATCH_LIST<TAB>OUTPUT_FILE`: the pairs of every match list,
 // one `NAME1 NAME2` per line, are taken out of --matches_file, and each list's output file holds what the run on
 // a MatchingFile of those pairs in line order writes: lfr_plan_create_from_wire_listed() expands the file's
-// matches, decoded once, on the device route).  `--n_threads` is accepted and
+// matches, decoded once, on the device route) and --versioned_scenes FILE (lines `MATCHES_FILE<TAB>OUTPUT_FILE<TAB>
+// INITIAL_SOLUTION<TAB>EARLIER_RECORD<TAB>RECORD_FILE`: a scene batch whose every scene is updated from its own
+// solution and record, or solved from zeros without one, and writes its own record: lfr_plan_update_solution_groups()
+// and lfr_plan_problem_record_groups() on the device route, lfr_wire_update_solution_groups() and
+// lfr_host_problem_record_groups() on the host route).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <algorithm>
@@ -123,6 +127,14 @@ int64_t lfr_plan_encode_solution_groups(lfr_plan* plan, void* stream, uint32_t n
                                         const uint64_t* name_off, const float* fact, const uint32_t* group_of_image,
                                         uint32_t n_groups, uint8_t* out, uint64_t cap, uint64_t* group_off,
                                         uint64_t* n_outside) __attribute__((weak));
+int lfr_plan_update_solution_groups(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                    const uint64_t* name_off, const uint32_t* group_of_image, uint32_t n_groups,
+                                    const uint8_t* const* files, const uint64_t* file_len, const uint8_t* const* records,
+                                    const uint64_t* record_len, uint64_t* n_held, uint32_t* n_touched,
+                                    uint32_t* n_changed) __attribute__((weak));
+int64_t lfr_plan_problem_record_groups(lfr_plan* plan, void* stream, uint32_t n_images, const uint8_t* names,
+                                       const uint64_t* name_off, const uint32_t* group_of_image, uint32_t n_groups,
+                                       uint8_t* out, uint64_t cap, uint64_t* group_off) __attribute__((weak));
 }
 
 namespace {
@@ -164,7 +176,8 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"update_initial_solution", false, false}, {"previous_matches_file", true, false},
                                {"record_file", true, false},  {"earlier_record_file", true, false},
                                {"query_images", true, true},  {"joint_queries", false, false},
-                               {"additional_scenes", true, false}, {"listed_pairs", true, false}};
+                               {"additional_scenes", true, false}, {"listed_pairs", true, false},
+                               {"versioned_scenes", true, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -187,7 +200,8 @@ struct Options {
   bool help = false, keep_initial_solution = false, carry_initial_solution = false, update_initial_solution = false,
        joint_queries = false;
   std::string matches_file, output_file, initial_solution;
-  std::optional<std::string> previous_matches_file, record_file, earlier_record_file, additional_scenes, listed_pairs;
+  std::optional<std::string> previous_matches_file, record_file, earlier_record_file, additional_scenes, listed_pairs,
+      versioned_scenes;
   std::vector<std::string> banned_images, fixed_images, query_images;
   uint64_t device = 0, gpus = 1;
 };
@@ -259,6 +273,7 @@ Options parse(int argc, char** argv) {
   o.earlier_record_file = given("earlier_record_file");
   o.additional_scenes = given("additional_scenes");
   o.listed_pairs = given("listed_pairs");
+  o.versioned_scenes = given("versioned_scenes");
   o.banned_images = repeated["banned_images"];
   o.fixed_images = repeated["fixed_images"];
   o.query_images = repeated["query_images"];
@@ -270,11 +285,13 @@ Options parse(int argc, char** argv) {
 }
 
 // The opt-in options the rules between options speak of
-enum Opt { kFixed, kStart, kKeep, kCarry, kUpdate, kPrevious, kRecord, kEarlier, kQuery, kJoint, kScenes, kLists, kNumOpts };
+enum Opt { kFixed, kStart, kKeep, kCarry, kUpdate, kPrevious, kRecord, kEarlier, kQuery, kJoint, kScenes, kLists, kVersioned,
+           kNumOpts };
 const char* const kOptName[kNumOpts] = {"--fixed_images",          "--initial_solution",    "--keep_initial_solution",
                                         "--carry_initial_solution", "--update_initial_solution", "--previous_matches_file",
                                         "--record_file",           "--earlier_record_file", "--query_images",
-                                        "--joint_queries",         "--additional_scenes",   "--listed_pairs"};
+                                        "--joint_queries",         "--additional_scenes",   "--listed_pairs",
+                                        "--versioned_scenes"};
 
 // `opt` needs `others[0]`, or excludes each of `others`
 struct Rule {
@@ -299,6 +316,9 @@ const std::vector<Rule> kRules = {
     {kJoint, true, {kQuery}},
     {kLists, false, [] { std::vector<Opt> v = kOneScene; v.push_back(kScenes); return v; }()},
     {kScenes, false, kOneScene},
+    // every scene of --versioned_scenes starts from its own solution and record, scene 0 from the ordinary flags;
+    // fixed images, kept and carried solutions, earlier MatchingFiles and queries stay one-scene options
+    {kVersioned, false, {kFixed, kKeep, kCarry, kPrevious, kQuery, kJoint, kScenes, kLists}},
 };
 
 // Exits 2 after the ERROR line of the first rule the command line breaks
@@ -306,7 +326,8 @@ void check_rules(const Options& o) {
   const bool set[kNumOpts] = {!o.fixed_images.empty(),       !o.initial_solution.empty(), o.keep_initial_solution,
                               o.carry_initial_solution,      o.update_initial_solution,   o.previous_matches_file.has_value(),
                               o.record_file.has_value(),     o.earlier_record_file.has_value(), !o.query_images.empty(),
-                              o.joint_queries,               o.additional_scenes.has_value(), o.listed_pairs.has_value()};
+                              o.joint_queries,               o.additional_scenes.has_value(), o.listed_pairs.has_value(),
+                              o.versioned_scenes.has_value()};
   for (const Rule& r : kRules) {
     if (!set[r.opt]) continue;
     for (const Opt b : r.others) {
@@ -314,13 +335,18 @@ void check_rules(const Options& o) {
       if (!r.needs && set[b]) fail(2, "ERROR: %s and %s exclude each other\n", kOptName[r.opt], kOptName[b]);
     }
   }
+  // a batch's scenes are updated or solved from zeros: a start point alone belongs to one scene
+  if (set[kVersioned] && set[kStart] && !set[kUpdate])
+    fail(2, "ERROR: %s: %s needs %s\n", kOptName[kVersioned], kOptName[kStart], kOptName[kUpdate]);
 }
 
 // How the solve starts (solve.cc:608-612): from zeros, or from --initial_solution joined, kept, or updated (alone,
-// since --previous_matches_file, since --earlier_record_file)
-enum class Start { kZeros, kJoin, kKeep, kUpdate, kUpdateSinceMatches, kUpdateSinceRecord };
+// since --previous_matches_file, since --earlier_record_file), or with --versioned_scenes every scene updated from its
+// own solution and record or from zeros
+enum class Start { kZeros, kJoin, kKeep, kUpdate, kUpdateSinceMatches, kUpdateSinceRecord, kScenes };
 
 Start start_mode(const Options& o) {
+  if (o.versioned_scenes) return Start::kScenes;
   if (o.initial_solution.empty()) return Start::kZeros;
   if (o.earlier_record_file) return Start::kUpdateSinceRecord;
   if (o.previous_matches_file) return Start::kUpdateSinceMatches;
@@ -342,6 +368,7 @@ Labelling labelling(const Options& o) {
   if (!o.query_images.empty()) return {Labelling::kQueries, "--query_images", "sub-scenes", "query list"};
   if (o.listed_pairs) return {Labelling::kLists, "--listed_pairs", "lists", "pair list"};
   if (o.additional_scenes) return {Labelling::kScenes, "--additional_scenes", "scenes", "scene list"};
+  if (o.versioned_scenes) return {Labelling::kScenes, "--versioned_scenes", "scenes", "scene list"};
   return {Labelling::kNone, nullptr, nullptr, nullptr};
 }
 
@@ -494,6 +521,49 @@ void read_tab_list(const TabList& kind, const std::string& path, StringPairs& ro
     if (!outputs.insert(r.second).second) fail(2, "ERROR: %s: two %s write '%s'\n", kind.option, kind.rows, r.second.c_str());
 }
 
+// The start files of one scene of --versioned_scenes; an empty path is none
+struct VersionedRow {
+  std::string initial, earlier;
+  std::optional<std::string> record;  // none: the scene writes no record (scene 0: no --record_file)
+};
+
+// The --versioned_scenes file: one `MATCHES_FILE<TAB>OUTPUT_FILE<TAB>INITIAL_SOLUTION<TAB>EARLIER_RECORD<TAB>RECORD_FILE`
+// per line (raw bytes; the last newline is optional; the last three fields may be empty), appended to `rows` and
+// `vrows` (scene 0's rows first).  Exits 2 after one ERROR line for an unreadable file, a malformed line, or a file
+// that two outputs or records (those of scene 0 included) would write.
+void read_versioned_list(const std::string& path, StringPairs& rows, std::vector<VersionedRow>& vrows) {
+  std::string text;
+  if (!read_file(path, text)) fail(2, "ERROR: cannot read the scene list file '%s'\n", path.c_str());
+  const std::vector<std::string> lines = lines_of(text);
+  for (size_t k = 0; k < lines.size(); ++k) {
+    const std::string& l = lines[k];
+    std::vector<std::string> f;
+    for (size_t at = 0;;) {
+      const size_t tab = l.find('\t', at);
+      f.push_back(l.substr(at, tab == std::string::npos ? std::string::npos : tab - at));
+      if (tab == std::string::npos) break;
+      at = tab + 1;
+    }
+    const char* why = l.empty()                                ? "it is empty"
+                      : f.size() < 5                           ? "it has fewer than four TABs"
+                      : f.size() > 5                           ? "it has more than four TABs"
+                      : f[0].empty()                           ? "its matches file is empty"
+                      : f[1].empty()                           ? "its output file is empty"
+                      : l.find('\0') != std::string::npos      ? "it holds a NUL byte"
+                      : f[2].empty() && !f[3].empty()          ? "it has an earlier record but no initial solution"
+                                                               : nullptr;
+    if (why)
+      fail(2, "ERROR: --versioned_scenes: line %zu is not MATCHES_FILE<TAB>OUTPUT_FILE<TAB>INITIAL_SOLUTION<TAB>"
+              "EARLIER_RECORD<TAB>RECORD_FILE: %s\n", k + 1, why);
+    rows.emplace_back(f[0], f[1]);
+    vrows.push_back({f[2], f[3], f[4].empty() ? std::optional<std::string>() : f[4]});
+  }
+  std::set<std::string> written;
+  for (size_t i = 0; i < rows.size(); ++i)
+    for (const std::string* w : {&rows[i].second, vrows[i].record ? &*vrows[i].record : nullptr})
+      if (w && !w->empty() && !written.insert(*w).second) fail(2, "ERROR: --versioned_scenes: two files written are '%s'\n", w->c_str());
+}
+
 // The --listed_pairs file: one match list per line (read_tab_list, appended to `rows` after list 0, every pair of
 // --matches_file), every match list read and split as compute_match_graph.py:97 splits it (the newline stripped,
 // single spaces; exactly two fields).  The lines (NAME1, NAME2) of every list, none for list 0.  Exits 2 after one
@@ -569,12 +639,33 @@ int read_previous(const std::string& path, PreviousMatches& pm) {
   return 0;
 }
 
+// The start of one scene of --versioned_scenes: its solution and earlier record, when it has them
+struct SceneStart {
+  bool has_file = false, has_record = false;
+  std::vector<uint8_t> file, record;
+};
+
 // What the start point reads besides the MatchingFiles: the start solution (mapped while the run needs it), the
-// earlier MatchingFile and the earlier record
+// earlier MatchingFile and the earlier record; with --versioned_scenes every scene's start, scene 0's copied from
+// the first two, and the argument arrays of the grouped update
 struct StartInputs {
   FileImage file;
   PreviousMatches previous;
   std::vector<uint8_t> earlier_record;
+  std::vector<SceneStart> scenes;
+  std::vector<const uint8_t*> files, records;  // NULL: none
+  std::vector<uint64_t> file_len, record_len;
+  bool any_file = false;
+  void point() {
+    for (const SceneStart& sc : scenes) {
+      files.push_back(sc.has_file ? (sc.file.empty() ? &kEmpty : sc.file.data()) : nullptr);
+      file_len.push_back(sc.file.size());
+      records.push_back(sc.has_record ? sc.record.data() : nullptr);
+      record_len.push_back(sc.record.size());
+      any_file = any_file || sc.has_file;
+    }
+  }
+  static constexpr uint8_t kEmpty = 0;  // the bytes of an empty SolutionFile
 };
 
 // Read and check the start inputs before any other work, so that their errors come before any output
@@ -600,6 +691,41 @@ void read_start_inputs(const Options& o, StartInputs& si) {
     if (!lfr::record::check(si.earlier_record.data(), si.earlier_record.size(), nullptr))
       fail(2, "ERROR: '%s' is not a problem record\n", path.c_str());
   }
+}
+
+// --versioned_scenes: every scene's start files read and checked (scene 0's by read_start_inputs(), before),
+// in scene order, before any other work.  Exits 2 after one ERROR line naming the list's line.
+void read_versioned_starts(const std::vector<VersionedRow>& vrows, StartInputs& si) {
+  si.scenes.resize(vrows.size());
+  SceneStart& s0 = si.scenes[0];
+  s0.has_file = !vrows[0].initial.empty();
+  s0.file.assign(si.file.data(), si.file.data() + si.file.size());
+  s0.has_record = !vrows[0].earlier.empty();
+  s0.record = si.earlier_record;
+  for (size_t k = 1; k < vrows.size(); ++k) {
+    SceneStart& sc = si.scenes[k];
+    const VersionedRow& v = vrows[k];
+    std::string text;
+    if (!v.initial.empty()) {
+      if (!read_file(v.initial, text))
+        fail(2, "ERROR: --versioned_scenes: line %zu: cannot read the initial solution file '%s'\n", k, v.initial.c_str());
+      sc.file.assign(text.begin(), text.end());
+      sc.has_file = true;
+      uint64_t ni = 0, nd = 0;
+      if (lfr_wire_decode_solution(sc.file.data(), sc.file.size(), &ni, &nd, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                   nullptr, nullptr) != LFR_OK)
+        fail(2, "ERROR: --versioned_scenes: line %zu: the initial solution file '%s' does not parse\n", k, v.initial.c_str());
+    }
+    if (!v.earlier.empty()) {
+      if (!read_file(v.earlier, text))
+        fail(2, "ERROR: --versioned_scenes: line %zu: cannot read the earlier record file '%s'\n", k, v.earlier.c_str());
+      sc.record.assign(text.begin(), text.end());
+      sc.has_record = true;
+      if (!lfr::record::check(sc.record.data(), sc.record.size(), nullptr))
+        fail(2, "ERROR: --versioned_scenes: line %zu: '%s' is not a problem record\n", k, v.earlier.c_str());
+    }
+  }
+  si.point();
 }
 
 // The pairs of all parts in order, with the batch member (scene) of every pair; image ids in order of first
@@ -842,7 +968,8 @@ bool device_route(const lfr_host_input& in, uint64_t gpus) {
                                  lfr_plan_start_from_solution && lfr_plan_keep_solution && lfr_plan_encode_solution_carried &&
                                  lfr_plan_update_solution && lfr_plan_update_solution_since && lfr_plan_problem_record &&
                                  lfr_plan_update_solution_since_record && lfr_plan_encode_solution_images &&
-                                 lfr_plan_encode_solution_groups && lfr_plan_create_from_wire_listed;
+                                 lfr_plan_encode_solution_groups && lfr_plan_create_from_wire_listed &&
+                                 lfr_plan_update_solution_groups && lfr_plan_problem_record_groups;
   const bool on_device = have_device_stage && lfr_graph_stage_on_device(&in, (int32_t)gpus) == 1;
   const char* force = std::getenv("LFR_GRAPH_STAGE");
   if (!force || !*force) return on_device;
@@ -945,19 +1072,40 @@ void print_times(Clock::time_point t_start, Clock::time_point t_solve) {
 }
 
 // What a route gives: the SolutionFile of every output k, bytes[off[k], off[k + 1]), the count of
-// solve.cc:666-669 and the problem record
+// solve.cc:666-669 and the problem record (with --versioned_scenes every scene's, record[record_off[k],
+// record_off[k + 1]))
 struct Result {
   HostArray<uint8_t> bytes;
   std::vector<uint64_t> off;
   uint64_t n_outside = 0;
   std::vector<uint8_t> record;
+  std::vector<uint64_t> record_off;
   bool encoded = true;  // false: the host route's encoder failed, which solve.cc:674-677 reports as a write failure
 };
+
+// --versioned_scenes: every scene's problem record, by one call `fill(out, cap, group_off)` into a buffer sized for
+// the `n_components` of the batch (16 bytes per header and per digest).  Exits 2 when it fails.
+template <class Fill>
+void problem_records(Result& r, size_t n_scenes, uint64_t n_components, Fill fill) {
+  r.record.resize(16 * (n_scenes + n_components));
+  r.record_off.assign(n_scenes + 1, 0);
+  const int64_t got = fill(r.record.data(), r.record.size(), r.record_off.data());
+  if (got < 0 || (uint64_t)got != r.record.size())
+    fail(2, "ERROR: the problem record failed (%d): %s\n", (int)got, lfr_last_error());
+}
+
+// Whether the run writes a problem record: --record_file (given, even with an empty path), or with
+// --versioned_scenes any scene's RECORD_FILE
+bool writes_records(const std::vector<VersionedRow>& vrows) {
+  for (const VersionedRow& v : vrows)
+    if (v.record) return true;
+  return false;
+}
 
 // The device route: the graph stage on the GPU (include/lfr_graph.h), from the mapped parts or from `in`'s decoded
 // matches; the problem stays in HBM for the solve and the SolutionFile is encoded there.
 Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps, const Staged& st, StartInputs& si,
-                  size_t n_out, bool decode_on_device, Clock::time_point t_start) {
+                  size_t n_out, bool record, bool decode_on_device, Clock::time_point t_start) {
   lfr_options opt;
   lfr_options_default(&opt);
   opt.device = (int32_t)o.device;
@@ -991,7 +1139,12 @@ Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps
   const uint8_t* file = si.file.data();
   const uint64_t file_len = si.file.size();
   int rc2 = st.any_fixed ? lfr_plan_fix_images(plan.get(), st.fixed.data(), n_ids) : LFR_OK;
-  if (rc2 == LFR_OK && start == Start::kUpdateSinceRecord) {
+  if (rc2 == LFR_OK && start == Start::kScenes) {
+    if (si.any_file)  // every scene from its own file and record, in one call; without any file all start at zero
+      rc2 = lfr_plan_update_solution_groups(plan.get(), nullptr, n_ids, names, name_off, st.image_group.data(), (uint32_t)n_out,
+                                            si.files.data(), si.file_len.data(), si.records.data(), si.record_len.data(),
+                                            nullptr, nullptr, nullptr);
+  } else if (rc2 == LFR_OK && start == Start::kUpdateSinceRecord) {
     rc2 = lfr_plan_update_solution_since_record(plan.get(), nullptr, file, file_len, n_ids, names, name_off,
                                                 si.earlier_record.data(), si.earlier_record.size(), nullptr, nullptr,
                                                 nullptr);
@@ -1025,7 +1178,12 @@ Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps
   print_times(t_start, t_solve);
 
   Result r;
-  if (o.record_file)
+  if (record && start == Start::kScenes)
+    problem_records(r, n_out, sz.n_components, [&](uint8_t* out, uint64_t cap, uint64_t* group_off) {
+      return lfr_plan_problem_record_groups(plan.get(), nullptr, n_ids, names, name_off, st.image_group.data(),
+                                            (uint32_t)n_out, out, cap, group_off);
+    });
+  else if (record)
     problem_record(r.record, [&](uint8_t* out, uint64_t cap) {
       return lfr_plan_problem_record(plan.get(), nullptr, n_ids, names, name_off, out, cap);
     });
@@ -1072,7 +1230,7 @@ Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps
 // The host route: the host graph stage (solve.cc:438-606) writing the edge records straight into page-locked
 // memory, the start point joined on the host, lfr_solve() / lfr_solve_multi() and the output assembly.
 Result run_host(const Options& o, Start start, const Labelling& lab, const Pairs& ps, Staged& st, StartInputs& si,
-                size_t n_out, Clock::time_point t_start) {
+                size_t n_out, bool record, Clock::time_point t_start) {
   const HostArray<lfr_edge> edges_buf = st.e_cap ? host_array<lfr_edge>(st.e_cap) : nullptr;
   lfr_edge* edges = edges_buf.get();
   st.in.edges_out = edges; st.in.edges_out_capacity = st.e_cap;
@@ -1112,7 +1270,14 @@ Result run_host(const Options& o, Start start, const Labelling& lab, const Pairs
     positions = positions_buf.get();
     std::memset(positions, 0, 2ull * N * sizeof(double));
     std::vector<uint8_t> has_entry(holds_entries(start) ? N : 0, 0);
-    if (start == Start::kUpdateSinceRecord) {
+    if (start == Start::kScenes) {
+      if (si.any_file &&
+          lfr_wire_update_solution_groups(n_ids, names, name_off, st.image_group.data(), (uint32_t)n_out, si.files.data(),
+                                          si.file_len.data(), si.records.data(), si.record_len.data(), &prob,
+                                          node_image.data(), node_feat.data(), positions, has_entry.data(), nullptr,
+                                          nullptr, nullptr) != LFR_OK)
+        fail(2, "ERROR: lfr_wire_update_solution_groups failed\n");
+    } else if (start == Start::kUpdateSinceRecord) {
       if (lfr_wire_update_solution_since_record(file, file_len, n_ids, names, name_off, &prob, node_image.data(),
                                                 node_feat.data(), si.earlier_record.data(), si.earlier_record.size(),
                                                 positions, has_entry.data(), nullptr, nullptr, nullptr) != LFR_OK)
@@ -1165,7 +1330,12 @@ Result run_host(const Options& o, Start start, const Labelling& lab, const Pairs
   print_times(t_start, t_solve);
 
   Result r;
-  if (o.record_file)
+  if (record && start == Start::kScenes)
+    problem_records(r, n_out, C, [&](uint8_t* out, uint64_t cap, uint64_t* group_off) {
+      return lfr_host_problem_record_groups(&prob, node_image.data(), node_feat.data(), n_ids, names, name_off,
+                                            st.image_group.data(), (uint32_t)n_out, out, cap, group_off);
+    });
+  else if (record)
     problem_record(r.record, [&](uint8_t* out, uint64_t cap) {
       return lfr_host_problem_record(&prob, node_image.data(), node_feat.data(), n_ids, names, name_off, out, cap);
     });
@@ -1272,12 +1442,18 @@ int run(int argc, char** argv) {
   // with --additional_scenes every listed scene (each scene's output is what its own run writes: the same command
   // with that scene's two files alone), or with --listed_pairs every listed match list (its output is what the same
   // command writes on a MatchingFile that holds the file's pair for every line of the list, in line order)
+  // with --versioned_scenes every listed scene, whose output and record are what its own run writes: the same
+  // command with that scene's files alone, updated from its initial solution (and earlier record) when it has one
   StringPairs rows{{o.matches_file, o.output_file}};
   std::vector<StringPairs> lists;
+  std::vector<VersionedRow> vrows{{o.initial_solution, o.earlier_record_file.value_or(""), o.record_file}};
   if (o.listed_pairs) lists = read_pair_lists(*o.listed_pairs, rows);
   if (o.additional_scenes) read_tab_list(kSceneList, *o.additional_scenes, rows);
+  if (o.versioned_scenes) read_versioned_list(*o.versioned_scenes, rows, vrows);
   StartInputs si;
   read_start_inputs(o, si);
+  if (o.versioned_scenes) read_versioned_starts(vrows, si);
+  const bool record = writes_records(vrows);
 
   // A one-shot process pays for CUDA's start-up (driver initialisation over every visible GPU, context
   // creation: 0.4-0.8 s on an 8-GPU box) more than for all of its work on a Fountain-scale scene.  Two
@@ -1304,8 +1480,8 @@ int run(int argc, char** argv) {
 
   cuda_start.join();  // page-locked memory needs the context
   const Clock::time_point t_start = Clock::now();
-  Result r = on_device ? run_device(o, start, lab, ps, st, si, rows.size(), decode_on_device, t_start)
-                       : run_host(o, start, lab, ps, st, si, rows.size(), t_start);
+  Result r = on_device ? run_device(o, start, lab, ps, st, si, rows.size(), record, decode_on_device, t_start)
+                       : run_host(o, start, lab, ps, st, si, rows.size(), record, t_start);
   si.file.release();
   std::printf("# points with at least one coordinate > 0.5: %llu\n", (unsigned long long)r.n_outside);  // solve.cc:670
   std::fflush(stdout);
@@ -1318,10 +1494,14 @@ int run(int argc, char** argv) {
     written = written && f.good();
   }
   if (!written) fail(255, "Failed to write proto object.\n");  // solve.cc:674-677
-  if (o.record_file) {
-    std::ofstream f(*o.record_file, std::ios::binary | std::ios::trunc);
-    if (f.good()) f.write(reinterpret_cast<const char*>(r.record.data()), (std::streamsize)r.record.size());
-    if (!f.good()) fail(255, "ERROR: cannot write the record file '%s'\n", o.record_file->c_str());
+  if (r.record_off.empty()) r.record_off = {0, r.record.size()};
+  for (size_t k = 0; record && k < vrows.size(); ++k) {  // scene order (one scene without --versioned_scenes)
+    if (!vrows[k].record) continue;
+    const std::string& path = *vrows[k].record;
+    std::ofstream f(path, std::ios::binary | std::ios::trunc);
+    const uint64_t n = r.record_off[k + 1] - r.record_off[k];
+    if (f.good()) f.write(reinterpret_cast<const char*>(r.record.data() + r.record_off[k]), (std::streamsize)n);
+    if (!f.good()) fail(255, "ERROR: cannot write the record file '%s'\n", path.c_str());
   }
   return 0;
 }

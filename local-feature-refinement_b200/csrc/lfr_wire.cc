@@ -716,6 +716,112 @@ int lfr_wire_update_solution_since_record(const uint8_t* buf, uint64_t len, uint
   return rc;
 }
 
+namespace {
+
+// The group of every component of `p`: its nodes' (one scene per component); LFR_EINVAL when a node's image has
+// no group below G or a component's nodes span two groups
+int component_groups(const lfr_problem* p, const uint32_t* node_image, uint32_t n_images, const uint32_t* group_of_image,
+                     uint32_t G, std::vector<uint32_t>& group) {
+  constexpr uint32_t kNone = 0xffffffffu;
+  if (n_images && !group_of_image) return LFR_EINVAL;
+  for (uint32_t k = 0; k < n_images; ++k)
+    if (group_of_image[k] >= G) return LFR_EINVAL;
+  group.assign(p->n_components, kNone);
+  for (uint32_t v = 0; v < p->n_nodes; ++v) {
+    uint32_t& g = group[p->comp[v]];
+    const uint32_t gv = group_of_image[node_image[v]];
+    if (g != kNone && g != gv) return LFR_EINVAL;
+    g = gv;
+  }
+  return LFR_OK;
+}
+
+}  // namespace
+
+int lfr_wire_update_solution_groups(uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                                    const uint32_t* group_of_image, uint32_t n_groups, const uint8_t* const* files,
+                                    const uint64_t* file_len, const uint8_t* const* records, const uint64_t* record_len,
+                                    const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat,
+                                    double* positions, uint8_t* held, uint64_t* n_held, uint32_t* n_touched,
+                                    uint32_t* n_changed) {
+  namespace rec = lfr::record;
+  namespace join = lfr::join;
+  if (!record_input_ok(p, node_image, node_feat, n_images, names, name_off)) return LFR_EINVAL;
+  const uint32_t N = p->n_nodes, C = p->n_components, G = n_groups;
+  if (N && (!positions || !held)) return LFR_EINVAL;
+  if (G && ((files && !file_len) || (records && !record_len))) return LFR_EINVAL;
+  std::vector<uint32_t> cgroup;
+  if (component_groups(p, node_image, n_images, group_of_image, G, cgroup) != LFR_OK) return LFR_EINVAL;
+  // every record checked, and its digests as (group, d0, d1), ascending
+  std::vector<std::array<uint64_t, 3>> earlier;
+  std::vector<uint8_t> has_record(G, 0);
+  for (uint32_t g = 0; records && g < G; ++g) {
+    if (!records[g]) continue;
+    uint64_t R = 0;
+    if (!rec::check(records[g], record_len[g], &R)) return LFR_EINVAL;
+    has_record[g] = 1;
+    for (uint64_t k = 0; k < R; ++k)
+      earlier.push_back({g, rec::load_u64(records[g] + rec::kHeaderBytes + 16 * k),
+                         rec::load_u64(records[g] + rec::kHeaderBytes + 16 * k + 8)});
+  }
+  join::Decoded d;
+  const uint8_t no_name = 0;
+  if (join::decode_groups(G, files, file_len, n_images, names ? names : &no_name, name_off, group_of_image, d) != LFR_OK)
+    return LFR_EINVAL;
+  // a component of a scene with a record is changed when its digest is not in that scene's record
+  std::vector<uint8_t> changed(C, 0);
+  uint32_t nc = 0;
+  if (std::find(has_record.begin(), has_record.end(), (uint8_t)1) != has_record.end()) {
+    const std::vector<Digest> dg = component_digests(p, node_image, node_feat, n_images, names, name_off);
+    for (uint32_t c = 0; c < C; ++c) {
+      if (cgroup[c] >= G || !has_record[cgroup[c]]) continue;
+      const std::array<uint64_t, 3> key{cgroup[c], dg[c].first, dg[c].second};
+      if (!std::binary_search(earlier.begin(), earlier.end(), key)) {
+        changed[c] = 1;
+        ++nc;
+      }
+    }
+  }
+  join::join_decoded(d, N, node_image, node_feat, positions, held, nullptr);
+  join::touch_components(N, p->comp, C, positions, held, n_held, n_touched, changed.data());
+  if (n_changed) *n_changed = nc;
+  return LFR_OK;
+}
+
+int64_t lfr_host_problem_record_groups(const lfr_problem* p, const uint32_t* node_image, const uint32_t* node_feat,
+                                       uint32_t n_images, const uint8_t* names, const uint64_t* name_off,
+                                       const uint32_t* group_of_image, uint32_t n_groups, uint8_t* out, uint64_t cap,
+                                       uint64_t* group_off) {
+  namespace rec = lfr::record;
+  if (!record_input_ok(p, node_image, node_feat, n_images, names, name_off) || !group_off) return LFR_EINVAL;
+  const uint32_t C = p->n_components, G = n_groups;
+  std::vector<uint32_t> cgroup;
+  if (component_groups(p, node_image, n_images, group_of_image, G, cgroup) != LFR_OK) return LFR_EINVAL;
+  std::vector<std::array<uint64_t, 3>> d(C);
+  {
+    const std::vector<Digest> dg = component_digests(p, node_image, node_feat, n_images, names, name_off);
+    for (uint32_t c = 0; c < C; ++c) d[c] = {cgroup[c], dg[c].first, dg[c].second};
+  }
+  std::sort(d.begin(), d.end());
+  // output g: its header, then its digests; group_off[g] = 16 g + 16 (the components of the groups before g)
+  std::vector<uint64_t> count(G, 0);
+  for (const auto& x : d) ++count[x[0]];
+  group_off[0] = 0;
+  for (uint32_t g = 0; g < G; ++g) group_off[g + 1] = group_off[g] + rec::record_bytes(count[g]);
+  const uint64_t need = group_off[G];
+  if (!out || cap < need) return (int64_t)need;
+  for (uint32_t g = 0; g < G; ++g) {
+    rec::store_u64(out + group_off[g], rec::kMagic);
+    rec::store_u64(out + group_off[g] + 8, count[g]);
+  }
+  for (uint32_t c = 0; c < C; ++c) {
+    uint8_t* at = out + rec::kHeaderBytes * (d[c][0] + 1) + 16 * (uint64_t)c;
+    rec::store_u64(at, d[c][1]);
+    rec::store_u64(at + 8, d[c][2]);
+  }
+  return (int64_t)need;
+}
+
 int64_t lfr_wire_encode_solution_carried(uint64_t n_images, const uint64_t* img_ptr, const uint8_t* names,
                                          const uint64_t* name_off, const float* fact, const uint32_t* feature_idx,
                                          const float* di, const float* dj, const uint8_t* file, uint64_t file_len,

@@ -148,21 +148,30 @@ def fixed_image_mask(image_names: List[str], fixed_images) -> np.ndarray:
 
 def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[bytes] = None,
                      keep_initial_solution: bool = False, update_initial_solution: bool = False,
-                     previous_matches: Optional[MatchSet] = None, previous_record: Optional[bytes] = None):
+                     previous_matches: Optional[MatchSet] = None, previous_record: Optional[bytes] = None,
+                     image_group: Optional[np.ndarray] = None, scene_solutions=None, scene_records=None):
     """The host route's problem initialisation with fixed images and a start solution: (the Problem to solve,
     whose is_root is the constant mask = reference root OR node of a fixed image OR, with
     `keep_initial_solution`, node with an entry in the start solution OR, with `update_initial_solution`,
     node of a component the start solution covers whole (wire.update_solution) and, with `previous_matches`,
     that is unchanged since that MatchingFile's run (wire.update_solution_since) or, with `previous_record`,
     whose digest is in that run's problem record (wire.update_solution_since_record); start positions [N, 2]
-    from wire.join_solution or wire.update_solution(_since(_record)), or None for zeros)."""
+    from wire.join_solution or wire.update_solution(_since(_record)), or None for zeros).
+
+    With `scene_solutions` (one per scene of `image_group`: SolutionFile bytes or None) every scene is updated as its
+    own run from its own file and, where scene_records[g] is not None, against that earlier record
+    (wire.update_solution_groups); a scene without a file solves from zeros."""
     from . import wire
     g = p.graph
     const = np.asarray(p.is_root) != 0
     if len(fixed_images) and g.n_nodes:
         const = const | fixed_image_mask(g.image_names, fixed_images)[np.asarray(g.node_image, np.int64)]
     start = None
-    if initial_solution is not None and update_initial_solution and previous_record is not None:
+    if scene_solutions is not None:
+        if any(x is not None for x in scene_solutions):
+            start, held, _, _, _ = wire.update_solution_groups(scene_solutions, p, image_group, scene_records)
+            const = const | held
+    elif initial_solution is not None and update_initial_solution and previous_record is not None:
         start, held, _, _, _ = wire.update_solution_since_record(initial_solution, p, previous_record)
         const = const | held
     elif initial_solution is not None and update_initial_solution and previous_matches is not None:
@@ -176,7 +185,7 @@ def constant_problem(p: Problem, fixed_images=(), initial_solution: Optional[byt
         start, _, has_entry = wire.join_solution(initial_solution, g.image_names, g.node_image, g.node_feat, entries=True)
         if keep_initial_solution:
             const = const | has_entry
-    if (len(fixed_images) or keep_initial_solution or update_initial_solution) and g.n_nodes:
+    if (len(fixed_images) or keep_initial_solution or update_initial_solution or scene_solutions is not None) and g.n_nodes:
         return dataclasses.replace(p, is_root=const.astype(np.uint8)), start
     return p, start
 
@@ -186,7 +195,8 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
            initial_solution: Optional[bytes] = None, keep_initial_solution: bool = False,
            update_initial_solution: bool = False, previous_matches=None, previous_record: Optional[bytes] = None,
            record_problem: bool = False, query_images=None, joint_queries: bool = False,
-           image_group: Optional[np.ndarray] = None):
+           image_group: Optional[np.ndarray] = None, scene_solutions=None, scene_records=None,
+           n_groups: Optional[int] = None):
     """MatchSet -> (Problem, positions, stats, Solution).  `solve_fn(problem)`
     may be supplied to drive a different executor (the multi-GPU path; give `n_devices`); with a start
     solution it is called as `solve_fn(problem, positions)`.
@@ -222,7 +232,11 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     message is the one a run on its group's pairs alone writes.
 
     `image_group` ([n_images], MatchSet.join_scenes) stages every group of ids as a scene of its own, as
-    refine_scenes() does; it excludes query_images (ValueError)."""
+    refine_scenes() does; it excludes query_images (ValueError).  With it, `n_groups` scenes, `scene_solutions`
+    (one SolutionFile or None per scene) and `scene_records` (one earlier problem record or None per scene) update
+    every scene as its own run (Plan.update_solution_groups, wire.update_solution_groups), and `record_problem`
+    makes the Solution's `record` the list of every scene's problem record (Plan.problem_record_groups,
+    wire.problem_record_groups)."""
     from .capi import Plan, load_b200
     from .graph import host_input_arrays, problem_from_stage
     if keep_initial_solution and initial_solution is None:
@@ -270,11 +284,14 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     if not graph_stage_on_device(lib, arrs, len(ms.image_names), n_devices):
         p = build_problem(ms, banned_images, log=log, image_group=image_group)
         q, start = constant_problem(p, fixed_images, initial_solution, keep_initial_solution, update_initial_solution,
-                                    previous_matches, previous_record)
+                                    previous_matches, previous_record, image_group, scene_solutions, scene_records)
         fn = solve_fn if solve_fn is not None else (lambda q_, x=None: solve_problem(q_, options, x))
         pos, st = fn(q) if start is None else fn(q, start)
         sol = assemble_solution(p, pos, written)
-        if record_problem:
+        if record_problem and image_group is not None:
+            from .wire import problem_record_groups
+            sol.record = problem_record_groups(p, image_group, n_groups)
+        elif record_problem:
             from .wire import problem_record
             sol.record = problem_record(p, ms.image_names)
         return p, pos, st, sol
@@ -282,7 +299,10 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
     try:
         if len(fixed_images) and fixed_image_mask(ms.image_names, fixed_images).any():
             plan.fix_images(fixed_image_mask(ms.image_names, fixed_images))
-        if update_initial_solution and previous_record is not None:
+        if scene_solutions is not None:
+            if any(x is not None for x in scene_solutions):
+                plan.update_solution_groups(scene_solutions, ms.image_names, image_group, scene_records)
+        elif update_initial_solution and previous_record is not None:
             plan.update_solution(initial_solution, ms.image_names, previous_record=previous_record)
         elif update_initial_solution and previous_matches is not None:
             prev = Plan.from_matches(lib, previous_matches, options=options)
@@ -305,7 +325,10 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
             pos, st = solve_problem(p, options)
         if timing is not None:
             timing["solver_ms"] = (time.perf_counter() - t1) * 1e3
-        record = plan.problem_record(ms.image_names) if record_problem else None
+        if record_problem and image_group is not None:
+            record = plan.problem_record_groups(ms.image_names, image_group, n_groups)
+        else:
+            record = plan.problem_record(ms.image_names) if record_problem else None
     finally:
         plan.close()
     sol = assemble_solution(p, pos, written)
@@ -315,28 +338,54 @@ def refine(ms: MatchSet, banned_images=(), options=None, log: Optional[Callable[
 
 def refine_scenes(match_sets: List[MatchSet], banned_images=(), options=None, log: Optional[Callable[[str], None]] = None,
                   solve_fn=None, n_devices: int = 1, timing: Optional[dict] = None,
-                  solutions: Optional[list] = None) -> List[bytes]:
+                  solutions: Optional[list] = None, initial_solutions=None, previous_records=None,
+                  record_problem: bool = False) -> List[bytes]:
     """--additional_scenes: refine many scenes in one run and return one SolutionFile per scene, each byte for
     byte what refine() + wire.encode_solution write for that scene alone with the same `banned_images` (names,
     applied to every scene).  The scenes are one ordinary run (MatchSet.join_scenes: every scene a sub-scene
     with its own image ids), so its route, `log` lines and statistics are those of the whole batch: the counts
     are the sums over the scenes' own runs and the maxima their maxima.  `solutions`, when given, receives
     every scene's Solution (its n_outside is the scene's own count).  More than 65535 image ids over all
-    scenes raise ValueError."""
+    scenes raise ValueError.
+
+    `initial_solutions` and `previous_records` (--versioned_scenes) are per-scene lists, None meaning none for that
+    scene: a scene with a SolutionFile is updated from it as refine(update_initial_solution=True) updates a scene
+    alone, against its own earlier problem record when it has one (a record without a SolutionFile raises
+    ValueError); a scene without one solves from zeros.  With `record_problem` every scene's Solution in
+    `solutions` gets the problem record of its own run in `record`.  Each scene's bytes and record are those of its
+    own run."""
+    G = len(match_sets)
+    for name, lst in (("initial_solutions", initial_solutions), ("previous_records", previous_records)):
+        if lst is not None and len(lst) != G:
+            raise ValueError("%s has %d entries for %d scenes" % (name, len(lst), G))
+    if previous_records is not None:
+        from .wire import record_is_valid
+        for k, r in enumerate(previous_records):
+            if r is not None and (initial_solutions is None or initial_solutions[k] is None):
+                raise ValueError("previous_records[%d] needs initial_solutions[%d]" % (k, k))
+            if r is not None and not record_is_valid(bytes(r)):
+                raise ValueError("previous_records[%d] is not a problem record" % k)
+    if initial_solutions is not None and previous_records is None:
+        previous_records = [None] * G
     return _refine_batch(match_sets, banned_images, options, log, solve_fn, n_devices, timing, solutions,
                          "additional_scenes: the scenes hold %d images, more than 65535; split the scene list over "
-                         "several runs")
+                         "several runs", initial_solutions, previous_records, record_problem)
 
 
-def _refine_batch(match_sets, banned_images, options, log, solve_fn, n_devices, timing, solutions, too_many: str):
+def _refine_batch(match_sets, banned_images, options, log, solve_fn, n_devices, timing, solutions, too_many: str,
+                  initial_solutions=None, previous_records=None, record_problem=False):
     """refine_scenes() and refine_lists(): `too_many` % n_ids is the ValueError past 65535 image ids."""
     from .wire import encode_solution
     ms, image_group = MatchSet.join_scenes(match_sets, banned_images)
     if len(ms.image_names) > 65535:
         raise ValueError(too_many % len(ms.image_names))
-    p, pos, _, _ = refine(ms, (), options, log=log, solve_fn=solve_fn, n_devices=n_devices, timing=timing,
-                          image_group=image_group)
+    p, pos, _, whole = refine(ms, (), options, log=log, solve_fn=solve_fn, n_devices=n_devices, timing=timing,
+                              image_group=image_group, scene_solutions=initial_solutions, scene_records=previous_records,
+                              n_groups=len(match_sets), record_problem=record_problem)
     sols = assemble_scene_solutions(p, pos, image_group, len(match_sets))
+    if record_problem:
+        for sol, rec in zip(sols, whole.record):
+            sol.record = rec
     if solutions is not None:
         solutions.extend(sols)
     return [encode_solution(s.image_names, s.fact, s.img_ptr, s.feature_idx, s.di, s.dj) for s in sols]

@@ -29,7 +29,8 @@ class WireMatches(C.Structure):
 WIRE_SYMBOLS = ["lfr_wire_scan_matches", "lfr_wire_decode_matches", "lfr_wire_walk_matches", "lfr_wire_encode_matches",
                 "lfr_wire_encode_solution", "lfr_wire_decode_solution", "lfr_wire_join_solution",
                 "lfr_wire_join_solution_entries", "lfr_wire_encode_solution_carried", "lfr_wire_update_solution",
-                "lfr_wire_update_solution_since", "lfr_host_problem_record", "lfr_wire_update_solution_since_record"]
+                "lfr_wire_update_solution_since", "lfr_host_problem_record", "lfr_wire_update_solution_since_record",
+                "lfr_wire_update_solution_groups", "lfr_host_problem_record_groups"]
 
 _bound = False
 
@@ -72,6 +73,13 @@ def _lib():
                                                             [C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64),
                                                              C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)])
         L.lfr_wire_update_solution_since_record.restype = C.c_int
+        L.lfr_wire_update_solution_groups.argtypes = ([C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32] +
+                                                      [C.c_void_p] * 9 + [C.POINTER(C.c_uint64), C.POINTER(C.c_uint32),
+                                                                            C.POINTER(C.c_uint32)])
+        L.lfr_wire_update_solution_groups.restype = C.c_int
+        L.lfr_host_problem_record_groups.argtypes = ([C.c_void_p] * 3 + [C.c_uint32] + [C.c_void_p] * 3 + [C.c_uint32] +
+                                                     [C.c_void_p, C.c_uint64, C.c_void_p])
+        L.lfr_host_problem_record_groups.restype = C.c_int64
         _bound = True
     return L
 
@@ -463,3 +471,66 @@ def update_solution_since_record(data: bytes, p, record: bytes):
     if rc != 0:
         raise RuntimeError("lfr_wire_update_solution_since_record failed (%d)" % rc)
     return pos, held.astype(bool), int(n.value), int(t.value), int(ch.value)
+
+
+def group_arrays(blobs):
+    """The (pointer array, length array, keep-alive list) of a C call's per-group byte buffers (files[], file_len[]
+    or records[], record_len[]): a NULL pointer where `blobs[g]` is None."""
+    keep = [None if b is None else np.frombuffer(bytes(b) or b"\0", dtype=np.uint8) for b in blobs]
+    ptrs = (C.c_void_p * max(len(blobs), 1))(*[None if k is None else k.ctypes.data for k in keep])
+    lens = np.array([0 if b is None else len(b) for b in blobs] or [0], np.uint64)
+    return ptrs, lens, keep
+
+
+def update_solution_groups(solutions, p, image_group, records=None):
+    """The host form of Plan.update_solution_groups (lfr_wire_update_solution_groups, include/lfr_host.h): every
+    scene g of Problem `p` (image id k in scene image_group[k]) updated as its own run from solutions[g]
+    (SolutionFile bytes, or None: every component of the scene is touched) and, where records[g] is not None, against
+    that earlier problem record.  Returns (positions [N, 2], held [N] bool, held nodes, touched components, changed
+    components).  Raises ValueError on a malformed record, ParseError on a SolutionFile the decoder rejects."""
+    L = _lib()
+    G = len(solutions)
+    records = [None] * G if records is None else list(records)
+    for r in records:
+        if r is not None and not record_is_valid(bytes(r)):
+            raise ValueError("malformed problem record")
+    for sol in solutions:
+        if sol is not None and not _solution_parses(bytes(sol)):
+            raise ParseError("Failed to parse proto object.")
+    s, keep, blob, off, img, feat = _record_args(p, None)
+    group = np.ascontiguousarray(image_group, dtype=np.uint32).reshape(-1)
+    fptr, flen, fkeep = group_arrays(solutions)
+    rptr, rlen, rkeep = group_arrays(records)
+    N = int(img.shape[0])
+    pos = np.zeros((N, 2), np.float64)
+    held = np.zeros(N, np.uint8)
+    n, t, ch = C.c_uint64(), C.c_uint32(), C.c_uint32()
+    rc = L.lfr_wire_update_solution_groups(len(off) - 1, blob.ctypes.data, off.ctypes.data,
+                                           group.ctypes.data if group.size else None, G, fptr, flen.ctypes.data, rptr,
+                                           rlen.ctypes.data, C.addressof(s), img.ctypes.data if N else None,
+                                           feat.ctypes.data if N else None, pos.ctypes.data if N else None,
+                                           held.ctypes.data if N else None, C.byref(n), C.byref(t), C.byref(ch))
+    del keep, fkeep, rkeep
+    if rc != 0:
+        raise RuntimeError("lfr_wire_update_solution_groups failed (%d)" % rc)
+    return pos, held.astype(bool), int(n.value), int(t.value), int(ch.value)
+
+
+def problem_record_groups(p, image_group, n_groups: int) -> List[bytes]:
+    """The problem record of every scene g < n_groups of Problem `p` on the host (lfr_host_problem_record_groups,
+    include/lfr_host.h), each byte for byte problem_record() of the scene's own run and Plan.problem_record_groups()."""
+    L = _lib()
+    s, keep, blob, off, img, feat = _record_args(p, None)
+    group = np.ascontiguousarray(image_group, dtype=np.uint32).reshape(-1)
+    goff = np.zeros(n_groups + 1, np.uint64)
+    N = int(img.shape[0])
+    args = (C.addressof(s), img.ctypes.data if N else None, feat.ctypes.data if N else None, len(off) - 1,
+            blob.ctypes.data, off.ctypes.data, group.ctypes.data if group.size else None, n_groups)
+    cap = 16 * (n_groups + int(p.n_components))
+    out = np.empty(max(cap, 1), np.uint8)
+    got = L.lfr_host_problem_record_groups(*args, out.ctypes.data, cap, goff.ctypes.data)
+    del keep
+    if got != cap:
+        raise RuntimeError("lfr_host_problem_record_groups failed (%d)" % got)
+    data = out[:cap].tobytes()
+    return [data[int(goff[g]):int(goff[g + 1])] for g in range(n_groups)]
