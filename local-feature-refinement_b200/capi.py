@@ -211,7 +211,9 @@ class Library:
 
     def check(self, rc: int, what: str) -> None:
         if rc != LFR_OK:
-            raise RuntimeError("lfr: %s failed (%d): %s" % (what, rc, self.last_error()))
+            e = RuntimeError("lfr: %s failed (%d): %s" % (what, rc, self.last_error()))
+            e.lfr_rc = rc   # LFR_ECUDA and LFR_ENODEV end a task stream (cli.run_task_stream)
+            raise e
 
     @property
     def has_graph_stage(self) -> bool:

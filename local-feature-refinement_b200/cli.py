@@ -45,6 +45,9 @@ the last three fields may be empty) updates many scenes in one run: a scene with
 from it (and against its earlier record) as --update_initial_solution updates it alone, one without solves from
 zeros, and each output and record file is byte for byte what that scene's own run writes (solver.refine_scenes with
 initial_solutions, previous_records and record_problem).  Scene 0's start comes from the ordinary flags.
+--task_stream FILE (with --device, --gpus and --n_threads alone) runs every line of FILE, read as it arrives, as a task
+in one process: each line's TAB-separated fields are the argument vector of one main() run, and `# task K: exit C`
+follows each on stdout, so torch and the library are loaded once (run_task_stream).
 
 The graph stage (solve.cc:438-606) runs where the library's size rule says
 (lfr_graph_stage_on_device, include/lfr_graph.h): on the device for large inputs
@@ -61,6 +64,7 @@ import os
 import subprocess
 import sys
 import time
+import traceback
 
 USAGE = """Options:
   --help                    print the help
@@ -84,7 +88,7 @@ _OPTIONS = [("help", False, False), ("matches_file", True, False), ("output_file
             ("update_initial_solution", False, False), ("previous_matches_file", True, False),
             ("record_file", True, False), ("earlier_record_file", True, False), ("query_images", True, True),
             ("joint_queries", False, False), ("additional_scenes", True, False),
-            ("listed_pairs", True, False), ("versioned_scenes", True, False)]
+            ("listed_pairs", True, False), ("versioned_scenes", True, False), ("task_stream", True, False)]
 
 
 def _find_option(name):
@@ -152,10 +156,10 @@ def parse_args(argv):
             sys.stdout.write("Patch Match graph problem solver\n\n" + USAGE)
             raise SystemExit(0)
         for req in ("matches_file", "output_file"):        # po::notify: required options, in declaration order
-            if req not in vals:
+            if req not in vals and "task_stream" not in vals:   # a task stream's tasks name their own files
                 raise _CliError("the option '--%s' is required but missing" % req)
         return argparse.Namespace(
-            matches_file=vals["matches_file"], output_file=vals["output_file"],
+            matches_file=vals.get("matches_file"), output_file=vals.get("output_file"),
             n_threads=_as_uint(vals, "n_threads", 8), banned_images=vals.get("banned_images", []),
             device=_as_uint(vals, "device", 0), gpus=_as_uint(vals, "gpus", 1), stats_json=vals.get("stats_json"),
             fixed_images=vals.get("fixed_images", []), initial_solution=vals.get("initial_solution"),
@@ -166,7 +170,7 @@ def parse_args(argv):
             record_file=vals.get("record_file"), earlier_record_file=vals.get("earlier_record_file"),
             query_images=vals.get("query_images"), joint_queries=bool(vals.get("joint_queries")),
             additional_scenes=vals.get("additional_scenes"), listed_pairs=vals.get("listed_pairs"),
-            versioned_scenes=vals.get("versioned_scenes"))
+            versioned_scenes=vals.get("versioned_scenes"), task_stream=vals.get("task_stream"), named=set(vals))
     except _CliError as e:                                  # solve.cc:397-401
         sys.stderr.write("ERROR: %s\n\n" % e)
         sys.stderr.write(USAGE)
@@ -194,7 +198,11 @@ _RULES = [("--keep_initial_solution", "needs", ["--initial_solution"]),
           # every scene of --versioned_scenes starts from its own solution and record, scene 0 from the ordinary flags
           ("--versioned_scenes", "excludes", ["--fixed_images", "--keep_initial_solution", "--carry_initial_solution",
                                               "--previous_matches_file", "--query_images", "--joint_queries",
-                                              "--additional_scenes", "--listed_pairs"])]
+                                              "--additional_scenes", "--listed_pairs"]),
+          # a task stream's command line sets the process alone (--device, --gpus, --n_threads): every task names
+          # its own files and options
+          ("--task_stream", "excludes", ["--matches_file", "--output_file", "--banned_images", "--stats_json"]
+           + _ONE_SCENE + ["--additional_scenes", "--listed_pairs", "--versioned_scenes"])]
 
 
 def _broken_rule(args):
@@ -409,7 +417,84 @@ def _run_batch(refine_batch, inputs, rows, args, opts, say, solve_fn, n_devices,
 
 def main(argv=None) -> int:
     args = parse_args(sys.argv[1:] if argv is None else argv)
+    if args.task_stream is not None:
+        return run_task_stream(args)
+    return _run(args)
 
+
+# library return codes after which the CUDA context may be unusable (include/lfr.h)
+_LOST = (-2, -3)   # LFR_ENODEV, LFR_ECUDA
+
+
+def _run_task(argv, stream):
+    """One task of a stream: (exit code, whether the context may be lost) of the run of `argv` as a one-shot process
+    runs it, under the stream's --device and --gpus; a task may not set those or --task_stream (exit code 2)."""
+    try:
+        args = parse_args(argv)
+        for name in ("task_stream", "device", "gpus"):
+            if name in args.named:
+                sys.stderr.write("ERROR: --%s is set once, on the task stream's command line\n" % name)
+                return 2, False
+        args.device, args.gpus = stream.device, stream.gpus
+        return _run(args), False
+    except SystemExit as e:   # as the interpreter turns it into an exit code
+        if e.code is None or isinstance(e.code, int):
+            return (e.code or 0) & 0xFF, False
+        sys.stderr.write("%s\n" % e.code)
+        return 1, False
+    except Exception as e:     # an uncaught exception: the traceback and exit code 1, as the interpreter ends a run
+        traceback.print_exc()
+        return 1, getattr(e, "lfr_rc", None) in _LOST
+
+
+def run_task_stream(args) -> int:
+    """--task_stream FILE: every line of FILE, read as it arrives (a FIFO or /dev/stdin serves), is one task whose
+    argument vector is the line's TAB-separated fields (none for an empty line), run as main() runs it.  After each,
+    its files are closed and `# task K: exit C` is on stdout, flushed, before the next line is read.  A failed task
+    ends itself alone, unless a library call returned LFR_ECUDA or LFR_ENODEV: the stream then ends with exit code 2.
+    The end of FILE ends it with 0.  lfr_solve_main.cc runs the same loop."""
+    broken = _broken_rule(args)
+    if broken:
+        sys.stderr.write(broken)
+        return 2
+    if "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        sys.stderr.write("ERROR: --task_stream: torchrun ranks do not run task streams; use --gpus N\n")
+        return 2
+    try:
+        fh = open(args.task_stream, "rb", buffering=0)
+    except OSError:
+        sys.stderr.write("ERROR: cannot read the task stream file '%s'\n" % args.task_stream)
+        return 2
+    with fh:
+        k = 0
+        while True:
+            line = _read_line(fh)
+            if line is None:
+                return 0
+            code, lost = _run_task([os.fsdecode(a) for a in line.split(b"\t")] if line else [], args)
+            sys.stderr.flush()
+            sys.stdout.write("# task %d: exit %d\n" % (k, code))
+            sys.stdout.flush()
+            if lost:
+                return 2
+            k += 1
+
+
+def _read_line(fh):
+    """The next line of the unbuffered file `fh` without its newline (the last one is optional), or None at its end.
+    Bytes are read one at a time, so no byte past the newline is taken before the task is done."""
+    buf = bytearray()
+    while True:
+        c = fh.read(1)
+        if not c:
+            return bytes(buf) if buf else None
+        if c == b"\n":
+            return bytes(buf)
+        buf += c
+
+
+def _run(args) -> int:
+    """One run of the parsed command line `args`."""
     from . import wire
     from .solver import GraphStageRouteError, refine, refine_lists, refine_scenes
 

@@ -49,7 +49,9 @@
 // INITIAL_SOLUTION<TAB>EARLIER_RECORD<TAB>RECORD_FILE`: a scene batch whose every scene is updated from its own
 // solution and record, or solved from zeros without one, and writes its own record: lfr_plan_update_solution_groups()
 // and lfr_plan_problem_record_groups() on the device route, lfr_wire_update_solution_groups() and
-// lfr_host_problem_record_groups() on the host route).  `--n_threads` is accepted and
+// lfr_host_problem_record_groups() on the host route) and --task_stream FILE (with --device, --gpus and --n_threads alone:
+// one process runs every line of FILE, read as it arrives, as a task, each line's TAB-separated fields its argument
+// vector, and prints `# task K: exit C` after each; run_stream()).  `--n_threads` is accepted and
 // ignored (the solve runs on the GPU).  local-feature-refinement_b200/cli.py is the same program in
 // Python; this one starts in milliseconds instead of importing numpy.
 #include <algorithm>
@@ -151,9 +153,11 @@ struct CliError {
   std::string msg;
 };
 
-// The end of the run with exit code `code`; its message is on stderr already
+// The end of the run with exit code `code`; its message is on stderr already.  `lost`: a library call returned
+// LFR_ECUDA or LFR_ENODEV, so the CUDA context may be unusable for any later run in the process.
 struct Exit {
   int code;
+  bool lost = false;
 };
 
 [[noreturn]] __attribute__((format(printf, 2, 3))) void fail(int code, const char* fmt, ...) {
@@ -162,6 +166,12 @@ struct Exit {
   std::vfprintf(stderr, fmt, ap);
   va_end(ap);
   throw Exit{code};
+}
+
+// Exits 2 after `ERROR: <what> failed (rc): <the library's message>` for a library call that returned `rc`
+[[noreturn]] void fail_call(const char* what, int rc) {
+  std::fprintf(stderr, "ERROR: %s failed (%d): %s\n", what, rc, lfr_last_error());
+  throw Exit{2, rc == LFR_ECUDA || rc == LFR_ENODEV};
 }
 
 struct OptionSpec {
@@ -177,7 +187,7 @@ const OptionSpec kOptions[] = {{"help", false, false},        {"matches_file", t
                                {"record_file", true, false},  {"earlier_record_file", true, false},
                                {"query_images", true, true},  {"joint_queries", false, false},
                                {"additional_scenes", true, false}, {"listed_pairs", true, false},
-                               {"versioned_scenes", true, false}};
+                               {"versioned_scenes", true, false}, {"task_stream", true, false}};
 
 // exact name, else unambiguous prefix (Boost.Program_options' default allow_guessing)
 const OptionSpec& find_option(const std::string& name) {
@@ -201,9 +211,10 @@ struct Options {
        joint_queries = false;
   std::string matches_file, output_file, initial_solution;
   std::optional<std::string> previous_matches_file, record_file, earlier_record_file, additional_scenes, listed_pairs,
-      versioned_scenes;
+      versioned_scenes, task_stream;
   std::vector<std::string> banned_images, fixed_images, query_images;
   uint64_t device = 0, gpus = 1;
+  std::set<std::string> named;  // every option the command line names
 };
 
 // Boost.Program_options semantics of solve.cc:387-401: long options, `--name value` or `--name=value`,
@@ -247,8 +258,10 @@ Options parse(int argc, char** argv) {
   Options o;
   o.help = flags.count("help") != 0;
   if (o.help) return o;
-  for (const char* req : {"matches_file", "output_file"})  // po::notify: required options, in declaration order
-    if (!single.count(req)) throw CliError{std::string("the option '--") + req + "' is required but missing"};
+  // po::notify: required options, in declaration order; a task stream's tasks name their own files
+  for (const char* req : {"matches_file", "output_file"})
+    if (!single.count(req) && !single.count("task_stream"))
+      throw CliError{std::string("the option '--") + req + "' is required but missing"};
   auto as_uint = [&](const char* name, uint64_t dflt) {  // lexical_cast<size_t>
     const auto it = single.find(name);
     if (it == single.end()) return dflt;
@@ -265,8 +278,9 @@ Options parse(int argc, char** argv) {
     const auto it = single.find(name);
     return it == single.end() ? std::optional<std::string>() : it->second;
   };
-  o.matches_file = single.at("matches_file");
-  o.output_file = single.at("output_file");
+  o.matches_file = given("matches_file").value_or("");
+  o.output_file = given("output_file").value_or("");
+  o.task_stream = given("task_stream");
   o.initial_solution = given("initial_solution").value_or("");
   o.previous_matches_file = given("previous_matches_file");
   o.record_file = given("record_file");
@@ -281,17 +295,22 @@ Options parse(int argc, char** argv) {
   o.carry_initial_solution = flags.count("carry_initial_solution") != 0;
   o.update_initial_solution = flags.count("update_initial_solution") != 0;
   o.joint_queries = flags.count("joint_queries") != 0;
+  for (const auto& kv : single) o.named.insert(kv.first);
+  for (const auto& kv : repeated)  // operator[] above added the repeatable options not given, empty
+    if (!kv.second.empty()) o.named.insert(kv.first);
+  o.named.insert(flags.begin(), flags.end());
   return o;
 }
 
 // The opt-in options the rules between options speak of
 enum Opt { kFixed, kStart, kKeep, kCarry, kUpdate, kPrevious, kRecord, kEarlier, kQuery, kJoint, kScenes, kLists, kVersioned,
-           kNumOpts };
+           kMatches, kOutput, kBanned, kTasks, kNumOpts };
 const char* const kOptName[kNumOpts] = {"--fixed_images",          "--initial_solution",    "--keep_initial_solution",
                                         "--carry_initial_solution", "--update_initial_solution", "--previous_matches_file",
                                         "--record_file",           "--earlier_record_file", "--query_images",
                                         "--joint_queries",         "--additional_scenes",   "--listed_pairs",
-                                        "--versioned_scenes"};
+                                        "--versioned_scenes",      "--matches_file",        "--output_file",
+                                        "--banned_images",         "--task_stream"};
 
 // `opt` needs `others[0]`, or excludes each of `others`
 struct Rule {
@@ -319,6 +338,10 @@ const std::vector<Rule> kRules = {
     // every scene of --versioned_scenes starts from its own solution and record, scene 0 from the ordinary flags;
     // fixed images, kept and carried solutions, earlier MatchingFiles and queries stay one-scene options
     {kVersioned, false, {kFixed, kKeep, kCarry, kPrevious, kQuery, kJoint, kScenes, kLists}},
+    // a task stream's command line sets the process alone (--device, --gpus, --n_threads): every task names its own
+    // files and options
+    {kTasks, false, {kMatches, kOutput, kBanned, kFixed, kStart, kKeep, kCarry, kUpdate, kPrevious, kRecord, kEarlier, kQuery,
+                     kJoint, kScenes, kLists, kVersioned}},
 };
 
 // Exits 2 after the ERROR line of the first rule the command line breaks
@@ -327,12 +350,15 @@ void check_rules(const Options& o) {
                               o.carry_initial_solution,      o.update_initial_solution,   o.previous_matches_file.has_value(),
                               o.record_file.has_value(),     o.earlier_record_file.has_value(), !o.query_images.empty(),
                               o.joint_queries,               o.additional_scenes.has_value(), o.listed_pairs.has_value(),
-                              o.versioned_scenes.has_value()};
+                              o.versioned_scenes.has_value(), o.named.count("matches_file") != 0,
+                              o.named.count("output_file") != 0, !o.banned_images.empty(), o.task_stream.has_value()};
   for (const Rule& r : kRules) {
     if (!set[r.opt]) continue;
     for (const Opt b : r.others) {
-      if (r.needs && !set[b]) fail(2, "ERROR: %s needs %s%s\n", kOptName[r.opt], kOptName[b], b == kStart ? " FILE" : "");
-      if (!r.needs && set[b]) fail(2, "ERROR: %s and %s exclude each other\n", kOptName[r.opt], kOptName[b]);
+      // the task stream excludes every option its command line names, whatever the value (an empty path too)
+      const bool on = r.opt == kTasks ? o.named.count(kOptName[b] + 2) != 0 : set[b];
+      if (r.needs && !on) fail(2, "ERROR: %s needs %s%s\n", kOptName[r.opt], kOptName[b], b == kStart ? " FILE" : "");
+      if (!r.needs && on) fail(2, "ERROR: %s and %s exclude each other\n", kOptName[r.opt], kOptName[b]);
     }
   }
   // a batch's scenes are updated or solved from zeros: a start point alone belongs to one scene
@@ -389,9 +415,18 @@ std::vector<std::string> matching_files(const std::string& path) {
 }
 
 // A file mapped read-only (a Madrid-scale MatchingFile is several GB: no second copy of it in memory).
+// Unmapped when released or destroyed, so that no run leaves a mapping behind, whichever way it ends.
 struct FileImage {
   const uint8_t* p = nullptr;
   size_t n = 0;
+  FileImage() = default;
+  FileImage(const FileImage&) = delete;
+  FileImage& operator=(const FileImage&) = delete;
+  FileImage(FileImage&& o) noexcept : p(o.p), n(o.n) {
+    o.p = nullptr;
+    o.n = 0;
+  }
+  ~FileImage() { release(); }
   bool open(const std::string& path) {
     const int fd = ::open(path.c_str(), O_RDONLY);
     if (fd < 0) return false;
@@ -1044,8 +1079,7 @@ void problem_record(std::vector<uint8_t>& record, Fill fill) {
   const int64_t need = fill(nullptr, 0);
   record.resize(need > 0 ? (size_t)need : 0);
   const int64_t got = need < 0 ? need : fill(record.data(), record.size());
-  if (got < 0 || (uint64_t)got != record.size())
-    fail(2, "ERROR: the problem record failed (%d): %s\n", (int)got, lfr_last_error());
+  if (got < 0 || (uint64_t)got != record.size()) fail_call("the problem record", (int)got);
 }
 
 using Clock = std::chrono::steady_clock;
@@ -1090,8 +1124,7 @@ void problem_records(Result& r, size_t n_scenes, uint64_t n_components, Fill fil
   r.record.resize(16 * (n_scenes + n_components));
   r.record_off.assign(n_scenes + 1, 0);
   const int64_t got = fill(r.record.data(), r.record.size(), r.record_off.data());
-  if (got < 0 || (uint64_t)got != r.record.size())
-    fail(2, "ERROR: the problem record failed (%d): %s\n", (int)got, lfr_last_error());
+  if (got < 0 || (uint64_t)got != r.record.size()) fail_call("the problem record", (int)got);
 }
 
 // Whether the run writes a problem record: --record_file (given, even with an empty path), or with
@@ -1129,8 +1162,7 @@ Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps
     fail(255, "Failed to parse proto object.\n");  // solve.cc:433-436, as the host decode
   if (rc == LFR_EINVAL || rc == LFR_EUNSUPPORTED)  // the input, as the host stage would reject it
     fail(2, "ERROR: the host graph stage rejected the input\n");
-  if (rc != LFR_OK)  // no device: the host route's message, from the same device check
-    fail(2, "ERROR: the solve failed (%d): %s\n", rc, lfr_last_error());
+  if (rc != LFR_OK) fail_call("the solve", rc);  // no device: the host route's message, from the same device check
 
   // problem initialisation (solve.cc:608-612) on the plan: the constant mask and the start point
   const uint32_t n_ids = st.n_ids();
@@ -1165,7 +1197,7 @@ Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps
     rc2 = (start == Start::kKeep ? lfr_plan_keep_solution : lfr_plan_start_from_solution)(
         plan.get(), nullptr, file, file_len, n_ids, names, name_off, nullptr);
   }
-  if (rc2 != LFR_OK) fail(2, "ERROR: the solve failed (%d): %s\n", rc2, lfr_last_error());
+  if (rc2 != LFR_OK) fail_call("the solve", rc2);
   print_sizes(sz);
 
   if (!o.carry_initial_solution) si.file.release();  // carried into the output otherwise
@@ -1173,7 +1205,7 @@ Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps
   if (sz.n_nodes) {
     int rc3 = lfr_plan_solve(plan.get(), nullptr);
     if (rc3 == LFR_OK) rc3 = lfr_plan_download(plan.get(), nullptr, nullptr, nullptr);  // waits for the solve, checks its error flag
-    if (rc3 != LFR_OK) fail(2, "ERROR: the solve failed (%d): %s\n", rc3, lfr_last_error());
+    if (rc3 != LFR_OK) fail_call("the solve", rc3);
   }
   print_times(t_start, t_solve);
 
@@ -1219,7 +1251,7 @@ Result run_device(const Options& o, Start start, const Labelling& lab, Pairs& ps
     need = encode(r.bytes.get(), cap);
   }
   plan.reset();
-  if (need < 0 || (uint64_t)need > cap) fail(2, "ERROR: the solve failed (%d): %s\n", (int)need, lfr_last_error());
+  if (need < 0 || (uint64_t)need > cap) fail_call("the solve", (int)need);
   if (lab.batched())
     for (uint64_t c : outside) r.n_outside += c;
   else
@@ -1324,8 +1356,7 @@ Result run_host(const Options& o, Start start, const Labelling& lab, const Pairs
     } else {
       rc3 = lfr_solve(&solve_prob, &opt, positions, &stats);
     }
-    if (rc3 != LFR_OK)  // no CPU fallback: without a CUDA device this is where the program stops
-      fail(2, "ERROR: the solve failed (%d): %s\n", rc3, lfr_last_error());
+    if (rc3 != LFR_OK) fail_call("the solve", rc3);  // no CPU fallback: without a CUDA device the program stops here
   }
   print_times(t_start, t_solve);
 
@@ -1420,8 +1451,9 @@ Result run_host(const Options& o, Start start, const Labelling& lab, const Pairs
   return r;
 }
 
-int run(int argc, char** argv) {
-  Options o;
+// The command line parsed into `o`, or the exit code of a run that ends there: 1 after Boost's error and the usage
+// on stderr (solve.cc:397-401), 0 after --help
+std::optional<int> parse_command_line(int argc, char** argv, Options& o) {
   try {
     o = parse(argc, argv);
   } catch (const CliError& e) {  // solve.cc:397-401
@@ -1434,6 +1466,37 @@ int run(int argc, char** argv) {
     std::fputs(kUsage, stdout);
     return 0;
   }
+  return std::nullopt;
+}
+
+// What a process sets once for all its runs.  A one-shot process pays for CUDA's start-up (driver initialisation
+// over every visible GPU, context creation: 0.4-0.8 s on an 8-GPU box) more than for all of its work on a
+// Fountain-scale scene.  Two measures: only the device that will be used is made visible (unless the caller already
+// chose), and the start-up runs on a helper thread while the first input is read, decoded and turned into a graph.
+struct Process {
+  uint64_t device = 0, gpus = 1;  // the device selection every run takes
+  bool started = false;
+  std::thread cuda_start;
+  void start(const Options& o) {
+    device = o.device;
+    gpus = o.gpus;
+    if (gpus <= 1 && !std::getenv("CUDA_VISIBLE_DEVICES")) {
+      setenv("CUDA_VISIBLE_DEVICES", std::to_string(device).c_str(), 1);
+      device = 0;
+    }
+    cuda_start = std::thread([] { lfr_host_free(lfr_host_alloc(64)); });
+    started = true;
+  }
+  void ready() {  // page-locked memory needs the context
+    if (cuda_start.joinable()) cuda_start.join();
+  }
+  ~Process() { ready(); }
+};
+
+// One run of the command line `o` under `proc`'s device selection, which it starts when no run has: everything from
+// the rules to the record files.  Returns 0 or throws Exit; either way every file, mapping, plan and page-locked
+// array it made is released by then (the library's per-device workspaces persist by design).
+int run_task(Options o, Process& proc) {
   check_rules(o);
   const Start start = start_mode(o);
   const Labelling lab = labelling(o);
@@ -1455,19 +1518,9 @@ int run(int argc, char** argv) {
   if (o.versioned_scenes) read_versioned_starts(vrows, si);
   const bool record = writes_records(vrows);
 
-  // A one-shot process pays for CUDA's start-up (driver initialisation over every visible GPU, context
-  // creation: 0.4-0.8 s on an 8-GPU box) more than for all of its work on a Fountain-scale scene.  Two
-  // measures: only the device that will be used is made visible (unless the caller already chose),
-  // and the start-up runs on a helper thread while the input is read, decoded and turned into a graph.
-  if (o.gpus <= 1 && !std::getenv("CUDA_VISIBLE_DEVICES")) {
-    setenv("CUDA_VISIBLE_DEVICES", std::to_string(o.device).c_str(), 1);
-    o.device = 0;
-  }
-  std::thread cuda_start([] { lfr_host_free(lfr_host_alloc(64)); });
-  struct Joiner {
-    std::thread& t;
-    ~Joiner() { if (t.joinable()) t.join(); }
-  } join_on_exit{cuda_start};
+  if (!proc.started) proc.start(o);
+  o.device = proc.device;
+  o.gpus = proc.gpus;
 
   Pairs ps = read_pairs(o.listed_pairs ? StringPairs{rows[0]} : rows);  // the lists' pairs are --matches_file's
   if (o.listed_pairs) select_listed_pairs(ps, rows, lists);
@@ -1478,7 +1531,7 @@ int run(int argc, char** argv) {
   Matches matches;
   if (!decode_on_device) decode_on_host(ps, matches, st.in);
 
-  cuda_start.join();  // page-locked memory needs the context
+  proc.ready();
   const Clock::time_point t_start = Clock::now();
   Result r = on_device ? run_device(o, start, lab, ps, st, si, rows.size(), record, decode_on_device, t_start)
                        : run_host(o, start, lab, ps, st, si, rows.size(), record, t_start);
@@ -1504,6 +1557,78 @@ int run(int argc, char** argv) {
     if (!f.good()) fail(255, "ERROR: cannot write the record file '%s'\n", path.c_str());
   }
   return 0;
+}
+
+// One task line's argument vector: the line split at TABs (paths with spaces need no quoting); none for an empty line
+std::vector<std::string> task_args(const std::string& line) {
+  std::vector<std::string> args;
+  for (size_t at = 0; !line.empty();) {
+    const size_t tab = line.find('\t', at);
+    args.push_back(line.substr(at, tab == std::string::npos ? std::string::npos : tab - at));
+    if (tab == std::string::npos) break;
+    at = tab + 1;
+  }
+  return args;
+}
+
+// The next line of `f` into `line`, without its newline (the last one is optional); false at the end of the file.
+// The read blocks until the line is there, so a FIFO or /dev/stdin serves as the file.
+bool read_line(std::FILE* f, std::string& line) {
+  line.clear();
+  int c;
+  while ((c = std::getc(f)) != EOF && c != '\n') line.push_back((char)c);
+  return c != EOF || !line.empty();
+}
+
+// One task of a stream: the run of `args` as a one-shot process would run it, except that the options the stream's
+// command line sets once (--task_stream, --device, --gpus) are refused with exit code 2
+int run_line(const std::vector<std::string>& args, Process& proc) {
+  std::vector<char*> argv{const_cast<char*>("solve")};
+  for (const std::string& a : args) argv.push_back(const_cast<char*>(a.c_str()));
+  Options o;
+  if (const std::optional<int> done = parse_command_line((int)argv.size(), argv.data(), o)) return *done;
+  for (const char* name : {"task_stream", "device", "gpus"})
+    if (o.named.count(name)) fail(2, "ERROR: --%s is set once, on the task stream's command line\n", name);
+  return run_task(o, proc);
+}
+
+// --task_stream FILE: one process runs every line of FILE as a task, in order, each as the one-shot run of that
+// argument vector would run it, so the start-up is paid once.  After a task its files are closed and `# task K:
+// exit C` is on stdout, flushed, before the next line is read: a task can read what the one before wrote, and a
+// client can wait for the line.  A failed task ends itself alone, unless a library call returned LFR_ECUDA or
+// LFR_ENODEV: the context may then be unusable, and the stream ends with exit code 2.  The end of FILE ends it with 0.
+int run_stream(const Options& so) {
+  const std::unique_ptr<std::FILE, int (*)(std::FILE*)> f(std::fopen(so.task_stream->c_str(), "rb"), &std::fclose);
+  if (!f) fail(2, "ERROR: cannot read the task stream file '%s'\n", so.task_stream->c_str());
+  Process proc;
+  proc.start(so);
+  std::string line;
+  for (unsigned long long k = 0; read_line(f.get(), line); ++k) {
+    int code;
+    bool lost = false;
+    try {
+      code = run_line(task_args(line), proc);
+    } catch (const Exit& e) {
+      code = e.code;
+      lost = e.lost;
+    }
+    std::fflush(stderr);
+    std::printf("# task %llu: exit %d\n", k, code);
+    std::fflush(stdout);
+    if (lost) return 2;
+  }
+  return 0;
+}
+
+int run(int argc, char** argv) {
+  Options o;
+  if (const std::optional<int> done = parse_command_line(argc, argv, o)) return *done;
+  if (o.task_stream) {
+    check_rules(o);
+    return run_stream(o);
+  }
+  Process proc;  // the one-shot run: the process part and one task
+  return run_task(o, proc);
 }
 
 }  // namespace
